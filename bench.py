@@ -8,19 +8,25 @@ Keras-Adam lr 3e-4, batch 65 536, synthetic N(0,1) inputs with labels from a fix
 
     python bench.py [--gpus N] [--steps K] [--warmup W]            # this repo's CUDA path (weak scaling: 65 536 rows/GPU)
     python bench.py --impl reference ...                           # the reference graph's CPU twin (host cores)
-    python bench.py --config C2|C3|C4|C4p                          # the other SURVEY 8d shapes (profiles/, not the driver)
+    python bench.py --config C2|C3|C4|C4p                          # the other SURVEY 8d shapes
+    python bench.py ... --dump-outputs DIR                         # + what the timed path computed in its last step
 
 Prints ONE JSON line (rank 0).
-  value / ms_per_step : device-resident throughput.  K steps per block between CUDA events (barrier + synchronize on
-                        both sides of every block), blocks repeated until the timed region is >= --min-seconds (2 s) so
-                        clocks and power are steady; the reported ms_per_step is the MEDIAN block (max over ranks).
+  value / ms_per_step : device-resident throughput.  Exactly K timed steps after W warm-up steps, between CUDA events
+                        (barrier + synchronize on both sides); ms_per_step = elapsed / K (max over ranks), and
+                        ms_per_step_median = the median of the K per-step event intervals.
   strong              : the same metric with the 65 536-row GLOBAL batch split over the N GPUs (SURVEY 8d "the metric as
                         stated"), measured in the same run (for N = 1 it equals value).
   e2e                 : the same step through the public API (model.train_on_batch) from pinned HOST buffers with the
-                        H2D copy and the D2H read of the metrics inside the timed region.
+                        H2D copy and the D2H read of the metrics inside the timed region (K more steps).
   roofline            : the dominant kernel's algorithmic FLOP/s (SURVEY 8d MAC counts) over its CUDA-event duration,
-                        against the measured dense bf16/fp16 tensor peak -- burst or sustained chosen from the SM clock
-                        sampled during the timed region.
+                        against the dense bf16/fp16 tensor peak (measured, or the H100 SXM data sheet's 989 TFLOP/s) --
+                        burst or sustained chosen from the SM clock sampled during the timed region.
+  --dump-outputs DIR  : after the K timed steps (rank 0), writes what that step path computed in its last step as float32
+                        .npy files: the metrics train_on_batch returned (metrics.npy, names in metrics_names.txt), the
+                        flat gradient vector with the step's statistics appended (grads_stats.npy) and the parameters after
+                        the optimizer update (params.npy).  Inputs, weights and noise are seeded, so two builds run with the
+                        same arguments can be compared output for output.
 See DESIGN.md section "Measurement".
 """
 import argparse
@@ -29,6 +35,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 
 import numpy as np
 
@@ -36,7 +43,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-METRIC = "training samples/sec (16-feat synthetic, batch 65k) at 1/2/4/8 B200; HBM GB/s"
+METRIC = "training samples/sec (16-feat synthetic, batch 65k) at 1/2/4/8 H100; HBM GB/s"
 LR = 3e-4
 N_DISTINCT_BATCHES = 16          # SURVEY.md 8d: N = 16 * 65536 rows, 16 steps per epoch
 
@@ -54,9 +61,9 @@ CONFIGS = {
     "C4p": dict(fdims=[1] * 50, enc=[128, 128], integ=[256, 256, 256], out=1, E=32, pe=False, nfreq=1, act="tanh", loss="bce",
                 batch=8192, note="BASELINE config 4: 50 shell features, batch 8192 (bf16 storage, 8 GPUs in BASELINE)"),
 }
-DTYPE_LABEL = {"fp32": "f32", "tf32": "tf32 (fp32 storage, kind::tf32 operands, fp32 accumulate)",
-               "fp16": "fp16 operands + fp32 accumulate (tcgen05 kind::f16; PE/exp/KL/loss/Adam fp32)",
-               "bf16": "bf16 operands + fp32 accumulate (tcgen05 kind::f16; PE/exp/KL/loss/Adam fp32)"}
+DTYPE_LABEL = {"fp32": "f32", "tf32": "tf32 (fp32 storage, tf32 wgmma operands, fp32 accumulate)",
+               "fp16": "fp16 operands + fp32 accumulate (wgmma f16; PE/exp/KL/loss/Adam fp32)",
+               "bf16": "bf16 operands + fp32 accumulate (wgmma bf16; PE/exp/KL/loss/Adam fp32)"}
 
 
 def synth_batches(cfg, rank, nb, batch, pinned):
@@ -143,14 +150,14 @@ def ncu_dram_traffic(group):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md 'clocks' line)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries, sampled into a temporary file)."""
     FIELDS = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
               "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
               "clocks_event_reasons.sw_power_cap")
 
     def __init__(self, index):
         self.proc = None
-        self.path = f"/tmp/dib_clocks_{os.getpid()}.csv"
+        self.path = os.path.join(tempfile.gettempdir(), f"dib_clocks_{os.getpid()}.csv")
         try:
             self.fh = open(self.path, "w")
             self.proc = subprocess.Popen(
@@ -194,13 +201,14 @@ def measured_peaks():
         return {"hbm_gbs": d["hbm_gbs"], "tflops_burst": d["bf16_tflops"],
                 "tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 "sustained_sm_mhz": (d.get("clocks_under_load") or {}).get("sm_mhz_median"), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "tflops_burst": 1590.0, "tflops_sustained": 1400.0, "sustained_sm_mhz": 1300.0,
-            "source": "fallback"}
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16/fp16 -- not a measured figure
+    return {"hbm_gbs": 3350.0, "tflops_burst": 989.0, "tflops_sustained": 989.0, "sustained_sm_mhz": None,
+            "source": "H100 SXM data sheet"}
 
 
 def pick_peak(peaks, clocks):
-    """Burst peak when the SM clock stayed near its maximum during the timed region (this step draws ~250 W of the
-    1000 W cap, so it does), the sustained figure when the clock sagged toward the power-capped GEMM's."""
+    """Burst peak when the SM clock stayed near its maximum during the timed region, the sustained figure when the clock
+    sagged toward the power-capped GEMM's."""
     sm, mx = (clocks or {}).get("sm_mhz"), (clocks or {}).get("sm_max_mhz")
     sus = peaks.get("sustained_sm_mhz") or 1400.0
     if sm and mx and sm < 0.5 * (mx + sus):
@@ -277,7 +285,7 @@ def workload_config(cfg, name, n_gpus=None, precision=None, per_gpu=None):
     per_gpu = cfg["batch"] if per_gpu is None else per_gpu
     return {"workload": f"{name}: {cfg['note']}; {per_gpu} rows/GPU",
             "global_batch": per_gpu * n_gpus, "per_gpu_batch": per_gpu, "parallelism": f"dp{n_gpus}", "precision": precision,
-            "l2": "no explicit flush: every step streams its intermediates through the 126 MB L2 (16-bit path ~0.33 GB of "
+            "l2": "no explicit flush: every step streams its intermediates through the 50 MB L2 (16-bit path ~0.3 GB of "
                   "activations/gradients/partials per 65536 rows), evicting the 16 rotating input batches between their uses"}
 
 
@@ -307,16 +315,19 @@ def main():
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--precision", default=os.environ.get("DIB_PRECISION", "fp16"), choices=["fp16", "bf16", "tf32", "fp32"],
-                    help="fp16 = fused tcgen05 kernels on fp16 operands (default, the headline); bf16 likewise; "
-                         "tf32 = kind::tf32 GEMMs on fp32 storage; fp32 = exact CUDA-core parity path")
+                    help="fp16 = fused wgmma kernels on fp16 operands (default, the headline); bf16 likewise; "
+                         "tf32 = tf32 wgmma GEMMs on fp32 storage; fp32 = exact CUDA-core parity path")
     ap.add_argument("--config", default="C0", choices=sorted(CONFIGS))
-    ap.add_argument("--min-seconds", type=float, default=2.0, help="lower bound on the device-timed region")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed step path computed in its last step to DIR/*.npy (float32)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-strong", action="store_true")
     ap.add_argument("--scaling", default="weak", choices=["weak", "strong"],
-                    help="what `value` reports -- weak (default, the driver's contract): the config batch per GPU; strong: the "
+                    help="what `value` reports -- weak (default): the config batch per GPU; strong: the "
                          "global batch split over the GPUs.  The other one is always reported under its own key.")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     cfg = CONFIGS[args.config]
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -358,80 +369,88 @@ def main():
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         return float(t.item())
 
-    def timed_blocks(step_fn, steps, min_seconds, max_blocks=4000):
-        """Blocks of exactly `steps` steps, each between CUDA events with barrier + synchronize on both sides; repeated
-        until the device-timed total reaches min_seconds.  Returns (median block ms [max over ranks], total s, blocks)."""
-        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        times, total, it = [], 0.0, 0
-        while True:
-            barrier()
-            ev0.record()
-            for _ in range(steps):
-                step_fn(it)
-                it += 1
-            ev1.record()
-            barrier()
-            ms = max_over_ranks(ev0.elapsed_time(ev1))
-            times.append(ms)
-            total += ms * 1e-3
-            if total >= min_seconds or len(times) >= max_blocks:
-                break
-        return float(np.median(times)), total, len(times)
+    def timed_steps(step_fn, steps):
+        """Exactly `steps` steps between CUDA events, barrier + synchronize on both sides; an event after every step.
+        Returns (total ms [max over ranks], median per-step ms)."""
+        evs = [torch.cuda.Event(enable_timing=True) for _ in range(steps + 1)]
+        barrier()
+        evs[0].record()
+        for i in range(steps):
+            step_fn(i)
+            evs[i + 1].record()
+        barrier()
+        per = [evs[i].elapsed_time(evs[i + 1]) for i in range(steps)]
+        return max_over_ranks(evs[0].elapsed_time(evs[-1])), float(np.median(per))
 
-    def measure(PB, min_seconds, with_e2e):
+    def dump_outputs(out_dir, metrics):
+        """What the timed path computed in its last step: the metrics train_on_batch returned, the gradient / statistics
+        vector of that step and the parameters after its update (float32; inputs, weights and noise are seeded)."""
+        os.makedirs(out_dir, exist_ok=True)
+        names = sorted(metrics)
+        np.save(os.path.join(out_dir, "metrics.npy"), np.array([metrics[k] for k in names], dtype=np.float32))
+        with open(os.path.join(out_dir, "metrics_names.txt"), "w") as fh:
+            fh.write("\n".join(names) + "\n")
+        np.save(os.path.join(out_dir, "grads_stats.npy"), model._gradstats.detach().float().cpu().numpy())
+        np.save(os.path.join(out_dir, "params.npy"), model.get_flat_weights().astype(np.float32))
+
+    def measure(PB, with_e2e, dump_dir=None):
         """Device-resident and (optionally) end-to-end throughput at PB rows per GPU."""
         xs_h, ys_h = synth_batches(cfg, rank, N_DISTINCT_BATCHES, PB, pinned=True)
         xs_d = [x.cuda(non_blocking=True) for x in xs_h]
         ys_d = [y.cuda(non_blocking=True) for y in ys_h]
         torch.cuda.synchronize()
+        last = {}
 
         def device_step(i):       # public API, device-resident batch, no host read inside the step
-            model.train_on_batch(xs_d[i % N_DISTINCT_BATCHES], ys_d[i % N_DISTINCT_BATCHES], sync=False)
+            last["out"] = model.train_on_batch(xs_d[i % N_DISTINCT_BATCHES], ys_d[i % N_DISTINCT_BATCHES], sync=False)
 
         for i in range(args.warmup):
             device_step(i)
         barrier()
         count = lambda: int(lib.dib_launch_count()) + int(getattr(model, "_replayed_launches", 0))   # eager + graph-replayed kernels
         launches0 = count()
-        blk_ms, total_s, nblk = timed_blocks(device_step, args.steps, min_seconds)
+        total_ms, med_ms = timed_steps(lambda i: device_step(args.warmup + i), args.steps)
         launches = count() - launches0
-        res = {"ms_per_step": blk_ms / args.steps, "timed_region_s": total_s, "blocks": nblk, "launches": launches,
-               "launches_per_step": launches / (nblk * args.steps), "xs_d": xs_d, "ys_d": ys_d}
+        if dump_dir and rank == 0:
+            dump_outputs(dump_dir, dict(last["out"].get()))
+        res = {"ms_per_step": total_ms / args.steps, "ms_per_step_median": med_ms, "timed_region_s": total_ms * 1e-3,
+               "launches": launches, "launches_per_step": launches / args.steps, "xs_d": xs_d, "ys_d": ys_d}
         res["value"] = PB * world / (res["ms_per_step"] * 1e-3)
         if with_e2e:
             for i in range(3):
                 model.train_on_batch(xs_h[i], ys_h[i], sync=False).get()
             pend = []
-            last = {}
+            seen = {}
 
             def e2e_step(i):
                 # every step: pinned host batch -> H2D (copy stream) -> step -> async D2H of the metrics into pinned memory
                 pend.append(model.train_on_batch(xs_h[i % N_DISTINCT_BATCHES], ys_h[i % N_DISTINCT_BATCHES], sync=False))
                 if len(pend) > 4:
-                    last.update(pend.pop(0).get())       # the host reads every step's result, a few steps behind the device
+                    seen.update(pend.pop(0).get())       # the host reads every step's result, a few steps behind the device
 
-            blk, tot, nb = timed_blocks(e2e_step, args.steps, min(min_seconds, 1.0))
+            tot, _ = timed_steps(e2e_step, args.steps)
             for p in pend:
-                last.update(p.get())
-            e2e_ms = blk / args.steps
+                seen.update(p.get())
+            e2e_ms = tot / args.steps
             res["e2e"] = {"value": PB * world / (e2e_ms * 1e-3), "unit": "samples/s", "ms_per_step": e2e_ms,
-                          "timed_region_s": tot, "blocks": nb,
+                          "timed_region_s": tot * 1e-3,
                           "h2d_bytes_per_step": int(xs_h[0].numel() * 4 + ys_h[0].numel() * 4),
                           "d2h_bytes_per_step": int((F + 3) * 4),
                           "api": "DistributedIBNet.train_on_batch(host x, host y, sync=False).get() -> metrics dict "
                                  "(H2D on a copy stream, D2H async)",
-                          "last_loss": last.get("loss")}
+                          "last_loss": seen.get("loss")}
         return res
 
     # ---------------- weak (config batch per GPU) and strong (global batch split) measurements
     sampler = ClockSampler(local_rank) if rank == 0 else None      # sampled under load: warm-up + timed regions
+    gpu_name = torch.cuda.get_device_name(local_rank)
     PB_weak = BATCH
     PB_strong = max(BATCH // world, 1)
     primary_PB = PB_weak if args.scaling == "weak" else PB_strong
-    prim = measure(primary_PB, args.min_seconds, with_e2e=True)
+    prim = measure(primary_PB, with_e2e=True, dump_dir=args.dump_outputs)
     other = None
     if world > 1 and not args.no_strong:
-        other = measure(PB_strong if args.scaling == "weak" else PB_weak, min(args.min_seconds, 1.0), with_e2e=False)
+        other = measure(PB_strong if args.scaling == "weak" else PB_weak, with_e2e=False)
     clocks = sampler.stop() if sampler else None
     weak, strong = (prim, other) if args.scaling == "weak" else (other, prim)
     if world == 1:
@@ -492,16 +511,17 @@ def main():
     if rank == 0:
         pack = lambda r, pb: None if r is None else {"value": r["value"], "unit": "samples/s", "ms_per_step": r["ms_per_step"],
                                                      "per_gpu_batch": pb, "global_batch": pb * world,
-                                                     "timed_region_s": r["timed_region_s"], "blocks": r["blocks"]}
+                                                     "timed_region_s": r["timed_region_s"]}
         line = {
             "metric": METRIC, "value": prim["value"], "unit": "samples/s", "n_gpus": world, "steps": args.steps,
-            "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": args.scaling,
+            "warmup": args.warmup, "ms_per_step": ms_per_step, "ms_per_step_median": prim["ms_per_step_median"],
+            "higher_is_better": True, "scaling": args.scaling,
             "vs_baseline": None, "dtype": DTYPE_LABEL[args.precision],
             "data": "synthetic", "config": workload_config(cfg, args.config, world, args.precision, PB),
-            "timed_region_s": prim["timed_region_s"], "blocks": prim["blocks"],
-            "timing": f"median of {prim['blocks']} blocks of {args.steps} steps (CUDA events, barrier+sync around each block, max over ranks)",
+            "timed_region_s": prim["timed_region_s"],
+            "timing": f"{args.steps} steps after {args.warmup} warm-up steps between CUDA events (barrier+sync on both sides, max over ranks)",
             "weak": pack(weak, PB_weak), "strong": pack(strong, PB_strong),
-            "clocks": clocks, "e2e": prim.get("e2e"),
+            "gpu": gpu_name, "clocks": clocks, "e2e": prim.get("e2e"),
             "gpu_launches": prim["launches"], "launches_per_step": prim["launches_per_step"],
             "roofline": roofline, "cpu_baseline": cpu_baseline, "host_nproc": os.cpu_count(),
             "library": os.path.relpath(_lib.library_path(), ROOT), "build": lib.dib_build_info().decode(),

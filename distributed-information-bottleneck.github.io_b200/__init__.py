@@ -1,8 +1,8 @@
-"""dib_b200 -- B200-native Distributed Information Bottleneck training engine.
+"""dib_b200 -- H100-native Distributed Information Bottleneck training engine.
 
 Drop-in for the hot path of distributed-information-bottleneck.github.io: ``models.DistributedIBNet`` /
 ``model.compile`` / ``model.fit`` / ``InfoBottleneckAnnealingCallback`` / ``SaveCompressionMatricesCallback``,
-backed by hand-written sm_100a CUDA kernels behind the C ABI of include/dib_b200.h.
+backed by hand-written sm_90a CUDA kernels behind the C ABI of include/dib_b200.h.
 """
 from . import ctw, keras_compat, models, parallel, utils                              # noqa: F401
 from .keras_compat import Adam, SGD, RMSprop, Callback, History, losses, optimizers           # noqa: F401

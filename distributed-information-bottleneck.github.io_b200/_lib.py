@@ -1,5 +1,5 @@
 """ctypes binding of libdib_b200.so (include/dib_b200.h).  There is deliberately NO fallback: if the CUDA
-library is missing or no B200 is visible, every compute entry point raises."""
+library is missing or no H100 is visible, every compute entry point raises."""
 import ctypes
 import os
 from ctypes import POINTER, c_char_p, c_float, c_int32, c_int64, c_size_t, c_uint32, c_uint64, c_void_p
@@ -11,7 +11,7 @@ ABI_VERSION = 2
 ACTIVATIONS = {None: 0, "linear": 0, "relu": 1, "tanh": 2, "leaky_relu": 3, "sigmoid": 4, "elu": 5}
 LOSSES = {"bce_logits": 0, "sparse_ce_logits": 1, "mse": 2, "external": 3, "bce_probs": 4}
 ENCODER_KINDS = {"mlp": 0, "simple": 1}
-# 'fp16' / 'bf16': fused 16-bit-operand tcgen05 kernels (fp32 accumulate); 'tf32': kind::tf32 GEMMs on fp32 storage;
+# 'fp16' / 'bf16': fused 16-bit-operand wgmma kernels (fp32 accumulate); 'tf32': tf32 wgmma GEMMs on fp32 storage;
 # 'fp32': exact CUDA-core FMA parity path.  See enum dib_precision in include/dib_b200.h.
 PRECISIONS = {"fp32": 0, "tf32": 1, "bf16": 2, "fp16": 3}
 

@@ -1,12 +1,12 @@
-"""Build libdib_b200.so (the C-ABI library of include/dib_b200.h) in-tree with nvcc for sm_100a.
+"""Build libdib_b200.so (the C-ABI library of include/dib_b200.h) in-tree with nvcc for the H100 (sm_90a).
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot.  No torch headers are involved:
-the library is plain CUDA C++ behind an extern "C" surface.
+The .so is a build product (git-ignored).  No torch headers are involved: the library is plain CUDA C++ behind an
+extern "C" surface.
 
 Every translation unit is compiled to its own object (in parallel, cached by content hash under csrc/_obj/) and the
 objects are linked into a temporary file that is renamed over the library, all under an fcntl lock, so that N ranks
 importing the package at once cannot interleave writes.  The source stamp hashes file CONTENTS under relative names:
-the same tree at another path (the GPU box snapshot) matches.  A stale prebuilt library is never used silently.
+the same tree at another path matches.  A stale prebuilt library is never used silently.
 """
 import fcntl
 import hashlib
@@ -25,7 +25,7 @@ STAMP = LIB_PATH + ".srchash"
 HEADER = os.path.join(PKG_DIR, "..", "include", "dib_b200.h")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]
 
@@ -112,7 +112,7 @@ def build_library(force=False, verbose=False):
             with ThreadPoolExecutor(max_workers=min(len(srcs), os.cpu_count() or 4)) as ex:
                 outs = list(ex.map(lambda s: _compile_one(nvcc, s, hdr, verbose), srcs))
             tmp = LIB_PATH + f".tmp{os.getpid()}"
-            res = subprocess.run([nvcc, "-shared", "-o", tmp] + [o for o, _ in outs],
+            res = subprocess.run([nvcc] + NVCC_FLAGS[:2] + ["-shared", "-o", tmp] + [o for o, _ in outs],
                                  capture_output=True, text=True)
             if res.returncode != 0:
                 raise RuntimeError("link failed:\n" + res.stdout + res.stderr)

@@ -75,10 +75,10 @@ struct dib_model {
   DibEncFusedDesc fdesc;
   void* d_fused_tables = nullptr;
   long long pack_off = 0;       // packed 16-bit encoder weights inside the workspace (float offset)
-  int kl_stride = 0, num_sms = 148, part_rows = kMaxSplits;
+  int kl_stride = 0, num_sms = 132, part_rows = kMaxSplits;
   // 16-bit integration network path (dib_int16.cu); offsets are FLOAT offsets into the workspace
   bool int16_ok = false;
-  long long emb16_off = 0, demb16_off = 0, headpart_off = 0, dbpart_off = 0, eps16_off = 0, a0g_off = 0;
+  long long emb16_off = 0, demb16_off = 0, headpart_off = 0, dbpart_off = 0;
   int head_stride = 0, dbpart_stride = 0;
   long long dbpart_layer = 0;       // floats per layer of the dgrad column-sum partials
   std::vector<long long> g16_off, dg16_off, w16_off;   // [1..Li], [1..Li], [0..Li-1]
@@ -98,8 +98,8 @@ struct dib_model {
 
 namespace {
 
-// precision modes: FP32 = CUDA-core FMA; TF32 = kind::tf32 grouped GEMMs on fp32 storage; FP16 / BF16 = the fused
-// 16-bit-operand kernels (dib_enc_fused.cu, dib_int16.cu) where the shapes allow, kind::tf32 GEMMs elsewhere
+// precision modes: FP32 = CUDA-core FMA; TF32 = tf32 wgmma grouped GEMMs on fp32 storage; FP16 / BF16 = the fused
+// 16-bit-operand kernels (dib_enc_fused.cu, dib_int16.cu) where the shapes allow, tf32 GEMMs elsewhere
 bool is_tc(const dib_model* h) { return h->precision != DIB_PREC_FP32; }
 bool want16(const dib_model* h) { return h->precision == DIB_PREC_FP16 || h->precision == DIB_PREC_BF16; }
 
@@ -157,8 +157,6 @@ void plan(dib_model* h) {
     const long long FE = (long long)h->F * h->E;
     h->emb16_off = take(c, (B * FE + 1) / 2);
     h->demb16_off = take(c, (B * FE + 1) / 2);
-    h->eps16_off = take(c, (B * FE + 1) / 2);      // the step's noise, 16-bit, from the forward to the backward kernel
-    h->a0g_off = take(c, B * h->F * 8);            // ... and its [pe|1] first-layer operand rows (16 x 16-bit per row and feature)
     h->g16_off.assign(h->Li + 1, 0); h->dg16_off.assign(h->Li + 1, 0); h->w16_off.assign(h->Li + 1, 0);
     for (int j = 1; j <= h->Li; ++j) {
       h->g16_off[j] = take(c, (B * h->int_arch[j - 1] + 1) / 2);
@@ -380,7 +378,6 @@ int run_forward(const Ctx& c, const float* x, const float* y, const float* eps, 
     const bool i16 = h->int16_ok && !h->force_int32 && !enc_only;
     if (i16) { io.emb = nullptr; io.emb16 = c.ws + h->emb16_off; io.ldemb16 = h->F * h->E; }
     if (enc_only) io.emb = nullptr;      // the caller's network consumes user_emb; nothing downstream reads the workspace copy
-    if (training && !eps && dib_enc_bwd_version() >= 2) { io.eps16 = c.ws + h->eps16_off; io.a0g = c.ws + h->a0g_off; }
     prof_begin(c, "enc_fused_fwd");
     DIB_CUDA_OK(dib_enc_fused_forward(d, io, c.st));
     prof_end(c);
@@ -531,14 +528,11 @@ int dib_debug_force_unfused(dib_model* h, int32_t on) {
   return 0;
 }
 
-// kernel-variant switch for A/B measurements: key 0 = fused encoder backward kernel (1 = single chain, 2 = two chains);
-// key 1 = integration FWD/DGRAD GEMMs with the weight slice resident in shared memory (1, default) or re-streamed (0)
+// kernel-variant switch for A/B measurements (keys documented in include/dib_b200.h)
 int dib_debug_set_variant(int32_t key, int32_t value) {
-  if (key == 0) { dib_enc_bwd_set_version(value); return 0; }
   if (key == 1) { dib_int16_rb_set(value); return 0; }
   if (key == 2) { dib_int16_head1_set(value); return 0; }
   if (key == 3) { dib_int16_fwd2_set(value); return 0; }
-  if (key == 4) { dib_int16_2sm_set(value); return 0; }
   if (key == 5) { dib_int16_dbg_set(value); return 0; }     // measurement only: wrong results
   return fail("dib_debug_set_variant: unknown key");
 }
@@ -599,7 +593,7 @@ int dib_debug_gemm_tc(int32_t mode, const float* A, int32_t lda, const float* B,
 const char* dib_last_error(void) { return g_last_error.c_str(); }
 
 const char* dib_build_info(void) {
-  return "dib_b200 abi=2 arch=sm_100a paths=fp32-simt,tf32-tcgen05,fp16-fused-tcgen05,bf16-fused-tcgen05";
+  return "dib_b200 abi=2 arch=sm_90a paths=fp32-simt,tf32-wgmma,fp16-fused-wgmma,bf16-fused-wgmma";
 }
 
 int32_t dib_model_info(const dib_model* h, char* out, size_t out_bytes) {
@@ -611,8 +605,8 @@ int32_t dib_model_info(const dib_model* h, char* out, size_t out_bytes) {
   std::string s = std::string("precision=") + pn[h->precision];
   if (!is_tc(h)) s += " encoders=simt-fp32 integration=simt-fp32 operands=fp32 accumulate=fp32";
   else {
-    s += fused ? std::string(" encoders=fused-tcgen05-") + k16 : std::string(" encoders=grouped-tcgen05-tf32");
-    s += i16 ? std::string(" integration=int16-tcgen05-") + k16 : std::string(" integration=tcgen05-tf32");
+    s += fused ? std::string(" encoders=fused-wgmma-") + k16 : std::string(" encoders=grouped-wgmma-tf32");
+    s += i16 ? std::string(" integration=int16-wgmma-") + k16 : std::string(" integration=wgmma-tf32");
     s += fused ? std::string(" operands=") + (h->precision == DIB_PREC_BF16 ? "bf16" : "fp16") : std::string(" operands=tf32");
     s += " accumulate=fp32";
   }
@@ -704,7 +698,7 @@ int dib_create(const dib_config* cfg, dib_model** out) {
     int dev = 0;
     cudaGetDevice(&dev);
     if (cudaDeviceGetAttribute(&h->num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || h->num_sms < 1)
-      h->num_sms = 148;
+      h->num_sms = 132;
   }
   plan(h);
 
@@ -963,7 +957,6 @@ int dib_train_step_phased(dib_model* h, const float* params, const float* x, con
     io.params = c.params; io.packed = c.ws + h->pack_off; io.x = x; io.ldx = h->D; io.n = n;
     io.eps = eps; io.seed = seed; io.step = step; io.step_dev = c.step_dev(); io.sample_offset = sample_offset;
     io.emb = nullptr; io.ldemb = 0; io.user_emb = nullptr; io.kl_part = nullptr; io.kl_stride = 0;
-    if (!eps && dib_enc_bwd_version() >= 2) { io.eps16 = c.ws + h->eps16_off; io.a0g = c.ws + h->a0g_off; }   // written by this step's forward
     DibEncFusedBwdIO b;
     if (i16) { b.d_emb = nullptr; b.ldd = 0; b.d_emb16 = c.ws + h->demb16_off; b.ldd16 = h->F * h->E; }
     else { b.d_emb = c.ws + h->d_emb.off; b.ldd = h->d_emb.ld; }
@@ -1123,7 +1116,6 @@ int dib_encoders_backward(dib_model* h, const float* params, const float* x, con
     io.params = c.params; io.packed = c.ws + h->pack_off; io.x = x; io.ldx = h->D; io.n = n;
     io.eps = eps; io.seed = seed; io.step = step; io.step_dev = c.step_dev(); io.sample_offset = sample_offset;
     io.emb = nullptr; io.ldemb = 0; io.user_emb = nullptr; io.kl_part = nullptr; io.kl_stride = 0;
-    if (!eps && dib_enc_bwd_version() >= 2) { io.eps16 = c.ws + h->eps16_off; io.a0g = c.ws + h->a0g_off; }   // written by this step's forward
     DibEncFusedBwdIO b;
     b.d_emb = d_emb; b.ldd = FE; b.beta_dev = bw; b.inv_batch = inv_global_batch;
     b.gscale = exp2f(ceilf(log2f(1.f / inv_global_batch)));

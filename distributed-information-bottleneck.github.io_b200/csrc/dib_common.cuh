@@ -1,4 +1,4 @@
-// dib_common.cuh -- shared device helpers for the B200 Distributed-IB engine (sm_100a).
+// dib_common.cuh -- shared device helpers of the Distributed-IB engine (H100, sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -99,20 +99,19 @@ __device__ __forceinline__ float dib_round_tf32(float x) {
 }
 __device__ __forceinline__ float dib_maybe_round(float x, int on) { return on ? dib_round_tf32(x) : x; }
 
-// 32-byte global stores / loads (sm_100: STG.E.ENL2.256 / LDG.E.ENL2.256).  A 16-byte store per lane to rows that are 512 B apart
-// writes HALF a 32-byte sector per lane and instruction; the epilogues that emit a row-contiguous 64 B per lane halve their store
-// instructions and L2 write transactions with these.  `p` must be 32-byte aligned.
-__device__ __forceinline__ void dib_st_global_v8(void* p, const uint32_t (&w)[8]) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-               ::"l"(p), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7]) : "memory");
-}
+// 32 consecutive bytes per thread as two 16-byte accesses (sm_90 has no 32-byte global load / store).  `p` must be 16-byte aligned.
 __device__ __forceinline__ void dib_st_global_v8(void* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d, uint32_t e, uint32_t f, uint32_t g, uint32_t h) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-               ::"l"(p), "r"(a), "r"(b), "r"(c), "r"(d), "r"(e), "r"(f), "r"(g), "r"(h) : "memory");
+  uint4* q = static_cast<uint4*>(p);
+  q[0] = make_uint4(a, b, c, d);
+  q[1] = make_uint4(e, f, g, h);
+}
+__device__ __forceinline__ void dib_st_global_v8(void* p, const uint32_t (&w)[8]) {
+  dib_st_global_v8(p, w[0], w[1], w[2], w[3], w[4], w[5], w[6], w[7]);
 }
 __device__ __forceinline__ void dib_ld_global_v8(const void* p, uint32_t (&w)[8]) {
-  asm volatile("ld.global.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7]) : "l"(p) : "memory");
+  const uint4* q = static_cast<const uint4*>(p);
+  const uint4 a = q[0], b = q[1];
+  w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w; w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
 }
 
 __device__ __forceinline__ float dib_warp_sum(float v) {

@@ -1,13 +1,19 @@
 // dib_int16.cu -- the integration network (models.py:81-84,122) in the tensor-core mode: 16-bit activations in HBM
-// (emb, g_k, dz_k as fp16 -> half the traffic of the fp32 layout), tcgen05.mma kind::f16 with fp32 accumulation.
+// (emb, g_k, dz_k as fp16 -> half the traffic of the fp32 layout), wgmma on 16-bit operands with fp32 accumulation.
 //
 //   * dib_int16_gemm_kernel<MODE>: TMA-fed, mbarrier-pipelined 128 x 128 tile GEMM (K step 64 = one 128-byte swizzle
-//     span) with fused epilogues:  FWD  g = act(A W + b) -> fp16;  DGRAD  dz_in = (dz W^T) * act'(g_in) -> fp16;
-//     WGRAD  dW = g^T dz over a batch slice -> fp32 split partial (scaled back by 1/S), db = colsum dz from the smem tiles.
+//     span) with fused epilogues:  FWD  g = act(A W + b) -> fp16;  DGRAD  dz_in = (dz W^T) * act'(g_in) -> fp16 and the
+//     column sums of dz_in (bias gradient of the layer below);  WGRAD  dW = g^T dz over a batch slice -> fp32 split partial
+//     (scaled back by 1/S).
 //   * dib_int16_head_kernel: the narrow output layer (out <= 16) fused with everything around it -- logits, compiled
 //     loss + accuracy, d loss / d logits, the dgrad into the last hidden layer (incl. its act') and the output layer's
 //     own weight/bias gradients -- one pass over the last hidden activation.
+//   * dib_int16_fwd2_kernel: the last two 256-wide hidden layers and the single-output head of models with out = 1.
 // Gradient operands are scaled by the power-of-two loss scale S (see dib_enc_fused.cu) to stay inside fp16 range.
+//
+// The GEMM kernels are warp-specialised: warps 0..7 are two consumer warpgroups (warpgroup g computes rows [64 g, 64 g + 64)
+// of the 128-row tile with m64nNk16 wgmma instructions, accumulators in registers, and runs the epilogue), warp 8 issues
+// the TMA loads of the shared-memory ring.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -15,20 +21,20 @@
 
 #include "dib_common.cuh"
 #include "dib_kernels.h"
-#include "dib_sm100.cuh"
+#include "dib_sm90.cuh"
 
 int dib_int16_rb_enabled();
 int dib_int16_head1_enabled();
-int dib_int16_2sm_enabled();
 
 namespace {
 
-using namespace sm100;
+using namespace sm90;
 
-constexpr int kBM = 128, kBN = 128, kBK = 64, kStages = 3;
+constexpr int kBM = 128, kBN = 128, kBK = 64, kStages = 3, kRbStages = 4;
 constexpr int kABytes = kBM * 128, kBBytes = kBN * 128, kStageBytes = kABytes + kBBytes;
-constexpr int kBarOff = kStages * kStageBytes;
-constexpr int kSmemTotal = kBarOff + 128 + 1024;
+constexpr int kConsumers = 256, kGemmThreads = kConsumers + 32;
+constexpr int kProducerWarp = kConsumers / 32;
+constexpr int kEmptyArrivals = kConsumers / 32;   // every consumer warp releases a stage once its MMAs have read it
 
 struct Int16Args {
   float* out32; uint16_t* out16; int ldc;       // WGRAD partial base (fp32) | FWD/DGRAD output (fp16)
@@ -54,52 +60,63 @@ __device__ __forceinline__ void unpack_h2(uint32_t u, float& a, float& b) {
   else { const float2 f = __half22float2(*reinterpret_cast<__half2*>(&u)); a = f.x; b = f.y; }
 }
 
-// Persistent: each CTA walks tiles blockIdx.x, +gridDim.x, ...; the shared-memory stage ring runs across tiles and the
-// fp32 accumulator is double-buffered in TMEM (2 x 128 columns), so the epilogue of tile i overlaps the mainloop of
-// tile i+1.  Warp roles: 0 TMA producer | 1 MMA issuer (+ TMEM owner) | 2..5 epilogue.
-template <int MODE, bool BF16>
-__global__ void __launch_bounds__(192, 2)
+__device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+
+// 16-bit operand tiles of one pipeline stage (TMA SWIZZLE_128B boxes, see map_k / map_mn):
+//   K-major  [rows][128 B]: a 16-deep k step is 32 B;  warpgroup g's 64 rows start 8 KB in
+//   MN-major [panels of 64 M/N][64 k-rows][128 B]: a 16-deep k step is 2048 B, panels 8 KB apart
+__device__ __forceinline__ uint64_t desc_kmaj(uint32_t base, int kk) { return gmma_desc(base + kk * 32, 16, 1024); }
+__device__ __forceinline__ uint64_t desc_mnmaj(uint32_t base, int kk) { return gmma_desc(base + kk * 2048, kBK * 128, 1024); }
+
+// the 8 lanes of a warp that share lane % 4 hold the same accumulator columns: sum them (fixed order); lanes 0..3 get the total
+__device__ __forceinline__ float quad_col_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 4);
+  v += __shfl_xor_sync(0xffffffffu, v, 8);
+  v += __shfl_xor_sync(0xffffffffu, v, 16);
+  return v;
+}
+
+// Persistent: each CTA walks tiles blockIdx.x, +gridDim.x, ...; the shared-memory stage ring runs across tiles, and two
+// CTAs per SM let one CTA's epilogue overlap the other's mainloop.
+// RB (FWD / DGRAD only): "resident B" -- each CTA owns ONE column tile, loads its [K x 128] slice of the weights once and
+// streams only the activation tiles; the MMAs and the epilogue are those of the streamed variant, so the results are
+// bit-identical.
+template <int MODE, bool BF16, bool RB>
+__global__ void __launch_bounds__(kGemmThreads, RB ? 1 : 2)
 dib_int16_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const Int16Args a,
-                      const __grid_constant__ CUtensorMap mapA2, const __grid_constant__ CUtensorMap mapB2, const Int16Args a2) {
+                      const __grid_constant__ CUtensorMap mapA2, const __grid_constant__ CUtensorMap mapB2, const Int16Args a2, int nkb) {
   // (a2, mapA2, mapB2): an optional SECOND weight-gradient problem walked by the same launch (a2.nsplit > 0, WGRAD only): the two
   // layers' tiles together fill one wave of CTAs, which neither fills alone
+  static_assert(!RB || MODE != DIB_GEMM_WGRAD, "resident-B variant: FWD / DGRAD only");
   constexpr bool A_MN = (MODE == DIB_GEMM_WGRAD), B_MN = (MODE != DIB_GEMM_DGRAD);
+  constexpr int S = RB ? kRbStages : kStages;
+  constexpr uint32_t kStep = RB ? kABytes : kStageBytes;          // bytes per ring stage
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sb = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* sg = smem_raw + (sb - smem_u32(smem_raw));
-  const uint32_t bar_base = sb + kBarOff;
+  const uint32_t sBres = sb, ring = RB ? sb + nkb * kBBytes : sb;  // RB: resident weight slice, then the A ring
+  const uint32_t bar_base = ring + S * kStep;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (kStages + s); };
-  auto tfull_bar = [&](int acc) { return bar_base + 8u * (2 * kStages + acc); };
-  auto tempty_bar = [&](int acc) { return bar_base + 8u * (2 * kStages + 2 + acc); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * kStages + 4);
-  volatile uint32_t* tmem_slot_g = reinterpret_cast<volatile uint32_t*>(sg + kBarOff + 8 * (2 * kStages + 4));
+  auto empty_bar = [&](int s) { return bar_base + 8u * (S + s); };
+  const uint32_t bfull_bar = bar_base + 8u * (2 * S);
 
-  __shared__ float colsum_s[4][kBN];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  __shared__ float colsum_s[kConsumers / 32][kBN];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int R0 = (MODE == DIB_GEMM_WGRAD) ? a.R : a.M, C0 = a.C;
   const int tiles_r = DIB_CEIL_DIV(R0, kBM), tiles_c = DIB_CEIL_DIV(C0, kBN);
   const int nsp = (MODE == DIB_GEMM_WGRAD) ? a.nsplit : 1;
   const int ntile0 = tiles_r * tiles_c * nsp;
   const bool two = (MODE == DIB_GEMM_WGRAD) && a2.nsplit > 0;
   const int tiles_r2 = two ? DIB_CEIL_DIV(a2.R, kBM) : 0, tiles_c2 = two ? DIB_CEIL_DIV(a2.C, kBN) : 0;
-  const int ntile = ntile0 + tiles_r2 * tiles_c2 * (two ? a2.nsplit : 0);
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&mapA); tma_prefetch_desc(&mapB);
-    if (two) { tma_prefetch_desc(&mapA2); tma_prefetch_desc(&mapB2); }
-    for (int s = 0; s < kStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    for (int acc = 0; acc < 2; ++acc) { mbar_init(tfull_bar(acc), 1); mbar_init(tempty_bar(acc), 4); }
-    fence_barrier_init();
-  }
-  if (warp == 1) { tmem_alloc(tmem_slot, 2 * kBN); tmem_relinquish(); }
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot_g;
+  const int ntile = RB ? tiles_r : ntile0 + tiles_r2 * tiles_c2 * (two ? a2.nsplit : 0);
+  // RB: this CTA's fixed column tile and its row tiles: blockIdx.x = col + tiles_c * k  (gridDim.x is a multiple of tiles_c)
+  const int rb_c0 = RB ? (blockIdx.x % tiles_c) * kBN : 0;
+  const int first = RB ? blockIdx.x / tiles_c : blockIdx.x, stride = RB ? gridDim.x / tiles_c : gridDim.x;
 
   int prob = 0;                                     // which problem the tile last decoded belongs to (per thread)
   auto decode = [&](int tile, int& r0, int& c0, int& split, int& t_begin, int& nk) {
+    if (RB) { prob = 0; split = 0; r0 = tile * kBM; c0 = rb_c0; t_begin = 0; nk = nkb; return; }
     prob = (two && tile >= ntile0) ? 1 : 0;
     if (prob) tile -= ntile0;
     const int tr = prob ? tiles_r2 : tiles_r, tcn = prob ? tiles_c2 : tiles_c;
@@ -115,635 +132,366 @@ dib_int16_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
     nk = t_end > t_begin ? DIB_CEIL_DIV(t_end - t_begin, kBK) : 0;
   };
 
-  if (warp == 0) {
-    if (lane == 0) {
-      uint32_t s = 0, ph = 0;
-      for (int tile = blockIdx.x; tile < ntile; tile += gridDim.x) {
-        int r0, c0, split, t_begin, nk;
-        decode(tile, r0, c0, split, t_begin, nk);
-        for (int k = 0; k < nk; ++k) {
-          mbar_wait(empty_bar(s), ph ^ 1);
-          mbar_expect_tx(full_bar(s), kStageBytes);
-          const uint32_t a_dst = sb + s * kStageBytes, b_dst = a_dst + kABytes;
-          const int t0 = t_begin + k * kBK;
-          const CUtensorMap* mA = prob ? &mapA2 : &mapA;
-          const CUtensorMap* mB = prob ? &mapB2 : &mapB;
-          if constexpr (A_MN) tma_load_3d(a_dst, mA, full_bar(s), 0, t0, r0 / 64);
-          else                tma_load_2d(a_dst, mA, full_bar(s), t0, r0);
-          if constexpr (B_MN) tma_load_3d(b_dst, mB, full_bar(s), 0, t0, c0 / 64);
-          else                tma_load_2d(b_dst, mB, full_bar(s), t0, c0);
-          if (++s == kStages) { s = 0; ph ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    {                                       // the whole warp runs the issue loop (uniform registers), one elected lane issues
-      constexpr uint32_t idesc = umma_idesc(BF16 ? 1u : 0u, A_MN ? 1u : 0u, B_MN ? 1u : 0u, kBN);
-      // K-major: 32 B inside the swizzle span; MN-major (16-bit, SWIZZLE_128B): 16 k-rows = 2048 B, panels 8 KB apart.
-      // Only the start-address field of the descriptors moves (stage, 16-deep k step) -- see umma_desc_lo.
-      const uint32_t a_lo0 = umma_desc_lo(sb, A_MN ? kBK * 128 : 16), b_lo0 = umma_desc_lo(sb + kABytes, B_MN ? kBK * 128 : 16);
-      const uint32_t d_hi = umma_desc_hi(1024);
-      constexpr uint32_t a_step = (A_MN ? 2048 : 32) >> 4, b_step = (B_MN ? 2048 : 32) >> 4, st_step = kStageBytes >> 4;
-      uint32_t s = 0, ph = 0, lt = 0;
-      for (int tile = blockIdx.x; tile < ntile; tile += gridDim.x) {
-        int r0, c0, split, t_begin, nk;
-        decode(tile, r0, c0, split, t_begin, nk);
-        if (nk == 0) continue;
-        const int acc = lt & 1;
-        mbar_wait(tempty_bar(acc), ((lt >> 1) & 1) ^ 1);           // the epilogue has drained this accumulator
-        tc_fence_after_sync();
-        const uint32_t d_tmem = tmem_base + acc * kBN;
-        for (int k = 0; k < nk; ++k) {
-          mbar_wait(full_bar(s), ph);
-          tc_fence_after_sync();
-          const uint32_t a_lo = a_lo0 + s * st_step, b_lo = b_lo0 + s * st_step;
-#pragma unroll
-          for (int kk = 0; kk < kBK / 16; ++kk)
-            umma_f16_w(d_tmem, umma_desc_join(a_lo + kk * a_step, d_hi), umma_desc_join(b_lo + kk * b_step, d_hi), idesc, (k > 0 || kk > 0) ? 1u : 0u);
-          umma_commit_w(empty_bar(s));
-          if (++s == kStages) { s = 0; ph ^= 1; }
-        }
-        umma_commit_w(tfull_bar(acc));
-        ++lt;
-      }
-    }
-  } else {
-    const int q = warp & 3;
-    uint32_t lt = 0;
-    for (int tile = blockIdx.x; tile < ntile; tile += gridDim.x) {
-      int r0, c0, split, t_begin, nk;
-      decode(tile, r0, c0, split, t_begin, nk);
-      const int acc = lt & 1;
-      const int r = r0 + q * 32 + lane;
-      const int R = prob ? a2.R : R0, C = prob ? a2.C : C0;
-      // the activation row that gates the gradient (DGRAD) is fetched one 32-column chunk ahead -- the first chunk before the wait
-      // for the accumulator -- so that its L2 / HBM latency never sits on the per-chunk critical path
-      uint32_t xpre[16], xnext[16];
-      auto load_x = [&](int cc, uint32_t (&dst)[16]) {
-        if (r < R && c0 + cc < C && a.X) {
-          uint32_t xa[8], xb[8];
-          dib_ld_global_v8(a.X + (long long)r * a.ldx + c0 + cc, xa);
-          dib_ld_global_v8(a.X + (long long)r * a.ldx + c0 + cc + 16, xb);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) { dst[j] = xa[j]; dst[8 + j] = xb[j]; }
-        }
-      };
-      if constexpr (MODE == DIB_GEMM_DGRAD) load_x(0, xpre);
-      if (nk > 0) { mbar_wait(tfull_bar(acc), (lt >> 1) & 1); tc_fence_after_sync(); }
-#pragma unroll 1
-      for (int cc = 0; cc < kBN; cc += 32) {
-        // the bias slice (FWD) is fetched BEFORE the TMEM load so that its latency hides under it (it sat behind
-        // tcgen05.wait::ld: 41 % of the FWD kernel's stall samples, profiles/r02_int16_ncu_full.txt)
-        const bool live = r < R && c0 + cc < C;
-        float4 bpre[8];
-        if constexpr (MODE == DIB_GEMM_FWD) {
-          if (live) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) bpre[j] = *reinterpret_cast<const float4*>(a.bias + c0 + cc + 4 * j);
-          }
-        }
-        if constexpr (MODE == DIB_GEMM_DGRAD) { if (cc + 32 < kBN) load_x(cc + 32, xnext); }
-        uint32_t v[32];
-        if (nk > 0) { tmem_ld_32x32b_x32(tmem_base + acc * kBN + ((uint32_t)(q * 32) << 16) + (uint32_t)cc, v); tmem_ld_wait(); }
-        else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = 0u;
-        }
-        if (r < R && c0 + cc < C && !(a.dbg & 1)) {          // C is a multiple of 64: a 32-column chunk is entirely inside or outside
-          const int c = c0 + cc;
-          if constexpr (MODE == DIB_GEMM_WGRAD) {
-            float* dst = (prob ? a2.out32 : a.out32) + (long long)split * a.split_stride + (long long)r * (prob ? a2.ldc : a.ldc) + c;
-#pragma unroll
-            for (int j = 0; j < 32; j += 8)
-              dib_st_global_v8(dst + j, __float_as_uint(__uint_as_float(v[j]) * a.out_scale), __float_as_uint(__uint_as_float(v[j + 1]) * a.out_scale),
-                               __float_as_uint(__uint_as_float(v[j + 2]) * a.out_scale), __float_as_uint(__uint_as_float(v[j + 3]) * a.out_scale),
-                               __float_as_uint(__uint_as_float(v[j + 4]) * a.out_scale), __float_as_uint(__uint_as_float(v[j + 5]) * a.out_scale),
-                               __float_as_uint(__uint_as_float(v[j + 6]) * a.out_scale), __float_as_uint(__uint_as_float(v[j + 7]) * a.out_scale));
-          } else {
-            uint16_t* dst = a.out16 + (long long)r * a.ldc + c;
-            uint32_t ow[16];
-            const uint16_t* xs = (MODE == DIB_GEMM_DGRAD && a.X) ? a.X + (long long)r * a.ldx + c : nullptr;
-#pragma unroll
-            for (int j = 0; j < 32; j += 8) {
-              float f[8];
-#pragma unroll
-              for (int k = 0; k < 8; ++k) f[k] = __uint_as_float(v[j + k]);
-              if constexpr (MODE == DIB_GEMM_FWD) {
-                const float4 b0 = bpre[j >> 2], b1 = bpre[(j >> 2) + 1];
-                const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-#pragma unroll
-                for (int k = 0; k < 8; ++k) f[k] = dib_act16(a.act, f[k] + bb[k], a.alpha);
-              } else if (xs) {
-                const uint32_t xw[4] = {xpre[j >> 1], xpre[(j >> 1) + 1], xpre[(j >> 1) + 2], xpre[(j >> 1) + 3]};
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                  float h0, h1;
-                  unpack_h2<BF16>(xw[k], h0, h1);
-                  f[2 * k] *= dib_act_grad(a.act, h0, a.alpha);
-                  f[2 * k + 1] *= dib_act_grad(a.act, h1, a.alpha);
-                }
-              }
-              ow[(j >> 1)] = pack_h2<BF16>(f[0], f[1]); ow[(j >> 1) + 1] = pack_h2<BF16>(f[2], f[3]);
-              ow[(j >> 1) + 2] = pack_h2<BF16>(f[4], f[5]); ow[(j >> 1) + 3] = pack_h2<BF16>(f[6], f[7]);
-              if (j & 8) dib_st_global_v8(dst + j - 8, ow[(j >> 1) - 4], ow[(j >> 1) - 3], ow[(j >> 1) - 2], ow[(j >> 1) - 1], ow[(j >> 1)], ow[(j >> 1) + 1], ow[(j >> 1) + 2], ow[(j >> 1) + 3]);
-              if constexpr (MODE == DIB_GEMM_DGRAD) {
-#pragma unroll
-                for (int k = 0; k < 8; ++k) v[j + k] = __float_as_uint(f[k]);     // keep the gated fp32 values for the column sums
-              }
-            }
-          }
-        } else if constexpr (MODE == DIB_GEMM_DGRAD) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = 0u;                                  // rows / columns outside the matrix add nothing
-        }
-        if constexpr (MODE == DIB_GEMM_DGRAD) {
-          if (a.dbias) {
-            // bias gradient of the layer below = column sums of the gradient just produced: 32 values per lane are
-            // transpose-reduced over the warp's 32 rows in 31 shuffles; lane L ends up with column L of this chunk
-            float w[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) w[j] = __uint_as_float(v[j]);
-#pragma unroll
-            for (int o = 16; o >= 1; o >>= 1) {
-#pragma unroll
-              for (int i = 0; i < o; ++i) {
-                const bool up = (lane & o) != 0;
-                const float send = up ? w[i] : w[i + o], keep = up ? w[i + o] : w[i];
-                w[i] = keep + __shfl_xor_sync(0xffffffffu, send, o);
-              }
-            }
-            colsum_s[q][cc + lane] = w[0];
-          }
-#pragma unroll
-          for (int j = 0; j < 16; ++j) xpre[j] = xnext[j];
-        }
-      }
-      if constexpr (MODE == DIB_GEMM_DGRAD) {
-        if (a.dbias) {
-          asm volatile("bar.sync 1, 128;" ::: "memory");
-          const int et = (warp - 2) * 32 + lane;               // one column of the tile per epilogue thread
-          if (c0 + et < C)
-            a.dbias[(long long)(r0 / kBM) * C + c0 + et] = (colsum_s[0][et] + colsum_s[1][et]) + (colsum_s[2][et] + colsum_s[3][et]);
-          asm volatile("bar.sync 1, 128;" ::: "memory");
-        }
-      }
-      if (nk > 0) {
-        tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(tempty_bar(acc));
-        ++lt;
-      }
-    }
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after_sync(); tmem_dealloc(tmem_base, 2 * kBN); }
-}
-
-// ====================================================================================================
-// Resident-B variant for FWD / DGRAD (the B operand is a weight matrix): with M = 65 536 rows and 128-row tiles the old
-// kernel re-fetched the [K x 128] weight tile from L2 for every one of the 512 row tiles -- at ~20 B/clk of L2
-// bandwidth per SM that traffic (not the MMAs) set the kernel time (ncu: long_scoreboard 44-57 %).  Here each persistent
-// CTA owns ONE column tile, loads its [K x BN] slice of the weights once (<= 128 KB of shared memory) and streams only
-// the activation tiles through a deeper ring; BN = 256 (full output width of the hidden layers) reads A exactly once.
-// Warp roles as above: 0 TMA producer | 1 MMA issuer (+ TMEM owner) | 2..5 epilogue.
-// ====================================================================================================
-constexpr int kRbStages = 5;
-template <int BN> constexpr int rb_tmem_cols() { return 2 * BN; }
-
-template <int MODE, bool BF16, int BN>
-__global__ void __launch_bounds__(192, 1)
-dib_int16_rb_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const Int16Args a, int nkb) {
-  static_assert(MODE != DIB_GEMM_WGRAD, "resident-B variant: FWD / DGRAD only");
-  constexpr bool B_MN = (MODE == DIB_GEMM_FWD);
-  constexpr int kBPanel = BN * 128;                    // bytes of one 64-deep k-block of the resident B slice
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t sb = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* sg = smem_raw + (sb - smem_u32(smem_raw));
-  const uint32_t sB = sb, sA = sb + nkb * kBPanel;      // resident B | A ring
-  const int bar_off = nkb * kBPanel + kRbStages * kABytes;
-  const uint32_t bar_base = sb + bar_off;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (kRbStages + s); };
-  auto tfull_bar = [&](int acc) { return bar_base + 8u * (2 * kRbStages + acc); };
-  auto tempty_bar = [&](int acc) { return bar_base + 8u * (2 * kRbStages + 2 + acc); };
-  const uint32_t bfull_bar = bar_base + 8u * (2 * kRbStages + 4);
-  const uint32_t tmem_slot = bar_base + 8u * (2 * kRbStages + 5);
-  volatile uint32_t* tmem_slot_g = reinterpret_cast<volatile uint32_t*>(sg + bar_off + 8 * (2 * kRbStages + 5));
-
-  __shared__ float colsum_s[4][BN];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int R = a.M, C = a.C;
-  const int tiles_r = DIB_CEIL_DIV(R, kBM), tiles_c = DIB_CEIL_DIV(C, BN);
-  // this CTA's fixed column tile and its row tiles: blockIdx.x = col + tiles_c * k  (gridDim.x is a multiple of tiles_c)
-  const int ctile = blockIdx.x % tiles_c, c0 = ctile * BN;
-  const int rfirst = blockIdx.x / tiles_c, rstep = gridDim.x / tiles_c;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&mapA); tma_prefetch_desc(&mapB);
-    for (int s = 0; s < kRbStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    for (int acc = 0; acc < 2; ++acc) { mbar_init(tfull_bar(acc), 1); mbar_init(tempty_bar(acc), 4); }
+  if (tid == 0) {
+    for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kEmptyArrivals); }
     mbar_init(bfull_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) { tmem_alloc(tmem_slot, rb_tmem_cols<BN>()); tmem_relinquish(); }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot_g;
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
+    // ============================================================== TMA producer (one lane)
     if (lane == 0) {
-      // the weight slice of this column tile, once
-      mbar_expect_tx(bfull_bar, (uint32_t)(nkb * kBPanel));
-      for (int k = 0; k < nkb; ++k) {
-        const uint32_t dst = sB + k * kBPanel;
-        // one box per k-block: FWD [BN/64 panels][64 k-rows][128 B] (MN-major), DGRAD [BN rows][128 B] (K-major)
-        if constexpr (B_MN) tma_load_3d(dst, &mapB, bfull_bar, 0, k * kBK, c0 / 64);
-        else                tma_load_2d(dst, &mapB, bfull_bar, k * kBK, c0);
-      }
-      uint32_t it = 0;
-      for (int rt = rfirst; rt < tiles_r; rt += rstep) {
-        for (int k = 0; k < nkb; ++k, ++it) {
-          const int s = it % kRbStages, ph = (it / kRbStages) & 1;
-          mbar_wait(empty_bar(s), ph ^ 1);
-          mbar_expect_tx(full_bar(s), kABytes);
-          tma_load_2d(sA + s * kABytes, &mapA, full_bar(s), k * kBK, rt * kBM);
+      tma_prefetch_desc(&mapA); tma_prefetch_desc(&mapB);
+      if (two) { tma_prefetch_desc(&mapA2); tma_prefetch_desc(&mapB2); }
+      if constexpr (RB) {                           // the weight slice of this column tile, once
+        mbar_expect_tx(bfull_bar, (uint32_t)(nkb * kBBytes));
+        for (int k = 0; k < nkb; ++k) {
+          // one box per k-block: FWD [2 panels][64 k-rows][128 B] (MN-major), DGRAD [128 rows][128 B] (K-major)
+          if constexpr (B_MN) tma_load_3d(sBres + k * kBBytes, &mapB, bfull_bar, 0, k * kBK, rb_c0 / 64);
+          else                tma_load_2d(sBres + k * kBBytes, &mapB, bfull_bar, k * kBK, rb_c0);
         }
       }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc(BF16 ? 1u : 0u, 0u, B_MN ? 1u : 0u, BN);
-      mbar_wait(bfull_bar, 0);
-      tc_fence_after_sync();
-      uint32_t it = 0, lt = 0;
-      for (int rt = rfirst; rt < tiles_r; rt += rstep, ++lt) {
-        const int acc = lt & 1;
-        mbar_wait(tempty_bar(acc), ((lt >> 1) & 1) ^ 1);           // the epilogue has drained this accumulator
-        tc_fence_after_sync();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int k = 0; k < nkb; ++k, ++it) {
-          const int s = it % kRbStages, ph = (it / kRbStages) & 1;
-          mbar_wait(full_bar(s), ph);
-          tc_fence_after_sync();
-          const uint32_t a_addr = sA + s * kABytes, b_addr = sB + k * kBPanel;
-#pragma unroll
-          for (int kk = 0; kk < kBK / 16; ++kk) {
-            // A K-major: 32 B inside the swizzle span.  B MN-major (FWD): 16 k-rows = 2048 B inside a [64 k x 64 n] panel,
-            // panels 8 KB apart; B K-major (DGRAD): rows = output columns, 128-row groups 16 KB apart handled by SBO = 1024.
-            const uint64_t adesc = umma_smem_desc(a_addr + kk * 32, 16, 1024);
-            const uint64_t bdesc = B_MN ? umma_smem_desc(b_addr + kk * 2048, kBK * 128, 1024) : umma_smem_desc(b_addr + kk * 32, 16, 1024);
-            umma_bf16(d_tmem, adesc, bdesc, idesc, (k > 0 || kk > 0) ? 1u : 0u);
-          }
-          umma_commit(empty_bar(s));
-        }
-        umma_commit(tfull_bar(acc));
-      }
-    }
-  } else {
-    const int q = warp & 3;
-    uint32_t lt = 0;
-    for (int rt = rfirst; rt < tiles_r; rt += rstep, ++lt) {
-      const int acc = lt & 1, r0 = rt * kBM;
-      mbar_wait(tfull_bar(acc), (lt >> 1) & 1); tc_fence_after_sync();
-      const int r = r0 + q * 32 + lane;
-#pragma unroll 1
-      for (int cc = 0; cc < BN; cc += 32) {
-        const bool live = r < R && c0 + cc < C;     // global operands of the epilogue first: their latency hides under the TMEM load
-        float4 bpre[8];
-        uint32_t xpre[16];
-        if constexpr (MODE == DIB_GEMM_FWD) {
-          if (live) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) bpre[j] = *reinterpret_cast<const float4*>(a.bias + c0 + cc + 4 * j);
-          }
-        }
-        if constexpr (MODE == DIB_GEMM_DGRAD) {
-          if (live && a.X) {
-            uint32_t xa[8], xb[8];
-            dib_ld_global_v8(a.X + (long long)r * a.ldx + c0 + cc, xa);
-            dib_ld_global_v8(a.X + (long long)r * a.ldx + c0 + cc + 16, xb);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) { xpre[j] = xa[j]; xpre[8 + j] = xb[j]; }
-          }
-        }
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem_base + acc * BN + ((uint32_t)(q * 32) << 16) + (uint32_t)cc, v);
-        tmem_ld_wait();
-        if (r < R && c0 + cc < C) {          // C is a multiple of 64: a 32-column chunk is entirely inside or outside
-          const int c = c0 + cc;
-          uint16_t* dst = a.out16 + (long long)r * a.ldc + c;
-          uint32_t ow[16];
-          const uint16_t* xs = (MODE == DIB_GEMM_DGRAD && a.X) ? a.X + (long long)r * a.ldx + c : nullptr;
-#pragma unroll
-          for (int j = 0; j < 32; j += 8) {
-            float f[8];
-#pragma unroll
-            for (int k = 0; k < 8; ++k) f[k] = __uint_as_float(v[j + k]);
-            if constexpr (MODE == DIB_GEMM_FWD) {
-              const float4 b0 = bpre[j >> 2], b1 = bpre[(j >> 2) + 1];
-              const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-#pragma unroll
-              for (int k = 0; k < 8; ++k) f[k] = dib_act16(a.act, f[k] + bb[k], a.alpha);
-            } else if (xs) {
-              const uint32_t xw[4] = {xpre[j >> 1], xpre[(j >> 1) + 1], xpre[(j >> 1) + 2], xpre[(j >> 1) + 3]};
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                float h0, h1;
-                unpack_h2<BF16>(xw[k], h0, h1);
-                f[2 * k] *= dib_act_grad(a.act, h0, a.alpha);
-                f[2 * k + 1] *= dib_act_grad(a.act, h1, a.alpha);
-              }
-            }
-            *reinterpret_cast<uint4*>(dst + j) = make_uint4(pack_h2<BF16>(f[0], f[1]), pack_h2<BF16>(f[2], f[3]), pack_h2<BF16>(f[4], f[5]), pack_h2<BF16>(f[6], f[7]));
-            if constexpr (MODE == DIB_GEMM_DGRAD) {
-#pragma unroll
-              for (int k = 0; k < 8; ++k) v[j + k] = __float_as_uint(f[k]);     // keep the gated fp32 values for the column sums
-            }
-          }
-        } else if constexpr (MODE == DIB_GEMM_DGRAD) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = 0u;                                  // rows / columns outside the matrix add nothing
-        }
-        if constexpr (MODE == DIB_GEMM_DGRAD) {
-          if (a.dbias) {
-            // bias gradient of the layer below = column sums of the gradient just produced (31-shuffle transpose-reduce)
-            float w[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) w[j] = __uint_as_float(v[j]);
-#pragma unroll
-            for (int o = 16; o >= 1; o >>= 1) {
-#pragma unroll
-              for (int i = 0; i < o; ++i) {
-                const bool up = (lane & o) != 0;
-                const float send = up ? w[i] : w[i + o], keep = up ? w[i + o] : w[i];
-                w[i] = keep + __shfl_xor_sync(0xffffffffu, send, o);
-              }
-            }
-            colsum_s[q][cc + lane] = w[0];
-          }
-        }
-      }
-      if constexpr (MODE == DIB_GEMM_DGRAD) {
-        if (a.dbias) {
-          asm volatile("bar.sync 1, 128;" ::: "memory");
-          const int et = (warp - 2) * 32 + lane;
-          for (int cidx = et; cidx < BN; cidx += 128)
-            if (c0 + cidx < C)
-              a.dbias[(long long)rt * C + c0 + cidx] = (colsum_s[0][cidx] + colsum_s[1][cidx]) + (colsum_s[2][cidx] + colsum_s[3][cidx]);
-          asm volatile("bar.sync 1, 128;" ::: "memory");
-        }
-      }
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc));
-    }
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after_sync(); tmem_dealloc(tmem_base, rb_tmem_cols<BN>()); }
-}
-
-// 32 values per lane over the warp's 32 rows -> lane L holds the column-L total (31 shuffles, fixed order)
-__device__ __forceinline__ float warp_colsum32(float (&w)[32], int lane) {
-#pragma unroll
-  for (int o = 16; o >= 1; o >>= 1) {
-#pragma unroll
-    for (int i = 0; i < o; ++i) {
-      const bool up = (lane & o) != 0;
-      const float send = up ? w[i] : w[i + o], keep = up ? w[i + o] : w[i];
-      w[i] = keep + __shfl_xor_sync(0xffffffffu, send, o);
-    }
-  }
-  return w[0];
-}
-
-// ====================================================================================================
-// CTA-pair variant (tcgen05 cta_group::2): the streamed GEMMs above move 64 FLOP per byte of L2->SM traffic with their
-// 128 x 128 tiles and run AT the L2 fabric's rate (fwd_l0: 268 MB in 32 us = 8.4 TB/s, 540 TFLOP/s).  Here two CTAs on the
-// two SMs of a TPC share one 256 x 256 output tile: each loads its own 128 rows of A and HALF of the B tile (128 of the 256
-// columns), one thread of the even CTA issues M = 256 MMAs that read both shared memories, and each CTA's TMEM receives its
-// 128 rows of the fp32 accumulator -> 128 FLOP per byte, half the traffic.  One CTA per SM, 6-stage ring of 32 KB per CTA,
-// accumulator double-buffered (2 x 256 TMEM columns), eight epilogue warps (two column halves).
-// Warp roles: 0 TMA producer (both CTAs) | 1 TMEM owner (both), MMA issuer (even CTA) | 2..9 epilogue.
-// ====================================================================================================
-constexpr int k2BN = 256, k2Stages = 6;
-constexpr int k2StageBytes = kABytes + kBBytes;
-constexpr int k2BarOff = k2Stages * k2StageBytes;
-constexpr int k2SmemTotal = k2BarOff + 256 + 1024;
-
-template <int MODE, bool BF16>
-__global__ void __launch_bounds__(320, 1)
-dib_int16_gemm2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const Int16Args a) {
-  constexpr bool A_MN = (MODE == DIB_GEMM_WGRAD), B_MN = (MODE != DIB_GEMM_DGRAD);
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t sb = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* sg = smem_raw + (sb - smem_u32(smem_raw));
-  const uint32_t bar_base = sb + k2BarOff;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (k2Stages + s); };
-  auto tfull_bar = [&](int acc) { return bar_base + 8u * (2 * k2Stages + acc); };
-  auto tempty_bar = [&](int acc) { return bar_base + 8u * (2 * k2Stages + 2 + acc); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * k2Stages + 4);
-  volatile uint32_t* tmem_slot_g = reinterpret_cast<volatile uint32_t*>(sg + k2BarOff + 8 * (2 * k2Stages + 4));
-
-  __shared__ float colsum_s[2][4][128];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int R = (MODE == DIB_GEMM_WGRAD) ? a.R : a.M, C = a.C;
-  const int tiles_rp = DIB_CEIL_DIV(R, 2 * kBM), tiles_c = DIB_CEIL_DIV(C, k2BN);
-  const int nsp = (MODE == DIB_GEMM_WGRAD) ? a.nsplit : 1;
-  const int ntile = tiles_rp * tiles_c * nsp;
-  const int cl = blockIdx.x >> 1, ncl = gridDim.x >> 1;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&mapA); tma_prefetch_desc(&mapB);
-    for (int s = 0; s < k2Stages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    for (int acc = 0; acc < 2; ++acc) { mbar_init(tfull_bar(acc), 1); mbar_init(tempty_bar(acc), 16); }
-    fence_barrier_init();
-  }
-  if (warp == 1) { tmem2_alloc(tmem_slot, 2 * k2BN); tmem2_relinquish(); }
-  tc_fence_before_sync();
-  cluster_sync_all();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot_g;
-
-  auto decode = [&](int tile, int& r0, int& c0, int& split, int& t_begin, int& nk) {
-    const int per = tiles_rp * tiles_c;
-    split = tile / per;
-    const int rem = tile - split * per;
-    r0 = (rem / tiles_c) * 2 * kBM + (int)rank * kBM; c0 = (rem % tiles_c) * k2BN;
-    int t_end;
-    if (MODE == DIB_GEMM_WGRAD) { t_begin = split * a.rows_per_split; t_end = min(a.M, t_begin + a.rows_per_split); }
-    else { t_begin = 0; t_end = a.T; }
-    nk = t_end > t_begin ? DIB_CEIL_DIV(t_end - t_begin, kBK) : 0;
-  };
-
-  if (warp == 0) {
-    if (lane == 0) {
       uint32_t s = 0, ph = 0;
-      const uint32_t fl0 = mapa_shared(full_bar(0), 0);          // the even CTA's barriers count both CTAs' bytes
-      for (int tile = cl; tile < ntile; tile += ncl) {
+      for (int tile = first; tile < ntile; tile += stride) {
         int r0, c0, split, t_begin, nk;
         decode(tile, r0, c0, split, t_begin, nk);
-        const int cb = c0 + (int)rank * kBN;                     // this CTA's half of the B tile
+        const CUtensorMap* mA = prob ? &mapA2 : &mapA;
+        const CUtensorMap* mB = prob ? &mapB2 : &mapB;
         for (int k = 0; k < nk; ++k) {
           mbar_wait(empty_bar(s), ph ^ 1);
-          if (rank == 0) mbar_expect_tx(full_bar(s), 2 * k2StageBytes);
-          const uint32_t fl = fl0 + 8u * s;
-          const uint32_t a_dst = sb + s * k2StageBytes, b_dst = a_dst + kABytes;
+          mbar_expect_tx(full_bar(s), kStep);
+          const uint32_t a_dst = ring + s * kStep, b_dst = a_dst + kABytes;
           const int t0 = t_begin + k * kBK;
-          if constexpr (A_MN) tma2_load_3d(a_dst, &mapA, fl, 0, t0, r0 / 64);
-          else                tma2_load_2d(a_dst, &mapA, fl, t0, r0);
-          if constexpr (B_MN) tma2_load_3d(b_dst, &mapB, fl, 0, t0, cb / 64);
-          else                tma2_load_2d(b_dst, &mapB, fl, t0, cb);
-          if (++s == k2Stages) { s = 0; ph ^= 1; }
+          if constexpr (A_MN) tma_load_3d(a_dst, mA, full_bar(s), 0, t0, r0 / 64);
+          else                tma_load_2d(a_dst, mA, full_bar(s), t0, r0);
+          if constexpr (!RB) {
+            if constexpr (B_MN) tma_load_3d(b_dst, mB, full_bar(s), 0, t0, c0 / 64);
+            else                tma_load_2d(b_dst, mB, full_bar(s), t0, c0);
+          }
+          if (++s == S) { s = 0; ph ^= 1; }
         }
-      }
-    }
-  } else if (warp == 1) {
-    if (rank == 0) {                       // the whole warp runs the issue loop (uniform registers), one elected lane issues
-      constexpr uint32_t idesc = umma_idesc(BF16 ? 1u : 0u, A_MN ? 1u : 0u, B_MN ? 1u : 0u, k2BN, 2 * kBM);
-      // descriptors: only the start-address field moves (stage, 16-deep k step) -- see umma_desc_lo
-      const uint32_t a_lo0 = umma_desc_lo(sb, A_MN ? kBK * 128 : 16), b_lo0 = umma_desc_lo(sb + kABytes, B_MN ? kBK * 128 : 16);
-      const uint32_t d_hi = umma_desc_hi(1024);
-      constexpr uint32_t a_step = (A_MN ? 2048 : 32) >> 4, b_step = (B_MN ? 2048 : 32) >> 4, st_step = k2StageBytes >> 4;
-      uint32_t s = 0, ph = 0, lt = 0;
-      for (int tile = cl; tile < ntile; tile += ncl) {
-        int r0, c0, split, t_begin, nk;
-        decode(tile, r0, c0, split, t_begin, nk);
-        if (nk == 0) continue;
-        const int acc = lt & 1;
-        mbar_wait(tempty_bar(acc), ((lt >> 1) & 1) ^ 1);           // both CTAs' epilogues have drained this accumulator
-        tc_fence_after_sync();
-        const uint32_t d_tmem = tmem_base + acc * k2BN;
-        for (int k = 0; k < nk; ++k) {
-          mbar_wait(full_bar(s), ph);
-          tc_fence_after_sync();
-          const uint32_t a_lo = a_lo0 + s * st_step, b_lo = b_lo0 + s * st_step;
-#pragma unroll
-          for (int kk = 0; kk < kBK / 16; ++kk)
-            umma2_f16_w(d_tmem, umma_desc_join(a_lo + kk * a_step, d_hi), umma_desc_join(b_lo + kk * b_step, d_hi), idesc, (k > 0 || kk > 0) ? 1u : 0u);
-          umma2_commit_w(empty_bar(s), 3);
-          if (++s == k2Stages) { s = 0; ph ^= 1; }
-        }
-        umma2_commit_w(tfull_bar(acc), 3);
-        ++lt;
       }
     }
   } else {
-    const int wg = (warp - 2) >> 2, wq = (warp - 2) & 3, q = warp & 3;
-    const int wcol = wg * 128;
-    uint32_t lt = 0;
-    for (int tile = cl; tile < ntile; tile += ncl) {
+    // ============================================================== consumer warpgroups: MMAs + epilogue
+    const int wg = tid >> 7, q = lane & 3;
+    const int rb = 64 * wg + 16 * (warp & 3) + (lane >> 2);       // tile row of this thread's accumulator elements
+    if constexpr (RB) mbar_wait(bfull_bar, 0);
+    uint32_t s = 0, ph = 0;
+    for (int tile = first; tile < ntile; tile += stride) {
       int r0, c0, split, t_begin, nk;
       decode(tile, r0, c0, split, t_begin, nk);
-      const int acc = lt & 1;
-      if (nk > 0) { mbar_wait(tfull_bar(acc), (lt >> 1) & 1); tc_fence_after_sync(); }
-      const int r = r0 + q * 32 + lane;
-#pragma unroll 1
-      for (int cc = wcol; cc < wcol + 128; cc += 32) {
-        const bool live = r < R && c0 + cc < C;
-        float4 bpre[8];
-        uint32_t xpre[16];
-        if constexpr (MODE == DIB_GEMM_FWD) {
-          if (live) {
+      float acc[64];
 #pragma unroll
-            for (int j = 0; j < 8; ++j) bpre[j] = *reinterpret_cast<const float4*>(a.bias + c0 + cc + 4 * j);
+      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+      if (nk > 0) {
+        uint32_t prev = 0;
+        for (int k = 0; k < nk; ++k) {
+          mbar_wait(full_bar(s), ph);
+          const uint32_t a_base = ring + s * kStep;
+          const uint32_t b_base = RB ? sBres + k * kBBytes : a_base + kABytes;
+          wgmma_fence();
+#pragma unroll
+          for (int kk = 0; kk < kBK / 16; ++kk) {
+            const uint64_t da = A_MN ? desc_mnmaj(a_base + wg * (kBK * 128), kk) : desc_kmaj(a_base + wg * 64 * 128, kk);
+            const uint64_t db = B_MN ? desc_mnmaj(b_base, kk) : desc_kmaj(b_base, kk);
+            wgmma_m64n128k16<BF16, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, (k > 0 || kk > 0) ? 1u : 0u);
           }
+          wgmma_commit();
+          wgmma_wait<1>();                                        // the previous stage's MMAs have read their operands
+          if (k > 0 && lane == 0) mbar_arrive(empty_bar(prev));
+          prev = s;
+          if (++s == S) { s = 0; ph ^= 1; }
         }
-        if constexpr (MODE == DIB_GEMM_DGRAD) {
-          if (live && a.X) {
-            uint32_t xa[8], xb[8];
-            dib_ld_global_v8(a.X + (long long)r * a.ldx + c0 + cc, xa);
-            dib_ld_global_v8(a.X + (long long)r * a.ldx + c0 + cc + 16, xb);
+        wgmma_wait<0>();
+        if (lane == 0) mbar_arrive(empty_bar(prev));
+        wgmma_fence_regs(acc);
+      }
+      // ---------------- epilogue: rows r0 + rb (+8), columns c0 + 8 j + 2 q (+1)
+      const int R = prob ? a2.R : R0, C = prob ? a2.C : C0;
+      float* const out32 = prob ? a2.out32 : a.out32;
+      const int ldc32 = prob ? a2.ldc : a.ldc;
 #pragma unroll
-            for (int j = 0; j < 8; ++j) { xpre[j] = xa[j]; xpre[8 + j] = xb[j]; }
-          }
-        }
-        uint32_t v[32];
-        if (nk > 0) { tmem_ld_32x32b_x32(tmem_base + acc * k2BN + ((uint32_t)(q * 32) << 16) + (uint32_t)cc, v); tmem_ld_wait(); }
-        else {
+      for (int j = 0; j < kBN / 8; ++j) {
+        const int c = c0 + 8 * j + 2 * q;
+        const bool cl = c < C;                              // C is even: a column pair is entirely inside or outside
+        float cs[2] = {0.f, 0.f};
+        float2 bias = make_float2(0.f, 0.f);
+        if constexpr (MODE == DIB_GEMM_FWD) { if (cl) bias = *reinterpret_cast<const float2*>(a.bias + c); }
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = 0u;
-        }
-        if (live && !(a.dbg & 1)) {
-          const int c = c0 + cc;
+        for (int h = 0; h < 2; ++h) {
+          const int r = r0 + rb + 8 * h;
+          const bool live = cl && r < R;
+          float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
           if constexpr (MODE == DIB_GEMM_WGRAD) {
-            float* dst = a.out32 + (long long)split * a.split_stride + (long long)r * a.ldc + c;
-#pragma unroll
-            for (int j = 0; j < 32; j += 8)
-              dib_st_global_v8(dst + j, __float_as_uint(__uint_as_float(v[j]) * a.out_scale), __float_as_uint(__uint_as_float(v[j + 1]) * a.out_scale),
-                               __float_as_uint(__uint_as_float(v[j + 2]) * a.out_scale), __float_as_uint(__uint_as_float(v[j + 3]) * a.out_scale),
-                               __float_as_uint(__uint_as_float(v[j + 4]) * a.out_scale), __float_as_uint(__uint_as_float(v[j + 5]) * a.out_scale),
-                               __float_as_uint(__uint_as_float(v[j + 6]) * a.out_scale), __float_as_uint(__uint_as_float(v[j + 7]) * a.out_scale));
+            if (live && !(a.dbg & 1))
+              *reinterpret_cast<float2*>(out32 + (long long)split * a.split_stride + (long long)r * ldc32 + c) =
+                  make_float2(v0 * a.out_scale, v1 * a.out_scale);
           } else {
-            uint16_t* dst = a.out16 + (long long)r * a.ldc + c;
-            uint32_t ow[16];
-            const bool gate = (MODE == DIB_GEMM_DGRAD) && a.X != nullptr;
-#pragma unroll
-            for (int j = 0; j < 32; j += 8) {
-              float f[8];
-#pragma unroll
-              for (int k = 0; k < 8; ++k) f[k] = __uint_as_float(v[j + k]);
-              if constexpr (MODE == DIB_GEMM_FWD) {
-                const float4 b0 = bpre[j >> 2], b1 = bpre[(j >> 2) + 1];
-                const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-#pragma unroll
-                for (int k = 0; k < 8; ++k) f[k] = dib_act16(a.act, f[k] + bb[k], a.alpha);
-              } else if (gate) {
-                const uint32_t xw[4] = {xpre[j >> 1], xpre[(j >> 1) + 1], xpre[(j >> 1) + 2], xpre[(j >> 1) + 3]};
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                  float h0, h1;
-                  unpack_h2<BF16>(xw[k], h0, h1);
-                  f[2 * k] *= dib_act_grad(a.act, h0, a.alpha);
-                  f[2 * k + 1] *= dib_act_grad(a.act, h1, a.alpha);
-                }
-              }
-              ow[(j >> 1)] = pack_h2<BF16>(f[0], f[1]); ow[(j >> 1) + 1] = pack_h2<BF16>(f[2], f[3]);
-              ow[(j >> 1) + 2] = pack_h2<BF16>(f[4], f[5]); ow[(j >> 1) + 3] = pack_h2<BF16>(f[6], f[7]);
-              if (j & 8) dib_st_global_v8(dst + j - 8, ow[(j >> 1) - 4], ow[(j >> 1) - 3], ow[(j >> 1) - 2], ow[(j >> 1) - 1], ow[(j >> 1)], ow[(j >> 1) + 1], ow[(j >> 1) + 2], ow[(j >> 1) + 3]);
-              if constexpr (MODE == DIB_GEMM_DGRAD) {
-#pragma unroll
-                for (int k = 0; k < 8; ++k) v[j + k] = __float_as_uint(f[k]);
-              }
+            if constexpr (MODE == DIB_GEMM_FWD) {
+              v0 = dib_act16(a.act, v0 + bias.x, a.alpha);
+              v1 = dib_act16(a.act, v1 + bias.y, a.alpha);
+            } else if (a.X) {
+              float x0 = 0.f, x1 = 0.f;
+              if (live) unpack_h2<BF16>(*reinterpret_cast<const uint32_t*>(a.X + (long long)r * a.ldx + c), x0, x1);
+              v0 *= dib_act_grad(a.act, x0, a.alpha);
+              v1 *= dib_act_grad(a.act, x1, a.alpha);
             }
+            if (live && !(a.dbg & 1)) *reinterpret_cast<uint32_t*>(a.out16 + (long long)r * a.ldc + c) = pack_h2<BF16>(v0, v1);
+            if (live) { cs[0] += v0; cs[1] += v1; }               // rows / columns outside the matrix add nothing
           }
-        } else if constexpr (MODE == DIB_GEMM_DGRAD) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = 0u;
         }
         if constexpr (MODE == DIB_GEMM_DGRAD) {
           if (a.dbias) {
-            float w[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) w[j] = __uint_as_float(v[j]);
-            colsum_s[wg][wq][cc - wcol + lane] = warp_colsum32(w, lane);
+            // bias gradient of the layer below = column sums of the gradient just produced: the warp's 16 rows here, the 8
+            // warps of the tile below
+            cs[0] = quad_col_sum(cs[0]); cs[1] = quad_col_sum(cs[1]);
+            if (lane < 4) { colsum_s[warp][8 * j + 2 * q] = cs[0]; colsum_s[warp][8 * j + 2 * q + 1] = cs[1]; }
           }
         }
       }
       if constexpr (MODE == DIB_GEMM_DGRAD) {
         if (a.dbias) {
-          if (wg == 0) asm volatile("bar.sync 1, 128;" ::: "memory"); else asm volatile("bar.sync 2, 128;" ::: "memory");
-          const int et = wq * 32 + lane;
-          if (r0 < R && c0 + wcol + et < C)
-            a.dbias[(long long)(r0 / kBM) * C + c0 + wcol + et] = (colsum_s[wg][0][et] + colsum_s[wg][1][et]) + (colsum_s[wg][2][et] + colsum_s[wg][3][et]);
-          if (wg == 0) asm volatile("bar.sync 1, 128;" ::: "memory"); else asm volatile("bar.sync 2, 128;" ::: "memory");
+          named_bar_sync(1, kConsumers);
+          if (tid < kBN && c0 + tid < C) {
+            float sum = 0.f;
+#pragma unroll
+            for (int w = 0; w < kConsumers / 32; ++w) sum += colsum_s[w][tid];
+            a.dbias[(long long)(r0 / kBM) * C + c0 + tid] = sum;
+          }
+          named_bar_sync(1, kConsumers);
         }
-      }
-      if (nk > 0) {
-        tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_cluster(mapa_shared(tempty_bar(acc), 0));
-        ++lt;
       }
     }
   }
-  tc_fence_before_sync();
-  cluster_sync_all();
-  if (warp == 1) { tc_fence_after_sync(); tmem2_dealloc(tmem_base, 2 * k2BN); }
+}
+
+// ====================================================================================================
+// Fused tail of the integration network for single-output models (C0, nb-radial): the last two hidden layers
+// (256 wide each) and the output head in ONE persistent kernel -- models.py:81-84,122 + the compiled loss.
+//   per 128-row tile:  L0  D0 = A W0   (A, W0 k-blocks streamed through a TMA ring; N = 256, fp32 in registers)
+//                      e0  g1 = act(D0 + b0) -> 16-bit -> swizzled shared tile (= L1's A operand) and -> HBM (the backward needs it)
+//                      L1  D1 = g1 W1  (W1 k-blocks through the same ring)
+//                      e1  g2 = act(D1 + b1) kept PACKED IN REGISTERS, logit = g2 . w + b, compiled loss / metric,
+//                          d loss / d logit, dg2 = dz w act'(g2) -> HBM, output-layer weight / bias gradients and the bias gradient
+//                          of the last hidden layer as per-CTA partials.
+// g2 never reaches HBM, and the head's re-read of it (and its launch) disappears.  A warp owns 16 whole rows of the
+// accumulator, so each row's logit is complete after a reduction over the 4 lanes that share the row.
+// ====================================================================================================
+constexpr int kF2N = 256, kF2Stages = 2;
+constexpr int kF2AB = kBM * 128, kF2BB = kF2N * 128, kF2Stage = kF2AB + kF2BB;      // 16 KB + 32 KB
+constexpr int kF2G1Off = kF2Stages * kF2Stage;
+constexpr int kF2BarOff = kF2G1Off + kBM * kF2N * 2;
+constexpr int kF2Smem = kF2BarOff + 64 + 1024;
+
+struct Fwd2Args {
+  const float *b0, *b1, *wout, *bout;
+  uint16_t* g1; int ldg1;             // out: first fused layer's activation [M x 256]
+  uint16_t* dg2; int lddg;            // out (training) or null: gradient w.r.t. the second fused layer's pre-activation, x gscale
+  const float* y; float* user_pred;
+  float* wpart; int wpart_stride; float *loss_part, *acc_part;
+  int M, nk0, act, out_act, loss;
+  float alpha, inv_batch, gscale;
+};
+
+// ACT is a template parameter: the activation switch inside the fully unrolled register-resident passes would otherwise be
+// evaluated per element.
+constexpr int kF2Threads = kConsumers + 128;      // + a producer warpgroup, so that setmaxnreg can move its registers to the consumers
+template <bool BF16, int ACT>
+__global__ void __launch_bounds__(kF2Threads, 1)
+dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapW0,
+                      const __grid_constant__ CUtensorMap mapW1, const Fwd2Args a) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t sb = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t bar_base = sb + kF2BarOff;
+  auto full_bar = [&](int s) { return bar_base + 8u * s; };
+  auto empty_bar = [&](int s) { return bar_base + 8u * (kF2Stages + s); };
+  const uint32_t g1s = sb + kF2G1Off;
+
+  __shared__ __align__(16) float s_b0[kF2N], s_b1[kF2N], s_w[kF2N];
+  __shared__ float s_colw[kConsumers / 32][kF2N], s_colb[kConsumers / 32][kF2N];
+  __shared__ float s_red[3][kConsumers / 32];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int ntile = DIB_CEIL_DIV(a.M, kBM);
+
+  for (int i = tid; i < kF2N; i += blockDim.x) { s_b0[i] = a.b0[i]; s_b1[i] = a.b1[i]; s_w[i] = a.wout[i]; }
+  if (tid == 0) {
+    for (int s = 0; s < kF2Stages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kEmptyArrivals); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp >= kProducerWarp) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp == kProducerWarp && lane == 0) {
+      tma_prefetch_desc(&mapA); tma_prefetch_desc(&mapW0); tma_prefetch_desc(&mapW1);
+      uint32_t s = 0, ph = 0;
+      for (int tile = blockIdx.x; tile < ntile; tile += gridDim.x) {
+        for (int k = 0; k < a.nk0; ++k) {
+          mbar_wait(empty_bar(s), ph ^ 1);
+          mbar_expect_tx(full_bar(s), kF2Stage);
+          const uint32_t dst = sb + s * kF2Stage;
+          tma_load_2d(dst, &mapA, full_bar(s), k * kBK, tile * kBM);
+          tma_load_3d(dst + kF2AB, &mapW0, full_bar(s), 0, k * kBK, 0);
+          if (++s == kF2Stages) { s = 0; ph ^= 1; }
+        }
+        for (int k = 0; k < kF2N / kBK; ++k) {
+          mbar_wait(empty_bar(s), ph ^ 1);
+          mbar_expect_tx(full_bar(s), kF2BB);
+          tma_load_3d(sb + s * kF2Stage + kF2AB, &mapW1, full_bar(s), 0, k * kBK, 0);
+          if (++s == kF2Stages) { s = 0; ph ^= 1; }
+        }
+      }
+    }
+    return;
+  }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");   // 128 x 40 + 256 x 232 <= 64 K registers
+
+  const int wg = tid >> 7, q = lane & 3;
+  const int rb = 64 * wg + 16 * (warp & 3) + (lane >> 2);
+  const bool train = a.dg2 != nullptr;
+  const float bout = a.bout[0];
+  float acc_dw = 0.f, acc_dbh = 0.f, lsum = 0.f, asum = 0.f, dbo = 0.f;     // column accumulators: column tid
+  uint32_t s = 0, ph = 0;
+  // one k-loop of m64n256k16 MMAs over `nk` ring stages; A from the ring (a_ring) or the shared g1 tile
+  auto mainloop = [&](float (&acc)[128], int nk, bool a_ring) {
+    uint32_t prev = 0;
+    for (int k = 0; k < nk; ++k) {
+      mbar_wait(full_bar(s), ph);
+      const uint32_t st = sb + s * kF2Stage;
+      const uint32_t a_base = a_ring ? st + wg * 64 * 128 : g1s + k * kF2AB + wg * 64 * 128;
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < kBK / 16; ++kk)
+        wgmma_m64n256k16<BF16, 0, 1>(acc, desc_kmaj(a_base, kk), desc_mnmaj(st + kF2AB, kk), (k > 0 || kk > 0) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (k > 0 && lane == 0) mbar_arrive(empty_bar(prev));
+      prev = s;
+      if (++s == kF2Stages) { s = 0; ph ^= 1; }
+    }
+    wgmma_wait<0>();
+    if (lane == 0) mbar_arrive(empty_bar(prev));
+    wgmma_fence_regs(acc);
+  };
+
+  for (int tile = blockIdx.x; tile < ntile; tile += gridDim.x) {
+    const long long row_lo = (long long)tile * kBM + rb;
+    float acc[128];
+#pragma unroll
+    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+    // ---------------- L0, e0: g1 = act(D0 + b0) -> shared tile (L1's A operand) and HBM
+    mainloop(acc, a.nk0, true);
+#pragma unroll
+    for (int j = 0; j < kF2N / 8; ++j) {
+      const int c = 8 * j + 2 * q;
+      const float2 bv = *reinterpret_cast<const float2*>(&s_b0[c]);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = rb + 8 * h;
+        const uint32_t w = pack_h2<BF16>(dib_act16(ACT, acc[4 * j + 2 * h] + bv.x, a.alpha), dib_act16(ACT, acc[4 * j + 2 * h + 1] + bv.y, a.alpha));
+        st_shared_b32(g1s + (c >> 6) * kF2AB + r * 128 + ((((c & 63) >> 3) ^ (r & 7)) << 4) + 4 * q, w);
+        if (row_lo + 8 * h < a.M) *reinterpret_cast<uint32_t*>(a.g1 + (row_lo + 8 * h) * a.ldg1 + c) = w;
+      }
+    }
+    fence_proxy_async_smem();
+    named_bar_sync(2 + wg, 128);                     // this warpgroup's rows of g1 are complete
+    // ---------------- L1, e1 pass 1: g2 = act(D1 + b1) packed into registers, partial logits
+#pragma unroll
+    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+    mainloop(acc, kF2N / kBK, false);
+    uint32_t g2p[64];
+    float zp[2] = {0.f, 0.f};
+#pragma unroll
+    for (int j = 0; j < kF2N / 8; ++j) {
+      const int c = 8 * j + 2 * q;
+      const float2 bv = *reinterpret_cast<const float2*>(&s_b1[c]), wv = *reinterpret_cast<const float2*>(&s_w[c]);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t p = pack_h2<BF16>(dib_act16(ACT, acc[4 * j + 2 * h] + bv.x, a.alpha), dib_act16(ACT, acc[4 * j + 2 * h + 1] + bv.y, a.alpha));
+        g2p[2 * j + h] = p;
+        float h0, h1;
+        unpack_h2<BF16>(p, h0, h1);
+        zp[h] = fmaf(h0, wv.x, zp[h]); zp[h] = fmaf(h1, wv.y, zp[h]);
+      }
+    }
+    // ---------------- logit, compiled loss / metric, d loss / d logit (the 4 lanes of a row compute it; lane q = 0 accumulates)
+    float dzs[2], ds[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      zp[h] += __shfl_xor_sync(0xffffffffu, zp[h], 1);
+      zp[h] += __shfl_xor_sync(0xffffffffu, zp[h], 2);
+      const long long row = row_lo + 8 * h;
+      const bool live = row < a.M;
+      const float z = dib_act(a.out_act, zp[h] + bout, a.alpha);
+      float dz = 0.f;
+      if (live && a.y) {
+        const float t = a.y[row];
+        float l;
+        if (a.loss == DIB_LOSS_BCE_LOGITS) { l = fmaxf(z, 0.f) - z * t + log1pf(expf(-fabsf(z))); dz = 1.f / (1.f + expf(-z)) - t; }
+        else if (a.loss == DIB_LOSS_BCE_PROBS) {
+          const float ep = 1e-7f, pc = fminf(fmaxf(z, ep), 1.f - ep);
+          l = -(t * logf(pc + ep) + (1.f - t) * logf(1.f - pc + ep));
+          dz = (z > ep && z < 1.f - ep) ? -t / (pc + ep) + (1.f - t) / (1.f - pc + ep) : 0.f;
+        } else if (a.loss == DIB_LOSS_SPARSE_CE_LOGITS) { l = 0.f; dz = 0.f; }        // one class: the softmax is constant
+        else { const float d = z - t; l = d * d; dz = 2.f * d; }
+        const float acc1 = a.loss == DIB_LOSS_SPARSE_CE_LOGITS ? ((int)t == 0 ? 1.f : 0.f) : (((z > 0.5f ? 1.f : 0.f) == t) ? 1.f : 0.f);
+        if (q == 0) { lsum += l; asum += acc1; }
+      }
+      if (a.user_pred && live && q == 0) a.user_pred[row] = z;
+      dzs[h] = live ? dz * a.inv_batch * dib_act_grad(a.out_act, z, a.alpha) : 0.f;
+      ds[h] = dzs[h] * a.gscale;
+      if (q == 0) dbo += dzs[h];
+    }
+    if (train) {
+      // ---------------- e1, pass 2: dg2 = ds w act'(g2) -> HBM; column sums of g2 dz (output-layer dW) and of dg2 (bias gradient)
+#pragma unroll
+      for (int j = 0; j < kF2N / 8; ++j) {
+        const int c = 8 * j + 2 * q;
+        const float2 wv = *reinterpret_cast<const float2*>(&s_w[c]);
+        float cw[2] = {0.f, 0.f}, cb[2] = {0.f, 0.f};
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float h0, h1;
+          unpack_h2<BF16>(g2p[2 * j + h], h0, h1);
+          const float d0 = ds[h] * wv.x * dib_act_grad(ACT, h0, a.alpha), d1 = ds[h] * wv.y * dib_act_grad(ACT, h1, a.alpha);
+          cw[0] += h0 * dzs[h]; cw[1] += h1 * dzs[h];
+          cb[0] += d0; cb[1] += d1;
+          if (row_lo + 8 * h < a.M) *reinterpret_cast<uint32_t*>(a.dg2 + (row_lo + 8 * h) * a.lddg + c) = pack_h2<BF16>(d0, d1);
+        }
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          cw[k] = quad_col_sum(cw[k]);
+          cb[k] = quad_col_sum(cb[k]);
+        }
+        if (lane < 4) {
+          s_colw[warp][c] = cw[0]; s_colw[warp][c + 1] = cw[1];
+          s_colb[warp][c] = cb[0]; s_colb[warp][c + 1] = cb[1];
+        }
+      }
+      // the 8 warps cover the tile's 128 rows: fixed-order combine into the thread-owned column
+      named_bar_sync(1, kConsumers);
+#pragma unroll
+      for (int w = 0; w < kConsumers / 32; ++w) { acc_dw += s_colw[w][tid]; acc_dbh += s_colb[w][tid]; }
+      named_bar_sync(1, kConsumers);
+    }
+  }
+  // ---------------- per-CTA partials, layout of the head kernels: [dWc (K) | dbc (1) | column sums of dg2 (K)], loss, accuracy
+  if (train) {
+    a.wpart[(long long)blockIdx.x * a.wpart_stride + tid] = acc_dw;
+    a.wpart[(long long)blockIdx.x * a.wpart_stride + kF2N + 1 + tid] = acc_dbh;
+  }
+  lsum = dib_warp_sum(lsum); asum = dib_warp_sum(asum); dbo = dib_warp_sum(dbo);
+  if (lane == 0) { s_red[0][warp] = lsum; s_red[1][warp] = asum; s_red[2][warp] = dbo; }
+  named_bar_sync(1, kConsumers);
+  if (tid == 0) {
+    float l = 0.f, ac = 0.f, b = 0.f;
+    for (int w = 0; w < kConsumers / 32; ++w) { l += s_red[0][w]; ac += s_red[1][w]; b += s_red[2][w]; }
+    a.loss_part[blockIdx.x] = l;
+    a.acc_part[blockIdx.x] = ac;
+    if (train) a.wpart[(long long)blockIdx.x * a.wpart_stride + kF2N] = b;
+  }
 }
 
 // ----------------------------------------------------------------------------------------------------
@@ -1047,283 +795,6 @@ dib_int16_head1_kernel(const uint16_t* __restrict__ g, int ldg, int K, const flo
   if (threadIdx.x == 0) { float a = 0.f; for (int ww = 0; ww < kHeadWarps; ++ww) a += sred[ww]; acc_part[blockIdx.x] = a; }
 }
 
-// ====================================================================================================
-// Fused tail of the integration network for single-output models (C0, nb-radial): the last two hidden layers
-// (256 wide each) and the output head in ONE persistent kernel -- models.py:81-84,122 + the compiled loss.
-//   per 128-row tile:  L0  D0 = A W0   (A, W0 k-blocks streamed through a 3-stage TMA ring; N = 256, fp32 in TMEM cols 0..255)
-//                      e0  g1 = act(D0 + b0) -> 16-bit -> swizzled shared tile (= L1's A operand) and -> HBM (the backward needs it)
-//                      L1  D1 = g1 W1  (W1 k-blocks through the same ring; TMEM cols 256..511), started per 64-column chunk of g1
-//                      e1  g2 = act(D1 + b1) kept PACKED IN REGISTERS (64 per thread), logit = g2 . w + b, compiled loss / metric,
-//                          d loss / d logit, dg2 = dz w act'(g2) -> HBM, output-layer weight / bias gradients and the bias gradient
-//                          of the last hidden layer as per-CTA partials.
-// g2 never reaches HBM, the head's re-read of it (and its launch) disappears, and L0 of tile i+1 runs under e1 of tile i.
-// Warp roles: 0 TMA producer | 1 MMA issuer (+ TMEM owner) | 2..5 epilogue columns 0..127 | 6..9 epilogue columns 128..255.
-// ====================================================================================================
-constexpr int kF2N = 256, kF2Stages = 3;
-constexpr int kF2AB = kBM * 128, kF2BB = kF2N * 128, kF2Stage = kF2AB + kF2BB;      // 16 KB + 32 KB
-constexpr int kF2G1Off = kF2Stages * kF2Stage;
-constexpr int kF2BarOff = kF2G1Off + kBM * kF2N * 2;
-constexpr int kF2Smem = kF2BarOff + 256 + 1024;
-
-struct Fwd2Args {
-  const float *b0, *b1, *wout, *bout;
-  uint16_t* g1; int ldg1;             // out: first fused layer's activation [M x 256]
-  uint16_t* dg2; int lddg;            // out (training) or null: gradient w.r.t. the second fused layer's pre-activation, x gscale
-  const float* y; float* user_pred;
-  float* wpart; int wpart_stride; float *loss_part, *acc_part;
-  int M, nk0, act, out_act, loss;
-  float alpha, inv_batch, gscale;
-};
-
-__device__ __forceinline__ void st_shared_v4u(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-
-// ACT is a template parameter: with the activation switch inside the fully unrolled register-resident passes the kernel grew to
-// 14.5 K SASS instructions (232 KB, jump tables per element) and ran instruction-fetch bound (ncu: no_instructions 37 % of samples).
-template <bool BF16, int ACT>
-__global__ void __launch_bounds__(320, 1)
-dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapW0,
-                      const __grid_constant__ CUtensorMap mapW1, const Fwd2Args a) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t sb = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* sg = smem_raw + (sb - smem_u32(smem_raw));
-  const uint32_t bar_base = sb + kF2BarOff;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (kF2Stages + s); };
-  const uint32_t d0_full = bar_base + 8u * (2 * kF2Stages), d1_full = d0_full + 8u, d1_empty = d0_full + 16u;
-  auto g1_ready = [&](int k) { return d0_full + 24u + 8u * k; };
-  const uint32_t tmem_slot = d0_full + 24u + 32u;
-  volatile uint32_t* tmem_slot_g = reinterpret_cast<volatile uint32_t*>(sg + kF2BarOff + 8 * (2 * kF2Stages) + 56);
-
-  __shared__ __align__(16) float s_b0[kF2N], s_b1[kF2N], s_w[kF2N];
-  __shared__ float s_z[2][2][kBM];
-  __shared__ float s_col[2][2][4][128];
-  __shared__ float s_red[3][4];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int ntile = DIB_CEIL_DIV(a.M, kBM);
-
-  for (int i = threadIdx.x; i < kF2N; i += blockDim.x) { s_b0[i] = a.b0[i]; s_b1[i] = a.b1[i]; s_w[i] = a.wout[i]; }
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&mapA); tma_prefetch_desc(&mapW0); tma_prefetch_desc(&mapW1);
-    for (int s = 0; s < kF2Stages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    mbar_init(d0_full, 1); mbar_init(d1_full, 1); mbar_init(d1_empty, 8);
-    for (int k = 0; k < 4; ++k) mbar_init(g1_ready(k), 4);
-    fence_barrier_init();
-  }
-  if (warp == 1) { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot_g;
-  const uint32_t g1s = sb + kF2G1Off;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      uint32_t s = 0, ph = 0;
-      for (int tile = blockIdx.x; tile < ntile; tile += gridDim.x) {
-        for (int k = 0; k < a.nk0; ++k) {
-          mbar_wait(empty_bar(s), ph ^ 1);
-          mbar_expect_tx(full_bar(s), kF2Stage);
-          const uint32_t dst = sb + s * kF2Stage;
-          tma_load_2d(dst, &mapA, full_bar(s), k * kBK, tile * kBM);
-          tma_load_3d(dst + kF2AB, &mapW0, full_bar(s), 0, k * kBK, 0);
-          if (++s == kF2Stages) { s = 0; ph ^= 1; }
-        }
-        for (int k = 0; k < kF2N / kBK; ++k) {
-          mbar_wait(empty_bar(s), ph ^ 1);
-          mbar_expect_tx(full_bar(s), kF2BB);
-          tma_load_3d(sb + s * kF2Stage + kF2AB, &mapW1, full_bar(s), 0, k * kBK, 0);
-          if (++s == kF2Stages) { s = 0; ph ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    {                                       // the whole warp runs the issue loop (uniform registers), one elected lane issues
-      constexpr uint32_t idesc = umma_idesc(BF16 ? 1u : 0u, 0u, 1u, kF2N);
-      // descriptors: only the start-address field moves (stage, 16-deep k step) -- see umma_desc_lo
-      const uint32_t a_lo0 = umma_desc_lo(sb, 16), b_lo0 = umma_desc_lo(sb + kF2AB, kBK * 128), g_lo0 = umma_desc_lo(g1s, 16);
-      const uint32_t d_hi = umma_desc_hi(1024);
-      constexpr uint32_t st_step = kF2Stage >> 4;
-      uint32_t s = 0, ph = 0, lt = 0;
-      for (int tile = blockIdx.x; tile < ntile; tile += gridDim.x, ++lt) {
-        // L0 -> D0.  D0 was drained by e0 of the previous tile: L1 of that tile (already issued) waited for all g1 chunks.
-        for (int k = 0; k < a.nk0; ++k) {
-          mbar_wait(full_bar(s), ph);
-          tc_fence_after_sync();
-          const uint32_t a_lo = a_lo0 + s * st_step, b_lo = b_lo0 + s * st_step;
-#pragma unroll
-          for (int kk = 0; kk < kBK / 16; ++kk)
-            umma_f16_w(tmem_base, umma_desc_join(a_lo + kk * 2, d_hi), umma_desc_join(b_lo + kk * 128, d_hi), idesc, (k > 0 || kk > 0) ? 1u : 0u);
-          umma_commit_w(empty_bar(s));
-          if (++s == kF2Stages) { s = 0; ph ^= 1; }
-        }
-        umma_commit_w(d0_full);
-        // L1 -> D1, k-block by k-block as e0 finishes the 64-column chunks of g1
-        mbar_wait(d1_empty, (lt & 1) ^ 1);
-        tc_fence_after_sync();
-#pragma unroll
-        for (int k = 0; k < kF2N / kBK; ++k) {
-          mbar_wait(g1_ready(k), lt & 1);
-          mbar_wait(full_bar(s), ph);
-          tc_fence_after_sync();
-          const uint32_t a_lo = g_lo0 + k * (kF2AB >> 4), b_lo = b_lo0 + s * st_step;
-#pragma unroll
-          for (int kk = 0; kk < kBK / 16; ++kk)
-            umma_f16_w(tmem_base + kF2N, umma_desc_join(a_lo + kk * 2, d_hi), umma_desc_join(b_lo + kk * 128, d_hi), idesc, (k > 0 || kk > 0) ? 1u : 0u);
-          umma_commit_w(empty_bar(s));
-          if (++s == kF2Stages) { s = 0; ph ^= 1; }
-        }
-        umma_commit_w(d1_full);
-      }
-    }
-  } else {
-    const int wg = (warp - 2) >> 2, wq = (warp - 2) & 3, q = warp & 3;       // TMEM lane quarter = warp id % 4
-    const int colbase = wg * 128, rt = q * 32 + lane;
-    const uint32_t lane_off = (uint32_t)(q * 32) << 16;
-    const bool train = a.dg2 != nullptr;
-    const float bout = a.bout[0];
-    float acc_dw = 0.f, acc_dbh = 0.f, lsum = 0.f, asum = 0.f, dbo = 0.f;     // column accumulators: column colbase + wq * 32 + lane
-    uint32_t lt = 0;
-    for (int tile = blockIdx.x; tile < ntile; tile += gridDim.x, ++lt) {
-      const long long row = (long long)tile * kBM + rt;
-      const bool live = row < a.M;
-      // ---------------- e0: g1 = act(D0 + b0)
-      mbar_wait(d0_full, lt & 1);
-      tc_fence_after_sync();
-#pragma unroll 1
-      for (int j = 0; j < 4; ++j) {
-        const int cc = colbase + 32 * j;
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem_base + lane_off + (uint32_t)cc, v);
-        tmem_ld_wait();
-        uint32_t q0 = 0, q1 = 0, q2 = 0, q3 = 0;
-#pragma unroll
-        for (int g = 0; g < 32; g += 8) {
-          const float4 ba = *reinterpret_cast<const float4*>(&s_b0[cc + g]), bb = *reinterpret_cast<const float4*>(&s_b0[cc + g + 4]);
-          const float bv[8] = {ba.x, ba.y, ba.z, ba.w, bb.x, bb.y, bb.z, bb.w};
-          float f[8];
-#pragma unroll
-          for (int k = 0; k < 8; ++k) f[k] = dib_act16(ACT, __uint_as_float(v[g + k]) + bv[k], a.alpha);
-          const uint32_t p0 = pack_h2<BF16>(f[0], f[1]), p1 = pack_h2<BF16>(f[2], f[3]), p2 = pack_h2<BF16>(f[4], f[5]), p3 = pack_h2<BF16>(f[6], f[7]);
-          const int c = cc + g;
-          st_shared_v4u(g1s + (c >> 6) * kF2AB + rt * 128 + ((((c & 63) >> 3) ^ (rt & 7)) << 4), p0, p1, p2, p3);
-          if (g & 8) { if (live) dib_st_global_v8(a.g1 + row * a.ldg1 + c - 8, q0, q1, q2, q3, p0, p1, p2, p3); }
-          else { q0 = p0; q1 = p1; q2 = p2; q3 = p3; }
-        }
-        if (j & 1) {                       // a 64-column chunk of g1 (one k-block of L1) is complete for this warp's rows
-          fence_proxy_async_smem();
-          tc_fence_before_sync();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(g1_ready(wg * 2 + (j >> 1)));
-        }
-      }
-      // ---------------- e1, pass 1: g2 = act(D1 + b1) packed into registers, partial logit
-      mbar_wait(d1_full, lt & 1);
-      tc_fence_after_sync();
-      uint32_t g2p[64];
-      float zp = 0.f;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int cc = colbase + 32 * j;
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem_base + lane_off + (uint32_t)(kF2N + cc), v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int g = 0; g < 32; g += 4) {
-          const float4 bv = *reinterpret_cast<const float4*>(&s_b1[cc + g]), wv = *reinterpret_cast<const float4*>(&s_w[cc + g]);
-          const uint32_t pa = pack_h2<BF16>(dib_act16(ACT, __uint_as_float(v[g]) + bv.x, a.alpha), dib_act16(ACT, __uint_as_float(v[g + 1]) + bv.y, a.alpha));
-          const uint32_t pb = pack_h2<BF16>(dib_act16(ACT, __uint_as_float(v[g + 2]) + bv.z, a.alpha), dib_act16(ACT, __uint_as_float(v[g + 3]) + bv.w, a.alpha));
-          g2p[j * 16 + (g >> 1)] = pa; g2p[j * 16 + (g >> 1) + 1] = pb;
-          float h0, h1, h2, h3;
-          unpack_h2<BF16>(pa, h0, h1); unpack_h2<BF16>(pb, h2, h3);
-          zp = fmaf(h0, wv.x, zp); zp = fmaf(h1, wv.y, zp); zp = fmaf(h2, wv.z, zp); zp = fmaf(h3, wv.w, zp);
-        }
-      }
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(d1_empty);
-      // ---------------- logit, compiled loss / metric, d loss / d logit (both column halves compute it; half 0 accumulates)
-      s_z[lt & 1][wg][rt] = zp;
-      asm volatile("bar.sync 3, 256;" ::: "memory");
-      float z = dib_act(a.out_act, (s_z[lt & 1][0][rt] + s_z[lt & 1][1][rt]) + bout, a.alpha);
-      float dz = 0.f;
-      if (live && a.y) {
-        const float t = a.y[row];
-        float l;
-        if (a.loss == DIB_LOSS_BCE_LOGITS) { l = fmaxf(z, 0.f) - z * t + log1pf(expf(-fabsf(z))); dz = 1.f / (1.f + expf(-z)) - t; }
-        else if (a.loss == DIB_LOSS_BCE_PROBS) {
-          const float ep = 1e-7f, pc = fminf(fmaxf(z, ep), 1.f - ep);
-          l = -(t * logf(pc + ep) + (1.f - t) * logf(1.f - pc + ep));
-          dz = (z > ep && z < 1.f - ep) ? -t / (pc + ep) + (1.f - t) / (1.f - pc + ep) : 0.f;
-        } else if (a.loss == DIB_LOSS_SPARSE_CE_LOGITS) { l = 0.f; dz = 0.f; }        // one class: the softmax is constant
-        else { const float d = z - t; l = d * d; dz = 2.f * d; }
-        const float acc = a.loss == DIB_LOSS_SPARSE_CE_LOGITS ? ((int)t == 0 ? 1.f : 0.f) : (((z > 0.5f ? 1.f : 0.f) == t) ? 1.f : 0.f);
-        if (wg == 0) { lsum += l; asum += acc; }
-      }
-      if (a.user_pred && live && wg == 0) a.user_pred[row] = z;
-      if (train) {
-        const float dzs = live ? dz * a.inv_batch * dib_act_grad(a.out_act, z, a.alpha) : 0.f;
-        const float ds = dzs * a.gscale;
-        if (wg == 0) dbo += dzs;
-        // ---------------- e1, pass 2: dg2 = ds w act'(g2) -> HBM; column sums of g2 dz (output-layer dW) and of dg2 (bias gradient)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int cc = colbase + 32 * j;
-          float wa[32], wb[32];
-          uint32_t dq[4] = {0u, 0u, 0u, 0u};
-#pragma unroll
-          for (int g = 0; g < 32; g += 8) {
-            const float4 w0 = *reinterpret_cast<const float4*>(&s_w[cc + g]), w1 = *reinterpret_cast<const float4*>(&s_w[cc + g + 4]);
-            const float wv[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
-            float d[8];
-#pragma unroll
-            for (int k = 0; k < 8; k += 2) {
-              float h0, h1;
-              unpack_h2<BF16>(g2p[j * 16 + ((g + k) >> 1)], h0, h1);
-              wa[g + k] = h0 * dzs; wa[g + k + 1] = h1 * dzs;
-              d[k] = ds * wv[k] * dib_act_grad(ACT, h0, a.alpha);
-              d[k + 1] = ds * wv[k + 1] * dib_act_grad(ACT, h1, a.alpha);
-              wb[g + k] = d[k]; wb[g + k + 1] = d[k + 1];
-            }
-            const uint32_t e0 = pack_h2<BF16>(d[0], d[1]), e1 = pack_h2<BF16>(d[2], d[3]), e2 = pack_h2<BF16>(d[4], d[5]), e3 = pack_h2<BF16>(d[6], d[7]);
-            if (g & 8) { if (live) dib_st_global_v8(a.dg2 + row * a.lddg + cc + g - 8, dq[0], dq[1], dq[2], dq[3], e0, e1, e2, e3); }
-            else { dq[0] = e0; dq[1] = e1; dq[2] = e2; dq[3] = e3; }
-          }
-          const float ca = warp_colsum32(wa, lane), cb = warp_colsum32(wb, lane);
-          s_col[wg][0][wq][32 * j + lane] = ca;
-          s_col[wg][1][wq][32 * j + lane] = cb;
-        }
-        // the four warps of this column half cover the tile's 128 rows: fixed-order combine into the thread-owned column
-        if (wg == 0) asm volatile("bar.sync 1, 128;" ::: "memory"); else asm volatile("bar.sync 2, 128;" ::: "memory");
-        const int t = wq * 32 + lane;
-        acc_dw += (s_col[wg][0][0][t] + s_col[wg][0][1][t]) + (s_col[wg][0][2][t] + s_col[wg][0][3][t]);
-        acc_dbh += (s_col[wg][1][0][t] + s_col[wg][1][1][t]) + (s_col[wg][1][2][t] + s_col[wg][1][3][t]);
-        if (wg == 0) asm volatile("bar.sync 1, 128;" ::: "memory"); else asm volatile("bar.sync 2, 128;" ::: "memory");
-      }
-    }
-    // ---------------- per-CTA partials, layout of the head kernels: [dWc (K) | dbc (1) | column sums of dg2 (K)], loss, accuracy
-    const int t = colbase + wq * 32 + lane;
-    if (train) {
-      a.wpart[(long long)blockIdx.x * a.wpart_stride + t] = acc_dw;
-      a.wpart[(long long)blockIdx.x * a.wpart_stride + kF2N + 1 + t] = acc_dbh;
-    }
-    if (wg == 0) {
-      lsum = dib_warp_sum(lsum); asum = dib_warp_sum(asum); dbo = dib_warp_sum(dbo);
-      if (lane == 0) { s_red[0][wq] = lsum; s_red[1][wq] = asum; s_red[2][wq] = dbo; }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (wq == 0 && lane == 0) {
-        a.loss_part[blockIdx.x] = (s_red[0][0] + s_red[0][1]) + (s_red[0][2] + s_red[0][3]);
-        a.acc_part[blockIdx.x] = (s_red[1][0] + s_red[1][1]) + (s_red[1][2] + s_red[1][3]);
-        if (train) a.wpart[(long long)blockIdx.x * a.wpart_stride + kF2N] = (s_red[2][0] + s_red[2][1]) + (s_red[2][2] + s_red[2][3]);
-      }
-    }
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after_sync(); tmem_dealloc(tmem_base, 512); }
-}
-
 template <bool BF16>
 __global__ void dib_f32_to_16_kernel(const float* __restrict__ src, uint16_t* __restrict__ dst, long long n) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1366,97 +837,64 @@ bool map_mn(CUtensorMap* m, const void* base, long long cols, long long krows, l
 }
 
 int g_num_sms16 = 0;
-template <int MODE, bool BF16>
-cudaError_t launch16(const CUtensorMap& mA, const CUtensorMap& mB, const Int16Args& a, dim3 tiles, cudaStream_t st) {
+int num_sms16() {
   if (!g_num_sms16) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&g_num_sms16, cudaDevAttrMultiProcessorCount, dev); }
-  const long long nt = (long long)tiles.x * tiles.y * tiles.z;
-  if (nt <= 0) return cudaSuccess;
-  dim3 grid((unsigned)(nt < 2ll * g_num_sms16 ? nt : 2ll * g_num_sms16));
+  return g_num_sms16;
+}
+
+constexpr int kGemmSmem = kStages * kStageBytes + 128 + 1024;
+
+// streamed launch: persistent grid of at most two CTAs per SM over `ntile` tiles (one or two problems)
+template <int MODE, bool BF16>
+cudaError_t launch16(const CUtensorMap& mA, const CUtensorMap& mB, const Int16Args& a, const CUtensorMap& mA2, const CUtensorMap& mB2,
+                     const Int16Args& a2, long long ntile, cudaStream_t st) {
+  if (ntile <= 0) return cudaSuccess;
+  const long long cap = 2ll * num_sms16();
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(dib_int16_gemm_kernel<MODE, BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal);
+    cudaError_t e = cudaFuncSetAttribute(dib_int16_gemm_kernel<MODE, BF16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemmSmem);
     if (e != cudaSuccess) return e;
     attr = true;
   }
-  Int16Args none{};
-  dib_int16_gemm_kernel<MODE, BF16><<<grid, 192, kSmemTotal, st>>>(mA, mB, a, mA, mB, none);
+  dib_int16_gemm_kernel<MODE, BF16, false><<<(unsigned)(ntile < cap ? ntile : cap), kGemmThreads, kGemmSmem, st>>>(mA, mB, a, mA2, mB2, a2, 0);
   dib_note_launch();
   return cudaGetLastError();
 }
 
-// two weight-gradient problems (same batch, same split stride) in one launch
-template <bool BF16>
-cudaError_t launch16_wgrad2(const CUtensorMap& mA, const CUtensorMap& mB, const Int16Args& a, const CUtensorMap& mA2, const CUtensorMap& mB2,
-                            const Int16Args& a2, cudaStream_t st) {
-  if (!g_num_sms16) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&g_num_sms16, cudaDevAttrMultiProcessorCount, dev); }
-  const long long nt = (long long)DIB_CEIL_DIV(a.R, kBM) * DIB_CEIL_DIV(a.C, kBN) * a.nsplit +
-                       (long long)DIB_CEIL_DIV(a2.R, kBM) * DIB_CEIL_DIV(a2.C, kBN) * a2.nsplit;
-  if (nt <= 0) return cudaSuccess;
-  dim3 grid((unsigned)(nt < 2ll * g_num_sms16 ? nt : 2ll * g_num_sms16));
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(dib_int16_gemm_kernel<DIB_GEMM_WGRAD, BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal);
-    if (e != cudaSuccess) return e;
-    attr = true;
-  }
-  dib_int16_gemm_kernel<DIB_GEMM_WGRAD, BF16><<<grid, 192, kSmemTotal, st>>>(mA, mB, a, mA2, mB2, a2);
-  dib_note_launch();
-  return cudaGetLastError();
+template <int MODE, bool BF16>
+cudaError_t launch16(const CUtensorMap& mA, const CUtensorMap& mB, const Int16Args& a, long long ntile, cudaStream_t st) {
+  Int16Args none{};
+  return launch16<MODE, BF16>(mA, mB, a, mA, mB, none, ntile, st);
 }
+
+int rb_smem(int nkb) { return nkb * kBBytes + kRbStages * kABytes + 128 + 1024; }
 
 // resident-B launch: grid = a multiple of the column-tile count, at most one CTA per SM
-template <int MODE, bool BF16, int BN>
+template <int MODE, bool BF16>
 cudaError_t launch_rb(const CUtensorMap& mA, const CUtensorMap& mB, const Int16Args& a, int nkb, cudaStream_t st) {
-  if (!g_num_sms16) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&g_num_sms16, cudaDevAttrMultiProcessorCount, dev); }
-  const int tiles_r = DIB_CEIL_DIV(a.M, kBM), tiles_c = DIB_CEIL_DIV(a.C, BN);
+  const int tiles_r = DIB_CEIL_DIV(a.M, kBM), tiles_c = DIB_CEIL_DIV(a.C, kBN);
   long long grid = (long long)tiles_r * tiles_c;
-  const long long cap = (long long)(g_num_sms16 / tiles_c) * tiles_c;
+  const long long cap = (long long)(num_sms16() / tiles_c) * tiles_c;
   if (grid > cap) grid = cap;
   if (grid <= 0) return cudaSuccess;
-  const int smem = nkb * BN * 128 + kRbStages * kABytes + 128 + 1024;
+  const int smem = rb_smem(nkb);
   static int attr_smem = 0;
   if (attr_smem < smem) {
-    cudaError_t e = cudaFuncSetAttribute(dib_int16_rb_kernel<MODE, BF16, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaError_t e = cudaFuncSetAttribute(dib_int16_gemm_kernel<MODE, BF16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return e;
     attr_smem = smem;
   }
-  dib_int16_rb_kernel<MODE, BF16, BN><<<(unsigned)grid, 192, smem, st>>>(mA, mB, a, nkb);
+  Int16Args none{};
+  CUtensorMap mnone = mA;
+  dib_int16_gemm_kernel<MODE, BF16, true><<<(unsigned)grid, kGemmThreads, smem, st>>>(mA, mB, a, mnone, mnone, none, nkb);
   dib_note_launch();
   return cudaGetLastError();
 }
 
-// CTA-pair launch: clusters of two CTAs (one per SM of a TPC), at most one cluster per SM pair
-template <int MODE, bool BF16>
-cudaError_t launch2(const CUtensorMap& mA, const CUtensorMap& mB, const Int16Args& a, cudaStream_t st) {
-  if (!g_num_sms16) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&g_num_sms16, cudaDevAttrMultiProcessorCount, dev); }
-  const int R = (MODE == DIB_GEMM_WGRAD) ? a.R : a.M;
-  const long long nt = (long long)DIB_CEIL_DIV(R, 2 * kBM) * DIB_CEIL_DIV(a.C, k2BN) * ((MODE == DIB_GEMM_WGRAD) ? a.nsplit : 1);
-  if (nt <= 0) return cudaSuccess;
-  const long long ncl = nt < g_num_sms16 / 2 ? nt : g_num_sms16 / 2;
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(dib_int16_gemm2_kernel<MODE, BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2SmemTotal);
-    if (e != cudaSuccess) return e;
-    attr = true;
-  }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(2 * ncl)); cfg.blockDim = dim3(320); cfg.dynamicSmemBytes = k2SmemTotal; cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-  cfg.attrs = at; cfg.numAttrs = 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, dib_int16_gemm2_kernel<MODE, BF16>, mA, mB, a);
-  dib_note_launch();
-  return e != cudaSuccess ? e : cudaGetLastError();
-}
-
-// BN for the resident-B kernel (0 = not eligible): the weight slice [T x BN] 16-bit plus the A ring must fit in shared memory
-int rb_pick_bn(int T, int C) {
-  if (!dib_int16_rb_enabled() || T % kBK != 0 || C % 64 != 0) return 0;
-  const int nkb = T / kBK, budget = 227 * 1024 - (kRbStages * kABytes + 128 + 1024) - 4 * 256 * 4 - 1024;
-  if (C % 256 == 0 && nkb * 256 * 128 <= budget) return 256;
-  if (nkb * 128 * 128 <= budget) return 128;
-  return 0;
+// the resident-B kernel applies when the [T x 128] weight slice and its A ring fit in shared memory
+bool rb_ok(int T, int C) {
+  if (!dib_int16_rb_enabled() || T % kBK != 0 || C % 64 != 0) return false;
+  return rb_smem(T / kBK) + (int)sizeof(float) * (kConsumers / 32) * kBN <= 227 * 1024;
 }
 
 }  // namespace
@@ -1467,18 +905,11 @@ void dib_int16_head1_set(int on) { g_int16_head1 = on ? 1 : 0; }
 
 int g_int16_dbg = 0;
 void dib_int16_dbg_set(int v) { g_int16_dbg = v; }
-static int g_int16_2sm = -1;             // CTA-pair (cta_group::2) GEMMs for output widths that are multiples of 256
-int dib_int16_2sm_enabled() {
-  if (g_int16_2sm < 0) { const char* e = getenv("DIB_INT16_2SM"); g_int16_2sm = (e && e[0] == '1') ? 1 : 0; }
-  return g_int16_2sm;
-}
-void dib_int16_2sm_set(int on) { g_int16_2sm = on ? 1 : 0; }
 
 static int g_int16_rb = -1;
 int dib_int16_rb_enabled() {
-  // measured on B200 at C0 (profiles/r02_int16_resident_b_ab.json): slower than the streamed kernels (fwd 48 vs 37 / 32 us,
-  // dgrad_l1 99 vs 63 us) -- one CTA per SM halves the epilogue warps per SM and the epilogue, not the L2 re-reads of the
-  // weights, is what paces these GEMMs.  Kept selectable (DIB_INT16_RB=1, dib_debug_set_variant(1, 1)); default off.
+  // off by default: an A/B variant (DIB_INT16_RB=1, dib_debug_set_variant(1, 1)) that keeps the weight slice in shared memory
+  // instead of re-reading it from L2 for every row tile, at one CTA per SM instead of two
   if (g_int16_rb < 0) { const char* e = getenv("DIB_INT16_RB"); g_int16_rb = (e && e[0] == '1') ? 1 : 0; }
   return g_int16_rb;
 }
@@ -1539,15 +970,10 @@ cudaError_t dib_int16_fwd(const void* g_in, int ld_in, const void* w16, const fl
   a.dbg = g_int16_dbg;
   a.out16 = static_cast<uint16_t*>(g_out); a.ldc = ld_out; a.bias = bias; a.M = M; a.T = K; a.C = N; a.act = act; a.alpha = alpha;
   a.out_scale = 1.f; a.nsplit = 1;
-  if (const int bn = rb_pick_bn(K, N)) {          // weights resident in shared memory, activations streamed
-    if (!map_mn(&mB, w16, N, K, N, bn / 64)) return cudaErrorInvalidValue;
-    if (bn == 256) return bf16 ? launch_rb<DIB_GEMM_FWD, true, 256>(mA, mB, a, K / kBK, st) : launch_rb<DIB_GEMM_FWD, false, 256>(mA, mB, a, K / kBK, st);
-    return bf16 ? launch_rb<DIB_GEMM_FWD, true, 128>(mA, mB, a, K / kBK, st) : launch_rb<DIB_GEMM_FWD, false, 128>(mA, mB, a, K / kBK, st);
-  }
-  if (dib_int16_2sm_enabled() && N % k2BN == 0)
-    return bf16 ? launch2<DIB_GEMM_FWD, true>(mA, mB, a, st) : launch2<DIB_GEMM_FWD, false>(mA, mB, a, st);
-  const dim3 tiles(DIB_CEIL_DIV(M, kBM), DIB_CEIL_DIV(N, kBN), 1);
-  return bf16 ? launch16<DIB_GEMM_FWD, true>(mA, mB, a, tiles, st) : launch16<DIB_GEMM_FWD, false>(mA, mB, a, tiles, st);
+  if (rb_ok(K, N))          // weights resident in shared memory, activations streamed
+    return bf16 ? launch_rb<DIB_GEMM_FWD, true>(mA, mB, a, K / kBK, st) : launch_rb<DIB_GEMM_FWD, false>(mA, mB, a, K / kBK, st);
+  const long long nt = (long long)DIB_CEIL_DIV(M, kBM) * DIB_CEIL_DIV(N, kBN);
+  return bf16 ? launch16<DIB_GEMM_FWD, true>(mA, mB, a, nt, st) : launch16<DIB_GEMM_FWD, false>(mA, mB, a, nt, st);
 }
 
 // dz_in[M x K] = (dz[M x N] W16[K x N]^T) * act'(g_in[M x K])      (g_in may be null: no activation, e.g. d_emb)
@@ -1561,15 +987,10 @@ cudaError_t dib_int16_dgrad(const void* dz, int ld_dz, const void* w16, const vo
   a.dbg = g_int16_dbg;
   a.out16 = static_cast<uint16_t*>(dz_in); a.ldc = ld_out; a.X = static_cast<const uint16_t*>(g_in); a.ldx = ld_g;
   a.M = M; a.T = N; a.C = K; a.act = act; a.alpha = alpha; a.out_scale = 1.f; a.nsplit = 1; a.dbias = colsum_part;
-  if (const int bn = rb_pick_bn(N, K)) {          // W^T slice resident, dz streamed
-    if (!map_k(&mB, w16, N, K, N, bn)) return cudaErrorInvalidValue;
-    if (bn == 256) return bf16 ? launch_rb<DIB_GEMM_DGRAD, true, 256>(mA, mB, a, N / kBK, st) : launch_rb<DIB_GEMM_DGRAD, false, 256>(mA, mB, a, N / kBK, st);
-    return bf16 ? launch_rb<DIB_GEMM_DGRAD, true, 128>(mA, mB, a, N / kBK, st) : launch_rb<DIB_GEMM_DGRAD, false, 128>(mA, mB, a, N / kBK, st);
-  }
-  if (dib_int16_2sm_enabled() && K % k2BN == 0)
-    return bf16 ? launch2<DIB_GEMM_DGRAD, true>(mA, mB, a, st) : launch2<DIB_GEMM_DGRAD, false>(mA, mB, a, st);
-  const dim3 tiles(DIB_CEIL_DIV(M, kBM), DIB_CEIL_DIV(K, kBN), 1);
-  return bf16 ? launch16<DIB_GEMM_DGRAD, true>(mA, mB, a, tiles, st) : launch16<DIB_GEMM_DGRAD, false>(mA, mB, a, tiles, st);
+  if (rb_ok(N, K))          // W^T slice resident, dz streamed
+    return bf16 ? launch_rb<DIB_GEMM_DGRAD, true>(mA, mB, a, N / kBK, st) : launch_rb<DIB_GEMM_DGRAD, false>(mA, mB, a, N / kBK, st);
+  const long long nt = (long long)DIB_CEIL_DIV(M, kBM) * DIB_CEIL_DIV(K, kBN);
+  return bf16 ? launch16<DIB_GEMM_DGRAD, true>(mA, mB, a, nt, st) : launch16<DIB_GEMM_DGRAD, false>(mA, mB, a, nt, st);
 }
 
 // dW[K x N] (fp32 split partials, * out_scale) = g_in[M x K]^T dz[M x N];  db = colsum dz
@@ -1584,10 +1005,8 @@ cudaError_t dib_int16_wgrad(const void* g_in, int ld_g, const void* dz, int ld_d
   a.out32 = dW_part; a.ldc = N; a.dbias = nullptr; a.M = M; a.T = 0; a.C = N; a.R = K; a.out_scale = out_scale;
   a.nsplit = nsplit; a.rows_per_split = rows_per_split; a.split_stride = split_stride;
   (void)db_part;   // bias gradients come from the kernel that PRODUCES dz (dgrad epilogue / output head), not from here
-  if (dib_int16_2sm_enabled() && N % k2BN == 0)
-    return bf16 ? launch2<DIB_GEMM_WGRAD, true>(mA, mB, a, st) : launch2<DIB_GEMM_WGRAD, false>(mA, mB, a, st);
-  const dim3 tiles(DIB_CEIL_DIV(N, kBN), DIB_CEIL_DIV(K, kBM), nsplit);
-  return bf16 ? launch16<DIB_GEMM_WGRAD, true>(mA, mB, a, tiles, st) : launch16<DIB_GEMM_WGRAD, false>(mA, mB, a, tiles, st);
+  const long long nt = (long long)DIB_CEIL_DIV(N, kBN) * DIB_CEIL_DIV(K, kBM) * nsplit;
+  return bf16 ? launch16<DIB_GEMM_WGRAD, true>(mA, mB, a, nt, st) : launch16<DIB_GEMM_WGRAD, false>(mA, mB, a, nt, st);
 }
 
 static int g_int16_fwd2 = -1;            // fused [hidden, hidden, head] kernel for single-output models (1, default) or the separate kernels (0)
@@ -1608,7 +1027,6 @@ cudaError_t dib_int16_fwd2_head(const void* g_in, int ld_in, int K0, const void*
                                 int M, float inv_batch, float gscale, void* dg2, float* user_pred, float* wpart, int wpart_stride,
                                 float* loss_part, float* acc_part, int* nblocks, int bf16, cudaStream_t st) {
   if (!encode_fn3()) return cudaErrorNotSupported;
-  if (!g_num_sms16) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&g_num_sms16, cudaDevAttrMultiProcessorCount, dev); }
   CUtensorMap mA, mW0, mW1;
   if (!map_k(&mA, g_in, K0, M, ld_in, kBM) || !map_mn(&mW0, w16_0, kF2N, K0, kF2N, kF2N / 64) || !map_mn(&mW1, w16_1, kF2N, kF2N, kF2N, kF2N / 64))
     return cudaErrorInvalidValue;
@@ -1618,7 +1036,7 @@ cudaError_t dib_int16_fwd2_head(const void* g_in, int ld_in, int K0, const void*
   a.loss_part = loss_part; a.acc_part = acc_part; a.M = M; a.nk0 = K0 / kBK; a.act = act; a.out_act = out_act; a.loss = loss;
   a.alpha = alpha; a.inv_batch = inv_batch; a.gscale = gscale;
   const int tiles = DIB_CEIL_DIV(M, kBM);
-  const int grid = tiles < g_num_sms16 ? tiles : g_num_sms16;
+  const int grid = tiles < num_sms16() ? tiles : num_sms16();
   *nblocks = grid;
   if (grid <= 0) return cudaSuccess;
   cudaError_t e = cudaErrorInvalidValue;
@@ -1628,7 +1046,7 @@ cudaError_t dib_int16_fwd2_head(const void* g_in, int ld_in, int K0, const void*
     e = attr ? cudaSuccess : cudaFuncSetAttribute(dib_int16_fwd2_kernel<BF, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, kF2Smem); \
     if (e != cudaSuccess) return e;                                                                                                  \
     attr = true;                                                                                                                     \
-    dib_int16_fwd2_kernel<BF, ACT><<<grid, 320, kF2Smem, st>>>(mA, mW0, mW1, a);                                                      \
+    dib_int16_fwd2_kernel<BF, ACT><<<grid, kF2Threads, kF2Smem, st>>>(mA, mW0, mW1, a);                                               \
   } while (0)
 #define DIB_F2_ACT(ACT) do { if (bf16) DIB_F2_LAUNCH(true, ACT); else DIB_F2_LAUNCH(false, ACT); } while (0)
   switch (act) {
@@ -1659,7 +1077,8 @@ cudaError_t dib_int16_wgrad_pair(const void* g_in0, int K0, const void* dz0, int
   a.dbg = b.dbg = g_int16_dbg;
   a.out32 = dW_part0; a.ldc = N0; a.M = M; a.C = N0; a.R = K0; a.out_scale = out_scale; a.nsplit = nsplit0; a.rows_per_split = rps0; a.split_stride = split_stride;
   b.out32 = dW_part1; b.ldc = N1; b.M = M; b.C = N1; b.R = K1; b.out_scale = out_scale; b.nsplit = nsplit1; b.rows_per_split = rps1; b.split_stride = split_stride;
-  return bf16 ? launch16_wgrad2<true>(mA, mB, a, mA2, mB2, b, st) : launch16_wgrad2<false>(mA, mB, a, mA2, mB2, b, st);
+  const long long nt = (long long)DIB_CEIL_DIV(K0, kBM) * DIB_CEIL_DIV(N0, kBN) * nsplit0 + (long long)DIB_CEIL_DIV(K1, kBM) * DIB_CEIL_DIV(N1, kBN) * nsplit1;
+  return bf16 ? launch16<DIB_GEMM_WGRAD, true>(mA, mB, a, mA2, mB2, b, nt, st) : launch16<DIB_GEMM_WGRAD, false>(mA, mB, a, mA2, mB2, b, nt, st);
 }
 
 int dib_int16_head_blocks(int num_sms) { return num_sms * 2; }

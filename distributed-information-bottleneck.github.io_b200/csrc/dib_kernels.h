@@ -27,7 +27,7 @@ struct DibGemmLaunch {
 
 cudaError_t dib_launch_gemm_simt(int mode, const DibGemmLaunch& L, cudaStream_t st);
 
-// TF32 tcgen05 path (dib_gemm_tc.cu); `hp` = host copies of the group's problem descriptors
+// TF32 wgmma path (dib_gemm_tc.cu); `hp` = host copies of the group's problem descriptors
 bool dib_gemm_tc_eligible(int mode, const DibGemmProblem* hp, int nprob, const float* params_base_hint);
 cudaError_t dib_launch_gemm_tc(int mode, const DibGemmLaunch& L, const DibGemmProblem* hp, cudaStream_t st);
 
@@ -135,11 +135,7 @@ struct DibEncFusedIO {
   float* emb; int ldemb; float* user_emb;
   float* kl_part; int kl_stride;
   void* emb16 = nullptr; int ldemb16 = 0;   // optional fp16 copy of emb (16-bit integration path)
-  void* eps16 = nullptr;                    // optional [n, F*32] 16-bit noise hand-off: forward writes, two-chain backward reads
-  void* a0g = nullptr;                      // optional [2 F, n, 8] 16-bit [pe|1] operand hand-off, k-halves as planes (same direction)
 };
-int dib_enc_bwd_version();
-void dib_enc_bwd_set_version(int v);
 size_t dib_enc_fused_pack_bytes(int F);
 long long dib_enc_fused_pack_zero_capacity(int F);
 int dib_enc_fused_fwd_ctas_per_sm();
@@ -176,8 +172,6 @@ cudaError_t dib_int16_wgrad_pair(const void* g_in0, int K0, const void* dz0, int
                                  int M, long long split_stride, float out_scale, int bf16, cudaStream_t st);
 int dib_int16_head_blocks(int num_sms);
 void dib_int16_dbg_set(int v);
-int dib_int16_2sm_enabled();
-void dib_int16_2sm_set(int on);
 int dib_int16_fwd2_enabled();
 void dib_int16_fwd2_set(int on);
 int dib_int16_fwd2_ok(int K0, int N1, int N2, int out_dim);

@@ -60,7 +60,7 @@ class optimizers:
             table = {"adam": Adam, "sgd": SGD, "rmsprop": RMSprop}
             if identifier.lower() in table:
                 return table[identifier.lower()]()
-        raise ValueError(f"optimizer {identifier!r} is not implemented by the B200 engine (adam, sgd, rmsprop are)")
+        raise ValueError(f"optimizer {identifier!r} is not implemented by the engine (adam, sgd, rmsprop are)")
 
 
 class _Loss:

@@ -23,7 +23,7 @@ from .keras_compat import Adam, RMSprop, SGD, Callback, History, optimizers, res
 
 def _require_cuda():
     if not torch.cuda.is_available():
-        raise _lib.DibError("dib_b200 needs a CUDA device (B200, sm_100a); there is no CPU path")
+        raise _lib.DibError("dib_b200 needs a CUDA device (H100, sm_90a); there is no CPU path")
 
 
 def _stream():
@@ -160,8 +160,8 @@ class DistributedIBNet:
         (nb-particle's shared particle encoder + set transformer: see :class:`SharedParticleEncoder`).
 
     Extra keyword-only arguments (not in the reference): ``device``, ``seed`` (weight init + noise stream),
-    ``precision`` ('fp32' exact-FMA parity path | 'tf32' kind::tf32 GEMMs | 'fp16' / 'bf16' fused 16-bit-operand
-    tcgen05 kernels with fp32 accumulation; ``model.kernel_info()`` says what a handle actually runs), ``process_group``
+    ``precision`` ('fp32' exact-FMA parity path | 'tf32' tf32 wgmma GEMMs | 'fp16' / 'bf16' fused 16-bit-operand
+    wgmma kernels with fp32 accumulation; ``model.kernel_info()`` says what a handle actually runs), ``process_group``
     (data-parallel group; defaults to the WORLD group when torch.distributed is initialised), ``leaky_alpha``.
     """
 
@@ -242,12 +242,9 @@ class DistributedIBNet:
         self._step_dev_dirty = False       # _train_step_count moved outside a graph replay: refill the device mirror
         self._replayed_launches = 0        # kernels launched by graph replays (dib_launch_count only sees eager launches)
         self._side_stream = None
-        # two-bucket all-reduce overlapped with the encoder backward: measured SLOWER than one flat all-reduce on 2 B200s
-        # (0.475 vs 0.444 ms/step strong, 0.758 vs 0.744 weak -- the second NCCL launch and the stream hand-offs cost more than
-        # the 0.8 MB bucket hides), so it is opt-in (DIB_OVERLAP_ALLREDUCE=1)
+        # two-bucket all-reduce overlapped with the encoder backward: opt-in (DIB_OVERLAP_ALLREDUCE=1); by default one flat
+        # all-reduce of [grads || stats] runs as an eager call between the backward graph and the optimizer graph
         self.overlap_allreduce = os.environ.get("DIB_OVERLAP_ALLREDUCE", "0") in ("1", "on", "true", "yes")
-        # (capturing the NCCL all-reduce inside the step's graph was tried on 2 B200s: no gain -- 0.611 vs 0.605 ms/step weak -- and
-        #  the processes hung at teardown; the all-reduce stays an eager call between the backward graph and the optimizer graph)
         self._inference_calls = 0          # fresh noise per un-seeded inference call (tf.random.normal, models.py:108)
         self.optimizer = None
         self.compiled_metrics_names = []

@@ -1,4 +1,4 @@
-/* dib_b200.h -- C ABI of the B200-native Distributed-IB training engine.
+/* dib_b200.h -- C ABI of the H100-native Distributed-IB training engine.
  *
  * The reference (distributed-information-bottleneck.github.io) has no FFI/plugin interface: its
  * hot path is a tf.keras Model whose arithmetic executes inside TensorFlow.  Each entry point
@@ -59,11 +59,11 @@ enum dib_loss {
 };
 
 /* arithmetic of the dense contractions; everything else (PE, exp, KL, loss, Adam, reductions) is fp32 in every mode
- * and all tensor-core modes accumulate in fp32 (TMEM).
+ * and all tensor-core modes accumulate in fp32 (wgmma register accumulators).
  *   FP32: CUDA-core FMA -- the exact parity path (the reference's tf.keras fp32 graph on a CPU).
- *   TF32: tcgen05.mma kind::tf32 on fp32 storage (10-bit mantissa, 8-bit exponent operands, rounded not truncated):
+ *   TF32: tf32 wgmma on fp32 storage (10-bit mantissa, 8-bit exponent operands, rounded not truncated):
  *         what stock TensorFlow does to an fp32 model on a tensor-core GPU.  Unfused grouped GEMMs.
- *   FP16: tcgen05.mma kind::f16 on fp16 operands (10-bit mantissa like TF32 but a 5-bit exponent: |value| <= 65504,
+ *   FP16: f16 wgmma on fp16 operands (10-bit mantissa like TF32 but a 5-bit exponent: |value| <= 65504,
  *         saturating conversions, gradients carried under a power-of-two loss scale) -- the fused per-feature encoder
  *         kernels and the 16-bit integration path; shapes outside their envelope run on the TF32 kernels.
  *   BF16: the same fused kernels on bf16 operands (7-bit mantissa, fp32's exponent range).
@@ -195,7 +195,7 @@ int dib_optimizer_step(int32_t kind, float* params, const float* grads, float* s
                        const float* lr_dev, int32_t* step_dev, float hyper0, float hyper1, float hyper2, void* stream);
 
 /* model.integration_network(emb) (models.py:84,122) as a stand-alone call: emb [n, F*E] -> out_pred [n, out] through the
- * Dense stack with the output activation, on the model's precision path (fp32 FMA / tf32 tcgen05). */
+ * Dense stack with the output activation, on the model's precision path (fp32 FMA / tf32 wgmma). */
 int dib_integration_forward(dib_model* h, const float* params, const float* emb, int64_t n, float* out_pred,
                             void* workspace, void* stream);
 
@@ -292,27 +292,24 @@ int dib_debug_gemm_tc(int32_t mode, const float* A, int32_t lda, const float* B,
 /* bring-up switch (bit mask): 1 = unfused encoder kernels, 2 = integration network on fp32-storage TF32 kernels. */
 int dib_debug_force_unfused(dib_model* h, int32_t on);
 
-/* process-wide kernel-variant switch for A/B measurements.  key 0: fused encoder backward kernel, value 1 = the
- * single-chain kernel of round 1, 2 = two chains on consecutive tiles (default; also DIB_ENC_BWD=1|2 in the environment).
- * key 1: 16-bit integration FWD / DGRAD GEMMs, 1 = weight slice resident in shared memory, 0 = re-streamed per tile (default:
- * measured faster; also DIB_INT16_RB=0|1).
+/* process-wide kernel-variant switch for A/B measurements.
+ * key 1: 16-bit integration FWD / DGRAD GEMMs, 1 = weight slice resident in shared memory, 0 = re-streamed per tile (default;
+ * also DIB_INT16_RB=0|1).  Both issue the same MMAs in the same order: results are bit-identical.
  * key 2: fused output head for output_dimensionality == 1, 1 = eight rows per pass with a lane-parallel loss (default), 0 = the
  * generic kernel.
  * key 3: single-output models whose last two hidden integration layers are 256 wide, 1 = those layers + the head + the loss as one
  * kernel (default; also DIB_INT16_FWD2=0|1), 0 = one kernel per layer and the head kernel of key 2.
- * key 4: 16-bit integration GEMMs whose output width is a multiple of 256, 1 = CTA-pair kernels (tcgen05 cta_group::2, 256 x 256 tile
- * per pair; also DIB_INT16_2SM=1), 0 = single-CTA 128 x 128 kernels (default: measured the same or faster).
  * key 5: MEASUREMENT ONLY, wrong results: 1 = the 16-bit GEMM epilogues skip their global stores (cost of the store path). */
 int dib_debug_set_variant(int32_t key, int32_t value);
 
 /* text of the last error raised on this thread ("" if none). */
 const char* dib_last_error(void);
 
-/* "sm_100a" etc: the architecture the kernels were compiled for, and the ABI version. */
+/* "sm_90a" etc: the architecture the kernels were compiled for, and the ABI version. */
 const char* dib_build_info(void);
 
 /* one line describing what THIS handle runs, e.g.
- * "precision=fp16 encoders=fused-tcgen05-f16 integration=int16-tcgen05-f16 operands=fp16 accumulate=fp32".
+ * "precision=fp16 encoders=fused-wgmma-f16 integration=int16-wgmma-f16 operands=fp16 accumulate=fp32".
  * Returns the number of bytes written (excluding the terminator), negative on error. */
 int32_t dib_model_info(const dib_model* h, char* out, size_t out_bytes);
 

@@ -18,6 +18,7 @@ the product path (dib_b200) never does.
 """
 from __future__ import annotations
 
+import ast
 import math
 from dataclasses import dataclass, field
 from typing import Callable, List, Optional, Sequence
@@ -153,6 +154,23 @@ def glorot_uniform_params(cfg: DIBConfig, rng: np.random.Generator, dtype=np.flo
         else:
             out.append(np.zeros(s, dtype=dtype))
     return np.concatenate(out)
+
+
+def golden_params(cfg: DIBConfig, rng: np.random.Generator) -> np.ndarray:
+    """Weights of a forward golden case (tests/golden/make_golden.py): glorot-uniform kernels, then small non-zero biases
+    from the same stream so that bias handling is pinned.  The goldens store the seed of `rng` and a checksum, not the vector."""
+    flat = glorot_uniform_params(cfg, rng, dtype=np.float32)
+    return flat + (rng.standard_normal(flat.size) * 0.05).astype(np.float32) * (flat == 0)
+
+
+def load_forward_golden(path):
+    """(cfg, arrays) of tests/golden/ref_forward_*.npz with arrays['params'] re-derived from the stored seed; the stored
+    float64 sum of the weights guards against a change of the random stream.  enc{i} hold the rows arrays['enc_rows']."""
+    z = dict(np.load(path))
+    cfg = DIBConfig(**ast.literal_eval(str(z["cfg"])))
+    z["params"] = golden_params(cfg, np.random.default_rng(int(z["seed"])))
+    assert np.sum(z["params"], dtype=np.float64) == float(z["params_sum"]), f"{path}: weights no longer re-derive from the seed"
+    return cfg, z
 
 
 def unflatten(cfg: DIBConfig, flat: np.ndarray):

@@ -15,7 +15,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100, sm_90a)")
 
 
 def pytest_collection_modifyitems(config, items):

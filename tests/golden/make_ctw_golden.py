@@ -1,6 +1,6 @@
-"""Generates tests/golden/ref_ctw.npz from the REFERENCE'S OWN native code: chaos/cppctw.cpp compiled where it lies
-(oracle/Makefile -> oracle/_ref/libctw_ref.so).  Run in the build container (needs /root/reference):
-    make -C oracle && python tests/golden/make_ctw_golden.py"""
+"""Generates tests/golden/ref_ctw.npz and ref_ctw_fresh.npz from the REFERENCE'S OWN native code: chaos/cppctw.cpp
+compiled where it lies (oracle/Makefile -> oracle/_ref/libctw_ref.so; needs a checkout of the reference, REF=<dir>):
+    make -C oracle REF=<reference checkout> && python tests/golden/make_ctw_golden.py"""
 import os
 import sys
 
@@ -34,8 +34,34 @@ def sequences():
     return out
 
 
+def fresh_sequences():
+    """Seeded random sequences with a long run (deep tails, depth > 512), and 300 short ones over small alphabets with runs
+    and periodic pieces that exercise the lazy tail extension (tests/test_ctw.py)."""
+    rng = np.random.default_rng(123)
+    fresh = []
+    for n, A in ((1, 3), (33, 2), (1000, 3), (6000, 4), (3000, 27)):
+        seq = rng.integers(0, A, n)
+        seq[n // 3: n // 3 + min(n // 4, 900)] = seq[0]
+        fresh.append((seq, A))
+    rng = np.random.default_rng(2024)
+    small = []
+    for trial in range(300):
+        A = int(rng.integers(1, 6))
+        n = int(rng.integers(1, 90))
+        kind = trial % 3
+        if kind == 0:
+            seq = rng.integers(0, A, n)
+        elif kind == 1:                                                       # runs
+            seq = np.repeat(rng.integers(0, A, max(n // 7, 1)), 7)[:n]
+        else:                                                                 # periodic with a defect
+            seq = np.tile(rng.integers(0, A, int(rng.integers(1, 5))), n)[:n]
+            seq[int(rng.integers(0, n))] = int(rng.integers(0, A))
+        small.append((seq, A))
+    return {"fresh": fresh, "small": small}
+
+
 def main():
-    assert ctw_oracle.reference_available(), "run `make -C oracle` first"
+    assert ctw_oracle.reference_available(), "run `make -C oracle REF=<reference checkout>` first"
     rec = {}
     for name, (seq, A) in sequences().items():
         rec[name + "_seq"] = seq.astype(np.int8)
@@ -43,6 +69,15 @@ def main():
         rec[name + "_H"] = np.float64(ctw_oracle.reference_estimate_entropy(seq, A))
         print(f"{name:>20s}  A={A:<3d} n={len(seq):<6d} H={rec[name + '_H']!r}")
     np.savez_compressed(os.path.join(HERE, "ref_ctw.npz"), **rec)
+    # sets of sequences: concatenated symbols, offsets, alphabet sizes, the reference's estimates
+    rec = {}
+    for name, cases in fresh_sequences().items():
+        rec[name + "_seqs"] = np.concatenate([seq for seq, _ in cases]).astype(np.int8)
+        rec[name + "_offsets"] = np.cumsum([0] + [len(seq) for seq, _ in cases]).astype(np.int64)
+        rec[name + "_A"] = np.array([A for _, A in cases], dtype=np.int32)
+        rec[name + "_H"] = np.array([ctw_oracle.reference_estimate_entropy(seq, A) for seq, A in cases], dtype=np.float64)
+        print(f"{name:>20s}  {len(cases)} sequences, H[:3]={rec[name + '_H'][:3]!r}")
+    np.savez_compressed(os.path.join(HERE, "ref_ctw_fresh.npz"), **rec)
 
 
 if __name__ == "__main__":

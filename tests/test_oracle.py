@@ -1,7 +1,6 @@
 """CPU: the oracle against (i) golden vectors produced by the reference's own code (tests/golden/
 make_golden.py), (ii) the closed-form known answers of SURVEY.md section 4, (iii) itself (finite differences,
 torch-autograd twin, data-parallel shard additivity)."""
-import ast
 import os
 
 import numpy as np
@@ -14,9 +13,7 @@ CASES = ["c0_small", "pendulum_like", "radial_like", "odd_shapes"]
 
 
 def load_case(golden_dir, name):
-    z = np.load(os.path.join(golden_dir, f"ref_forward_{name}.npz"))
-    cfg = O.DIBConfig(**ast.literal_eval(str(z["cfg"])))
-    return cfg, z
+    return O.load_forward_golden(os.path.join(golden_dir, f"ref_forward_{name}.npz"))
 
 
 @pytest.mark.parametrize("name", CASES)
@@ -29,7 +26,7 @@ def test_forward_matches_reference_code(golden_dir, name):
     encs, _ = O.unflatten(cfg, z["params"].astype(np.float64))
     xs = O.split_features(cfg, z["x"].astype(np.float64))
     for i in range(cfg.number_features):
-        np.testing.assert_allclose(O.encoder_forward(cfg, encs[i], xs[i]), z[f"enc{i}"], rtol=1e-12, atol=1e-12)
+        np.testing.assert_allclose(O.encoder_forward(cfg, encs[i], xs[i])[z["enc_rows"]], z[f"enc{i}"], rtol=1e-12, atol=1e-12)
 
 
 def test_beta_schedule_golden_and_kat(golden_dir):

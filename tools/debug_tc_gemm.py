@@ -1,4 +1,4 @@
-"""Bring-up probe for the tcgen05 GEMM kernel: structured operands whose product reveals which element each MMA
+"""Bring-up probe for the TF32 wgmma GEMM kernel: structured operands whose product reveals which element each MMA
 lane actually read.  Run on the GPU box:  python tools/debug_tc_gemm.py"""
 import ctypes
 import sys, os
