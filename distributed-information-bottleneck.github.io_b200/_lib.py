@@ -92,7 +92,6 @@ SIGNATURES = {
                                     c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int64, c_int32,
                                     c_void_p]),
     "dib_debug_force_unfused": (c_int32, [c_void_p, c_int32]),
-    "dib_debug_set_variant": (c_int32, [c_int32, c_int32]),
     "dib_last_error": (c_char_p, []),
     "dib_build_info": (c_char_p, []),
     "dib_model_info": (c_int32, [c_void_p, c_char_p, c_size_t]),

@@ -71,7 +71,7 @@ struct dib_model {
   std::vector<int> int_fwd, int_dgrad, int_wgrad;
   std::vector<int> enc_maxK;                        // max over features of fan-in of layer j
   // fused per-feature encoder kernels (tensor-core mode; dib_enc_fused.cu)
-  bool fused_ok = false, fused_bwd_ok = false, force_unfused = false, force_int32 = false;
+  bool fused_ok = false;
   DibEncFusedDesc fdesc;
   void* d_fused_tables = nullptr;
   long long pack_off = 0;       // packed 16-bit encoder weights inside the workspace (float offset)
@@ -84,6 +84,13 @@ struct dib_model {
   std::vector<long long> g16_off, dg16_off, w16_off;   // [1..Li], [1..Li], [0..Li-1]
   int head_blocks = 0, lossacc_cap = 0;
   int head_used = 0;                // rows of the head partials the last forward wrote (fused tail kernel: its CTA count)
+  // the kernels this handle runs (set_route): every forward / backward / dib_model_info reads the choice from here
+  struct Route {
+    bool enc_fused = false;         // fused per-feature encoder kernels (else PE + grouped GEMMs + reparam kernels)
+    bool int16 = false;             // 16-bit integration network (else per-layer TF32 GEMMs + dib_launch_loss)
+    bool tail_fused = false;        // int16: last two hidden layers + head + loss as one kernel (dib_int16_fwd2_head)
+    bool head1 = false;             // int16, no fused tail: the out = 1 head kernel instead of the generic one
+  } route;
   // custom-step variants (SURVEY 8f3)
   float lv_off = 0.f, kl_exp = 1.f, kl_scale = 1.f;
   const uint32_t* step_dev = nullptr;  // optional device-resident addend of the Philox step word (dib_set_noise_step_device)
@@ -107,6 +114,30 @@ int enc_fan_in(const dib_model* h, int f, int j) { return j == 0 ? h->w_in[f] : 
 int enc_fan_out(const dib_model* h, int j) { return j < h->L ? h->enc_arch[j] : 2 * h->E; }
 int int_fan_in(const dib_model* h, int j) { return j == 0 ? h->F * h->E : h->int_arch[j - 1]; }
 int int_fan_out(const dib_model* h, int j) { return j < h->Li ? h->int_arch[j] : h->out; }
+
+// the one place the kernel path is chosen.  fused_ok / int16_ok are what dib_create found the shapes to support; the bits of
+// `unfused` (dib_debug_force_unfused) turn paths off: 1 = fused encoders, 2 = 16-bit integration network (it reads the fp16
+// embedding only the fused encoders write), 4 = fused integration tail, 8 = out = 1 head kernel.
+void set_route(dib_model* h, int unfused) {
+  dib_model::Route& r = h->route;
+  r.enc_fused = h->fused_ok && !(unfused & 1);
+  r.int16 = r.enc_fused && h->int16_ok && !(unfused & 2);
+  r.tail_fused = r.int16 && !(unfused & 4) && h->Li >= 2 &&
+                 dib_int16_fwd2_ok(int_fan_in(h, h->Li - 2), int_fan_out(h, h->Li - 2), int_fan_out(h, h->Li - 1), h->out);
+  r.head1 = r.int16 && !r.tail_fused && h->out == 1 && !(unfused & 8);
+}
+
+// power-of-two loss scale of the 16-bit gradient operands (see dib_enc_fused.cu)
+float loss_scale(float inv_batch) { return exp2f(ceilf(log2f(1.f / inv_batch))); }
+
+// deterministic split of the batch for the weight gradients
+struct Split { long long rps; int nsplit; };
+Split batch_split(long long n) {
+  long long rps = DIB_CEIL_DIV(n, (long long)kMaxSplits);
+  if (rps < 256) rps = 256;
+  rps = DIB_ROUND_UP(rps, 64);      // whole k-blocks of every WGRAD kernel (32 rows for the TF32 ones, 64 for the 16-bit ones)
+  return {rps, (int)DIB_CEIL_DIV(n, rps)};
+}
 
 long long take(long long& cursor, long long floats) {
   const long long off = cursor;
@@ -333,139 +364,159 @@ int check_call(const dib_model* h, const void* params, const void* x, int64_t n,
   return 0;
 }
 
-// PE -> encoder layers (all features) -> reparam/KL -> integration layers -> loss/metrics
-struct NoiseKey { uint64_t seed; uint32_t step; uint64_t sample_offset; bool training; };
+// noise of one forward: the caller's eps, or Philox (seed, step, sample_offset); training turns Dropout on
+struct NoiseKey { const float* eps; uint64_t seed; uint32_t step; uint64_t sample_offset; bool training; };
 int encode_all(const Ctx& c, const float* x, int ldx, int rnd, const int* row_index, int64_t n_src, const NoiseKey* key = nullptr);
 
-int run_forward(const Ctx& c, const float* x, const float* y, const float* eps, uint64_t seed, uint32_t step,
-                uint64_t sample_offset, float inv_batch, bool training, float* user_pred, float* user_emb,
-                float* out_stats, bool enc_only = false) {
+DibReparamArgs reparam_args(const Ctx& c, const NoiseKey& nk) {
+  const dib_model* h = c.h;
+  DibReparamArgs ra;
+  ra.enc_out = c.ws + h->enc_out.off; ra.feat_stride = h->enc_out.feat_stride; ra.ldo = h->enc_out.ld;
+  ra.eps = nk.eps; ra.seed = nk.seed; ra.step = nk.step; ra.step_dev = c.step_dev(); ra.sample_offset = nk.sample_offset;
+  ra.F = h->F; ra.E = h->E; ra.n = c.n; ra.round_out = is_tc(h) ? 1 : 0;
+  return ra;
+}
+
+// inputs of the fused encoder kernels; the forward adds its outputs
+DibEncFusedIO fused_io(const Ctx& c, const float* x, const NoiseKey& nk) {
+  DibEncFusedIO io;
+  io.params = c.params; io.packed = c.ws + c.h->pack_off; io.x = x; io.ldx = c.h->D; io.n = c.n;
+  io.eps = nk.eps; io.seed = nk.seed; io.step = nk.step; io.step_dev = c.step_dev(); io.sample_offset = nk.sample_offset;
+  io.emb = nullptr; io.ldemb = 0; io.user_emb = nullptr; io.kl_part = nullptr; io.kl_stride = 0;
+  return io;
+}
+
+// 16-bit activation entering integration layer j
+const void* int16_in(const Ctx& c, int j) {
+  return j == 0 ? (const void*)(c.ws + c.h->emb16_off) : (const void*)(c.ws + c.h->g16_off[j]);
+}
+
+// encoder half of the forward: PE -> encoder layers (all features) -> reparam / KL partials.  Writes the embedding the
+// integration half reads (fp32 workspace copy, or the fp16 copy of the 16-bit integration network; neither when enc_only:
+// the caller's network consumes user_emb) and *nblk_kl = KL partials per feature.
+int forward_encoders(const Ctx& c, const float* x, const NoiseKey& nk, float* user_emb, bool enc_only, int* nblk_kl) {
   dib_model* h = c.h;
-  const int rnd = is_tc(h) ? 1 : 0;
-  const bool fast_path = h->fused_ok && rnd && (!training || h->fused_bwd_ok) && !h->force_unfused && h->int16_ok && !h->force_int32;
-  if (rnd && !fast_path) {
+  if (!h->route.enc_fused) {
+    if (encode_all(c, x, h->D, is_tc(h) ? 1 : 0, nullptr, 0, &nk)) return 1;
+    prof_begin(c, "reparam_kl_fwd");
+    DIB_CUDA_OK(dib_launch_reparam_fwd(reparam_args(c, nk), c.ws + h->emb.off, h->emb.ld, user_emb, c.ws + h->kl_part_off,
+                                       h->kl_stride, c.st));
+    prof_end(c);
+    *nblk_kl = (int)DIB_CEIL_DIV((long long)c.n, (long long)kRowsPerBlock);
+    return 0;
+  }
+  const long long want = (long long)h->F * DIB_CEIL_DIV((long long)c.n, 128ll);
+  const long long cap = (long long)h->num_sms * dib_enc_fused_fwd_ctas_per_sm();
+  DibEncFusedDesc d = h->fdesc;
+  d.logvar_offset = h->lv_off;
+  d.grid = (int)(want < cap ? want : cap);
+  *nblk_kl = DIB_CEIL_DIV(d.grid, h->F);
+  prof_begin(c, "enc_pack_weights");
+  {
+    const long long zn = (long long)h->F * h->kl_stride, zcap = dib_enc_fused_pack_zero_capacity(h->F);
+    // the pack kernel also clears the KL partial table when it fits its grid
+    if (zn <= zcap) DIB_CUDA_OK(dib_enc_fused_pack(d, c.params, c.ws + h->pack_off, c.ws + h->kl_part_off, zn, c.st));
+    else {
+      DIB_CUDA_OK(dib_enc_fused_pack(d, c.params, c.ws + h->pack_off, nullptr, 0, c.st));
+      DIB_CUDA_OK(cudaMemsetAsync(c.ws + h->kl_part_off, 0, sizeof(float) * (size_t)zn, c.st));
+    }
+  }
+  prof_end(c);
+  const bool i16 = h->route.int16 && !enc_only;
+  DibEncFusedIO io = fused_io(c, x, nk);
+  io.emb = i16 || enc_only ? nullptr : c.ws + h->emb.off; io.ldemb = h->emb.ld; io.user_emb = user_emb;
+  io.kl_part = c.ws + h->kl_part_off; io.kl_stride = h->kl_stride;
+  if (i16) { io.emb16 = c.ws + h->emb16_off; io.ldemb16 = h->F * h->E; }
+  prof_begin(c, "enc_fused_fwd");
+  DIB_CUDA_OK(dib_enc_fused_forward(d, io, c.st));
+  prof_end(c);
+  return 0;
+}
+
+// integration half of the forward: integration layers -> prediction, compiled loss / metrics, d loss / d prediction
+// (training) -> the stats row
+int forward_integration(const Ctx& c, const float* y, float inv_batch, bool training, float* user_pred, float* out_stats,
+                        int nblk_kl) {
+  dib_model* h = c.h;
+  auto finalize = [&](int nblk_loss) {
+    return dib_launch_finalize_stats(c.ws + h->kl_part_off, h->kl_stride, nblk_kl, c.ws + h->loss_part_off, c.ws + h->acc_part_off,
+                                     nblk_loss, h->F, c.n, y != nullptr, out_stats, c.st);
+  };
+  if (!h->route.int16) {
+    for (int j = 0; j <= h->Li; ++j) {
+      prof_begin(c, "int_fwd_l", j);
+      if (gemm(c, DIB_GEMM_FWD, h->int_fwd[j], 1, int_fan_out(h, j), 0, 1, 0)) return 1;
+      prof_end(c);
+    }
+    prof_begin(c, "loss_stats");
+    DIB_CUDA_OK(dib_launch_loss(h->loss, h->out_act, h->alpha, c.ws + h->pred.off, h->pred.ld, y, h->out, c.n, inv_batch,
+                                training ? c.ws + h->d_pred.off : nullptr, user_pred, c.ws + h->loss_part_off,
+                                c.ws + h->acc_part_off, is_tc(h) ? 1 : 0, c.st));
+    DIB_CUDA_OK(finalize((int)DIB_CEIL_DIV((long long)c.n, (long long)kRowsPerBlock)));
+    prof_end(c);
+    return 0;
+  }
+  // ---------------- integration network on 16-bit activations + fused output head
+  const int bf = h->precision == DIB_PREC_BF16 ? 1 : 0;
+  prof_begin(c, "int16_pack_weights");
+  {
+    std::vector<const float*> wsrc; std::vector<void*> wdst; std::vector<long long> wn;
+    for (int j = 0; j < h->Li; ++j) {
+      wsrc.push_back(c.params + h->intW[j]); wdst.push_back(c.ws + h->w16_off[j]);
+      wn.push_back((long long)int_fan_in(h, j) * int_fan_out(h, j));
+    }
+    DIB_CUDA_OK(dib_int16_convert_many(wsrc.data(), wdst.data(), wn.data(), h->Li, bf, c.st));
+  }
+  prof_end(c);
+  const float gscale = training ? loss_scale(inv_batch) : 1.f;
+  void* const dg = training ? (void*)(c.ws + h->dg16_off[h->Li]) : nullptr;
+  const int n_plain = h->route.tail_fused ? h->Li - 2 : h->Li;
+  for (int j = 0; j < n_plain; ++j) {
+    prof_begin(c, "int16_fwd_l", j);
+    DIB_CUDA_OK(dib_int16_fwd(int16_in(c, j), int_fan_in(h, j), c.ws + h->w16_off[j], c.params + h->intB[j], c.ws + h->g16_off[j + 1],
+                              int_fan_out(h, j), c.n, int_fan_in(h, j), int_fan_out(h, j), h->act, h->alpha, bf, c.st));
+    prof_end(c);
+  }
+  if (h->route.tail_fused) {
+    // the last two hidden layers and the head run as ONE kernel (g2 stays on chip)
+    const int j0 = h->Li - 2, j1 = h->Li - 1;
+    prof_begin(c, "int16_fwd2_head");
+    DIB_CUDA_OK(dib_int16_fwd2_head(int16_in(c, j0), int_fan_in(h, j0), int_fan_in(h, j0), c.ws + h->w16_off[j0], c.params + h->intB[j0],
+                                    c.ws + h->w16_off[j1], c.params + h->intB[j1], c.ws + h->g16_off[j1], c.params + h->intW[h->Li],
+                                    c.params + h->intB[h->Li], h->act, h->out_act, h->alpha, h->loss, y, c.n, inv_batch, gscale, dg,
+                                    user_pred, c.ws + h->headpart_off, h->head_stride, c.ws + h->loss_part_off, c.ws + h->acc_part_off,
+                                    &h->head_used, bf, c.st));
+    DIB_CUDA_OK(finalize(h->head_used));
+    prof_end(c);
+    return 0;
+  }
+  const int Kh = h->int_arch[h->Li - 1];
+  h->head_used = h->head_blocks;
+  prof_begin(c, "int16_head_loss");
+  DIB_CUDA_OK(dib_int16_head(c.ws + h->g16_off[h->Li], Kh, Kh, c.params + h->intW[h->Li], c.params + h->intB[h->Li], h->out,
+                             h->out_act, h->act, h->alpha, h->loss, y, c.n, inv_batch, gscale, dg, Kh, user_pred, c.ws + h->headpart_off,
+                             h->head_stride, c.ws + h->loss_part_off, c.ws + h->acc_part_off, h->head_blocks, h->route.head1, bf, c.st));
+  DIB_CUDA_OK(finalize(h->head_blocks));
+  prof_end(c);
+  return 0;
+}
+
+int run_forward(const Ctx& c, const float* x, const float* y, const NoiseKey& nk, float inv_batch, float* user_pred,
+                float* user_emb, float* out_stats, bool enc_only = false) {
+  dib_model* h = c.h;
+  if (is_tc(h) && !h->route.int16) {      // TF32 GEMMs read the weights through a TF32-rounded copy
     prof_begin(c, "weights_tf32_shadow");
     DIB_CUDA_OK(dib_launch_round_copy(c.params, c.ws + h->wshadow_off, h->P, c.st));
     prof_end(c);
   }
-  // fused encoder path: only when the backward does not need the per-layer activations in HBM
-  const bool fused = h->fused_ok && rnd && (!training || h->fused_bwd_ok) && !h->force_unfused;
-  int nblk_kl = (int)DIB_CEIL_DIV((long long)c.n, (long long)kRowsPerBlock);
-  if (fused) {
-    const int ntiles = (int)DIB_CEIL_DIV((long long)c.n, 128ll);
-    long long want = (long long)h->F * ntiles;
-    DibEncFusedDesc d = h->fdesc;
-    d.logvar_offset = h->lv_off;
-    const long long cap = (long long)h->num_sms * dib_enc_fused_fwd_ctas_per_sm();
-    d.grid = (int)(want < cap ? want : cap);
-    nblk_kl = DIB_CEIL_DIV(d.grid, h->F);
-    prof_begin(c, "enc_pack_weights");
-    {
-      const long long zn = (long long)h->F * h->kl_stride, zcap = dib_enc_fused_pack_zero_capacity(h->F);
-      // the pack kernel also clears the KL partial table when it fits its grid
-      if (zn <= zcap) DIB_CUDA_OK(dib_enc_fused_pack(d, c.params, c.ws + h->pack_off, c.ws + h->kl_part_off, zn, c.st));
-      else {
-        DIB_CUDA_OK(dib_enc_fused_pack(d, c.params, c.ws + h->pack_off, nullptr, 0, c.st));
-        DIB_CUDA_OK(cudaMemsetAsync(c.ws + h->kl_part_off, 0, sizeof(float) * (size_t)zn, c.st));
-      }
-    }
-    prof_end(c);
-    DibEncFusedIO io;
-    io.params = c.params; io.packed = c.ws + h->pack_off; io.x = x; io.ldx = h->D; io.n = c.n;
-    io.eps = eps; io.seed = seed; io.step = step; io.step_dev = c.step_dev(); io.sample_offset = sample_offset;
-    io.emb = c.ws + h->emb.off; io.ldemb = h->emb.ld; io.user_emb = user_emb;
-    io.kl_part = c.ws + h->kl_part_off; io.kl_stride = h->kl_stride;
-    const bool i16 = h->int16_ok && !h->force_int32 && !enc_only;
-    if (i16) { io.emb = nullptr; io.emb16 = c.ws + h->emb16_off; io.ldemb16 = h->F * h->E; }
-    if (enc_only) io.emb = nullptr;      // the caller's network consumes user_emb; nothing downstream reads the workspace copy
-    prof_begin(c, "enc_fused_fwd");
-    DIB_CUDA_OK(dib_enc_fused_forward(d, io, c.st));
-    prof_end(c);
-    if (enc_only) {
-      DIB_CUDA_OK(dib_launch_finalize_stats(c.ws + h->kl_part_off, h->kl_stride, nblk_kl, c.ws + h->loss_part_off,
-                                            c.ws + h->acc_part_off, 0, h->F, c.n, 0, out_stats, c.st));
-      return 0;
-    }
-    if (i16) {
-      const int bf = h->precision == DIB_PREC_BF16 ? 1 : 0;
-      // ---------------- integration network on 16-bit activations + fused output head
-      prof_begin(c, "int16_pack_weights");
-      {
-        std::vector<const float*> wsrc; std::vector<void*> wdst; std::vector<long long> wn;
-        for (int j = 0; j < h->Li; ++j) {
-          wsrc.push_back(c.params + h->intW[j]); wdst.push_back(c.ws + h->w16_off[j]);
-          wn.push_back((long long)int_fan_in(h, j) * int_fan_out(h, j));
-        }
-        DIB_CUDA_OK(dib_int16_convert_many(wsrc.data(), wdst.data(), wn.data(), h->Li, bf, c.st));
-      }
-      prof_end(c);
-      const int Kh = h->int_arch[h->Li - 1];
-      const float gscale = training ? exp2f(ceilf(log2f(1.f / inv_batch))) : 1.f;
-      // single-output models: the last two hidden layers and the head run as ONE kernel (g2 stays on chip)
-      const bool fwd2 = h->Li >= 2 && dib_int16_fwd2_ok(int_fan_in(h, h->Li - 2), int_fan_out(h, h->Li - 2), int_fan_out(h, h->Li - 1), h->out);
-      const int n_plain = fwd2 ? h->Li - 2 : h->Li;
-      for (int j = 0; j < n_plain; ++j) {
-        prof_begin(c, "int16_fwd_l", j);
-        DIB_CUDA_OK(dib_int16_fwd(j == 0 ? (const void*)(c.ws + h->emb16_off) : (const void*)(c.ws + h->g16_off[j]), int_fan_in(h, j),
-                                  c.ws + h->w16_off[j], c.params + h->intB[j], c.ws + h->g16_off[j + 1], int_fan_out(h, j), c.n,
-                                  int_fan_in(h, j), int_fan_out(h, j), h->act, h->alpha, bf, c.st));
-        prof_end(c);
-      }
-      if (fwd2) {
-        const int j0 = h->Li - 2, j1 = h->Li - 1;
-        prof_begin(c, "int16_fwd2_head");
-        DIB_CUDA_OK(dib_int16_fwd2_head(j0 == 0 ? (const void*)(c.ws + h->emb16_off) : (const void*)(c.ws + h->g16_off[j0]), int_fan_in(h, j0),
-                                        int_fan_in(h, j0), c.ws + h->w16_off[j0], c.params + h->intB[j0], c.ws + h->w16_off[j1],
-                                        c.params + h->intB[j1], c.ws + h->g16_off[j1], c.params + h->intW[h->Li], c.params + h->intB[h->Li],
-                                        h->act, h->out_act, h->alpha, h->loss, y, c.n, inv_batch, gscale,
-                                        training ? (void*)(c.ws + h->dg16_off[h->Li]) : nullptr, user_pred, c.ws + h->headpart_off,
-                                        h->head_stride, c.ws + h->loss_part_off, c.ws + h->acc_part_off, &h->head_used, bf, c.st));
-        DIB_CUDA_OK(dib_launch_finalize_stats(c.ws + h->kl_part_off, h->kl_stride, nblk_kl, c.ws + h->loss_part_off,
-                                              c.ws + h->acc_part_off, h->head_used, h->F, c.n, y != nullptr, out_stats, c.st));
-        prof_end(c);
-        return 0;
-      }
-      h->head_used = h->head_blocks;
-      prof_begin(c, "int16_head_loss");
-      DIB_CUDA_OK(dib_int16_head(c.ws + h->g16_off[h->Li], Kh, Kh, c.params + h->intW[h->Li], c.params + h->intB[h->Li], h->out,
-                                 h->out_act, h->act, h->alpha, h->loss, y, c.n, inv_batch, gscale,
-                                 training ? (void*)(c.ws + h->dg16_off[h->Li]) : nullptr, Kh, user_pred, c.ws + h->headpart_off,
-                                 h->head_stride, c.ws + h->loss_part_off, c.ws + h->acc_part_off, h->head_blocks, bf, c.st));
-      DIB_CUDA_OK(dib_launch_finalize_stats(c.ws + h->kl_part_off, h->kl_stride, nblk_kl, c.ws + h->loss_part_off,
-                                            c.ws + h->acc_part_off, h->head_blocks, h->F, c.n, y != nullptr, out_stats, c.st));
-      prof_end(c);
-      return 0;
-    }
-  } else {
-  const NoiseKey nk{seed, step, sample_offset, training};
-  if (encode_all(c, x, h->D, rnd, nullptr, 0, &nk)) return 1;
-  DibReparamArgs ra;
-  ra.enc_out = c.ws + h->enc_out.off; ra.feat_stride = h->enc_out.feat_stride; ra.ldo = h->enc_out.ld;
-  ra.eps = eps; ra.seed = seed; ra.step = step; ra.step_dev = c.step_dev(); ra.sample_offset = sample_offset;
-  ra.F = h->F; ra.E = h->E; ra.n = c.n; ra.round_out = rnd;
-  prof_begin(c, "reparam_kl_fwd");
-  DIB_CUDA_OK(dib_launch_reparam_fwd(ra, c.ws + h->emb.off, h->emb.ld, user_emb, c.ws + h->kl_part_off, h->kl_stride, c.st));
-  prof_end(c);
+  int nblk_kl = 0;
+  if (forward_encoders(c, x, nk, user_emb, enc_only, &nblk_kl)) return 1;
   if (enc_only) {
     DIB_CUDA_OK(dib_launch_finalize_stats(c.ws + h->kl_part_off, h->kl_stride, nblk_kl, c.ws + h->loss_part_off,
                                           c.ws + h->acc_part_off, 0, h->F, c.n, 0, out_stats, c.st));
     return 0;
   }
-  }
-  for (int j = 0; j <= h->Li; ++j) {
-    prof_begin(c, "int_fwd_l", j);
-    if (gemm(c, DIB_GEMM_FWD, h->int_fwd[j], 1, int_fan_out(h, j), 0, 1, 0)) return 1;
-    prof_end(c);
-  }
-  prof_begin(c, "loss_stats");
-  DIB_CUDA_OK(dib_launch_loss(h->loss, h->out_act, h->alpha, c.ws + h->pred.off, h->pred.ld, y, h->out, c.n, inv_batch,
-                              training ? c.ws + h->d_pred.off : nullptr, user_pred, c.ws + h->loss_part_off,
-                              c.ws + h->acc_part_off, rnd, c.st));
-  const int nblk = (int)DIB_CEIL_DIV((long long)c.n, (long long)kRowsPerBlock);
-  DIB_CUDA_OK(dib_launch_finalize_stats(c.ws + h->kl_part_off, h->kl_stride, nblk_kl, c.ws + h->loss_part_off,
-                                        c.ws + h->acc_part_off, nblk, h->F, c.n, y != nullptr, out_stats, c.st));
-  prof_end(c);
-  return 0;
+  return forward_integration(c, y, inv_batch, nk.training, user_pred, out_stats, nblk_kl);
 }
 
 // every feature encoder on n rows of x (deterministic part: mu | logvar incl. the offset) into the enc_out workspace
@@ -511,6 +562,59 @@ int ib_weight(const Ctx& c, const float* beta_dev, const float* stats, float inv
   return 0;
 }
 
+// encoder backward from d emb -- fp32 (d_emb, ldd) or the fp16 copy the 16-bit integration backward leaves, already x the loss
+// scale (d_emb16) -- into the split-partial table: the encoder parameters' weight-gradient partials in rows [0, *nrows).
+// Relies on the workspace as the forward of the same (x, noise) left it.
+int backward_encoders(const Ctx& c, const float* x, const NoiseKey& nk, const float* d_emb, int ldd, const void* d_emb16,
+                      const float* beta_w, float inv_batch, const Split& sp, int* nrows) {
+  dib_model* h = c.h;
+  float* part = c.ws + h->part_off;
+  if (h->route.enc_fused) {
+    const long long p_enc = h->intW[0];
+    const long long want = (long long)h->F * DIB_CEIL_DIV((long long)c.n, 128ll);
+    DibEncFusedDesc d = h->fdesc;
+    d.grid = (int)(want < h->num_sms ? want : h->num_sms);
+    const int slots_max = DIB_CEIL_DIV(d.grid, h->F), slots_min = d.grid / h->F;
+    // features served by one CTA fewer leave their last slot unwritten: zero it (ENCODER range only -- the
+    // integration network's batch-split partials live in the same rows beyond p_enc)
+    for (int srow = slots_min; srow < slots_max; ++srow)
+      DIB_CUDA_OK(cudaMemsetAsync(part + (long long)srow * h->Pp, 0, sizeof(float) * (size_t)p_enc, c.st));
+    DibEncFusedBwdIO b;
+    b.d_emb = d_emb; b.ldd = ldd; b.d_emb16 = d_emb16; b.ldd16 = d_emb16 ? h->F * h->E : 0;
+    b.beta_dev = beta_w; b.inv_batch = inv_batch; b.gscale = loss_scale(inv_batch); b.part = part; b.split_stride = h->Pp;
+    prof_begin(c, "enc_fused_bwd");
+    DIB_CUDA_OK(dib_enc_fused_backward(d, fused_io(c, x, nk), b, c.st));
+    prof_end(c);
+    *nrows = slots_max;
+    return 0;
+  }
+  prof_begin(c, "reparam_kl_bwd");
+  DIB_CUDA_OK(dib_launch_reparam_bwd(reparam_args(c, nk), d_emb, ldd, beta_w, inv_batch, c.ws + h->d_out.off, c.st));
+  prof_end(c);
+  if (h->simple) {
+    prof_begin(c, "simple_enc_wgrad");
+    DIB_CUDA_OK(dib_launch_simple_enc_wgrad(x, h->D, h->d_xoff, c.ws + h->d_out.off, h->d_out.feat_stride, h->d_out.ld, h->F, h->E,
+                                            c.n, sp.nsplit, (int)sp.rps, part, h->Pp, c.st));
+    prof_end(c);
+  }
+  for (int j = h->L; j >= 0 && !h->simple; --j) {
+    prof_begin(c, "enc_wgrad_l", j);
+    if (gemm(c, DIB_GEMM_WGRAD, h->enc_wgrad[j], h->F, enc_fan_out(h, j), h->enc_maxK[j], sp.nsplit, (int)sp.rps)) return 1;
+    prof_end(c);
+    if (j >= 1) {
+      prof_begin(c, "enc_dgrad_l", j);
+      if (gemm(c, DIB_GEMM_DGRAD, h->enc_dgrad[j], h->F, h->enc_arch[j - 1], 0, 1, 0)) return 1;
+      if (h->drop > 0.f)                   // Dropout backward: the same keep mask, scaled
+        DIB_CUDA_OK(dib_launch_dropout(nullptr, c.ws + h->d_enc[j].off, h->d_enc[j].feat_stride, h->d_enc[j].ld, h->enc_arch[j - 1],
+                                       h->F, c.n, h->drop, nk.seed, nk.step, c.step_dev(), nk.sample_offset, j, -1, 1,
+                                       is_tc(h) ? 1 : 0, c.st));
+      prof_end(c);
+    }
+  }
+  *nrows = sp.nsplit;
+  return 0;
+}
+
 }  // namespace
 
 // =================================================================================================
@@ -520,21 +624,11 @@ extern "C" {
 
 uint64_t dib_launch_count(void) { return g_launches.load(); }
 
-// bring-up switch: 1 = never use the fused encoder kernels (compare fused vs unfused tensor-core paths)
+// bring-up switch (bit mask documented in include/dib_b200.h): this handle's reference kernels instead of the fused ones
 int dib_debug_force_unfused(dib_model* h, int32_t on) {
   if (!h) return fail("null model handle");
-  h->force_unfused = (on & 1) != 0;      // bit 0: unfused encoder kernels
-  h->force_int32 = (on & 2) != 0;        // bit 1: integration network on the fp32-storage TF32 kernels
+  set_route(h, on);
   return 0;
-}
-
-// kernel-variant switch for A/B measurements (keys documented in include/dib_b200.h)
-int dib_debug_set_variant(int32_t key, int32_t value) {
-  if (key == 1) { dib_int16_rb_set(value); return 0; }
-  if (key == 2) { dib_int16_head1_set(value); return 0; }
-  if (key == 3) { dib_int16_fwd2_set(value); return 0; }
-  if (key == 5) { dib_int16_dbg_set(value); return 0; }     // measurement only: wrong results
-  return fail("dib_debug_set_variant: unknown key");
 }
 
 int dib_profile_enable(dib_model* h, int32_t on) {
@@ -599,8 +693,7 @@ const char* dib_build_info(void) {
 int32_t dib_model_info(const dib_model* h, char* out, size_t out_bytes) {
   if (!h || !out || out_bytes < 2) { fail("dib_model_info: bad arguments"); return -1; }
   static const char* pn[] = {"fp32", "tf32", "bf16", "fp16"};
-  const bool fused = h->fused_ok && h->fused_bwd_ok && !h->force_unfused;
-  const bool i16 = fused && h->int16_ok && !h->force_int32;
+  const bool fused = h->route.enc_fused, i16 = h->route.int16;
   const char* k16 = h->precision == DIB_PREC_BF16 ? "bf16" : "f16";
   std::string s = std::string("precision=") + pn[h->precision];
   if (!is_tc(h)) s += " encoders=simt-fp32 integration=simt-fp32 operands=fp32 accumulate=fp32";
@@ -745,7 +838,6 @@ int dib_create(const dib_config* cfg, dib_model** out) {
         d.w0_off = lt; d.b0_off = lt + F; d.w1_off = lt + 2 * F; d.b1_off = lt + 3 * F; d.w2_off = lt + 4 * F;
         d.b2_off = lt + 5 * F; d.x_off = it; d.fdim = it + F;
         h->fused_ok = true;
-        h->fused_bwd_ok = true;
         // 16-bit integration path: hidden widths multiples of 128, last hidden width 256, narrow output head
         // (the fused head owns the compiled loss, so a caller-owned loss takes the TF32 integration kernels)
         bool iok = h->Li >= 1 && (h->F * h->E) % 64 == 0 && h->int_arch[h->Li - 1] == 256 && h->out <= 16 &&
@@ -755,6 +847,7 @@ int dib_create(const dib_config* cfg, dib_model** out) {
       }
     }
   }
+  set_route(h, 0);
   *out = h;
   return 0;
 }
@@ -794,7 +887,7 @@ int dib_forward(dib_model* h, const float* params, const float* x, const float* 
   if (!out_stats) return fail("dib_forward: out_stats is required");
   Ctx c{h, params, static_cast<float*>(workspace), static_cast<cudaStream_t>(stream), (int)n};
   if (n == 0) { DIB_CUDA_OK(cudaMemsetAsync(out_stats, 0, sizeof(float) * (h->F + 3), c.st)); return 0; }
-  return run_forward(c, x, y, eps, seed, step, sample_offset, 0.f, false, out_pred, out_emb, out_stats);
+  return run_forward(c, x, y, NoiseKey{eps, seed, step, sample_offset, false}, 0.f, out_pred, out_emb, out_stats);
 }
 
 int dib_encode_feature(dib_model* h, const float* params, int32_t feature, const float* x_i, int64_t n,
@@ -850,29 +943,23 @@ int dib_train_step_phased(dib_model* h, const float* params, const float* x, con
     return 0;
   }
   const bool nonlinear = h->kl_exp != 1.f || h->kl_scale != 1.f;
+  const NoiseKey nk{eps, seed, step, sample_offset, true};
   if (phA) {
-    if (run_forward(c, x, y, eps, seed, step, sample_offset, inv_global_batch, true, nullptr, nullptr, out_stats)) return 1;
+    if (run_forward(c, x, y, nk, inv_global_batch, nullptr, nullptr, out_stats)) return 1;
     const float* bw = nullptr;
     if (ib_weight(c, beta_dev, out_stats, inv_global_batch, &bw)) return 1;
   }
   // weight of the per-sample KL gradients in the encoder backward: beta, or d(beta*scale*KL^p)/dKL left in the workspace by phase 1
   const float* beta_w = nonlinear ? c.ws + h->beta_eff_off : beta_dev;
-
-  // deterministic split of the batch for the weight gradients
-  long long rps = DIB_CEIL_DIV((long long)n, (long long)kMaxSplits);
-  if (rps < 256) rps = 256;
-  rps = DIB_ROUND_UP(rps, 64);      // whole k-blocks of every WGRAD kernel (32 rows for the TF32 ones, 64 for the 16-bit ones)
-  const int nsplit = (int)DIB_CEIL_DIV((long long)n, rps);
+  const Split sp = batch_split(n);
   float* part = c.ws + h->part_off;
-
-  const bool fused_enc = h->fused_ok && h->fused_bwd_ok && !h->force_unfused;
-  const bool i16 = fused_enc && h->int16_ok && !h->force_int32;
-  const float gscale = exp2f(ceilf(log2f(1.f / inv_global_batch)));
+  const dib_model::Route& r = h->route;
 
   std::vector<DibReduceSeg> segs;          // fixed-order reductions of the step; whole steps (phases == 3) run them as ONE launch at the end
   // ---------------------------------------------------------------- phase 1: integration network backward
-  if (phA && i16) {
+  if (phA && r.int16) {
     const int bf = h->precision == DIB_PREC_BF16 ? 1 : 0;
+    const float gscale = loss_scale(inv_global_batch);
     const int Kh = h->int_arch[h->Li - 1];
     const int row_tiles = (int)DIB_CEIL_DIV((long long)n, 128ll);
     const long long p_head = h->intW[h->Li];
@@ -893,8 +980,7 @@ int dib_train_step_phased(dib_model* h, const float* params, const float* x, con
         segs.push_back({c.ws + h->dbpart_off + (long long)j * h->dbpart_layer, K, row_tiles, K, 1.f / gscale, grads_flat + h->intB[j - 1]});
       prof_end(c);
     }
-    std::vector<int> nsplit_of(h->Li, nsplit);
-    auto in_of = [&](int j) { return j == 0 ? (const void*)(c.ws + h->emb16_off) : (const void*)(c.ws + h->g16_off[j]); };
+    std::vector<int> nsplit_of(h->Li, sp.nsplit);
     auto tiles_of = [&](int j) { return DIB_CEIL_DIV(int_fan_in(h, j), 128) * DIB_CEIL_DIV(int_fan_out(h, j), 128); };
     int j = h->Li - 1;
     for (; j >= 1; j -= 2) {          // layers (j, j-1) together
@@ -906,22 +992,22 @@ int dib_train_step_phased(dib_model* h, const float* params, const float* x, con
       const int ns2 = (int)DIB_CEIL_DIV((long long)n, rps2);
       nsplit_of[j] = nsplit_of[j - 1] = ns2;
       prof_begin(c, "int16_wgrad_pair_l", j - 1);
-      DIB_CUDA_OK(dib_int16_wgrad_pair(in_of(j), int_fan_in(h, j), c.ws + h->dg16_off[j + 1], int_fan_out(h, j), part + h->intW[j], ns2, (int)rps2,
-                                       in_of(j - 1), int_fan_in(h, j - 1), c.ws + h->dg16_off[j], int_fan_out(h, j - 1), part + h->intW[j - 1], ns2,
-                                       (int)rps2, (int)n, h->Pp, 1.f / gscale, bf, c.st));
+      DIB_CUDA_OK(dib_int16_wgrad_pair(int16_in(c, j), int_fan_in(h, j), c.ws + h->dg16_off[j + 1], int_fan_out(h, j), part + h->intW[j],
+                                       ns2, (int)rps2, int16_in(c, j - 1), int_fan_in(h, j - 1), c.ws + h->dg16_off[j], int_fan_out(h, j - 1),
+                                       part + h->intW[j - 1], ns2, (int)rps2, (int)n, h->Pp, 1.f / gscale, bf, c.st));
       prof_end(c);
     }
     if (j == 0) {
       prof_begin(c, "int16_wgrad_l", 0);
-      DIB_CUDA_OK(dib_int16_wgrad(in_of(0), int_fan_in(h, 0), c.ws + h->dg16_off[1], int_fan_out(h, 0), part + h->intW[0], nullptr, (int)n,
-                                  int_fan_in(h, 0), int_fan_out(h, 0), nsplit, (int)rps, h->Pp, 1.f / gscale, bf, c.st));
+      DIB_CUDA_OK(dib_int16_wgrad(int16_in(c, 0), int_fan_in(h, 0), c.ws + h->dg16_off[1], int_fan_out(h, 0), part + h->intW[0], (int)n,
+                                  int_fan_in(h, 0), int_fan_out(h, 0), sp.nsplit, (int)sp.rps, h->Pp, 1.f / gscale, bf, c.st));
       prof_end(c);
     }
     prof_begin(c, "int_split_reduce");
     for (int q = 0; q < h->Li; ++q)     // hidden-layer kernels: batch-split partials
       segs.push_back({part + h->intW[q], h->Pp, nsplit_of[q], (long long)int_fan_in(h, q) * int_fan_out(h, q), 1.f, grads_flat + h->intW[q]});
     segs.push_back({c.ws + h->headpart_off, h->head_stride, h->head_used, h->P - p_head, 1.f, grads_flat + p_head});
-    if (!(phB && fused_enc)) {               // phase-1-only call (or unfused encoders): reduce now
+    if (!phB) {               // phase-1-only call: reduce now (the 16-bit path implies the fused encoders, which reduce with these)
       DIB_CUDA_OK(dib_launch_reduce_segments(segs.data(), (int)segs.size(), c.st));
       segs.clear();
     }
@@ -930,75 +1016,31 @@ int dib_train_step_phased(dib_model* h, const float* params, const float* x, con
     // integration network backward (GradientTape through models.py:122)
     for (int j = h->Li; j >= 0; --j) {
       prof_begin(c, "int_wgrad_l", j);
-      if (gemm(c, DIB_GEMM_WGRAD, h->int_wgrad[j], 1, int_fan_out(h, j), int_fan_in(h, j), nsplit, (int)rps)) return 1;
+      if (gemm(c, DIB_GEMM_WGRAD, h->int_wgrad[j], 1, int_fan_out(h, j), int_fan_in(h, j), sp.nsplit, (int)sp.rps)) return 1;
       prof_end(c);
       prof_begin(c, "int_dgrad_l", j);
       if (gemm(c, DIB_GEMM_DGRAD, h->int_dgrad[j], 1, int_fan_in(h, j), 0, 1, 0)) return 1;
       prof_end(c);
     }
     prof_begin(c, "int_split_reduce");
-    DIB_CUDA_OK(dib_launch_reduce_partials(part + p_enc, h->Pp, nsplit, h->P - p_enc, grads_flat + p_enc, c.st));
+    DIB_CUDA_OK(dib_launch_reduce_partials(part + p_enc, h->Pp, sp.nsplit, h->P - p_enc, grads_flat + p_enc, c.st));
     prof_end(c);
   }
   if (!phB) return 0;
 
   // ---------------------------------------------------------------- phase 2: encoder backward
-  if (fused_enc) {
-    const int ntiles = (int)DIB_CEIL_DIV((long long)n, 128ll);
-    const long long want = (long long)h->F * ntiles;
-    DibEncFusedDesc d = h->fdesc;
-    d.grid = (int)(want < h->num_sms ? want : h->num_sms);
-    const int slots_max = DIB_CEIL_DIV(d.grid, h->F), slots_min = d.grid / h->F;
-    // features served by one CTA fewer leave their last slot unwritten: zero it (ENCODER range only -- the
-    // integration network's batch-split partials live in the same rows beyond p_enc)
-    for (int srow = slots_min; srow < slots_max; ++srow)
-      DIB_CUDA_OK(cudaMemsetAsync(part + (long long)srow * h->Pp, 0, sizeof(float) * (size_t)p_enc, c.st));
-    DibEncFusedIO io;
-    io.params = c.params; io.packed = c.ws + h->pack_off; io.x = x; io.ldx = h->D; io.n = n;
-    io.eps = eps; io.seed = seed; io.step = step; io.step_dev = c.step_dev(); io.sample_offset = sample_offset;
-    io.emb = nullptr; io.ldemb = 0; io.user_emb = nullptr; io.kl_part = nullptr; io.kl_stride = 0;
-    DibEncFusedBwdIO b;
-    if (i16) { b.d_emb = nullptr; b.ldd = 0; b.d_emb16 = c.ws + h->demb16_off; b.ldd16 = h->F * h->E; }
-    else { b.d_emb = c.ws + h->d_emb.off; b.ldd = h->d_emb.ld; }
-    b.beta_dev = beta_w; b.inv_batch = inv_global_batch; b.gscale = gscale; b.part = part; b.split_stride = h->Pp;
-    prof_begin(c, "enc_fused_bwd");
-    DIB_CUDA_OK(dib_enc_fused_backward(d, io, b, c.st));
-    prof_end(c);
-    prof_begin(c, "enc_split_reduce");
-    segs.push_back({part, h->Pp, slots_max, p_enc, 1.f, grads_flat});
-    DIB_CUDA_OK(dib_launch_reduce_segments(segs.data(), (int)segs.size(), c.st));
-    prof_end(c);
-    return 0;
-  }
-  DibReparamArgs ra;
-  ra.enc_out = c.ws + h->enc_out.off; ra.feat_stride = h->enc_out.feat_stride; ra.ldo = h->enc_out.ld;
-  ra.eps = eps; ra.seed = seed; ra.step = step; ra.step_dev = c.step_dev(); ra.sample_offset = sample_offset;
-  ra.F = h->F; ra.E = h->E; ra.n = n; ra.round_out = is_tc(h) ? 1 : 0;
-  prof_begin(c, "reparam_kl_bwd");
-  DIB_CUDA_OK(dib_launch_reparam_bwd(ra, c.ws + h->d_emb.off, h->d_emb.ld, beta_w, inv_global_batch,
-                                     c.ws + h->d_out.off, c.st));
-  prof_end(c);
-  if (h->simple) {
-    prof_begin(c, "simple_enc_wgrad");
-    DIB_CUDA_OK(dib_launch_simple_enc_wgrad(x, h->D, h->d_xoff, c.ws + h->d_out.off, h->d_out.feat_stride, h->d_out.ld, h->F, h->E,
-                                            n, nsplit, (int)rps, part, h->Pp, c.st));
-    prof_end(c);
-  }
-  for (int j = h->L; j >= 0 && !h->simple; --j) {
-    prof_begin(c, "enc_wgrad_l", j);
-    if (gemm(c, DIB_GEMM_WGRAD, h->enc_wgrad[j], h->F, enc_fan_out(h, j), h->enc_maxK[j], nsplit, (int)rps)) return 1;
-    prof_end(c);
-    if (j >= 1) {
-      prof_begin(c, "enc_dgrad_l", j);
-      if (gemm(c, DIB_GEMM_DGRAD, h->enc_dgrad[j], h->F, h->enc_arch[j - 1], 0, 1, 0)) return 1;
-      if (h->drop > 0.f)                   // Dropout backward: the same keep mask, scaled
-        DIB_CUDA_OK(dib_launch_dropout(nullptr, c.ws + h->d_enc[j].off, h->d_enc[j].feat_stride, h->d_enc[j].ld, h->enc_arch[j - 1],
-                                       h->F, n, h->drop, seed, step, c.step_dev(), sample_offset, j, -1, 1, is_tc(h) ? 1 : 0, c.st));
-      prof_end(c);
-    }
-  }
+  int nrows = 0;
+  const bool d16 = r.int16;                // the 16-bit integration backward leaves d emb in fp16
+  if (backward_encoders(c, x, nk, d16 ? nullptr : c.ws + h->d_emb.off, d16 ? 0 : h->d_emb.ld, d16 ? c.ws + h->demb16_off : nullptr,
+                        beta_w, inv_global_batch, sp, &nrows))
+    return 1;
   prof_begin(c, "enc_split_reduce");
-  DIB_CUDA_OK(dib_launch_reduce_partials(part, h->Pp, nsplit, p_enc, grads_flat, c.st));
+  if (r.enc_fused) {
+    segs.push_back({part, h->Pp, nrows, p_enc, 1.f, grads_flat});
+    DIB_CUDA_OK(dib_launch_reduce_segments(segs.data(), (int)segs.size(), c.st));
+  } else {
+    DIB_CUDA_OK(dib_launch_reduce_partials(part, h->Pp, nrows, p_enc, grads_flat, c.st));
+  }
   prof_end(c);
   return 0;
 }
@@ -1079,7 +1121,7 @@ int dib_encoders_forward(dib_model* h, const float* params, const float* x, int6
   if (!out_emb || !out_stats) return fail("dib_encoders_forward: out_emb and out_stats are required");
   Ctx c{h, params, static_cast<float*>(workspace), static_cast<cudaStream_t>(stream), (int)n};
   if (n == 0) { DIB_CUDA_OK(cudaMemsetAsync(out_stats, 0, sizeof(float) * (h->F + 3), c.st)); return 0; }
-  return run_forward(c, x, nullptr, eps, seed, step, sample_offset, 0.f, false, nullptr, out_emb, out_stats, true);
+  return run_forward(c, x, nullptr, NoiseKey{eps, seed, step, sample_offset, false}, 0.f, nullptr, out_emb, out_stats, true);
 }
 
 int dib_encoders_backward(dib_model* h, const float* params, const float* x, const float* d_emb, int64_t n,
@@ -1092,56 +1134,13 @@ int dib_encoders_backward(dib_model* h, const float* params, const float* x, con
   DIB_CUDA_OK(cudaMemsetAsync(grads_flat, 0, sizeof(float) * h->P, c.st));
   if (n == 0) { DIB_CUDA_OK(cudaMemsetAsync(out_stats, 0, sizeof(float) * (h->F + 3), c.st)); return 0; }
   // the forward is recomputed here (training mode keeps what the backward needs); user_emb is not needed again
-  if (run_forward(c, x, nullptr, eps, seed, step, sample_offset, inv_global_batch, true, nullptr, nullptr, out_stats, true)) return 1;
+  const NoiseKey nk{eps, seed, step, sample_offset, true};
+  if (run_forward(c, x, nullptr, nk, inv_global_batch, nullptr, nullptr, out_stats, true)) return 1;
   const float* bw = beta_dev;
   if (ib_weight(c, beta_dev, out_stats, inv_global_batch, &bw)) return 1;
-  long long rps = DIB_CEIL_DIV((long long)n, (long long)kMaxSplits);
-  if (rps < 256) rps = 256;
-  rps = DIB_ROUND_UP(rps, 64);      // whole k-blocks of every WGRAD kernel (32 rows for the TF32 ones, 64 for the 16-bit ones)
-  const int nsplit = (int)DIB_CEIL_DIV((long long)n, rps);
-  const long long p_enc = h->intW[0];
-  const int FE = h->F * h->E;
-  const bool fused = h->fused_ok && h->fused_bwd_ok && !h->force_unfused;
-  float* part = c.ws + h->part_off;
-  if (fused) {
-    const int ntiles = (int)DIB_CEIL_DIV((long long)n, 128ll);
-    const long long want = (long long)h->F * ntiles;
-    DibEncFusedDesc d = h->fdesc;
-    d.logvar_offset = h->lv_off;
-    d.grid = (int)(want < h->num_sms ? want : h->num_sms);
-    const int slots_max = DIB_CEIL_DIV(d.grid, h->F), slots_min = d.grid / h->F;
-    for (int srow = slots_min; srow < slots_max; ++srow)
-      DIB_CUDA_OK(cudaMemsetAsync(part + (long long)srow * h->Pp, 0, sizeof(float) * (size_t)p_enc, c.st));
-    DibEncFusedIO io;
-    io.params = c.params; io.packed = c.ws + h->pack_off; io.x = x; io.ldx = h->D; io.n = n;
-    io.eps = eps; io.seed = seed; io.step = step; io.step_dev = c.step_dev(); io.sample_offset = sample_offset;
-    io.emb = nullptr; io.ldemb = 0; io.user_emb = nullptr; io.kl_part = nullptr; io.kl_stride = 0;
-    DibEncFusedBwdIO b;
-    b.d_emb = d_emb; b.ldd = FE; b.beta_dev = bw; b.inv_batch = inv_global_batch;
-    b.gscale = exp2f(ceilf(log2f(1.f / inv_global_batch)));
-    b.part = part; b.split_stride = h->Pp;
-    DIB_CUDA_OK(dib_enc_fused_backward(d, io, b, c.st));
-    DIB_CUDA_OK(dib_launch_reduce_partials(part, h->Pp, slots_max, p_enc, grads_flat, c.st));
-    return 0;
-  }
-  DibReparamArgs ra;
-  ra.enc_out = c.ws + h->enc_out.off; ra.feat_stride = h->enc_out.feat_stride; ra.ldo = h->enc_out.ld;
-  ra.eps = eps; ra.seed = seed; ra.step = step; ra.step_dev = c.step_dev(); ra.sample_offset = sample_offset;
-  ra.F = h->F; ra.E = h->E; ra.n = n; ra.round_out = is_tc(h) ? 1 : 0;
-  DIB_CUDA_OK(dib_launch_reparam_bwd(ra, d_emb, FE, bw, inv_global_batch, c.ws + h->d_out.off, c.st));
-  if (h->simple) {
-    DIB_CUDA_OK(dib_launch_simple_enc_wgrad(x, h->D, h->d_xoff, c.ws + h->d_out.off, h->d_out.feat_stride, h->d_out.ld, h->F, h->E,
-                                            n, nsplit, (int)rps, part, h->Pp, c.st));
-  } else {
-    for (int j = h->L; j >= 0; --j) {
-      if (gemm(c, DIB_GEMM_WGRAD, h->enc_wgrad[j], h->F, enc_fan_out(h, j), h->enc_maxK[j], nsplit, (int)rps)) return 1;
-      if (j >= 1 && gemm(c, DIB_GEMM_DGRAD, h->enc_dgrad[j], h->F, h->enc_arch[j - 1], 0, 1, 0)) return 1;
-      if (j >= 1 && h->drop > 0.f)
-        DIB_CUDA_OK(dib_launch_dropout(nullptr, c.ws + h->d_enc[j].off, h->d_enc[j].feat_stride, h->d_enc[j].ld, h->enc_arch[j - 1],
-                                       h->F, n, h->drop, seed, step, c.step_dev(), sample_offset, j, -1, 1, is_tc(h) ? 1 : 0, c.st));
-    }
-  }
-  DIB_CUDA_OK(dib_launch_reduce_partials(part, h->Pp, nsplit, p_enc, grads_flat, c.st));
+  int nrows = 0;
+  if (backward_encoders(c, x, nk, d_emb, h->F * h->E, nullptr, bw, inv_global_batch, batch_split(n), &nrows)) return 1;
+  DIB_CUDA_OK(dib_launch_reduce_partials(c.ws + h->part_off, h->Pp, nrows, h->intW[0], grads_flat, c.st));
   return 0;
 }
 

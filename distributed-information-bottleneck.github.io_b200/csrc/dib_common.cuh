@@ -47,6 +47,23 @@ __device__ __forceinline__ float dib_act_grad(int act, float h, float alpha) {
   }
 }
 
+// One output of the compiled loss and metrics=['accuracy'] for target t: BCE on logits, keras.backend.binary_crossentropy
+// on probabilities, or MSE (every other loss).  Adds the loss term to l and the accuracy hit to acc and returns d loss / d z,
+// all unscaled: the callers apply 1/out, 1/batch and the output activation's derivative.  The sum is formed inside each
+// branch so that it contracts with the term (l += d * d is one FMA).  A caller that wants the bare term starts from l = -0.f,
+// which x + -0.f leaves exact.  The softmax cross-entropy couples the outputs and stays with its callers.
+__device__ __forceinline__ float dib_loss_add(int loss, float z, float t, float& l, float& acc) {
+  float g;
+  if (loss == DIB_LOSS_BCE_LOGITS) { l += fmaxf(z, 0.f) - z * t + log1pf(expf(-fabsf(z))); g = 1.f / (1.f + expf(-z)) - t; }
+  else if (loss == DIB_LOSS_BCE_PROBS) {
+    const float ep = 1e-7f, pc = fminf(fmaxf(z, ep), 1.f - ep);
+    l -= t * logf(pc + ep) + (1.f - t) * logf(1.f - pc + ep);
+    g = (z > ep && z < 1.f - ep) ? -t / (pc + ep) + (1.f - t) / (1.f - pc + ep) : 0.f;
+  } else { const float d = z - t; l += d * d; g = 2.f * d; }
+  acc += ((z > 0.5f ? 1.f : 0.f) == t) ? 1.f : 0.f;
+  return g;
+}
+
 // ---------------------------------------------------------------------------------------------
 // Philox4x32-10 noise; contract documented in oracle/philox.py (the CPU restatement used by tests).
 // ---------------------------------------------------------------------------------------------

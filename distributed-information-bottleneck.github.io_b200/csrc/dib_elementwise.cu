@@ -160,21 +160,8 @@ dib_loss_kernel(int loss, int out_act, float alpha, const float* __restrict__ pr
       } else {
         const float* yy = y + row * out_dim;
         for (int j = 0; j < out_dim; ++j) {
-          const float zz = z[j], t = yy[j];
-          float g;
-          if (loss == DIB_LOSS_BCE_LOGITS) {
-            l += fmaxf(zz, 0.f) - zz * t + log1pf(expf(-fabsf(zz)));
-            g = 1.f / (1.f + expf(-zz)) - t;
-          } else if (loss == DIB_LOSS_BCE_PROBS) {          // keras.backend.binary_crossentropy on probabilities
-            const float ep = 1e-7f, pc = fminf(fmaxf(zz, ep), 1.f - ep);
-            l -= t * logf(pc + ep) + (1.f - t) * logf(1.f - pc + ep);
-            g = (zz > ep && zz < 1.f - ep) ? -t / (pc + ep) + (1.f - t) / (1.f - pc + ep) : 0.f;
-          } else {
-            const float d = zz - t;
-            l += d * d;
-            g = 2.f * d;
-          }
-          acc += ((zz > 0.5f ? 1.f : 0.f) == t) ? 1.f : 0.f;
+          const float zz = z[j];
+          const float g = dib_loss_add(loss, zz, yy[j], l, acc);
           if (dz) dz[j] = dib_maybe_round(g * inv_out * inv_batch * dib_act_grad(out_act, zz, alpha), round_out);
         }
         l *= inv_out;
@@ -223,34 +210,6 @@ __global__ void dib_reduce_partials_kernel(const float* __restrict__ part, long 
   }
   for (; k < nsplit; ++k) s += part[(long long)k * split_stride + i];
   out[i] = s;
-}
-
-// out[i] = scale * sum_rows part[row][i] for MANY rows and few columns: 32 outputs x 8 row lanes per block, fixed order
-__global__ void __launch_bounds__(256)
-dib_reduce_tall_kernel(const float* __restrict__ part, long long row_stride, int nrows, long long count, float scale,
-                       float* __restrict__ out) {
-  __shared__ float red[8][32];
-  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-  const long long i = (long long)blockIdx.x * 32 + tx;
-  float s = 0.f;
-  if (i < count) {
-    int r = ty;
-    for (; r + 56 < nrows; r += 64) {
-      float v[8];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) v[u] = part[(long long)(r + 8 * u) * row_stride + i];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) s += v[u];
-    }
-    for (; r < nrows; r += 8) s += part[(long long)r * row_stride + i];
-  }
-  red[ty][tx] = s;
-  __syncthreads();
-  if (ty == 0 && i < count) {
-    float t = 0.f;
-    for (int k = 0; k < 8; ++k) t += red[k][tx];
-    out[i] = t * scale;
-  }
 }
 
 __global__ void dib_round_copy_kernel(const float* __restrict__ src, float* __restrict__ dst, long long count) {
@@ -597,14 +556,6 @@ cudaError_t dib_launch_reduce_segments(const DibReduceSeg* segs, int nseg, cudaS
     dib_reduce_segments_kernel<<<nb, 256, 0, st>>>(A);
     dib_note_launch();
   }
-  return cudaGetLastError();
-}
-
-cudaError_t dib_launch_reduce_tall(const float* part, long long row_stride, int nrows, int64_t count, float scale, float* out,
-                                   cudaStream_t st) {
-  if (count <= 0) return cudaSuccess;
-  dib_reduce_tall_kernel<<<nblocks(count, 32), 256, 0, st>>>(part, row_stride, nrows, count, scale, out);
-  dib_note_launch();
   return cudaGetLastError();
 }
 

@@ -7,8 +7,10 @@
 //     (scaled back by 1/S).
 //   * dib_int16_head_kernel: the narrow output layer (out <= 16) fused with everything around it -- logits, compiled
 //     loss + accuracy, d loss / d logits, the dgrad into the last hidden layer (incl. its act') and the output layer's
-//     own weight/bias gradients -- one pass over the last hidden activation.
+//     own weight/bias gradients -- one pass over the last hidden activation.  dib_int16_head1_kernel: the same for out = 1.
 //   * dib_int16_fwd2_kernel: the last two 256-wide hidden layers and the single-output head of models with out = 1.
+// Which tail and which head kernel run is the caller's choice (the model handle's route in dib_api.cu); nothing here
+// reads process-wide state.
 // Gradient operands are scaled by the power-of-two loss scale S (see dib_enc_fused.cu) to stay inside fp16 range.
 //
 // The GEMM kernels are warp-specialised: warps 0..7 are two consumer warpgroups (warpgroup g computes rows [64 g, 64 g + 64)
@@ -17,20 +19,16 @@
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
-#include <stdlib.h>
 
 #include "dib_common.cuh"
 #include "dib_kernels.h"
 #include "dib_sm90.cuh"
 
-int dib_int16_rb_enabled();
-int dib_int16_head1_enabled();
-
 namespace {
 
 using namespace sm90;
 
-constexpr int kBM = 128, kBN = 128, kBK = 64, kStages = 3, kRbStages = 4;
+constexpr int kBM = 128, kBN = 128, kBK = 64, kStages = 3;
 constexpr int kABytes = kBM * 128, kBBytes = kBN * 128, kStageBytes = kABytes + kBBytes;
 constexpr int kConsumers = 256, kGemmThreads = kConsumers + 32;
 constexpr int kProducerWarp = kConsumers / 32;
@@ -44,7 +42,6 @@ struct Int16Args {
   int M, T, C, R, act;
   float alpha, out_scale;
   int nsplit, rows_per_split; long long split_stride;
-  int dbg;                                    // measurement only (dib_debug_set_variant key 5): 1 = skip the epilogue's global stores
 };
 
 template <bool BF16>
@@ -80,26 +77,18 @@ __device__ __forceinline__ float quad_col_sum(float v) {
 
 // Persistent: each CTA walks tiles blockIdx.x, +gridDim.x, ...; the shared-memory stage ring runs across tiles, and two
 // CTAs per SM let one CTA's epilogue overlap the other's mainloop.
-// RB (FWD / DGRAD only): "resident B" -- each CTA owns ONE column tile, loads its [K x 128] slice of the weights once and
-// streams only the activation tiles; the MMAs and the epilogue are those of the streamed variant, so the results are
-// bit-identical.
-template <int MODE, bool BF16, bool RB>
-__global__ void __launch_bounds__(kGemmThreads, RB ? 1 : 2)
+template <int MODE, bool BF16>
+__global__ void __launch_bounds__(kGemmThreads, 2)
 dib_int16_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const Int16Args a,
-                      const __grid_constant__ CUtensorMap mapA2, const __grid_constant__ CUtensorMap mapB2, const Int16Args a2, int nkb) {
+                      const __grid_constant__ CUtensorMap mapA2, const __grid_constant__ CUtensorMap mapB2, const Int16Args a2) {
   // (a2, mapA2, mapB2): an optional SECOND weight-gradient problem walked by the same launch (a2.nsplit > 0, WGRAD only): the two
   // layers' tiles together fill one wave of CTAs, which neither fills alone
-  static_assert(!RB || MODE != DIB_GEMM_WGRAD, "resident-B variant: FWD / DGRAD only");
   constexpr bool A_MN = (MODE == DIB_GEMM_WGRAD), B_MN = (MODE != DIB_GEMM_DGRAD);
-  constexpr int S = RB ? kRbStages : kStages;
-  constexpr uint32_t kStep = RB ? kABytes : kStageBytes;          // bytes per ring stage
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t sb = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t sBres = sb, ring = RB ? sb + nkb * kBBytes : sb;  // RB: resident weight slice, then the A ring
-  const uint32_t bar_base = ring + S * kStep;
+  const uint32_t ring = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t bar_base = ring + kStages * kStageBytes;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (S + s); };
-  const uint32_t bfull_bar = bar_base + 8u * (2 * S);
+  auto empty_bar = [&](int s) { return bar_base + 8u * (kStages + s); };
 
   __shared__ float colsum_s[kConsumers / 32][kBN];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -109,14 +98,10 @@ dib_int16_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
   const int ntile0 = tiles_r * tiles_c * nsp;
   const bool two = (MODE == DIB_GEMM_WGRAD) && a2.nsplit > 0;
   const int tiles_r2 = two ? DIB_CEIL_DIV(a2.R, kBM) : 0, tiles_c2 = two ? DIB_CEIL_DIV(a2.C, kBN) : 0;
-  const int ntile = RB ? tiles_r : ntile0 + tiles_r2 * tiles_c2 * (two ? a2.nsplit : 0);
-  // RB: this CTA's fixed column tile and its row tiles: blockIdx.x = col + tiles_c * k  (gridDim.x is a multiple of tiles_c)
-  const int rb_c0 = RB ? (blockIdx.x % tiles_c) * kBN : 0;
-  const int first = RB ? blockIdx.x / tiles_c : blockIdx.x, stride = RB ? gridDim.x / tiles_c : gridDim.x;
+  const int ntile = ntile0 + tiles_r2 * tiles_c2 * (two ? a2.nsplit : 0);
 
   int prob = 0;                                     // which problem the tile last decoded belongs to (per thread)
   auto decode = [&](int tile, int& r0, int& c0, int& split, int& t_begin, int& nk) {
-    if (RB) { prob = 0; split = 0; r0 = tile * kBM; c0 = rb_c0; t_begin = 0; nk = nkb; return; }
     prob = (two && tile >= ntile0) ? 1 : 0;
     if (prob) tile -= ntile0;
     const int tr = prob ? tiles_r2 : tiles_r, tcn = prob ? tiles_c2 : tiles_c;
@@ -133,8 +118,7 @@ dib_int16_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
   };
 
   if (tid == 0) {
-    for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kEmptyArrivals); }
-    mbar_init(bfull_bar, 1);
+    for (int s = 0; s < kStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kEmptyArrivals); }
     fence_barrier_init();
   }
   __syncthreads();
@@ -144,32 +128,22 @@ dib_int16_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
     if (lane == 0) {
       tma_prefetch_desc(&mapA); tma_prefetch_desc(&mapB);
       if (two) { tma_prefetch_desc(&mapA2); tma_prefetch_desc(&mapB2); }
-      if constexpr (RB) {                           // the weight slice of this column tile, once
-        mbar_expect_tx(bfull_bar, (uint32_t)(nkb * kBBytes));
-        for (int k = 0; k < nkb; ++k) {
-          // one box per k-block: FWD [2 panels][64 k-rows][128 B] (MN-major), DGRAD [128 rows][128 B] (K-major)
-          if constexpr (B_MN) tma_load_3d(sBres + k * kBBytes, &mapB, bfull_bar, 0, k * kBK, rb_c0 / 64);
-          else                tma_load_2d(sBres + k * kBBytes, &mapB, bfull_bar, k * kBK, rb_c0);
-        }
-      }
       uint32_t s = 0, ph = 0;
-      for (int tile = first; tile < ntile; tile += stride) {
+      for (int tile = blockIdx.x; tile < ntile; tile += gridDim.x) {
         int r0, c0, split, t_begin, nk;
         decode(tile, r0, c0, split, t_begin, nk);
         const CUtensorMap* mA = prob ? &mapA2 : &mapA;
         const CUtensorMap* mB = prob ? &mapB2 : &mapB;
         for (int k = 0; k < nk; ++k) {
           mbar_wait(empty_bar(s), ph ^ 1);
-          mbar_expect_tx(full_bar(s), kStep);
-          const uint32_t a_dst = ring + s * kStep, b_dst = a_dst + kABytes;
+          mbar_expect_tx(full_bar(s), kStageBytes);
+          const uint32_t a_dst = ring + s * kStageBytes, b_dst = a_dst + kABytes;
           const int t0 = t_begin + k * kBK;
           if constexpr (A_MN) tma_load_3d(a_dst, mA, full_bar(s), 0, t0, r0 / 64);
           else                tma_load_2d(a_dst, mA, full_bar(s), t0, r0);
-          if constexpr (!RB) {
-            if constexpr (B_MN) tma_load_3d(b_dst, mB, full_bar(s), 0, t0, c0 / 64);
-            else                tma_load_2d(b_dst, mB, full_bar(s), t0, c0);
-          }
-          if (++s == S) { s = 0; ph ^= 1; }
+          if constexpr (B_MN) tma_load_3d(b_dst, mB, full_bar(s), 0, t0, c0 / 64);
+          else                tma_load_2d(b_dst, mB, full_bar(s), t0, c0);
+          if (++s == kStages) { s = 0; ph ^= 1; }
         }
       }
     }
@@ -177,9 +151,8 @@ dib_int16_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
     // ============================================================== consumer warpgroups: MMAs + epilogue
     const int wg = tid >> 7, q = lane & 3;
     const int rb = 64 * wg + 16 * (warp & 3) + (lane >> 2);       // tile row of this thread's accumulator elements
-    if constexpr (RB) mbar_wait(bfull_bar, 0);
     uint32_t s = 0, ph = 0;
-    for (int tile = first; tile < ntile; tile += stride) {
+    for (int tile = blockIdx.x; tile < ntile; tile += gridDim.x) {
       int r0, c0, split, t_begin, nk;
       decode(tile, r0, c0, split, t_begin, nk);
       float acc[64];
@@ -189,8 +162,8 @@ dib_int16_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
         uint32_t prev = 0;
         for (int k = 0; k < nk; ++k) {
           mbar_wait(full_bar(s), ph);
-          const uint32_t a_base = ring + s * kStep;
-          const uint32_t b_base = RB ? sBres + k * kBBytes : a_base + kABytes;
+          const uint32_t a_base = ring + s * kStageBytes;
+          const uint32_t b_base = a_base + kABytes;
           wgmma_fence();
 #pragma unroll
           for (int kk = 0; kk < kBK / 16; ++kk) {
@@ -202,7 +175,7 @@ dib_int16_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
           wgmma_wait<1>();                                        // the previous stage's MMAs have read their operands
           if (k > 0 && lane == 0) mbar_arrive(empty_bar(prev));
           prev = s;
-          if (++s == S) { s = 0; ph ^= 1; }
+          if (++s == kStages) { s = 0; ph ^= 1; }
         }
         wgmma_wait<0>();
         if (lane == 0) mbar_arrive(empty_bar(prev));
@@ -225,7 +198,7 @@ dib_int16_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
           const bool live = cl && r < R;
           float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
           if constexpr (MODE == DIB_GEMM_WGRAD) {
-            if (live && !(a.dbg & 1))
+            if (live)
               *reinterpret_cast<float2*>(out32 + (long long)split * a.split_stride + (long long)r * ldc32 + c) =
                   make_float2(v0 * a.out_scale, v1 * a.out_scale);
           } else {
@@ -238,7 +211,7 @@ dib_int16_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
               v0 *= dib_act_grad(a.act, x0, a.alpha);
               v1 *= dib_act_grad(a.act, x1, a.alpha);
             }
-            if (live && !(a.dbg & 1)) *reinterpret_cast<uint32_t*>(a.out16 + (long long)r * a.ldc + c) = pack_h2<BF16>(v0, v1);
+            if (live) *reinterpret_cast<uint32_t*>(a.out16 + (long long)r * a.ldc + c) = pack_h2<BF16>(v0, v1);
             if (live) { cs[0] += v0; cs[1] += v1; }               // rows / columns outside the matrix add nothing
           }
         }
@@ -428,15 +401,9 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
       float dz = 0.f;
       if (live && a.y) {
         const float t = a.y[row];
-        float l;
-        if (a.loss == DIB_LOSS_BCE_LOGITS) { l = fmaxf(z, 0.f) - z * t + log1pf(expf(-fabsf(z))); dz = 1.f / (1.f + expf(-z)) - t; }
-        else if (a.loss == DIB_LOSS_BCE_PROBS) {
-          const float ep = 1e-7f, pc = fminf(fmaxf(z, ep), 1.f - ep);
-          l = -(t * logf(pc + ep) + (1.f - t) * logf(1.f - pc + ep));
-          dz = (z > ep && z < 1.f - ep) ? -t / (pc + ep) + (1.f - t) / (1.f - pc + ep) : 0.f;
-        } else if (a.loss == DIB_LOSS_SPARSE_CE_LOGITS) { l = 0.f; dz = 0.f; }        // one class: the softmax is constant
-        else { const float d = z - t; l = d * d; dz = 2.f * d; }
-        const float acc1 = a.loss == DIB_LOSS_SPARSE_CE_LOGITS ? ((int)t == 0 ? 1.f : 0.f) : (((z > 0.5f ? 1.f : 0.f) == t) ? 1.f : 0.f);
+        float l = -0.f, acc1 = -0.f;
+        if (a.loss == DIB_LOSS_SPARSE_CE_LOGITS) { l = 0.f; acc1 = (int)t == 0 ? 1.f : 0.f; }   // one class: the softmax is constant
+        else dz = dib_loss_add(a.loss, z, t, l, acc1);
         if (q == 0) { lsum += l; asum += acc1; }
       }
       if (a.user_pred && live && q == 0) a.user_pred[row] = z;
@@ -571,14 +538,7 @@ dib_int16_head_kernel(const uint16_t* __restrict__ g, int ldg, int K, const floa
         } else {
 #pragma unroll
           for (int o = 0; o < OUT; ++o) if (o < out_dim) {
-            const float t = y[row * out_dim + o];
-            if (loss == DIB_LOSS_BCE_LOGITS) { l += fmaxf(z[o], 0.f) - z[o] * t + log1pf(expf(-fabsf(z[o]))); dz[o] = (1.f / (1.f + expf(-z[o])) - t) * inv_out; }
-            else if (loss == DIB_LOSS_BCE_PROBS) {
-              const float ep = 1e-7f, pc = fminf(fmaxf(z[o], ep), 1.f - ep);
-              l -= t * logf(pc + ep) + (1.f - t) * logf(1.f - pc + ep);
-              dz[o] = (z[o] > ep && z[o] < 1.f - ep) ? (-t / (pc + ep) + (1.f - t) / (1.f - pc + ep)) * inv_out : 0.f;
-            } else { const float d = z[o] - t; l += d * d; dz[o] = 2.f * d * inv_out; }
-            acc += ((z[o] > 0.5f ? 1.f : 0.f) == t) ? 1.f : 0.f;
+            dz[o] = dib_loss_add(loss, z[o], y[row * out_dim + o], l, acc) * inv_out;
           }
           l *= inv_out; acc *= inv_out;
         }
@@ -720,15 +680,9 @@ dib_int16_head1_kernel(const uint16_t* __restrict__ g, int ldg, int K, const flo
     float dz = 0.f;
     if (live && y) {
       const float t = y[mrow];
-      float l;
-      if (loss == DIB_LOSS_BCE_LOGITS) { l = fmaxf(z, 0.f) - z * t + log1pf(expf(-fabsf(z))); dz = 1.f / (1.f + expf(-z)) - t; }
-      else if (loss == DIB_LOSS_BCE_PROBS) {
-        const float ep = 1e-7f, pc = fminf(fmaxf(z, ep), 1.f - ep);
-        l = -(t * logf(pc + ep) + (1.f - t) * logf(1.f - pc + ep));
-        dz = (z > ep && z < 1.f - ep) ? -t / (pc + ep) + (1.f - t) / (1.f - pc + ep) : 0.f;
-      } else if (loss == DIB_LOSS_SPARSE_CE_LOGITS) { l = 0.f; dz = 0.f; }        // one class: the softmax is constant
-      else { const float d = z - t; l = d * d; dz = 2.f * d; }
-      const float acc = loss == DIB_LOSS_SPARSE_CE_LOGITS ? ((int)t == 0 ? 1.f : 0.f) : (((z > 0.5f ? 1.f : 0.f) == t) ? 1.f : 0.f);
+      float l = -0.f, acc = -0.f;
+      if (loss == DIB_LOSS_SPARSE_CE_LOGITS) { l = 0.f; acc = (int)t == 0 ? 1.f : 0.f; }        // one class: the softmax is constant
+      else dz = dib_loss_add(loss, z, t, l, acc);
       if (lane < ROWS) { lsum += l; asum += acc; }
     }
     if (user_pred && live && lane < ROWS) user_pred[mrow] = z;
@@ -795,15 +749,6 @@ dib_int16_head1_kernel(const uint16_t* __restrict__ g, int ldg, int K, const flo
   if (threadIdx.x == 0) { float a = 0.f; for (int ww = 0; ww < kHeadWarps; ++ww) a += sred[ww]; acc_part[blockIdx.x] = a; }
 }
 
-template <bool BF16>
-__global__ void dib_f32_to_16_kernel(const float* __restrict__ src, uint16_t* __restrict__ dst, long long n) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) {
-    if constexpr (BF16) { const __nv_bfloat16 b = __float2bfloat16_rn(src[i]); dst[i] = *reinterpret_cast<const uint16_t*>(&b); }
-    else { const __half b = __float2half_rn(src[i]); dst[i] = *reinterpret_cast<const uint16_t*>(&b); }
-  }
-}
-
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -852,11 +797,11 @@ cudaError_t launch16(const CUtensorMap& mA, const CUtensorMap& mB, const Int16Ar
   const long long cap = 2ll * num_sms16();
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(dib_int16_gemm_kernel<MODE, BF16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemmSmem);
+    cudaError_t e = cudaFuncSetAttribute(dib_int16_gemm_kernel<MODE, BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemmSmem);
     if (e != cudaSuccess) return e;
     attr = true;
   }
-  dib_int16_gemm_kernel<MODE, BF16, false><<<(unsigned)(ntile < cap ? ntile : cap), kGemmThreads, kGemmSmem, st>>>(mA, mB, a, mA2, mB2, a2, 0);
+  dib_int16_gemm_kernel<MODE, BF16><<<(unsigned)(ntile < cap ? ntile : cap), kGemmThreads, kGemmSmem, st>>>(mA, mB, a, mA2, mB2, a2);
   dib_note_launch();
   return cudaGetLastError();
 }
@@ -867,55 +812,6 @@ cudaError_t launch16(const CUtensorMap& mA, const CUtensorMap& mB, const Int16Ar
   return launch16<MODE, BF16>(mA, mB, a, mA, mB, none, ntile, st);
 }
 
-int rb_smem(int nkb) { return nkb * kBBytes + kRbStages * kABytes + 128 + 1024; }
-
-// resident-B launch: grid = a multiple of the column-tile count, at most one CTA per SM
-template <int MODE, bool BF16>
-cudaError_t launch_rb(const CUtensorMap& mA, const CUtensorMap& mB, const Int16Args& a, int nkb, cudaStream_t st) {
-  const int tiles_r = DIB_CEIL_DIV(a.M, kBM), tiles_c = DIB_CEIL_DIV(a.C, kBN);
-  long long grid = (long long)tiles_r * tiles_c;
-  const long long cap = (long long)(num_sms16() / tiles_c) * tiles_c;
-  if (grid > cap) grid = cap;
-  if (grid <= 0) return cudaSuccess;
-  const int smem = rb_smem(nkb);
-  static int attr_smem = 0;
-  if (attr_smem < smem) {
-    cudaError_t e = cudaFuncSetAttribute(dib_int16_gemm_kernel<MODE, BF16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return e;
-    attr_smem = smem;
-  }
-  Int16Args none{};
-  CUtensorMap mnone = mA;
-  dib_int16_gemm_kernel<MODE, BF16, true><<<(unsigned)grid, kGemmThreads, smem, st>>>(mA, mB, a, mnone, mnone, none, nkb);
-  dib_note_launch();
-  return cudaGetLastError();
-}
-
-// the resident-B kernel applies when the [T x 128] weight slice and its A ring fit in shared memory
-bool rb_ok(int T, int C) {
-  if (!dib_int16_rb_enabled() || T % kBK != 0 || C % 64 != 0) return false;
-  return rb_smem(T / kBK) + (int)sizeof(float) * (kConsumers / 32) * kBN <= 227 * 1024;
-}
-
-}  // namespace
-
-static int g_int16_head1 = 1;           // single-output head: 8-rows-per-pass kernel (1, default) or the generic one (0)
-int dib_int16_head1_enabled() { return g_int16_head1; }
-void dib_int16_head1_set(int on) { g_int16_head1 = on ? 1 : 0; }
-
-int g_int16_dbg = 0;
-void dib_int16_dbg_set(int v) { g_int16_dbg = v; }
-
-static int g_int16_rb = -1;
-int dib_int16_rb_enabled() {
-  // off by default: an A/B variant (DIB_INT16_RB=1, dib_debug_set_variant(1, 1)) that keeps the weight slice in shared memory
-  // instead of re-reading it from L2 for every row tile, at one CTA per SM instead of two
-  if (g_int16_rb < 0) { const char* e = getenv("DIB_INT16_RB"); g_int16_rb = (e && e[0] == '1') ? 1 : 0; }
-  return g_int16_rb;
-}
-void dib_int16_rb_set(int on) { g_int16_rb = on ? 1 : 0; }
-
-namespace {
 struct ConvSegs { const float* src[8]; uint16_t* dst[8]; long long first[9]; int nseg; };
 template <bool BF16>
 __global__ void dib_f32_to_16_segs_kernel(const ConvSegs A) {
@@ -951,14 +847,6 @@ cudaError_t dib_int16_convert_many(const float* const* src, void* const* dst16, 
   return cudaGetLastError();
 }
 
-cudaError_t dib_int16_convert(const float* src, void* dst16, long long n, int bf16, cudaStream_t st) {
-  if (n <= 0) return cudaSuccess;
-  if (bf16) dib_f32_to_16_kernel<true><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(src, static_cast<uint16_t*>(dst16), n);
-  else dib_f32_to_16_kernel<false><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(src, static_cast<uint16_t*>(dst16), n);
-  dib_note_launch();
-  return cudaGetLastError();
-}
-
 // g_out[M x N] = act(g_in[M x K] W16[K x N] + bias)
 cudaError_t dib_int16_fwd(const void* g_in, int ld_in, const void* w16, const float* bias, void* g_out, int ld_out, int M,
                           int K, int N, int act, float alpha, int bf16, cudaStream_t st) {
@@ -967,11 +855,8 @@ cudaError_t dib_int16_fwd(const void* g_in, int ld_in, const void* w16, const fl
   if (!map_k(&mA, g_in, K, M, ld_in, kBM) || !map_mn(&mB, w16, N, K, N, kBN / 64))
     return cudaErrorInvalidValue;
   Int16Args a{};
-  a.dbg = g_int16_dbg;
   a.out16 = static_cast<uint16_t*>(g_out); a.ldc = ld_out; a.bias = bias; a.M = M; a.T = K; a.C = N; a.act = act; a.alpha = alpha;
   a.out_scale = 1.f; a.nsplit = 1;
-  if (rb_ok(K, N))          // weights resident in shared memory, activations streamed
-    return bf16 ? launch_rb<DIB_GEMM_FWD, true>(mA, mB, a, K / kBK, st) : launch_rb<DIB_GEMM_FWD, false>(mA, mB, a, K / kBK, st);
   const long long nt = (long long)DIB_CEIL_DIV(M, kBM) * DIB_CEIL_DIV(N, kBN);
   return bf16 ? launch16<DIB_GEMM_FWD, true>(mA, mB, a, nt, st) : launch16<DIB_GEMM_FWD, false>(mA, mB, a, nt, st);
 }
@@ -984,39 +869,29 @@ cudaError_t dib_int16_dgrad(const void* dz, int ld_dz, const void* w16, const vo
   if (!map_k(&mA, dz, N, M, ld_dz, kBM) || !map_k(&mB, w16, N, K, N, kBN))
     return cudaErrorInvalidValue;
   Int16Args a{};
-  a.dbg = g_int16_dbg;
   a.out16 = static_cast<uint16_t*>(dz_in); a.ldc = ld_out; a.X = static_cast<const uint16_t*>(g_in); a.ldx = ld_g;
   a.M = M; a.T = N; a.C = K; a.act = act; a.alpha = alpha; a.out_scale = 1.f; a.nsplit = 1; a.dbias = colsum_part;
-  if (rb_ok(N, K))          // W^T slice resident, dz streamed
-    return bf16 ? launch_rb<DIB_GEMM_DGRAD, true>(mA, mB, a, N / kBK, st) : launch_rb<DIB_GEMM_DGRAD, false>(mA, mB, a, N / kBK, st);
   const long long nt = (long long)DIB_CEIL_DIV(M, kBM) * DIB_CEIL_DIV(K, kBN);
   return bf16 ? launch16<DIB_GEMM_DGRAD, true>(mA, mB, a, nt, st) : launch16<DIB_GEMM_DGRAD, false>(mA, mB, a, nt, st);
 }
 
-// dW[K x N] (fp32 split partials, * out_scale) = g_in[M x K]^T dz[M x N];  db = colsum dz
-cudaError_t dib_int16_wgrad(const void* g_in, int ld_g, const void* dz, int ld_dz, float* dW_part, float* db_part, int M, int K,
-                            int N, int nsplit, int rows_per_split, long long split_stride, float out_scale, int bf16, cudaStream_t st) {
+// dW[K x N] (fp32 split partials, * out_scale) = g_in[M x K]^T dz[M x N].  The bias gradients come from the kernel that
+// produces dz (dgrad epilogue / output head), not from here.
+cudaError_t dib_int16_wgrad(const void* g_in, int ld_g, const void* dz, int ld_dz, float* dW_part, int M, int K, int N, int nsplit,
+                            int rows_per_split, long long split_stride, float out_scale, int bf16, cudaStream_t st) {
   if (!encode_fn3()) return cudaErrorNotSupported;
   CUtensorMap mA, mB;
   if (!map_mn(&mA, g_in, K, M, ld_g, kBM / 64) || !map_mn(&mB, dz, N, M, ld_dz, kBN / 64))
     return cudaErrorInvalidValue;
   Int16Args a{};
-  a.dbg = g_int16_dbg;
   a.out32 = dW_part; a.ldc = N; a.dbias = nullptr; a.M = M; a.T = 0; a.C = N; a.R = K; a.out_scale = out_scale;
   a.nsplit = nsplit; a.rows_per_split = rows_per_split; a.split_stride = split_stride;
-  (void)db_part;   // bias gradients come from the kernel that PRODUCES dz (dgrad epilogue / output head), not from here
   const long long nt = (long long)DIB_CEIL_DIV(N, kBN) * DIB_CEIL_DIV(K, kBM) * nsplit;
   return bf16 ? launch16<DIB_GEMM_WGRAD, true>(mA, mB, a, nt, st) : launch16<DIB_GEMM_WGRAD, false>(mA, mB, a, nt, st);
 }
 
-static int g_int16_fwd2 = -1;            // fused [hidden, hidden, head] kernel for single-output models (1, default) or the separate kernels (0)
-int dib_int16_fwd2_enabled() {
-  if (g_int16_fwd2 < 0) { const char* e = getenv("DIB_INT16_FWD2"); g_int16_fwd2 = (e && e[0] == '0') ? 0 : 1; }
-  return g_int16_fwd2;
-}
-void dib_int16_fwd2_set(int on) { g_int16_fwd2 = on ? 1 : 0; }
-int dib_int16_fwd2_ok(int K0, int N1, int N2, int out_dim) {
-  return dib_int16_fwd2_enabled() && K0 % kBK == 0 && K0 >= kBK && N1 == kF2N && N2 == kF2N && out_dim == 1;
+bool dib_int16_fwd2_ok(int K0, int N1, int N2, int out_dim) {
+  return K0 % kBK == 0 && K0 >= kBK && N1 == kF2N && N2 == kF2N && out_dim == 1;
 }
 
 // g1 = act(g_in W0 + b0) -> HBM;  g2 = act(g1 W1 + b1) (on chip);  logit = g2 . wout + bout;  compiled loss / metric;
@@ -1074,7 +949,6 @@ cudaError_t dib_int16_wgrad_pair(const void* g_in0, int K0, const void* dz0, int
       !map_mn(&mA2, g_in1, K1, M, K1, kBM / 64) || !map_mn(&mB2, dz1, N1, M, N1, kBN / 64))
     return cudaErrorInvalidValue;
   Int16Args a{}, b{};
-  a.dbg = b.dbg = g_int16_dbg;
   a.out32 = dW_part0; a.ldc = N0; a.M = M; a.C = N0; a.R = K0; a.out_scale = out_scale; a.nsplit = nsplit0; a.rows_per_split = rps0; a.split_stride = split_stride;
   b.out32 = dW_part1; b.ldc = N1; b.M = M; b.C = N1; b.R = K1; b.out_scale = out_scale; b.nsplit = nsplit1; b.rows_per_split = rps1; b.split_stride = split_stride;
   const long long nt = (long long)DIB_CEIL_DIV(K0, kBM) * DIB_CEIL_DIV(N0, kBN) * nsplit0 + (long long)DIB_CEIL_DIV(K1, kBM) * DIB_CEIL_DIV(N1, kBN) * nsplit1;
@@ -1086,14 +960,14 @@ int dib_int16_head_blocks(int num_sms) { return num_sms * 2; }
 cudaError_t dib_int16_head(const void* g, int ldg, int K, const float* Wc, const float* bc, int out_dim, int out_act, int hid_act,
                            float alpha, int loss, const float* y, long long n, float inv_batch, float gscale, void* dg, int lddg,
                            float* user_pred, float* wpart, int wpart_stride, float* loss_part, float* acc_part, int nblocks,
-                           int bf16, cudaStream_t st) {
-  if (out_dim > kHeadMaxOut || out_dim < 1 || K != 256) return cudaErrorInvalidValue;
+                           bool head1, int bf16, cudaStream_t st) {
+  if (out_dim > kHeadMaxOut || out_dim < 1 || K != 256 || (head1 && out_dim != 1)) return cudaErrorInvalidValue;
 #define DIB_HEAD_T(OUT, BF)                                                                                             \
   dib_int16_head_kernel<8, OUT, (OUT <= 2 ? 4 : 1), BF><<<nblocks, kHeadWarps * 32, 0, st>>>(static_cast<const uint16_t*>(g), ldg, K, Wc, bc, out_dim,  \
       out_act, hid_act, alpha, loss, y, n, inv_batch, gscale, static_cast<uint16_t*>(dg), lddg, user_pred, wpart, wpart_stride, \
       loss_part, acc_part)
 #define DIB_HEAD(OUT) do { if (bf16) DIB_HEAD_T(OUT, true); else DIB_HEAD_T(OUT, false); } while (0)
-  if (out_dim == 1 && dib_int16_head1_enabled()) {
+  if (head1) {
     if (bf16) dib_int16_head1_kernel<true><<<nblocks, kHeadWarps * 32, 0, st>>>(static_cast<const uint16_t*>(g), ldg, K, Wc, bc, out_act,
         hid_act, alpha, loss, y, n, inv_batch, gscale, static_cast<uint16_t*>(dg), lddg, user_pred, wpart, wpart_stride, loss_part, acc_part);
     else dib_int16_head1_kernel<false><<<nblocks, kHeadWarps * 32, 0, st>>>(static_cast<const uint16_t*>(g), ldg, K, Wc, bc, out_act,

@@ -152,7 +152,6 @@ cudaError_t dib_enc_fused_backward(const DibEncFusedDesc& d, const DibEncFusedIO
                                    cudaStream_t st);
 
 // ---- 16-bit integration network path (dib_int16.cu) ----
-cudaError_t dib_int16_convert(const float* src, void* dst16, long long n, int bf16, cudaStream_t st);
 cudaError_t dib_int16_convert_many(const float* const* src, void* const* dst16, const long long* n, int count, int bf16, cudaStream_t st);
 cudaError_t dib_int16_fwd(const void* g_in, int ld_in, const void* w16, const float* bias, void* g_out, int ld_out, int M,
                           int K, int N, int act, float alpha, int bf16, cudaStream_t st);
@@ -163,29 +162,23 @@ cudaError_t dib_int16_dgrad(const void* dz, int ld_dz, const void* w16, const vo
 struct DibReduceSeg { const float* src; long long row_stride; int nrows; long long count; float scale; float* dst; };
 constexpr int kDibMaxReduceSegs = 8;
 cudaError_t dib_launch_reduce_segments(const DibReduceSeg* segs, int nseg, cudaStream_t st);
-cudaError_t dib_launch_reduce_tall(const float* part, long long row_stride, int nrows, int64_t count, float scale, float* out,
-                                   cudaStream_t st);
-cudaError_t dib_int16_wgrad(const void* g_in, int ld_g, const void* dz, int ld_dz, float* dW_part, float* db_part, int M, int K,
-                            int N, int nsplit, int rows_per_split, long long split_stride, float out_scale, int bf16, cudaStream_t st);
+cudaError_t dib_int16_wgrad(const void* g_in, int ld_g, const void* dz, int ld_dz, float* dW_part, int M, int K, int N, int nsplit,
+                            int rows_per_split, long long split_stride, float out_scale, int bf16, cudaStream_t st);
 cudaError_t dib_int16_wgrad_pair(const void* g_in0, int K0, const void* dz0, int N0, float* dW_part0, int nsplit0, int rps0,
                                  const void* g_in1, int K1, const void* dz1, int N1, float* dW_part1, int nsplit1, int rps1,
                                  int M, long long split_stride, float out_scale, int bf16, cudaStream_t st);
 int dib_int16_head_blocks(int num_sms);
-void dib_int16_dbg_set(int v);
-int dib_int16_fwd2_enabled();
-void dib_int16_fwd2_set(int on);
-int dib_int16_fwd2_ok(int K0, int N1, int N2, int out_dim);
+// shapes the fused tail kernel (dib_int16_fwd2_head) handles: fan-in K0 of its first layer, its two widths, the output width
+bool dib_int16_fwd2_ok(int K0, int N1, int N2, int out_dim);
 cudaError_t dib_int16_fwd2_head(const void* g_in, int ld_in, int K0, const void* w16_0, const float* b0, const void* w16_1, const float* b1,
                                 void* g1, const float* wout, const float* bout, int act, int out_act, float alpha, int loss, const float* y,
                                 int M, float inv_batch, float gscale, void* dg2, float* user_pred, float* wpart, int wpart_stride,
                                 float* loss_part, float* acc_part, int* nblocks, int bf16, cudaStream_t st);
-int dib_int16_rb_enabled();
-void dib_int16_rb_set(int on);
-void dib_int16_head1_set(int on);
+// head1: the out = 1 kernel (8 rows per pass) instead of the generic one
 cudaError_t dib_int16_head(const void* g, int ldg, int K, const float* Wc, const float* bc, int out_dim, int out_act, int hid_act,
                            float alpha, int loss, const float* y, long long n, float inv_batch, float gscale, void* dg, int lddg,
                            float* user_pred, float* wpart, int wpart_stride, float* loss_part, float* acc_part, int nblocks,
-                           int bf16, cudaStream_t st);
+                           bool head1, int bf16, cudaStream_t st);
 
 cudaError_t dib_launch_mi_sandwich(const float* mu_logvar, int64_t n, int E, const float* eps, uint64_t seed, uint32_t step,
                                    float* row_scratch, float* out2, cudaStream_t st);

@@ -666,8 +666,11 @@ class DistributedIBNet:
             return self._gradstats[:P].clone(), self._gradstats[P:].clone()
 
     def debug_force_unfused(self, on=True, batch_hint=1):
-        """Bring-up switch: keep the tensor-core mode on the unfused kernels (fused-vs-unfused comparisons)."""
-        self._force_unfused = int(on)          # bit 0: unfused encoders, bit 1: fp32-storage integration network
+        """Bring-up switch: keep the tensor-core mode on the reference kernels (fused-vs-unfused comparisons).
+
+        ``on`` is a bit mask (``True`` = 1): 1 = unfused encoders, 2 = fp32-storage TF32 integration network, 4 = no fused
+        integration tail (per-layer 16-bit GEMMs plus a head kernel), 8 = the generic head kernel even when out = 1."""
+        self._force_unfused = int(on)
         if self._handle is not None:
             _lib.check(self._lib.dib_debug_force_unfused(self._handle, int(on)))
 

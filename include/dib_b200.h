@@ -289,18 +289,10 @@ int dib_debug_gemm_tc(int32_t mode, const float* A, int32_t lda, const float* B,
                       float* X, int32_t ldx, int32_t M, int32_t T, int32_t Ccols, int32_t R, int32_t act,
                       int32_t nsplit, int32_t rows_per_split, int64_t split_stride, int32_t use_simt, void* stream);
 
-/* bring-up switch (bit mask): 1 = unfused encoder kernels, 2 = integration network on fp32-storage TF32 kernels. */
+/* bring-up switch for THIS handle (bit mask, 0 = the default kernels): 1 = unfused encoder kernels, 2 = integration network on
+ * fp32-storage TF32 kernels, 4 = no fused integration tail (per-layer 16-bit GEMMs plus a head kernel), 8 = the generic head
+ * kernel even when output_dimensionality == 1.  dib_model_info reports the resulting path. */
 int dib_debug_force_unfused(dib_model* h, int32_t on);
-
-/* process-wide kernel-variant switch for A/B measurements.
- * key 1: 16-bit integration FWD / DGRAD GEMMs, 1 = weight slice resident in shared memory, 0 = re-streamed per tile (default;
- * also DIB_INT16_RB=0|1).  Both issue the same MMAs in the same order: results are bit-identical.
- * key 2: fused output head for output_dimensionality == 1, 1 = eight rows per pass with a lane-parallel loss (default), 0 = the
- * generic kernel.
- * key 3: single-output models whose last two hidden integration layers are 256 wide, 1 = those layers + the head + the loss as one
- * kernel (default; also DIB_INT16_FWD2=0|1), 0 = one kernel per layer and the head kernel of key 2.
- * key 5: MEASUREMENT ONLY, wrong results: 1 = the 16-bit GEMM epilogues skip their global stores (cost of the store path). */
-int dib_debug_set_variant(int32_t key, int32_t value);
 
 /* text of the last error raised on this thread ("" if none). */
 const char* dib_last_error(void);

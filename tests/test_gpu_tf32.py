@@ -128,45 +128,11 @@ def test_fused_encoder_kernels_match_unfused_and_fp32(shape):
                 off += n
 
 
-@pytest.mark.parametrize("shape", ["c0", "radial3"])
-def test_int16_resident_weight_gemms_match_streamed_kernels_bitwise(shape):
-    """The integration FWD / DGRAD GEMMs with the weight slice resident in shared memory (BN = 128 / 256, one CTA per SM)
-    issue the same MMAs in the same order as the streamed-B kernels they replace: predictions, gradients and statistics
-    must be bit-identical, incl. a ragged last row tile."""
-    from dib_b200 import _lib
-    lib = _lib.load()
-    if shape == "c0":
-        cfg, D = O.DIBConfig([1] * 16, [128, 128], [256, 256], 1), 16
-    else:
-        cfg, D = O.DIBConfig([1] * 12, [128, 128], [256, 256, 256], 3, activation_fn="tanh", use_positional_encoding=False), 12
-    rng = np.random.default_rng(5)
-    p = O.glorot_uniform_params(cfg, rng)
-    p = p + (p == 0) * (0.05 * rng.standard_normal(p.size)).astype(np.float32)
-    B = 128 * 37 + 19
-    x = rng.standard_normal((B, D)).astype(np.float32)
-    y = rng.standard_normal((B, cfg.output_dimensionality)).astype(np.float32)
-    res = {}
-    try:
-        for rb in (0, 1):
-            _lib.check(lib.dib_debug_set_variant(1, rb))
-            m = build_model(cfg, precision="fp16", loss="mse")
-            m.set_flat_weights(p)
-            m.beta.assign(0.02)
-            pred = m(x, step=2)
-            g, st = m.compute_gradients(x, y, step=2)
-            res[rb] = (np.asarray(pred), g.cpu().numpy(), st.cpu().numpy())
-    finally:
-        _lib.check(lib.dib_debug_set_variant(1, 0))
-    for a, b in zip(res[0], res[1]):
-        np.testing.assert_array_equal(a, b)
-
-
 @pytest.mark.parametrize("loss_name", ["bce_logits", "mse"])
-def test_single_output_head_kernel_matches_generic_head(loss_name):
-    """The out = 1 output-head kernel (8 rows per pass, transposing butterfly, lane-parallel loss) against the generic head:
-    same arithmetic per row, a different (still fixed) summation tree for the 256-term logit -> fp32 round-off only."""
-    from dib_b200 import _lib
-    lib = _lib.load()
+def test_single_output_head_kernel_matches_generic_head_without_fused_tail(loss_name):
+    """The out = 1 output-head kernel (8 rows per pass, transposing butterfly, lane-parallel loss) against the generic head,
+    both behind the per-layer integration GEMMs (no fused tail): same arithmetic per row, a different (still fixed)
+    summation tree for the 256-term logit -> fp32 round-off only."""
     cfg = O.DIBConfig([1] * 16, [128, 128], [256, 256], 1)
     rng = np.random.default_rng(6)
     p = O.glorot_uniform_params(cfg, rng)
@@ -175,19 +141,16 @@ def test_single_output_head_kernel_matches_generic_head(loss_name):
     x = rng.standard_normal((B, 16)).astype(np.float32)
     y = (x[:, :1] * x[:, 1:2] > 0).astype(np.float32) if loss_name == "bce_logits" else rng.standard_normal((B, 1)).astype(np.float32)
     res = {}
-    try:
-        for v in (0, 1):
-            _lib.check(lib.dib_debug_set_variant(2, v))
-            m = build_model(cfg, precision="fp16", loss=loss_name)
-            m.set_flat_weights(p)
-            m.beta.assign(0.02)
-            pred = m(x, step=2)
-            g, st = m.compute_gradients(x, y, step=2)
-            g2, _ = m.compute_gradients(x, y, step=2)
-            assert torch.equal(g, g2)                                            # deterministic
-            res[v] = (np.asarray(pred), g.cpu().numpy(), st.cpu().numpy())
-    finally:
-        _lib.check(lib.dib_debug_set_variant(2, 1))
+    for v, mask in ((0, 4 | 8), (1, 4)):                  # 4: no fused tail; 8: generic head even for out = 1
+        m = build_model(cfg, precision="fp16", loss=loss_name)
+        m.debug_force_unfused(mask)
+        m.set_flat_weights(p)
+        m.beta.assign(0.02)
+        pred = m(x, step=2)
+        g, st = m.compute_gradients(x, y, step=2)
+        g2, _ = m.compute_gradients(x, y, step=2)
+        assert torch.equal(g, g2)                                            # deterministic
+        res[v] = (np.asarray(pred), g.cpu().numpy(), st.cpu().numpy())
     assert rel_err(res[1][0], res[0][0]) < 1e-5
     assert rel_err(res[1][1], res[0][1]) < 2e-4          # the 16-bit rounding of dg can flip on a 1-ulp change of the logit
     np.testing.assert_allclose(res[1][2], res[0][2], rtol=1e-5)
@@ -195,34 +158,29 @@ def test_single_output_head_kernel_matches_generic_head(loss_name):
 
 @pytest.mark.parametrize("precision,act,loss_name,integ", [("fp16", "relu", "bce_logits", [256, 256]), ("bf16", "tanh", "mse", [256, 256]),
                                                         ("fp16", "tanh", "bce_logits", [128, 256, 256])])
-def test_fused_integration_tail_matches_per_layer_kernels(precision, act, loss_name, integ):
+def test_fused_integration_tail_matches_per_layer_route(precision, act, loss_name, integ):
     """The fused [hidden 256, hidden 256, head, loss] kernel (dib_int16_fwd2_kernel) against the per-layer GEMM kernels + head:
     the same 16-bit roundings of g1 / g2 / dg2, fp32 round-off differences only in the 256-term logit and the partial sums.
     Ragged last tile, a non-power-of-two number of tiles, a deeper integration network (one plain layer before the fused tail)."""
-    from dib_b200 import _lib
-    lib = _lib.load()
     cfg = O.DIBConfig([1] * 16, [128, 128], integ, 1, activation_fn=act)
     rng = np.random.default_rng(16)
     p = O.glorot_uniform_params(cfg, rng)
     p = p + (p == 0) * (0.05 * rng.standard_normal(p.size)).astype(np.float32)
     res = {}
-    try:
-        for B in (128 * 3 + 17, 128 * 160 + 77):
-            x = rng.standard_normal((B, 16)).astype(np.float32)
-            y = (x[:, :1] * x[:, 1:2] > 0).astype(np.float32) if loss_name == "bce_logits" else rng.standard_normal((B, 1)).astype(np.float32)
-            for v in (0, 1):
-                _lib.check(lib.dib_debug_set_variant(3, v))
-                m = build_model(cfg, precision=precision, loss=loss_name)
-                m.set_flat_weights(p)
-                m.beta.assign(0.02)
-                pred = m(x, step=2)
-                g, st = m.compute_gradients(x, y, step=2)
-                g2, _ = m.compute_gradients(x, y, step=2)
-                assert torch.equal(g, g2)                                            # deterministic
-                assert torch.isfinite(g).all()
-                res[v] = (np.asarray(pred), g.cpu().numpy(), st.cpu().numpy())
-            assert rel_err(res[1][0], res[0][0]) < 1e-5
-            assert rel_err(res[1][1], res[0][1]) < 2e-4      # a 1-ulp change of the logit can flip a 16-bit rounding of dg2
-            np.testing.assert_allclose(res[1][2], res[0][2], rtol=1e-5)
-    finally:
-        _lib.check(lib.dib_debug_set_variant(3, 1))
+    for B in (128 * 3 + 17, 128 * 160 + 77):
+        x = rng.standard_normal((B, 16)).astype(np.float32)
+        y = (x[:, :1] * x[:, 1:2] > 0).astype(np.float32) if loss_name == "bce_logits" else rng.standard_normal((B, 1)).astype(np.float32)
+        for v in (0, 1):
+            m = build_model(cfg, precision=precision, loss=loss_name)
+            m.debug_force_unfused(0 if v else 4)                                 # 4: per-layer kernels instead of the fused tail
+            m.set_flat_weights(p)
+            m.beta.assign(0.02)
+            pred = m(x, step=2)
+            g, st = m.compute_gradients(x, y, step=2)
+            g2, _ = m.compute_gradients(x, y, step=2)
+            assert torch.equal(g, g2)                                            # deterministic
+            assert torch.isfinite(g).all()
+            res[v] = (np.asarray(pred), g.cpu().numpy(), st.cpu().numpy())
+        assert rel_err(res[1][0], res[0][0]) < 1e-5
+        assert rel_err(res[1][1], res[0][1]) < 2e-4      # a 1-ulp change of the logit can flip a 16-bit rounding of dg2
+        np.testing.assert_allclose(res[1][2], res[0][2], rtol=1e-5)
