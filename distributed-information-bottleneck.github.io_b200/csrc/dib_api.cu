@@ -615,6 +615,83 @@ int backward_encoders(const Ctx& c, const float* x, const NoiseKey& nk, const fl
   return 0;
 }
 
+// integration network backward (GradientTape through models.py:122) from d loss / d prediction, as the forward of the step left
+// it, down to the d emb backward_encoders reads.  16-bit route: its fixed-order reductions (bias gradients from the head / dgrad
+// column sums, batch-split weight-gradient partials, the output layer's per-CTA partials) are appended to *segs for the caller to
+// run in one launch with the encoder segment (the 16-bit route implies the fused encoders).  Per-layer GEMM route:
+// grads_flat[p_enc, P) is final on return.
+int backward_integration(const Ctx& c, float inv_batch, const Split& sp, float* grads_flat, std::vector<DibReduceSeg>* segs) {
+  dib_model* h = c.h;
+  float* part = c.ws + h->part_off;
+  if (!h->route.int16) {
+    const long long p_enc = h->intW[0];
+    for (int j = h->Li; j >= 0; --j) {
+      prof_begin(c, "int_wgrad_l", j);
+      if (gemm(c, DIB_GEMM_WGRAD, h->int_wgrad[j], 1, int_fan_out(h, j), int_fan_in(h, j), sp.nsplit, (int)sp.rps)) return 1;
+      prof_end(c);
+      prof_begin(c, "int_dgrad_l", j);
+      if (gemm(c, DIB_GEMM_DGRAD, h->int_dgrad[j], 1, int_fan_in(h, j), 0, 1, 0)) return 1;
+      prof_end(c);
+    }
+    prof_begin(c, "int_split_reduce");
+    DIB_CUDA_OK(dib_launch_reduce_partials(part + p_enc, h->Pp, sp.nsplit, h->P - p_enc, grads_flat + p_enc, c.st));
+    prof_end(c);
+    return 0;
+  }
+  const int bf = h->precision == DIB_PREC_BF16 ? 1 : 0;
+  const float gscale = loss_scale(inv_batch);
+  const int Kh = h->int_arch[h->Li - 1];
+  const int row_tiles = (int)DIB_CEIL_DIV((long long)c.n, 128ll);
+  const long long p_head = h->intW[h->Li];
+  // bias gradient of the last hidden layer: column sums of dg accumulated by the output head
+  segs->push_back({c.ws + h->headpart_off + (long long)Kh * h->out + h->out, h->head_stride, h->head_used, Kh, 1.f / gscale,
+                   grads_flat + h->intB[h->Li - 1]});
+  // the dgrad chain first (layer j's dgrad produces the gradient layer j-1's wgrad consumes), then the weight gradients in PAIRS of
+  // layers per launch: one layer's [K/128 x N/128 x splits] tiles do not fill the 2 x SMs CTA slots, two layers' tiles do
+  for (int j = h->Li - 1; j >= 0; --j) {
+    const int K = int_fan_in(h, j), N = int_fan_out(h, j);
+    prof_begin(c, "int16_dgrad_l", j);
+    DIB_CUDA_OK(dib_int16_dgrad(c.ws + h->dg16_off[j + 1], N, c.ws + h->w16_off[j], j > 0 ? (const void*)(c.ws + h->g16_off[j]) : nullptr,
+                                K, j > 0 ? (void*)(c.ws + h->dg16_off[j]) : (void*)(c.ws + h->demb16_off), K, c.n, K, N, h->act,
+                                h->alpha, j > 0 ? c.ws + h->dbpart_off + (long long)j * h->dbpart_layer : nullptr, bf, c.st));
+    if (j > 0)   // bias gradient of layer j-1 = column sums of the gradient this dgrad just produced
+      segs->push_back({c.ws + h->dbpart_off + (long long)j * h->dbpart_layer, K, row_tiles, K, 1.f / gscale, grads_flat + h->intB[j - 1]});
+    prof_end(c);
+  }
+  std::vector<int> nsplit_of(h->Li, sp.nsplit);
+  auto tiles_of = [&](int j) { return DIB_CEIL_DIV(int_fan_in(h, j), 128) * DIB_CEIL_DIV(int_fan_out(h, j), 128); };
+  auto wgrad_of = [&](int j, int nsplit, int rps) {
+    return DibInt16Wgrad{int16_in(c, j), int_fan_in(h, j), c.ws + h->dg16_off[j + 1], int_fan_out(h, j), part + h->intW[j], nsplit, rps};
+  };
+  int j = h->Li - 1;
+  for (; j >= 1; j -= 2) {          // layers (j, j-1) together
+    long long ns = (2ll * h->num_sms) / (tiles_of(j) + tiles_of(j - 1));
+    if (ns > h->part_rows) ns = h->part_rows;
+    if (ns > (long long)c.n / 256) ns = (long long)c.n / 256;
+    if (ns < 1) ns = 1;
+    const long long rps2 = DIB_ROUND_UP(DIB_CEIL_DIV((long long)c.n, ns), 64);
+    const int ns2 = (int)DIB_CEIL_DIV((long long)c.n, rps2);
+    nsplit_of[j] = nsplit_of[j - 1] = ns2;
+    const DibInt16Wgrad pair[2] = {wgrad_of(j, ns2, (int)rps2), wgrad_of(j - 1, ns2, (int)rps2)};
+    prof_begin(c, "int16_wgrad_pair_l", j - 1);
+    DIB_CUDA_OK(dib_int16_wgrad(pair, 2, c.n, h->Pp, 1.f / gscale, bf, c.st));
+    prof_end(c);
+  }
+  if (j == 0) {                     // an odd layer count leaves layer 0 alone
+    const DibInt16Wgrad l0 = wgrad_of(0, sp.nsplit, (int)sp.rps);
+    prof_begin(c, "int16_wgrad_l", 0);
+    DIB_CUDA_OK(dib_int16_wgrad(&l0, 1, c.n, h->Pp, 1.f / gscale, bf, c.st));
+    prof_end(c);
+  }
+  // an empty range: these reductions run in the caller's one launch, timed under enc_split_reduce
+  prof_begin(c, "int_split_reduce");
+  for (int q = 0; q < h->Li; ++q)     // hidden-layer kernels: batch-split partials
+    segs->push_back({part + h->intW[q], h->Pp, nsplit_of[q], (long long)int_fan_in(h, q) * int_fan_out(h, q), 1.f, grads_flat + h->intW[q]});
+  segs->push_back({c.ws + h->headpart_off, h->head_stride, h->head_used, h->P - p_head, 1.f, grads_flat + p_head});
+  prof_end(c);
+  return 0;
+}
+
 }  // namespace
 
 // =================================================================================================
@@ -920,122 +997,35 @@ int dib_encode_feature(dib_model* h, const float* params, int32_t feature, const
   return 0;
 }
 
-// phases: 1 = forward + compiled loss + integration-network backward (grads_flat[first integration parameter ..) final),
-//         2 = encoder backward (grads_flat[0 .. first integration parameter) final); 3 = both (= dib_train_step).
-// Phase 2 relies on the workspace exactly as phase 1 left it (same x, eps / seed / step, n).
-int dib_train_step_phased(dib_model* h, const float* params, const float* x, const float* y, int64_t n, const float* beta_dev,
-                          float inv_global_batch, const float* eps, uint64_t seed, uint32_t step, uint64_t sample_offset,
-                          float* grads_flat, float* out_stats, void* workspace, int32_t phases, void* stream) {
+int dib_train_step(dib_model* h, const float* params, const float* x, const float* y, int64_t n, const float* beta_dev,
+                   float inv_global_batch, const float* eps, uint64_t seed, uint32_t step, uint64_t sample_offset,
+                   float* grads_flat, float* out_stats, void* workspace, void* stream) {
   if (check_call(h, params, x, n, workspace)) return 1;
   if ((!y && n > 0) || !beta_dev || !grads_flat || !out_stats)
     return fail("dib_train_step: y, beta_dev, grads_flat and out_stats are required");
-  if (phases < 1 || phases > 3) return fail("dib_train_step_phased: phases must be 1, 2 or 3");
-  const bool phA = (phases & 1) != 0, phB = (phases & 2) != 0;
   Ctx c{h, params, static_cast<float*>(workspace), static_cast<cudaStream_t>(stream), (int)n};
   c.dev_step = true;
-  const long long p_enc = h->intW[0];                // encoder parameters occupy [0, p_enc)
   if (n == 0) {
-    if (phB) DIB_CUDA_OK(cudaMemsetAsync(grads_flat, 0, sizeof(float) * p_enc, c.st));
-    if (phA) {
-      DIB_CUDA_OK(cudaMemsetAsync(grads_flat + p_enc, 0, sizeof(float) * (h->P - p_enc), c.st));
-      DIB_CUDA_OK(cudaMemsetAsync(out_stats, 0, sizeof(float) * (h->F + 3), c.st));
-    }
+    DIB_CUDA_OK(cudaMemsetAsync(grads_flat, 0, sizeof(float) * h->P, c.st));
+    DIB_CUDA_OK(cudaMemsetAsync(out_stats, 0, sizeof(float) * (h->F + 3), c.st));
     return 0;
   }
-  const bool nonlinear = h->kl_exp != 1.f || h->kl_scale != 1.f;
   const NoiseKey nk{eps, seed, step, sample_offset, true};
-  if (phA) {
-    if (run_forward(c, x, y, nk, inv_global_batch, nullptr, nullptr, out_stats)) return 1;
-    const float* bw = nullptr;
-    if (ib_weight(c, beta_dev, out_stats, inv_global_batch, &bw)) return 1;
-  }
-  // weight of the per-sample KL gradients in the encoder backward: beta, or d(beta*scale*KL^p)/dKL left in the workspace by phase 1
-  const float* beta_w = nonlinear ? c.ws + h->beta_eff_off : beta_dev;
+  if (run_forward(c, x, y, nk, inv_global_batch, nullptr, nullptr, out_stats)) return 1;
+  const float* beta_w = nullptr;           // weight of the per-sample KL gradients in the encoder backward
+  if (ib_weight(c, beta_dev, out_stats, inv_global_batch, &beta_w)) return 1;
   const Split sp = batch_split(n);
-  float* part = c.ws + h->part_off;
-  const dib_model::Route& r = h->route;
-
-  std::vector<DibReduceSeg> segs;          // fixed-order reductions of the step; whole steps (phases == 3) run them as ONE launch at the end
-  // ---------------------------------------------------------------- phase 1: integration network backward
-  if (phA && r.int16) {
-    const int bf = h->precision == DIB_PREC_BF16 ? 1 : 0;
-    const float gscale = loss_scale(inv_global_batch);
-    const int Kh = h->int_arch[h->Li - 1];
-    const int row_tiles = (int)DIB_CEIL_DIV((long long)n, 128ll);
-    const long long p_head = h->intW[h->Li];
-    // every fixed-order reduction of this phase runs as ONE launch at its end (bias gradients from the head / dgrad column sums,
-    // batch-split weight-gradient partials, the output layer's per-CTA partials)
-    // bias gradient of the last hidden layer: column sums of dg accumulated by the output head
-    segs.push_back({c.ws + h->headpart_off + (long long)Kh * h->out + h->out, h->head_stride, h->head_used, Kh, 1.f / gscale,
-                    grads_flat + h->intB[h->Li - 1]});
-    // the dgrad chain first (layer j's dgrad produces the gradient layer j-1's wgrad consumes), then the weight gradients in PAIRS of
-    // layers per launch: one layer's [K/128 x N/128 x splits] tiles do not fill the 2 x SMs CTA slots, two layers' tiles do
-    for (int j = h->Li - 1; j >= 0; --j) {
-      const int K = int_fan_in(h, j), N = int_fan_out(h, j);
-      prof_begin(c, "int16_dgrad_l", j);
-      DIB_CUDA_OK(dib_int16_dgrad(c.ws + h->dg16_off[j + 1], N, c.ws + h->w16_off[j], j > 0 ? (const void*)(c.ws + h->g16_off[j]) : nullptr,
-                                  K, j > 0 ? (void*)(c.ws + h->dg16_off[j]) : (void*)(c.ws + h->demb16_off), K, (int)n, K, N, h->act,
-                                  h->alpha, j > 0 ? c.ws + h->dbpart_off + (long long)j * h->dbpart_layer : nullptr, bf, c.st));
-      if (j > 0)   // bias gradient of layer j-1 = column sums of the gradient this dgrad just produced
-        segs.push_back({c.ws + h->dbpart_off + (long long)j * h->dbpart_layer, K, row_tiles, K, 1.f / gscale, grads_flat + h->intB[j - 1]});
-      prof_end(c);
-    }
-    std::vector<int> nsplit_of(h->Li, sp.nsplit);
-    auto tiles_of = [&](int j) { return DIB_CEIL_DIV(int_fan_in(h, j), 128) * DIB_CEIL_DIV(int_fan_out(h, j), 128); };
-    int j = h->Li - 1;
-    for (; j >= 1; j -= 2) {          // layers (j, j-1) together
-      long long ns = (2ll * h->num_sms) / (tiles_of(j) + tiles_of(j - 1));
-      if (ns > h->part_rows) ns = h->part_rows;
-      if (ns > (long long)n / 256) ns = (long long)n / 256;
-      if (ns < 1) ns = 1;
-      const long long rps2 = DIB_ROUND_UP(DIB_CEIL_DIV((long long)n, ns), 64);
-      const int ns2 = (int)DIB_CEIL_DIV((long long)n, rps2);
-      nsplit_of[j] = nsplit_of[j - 1] = ns2;
-      prof_begin(c, "int16_wgrad_pair_l", j - 1);
-      DIB_CUDA_OK(dib_int16_wgrad_pair(int16_in(c, j), int_fan_in(h, j), c.ws + h->dg16_off[j + 1], int_fan_out(h, j), part + h->intW[j],
-                                       ns2, (int)rps2, int16_in(c, j - 1), int_fan_in(h, j - 1), c.ws + h->dg16_off[j], int_fan_out(h, j - 1),
-                                       part + h->intW[j - 1], ns2, (int)rps2, (int)n, h->Pp, 1.f / gscale, bf, c.st));
-      prof_end(c);
-    }
-    if (j == 0) {
-      prof_begin(c, "int16_wgrad_l", 0);
-      DIB_CUDA_OK(dib_int16_wgrad(int16_in(c, 0), int_fan_in(h, 0), c.ws + h->dg16_off[1], int_fan_out(h, 0), part + h->intW[0], (int)n,
-                                  int_fan_in(h, 0), int_fan_out(h, 0), sp.nsplit, (int)sp.rps, h->Pp, 1.f / gscale, bf, c.st));
-      prof_end(c);
-    }
-    prof_begin(c, "int_split_reduce");
-    for (int q = 0; q < h->Li; ++q)     // hidden-layer kernels: batch-split partials
-      segs.push_back({part + h->intW[q], h->Pp, nsplit_of[q], (long long)int_fan_in(h, q) * int_fan_out(h, q), 1.f, grads_flat + h->intW[q]});
-    segs.push_back({c.ws + h->headpart_off, h->head_stride, h->head_used, h->P - p_head, 1.f, grads_flat + p_head});
-    if (!phB) {               // phase-1-only call: reduce now (the 16-bit path implies the fused encoders, which reduce with these)
-      DIB_CUDA_OK(dib_launch_reduce_segments(segs.data(), (int)segs.size(), c.st));
-      segs.clear();
-    }
-    prof_end(c);
-  } else if (phA) {
-    // integration network backward (GradientTape through models.py:122)
-    for (int j = h->Li; j >= 0; --j) {
-      prof_begin(c, "int_wgrad_l", j);
-      if (gemm(c, DIB_GEMM_WGRAD, h->int_wgrad[j], 1, int_fan_out(h, j), int_fan_in(h, j), sp.nsplit, (int)sp.rps)) return 1;
-      prof_end(c);
-      prof_begin(c, "int_dgrad_l", j);
-      if (gemm(c, DIB_GEMM_DGRAD, h->int_dgrad[j], 1, int_fan_in(h, j), 0, 1, 0)) return 1;
-      prof_end(c);
-    }
-    prof_begin(c, "int_split_reduce");
-    DIB_CUDA_OK(dib_launch_reduce_partials(part + p_enc, h->Pp, sp.nsplit, h->P - p_enc, grads_flat + p_enc, c.st));
-    prof_end(c);
-  }
-  if (!phB) return 0;
-
-  // ---------------------------------------------------------------- phase 2: encoder backward
+  std::vector<DibReduceSeg> segs;          // fixed-order reductions of the step, run as ONE launch at the end
+  if (backward_integration(c, inv_global_batch, sp, grads_flat, &segs)) return 1;
   int nrows = 0;
-  const bool d16 = r.int16;                // the 16-bit integration backward leaves d emb in fp16
+  const bool d16 = h->route.int16;         // the 16-bit integration backward leaves d emb in fp16
   if (backward_encoders(c, x, nk, d16 ? nullptr : c.ws + h->d_emb.off, d16 ? 0 : h->d_emb.ld, d16 ? c.ws + h->demb16_off : nullptr,
                         beta_w, inv_global_batch, sp, &nrows))
     return 1;
+  float* part = c.ws + h->part_off;
+  const long long p_enc = h->intW[0];      // encoder parameters occupy [0, p_enc)
   prof_begin(c, "enc_split_reduce");
-  if (r.enc_fused) {
+  if (h->route.enc_fused) {
     segs.push_back({part, h->Pp, nrows, p_enc, 1.f, grads_flat});
     DIB_CUDA_OK(dib_launch_reduce_segments(segs.data(), (int)segs.size(), c.st));
   } else {
@@ -1043,13 +1033,6 @@ int dib_train_step_phased(dib_model* h, const float* params, const float* x, con
   }
   prof_end(c);
   return 0;
-}
-
-int dib_train_step(dib_model* h, const float* params, const float* x, const float* y, int64_t n, const float* beta_dev,
-                   float inv_global_batch, const float* eps, uint64_t seed, uint32_t step, uint64_t sample_offset,
-                   float* grads_flat, float* out_stats, void* workspace, void* stream) {
-  return dib_train_step_phased(h, params, x, y, n, beta_dev, inv_global_batch, eps, seed, step, sample_offset, grads_flat,
-                               out_stats, workspace, 3, stream);
 }
 
 // Philox 'step' word from device memory (CUDA-Graph replay: a captured launch cannot carry a fresh by-value step):

@@ -806,12 +806,6 @@ cudaError_t launch16(const CUtensorMap& mA, const CUtensorMap& mB, const Int16Ar
   return cudaGetLastError();
 }
 
-template <int MODE, bool BF16>
-cudaError_t launch16(const CUtensorMap& mA, const CUtensorMap& mB, const Int16Args& a, long long ntile, cudaStream_t st) {
-  Int16Args none{};
-  return launch16<MODE, BF16>(mA, mB, a, mA, mB, none, ntile, st);
-}
-
 struct ConvSegs { const float* src[8]; uint16_t* dst[8]; long long first[9]; int nseg; };
 template <bool BF16>
 __global__ void dib_f32_to_16_segs_kernel(const ConvSegs A) {
@@ -858,7 +852,8 @@ cudaError_t dib_int16_fwd(const void* g_in, int ld_in, const void* w16, const fl
   a.out16 = static_cast<uint16_t*>(g_out); a.ldc = ld_out; a.bias = bias; a.M = M; a.T = K; a.C = N; a.act = act; a.alpha = alpha;
   a.out_scale = 1.f; a.nsplit = 1;
   const long long nt = (long long)DIB_CEIL_DIV(M, kBM) * DIB_CEIL_DIV(N, kBN);
-  return bf16 ? launch16<DIB_GEMM_FWD, true>(mA, mB, a, nt, st) : launch16<DIB_GEMM_FWD, false>(mA, mB, a, nt, st);
+  return bf16 ? launch16<DIB_GEMM_FWD, true>(mA, mB, a, mA, mB, Int16Args{}, nt, st)
+              : launch16<DIB_GEMM_FWD, false>(mA, mB, a, mA, mB, Int16Args{}, nt, st);
 }
 
 // dz_in[M x K] = (dz[M x N] W16[K x N]^T) * act'(g_in[M x K])      (g_in may be null: no activation, e.g. d_emb)
@@ -872,22 +867,30 @@ cudaError_t dib_int16_dgrad(const void* dz, int ld_dz, const void* w16, const vo
   a.out16 = static_cast<uint16_t*>(dz_in); a.ldc = ld_out; a.X = static_cast<const uint16_t*>(g_in); a.ldx = ld_g;
   a.M = M; a.T = N; a.C = K; a.act = act; a.alpha = alpha; a.out_scale = 1.f; a.nsplit = 1; a.dbias = colsum_part;
   const long long nt = (long long)DIB_CEIL_DIV(M, kBM) * DIB_CEIL_DIV(K, kBN);
-  return bf16 ? launch16<DIB_GEMM_DGRAD, true>(mA, mB, a, nt, st) : launch16<DIB_GEMM_DGRAD, false>(mA, mB, a, nt, st);
+  return bf16 ? launch16<DIB_GEMM_DGRAD, true>(mA, mB, a, mA, mB, Int16Args{}, nt, st)
+              : launch16<DIB_GEMM_DGRAD, false>(mA, mB, a, mA, mB, Int16Args{}, nt, st);
 }
 
-// dW[K x N] (fp32 split partials, * out_scale) = g_in[M x K]^T dz[M x N].  The bias gradients come from the kernel that
-// produces dz (dgrad epilogue / output head), not from here.
-cudaError_t dib_int16_wgrad(const void* g_in, int ld_g, const void* dz, int ld_dz, float* dW_part, int M, int K, int N, int nsplit,
-                            int rows_per_split, long long split_stride, float out_scale, int bf16, cudaStream_t st) {
+// dW (fp32 split partials, * out_scale) = g_in^T dz of one or two layers.  Two layers' tiles fill a wave of CTAs that one
+// layer's do not.  The bias gradients come from the kernel that produces dz (dgrad epilogue / output head), not from here.
+cudaError_t dib_int16_wgrad(const DibInt16Wgrad* layers, int count, int M, long long split_stride, float out_scale, int bf16,
+                            cudaStream_t st) {
+  if (count < 1 || count > 2) return cudaErrorInvalidValue;
   if (!encode_fn3()) return cudaErrorNotSupported;
-  CUtensorMap mA, mB;
-  if (!map_mn(&mA, g_in, K, M, ld_g, kBM / 64) || !map_mn(&mB, dz, N, M, ld_dz, kBN / 64))
-    return cudaErrorInvalidValue;
-  Int16Args a{};
-  a.out32 = dW_part; a.ldc = N; a.dbias = nullptr; a.M = M; a.T = 0; a.C = N; a.R = K; a.out_scale = out_scale;
-  a.nsplit = nsplit; a.rows_per_split = rows_per_split; a.split_stride = split_stride;
-  const long long nt = (long long)DIB_CEIL_DIV(N, kBN) * DIB_CEIL_DIV(K, kBM) * nsplit;
-  return bf16 ? launch16<DIB_GEMM_WGRAD, true>(mA, mB, a, nt, st) : launch16<DIB_GEMM_WGRAD, false>(mA, mB, a, nt, st);
+  CUtensorMap mA[2], mB[2];
+  Int16Args a[2] = {};              // a[1].nsplit == 0: no second problem
+  long long nt = 0;
+  for (int q = 0; q < count; ++q) {
+    const DibInt16Wgrad& l = layers[q];
+    if (!map_mn(&mA[q], l.g_in, l.K, M, l.K, kBM / 64) || !map_mn(&mB[q], l.dz, l.N, M, l.N, kBN / 64))
+      return cudaErrorInvalidValue;
+    a[q].out32 = l.dW_part; a[q].ldc = l.N; a[q].M = M; a[q].C = l.N; a[q].R = l.K; a[q].out_scale = out_scale;
+    a[q].nsplit = l.nsplit; a[q].rows_per_split = l.rows_per_split; a[q].split_stride = split_stride;
+    nt += (long long)DIB_CEIL_DIV(l.K, kBM) * DIB_CEIL_DIV(l.N, kBN) * l.nsplit;
+  }
+  if (count == 1) { mA[1] = mA[0]; mB[1] = mB[0]; }
+  return bf16 ? launch16<DIB_GEMM_WGRAD, true>(mA[0], mB[0], a[0], mA[1], mB[1], a[1], nt, st)
+              : launch16<DIB_GEMM_WGRAD, false>(mA[0], mB[0], a[0], mA[1], mB[1], a[1], nt, st);
 }
 
 bool dib_int16_fwd2_ok(int K0, int N1, int N2, int out_dim) {
@@ -937,22 +940,6 @@ cudaError_t dib_int16_fwd2_head(const void* g_in, int ld_in, int K0, const void*
 #undef DIB_F2_LAUNCH
   dib_note_launch();
   return cudaGetLastError();
-}
-
-// the weight gradients of TWO layers in one launch (same batch M, same partial stride): dW_j = g_in_j^T dz_j over batch slices
-cudaError_t dib_int16_wgrad_pair(const void* g_in0, int K0, const void* dz0, int N0, float* dW_part0, int nsplit0, int rps0,
-                                 const void* g_in1, int K1, const void* dz1, int N1, float* dW_part1, int nsplit1, int rps1,
-                                 int M, long long split_stride, float out_scale, int bf16, cudaStream_t st) {
-  if (!encode_fn3()) return cudaErrorNotSupported;
-  CUtensorMap mA, mB, mA2, mB2;
-  if (!map_mn(&mA, g_in0, K0, M, K0, kBM / 64) || !map_mn(&mB, dz0, N0, M, N0, kBN / 64) ||
-      !map_mn(&mA2, g_in1, K1, M, K1, kBM / 64) || !map_mn(&mB2, dz1, N1, M, N1, kBN / 64))
-    return cudaErrorInvalidValue;
-  Int16Args a{}, b{};
-  a.out32 = dW_part0; a.ldc = N0; a.M = M; a.C = N0; a.R = K0; a.out_scale = out_scale; a.nsplit = nsplit0; a.rows_per_split = rps0; a.split_stride = split_stride;
-  b.out32 = dW_part1; b.ldc = N1; b.M = M; b.C = N1; b.R = K1; b.out_scale = out_scale; b.nsplit = nsplit1; b.rows_per_split = rps1; b.split_stride = split_stride;
-  const long long nt = (long long)DIB_CEIL_DIV(K0, kBM) * DIB_CEIL_DIV(N0, kBN) * nsplit0 + (long long)DIB_CEIL_DIV(K1, kBM) * DIB_CEIL_DIV(N1, kBN) * nsplit1;
-  return bf16 ? launch16<DIB_GEMM_WGRAD, true>(mA, mB, a, mA2, mB2, b, nt, st) : launch16<DIB_GEMM_WGRAD, false>(mA, mB, a, mA2, mB2, b, nt, st);
 }
 
 int dib_int16_head_blocks(int num_sms) { return num_sms * 2; }

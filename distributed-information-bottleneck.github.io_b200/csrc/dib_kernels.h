@@ -162,11 +162,12 @@ cudaError_t dib_int16_dgrad(const void* dz, int ld_dz, const void* w16, const vo
 struct DibReduceSeg { const float* src; long long row_stride; int nrows; long long count; float scale; float* dst; };
 constexpr int kDibMaxReduceSegs = 8;
 cudaError_t dib_launch_reduce_segments(const DibReduceSeg* segs, int nseg, cudaStream_t st);
-cudaError_t dib_int16_wgrad(const void* g_in, int ld_g, const void* dz, int ld_dz, float* dW_part, int M, int K, int N, int nsplit,
-                            int rows_per_split, long long split_stride, float out_scale, int bf16, cudaStream_t st);
-cudaError_t dib_int16_wgrad_pair(const void* g_in0, int K0, const void* dz0, int N0, float* dW_part0, int nsplit0, int rps0,
-                                 const void* g_in1, int K1, const void* dz1, int N1, float* dW_part1, int nsplit1, int rps1,
-                                 int M, long long split_stride, float out_scale, int bf16, cudaStream_t st);
+// one layer's weight gradient: fp32 split partials of dW[K x N] = g_in[M x K]^T dz[M x N] (leading dimensions K and N) over
+// nsplit batch slices of rows_per_split rows
+struct DibInt16Wgrad { const void* g_in; int K; const void* dz; int N; float* dW_part; int nsplit; int rows_per_split; };
+// the weight gradients of one or two layers (count = 1 or 2) in one launch, same batch M and partial stride
+cudaError_t dib_int16_wgrad(const DibInt16Wgrad* layers, int count, int M, long long split_stride, float out_scale, int bf16,
+                            cudaStream_t st);
 int dib_int16_head_blocks(int num_sms);
 // shapes the fused tail kernel (dib_int16_fwd2_head) handles: fan-in K0 of its first layer, its two widths, the output width
 bool dib_int16_fwd2_ok(int K0, int N1, int N2, int out_dim);

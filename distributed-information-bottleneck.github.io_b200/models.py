@@ -241,10 +241,6 @@ class DistributedIBNet:
         self._step_dev_active = False
         self._step_dev_dirty = False       # _train_step_count moved outside a graph replay: refill the device mirror
         self._replayed_launches = 0        # kernels launched by graph replays (dib_launch_count only sees eager launches)
-        self._side_stream = None
-        # two-bucket all-reduce overlapped with the encoder backward: opt-in (DIB_OVERLAP_ALLREDUCE=1); by default one flat
-        # all-reduce of [grads || stats] runs as an eager call between the backward graph and the optimizer graph
-        self.overlap_allreduce = os.environ.get("DIB_OVERLAP_ALLREDUCE", "0") in ("1", "on", "true", "yes")
         self._inference_calls = 0          # fresh noise per un-seeded inference call (tf.random.normal, models.py:108)
         self.optimizer = None
         self.compiled_metrics_names = []
@@ -462,18 +458,18 @@ class DistributedIBNet:
         _lib.check(self._lib.dib_set_noise_step_device(self._handle, _lib.ptr(self._noise_step_dev) if on else None))
         self._step_dev_active = on
 
-    def _backward(self, x, y, global_batch, eps=None, sample_offset=0, step=None, phases=3, device_step=False):
-        """dib_train_step[_phased]: forward + reverse mode into self._gradstats = [grads (P) || stats (F+3)]."""
+    def _backward(self, x, y, global_batch, eps=None, sample_offset=0, step=None, device_step=False):
+        """dib_train_step: forward + reverse mode into self._gradstats = [grads (P) || stats (F+3)]."""
         n = x.shape[0]
         self._ensure_handle(n)
         P = self._P
         self._set_device_step(device_step)
         st = 0 if device_step else (self._train_step_count if step is None else step)
-        _lib.check(self._lib.dib_train_step_phased(
+        _lib.check(self._lib.dib_train_step(
             self._handle, _lib.ptr(self._params), _lib.ptr(x), _lib.ptr(y), n, _lib.ptr(self.beta._dev),
             1.0 / float(global_batch), _lib.ptr(eps), self.noise_seed, int(st) & 0xFFFFFFFF,
             int(sample_offset), _lib.ptr(self._gradstats), _lib.ptr(self._gradstats[P:]), _lib.ptr(self._workspace),
-            int(phases), _stream()))
+            _stream()))
 
     def apply_gradients(self, flat_grads):
         """optimizer.apply_gradients(zip(grads, model.trainable_variables)) of the custom loops (train.py:217-219,
@@ -504,27 +500,9 @@ class DistributedIBNet:
     def _adam(self):
         self._optimizer_update(self._gradstats)
 
-    def _reduce_overlapped(self, world, run_phase1, run_phase2):
-        """The data-parallel exchange in two buckets: [integration grads || stats] is all-reduced on a side stream while
-        the encoder backward (phase 2) runs; [encoder grads] follows on the compute stream.  One process per GPU, NCCL."""
-        pe = self._p_enc
-        run_phase1()
-        if self._side_stream is None:
-            self._side_stream = torch.cuda.Stream(device=self.device)
-        side, main = self._side_stream, torch.cuda.current_stream()
-        side.wait_stream(main)
-        with torch.cuda.stream(side):
-            work = parallel.allreduce_sum_async(self._gradstats[pe:], self.process_group)
-        run_phase2()
-        parallel.allreduce_sum_(self._gradstats[:pe], self.process_group)
-        if work is not None:
-            work.wait()                      # the compute stream waits for bucket 1 (no host sync)
-        main.wait_stream(side)
-
     def _train_step(self, x, y, global_batch, eps=None, sample_offset=0):
-        """backward, all-reduce over the data-parallel group, Keras-Adam.  Replayed from CUDA graphs once a
-        (batch size, offset) combination has run eagerly twice; the all-reduce is split into two buckets so that the
-        first overlaps the encoder backward."""
+        """backward, one flat all-reduce of [grads || stats] over the data-parallel group, Keras-Adam.  Replayed from
+        CUDA graphs once a (batch size, offset) combination has run eagerly twice."""
         P = self._P
         world, _ = parallel.world_and_rank(self.process_group)
         key = (int(x.shape[0]), int(global_batch), int(sample_offset), world)
@@ -535,12 +513,8 @@ class DistributedIBNet:
             if g is not None:
                 return self._replay_step(g, x, y, world)
             self._graph_seen[key] = self._graph_seen.get(key, 0) + 1
-        if world > 1 and self.overlap_allreduce:
-            self._reduce_overlapped(world, lambda: self._backward(x, y, global_batch, eps, sample_offset, phases=1),
-                                    lambda: self._backward(x, y, global_batch, eps, sample_offset, phases=2))
-        else:
-            self._backward(x, y, global_batch, eps, sample_offset)
-            parallel.allreduce_sum_(self._gradstats, self.process_group)
+        self._backward(x, y, global_batch, eps, sample_offset)
+        parallel.allreduce_sum_(self._gradstats, self.process_group)
         self._adam()
         self._train_step_count += 1
         self._step_dev_dirty = True
@@ -550,7 +524,7 @@ class DistributedIBNet:
     def _capture_step(self, key):
         """Capture the step for one (n, global_batch, sample_offset, world) into CUDA graphs.  Single GPU: ONE graph
         (forward + backward + Adam + noise-step increment).  Data parallel: two graphs (backward | Adam) with the NCCL all-reduce
-        issued eagerly between them (three -- phase 1 | phase 2 | Adam -- for the opt-in two-bucket overlap).  Inputs are copied into static buffers before each replay; beta,
+        issued eagerly between them.  Inputs are copied into static buffers before each replay; beta,
         learning rate, the Adam step and the Philox step are device scalars, so nothing by-value changes between replays."""
         n, global_batch, sample_offset, world = key
         D = sum(self.feature_dimensionalities)
@@ -578,10 +552,6 @@ class DistributedIBNet:
 
                 if world == 1:
                     cap(lambda: (self._backward(gx, gy, global_batch, None, sample_offset, device_step=True), tail()))
-                elif self.overlap_allreduce:
-                    cap(lambda: self._backward(gx, gy, global_batch, None, sample_offset, phases=1, device_step=True))
-                    cap(lambda: self._backward(gx, gy, global_batch, None, sample_offset, phases=2, device_step=True))
-                    cap(tail)
                 else:        # one all-reduce between backward and optimizer: two graphs
                     cap(lambda: self._backward(gx, gy, global_batch, None, sample_offset, device_step=True))
                     cap(tail)
@@ -608,9 +578,6 @@ class DistributedIBNet:
         g["y"].copy_(y.reshape(g["y"].shape), non_blocking=True)
         if world == 1:
             g["graphs"][0].replay()
-        elif self.overlap_allreduce:
-            self._reduce_overlapped(world, g["graphs"][0].replay, g["graphs"][1].replay)
-            g["graphs"][2].replay()
         else:
             g["graphs"][0].replay()
             parallel.allreduce_sum_(self._gradstats, self.process_group)

@@ -28,11 +28,3 @@ def allreduce_sum_(flat: torch.Tensor, group=None):
     if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
         dist.all_reduce(flat, op=dist.ReduceOp.SUM, group=group)
     return flat
-
-
-def allreduce_sum_async(flat: torch.Tensor, group=None):
-    """Asynchronous in-place sum on the CURRENT stream's NCCL channel; returns the work handle (``.wait()`` makes the then
-    current stream wait for it) or None for a single process."""
-    if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
-        return dist.all_reduce(flat, op=dist.ReduceOp.SUM, group=group, async_op=True)
-    return None

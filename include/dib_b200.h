@@ -162,19 +162,8 @@ int dib_encoders_backward(dib_model* h, const float* params, const float* x, con
                           const float* beta_dev, float inv_global_batch, const float* eps, uint64_t seed, uint32_t step,
                           uint64_t sample_offset, float* grads_flat, float* out_stats, void* workspace, void* stream);
 
-/* dib_train_step in two halves, for overlapping the data-parallel collective with the encoder backward:
- *   phases = 1: forward + compiled loss + integration-network backward -> grads_flat[first integration parameter, P) and
- *               out_stats are final (bucket 1 can be all-reduced while phase 2 runs);
- *   phases = 2: encoder backward -> grads_flat[0, first integration parameter) final.  Same arguments as the phase-1 call;
- *   phases = 3: both (== dib_train_step).
- * The first integration parameter is offsets[v] of variable v = number_features * (encoder variables per feature). */
-int dib_train_step_phased(dib_model* h, const float* params, const float* x, const float* y, int64_t n,
-                          const float* beta_dev, float inv_global_batch,
-                          const float* eps, uint64_t seed, uint32_t step, uint64_t sample_offset,
-                          float* grads_flat, float* out_stats, void* workspace, int32_t phases, void* stream);
-
 /* CUDA-Graph replay: a captured launch cannot carry a fresh by-value `step`, so the Philox step word may come from device
- * memory: when step_dev != NULL every later dib_train_step[_phased] call of this handle uses step + *step_dev (dib_forward
+ * memory: when step_dev != NULL every later dib_train_step call of this handle uses step + *step_dev (dib_forward
  * and the encoder-only entry points keep the by-value step).  The caller owns the counter and advances it (on the stream)
  * between steps.  NULL restores the by-value behaviour. */
 int dib_set_noise_step_device(dib_model* h, const uint32_t* step_dev);
