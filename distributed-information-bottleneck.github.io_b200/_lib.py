@@ -6,10 +6,10 @@ from ctypes import POINTER, c_char_p, c_float, c_int32, c_int64, c_size_t, c_uin
 
 from . import build as _build
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 
 ACTIVATIONS = {None: 0, "linear": 0, "relu": 1, "tanh": 2, "leaky_relu": 3, "sigmoid": 4, "elu": 5}
-LOSSES = {"bce_logits": 0, "sparse_ce_logits": 1, "mse": 2, "external": 3, "bce_probs": 4}
+LOSSES = {"bce_logits": 0, "sparse_ce_logits": 1, "mse": 2, "external": 3, "bce_probs": 4, "infonce": 5}
 ENCODER_KINDS = {"mlp": 0, "simple": 1}
 # 'fp16' / 'bf16': fused 16-bit-operand wgmma kernels (fp32 accumulate); 'tf32': tf32 wgmma GEMMs on fp32 storage;
 # 'fp32': exact CUDA-core FMA parity path.  See enum dib_precision in include/dib_b200.h.
@@ -40,6 +40,12 @@ class DibConfig(ctypes.Structure):
         ("kl_loss_scale", c_float),
         ("encoder_kind", c_int32),
         ("dropout_rate", c_float),
+        # abi_version 3: DIB_LOSS_INFONCE's output encoder and loss
+        ("y_dimensionality", c_int32),
+        ("number_y_encoder_layers", c_int32),
+        ("y_encoder_architecture", POINTER(c_int32)),
+        ("infonce_similarity", c_int32),
+        ("infonce_temperature", c_float),
     ]
 
 
@@ -62,6 +68,7 @@ SIGNATURES = {
     "dib_optimizer_step": (c_int32, [c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_float,
                                      c_float, c_float, c_void_p]),
     "dib_integration_forward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
+    "dib_output_encoder_forward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
     "dib_positional_encoding": (c_int32, [c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p]),
     "dib_metrics_update": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_void_p]),
     "dib_metrics_update_ex": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_float, c_float, c_void_p]),

@@ -91,6 +91,19 @@ struct dib_model {
     bool tail_fused = false;        // int16: last two hidden layers + head + loss as one kernel (dib_int16_fwd2_head)
     bool head1 = false;             // int16, no fused tail: the out = 1 head kernel instead of the generic one
   } route;
+  // DIB_LOSS_INFONCE (train.py:180-289): the output encoder y -> [PE] -> Dense(y_arch[j], act)... -> Dense(out), its variables
+  // after the model's in the flat buffer, and the streaming InfoNCE loss (dib_infonce_stream.cu)
+  long long Px = 0;                 // end of the model's own parameters (== P without an output encoder)
+  int ydim = 0, Ly = 0, sim_kind = 0, ldype = 0;
+  float temperature = 1.f;
+  std::vector<int> y_arch;
+  std::vector<long long> yW, yB;    // [j]
+  Buf ype, y_out, d_y_out;          // PE(y), e2 = output_encoder(y), d loss / d e2
+  std::vector<Buf> y_act, d_yact;   // index 1..Ly
+  long long nce_off = 0;            // 3 * max_batch floats of InfoNCE scratch
+  std::vector<int> y_fwd, y_dgrad, y_wgrad;
+  int* d_ycol_src = nullptr;
+  int* d_ycol_freq = nullptr;
   // custom-step variants (SURVEY 8f3)
   float lv_off = 0.f, kl_exp = 1.f, kl_scale = 1.f;
   const uint32_t* step_dev = nullptr;  // optional device-resident addend of the Philox step word (dib_set_noise_step_device)
@@ -114,6 +127,9 @@ int enc_fan_in(const dib_model* h, int f, int j) { return j == 0 ? h->w_in[f] : 
 int enc_fan_out(const dib_model* h, int j) { return j < h->L ? h->enc_arch[j] : 2 * h->E; }
 int int_fan_in(const dib_model* h, int j) { return j == 0 ? h->F * h->E : h->int_arch[j - 1]; }
 int int_fan_out(const dib_model* h, int j) { return j < h->Li ? h->int_arch[j] : h->out; }
+bool infonce(const dib_model* h) { return h->loss == DIB_LOSS_INFONCE; }
+int y_fan_in(const dib_model* h, int j) { return j == 0 ? h->ydim * h->nfreq : h->y_arch[j - 1]; }
+int y_fan_out(const dib_model* h, int j) { return j < h->Ly ? h->y_arch[j] : h->out; }
 
 // the one place the kernel path is chosen.  fused_ok / int16_ok are what dib_create found the shapes to support; the bits of
 // `unfused` (dib_debug_force_unfused) turn paths off: 1 = fused encoders, 2 = 16-bit integration network (it reads the fp16
@@ -206,6 +222,16 @@ void plan(dib_model* h) {
   h->beta_eff_off = take(c, 64);
   h->wshadow_off = take(c, h->Pp);      // TF32-rounded copy of the parameters (tensor-core mode B operands)
   h->pack_off = take(c, (long long)(dib_enc_fused_pack_bytes(h->F) + 3) / 4);
+  if (infonce(h)) {                     // the output encoder's activations and gradients, the InfoNCE scratch: all O(max_batch)
+    h->ype = make_buf(c, B, h->ldype, 1);
+    h->y_act.assign(h->Ly + 1, Buf());
+    h->d_yact.assign(h->Ly + 1, Buf());
+    for (int j = 1; j <= h->Ly; ++j) h->y_act[j] = make_buf(c, B, h->y_arch[j - 1], 1);
+    h->y_out = make_buf(c, B, h->out, 1);
+    h->d_y_out = make_buf(c, B, h->out, 1);
+    for (int j = 1; j <= h->Ly; ++j) h->d_yact[j] = make_buf(c, B, h->y_arch[j - 1], 1);
+    h->nce_off = take(c, 3 * B);
+  }
   h->ws_floats = c;
 }
 
@@ -302,6 +328,48 @@ void build_problems(dib_model* h, std::vector<DibGemmProblem>& v) {
     p.c_off = h->intW[j]; p.ldc = int_fan_out(h, j);
     p.x_off = h->intB[j];
     p.R = int_fan_in(h, j); p.C = int_fan_out(h, j);
+    v.push_back(p);
+  }
+  if (!infonce(h)) return;
+  // the output encoder: the same three modes on its own buffers (train.py:186-193)
+  const int Ly = h->Ly;
+  h->y_fwd.assign(Ly + 1, -1); h->y_dgrad.assign(Ly + 1, -1); h->y_wgrad.assign(Ly + 1, -1);
+  auto yA = [&](int j, long long& off, int& ld) {
+    if (j == 0) { off = h->ype.off; ld = h->ldype; } else { off = h->y_act[j].off; ld = h->y_act[j].ld; }
+  };
+  auto yDZ = [&](int j, long long& off, int& ld) {
+    const Buf& b = j == Ly ? h->d_y_out : h->d_yact[j + 1];
+    off = b.off; ld = b.ld;
+  };
+  for (int j = 0; j <= Ly; ++j) {
+    h->y_fwd[j] = (int)v.size();
+    DibGemmProblem p = zero();
+    yA(j, p.a_off, p.lda);
+    p.b_off = h->yW[j]; p.ldb = y_fan_out(h, j);
+    const Buf& o = j < Ly ? h->y_act[j + 1] : h->y_out;
+    p.c_off = o.off; p.ldc = o.ld;
+    p.x_off = h->yB[j];
+    p.T = y_fan_in(h, j); p.C = y_fan_out(h, j); p.act = j < Ly ? h->act : DIB_ACT_LINEAR;
+    v.push_back(p);
+  }
+  for (int j = 1; j <= Ly; ++j) {         // no gradient is taken with respect to y itself
+    h->y_dgrad[j] = (int)v.size();
+    DibGemmProblem p = zero();
+    yDZ(j, p.a_off, p.lda);
+    p.b_off = h->yW[j]; p.ldb = y_fan_out(h, j);
+    p.c_off = h->d_yact[j].off; p.ldc = h->d_yact[j].ld;
+    p.x_off = h->y_act[j].off; p.ldx = h->y_act[j].ld; p.act = h->act;
+    p.T = y_fan_out(h, j); p.C = y_fan_in(h, j);
+    v.push_back(p);
+  }
+  for (int j = 0; j <= Ly; ++j) {
+    h->y_wgrad[j] = (int)v.size();
+    DibGemmProblem p = zero();
+    yA(j, p.a_off, p.lda);
+    yDZ(j, p.b_off, p.ldb);
+    p.c_off = h->yW[j]; p.ldc = y_fan_out(h, j);
+    p.x_off = h->yB[j];
+    p.R = y_fan_in(h, j); p.C = y_fan_out(h, j);
     v.push_back(p);
   }
 }
@@ -433,6 +501,44 @@ int forward_encoders(const Ctx& c, const float* x, const NoiseKey& nk, float* us
   return 0;
 }
 
+// DIB_LOSS_INFONCE with targets, after the integration network wrote e1 = pred: output encoder e2 = output_encoder(y), the
+// streaming InfoNCE loss into the stats row and, training, d loss / d e1 into d_pred (what the DIB_LOSS_EXTERNAL backward reads)
+// and d loss / d e2 into d_y_out (what backward_output_encoder reads)
+int forward_infonce(const Ctx& c, const float* y, bool training, float* user_pred, float* out_stats, int nblk_kl) {
+  dib_model* h = c.h;
+  const int rnd = is_tc(h) ? 1 : 0;
+  prof_begin(c, "y_pe");
+  DIB_CUDA_OK(dib_launch_pe(y, h->ydim, 0, h->d_ycol_src, h->d_ycol_freq, 0, h->ldype, c.ws + h->ype.off, h->ldype, 0, c.n, rnd, c.st));
+  prof_end(c);
+  for (int j = 0; j <= h->Ly; ++j) {
+    prof_begin(c, "y_fwd_l", j);
+    if (gemm(c, DIB_GEMM_FWD, h->y_fwd[j], 1, y_fan_out(h, j), 0, 1, 0)) return 1;
+    prof_end(c);
+  }
+  DibInfonceStream a;
+  a.kind = h->sim_kind; a.temperature = h->temperature;
+  a.e1 = c.ws + h->pred.off; a.ld1 = h->pred.ld;
+  a.e2 = c.ws + h->y_out.off; a.ld2 = h->y_out.ld;
+  a.n = c.n; a.d = h->out;
+  a.scratch = c.ws + h->nce_off;
+  a.loss_sum = c.ws + h->loss_part_off; a.acc_zero = c.ws + h->acc_part_off;
+  a.d_e1 = c.ws + h->d_pred.off; a.ld_d1 = h->d_pred.ld;
+  a.d_e2 = c.ws + h->d_y_out.off; a.ld_d2 = h->d_y_out.ld;
+  a.round_out = rnd;
+  prof_begin(c, "infonce_loss_stats");
+  DIB_CUDA_OK(dib_launch_infonce_stream_loss(a, c.st));
+  DIB_CUDA_OK(dib_launch_finalize_stats(c.ws + h->kl_part_off, h->kl_stride, nblk_kl, c.ws + h->loss_part_off, c.ws + h->acc_part_off,
+                                        1, h->F, c.n, 1, out_stats, c.st));
+  prof_end(c);
+  if (user_pred) DIB_CUDA_OK(dib_launch_copy2d(c.ws + h->pred.off, h->pred.ld, user_pred, h->out, h->out, c.n, c.st));
+  if (training) {
+    prof_begin(c, "infonce_grads");
+    DIB_CUDA_OK(dib_launch_infonce_stream_grads(a, c.st));
+    prof_end(c);
+  }
+  return 0;
+}
+
 // integration half of the forward: integration layers -> prediction, compiled loss / metrics, d loss / d prediction
 // (training) -> the stats row
 int forward_integration(const Ctx& c, const float* y, float inv_batch, bool training, float* user_pred, float* out_stats,
@@ -448,6 +554,7 @@ int forward_integration(const Ctx& c, const float* y, float inv_batch, bool trai
       if (gemm(c, DIB_GEMM_FWD, h->int_fwd[j], 1, int_fan_out(h, j), 0, 1, 0)) return 1;
       prof_end(c);
     }
+    if (infonce(h) && y) return forward_infonce(c, y, training, user_pred, out_stats, nblk_kl);
     prof_begin(c, "loss_stats");
     DIB_CUDA_OK(dib_launch_loss(h->loss, h->out_act, h->alpha, c.ws + h->pred.off, h->pred.ld, y, h->out, c.n, inv_batch,
                                 training ? c.ws + h->d_pred.off : nullptr, user_pred, c.ws + h->loss_part_off,
@@ -634,7 +741,7 @@ int backward_integration(const Ctx& c, float inv_batch, const Split& sp, float* 
       prof_end(c);
     }
     prof_begin(c, "int_split_reduce");
-    DIB_CUDA_OK(dib_launch_reduce_partials(part + p_enc, h->Pp, sp.nsplit, h->P - p_enc, grads_flat + p_enc, c.st));
+    DIB_CUDA_OK(dib_launch_reduce_partials(part + p_enc, h->Pp, sp.nsplit, h->Px - p_enc, grads_flat + p_enc, c.st));
     prof_end(c);
     return 0;
   }
@@ -687,7 +794,26 @@ int backward_integration(const Ctx& c, float inv_batch, const Split& sp, float* 
   prof_begin(c, "int_split_reduce");
   for (int q = 0; q < h->Li; ++q)     // hidden-layer kernels: batch-split partials
     segs->push_back({part + h->intW[q], h->Pp, nsplit_of[q], (long long)int_fan_in(h, q) * int_fan_out(h, q), 1.f, grads_flat + h->intW[q]});
-  segs->push_back({c.ws + h->headpart_off, h->head_stride, h->head_used, h->P - p_head, 1.f, grads_flat + p_head});
+  segs->push_back({c.ws + h->headpart_off, h->head_stride, h->head_used, h->Px - p_head, 1.f, grads_flat + p_head});
+  prof_end(c);
+  return 0;
+}
+
+// the output encoder's backward from the d loss / d e2 forward_infonce left, into grads_flat[Px, P)
+int backward_output_encoder(const Ctx& c, const Split& sp, float* grads_flat) {
+  dib_model* h = c.h;
+  for (int j = h->Ly; j >= 0; --j) {
+    prof_begin(c, "y_wgrad_l", j);
+    if (gemm(c, DIB_GEMM_WGRAD, h->y_wgrad[j], 1, y_fan_out(h, j), y_fan_in(h, j), sp.nsplit, (int)sp.rps)) return 1;
+    prof_end(c);
+    if (j >= 1) {
+      prof_begin(c, "y_dgrad_l", j);
+      if (gemm(c, DIB_GEMM_DGRAD, h->y_dgrad[j], 1, y_fan_in(h, j), 0, 1, 0)) return 1;
+      prof_end(c);
+    }
+  }
+  prof_begin(c, "y_split_reduce");
+  DIB_CUDA_OK(dib_launch_reduce_partials(c.ws + h->part_off + h->Px, h->Pp, sp.nsplit, h->P - h->Px, grads_flat + h->Px, c.st));
   prof_end(c);
   return 0;
 }
@@ -764,7 +890,7 @@ int dib_debug_gemm_tc(int32_t mode, const float* A, int32_t lda, const float* B,
 const char* dib_last_error(void) { return g_last_error.c_str(); }
 
 const char* dib_build_info(void) {
-  return "dib_b200 abi=2 arch=sm_90a paths=fp32-simt,tf32-wgmma,fp16-fused-wgmma,bf16-fused-wgmma";
+  return "dib_b200 abi=3 arch=sm_90a paths=fp32-simt,tf32-wgmma,fp16-fused-wgmma,bf16-fused-wgmma";
 }
 
 int32_t dib_model_info(const dib_model* h, char* out, size_t out_bytes) {
@@ -780,6 +906,8 @@ int32_t dib_model_info(const dib_model* h, char* out, size_t out_bytes) {
     s += fused ? std::string(" operands=") + (h->precision == DIB_PREC_BF16 ? "bf16" : "fp16") : std::string(" operands=tf32");
     s += " accumulate=fp32";
   }
+  if (infonce(h))
+    s += std::string(" output_encoder=") + (is_tc(h) ? "wgmma-tf32" : "simt-fp32") + " loss=infonce-stream-fp32";
   const size_t k = s.size() < out_bytes - 1 ? s.size() : out_bytes - 1;
   memcpy(out, s.data(), k); out[k] = 0;
   return (int32_t)k;
@@ -788,7 +916,8 @@ int32_t dib_model_info(const dib_model* h, char* out, size_t out_bytes) {
 int dib_create(const dib_config* cfg, dib_model** out) {
   if (!cfg || !out) return fail("dib_create: null argument");
   *out = nullptr;
-  if (cfg->abi_version != DIB_ABI_VERSION) return fail("dib_create: abi_version mismatch");
+  // an abi_version 2 struct ends before the InfoNCE fields: read only its prefix
+  if (cfg->abi_version != 2 && cfg->abi_version != DIB_ABI_VERSION) return fail("dib_create: abi_version mismatch");
   if (cfg->number_features < 1 || cfg->feature_embedding_dimension < 1 || cfg->output_dimensionality < 1 ||
       cfg->max_batch < 1 || cfg->number_encoder_layers < 0 || cfg->number_integration_layers < 0)
     return fail("dib_create: invalid sizes");
@@ -798,7 +927,18 @@ int dib_create(const dib_config* cfg, dib_model** out) {
   if (cfg->activation_fn < 0 || cfg->activation_fn > DIB_ACT_ELU || cfg->output_activation_fn < 0 ||
       cfg->output_activation_fn > DIB_ACT_ELU)
     return fail("dib_create: unknown activation");
-  if (cfg->loss < 0 || cfg->loss > DIB_LOSS_BCE_PROBS) return fail("dib_create: unknown loss");
+  if (cfg->loss < 0 || cfg->loss > DIB_LOSS_INFONCE || (cfg->loss == DIB_LOSS_INFONCE && cfg->abi_version < 3))
+    return fail("dib_create: unknown loss");
+  if (cfg->loss == DIB_LOSS_INFONCE) {
+    if (cfg->y_dimensionality < 1 || cfg->number_y_encoder_layers < 0 || (cfg->number_y_encoder_layers > 0 && !cfg->y_encoder_architecture))
+      return fail("dib_create: InfoNCE needs y_dimensionality >= 1 and an output-encoder architecture");
+    for (int j = 0; j < cfg->number_y_encoder_layers; ++j)
+      if (cfg->y_encoder_architecture[j] < 1) return fail("dib_create: output-encoder width < 1");
+    if (cfg->infonce_similarity < 0 || cfg->infonce_similarity > 4) return fail("dib_create: unknown InfoNCE similarity");
+    if (!(cfg->infonce_temperature > 0.f)) return fail("dib_create: InfoNCE temperature must be > 0");
+    if (cfg->output_dimensionality > 512) return fail("dib_create: InfoNCE needs output_dimensionality <= 512");
+    if (cfg->output_activation_fn != DIB_ACT_LINEAR) return fail("dib_create: InfoNCE needs a linear output (train.py:117)");
+  }
   dib_model* h = new (std::nothrow) dib_model();
   if (!h) return fail("dib_create: out of host memory");
   h->F = cfg->number_features; h->L = cfg->number_encoder_layers; h->Li = cfg->number_integration_layers;
@@ -811,6 +951,11 @@ int dib_create(const dib_config* cfg, dib_model** out) {
   h->kl_scale = cfg->kl_loss_scale == 0.f ? 1.f : cfg->kl_loss_scale;
   h->simple = cfg->encoder_kind == DIB_ENCODER_SIMPLE;
   h->drop = cfg->dropout_rate;
+  if (infonce(h)) {
+    h->ydim = cfg->y_dimensionality; h->Ly = cfg->number_y_encoder_layers;
+    h->y_arch.assign(cfg->y_encoder_architecture, cfg->y_encoder_architecture + h->Ly);
+    h->sim_kind = cfg->infonce_similarity; h->temperature = cfg->infonce_temperature;
+  }
   if (!(h->drop >= 0.f && h->drop < 1.f)) { delete h; return fail("dib_create: dropout_rate must be in [0, 1)"); }
   if (cfg->encoder_kind != DIB_ENCODER_MLP && cfg->encoder_kind != DIB_ENCODER_SIMPLE) { delete h; return fail("dib_create: unknown encoder_kind"); }
   if (!(h->kl_exp > 0.f)) { delete h; return fail("dib_create: kl_loss_exponent must be > 0"); }
@@ -840,6 +985,12 @@ int dib_create(const dib_config* cfg, dib_model** out) {
     h->D += d;
   }
   h->ldpe = (int)col_src.size();
+  // the output encoder's positional encoding: one block per frequency over the y columns (train.py:187-188)
+  std::vector<int> ycol_src, ycol_freq;
+  for (int blk = 0; infonce(h) && blk < h->nfreq; ++blk)
+    for (int k = 0; k < h->ydim; ++k) { ycol_src.push_back(k); ycol_freq.push_back(blk == 0 ? 0 : (1 << blk)); }
+  while (ycol_src.size() % 4) { ycol_src.push_back(-1); ycol_freq.push_back(0); }
+  h->ldype = (int)ycol_src.size();
 
   // flat parameter layout (Keras variable order: per feature W,b per layer; then the integration network)
   long long off = 0;
@@ -863,6 +1014,11 @@ int dib_create(const dib_config* cfg, dib_model** out) {
     h->intW.push_back(add_var(int_fan_in(h, j), int_fan_out(h, j)));
     h->intB.push_back(add_var(0, int_fan_out(h, j)));
   }
+  h->Px = off;
+  for (int j = 0; infonce(h) && j <= h->Ly; ++j) {     // all_trainable_variables = model + output_encoder (train.py:198)
+    h->yW.push_back(add_var(y_fan_in(h, j), y_fan_out(h, j)));
+    h->yB.push_back(add_var(0, y_fan_out(h, j)));
+  }
   h->P = off; h->Pp = DIB_ROUND_UP(off, 64);
   {
     int dev = 0;
@@ -885,6 +1041,12 @@ int dib_create(const dib_config* cfg, dib_model** out) {
   if (e == cudaSuccess) e = cudaMemcpy(h->d_col_src, col_src.data(), col_src.size() * sizeof(int), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemcpy(h->d_col_freq, col_freq.data(), col_freq.size() * sizeof(int), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemcpy(h->d_col_feat, col_feat.data(), col_feat.size() * sizeof(int), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && infonce(h)) {
+    e = cudaMalloc(&h->d_ycol_src, ycol_src.size() * sizeof(int));
+    if (e == cudaSuccess) e = cudaMalloc(&h->d_ycol_freq, ycol_freq.size() * sizeof(int));
+    if (e == cudaSuccess) e = cudaMemcpy(h->d_ycol_src, ycol_src.data(), ycol_src.size() * sizeof(int), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(h->d_ycol_freq, ycol_freq.data(), ycol_freq.size() * sizeof(int), cudaMemcpyHostToDevice);
+  }
   if (e != cudaSuccess) {
     std::string msg = std::string("dib_create: CUDA error: ") + cudaGetErrorString(e);
     dib_destroy(h);
@@ -916,9 +1078,9 @@ int dib_create(const dib_config* cfg, dib_model** out) {
         d.b2_off = lt + 5 * F; d.x_off = it; d.fdim = it + F;
         h->fused_ok = true;
         // 16-bit integration path: hidden widths multiples of 128, last hidden width 256, narrow output head
-        // (the fused head owns the compiled loss, so a caller-owned loss takes the TF32 integration kernels)
+        // (the fused head owns the compiled loss, so a caller-owned loss and InfoNCE take the TF32 integration kernels)
         bool iok = h->Li >= 1 && (h->F * h->E) % 64 == 0 && h->int_arch[h->Li - 1] == 256 && h->out <= 16 &&
-                   h->loss != DIB_LOSS_EXTERNAL;
+                   h->loss != DIB_LOSS_EXTERNAL && h->loss != DIB_LOSS_INFONCE;
         for (int j = 0; iok && j < h->Li; ++j) iok = h->int_arch[j] % 128 == 0 && (h->intB[j] & 3) == 0;
         h->int16_ok = iok;
       }
@@ -937,6 +1099,8 @@ void dib_destroy(dib_model* h) {
   if (h->d_col_feat) cudaFree(h->d_col_feat);
   if (h->d_xoff) cudaFree(h->d_xoff);
   if (h->d_fused_tables) cudaFree(h->d_fused_tables);
+  if (h->d_ycol_src) cudaFree(h->d_ycol_src);
+  if (h->d_ycol_freq) cudaFree(h->d_ycol_freq);
   for (auto& r : h->prof) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
   delete h;
 }
@@ -1017,6 +1181,7 @@ int dib_train_step(dib_model* h, const float* params, const float* x, const floa
   const Split sp = batch_split(n);
   std::vector<DibReduceSeg> segs;          // fixed-order reductions of the step, run as ONE launch at the end
   if (backward_integration(c, inv_global_batch, sp, grads_flat, &segs)) return 1;
+  if (infonce(h) && backward_output_encoder(c, sp, grads_flat)) return 1;
   int nrows = 0;
   const bool d16 = h->route.int16;         // the 16-bit integration backward leaves d emb in fp16
   if (backward_encoders(c, x, nk, d16 ? nullptr : c.ws + h->d_emb.off, d16 ? 0 : h->d_emb.ld, d16 ? c.ws + h->demb16_off : nullptr,
@@ -1076,6 +1241,21 @@ int dib_integration_forward(dib_model* h, const float* params, const float* emb,
   for (int j = 0; j <= h->Li; ++j)
     if (gemm(c, DIB_GEMM_FWD, h->int_fwd[j], 1, int_fan_out(h, j), 0, 1, 0)) return 1;
   DIB_CUDA_OK(dib_launch_copy2d(c.ws + h->pred.off, h->pred.ld, out_pred, h->out, h->out, n, c.st));
+  return 0;
+}
+
+int dib_output_encoder_forward(dib_model* h, const float* params, const float* y, int64_t n, float* out, void* workspace, void* stream) {
+  if (check_call(h, params, y, n, workspace)) return 1;
+  if (!infonce(h)) return fail("dib_output_encoder_forward: the model has no output encoder (loss is not DIB_LOSS_INFONCE)");
+  if (!out) return fail("dib_output_encoder_forward: null output");
+  if (n == 0) return 0;
+  Ctx c{h, params, static_cast<float*>(workspace), static_cast<cudaStream_t>(stream), (int)n};
+  const int rnd = is_tc(h) ? 1 : 0;
+  if (rnd) DIB_CUDA_OK(dib_launch_round_copy(c.params, c.ws + h->wshadow_off, h->P, c.st));
+  DIB_CUDA_OK(dib_launch_pe(y, h->ydim, 0, h->d_ycol_src, h->d_ycol_freq, 0, h->ldype, c.ws + h->ype.off, h->ldype, 0, c.n, rnd, c.st));
+  for (int j = 0; j <= h->Ly; ++j)
+    if (gemm(c, DIB_GEMM_FWD, h->y_fwd[j], 1, y_fan_out(h, j), 0, 1, 0)) return 1;
+  DIB_CUDA_OK(dib_launch_copy2d(c.ws + h->y_out.off, h->y_out.ld, out, h->out, h->out, n, c.st));
   return 0;
 }
 

@@ -91,6 +91,23 @@ cudaError_t dib_launch_similarity(int kind, const float* e1, int64_t n, const fl
 cudaError_t dib_launch_infonce_head(int kind, const float* e1, const float* e2, int64_t n, int d, float temperature,
                                     float* scratch, float* out_loss, float* d_e1, float* d_e2, cudaStream_t st);
 
+// the InfoNCE loss of DIB_LOSS_INFONCE with memory linear in n (dib_infonce_stream.cu): e1 [n, d] (ld1), e2 [n, d] (ld2), d <= 512
+struct DibInfonceStream {
+  int kind; float temperature;
+  const float* e1; int ld1;
+  const float* e2; int ld2;
+  int64_t n; int d;
+  float* scratch;                  // 3n floats: row log-sum-exps | column log-sum-exps | diagonal of S
+  float* loss_sum;                 // [1] = sum_i (r_i + c_i - 2 s_ii) = n * loss
+  float* acc_zero;                 // [1] = 0 (the accuracy slot of the stats), nullable
+  float* d_e1; int ld_d1;          // d loss / d e1, d loss / d e2 (pad columns zeroed); each nullable
+  float* d_e2; int ld_d2;
+  int round_out;                   // round the gradients to the TF32 grid (tensor-core operands)
+};
+// the row / column sweeps and the loss; then (after it, reading its scratch) the two gradient sweeps
+cudaError_t dib_launch_infonce_stream_loss(const DibInfonceStream& a, cudaStream_t st);
+cudaError_t dib_launch_infonce_stream_grads(const DibInfonceStream& a, cudaStream_t st);
+
 cudaError_t dib_launch_metrics_update(const float* stats, const float* beta_dev, float* acc, int F, float kl_exponent,
                                       float kl_scale, cudaStream_t st);
 

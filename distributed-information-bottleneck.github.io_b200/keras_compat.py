@@ -90,10 +90,40 @@ class MeanSquaredError(_Loss):
         super().__init__(from_logits=True, name=name)
 
 
+class InfoNCE(_Loss):
+    """The InfoNCE path of train.py:180-289 (``--infonce_loss``; the double pendulum's loss, data.py:131) as a compiled loss.
+
+    The model is trained together with an output encoder for y -- positional encoding as the model's, ``Dense(h,
+    activation_fn)`` for every width of ``y_encoder_architecture``, then a linear ``Dense(output_dimensionality)``
+    (train.py:186-193) -- on the symmetric InfoNCE of train.py:201-213 between ``model(x)`` and ``output_encoder(y)``:
+    ``mean_i CE(i, S[i,:]) + mean_i CE(i, S^T[i,:])`` with ``S = get_scaled_similarity(., ., similarity, temperature)``.
+    Defaults are train.py:55-62's.  ``y_dimensionality`` is the width of y (it sizes the output encoder)."""
+    kind = "infonce"
+
+    def __init__(self, y_dimensionality, y_encoder_architecture=(128, 128), similarity="l2", temperature=1.0, name=None):
+        from .utils import SIMILARITY_TYPES
+        super().__init__(from_logits=True, name=name)
+        if similarity not in SIMILARITY_TYPES:
+            raise ValueError(f"similarity must be one of {sorted(SIMILARITY_TYPES)}, got {similarity!r}")
+        if not float(temperature) > 0:
+            raise ValueError("temperature must be > 0")
+        self.y_dimensionality = int(y_dimensionality)
+        self.y_encoder_architecture = [int(h) for h in y_encoder_architecture]
+        if self.y_dimensionality < 1 or any(h < 1 for h in self.y_encoder_architecture):
+            raise ValueError("y_dimensionality and the output-encoder widths must be >= 1")
+        self.similarity = similarity
+        self.temperature = float(temperature)
+
+    def spec(self):
+        """What shapes the handle: equal specs share the output encoder's layout and kernels."""
+        return (self.y_dimensionality, tuple(self.y_encoder_architecture), self.similarity, self.temperature)
+
+
 class losses:
     BinaryCrossentropy = BinaryCrossentropy
     SparseCategoricalCrossentropy = SparseCategoricalCrossentropy
     MeanSquaredError = MeanSquaredError
+    InfoNCE = InfoNCE
 
 
 def resolve_loss(loss):
@@ -114,6 +144,9 @@ def resolve_loss(loss):
             return "bce_probs"
         if key in ("external", "custom"):       # GradientTape-style loops: the caller owns the task loss
             return "external"
+        if key == "infonce":                    # what data.py:131 returns for the pendulum
+            raise ValueError("loss='infonce' needs the width of y and the output-encoder architecture: "
+                             "compile with loss=losses.InfoNCE(y_dimensionality=..., y_encoder_architecture=[...])")
     raise ValueError(f"unsupported loss {loss!r}")
 
 

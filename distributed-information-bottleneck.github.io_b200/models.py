@@ -18,7 +18,7 @@ import torch
 
 from . import _lib
 from . import parallel
-from .keras_compat import Adam, RMSprop, SGD, Callback, History, optimizers, resolve_loss
+from .keras_compat import Adam, InfoNCE, RMSprop, SGD, Callback, History, optimizers, resolve_loss
 
 
 def _require_cuda():
@@ -147,6 +147,42 @@ class _IntegrationNetwork(_Network):
         return _as_numpy_like(emb, out)
 
 
+class _OutputEncoder(_Network):
+    """model.output_encoder of a model compiled with ``losses.InfoNCE`` (train.py:186-193): deterministic
+    [n, y_dimensionality] -> [n, output_dimensionality].  Runs dib_output_encoder_forward."""
+
+    def __call__(self, y, training=None):
+        m = self._model
+        with torch.cuda.device(m.device):
+            t = m._targets(y)
+            n = t.shape[0]
+            m._ensure_handle(n)
+            out = torch.empty(n, m.output_dimensionality, dtype=torch.float32, device=m.device)
+            _lib.check(m._lib.dib_output_encoder_forward(m._handle, _lib.ptr(m._params), _lib.ptr(t), n, _lib.ptr(out),
+                                                         _lib.ptr(m._workspace), _stream()))
+        return _as_numpy_like(y, out)
+
+
+def infonce_epoch_batches(n, batch_size):
+    """The training batches of one InfoNCE epoch (train.py:222-231): InfoNCE needs full, equal batches, so an epoch is
+    floor(n / batch_size) consecutive slices [b0, b1) of that epoch's permutation and the remainder is dropped."""
+    n, batch_size = int(n), int(batch_size)
+    if n < batch_size:
+        raise ValueError(f"InfoNCE needs at least one full batch: {n} samples < batch_size {batch_size}")
+    return [(k * batch_size, (k + 1) * batch_size) for k in range(n // batch_size)]
+
+
+def infonce_validation_batches(n, batch_size):
+    """The validation batches of InfoNCE (train.py:233-234: ``repeat().shuffle().batch(B).take(n // B + 1)``):
+    floor(n / batch_size) + 1 full batches of positions into the validation permutation, repeated end to end, so the
+    last batch wraps around.  Returns an int64 array [batches, batch_size]."""
+    n, batch_size = int(n), int(batch_size)
+    if n < 1:
+        raise ValueError("empty validation set")
+    nb = n // batch_size + 1
+    return np.arange(nb * batch_size, dtype=np.int64).reshape(nb, batch_size) % n
+
+
 class DistributedIBNet:
     """Distributed IB model where each feature is passed through its own probabilistic encoder MLP
     (models.py:26-123; ``dropout_rate``/``training`` from nb-radial cell 5).
@@ -215,6 +251,7 @@ class DistributedIBNet:
 
         self._lib = _lib.load()
         self._loss_kind = "bce_logits"
+        self._infonce = None               # the compiled losses.InfoNCE: its output encoder is part of the parameters
         self._handle = None
         self._handle_key = None
         self._workspace = None
@@ -249,8 +286,10 @@ class DistributedIBNet:
         n_enc_vars = 2 if self.encoder_kind == "simple" else 2 * (len(self.feature_encoder_architecture) + 1)
         self.feature_encoders = [                                            # models.py:79
             _FeatureEncoder(self, i, range(i * n_enc_vars, (i + 1) * n_enc_vars)) for i in range(self.number_features)]
+        self._n_model_vars = len(self._var_off)
         self.integration_network = _IntegrationNetwork(                      # models.py:84
-            self, range(self.number_features * n_enc_vars, len(self._var_off)))
+            self, range(self.number_features * n_enc_vars, self._n_model_vars))
+        self.output_encoder = None                                           # losses.InfoNCE: train.py:186-193
         self._p_enc = int(self._var_off[self.number_features * n_enc_vars])  # first integration-network parameter
 
     # ------------------------------------------------------------------ library handle / buffers
@@ -260,6 +299,10 @@ class DistributedIBNet:
         L, Li = len(self.feature_encoder_architecture), len(self.integration_network_architecture)
         self._c_ea = (ctypes.c_int32 * max(L, 1))(*self.feature_encoder_architecture)
         self._c_ia = (ctypes.c_int32 * max(Li, 1))(*self.integration_network_architecture)
+        nce = self._infonce
+        y_arch = nce.y_encoder_architecture if nce is not None else []
+        self._c_ya = (ctypes.c_int32 * max(len(y_arch), 1))(*y_arch)
+        from .utils import SIMILARITY_TYPES
         return _lib.DibConfig(
             abi_version=_lib.ABI_VERSION, number_features=F, feature_dimensionalities=self._c_fd,
             number_encoder_layers=L, feature_encoder_architecture=self._c_ea,
@@ -272,7 +315,10 @@ class DistributedIBNet:
             output_activation_fn=_lib.ACTIVATIONS[self.output_activation_fn],
             loss=_lib.LOSSES[self._loss_kind], precision=_lib.PRECISIONS[self.precision], max_batch=int(max_batch),
             logvar_offset=self.logvar_offset, kl_loss_exponent=self.kl_loss_exponent, kl_loss_scale=self.kl_loss_scale,
-            encoder_kind=_lib.ENCODER_KINDS[self.encoder_kind], dropout_rate=self.dropout_rate)
+            encoder_kind=_lib.ENCODER_KINDS[self.encoder_kind], dropout_rate=self.dropout_rate,
+            y_dimensionality=nce.y_dimensionality if nce is not None else 0, number_y_encoder_layers=len(y_arch),
+            y_encoder_architecture=self._c_ya, infonce_similarity=SIMILARITY_TYPES[nce.similarity] if nce is not None else 0,
+            infonce_temperature=nce.temperature if nce is not None else 1.0)
 
     def _query_layout(self):
         with torch.cuda.device(self.device):
@@ -289,7 +335,7 @@ class DistributedIBNet:
                 self._lib.dib_destroy(h)
 
     def _ensure_handle(self, n):
-        key = (self._loss_kind, self.precision)
+        key = (self._loss_kind, self.precision, self._infonce.spec() if self._infonce is not None else None)
         if self._handle is not None and self._handle_key == key and n <= self._max_batch:
             return
         self._release_handle()
@@ -336,6 +382,9 @@ class DistributedIBNet:
 
     def _init_glorot_uniform(self):
         """Keras Dense defaults: kernel glorot_uniform, bias zeros (third-party behaviour; RNG stream is ours)."""
+        self._params.copy_(self._glorot_flat())
+
+    def _glorot_flat(self):
         g = torch.Generator(device="cpu")
         g.manual_seed(self.seed)
         flat = torch.zeros(self._P, dtype=torch.float32)
@@ -346,7 +395,31 @@ class DistributedIBNet:
             elif r > 0:
                 lim = math.sqrt(6.0 / (r + c))
                 flat[off:off + r * c] = (torch.rand(r * c, generator=g) * 2 - 1) * lim
-        self._params.copy_(flat)
+        return flat
+
+    def _set_output_encoder(self, nce):
+        """Lay the output encoder of ``nce`` (a losses.InfoNCE, or None) out after the model's variables: the flat buffer,
+        the optimizer slots and [grads || stats] grow or shrink, the model's weights and slots are kept, and the output
+        encoder starts from the glorot-uniform values a fresh model of the joint layout gets from ``seed``."""
+        old_spec = self._infonce.spec() if self._infonce is not None else None
+        new_spec = nce.spec() if nce is not None else None
+        self._infonce = nce
+        if old_spec == new_spec:
+            return
+        keep = self._var_off[self._n_model_vars] if self._n_model_vars < len(self._var_off) else self._P
+        self._release_handle()
+        self._graphs.clear(); self._graph_seen.clear()
+        self._query_layout()
+        with torch.cuda.device(self.device):
+            params = self._glorot_flat().to(self.device)
+            params[:keep] = self._params[:keep]
+            m, v = torch.zeros_like(params), torch.zeros_like(params)
+            m[:keep], v[:keep] = self._m[:keep], self._v[:keep]
+            self._params, self._m, self._v = params, m, v
+            self._gradstats = torch.zeros(self._P + self.number_features + 3, dtype=torch.float32, device=self.device)
+        self._staging = None
+        self.output_encoder = (_OutputEncoder(self, range(self._n_model_vars, len(self._var_off)))
+                               if nce is not None else None)
 
     # ------------------------------------------------------------------ Keras-like variable access
     @property
@@ -389,7 +462,17 @@ class DistributedIBNet:
         return t.contiguous()
 
     def _y_cols(self):
+        if self._infonce is not None:
+            return self._infonce.y_dimensionality
         return 0 if self._loss_kind == "sparse_ce_logits" else self.output_dimensionality
+
+    def _targets(self, y):
+        """y on the device as [n, _y_cols()]; an InfoNCE model checks the width (it sizes the output encoder)."""
+        if self._infonce is not None:
+            shape = tuple(y.shape)
+            if len(shape) not in (1, 2) or (shape[-1] if len(shape) == 2 else 1) != self._infonce.y_dimensionality:
+                raise ValueError(f"y has shape {shape}; the InfoNCE output encoder takes [n, {self._infonce.y_dimensionality}]")
+        return self._to_device(y, self._y_cols())
 
     # ------------------------------------------------------------------ compute entry points
     def _forward(self, x, y, eps, step, sample_offset, want_pred=True, want_emb=False, stats_out=None):
@@ -590,7 +673,7 @@ class DistributedIBNet:
         (flat gradient of task + beta*sum KL w.r.t. trainable_variables, statistics vector) as device tensors."""
         with torch.cuda.device(self.device):
             xd = self._to_device(x, sum(self.feature_dimensionalities))
-            yd = self._to_device(y, self._y_cols())
+            yd = self._targets(y)
             e = self._to_device(eps) if eps is not None else None
             self._backward(xd, yd, global_batch or max(xd.shape[0], 1), e, sample_offset, step)
             return self._gradstats[:self._P].clone(), self._gradstats[self._P:].clone()
@@ -695,15 +778,29 @@ class DistributedIBNet:
         new_opt = optimizers.get(optimizer)
         if new_opt is not self.optimizer:        # a fresh Keras optimizer has fresh slots and iteration count
             self._m.zero_(); self._v.zero_(); self._step_dev.zero_()
-        self.optimizer = new_opt
-        self._loss_kind = resolve_loss(loss)
-        self.compiled_metrics_names = []
+        kind = resolve_loss(loss)
+        if kind == "infonce":
+            if metrics:
+                raise ValueError("losses.InfoNCE has no accuracy: compile it without metrics (train.py:180-289 tracks none)")
+            if self.output_activation_fn is not None:
+                raise ValueError("losses.InfoNCE needs output_activation_fn=None: the prediction is the InfoNCE embedding "
+                                 "(train.py:117)")
+            self._check_single_rank()
         for m in (metrics or []):
             if m not in ("accuracy", "acc"):
                 raise ValueError(f"only metrics=['accuracy'] is implemented (reference data.py:67), got {m!r}")
-            self.compiled_metrics_names.append("accuracy")
+        self.optimizer = new_opt
+        self._loss_kind = kind
+        self._set_output_encoder(loss if kind == "infonce" else None)
+        self.compiled_metrics_names = ["accuracy" for _ in (metrics or [])]
         self._lr_host = None
         self._sync_lr()
+
+    def _check_single_rank(self):
+        if parallel.world_and_rank(self.process_group)[0] > 1:
+            raise NotImplementedError(
+                "losses.InfoNCE couples every row of the global batch; data-parallel InfoNCE needs an all-gather of both "
+                "embeddings and is not implemented: train it in a process group of one rank")
 
     def _sync_lr(self):
         """Device copy of optimizer.learning_rate (the step kernels read it from memory so that a schedule needs no re-capture);
@@ -728,7 +825,7 @@ class DistributedIBNet:
             world, rank = parallel.world_and_rank(self.process_group)
             host_x = not (isinstance(x, torch.Tensor) and x.is_cuda)
             if sync or not host_x:
-                xd, yd = self._to_device(x, D), self._to_device(y, self._y_cols())
+                xd, yd = self._to_device(x, D), self._targets(y)
                 n = xd.shape[0]
                 stats = self._train_step(xd, yd, global_batch=n * world, sample_offset=rank * n)
                 res = PendingBatchResult(self, stats.detach().clone() if not sync else stats, None, None)
@@ -787,18 +884,29 @@ class DistributedIBNet:
         loss, accuracy, KL{i}, beta and their val_ twins.
 
         Data-parallel: with torch.distributed initialised every rank passes the SAME x, y; each global batch is
-        split into contiguous row ranges per rank, so the result does not depend on the number of GPUs."""
+        split into contiguous row ranges per rank, so the result does not depend on the number of GPUs.
+
+        Compiled with ``losses.InfoNCE`` this runs train.py:180-289's InfoNCE training, which needs full, equal batches:
+        an epoch is floor(N / batch_size) batches of the epoch permutation (the remainder is dropped; N < batch_size is an
+        error) and validation takes floor(Nv / batch_size) + 1 full batches from the repeated validation permutation.
+        History keys are loss (= InfoNCE + beta * sum KL, so ``loss - beta * sum KL`` is the InfoNCE term), KL{i}, beta and
+        their val_ twins.  beta follows the annealing callback's on_epoch_begin, i.e. it is set before an epoch's first
+        step; the reference's custom loop assigns it after that step (train.py:245-250), one step late.  One process only."""
         if self.optimizer is None:
             raise RuntimeError("call compile() first")
         batch_size = 32 if batch_size is None else int(batch_size)
         world, rank = parallel.world_and_rank(self.process_group)
         D = sum(self.feature_dimensionalities)
+        nce = self._infonce is not None
+        if nce:
+            self._check_single_rank()
         with torch.cuda.device(self.device):
-            xd, yd = self._to_device(x, D), self._to_device(y, self._y_cols())
+            xd, yd = self._to_device(x, D), self._targets(y)
             N = xd.shape[0]
+            plan = infonce_epoch_batches(N, batch_size) if nce else None
             xv = yv = None
             if validation_data is not None:
-                xv, yv = self._to_device(validation_data[0], D), self._to_device(validation_data[1], self._y_cols())
+                xv, yv = self._to_device(validation_data[0], D), self._targets(validation_data[1])
             history = History()
             cbs = list(callbacks or []) + [history]
             for cb in cbs:
@@ -814,18 +922,25 @@ class DistributedIBNet:
                 if shuffle:
                     perm = self.epoch_permutation(epoch, N)
                 self._epoch_acc.zero_()
-                for b0 in range(0, N, batch_size):
-                    b1 = min(b0 + batch_size, N)
-                    lo, hi = parallel.shard_range(b1 - b0, rank, world)
-                    if shuffle:
-                        idx = perm[b0 + lo:b0 + hi]
-                        xb, yb = xd.index_select(0, idx), yd.index_select(0, idx)
-                    else:
-                        xb, yb = xd[b0 + lo:b0 + hi], yd[b0 + lo:b0 + hi]
-                    stats = self._train_step(xb, yb, global_batch=b1 - b0, sample_offset=lo)
-                    self._metrics_update(stats)
+                if nce:                                                      # full batches only, one process
+                    for b0, b1 in plan:
+                        idx = perm[b0:b1] if shuffle else slice(b0, b1)
+                        self._metrics_update(self._train_step(xd[idx], yd[idx], global_batch=b1 - b0))
+                else:
+                    for b0 in range(0, N, batch_size):
+                        b1 = min(b0 + batch_size, N)
+                        lo, hi = parallel.shard_range(b1 - b0, rank, world)
+                        if shuffle:
+                            idx = perm[b0 + lo:b0 + hi]
+                            xb, yb = xd.index_select(0, idx), yd.index_select(0, idx)
+                        else:
+                            xb, yb = xd[b0 + lo:b0 + hi], yd[b0 + lo:b0 + hi]
+                        stats = self._train_step(xb, yb, global_batch=b1 - b0, sample_offset=lo)
+                        self._metrics_update(stats)
                 logs = self._read_epoch_logs()
-                if xv is not None:
+                if xv is not None and nce:
+                    logs.update(self._evaluate_infonce_into_logs(xv, yv, batch_size, epoch, (2 ** 31 + epoch)))
+                elif xv is not None:
                     logs.update(self._evaluate_into_logs(xv, yv, batch_size, epoch, world, rank))
                 if verbose not in (False, 0) and rank == 0:          # 'auto' -> 1 like Keras outside notebooks
                     print(f"Epoch {epoch + 1}/{epochs} - " + " - ".join(
@@ -851,13 +966,39 @@ class DistributedIBNet:
             self._metrics_update(stats)
         return self._read_epoch_logs(prefix="val_")
 
+    def _evaluate_infonce_into_logs(self, xv, yv, batch_size, perm_key, step):
+        """InfoNCE validation (train.py:233-234, 264-270): floor(Nv / B) + 1 full batches drawn from the repeated validation
+        permutation (:func:`infonce_validation_batches`), noise keyed by (step, position in the repeated stream)."""
+        Nv = xv.shape[0]
+        pos = torch.from_numpy(infonce_validation_batches(Nv, batch_size)).to(self.device)
+        idx_all = self.validation_permutation(perm_key, Nv)[pos]
+        self._epoch_acc.zero_()
+        stats = torch.empty(self.number_features + 3, dtype=torch.float32, device=self.device)
+        for k in range(idx_all.shape[0]):
+            idx = idx_all[k]
+            self._forward(xv.index_select(0, idx), yv.index_select(0, idx), None, step, k * int(batch_size), want_pred=False,
+                          stats_out=stats)
+            self._metrics_update(stats)
+        return self._read_epoch_logs(prefix="val_")
+
+    def validation_permutation(self, key, n):
+        """The shuffle of the InfoNCE validation set for ``key`` (the epoch in fit; our RNG stream)."""
+        gen = torch.Generator(device=self.device)
+        gen.manual_seed((self.seed << 20) + (1 << 19) + int(key))
+        return torch.randperm(n, generator=gen, device=self.device)
+
     def evaluate(self, x, y, batch_size=32, return_dict=True, **_):
         with torch.cuda.device(self.device):
             world, rank = parallel.world_and_rank(self.process_group)
             D = sum(self.feature_dimensionalities)
             self._inference_calls += 1           # a fresh noise draw per evaluate() call
-            logs = self._evaluate_into_logs(self._to_device(x, D), self._to_device(y, self._y_cols()), int(batch_size),
-                                            (1 << 29) | (self._inference_calls & 0x1FFFFFFF), world, rank)
+            key = (1 << 29) | (self._inference_calls & 0x1FFFFFFF)
+            if self._infonce is not None:
+                self._check_single_rank()
+                logs = self._evaluate_infonce_into_logs(self._to_device(x, D), self._targets(y), int(batch_size), key, key)
+            else:
+                logs = self._evaluate_into_logs(self._to_device(x, D), self._to_device(y, self._y_cols()), int(batch_size),
+                                                key, world, rank)
         logs = {k[len("val_"):]: v for k, v in logs.items()}
         return logs if return_dict else [logs["loss"]] + [logs[m] for m in self.compiled_metrics_names]
 

@@ -33,7 +33,8 @@
 extern "C" {
 #endif
 
-#define DIB_ABI_VERSION 2
+/* 3 appends the InfoNCE fields to dib_config; dib_create still accepts abi_version 2 structs and reads only their prefix. */
+#define DIB_ABI_VERSION 3
 
 /* activation_fn strings accepted by tf.keras.layers.Dense in the reference's call sites
  * (train.py:37 'relu', nb-radial 'tanh', nb-bool LeakyReLU, None). */
@@ -55,7 +56,16 @@ enum dib_loss {
   /* tf.keras.losses.BinaryCrossentropy() on PROBABILITIES (from_logits=False, the Keras default; use with
    * output_activation_fn = sigmoid): -[y log(p~ + eps) + (1-y) log(1 - p~ + eps)], p~ = clip(p, eps, 1-eps), eps = 1e-7
    * (keras.backend.binary_crossentropy); the gradient is zero where p is clipped. */
-  DIB_LOSS_BCE_PROBS = 4
+  DIB_LOSS_BCE_PROBS = 4,
+  /* the InfoNCE path of train.py:180-289 (--infonce_loss; data.py:131's double pendulum): the model is trained together
+   * with an OUTPUT ENCODER for y (train.py:186-193: positional encoding as the model's, Dense(h, activation_fn) for every
+   * width of y_encoder_architecture, then a linear Dense(output_dimensionality)), whose variables follow the model's in the
+   * flat buffer (train.py:198).  y is the raw [n, y_dimensionality] target.  Task loss = the symmetric InfoNCE of
+   * train.py:203-213 over the [n, n] similarity matrix of (pred, output_encoder(y)), computed by streaming kernels whose
+   * memory is linear in n (the matrix is never stored).  It couples every row of the batch, so n is the whole batch:
+   * inv_global_batch scales only the beta*KL term.  Stats: task-loss slot = n * loss, accuracy slot 0.
+   * Needs abi_version >= 3, output_activation_fn = DIB_ACT_LINEAR and output_dimensionality <= 512. */
+  DIB_LOSS_INFONCE = 5
 };
 
 /* arithmetic of the dense contractions; everything else (PE, exp, KL, loss, Adam, reductions) is fp32 in every mode
@@ -103,6 +113,12 @@ typedef struct dib_config {
   float   dropout_rate;              /* nb-radial cell 5: tf.keras.layers.Dropout(rate) after every hidden Dense of the feature
                                         encoders, active in dib_train_step only (Keras training=True); masks from the Philox
                                         stream (oracle/philox.py :: dropout_keep).  Encoders then run on the unfused kernels. */
+  /* ---- abi_version >= 3: the output encoder and loss of DIB_LOSS_INFONCE (ignored for every other loss) ---- */
+  int32_t y_dimensionality;          /* width of y                                  train.py:186 */
+  int32_t number_y_encoder_layers;   /* len(y_encoder_architecture) */
+  const int32_t* y_encoder_architecture; /* hidden widths (--infonce_y_encoder_architecture)  train.py:189-190 */
+  int32_t infonce_similarity;        /* 0 'l2sq' | 1 'l2' | 2 'l1' | 3 'linf' | 4 'cosine' (dib_scaled_similarity kinds) */
+  float   infonce_temperature;       /* > 0                                          train.py:204 */
 } dib_config;
 
 typedef struct dib_model dib_model;
@@ -111,14 +127,16 @@ typedef struct dib_model dib_model;
 int dib_create(const dib_config* cfg, dib_model** out);
 void dib_destroy(dib_model* h);
 
-/* number of trainable parameters == sum over model.trainable_variables (train.py:198). */
+/* number of trainable parameters == sum over model.trainable_variables (train.py:198); with DIB_LOSS_INFONCE also the
+ * output encoder's (all_trainable_variables = model vars + output_encoder vars, train.py:198). */
 int64_t dib_param_count(const dib_model* h);
 
 /* For every variable v (in flat order) its offset and shape: offsets[v], rows[v] (fan-in, or 0 for a
  * bias), cols[v].  Pass NULLs to query the number of variables (return value, negative on error). */
 int dib_param_layout(const dib_model* h, int64_t* offsets, int32_t* rows, int32_t* cols, int32_t capacity);
 
-/* bytes of scratch the caller must provide to forward / train_step / encode calls.  The workspace pointer must be 256-byte
+/* bytes of scratch the caller must provide to forward / train_step / encode calls (linear in max_batch, DIB_LOSS_INFONCE
+ * included).  The workspace pointer must be 256-byte
  * aligned and `params` 16-byte aligned (checked; cudaMalloc / torch allocations are). */
 size_t dib_workspace_bytes(const dib_model* h);
 
@@ -127,7 +145,7 @@ int32_t dib_stats_count(const dib_model* h);
 
 /* DistributedIBNet.call (models.py:96-123) + compiled loss/metrics, no gradient: the validation pass of
  * Model.fit (train.py:157-166; noise is sampled in validation too, train.py:264-265).
- *   x [n, sum d_i]; y [n, out] (class index as float for sparse CE) or NULL; eps [n, F, E] or NULL ->
+ *   x [n, sum d_i]; y [n, out] (class index as float for sparse CE; DIB_LOSS_INFONCE: [n, y_dimensionality]) or NULL; eps [n, F, E] or NULL ->
  *   Philox4x32-10 keyed (seed, step, feature, sample_offset + row, dim), see oracle/philox.py;
  *   out_pred [n, out] or NULL; out_emb [n, F*E] or NULL; out_stats [dib_stats_count] (zeroed by the call). */
 int dib_forward(dib_model* h, const float* params, const float* x, const float* y, int64_t n,
@@ -142,7 +160,9 @@ int dib_encode_feature(dib_model* h, const float* params, int32_t feature, const
 /* One Keras train_step minus the optimizer: forward, loss = task + beta*sum_i KL_i (models.py:118),
  * reverse mode (GradientTape in Model.fit / nb-bool cell 6).  grads_flat [P] receives
  * d(loss)/d(params) * (n_local-sum scaled by inv_global_batch); out_stats as in dib_forward.
- * grads_flat and out_stats may be adjacent in one buffer so that one all-reduce covers both. */
+ * grads_flat and out_stats may be adjacent in one buffer so that one all-reduce covers both.
+ * DIB_LOSS_INFONCE: forward, output-encoder forward, streaming InfoNCE (d pred, d output-encoder output), the model's backward
+ * from d pred, the output encoder's backward into its slice of grads_flat -- one stream-ordered sequence, no host sync. */
 int dib_train_step(dib_model* h, const float* params, const float* x, const float* y, int64_t n,
                    const float* beta_dev, float inv_global_batch,
                    const float* eps, uint64_t seed, uint32_t step, uint64_t sample_offset,
@@ -187,6 +207,10 @@ int dib_optimizer_step(int32_t kind, float* params, const float* grads, float* s
  * Dense stack with the output activation, on the model's precision path (fp32 FMA / tf32 wgmma). */
 int dib_integration_forward(dib_model* h, const float* params, const float* emb, int64_t n, float* out_pred,
                             void* workspace, void* stream);
+
+/* output_encoder(y) of a DIB_LOSS_INFONCE model (train.py:186-193, deterministic): y [n, y_dimensionality] -> out [n, output_dimensionality]
+ * on the model's precision path (fp32 FMA / tf32 wgmma). */
+int dib_output_encoder_forward(dib_model* h, const float* params, const float* y, int64_t n, float* out, void* workspace, void* stream);
 
 /* models.PositionalEncoding.call (models.py:12-23) as a stand-alone call: x [n, d] ->
  * out [n, d * number_frequencies] = concat([x] + [sin(2^k x) for k = 1 .. number_frequencies-1], -1), block-major. */
