@@ -6,11 +6,12 @@ from ctypes import POINTER, c_char_p, c_float, c_int32, c_int64, c_size_t, c_uin
 
 from . import build as _build
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 ACTIVATIONS = {None: 0, "linear": 0, "relu": 1, "tanh": 2, "leaky_relu": 3, "sigmoid": 4, "elu": 5}
 LOSSES = {"bce_logits": 0, "sparse_ce_logits": 1, "mse": 2, "external": 3, "bce_probs": 4, "infonce": 5}
 ENCODER_KINDS = {"mlp": 0, "simple": 1}
+INTEGRATION_KINDS = {"mlp": 0, "set_transformer": 1}
 # 'fp16' / 'bf16': fused 16-bit-operand wgmma kernels (fp32 accumulate); 'tf32': tf32 wgmma GEMMs on fp32 storage;
 # 'fp32': exact CUDA-core FMA parity path.  See enum dib_precision in include/dib_b200.h.
 PRECISIONS = {"fp32": 0, "tf32": 1, "bf16": 2, "fp16": 3}
@@ -46,6 +47,16 @@ class DibConfig(ctypes.Structure):
         ("y_encoder_architecture", POINTER(c_int32)),
         ("infonce_similarity", c_int32),
         ("infonce_temperature", c_float),
+        # abi_version 4: the integration network (the set transformer of nb-particle cell 8)
+        ("integration_kind", c_int32),
+        ("set_size", c_int32),
+        ("number_attention_blocks", c_int32),
+        ("number_heads", c_int32),
+        ("key_dim", c_int32),
+        ("number_ff_layers", c_int32),
+        ("ff_architecture", POINTER(c_int32)),
+        ("ff_activation_fn", c_int32),
+        ("layer_norm_epsilon", c_float),
     ]
 
 

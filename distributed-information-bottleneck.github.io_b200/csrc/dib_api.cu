@@ -104,6 +104,25 @@ struct dib_model {
   std::vector<int> y_fwd, y_dgrad, y_wgrad;
   int* d_ycol_src = nullptr;
   int* d_ycol_freq = nullptr;
+  // DIB_INTEGRATION_SET_TRANSFORMER (nb-particle cell 8, dib_set_attn.cu): the encoder and the attention blocks run on
+  // n * Ls particle rows (maxB counts rows, maxSets sets), the head on the n set means
+  bool st = false;
+  int Ls = 1, nblk = 0, heads = 0, dkey = 0, hdk = 0, ff_act = 0;
+  float ln_eps = 1e-3f;
+  long long maxSets = 0;
+  std::vector<int> ff_arch;
+  struct StBlock {
+    long long Wq, bq, Wk, bk, Wv, bv, Wo, bo, g1, be1, g2, be2;
+    std::vector<long long> ffW, ffB;                  // [j]
+    Buf q, k, v, o, a, hh, xout;                      // Q, K, V, attention output (heads concatenated), its projection, LN1, LN2
+    std::vector<Buf> ff;                              // index 1..nff: output of FF layer j-1
+    long long lse = 0, mean1 = 0, rstd1 = 0, mean2 = 0, rstd2 = 0;
+    int qkv_fwd = -1, o_fwd = -1, qkv_dgrad = -1, o_dgrad = -1, qkv_wgrad = -1, o_wgrad = -1;
+    std::vector<int> ff_fwd, ff_dgrad, ff_wgrad;
+  };
+  std::vector<StBlock> blk;
+  Buf dq, dk, dv, d_o, dz1, dz2, dh_ff, dxq, dxk, dxv, pooled, d_pooled;   // backward scratch shared by the blocks
+  std::vector<Buf> d_ff;                             // index 1..nff
   // custom-step variants (SURVEY 8f3)
   float lv_off = 0.f, kl_exp = 1.f, kl_scale = 1.f;
   const uint32_t* step_dev = nullptr;  // optional device-resident addend of the Philox step word (dib_set_noise_step_device)
@@ -130,6 +149,8 @@ int int_fan_out(const dib_model* h, int j) { return j < h->Li ? h->int_arch[j] :
 bool infonce(const dib_model* h) { return h->loss == DIB_LOSS_INFONCE; }
 int y_fan_in(const dib_model* h, int j) { return j == 0 ? h->ydim * h->nfreq : h->y_arch[j - 1]; }
 int y_fan_out(const dib_model* h, int j) { return j < h->Ly ? h->y_arch[j] : h->out; }
+int ff_fan_in(const dib_model* h, int j) { return j == 0 ? h->E : h->ff_arch[j - 1]; }
+int nff(const dib_model* h) { return (int)h->ff_arch.size(); }
 
 // the one place the kernel path is chosen.  fused_ok / int16_ok are what dib_create found the shapes to support; the bits of
 // `unfused` (dib_debug_force_unfused) turn paths off: 1 = fused encoders, 2 = 16-bit integration network (it reads the fp16
@@ -183,11 +204,12 @@ void plan(dib_model* h) {
   h->emb = make_buf(c, B, h->F * h->E, 1);
   h->int_act.assign(h->Li + 1, Buf());
   h->d_int.assign(h->Li + 1, Buf());
-  for (int j = 1; j <= h->Li; ++j) h->int_act[j] = make_buf(c, B, h->int_arch[j - 1], 1);
-  h->pred = make_buf(c, B, h->out, 1);
+  const long long Bi = h->st ? h->maxSets : B;    // rows of the integration network (the set transformer's head: sets)
+  for (int j = 1; j <= h->Li; ++j) h->int_act[j] = make_buf(c, Bi, h->int_arch[j - 1], 1);
+  h->pred = make_buf(c, Bi, h->out, 1);
   // backward
-  h->d_pred = make_buf(c, B, h->out, 1);
-  for (int j = 1; j <= h->Li; ++j) h->d_int[j] = make_buf(c, B, h->int_arch[j - 1], 1);
+  h->d_pred = make_buf(c, Bi, h->out, 1);
+  for (int j = 1; j <= h->Li; ++j) h->d_int[j] = make_buf(c, Bi, h->int_arch[j - 1], 1);
   h->d_emb = make_buf(c, B, h->F * h->E, 1);
   h->d_out = make_buf(c, B, 2 * h->E, h->F);
   for (int j = 1; j <= h->L; ++j) h->d_enc[j] = make_buf(c, B, h->enc_arch[j - 1], h->F);
@@ -232,7 +254,92 @@ void plan(dib_model* h) {
     for (int j = 1; j <= h->Ly; ++j) h->d_yact[j] = make_buf(c, B, h->y_arch[j - 1], 1);
     h->nce_off = take(c, 3 * B);
   }
+  if (h->st) {                          // per block what its backward reads; one set of backward scratch for all blocks
+    const int E = h->E, nf = nff(h);
+    for (auto& b : h->blk) {
+      b.q = make_buf(c, B, h->hdk, 1); b.k = make_buf(c, B, h->hdk, 1); b.v = make_buf(c, B, h->hdk, 1);
+      b.o = make_buf(c, B, h->hdk, 1);
+      b.lse = take(c, h->maxSets * h->heads * h->Ls);
+      b.a = make_buf(c, B, E, 1);
+      b.mean1 = take(c, B); b.rstd1 = take(c, B);
+      b.hh = make_buf(c, B, E, 1);
+      b.ff.assign(nf + 1, Buf());
+      for (int j = 1; j <= nf; ++j) b.ff[j] = make_buf(c, B, h->ff_arch[j - 1], 1);
+      b.mean2 = take(c, B); b.rstd2 = take(c, B);
+      b.xout = make_buf(c, B, E, 1);
+    }
+    h->dq = make_buf(c, B, h->hdk, 1); h->dk = make_buf(c, B, h->hdk, 1); h->dv = make_buf(c, B, h->hdk, 1);
+    h->d_o = make_buf(c, B, h->hdk, 1);
+    h->dz1 = make_buf(c, B, E, 1); h->dz2 = make_buf(c, B, E, 1); h->dh_ff = make_buf(c, B, E, 1);
+    h->dxq = make_buf(c, B, E, 1); h->dxk = make_buf(c, B, E, 1); h->dxv = make_buf(c, B, E, 1);
+    h->d_ff.assign(nf + 1, Buf());
+    for (int j = 1; j <= nf; ++j) h->d_ff[j] = make_buf(c, B, h->ff_arch[j - 1], 1);
+    h->pooled = make_buf(c, h->maxSets, E, 1);
+    h->d_pooled = make_buf(c, h->maxSets, E, 1);
+  }
   h->ws_floats = c;
+}
+
+// the dense layers of the attention blocks, all on n * Ls particle rows: Q / K / V as one group of three problems (same
+// input, kernels [E, h*dk]), the output projection [h*dk, E], the FF stack; each in the three GEMM modes
+void build_set_problems(dib_model* h, std::vector<DibGemmProblem>& v) {
+  auto zero = [] { DibGemmProblem p; memset(&p, 0, sizeof(p)); return p; };
+  const int E = h->E, hdk = h->hdk, nf = nff(h);
+  auto prob = [&](const Buf& a, long long b_off, int ldb, long long c_off, int ldc, long long x_off, int ldx, int T, int C, int R,
+                  int act) {
+    DibGemmProblem p = zero();
+    p.a_off = a.off; p.lda = a.ld; p.b_off = b_off; p.ldb = ldb; p.c_off = c_off; p.ldc = ldc; p.x_off = x_off; p.ldx = ldx;
+    p.T = T; p.C = C; p.R = R; p.act = act;
+    v.push_back(p);
+  };
+  for (int b = 0; b < h->nblk; ++b) {
+    dib_model::StBlock& k = h->blk[b];
+    const Buf& x = b == 0 ? h->emb : h->blk[b - 1].xout;
+    const long long W[3] = {k.Wq, k.Wk, k.Wv}, bias[3] = {k.bq, k.bk, k.bv};
+    const Buf* qkv[3] = {&k.q, &k.k, &k.v};
+    const Buf* dqkv[3] = {&h->dq, &h->dk, &h->dv};
+    const Buf* dx[3] = {&h->dxq, &h->dxk, &h->dxv};
+    k.qkv_fwd = (int)v.size();
+    for (int i = 0; i < 3; ++i) prob(x, W[i], hdk, qkv[i]->off, qkv[i]->ld, bias[i], 0, E, hdk, 0, DIB_ACT_LINEAR);
+    k.o_fwd = (int)v.size();
+    prob(k.o, k.Wo, E, k.a.off, k.a.ld, k.bo, 0, hdk, E, 0, DIB_ACT_LINEAR);
+    k.ff_fwd.assign(nf, -1); k.ff_dgrad.assign(nf, -1); k.ff_wgrad.assign(nf, -1);
+    for (int j = 0; j < nf; ++j) {
+      k.ff_fwd[j] = (int)v.size();
+      prob(j == 0 ? k.hh : k.ff[j], k.ffW[j], h->ff_arch[j], k.ff[j + 1].off, k.ff[j + 1].ld, k.ffB[j], 0, ff_fan_in(h, j), h->ff_arch[j], 0,
+           h->ff_act);
+    }
+    for (int j = 0; j < nf; ++j) {       // d (pre-activation of FF layer j) -> d (its input); layer 0's input is H (no activation)
+      k.ff_dgrad[j] = (int)v.size();
+      const Buf& o = j == 0 ? h->dh_ff : h->d_ff[j];
+      prob(h->d_ff[j + 1], k.ffW[j], h->ff_arch[j], o.off, o.ld, j == 0 ? 0 : k.ff[j].off, j == 0 ? 0 : k.ff[j].ld, h->ff_arch[j],
+           ff_fan_in(h, j), 0, j == 0 ? DIB_ACT_LINEAR : h->ff_act);
+      k.ff_wgrad[j] = (int)v.size();
+      DibGemmProblem p = zero();
+      const Buf& a = j == 0 ? k.hh : k.ff[j];
+      p.a_off = a.off; p.lda = a.ld; p.b_off = h->d_ff[j + 1].off; p.ldb = h->d_ff[j + 1].ld;
+      p.c_off = k.ffW[j]; p.ldc = h->ff_arch[j]; p.x_off = k.ffB[j]; p.R = ff_fan_in(h, j); p.C = h->ff_arch[j];
+      v.push_back(p);
+    }
+    k.o_dgrad = (int)v.size();
+    prob(h->dz1, k.Wo, E, h->d_o.off, h->d_o.ld, 0, 0, E, hdk, 0, DIB_ACT_LINEAR);
+    k.o_wgrad = (int)v.size();
+    {
+      DibGemmProblem p = zero();
+      p.a_off = k.o.off; p.lda = k.o.ld; p.b_off = h->dz1.off; p.ldb = h->dz1.ld;
+      p.c_off = k.Wo; p.ldc = E; p.x_off = k.bo; p.R = hdk; p.C = E;
+      v.push_back(p);
+    }
+    k.qkv_dgrad = (int)v.size();
+    for (int i = 0; i < 3; ++i) prob(*dqkv[i], W[i], hdk, dx[i]->off, dx[i]->ld, 0, 0, hdk, E, 0, DIB_ACT_LINEAR);
+    k.qkv_wgrad = (int)v.size();
+    for (int i = 0; i < 3; ++i) {
+      DibGemmProblem p = zero();
+      p.a_off = x.off; p.lda = x.ld; p.b_off = dqkv[i]->off; p.ldb = dqkv[i]->ld;
+      p.c_off = W[i]; p.ldc = hdk; p.x_off = bias[i]; p.R = E; p.C = hdk;
+      v.push_back(p);
+    }
+  }
 }
 
 void build_problems(dib_model* h, std::vector<DibGemmProblem>& v) {
@@ -290,8 +397,9 @@ void build_problems(dib_model* h, std::vector<DibGemmProblem>& v) {
       v.push_back(p);
     }
   }
+  const Buf& int_in = h->st ? h->pooled : h->emb;     // the set transformer's head reads the set means
   auto intA = [&](int j, long long& off, int& ld) {
-    if (j == 0) { off = h->emb.off; ld = h->emb.ld; } else { off = h->int_act[j].off; ld = h->int_act[j].ld; }
+    if (j == 0) { off = int_in.off; ld = int_in.ld; } else { off = h->int_act[j].off; ld = h->int_act[j].ld; }
   };
   auto intDZ = [&](int j, long long& off, int& ld) {
     const Buf& b = j == Li ? h->d_pred : h->d_int[j + 1];
@@ -313,7 +421,7 @@ void build_problems(dib_model* h, std::vector<DibGemmProblem>& v) {
     DibGemmProblem p = zero();
     intDZ(j, p.a_off, p.lda);
     p.b_off = h->intW[j]; p.ldb = int_fan_out(h, j);
-    const Buf& o = j == 0 ? h->d_emb : h->d_int[j];
+    const Buf& o = j == 0 ? (h->st ? h->d_pooled : h->d_emb) : h->d_int[j];
     p.c_off = o.off; p.ldc = o.ld;
     if (j > 0) { p.x_off = h->int_act[j].off; p.ldx = h->int_act[j].ld; p.act = h->act; }
     else { p.act = DIB_ACT_LINEAR; }
@@ -330,6 +438,7 @@ void build_problems(dib_model* h, std::vector<DibGemmProblem>& v) {
     p.R = int_fan_in(h, j); p.C = int_fan_out(h, j);
     v.push_back(p);
   }
+  if (h->st) build_set_problems(h, v);
   if (!infonce(h)) return;
   // the output encoder: the same three modes on its own buffers (train.py:186-193)
   const int Ly = h->Ly;
@@ -429,6 +538,13 @@ int check_call(const dib_model* h, const void* params, const void* x, int64_t n,
   if (n < 0 || n > h->maxB) return fail("n = " + std::to_string(n) + " exceeds config.max_batch = " + std::to_string(h->maxB));
   if (reinterpret_cast<uintptr_t>(ws) & 255) return fail("workspace must be 256-byte aligned");
   if (reinterpret_cast<uintptr_t>(params) & 15) return fail("params must be 16-byte aligned");
+  return 0;
+}
+
+// calls whose n counts sets on a set-transformer handle (check_call bounds particle rows)
+int check_sets(const dib_model* h, int64_t n) {
+  if (h->st && n > h->maxSets)
+    return fail("n = " + std::to_string(n) + " sets exceeds config.max_batch = " + std::to_string(h->maxSets));
   return 0;
 }
 
@@ -818,6 +934,156 @@ int backward_output_encoder(const Ctx& c, const Split& sp, float* grads_flat) {
   return 0;
 }
 
+// ---- DIB_INTEGRATION_SET_TRANSFORMER: c.n = particle rows (sets * Ls) -----------------------------------------------
+DibAttnArgs attn_args(const Ctx& c, const dib_model::StBlock& k) {
+  const dib_model* h = c.h;
+  DibAttnArgs a;
+  a.q = c.ws + k.q.off; a.k = c.ws + k.k.off; a.v = c.ws + k.v.off; a.ld = k.q.ld;
+  a.o = c.ws + k.o.off; a.lse = c.ws + k.lse;
+  a.sets = c.n / h->Ls; a.heads = h->heads; a.L = h->Ls; a.dk = h->dkey;
+  a.round_out = is_tc(h) ? 1 : 0;
+  a.dout = c.ws + h->d_o.off; a.dq = c.ws + h->dq.off; a.dk_ = c.ws + h->dk.off; a.dv = c.ws + h->dv.off;
+  return a;
+}
+
+DibLayerNorm ln_args(const Ctx& c, const Buf& a, const Buf& b, long long gamma, long long beta, const Buf& y, long long mean,
+                     long long rstd) {
+  DibLayerNorm l;
+  l.a = c.ws + a.off; l.b = c.ws + b.off; l.ld = a.ld; l.rows = c.n; l.E = c.h->E;
+  l.gamma = c.params + gamma; l.beta = c.params + beta; l.epsilon = c.h->ln_eps;
+  l.y = c.ws + y.off; l.mean = c.ws + mean; l.rstd = c.ws + rstd;
+  l.round_out = is_tc(c.h) ? 1 : 0;
+  return l;
+}
+
+// the attention blocks from the embeddings in h->emb, then the mean over each set's particles into h->pooled
+int forward_set_blocks(const Ctx& c) {
+  dib_model* h = c.h;
+  for (int b = 0; b < h->nblk; ++b) {
+    const dib_model::StBlock& k = h->blk[b];
+    const Buf& x = b == 0 ? h->emb : h->blk[b - 1].xout;
+    prof_begin(c, "st_qkv_fwd_b", b);
+    if (gemm(c, DIB_GEMM_FWD, k.qkv_fwd, 3, h->hdk, 0, 1, 0)) return 1;
+    prof_end(c);
+    prof_begin(c, "st_attn_fwd_b", b);
+    DIB_CUDA_OK(dib_launch_attn_fwd(attn_args(c, k), c.st));
+    prof_end(c);
+    prof_begin(c, "st_out_proj_ln1_fwd_b", b);
+    if (gemm(c, DIB_GEMM_FWD, k.o_fwd, 1, h->E, 0, 1, 0)) return 1;
+    DIB_CUDA_OK(dib_launch_ln_fwd(ln_args(c, x, k.a, k.g1, k.be1, k.hh, k.mean1, k.rstd1), c.st));
+    prof_end(c);
+    prof_begin(c, "st_ff_ln2_fwd_b", b);
+    for (int j = 0; j < nff(h); ++j)
+      if (gemm(c, DIB_GEMM_FWD, k.ff_fwd[j], 1, h->ff_arch[j], 0, 1, 0)) return 1;
+    DIB_CUDA_OK(dib_launch_ln_fwd(ln_args(c, k.hh, k.ff[nff(h)], k.g2, k.be2, k.xout, k.mean2, k.rstd2), c.st));
+    prof_end(c);
+  }
+  const Buf& last = h->nblk ? h->blk[h->nblk - 1].xout : h->emb;
+  prof_begin(c, "st_pool_fwd");
+  DIB_CUDA_OK(dib_launch_pool_fwd(c.ws + last.off, last.ld, h->E, h->Ls, c.n / h->Ls, c.ws + h->pooled.off, h->pooled.ld,
+                                  is_tc(h) ? 1 : 0, c.st));
+  prof_end(c);
+  return 0;
+}
+
+// the blocks' backward from d pooled (the head's DGRAD output) down to d emb, the blocks' weight-gradient and LayerNorm partials
+// in rows [0, sp.nsplit) of the split table
+int backward_set_blocks(const Ctx& c, const Split& sp) {
+  dib_model* h = c.h;
+  const int nf = nff(h);
+  float* part = c.ws + h->part_off;
+  auto ln_bwd = [&](const DibLayerNorm& l, const float* const dy[4], const float* dy_pool, const Buf& d_res, const Buf* d_branch,
+                    long long g, long long be) {
+    DibLayerNormBwd b;
+    for (int q = 0; q < 4; ++q) b.dy[q] = dy[q];
+    b.dy_pool = dy_pool; b.pool_rows = h->Ls; b.pool_scale = 1.f / (float)h->Ls;
+    b.d_res = c.ws + d_res.off; b.d_branch = d_branch ? c.ws + d_branch->off : nullptr; b.branch_act = h->ff_act; b.alpha = h->alpha;
+    b.part = part; b.split_stride = h->Pp; b.gamma_off = g; b.beta_off = be; b.nsplit = sp.nsplit; b.rows_per_split = sp.rps;
+    return dib_launch_ln_bwd(l, b, c.st);
+  };
+  for (int b = h->nblk - 1; b >= 0; --b) {
+    const dib_model::StBlock& k = h->blk[b];
+    const Buf& x = b == 0 ? h->emb : h->blk[b - 1].xout;
+    prof_begin(c, "st_ln2_ff_bwd_b", b);
+    {
+      const bool last = b == h->nblk - 1;
+      const float* dy[4] = {last ? nullptr : c.ws + h->dz1.off, last ? nullptr : c.ws + h->dxq.off, last ? nullptr : c.ws + h->dxk.off,
+                            last ? nullptr : c.ws + h->dxv.off};
+      DIB_CUDA_OK(ln_bwd(ln_args(c, k.hh, k.ff[nf], k.g2, k.be2, k.xout, k.mean2, k.rstd2), dy, last ? c.ws + h->d_pooled.off : nullptr,
+                         h->dz2, &h->d_ff[nf], k.g2, k.be2));
+    }
+    for (int j = nf - 1; j >= 0; --j) {
+      if (gemm(c, DIB_GEMM_WGRAD, k.ff_wgrad[j], 1, h->ff_arch[j], ff_fan_in(h, j), sp.nsplit, (int)sp.rps)) return 1;
+      if (gemm(c, DIB_GEMM_DGRAD, k.ff_dgrad[j], 1, ff_fan_in(h, j), 0, 1, 0)) return 1;
+    }
+    prof_end(c);
+    prof_begin(c, "st_ln1_out_proj_bwd_b", b);
+    {
+      const float* dy[4] = {c.ws + h->dz2.off, c.ws + h->dh_ff.off, nullptr, nullptr};
+      DIB_CUDA_OK(ln_bwd(ln_args(c, x, k.a, k.g1, k.be1, k.hh, k.mean1, k.rstd1), dy, nullptr, h->dz1, nullptr, k.g1, k.be1));
+    }
+    if (gemm(c, DIB_GEMM_WGRAD, k.o_wgrad, 1, h->E, h->hdk, sp.nsplit, (int)sp.rps)) return 1;
+    if (gemm(c, DIB_GEMM_DGRAD, k.o_dgrad, 1, h->hdk, 0, 1, 0)) return 1;
+    prof_end(c);
+    prof_begin(c, "st_attn_bwd_b", b);
+    DIB_CUDA_OK(dib_launch_attn_bwd(attn_args(c, k), c.st));
+    prof_end(c);
+    prof_begin(c, "st_qkv_bwd_b", b);
+    if (gemm(c, DIB_GEMM_WGRAD, k.qkv_wgrad, 3, h->hdk, h->E, sp.nsplit, (int)sp.rps)) return 1;
+    if (gemm(c, DIB_GEMM_DGRAD, k.qkv_dgrad, 3, h->E, 0, 1, 0)) return 1;
+    prof_end(c);
+  }
+  // d emb = block 0's residual-path gradient + its Q / K / V input gradients (dib_create requires at least one block)
+  DibSumRows s;
+  s.dst = c.ws + h->d_emb.off; s.count = (long long)c.n * h->d_emb.ld;
+  s.src[0] = c.ws + h->dz1.off; s.src[1] = c.ws + h->dxq.off; s.src[2] = c.ws + h->dxk.off; s.src[3] = c.ws + h->dxv.off;
+  prof_begin(c, "st_d_emb");
+  DIB_CUDA_OK(dib_launch_sum_rows(s, c.st));
+  prof_end(c);
+  return 0;
+}
+
+// dib_forward / dib_train_step's forward for the set transformer: cs.n counts sets
+int run_forward_set(const Ctx& cs, const float* x, const float* y, const NoiseKey& nk, float inv_batch, float* user_pred,
+                    float* user_emb, float* out_stats) {
+  dib_model* h = cs.h;
+  Ctx c = cs;
+  c.n = cs.n * h->Ls;
+  NoiseKey nr = nk;
+  nr.sample_offset = nk.sample_offset * (uint64_t)h->Ls;     // noise keyed by the global particle row
+  if (is_tc(h)) {
+    prof_begin(c, "weights_tf32_shadow");
+    DIB_CUDA_OK(dib_launch_round_copy(c.params, c.ws + h->wshadow_off, h->P, c.st));
+    prof_end(c);
+  }
+  int nblk_kl = 0;
+  if (forward_encoders(c, x, nr, user_emb, false, &nblk_kl)) return 1;
+  if (forward_set_blocks(c)) return 1;
+  return forward_integration(cs, y, inv_batch, nk.training, user_pred, out_stats, nblk_kl);
+}
+
+int train_step_set(const Ctx& cs, const float* x, const float* y, const NoiseKey& nk, const float* beta_dev, float inv_global_batch,
+                   float* grads_flat, float* out_stats) {
+  dib_model* h = cs.h;
+  if (run_forward_set(cs, x, y, nk, inv_global_batch, nullptr, nullptr, out_stats)) return 1;
+  const float* beta_w = nullptr;
+  if (ib_weight(cs, beta_dev, out_stats, inv_global_batch, &beta_w)) return 1;
+  std::vector<DibReduceSeg> segs;          // unused: the head runs on the per-layer GEMM route, which reduces its own range
+  if (backward_integration(cs, inv_global_batch, batch_split(cs.n), grads_flat, &segs)) return 1;
+  Ctx c = cs;
+  c.n = cs.n * h->Ls;
+  NoiseKey nr = nk;
+  nr.sample_offset = nk.sample_offset * (uint64_t)h->Ls;
+  const Split sp = batch_split(c.n);
+  if (backward_set_blocks(c, sp)) return 1;
+  int nrows = 0;
+  if (backward_encoders(c, x, nr, c.ws + h->d_emb.off, h->d_emb.ld, nullptr, beta_w, inv_global_batch, sp, &nrows)) return 1;
+  prof_begin(c, "enc_blocks_split_reduce");   // the encoder and the blocks: [0, first head parameter)
+  DIB_CUDA_OK(dib_launch_reduce_partials(c.ws + h->part_off, h->Pp, nrows, h->intW[0], grads_flat, c.st));
+  prof_end(c);
+  return 0;
+}
+
 }  // namespace
 
 // =================================================================================================
@@ -890,7 +1156,7 @@ int dib_debug_gemm_tc(int32_t mode, const float* A, int32_t lda, const float* B,
 const char* dib_last_error(void) { return g_last_error.c_str(); }
 
 const char* dib_build_info(void) {
-  return "dib_b200 abi=3 arch=sm_90a paths=fp32-simt,tf32-wgmma,fp16-fused-wgmma,bf16-fused-wgmma";
+  return "dib_b200 abi=4 arch=sm_90a paths=fp32-simt,tf32-wgmma,fp16-fused-wgmma,bf16-fused-wgmma";
 }
 
 int32_t dib_model_info(const dib_model* h, char* out, size_t out_bytes) {
@@ -906,6 +1172,8 @@ int32_t dib_model_info(const dib_model* h, char* out, size_t out_bytes) {
     s += fused ? std::string(" operands=") + (h->precision == DIB_PREC_BF16 ? "bf16" : "fp16") : std::string(" operands=tf32");
     s += " accumulate=fp32";
   }
+  if (h->st)
+    s += std::string(" set_transformer=attention-simt-fp32,layernorm-simt-fp32,dense-") + (is_tc(h) ? "wgmma-tf32" : "simt-fp32");
   if (infonce(h))
     s += std::string(" output_encoder=") + (is_tc(h) ? "wgmma-tf32" : "simt-fp32") + " loss=infonce-stream-fp32";
   const size_t k = s.size() < out_bytes - 1 ? s.size() : out_bytes - 1;
@@ -917,7 +1185,29 @@ int dib_create(const dib_config* cfg, dib_model** out) {
   if (!cfg || !out) return fail("dib_create: null argument");
   *out = nullptr;
   // an abi_version 2 struct ends before the InfoNCE fields: read only its prefix
-  if (cfg->abi_version != 2 && cfg->abi_version != DIB_ABI_VERSION) return fail("dib_create: abi_version mismatch");
+  if (cfg->abi_version < 2 || cfg->abi_version > DIB_ABI_VERSION) return fail("dib_create: abi_version mismatch");
+  const int kind = cfg->abi_version >= 4 ? cfg->integration_kind : DIB_INTEGRATION_MLP;
+  if (kind != DIB_INTEGRATION_MLP && kind != DIB_INTEGRATION_SET_TRANSFORMER) return fail("dib_create: unknown integration_kind");
+  if (kind == DIB_INTEGRATION_SET_TRANSFORMER) {
+    const int E = cfg->feature_embedding_dimension;
+    if (cfg->set_size < 1 || cfg->set_size > 64) return fail("dib_create: set transformer needs set_size in [1, 64]");
+    if (cfg->number_features != 1) return fail("dib_create: set transformer needs number_features == 1 (one shared particle encoder)");
+    if (cfg->number_attention_blocks < 1 || cfg->number_heads < 1 || cfg->key_dim < 1 || cfg->key_dim > 128)
+      return fail("dib_create: set transformer needs >= 1 attention block, >= 1 head and key_dim in [1, 128]");
+    if (((long long)cfg->number_heads * cfg->key_dim) % 4 || E % 4 || E > 128)
+      return fail("dib_create: set transformer needs number_heads * key_dim and E multiples of 4 and E <= 128");
+    if (cfg->number_ff_layers < 1 || !cfg->ff_architecture || cfg->ff_architecture[cfg->number_ff_layers - 1] != E)
+      return fail("dib_create: set transformer needs an FF stack whose last width equals E (the residual adds it to the input)");
+    for (int j = 0; j < cfg->number_ff_layers; ++j)
+      if (cfg->ff_architecture[j] < 1) return fail("dib_create: FF width < 1");
+    if (cfg->ff_activation_fn < 0 || cfg->ff_activation_fn > DIB_ACT_ELU) return fail("dib_create: unknown FF activation");
+    if (cfg->loss == DIB_LOSS_SPARSE_CE_LOGITS || cfg->loss == DIB_LOSS_INFONCE)
+      return fail("dib_create: set transformer supports BCE (logits or probabilities), MSE and the external loss");
+    if (cfg->dropout_rate != 0.f) return fail("dib_create: set transformer has no dropout");
+    if (cfg->max_batch > 65535 || cfg->max_batch * cfg->set_size > 0x7fffffffll)
+      return fail("dib_create: set transformer needs max_batch <= 65535 sets");
+    if (!(cfg->layer_norm_epsilon >= 0.f)) return fail("dib_create: layer_norm_epsilon must be >= 0");
+  }
   if (cfg->number_features < 1 || cfg->feature_embedding_dimension < 1 || cfg->output_dimensionality < 1 ||
       cfg->max_batch < 1 || cfg->number_encoder_layers < 0 || cfg->number_integration_layers < 0)
     return fail("dib_create: invalid sizes");
@@ -955,6 +1245,17 @@ int dib_create(const dib_config* cfg, dib_model** out) {
     h->ydim = cfg->y_dimensionality; h->Ly = cfg->number_y_encoder_layers;
     h->y_arch.assign(cfg->y_encoder_architecture, cfg->y_encoder_architecture + h->Ly);
     h->sim_kind = cfg->infonce_similarity; h->temperature = cfg->infonce_temperature;
+  }
+  if (kind == DIB_INTEGRATION_SET_TRANSFORMER) {
+    h->st = true;
+    h->Ls = cfg->set_size; h->nblk = cfg->number_attention_blocks; h->heads = cfg->number_heads; h->dkey = cfg->key_dim;
+    h->hdk = h->heads * h->dkey;
+    h->ff_arch.assign(cfg->ff_architecture, cfg->ff_architecture + cfg->number_ff_layers);
+    h->ff_act = cfg->ff_activation_fn;
+    h->ln_eps = cfg->layer_norm_epsilon == 0.f ? 1e-3f : cfg->layer_norm_epsilon;
+    h->maxSets = cfg->max_batch;
+    h->maxB = cfg->max_batch * h->Ls;      // encoder and block buffers hold particle rows
+    h->blk.assign(h->nblk, dib_model::StBlock());
   }
   if (!(h->drop >= 0.f && h->drop < 1.f)) { delete h; return fail("dib_create: dropout_rate must be in [0, 1)"); }
   if (cfg->encoder_kind != DIB_ENCODER_MLP && cfg->encoder_kind != DIB_ENCODER_SIMPLE) { delete h; return fail("dib_create: unknown encoder_kind"); }
@@ -1010,6 +1311,15 @@ int dib_create(const dib_config* cfg, dib_model** out) {
       h->encB[f].push_back(add_var(0, enc_fan_out(h, j)));
     }
   }
+  for (auto& k : h->blk) {                 // Keras functional order inside each attention block
+    k.Wq = add_var(h->E, h->hdk); k.bq = add_var(0, h->hdk);
+    k.Wk = add_var(h->E, h->hdk); k.bk = add_var(0, h->hdk);
+    k.Wv = add_var(h->E, h->hdk); k.bv = add_var(0, h->hdk);
+    k.Wo = add_var(h->hdk, h->E); k.bo = add_var(0, h->E);
+    k.g1 = add_var(0, h->E); k.be1 = add_var(0, h->E);
+    for (int j = 0; j < nff(h); ++j) { k.ffW.push_back(add_var(ff_fan_in(h, j), h->ff_arch[j])); k.ffB.push_back(add_var(0, h->ff_arch[j])); }
+    k.g2 = add_var(0, h->E); k.be2 = add_var(0, h->E);
+  }
   for (int j = 0; j <= h->Li; ++j) {
     h->intW.push_back(add_var(int_fan_in(h, j), int_fan_out(h, j)));
     h->intB.push_back(add_var(0, int_fan_out(h, j)));
@@ -1047,6 +1357,7 @@ int dib_create(const dib_config* cfg, dib_model** out) {
     if (e == cudaSuccess) e = cudaMemcpy(h->d_ycol_src, ycol_src.data(), ycol_src.size() * sizeof(int), cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMemcpy(h->d_ycol_freq, ycol_freq.data(), ycol_freq.size() * sizeof(int), cudaMemcpyHostToDevice);
   }
+  if (e == cudaSuccess && h->st) e = dib_attn_prepare();
   if (e != cudaSuccess) {
     std::string msg = std::string("dib_create: CUDA error: ") + cudaGetErrorString(e);
     dib_destroy(h);
@@ -1054,7 +1365,7 @@ int dib_create(const dib_config* cfg, dib_model** out) {
   }
   // ---- fused encoder kernels: two hidden layers of 128, E = 32, first-layer fan-in (+ bias column) <= 16
   {
-    bool ok = want16(h) && h->drop == 0.f && h->L == 2 && h->enc_arch[0] == 128 && h->enc_arch[1] == 128 && h->E == 32;
+    bool ok = want16(h) && !h->st && h->drop == 0.f && h->L == 2 && h->enc_arch[0] == 128 && h->enc_arch[1] == 128 && h->E == 32;
     for (int f = 0; ok && f < h->F; ++f) ok = h->w_in[f] + 1 <= 16;
     if (ok) {
       const int F = h->F;
@@ -1124,10 +1435,11 @@ int dib_forward(dib_model* h, const float* params, const float* x, const float* 
                 const float* eps, uint64_t seed, uint32_t step, uint64_t sample_offset, float* out_pred, float* out_emb,
                 float* out_stats, void* workspace, void* stream) {
   (void)beta_dev;
-  if (check_call(h, params, x, n, workspace)) return 1;
+  if (check_call(h, params, x, n, workspace) || check_sets(h, n)) return 1;
   if (!out_stats) return fail("dib_forward: out_stats is required");
   Ctx c{h, params, static_cast<float*>(workspace), static_cast<cudaStream_t>(stream), (int)n};
   if (n == 0) { DIB_CUDA_OK(cudaMemsetAsync(out_stats, 0, sizeof(float) * (h->F + 3), c.st)); return 0; }
+  if (h->st) return run_forward_set(c, x, y, NoiseKey{eps, seed, step, sample_offset, false}, 0.f, out_pred, out_emb, out_stats);
   return run_forward(c, x, y, NoiseKey{eps, seed, step, sample_offset, false}, 0.f, out_pred, out_emb, out_stats);
 }
 
@@ -1164,7 +1476,7 @@ int dib_encode_feature(dib_model* h, const float* params, int32_t feature, const
 int dib_train_step(dib_model* h, const float* params, const float* x, const float* y, int64_t n, const float* beta_dev,
                    float inv_global_batch, const float* eps, uint64_t seed, uint32_t step, uint64_t sample_offset,
                    float* grads_flat, float* out_stats, void* workspace, void* stream) {
-  if (check_call(h, params, x, n, workspace)) return 1;
+  if (check_call(h, params, x, n, workspace) || check_sets(h, n)) return 1;
   if ((!y && n > 0) || !beta_dev || !grads_flat || !out_stats)
     return fail("dib_train_step: y, beta_dev, grads_flat and out_stats are required");
   Ctx c{h, params, static_cast<float*>(workspace), static_cast<cudaStream_t>(stream), (int)n};
@@ -1175,6 +1487,7 @@ int dib_train_step(dib_model* h, const float* params, const float* x, const floa
     return 0;
   }
   const NoiseKey nk{eps, seed, step, sample_offset, true};
+  if (h->st) return train_step_set(c, x, y, nk, beta_dev, inv_global_batch, grads_flat, out_stats);
   if (run_forward(c, x, y, nk, inv_global_batch, nullptr, nullptr, out_stats)) return 1;
   const float* beta_w = nullptr;           // weight of the per-sample KL gradients in the encoder backward
   if (ib_weight(c, beta_dev, out_stats, inv_global_batch, &beta_w)) return 1;
@@ -1229,14 +1542,22 @@ int dib_optimizer_step(int32_t kind, float* params, const float* grads, float* s
 
 int dib_integration_forward(dib_model* h, const float* params, const float* emb, int64_t n, float* out_pred,
                             void* workspace, void* stream) {
-  if (check_call(h, params, emb, n, workspace)) return 1;
+  if (check_call(h, params, emb, n, workspace) || check_sets(h, n)) return 1;
   if (!out_pred) return fail("dib_integration_forward: null output");
   if (n == 0) return 0;
   Ctx c{h, params, static_cast<float*>(workspace), static_cast<cudaStream_t>(stream), (int)n};
   const int FE = h->F * h->E;
   if (is_tc(h)) DIB_CUDA_OK(dib_launch_round_copy(c.params, c.ws + h->wshadow_off, h->P, c.st));
-  DIB_CUDA_OK(dib_launch_copy2d(emb, FE, c.ws + h->emb.off, h->emb.ld, FE, n, c.st));
-  if (h->emb.ld > FE)          // zero the padded operand columns
+  if (h->st) {                 // emb [n, Ls, E] (E is a multiple of 4: no padded columns) through the blocks and the mean
+    Ctx cr = c;
+    cr.n = (int)n * h->Ls;
+    if (is_tc(h)) DIB_CUDA_OK(dib_launch_round_copy(emb, c.ws + h->emb.off, (int64_t)cr.n * FE, c.st));
+    else DIB_CUDA_OK(dib_launch_copy2d(emb, FE, c.ws + h->emb.off, h->emb.ld, FE, cr.n, c.st));
+    if (forward_set_blocks(cr)) return 1;
+  } else {
+    DIB_CUDA_OK(dib_launch_copy2d(emb, FE, c.ws + h->emb.off, h->emb.ld, FE, n, c.st));
+  }
+  if (!h->st && h->emb.ld > FE)          // zero the padded operand columns
     DIB_CUDA_OK(cudaMemset2DAsync(c.ws + h->emb.off + FE, sizeof(float) * h->emb.ld, 0, sizeof(float) * (h->emb.ld - FE), (size_t)n, c.st));
   for (int j = 0; j <= h->Li; ++j)
     if (gemm(c, DIB_GEMM_FWD, h->int_fwd[j], 1, int_fan_out(h, j), 0, 1, 0)) return 1;
@@ -1281,6 +1602,7 @@ int dib_metrics_update(const float* stats, const float* beta_dev, float* acc, in
 int dib_encoders_forward(dib_model* h, const float* params, const float* x, int64_t n, const float* eps, uint64_t seed,
                          uint32_t step, uint64_t sample_offset, float* out_emb, float* out_stats, void* workspace, void* stream) {
   if (check_call(h, params, x, n, workspace)) return 1;
+  if (h->st) return fail("dib_encoders_forward: a set-transformer model trains its encoder through dib_train_step");
   if (!out_emb || !out_stats) return fail("dib_encoders_forward: out_emb and out_stats are required");
   Ctx c{h, params, static_cast<float*>(workspace), static_cast<cudaStream_t>(stream), (int)n};
   if (n == 0) { DIB_CUDA_OK(cudaMemsetAsync(out_stats, 0, sizeof(float) * (h->F + 3), c.st)); return 0; }
@@ -1291,6 +1613,7 @@ int dib_encoders_backward(dib_model* h, const float* params, const float* x, con
                           const float* beta_dev, float inv_global_batch, const float* eps, uint64_t seed, uint32_t step,
                           uint64_t sample_offset, float* grads_flat, float* out_stats, void* workspace, void* stream) {
   if (check_call(h, params, x, n, workspace)) return 1;
+  if (h->st) return fail("dib_encoders_backward: a set-transformer model trains its encoder through dib_train_step");
   if ((!d_emb && n > 0) || !beta_dev || !grads_flat || !out_stats)
     return fail("dib_encoders_backward: d_emb, beta_dev, grads_flat and out_stats are required");
   Ctx c{h, params, static_cast<float*>(workspace), static_cast<cudaStream_t>(stream), (int)n};

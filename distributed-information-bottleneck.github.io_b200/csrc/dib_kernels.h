@@ -198,6 +198,44 @@ cudaError_t dib_int16_head(const void* g, int ldg, int K, const float* Wc, const
                            float* user_pred, float* wpart, int wpart_stride, float* loss_part, float* acc_part, int nblocks,
                            bool head1, int bf16, cudaStream_t st);
 
+// ---- the set-attention integration network (dib_set_attn.cu; integration_kind 1) ----
+// attention core of one block: q, k, v, o (and dout, dq, dk, dv) are [sets * L, heads * dk] with leading dimension ld; lse
+// [sets, heads, L] is the row log-sum-exp the forward keeps for the backward.  One CTA per (head, set), L <= 64, dk <= 128.
+struct DibAttnArgs {
+  const float* q; const float* k; const float* v; int ld;
+  float* o; float* lse;
+  long long sets; int heads, L, dk;
+  int round_out;
+  const float* dout; float* dq; float* dk_; float* dv;
+};
+size_t dib_attn_smem_bytes(int L, int dk, bool backward);
+cudaError_t dib_attn_prepare();   // once per model: the kernels' shared-memory opt-in
+cudaError_t dib_launch_attn_fwd(const DibAttnArgs& a, cudaStream_t st);
+cudaError_t dib_launch_attn_bwd(const DibAttnArgs& a, cudaStream_t st);
+// LayerNorm(a + b) over the last axis of [rows, E] (E <= 128, leading dimension ld); mean / rstd [rows] are kept
+struct DibLayerNorm {
+  const float* a; const float* b; int ld; long long rows; int E;
+  const float* gamma; const float* beta; float epsilon;
+  float* y; float* mean; float* rstd;
+  int round_out;
+};
+// its backward: dy = sum of dy[0..4) (nullable, [rows, ld]) + dy_pool[row / pool_rows] * pool_scale (nullable);
+// d_res = d(a + b); d_branch (nullable) = d_res * act'(b) (b is the output of a Dense with activation branch_act);
+// d gamma / d beta partials of CTA s at part + s * split_stride + gamma_off / beta_off, CTA s owning rows_per_split rows
+struct DibLayerNormBwd {
+  const float* dy[4]; const float* dy_pool; int pool_rows; float pool_scale;
+  float* d_res; float* d_branch; int branch_act; float alpha;
+  float* part; long long split_stride; long long gamma_off, beta_off; int nsplit; long long rows_per_split;
+};
+cudaError_t dib_launch_ln_fwd(const DibLayerNorm& a, cudaStream_t st);
+cudaError_t dib_launch_ln_bwd(const DibLayerNorm& a, const DibLayerNormBwd& b, cudaStream_t st);
+// out[s] = mean over the L rows of set s of x [sets * L, ld] (E live columns), out [sets, ldo]
+cudaError_t dib_launch_pool_fwd(const float* x, int ld, int E, int L, int64_t sets, float* out, int ldo, int round_out,
+                                cudaStream_t st);
+// dst[i] = sum of the non-null src[q][i], i < count
+struct DibSumRows { const float* src[4]; float* dst; long long count; };
+cudaError_t dib_launch_sum_rows(const DibSumRows& a, cudaStream_t st);
+
 cudaError_t dib_launch_mi_sandwich(const float* mu_logvar, int64_t n, int E, const float* eps, uint64_t seed, uint32_t step,
                                    float* row_scratch, float* out2, cudaStream_t st);
 // G = features x batches groups of n rows in one launch, float64 accumulation; group g uses the noise stream

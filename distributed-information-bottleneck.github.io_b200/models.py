@@ -1225,3 +1225,188 @@ class SharedParticleEncoder:
 
     def apply_gradients(self, flat_grads):
         self.net.apply_gradients(flat_grads)
+
+
+def set_transformer_param_specs(d, encoder_arch, E, L, number_heads, key_dim, number_attention_blocks, ff_arch_per_block,
+                                final_processing_arch, output_dimensionality, number_positional_encoding_frequencies=5):
+    """Every trainable variable of :class:`SetTransformerIBNet` in flat order (nb-particle cell 8's all_trainable_variables):
+    a list of (name, shape, init) where init is ('glorot', fan_in, fan_out), 'zeros' or 'ones'.  The attention kernels keep
+    their Keras shapes [E, h, dk] / [h, dk, E] here (the flat layout reports them as [E, h*dk] / [h*dk, E]); their glorot
+    fans follow Keras' ``_compute_fans`` [KERAS]: fan_in = shape[-2] * prod(shape[:-2]), fan_out = shape[-1] * prod(shape[:-2])."""
+    def dense(name, i, o):
+        return [(name + "/kernel", (i, o), ("glorot", i, o)), (name + "/bias", (o,), "zeros")]
+    specs = []
+    width = d * number_positional_encoding_frequencies if number_positional_encoding_frequencies > 1 else d
+    dims = [width] + list(encoder_arch) + [2 * E]
+    for k in range(len(dims) - 1):
+        specs += dense(f"encoder/dense{k}", dims[k], dims[k + 1])
+    h, dk = number_heads, key_dim
+    for b in range(number_attention_blocks):
+        p = f"block{b}/"
+        for q in ("query", "key", "value"):
+            specs += [(p + q + "/kernel", (E, h, dk), ("glorot", h * E, dk * E)), (p + q + "/bias", (h, dk), "zeros")]
+        specs += [(p + "attention_output/kernel", (h, dk, E), ("glorot", dk * h, E * h)), (p + "attention_output/bias", (E,), "zeros")]
+        specs += [(p + "ln1/gamma", (E,), "ones"), (p + "ln1/beta", (E,), "zeros")]
+        ff = [E] + list(ff_arch_per_block)
+        for k in range(len(ff) - 1):
+            specs += dense(p + f"ff{k}", ff[k], ff[k + 1])
+        specs += [(p + "ln2/gamma", (E,), "ones"), (p + "ln2/beta", (E,), "zeros")]
+    head = [E] + list(final_processing_arch) + [output_dimensionality]
+    for k in range(len(head) - 1):
+        specs += dense(f"head/dense{k}", head[k], head[k + 1])
+    return specs
+
+
+def check_set_transformer_args(particle_feature_dimensions, particle_encoder_arch_spec, bottleneck_dimension, number_particles,
+                               key_dim, number_heads, number_attention_blocks, ff_arch_per_block, ff_activation_fn,
+                               final_processing_arch, activation_fn, output_dimensionality, precision):
+    """The constructor checks of :class:`SetTransformerIBNet` (host only: they run before any device call)."""
+    E, L = int(bottleneck_dimension), int(number_particles)
+    if int(particle_feature_dimensions) < 1 or int(output_dimensionality) < 1:
+        raise ValueError("particle_feature_dimensions and output_dimensionality must be >= 1")
+    if any(int(w) < 1 for w in list(particle_encoder_arch_spec) + list(final_processing_arch) + list(ff_arch_per_block)):
+        raise ValueError("layer widths must be >= 1")
+    if not 1 <= L <= 64:
+        raise ValueError(f"number_particles must be in [1, 64] (one attention problem per set and head in shared memory), got {L}")
+    if not 1 <= int(key_dim) <= 128 or int(number_heads) < 1 or int(number_attention_blocks) < 1:
+        raise ValueError("the attention needs key_dim in [1, 128], number_heads >= 1 and number_attention_blocks >= 1")
+    if (int(number_heads) * int(key_dim)) % 4 or E % 4 or E > 128:
+        raise ValueError("number_heads * key_dim and bottleneck_dimension must be multiples of 4, bottleneck_dimension <= 128")
+    if not ff_arch_per_block or int(ff_arch_per_block[-1]) != E:
+        raise ValueError(f"the last width of ff_arch_per_block must equal bottleneck_dimension ({E}): the block adds FF(H) to H")
+    for a in (ff_activation_fn, activation_fn):
+        if a not in _lib.ACTIVATIONS:
+            raise ValueError(f"unsupported activation {a!r}")
+    if precision not in _lib.PRECISIONS:
+        raise ValueError(f"precision must be one of {sorted(_lib.PRECISIONS)}, got {precision!r}")
+
+
+class _ParticleEncoder(_FeatureEncoder):
+    """model.particle_encoder: [..., d] -> [..., 2E] = (mu || logvar), logvar offset applied (dib_encode_feature on particle
+    rows).  ``utils.estimate_mi_sandwich_bounds(model.particle_encoder, particles [N, d])`` works on it."""
+
+    def __call__(self, x, training=None):
+        t = x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32))
+        out = self._model._encode_feature(0, t)
+        return _as_numpy_like(x, out.reshape(*t.shape[:-1], out.shape[-1]))
+
+
+class _SetTransformer(_Network):
+    """model.set_transformer: embeddings [n, L, E] -> [n, out] through the attention blocks, the mean over the particles and
+    the head (dib_integration_forward), deterministic, on the model's precision path."""
+
+    def __call__(self, embs, training=None):
+        m = self._model
+        with torch.cuda.device(m.device):
+            e = m._to_device(embs, m.number_particles * m.feature_embedding_dimension)
+            n = e.shape[0]
+            m._ensure_handle(n)
+            out = torch.empty(n, m.output_dimensionality, dtype=torch.float32, device=m.device)
+            _lib.check(m._lib.dib_integration_forward(m._handle, _lib.ptr(m._params), _lib.ptr(e), n, _lib.ptr(out),
+                                                      _lib.ptr(m._workspace), _stream()))
+        return _as_numpy_like(embs, out)
+
+
+class SetTransformerIBNet(DistributedIBNet):
+    """nb-particle cell 8 (BASELINE config 5): a shared particle encoder (positional encoding -> Dense stack -> (mu, logvar),
+    logvar + ``logvar_initialization``, reparameterised per particle) feeding a set transformer -- ``number_attention_blocks``
+    blocks of ``H = LayerNorm(x + MultiHeadAttention(number_heads, key_dim)(x, x, x))``, ``x = LayerNorm(H + FF(H))`` --, the
+    mean over the particles and a Dense head.  Loss = compiled loss + beta * KL, the KL summed over dims and particles and
+    averaged over sets.  The whole step runs in the library (dib_config.integration_kind = set transformer), so ``compile`` /
+    ``fit`` / ``train_on_batch`` / ``evaluate`` / ``predict``, CUDA-graph replay and the data-parallel all-reduce are the
+    ones of :class:`DistributedIBNet`.
+
+    ``x`` is [N, number_particles, particle_feature_dimensions] and ``y`` [N, output_dimensionality]; batches count sets.
+    ``model.particle_encoder(x)`` returns mu || logvar per particle and ``model.set_transformer(embs)`` runs the network
+    after the encoder.  History keys: loss, accuracy (with metrics=['accuracy']), KL0 (per set), beta and their val_ twins.
+    ``fp16`` / ``bf16`` run every dense layer on the TF32 kernels; the attention and LayerNorm kernels are fp32 in every mode."""
+
+    def __init__(self, particle_feature_dimensions, particle_encoder_arch_spec, bottleneck_dimension=32, number_particles=50,
+                 key_dim=128, number_heads=12, number_attention_blocks=6, ff_arch_per_block=None, ff_activation_fn='relu',
+                 final_processing_arch=(256,), activation_fn='leaky_relu', leaky_alpha=0.1, output_dimensionality=1,
+                 logvar_initialization=-3., number_positional_encoding_frequencies=5, precision='fp32', **kw):
+        E = int(bottleneck_dimension)
+        ff = [128, E] if ff_arch_per_block is None else [int(w) for w in ff_arch_per_block]
+        check_set_transformer_args(particle_feature_dimensions, particle_encoder_arch_spec, E, number_particles, key_dim,
+                                   number_heads, number_attention_blocks, ff, ff_activation_fn, final_processing_arch,
+                                   activation_fn, output_dimensionality, precision)
+        self.particle_feature_dimensions = int(particle_feature_dimensions)
+        self.number_particles = int(number_particles)
+        self.key_dim, self.number_heads = int(key_dim), int(number_heads)
+        self.number_attention_blocks = int(number_attention_blocks)
+        self.ff_arch_per_block, self.ff_activation_fn = ff, ff_activation_fn
+        self.final_processing_arch = [int(w) for w in final_processing_arch]
+        # the host sees one row of number_particles * d values per set; the library runs the encoder on the particle rows
+        super().__init__([self.number_particles * self.particle_feature_dimensions], list(particle_encoder_arch_spec),
+                         self.final_processing_arch, output_dimensionality,
+                         use_positional_encoding=number_positional_encoding_frequencies > 1,
+                         number_positional_encoding_frequencies=number_positional_encoding_frequencies,
+                         activation_fn=activation_fn, feature_embedding_dimension=E, output_activation_fn=None,
+                         precision=precision, leaky_alpha=leaky_alpha, logvar_offset=logvar_initialization, **kw)
+        n_enc = 2 * (len(self.feature_encoder_architecture) + 1)
+        self.particle_encoder = _ParticleEncoder(self, 0, range(n_enc))
+        self.feature_encoders = [self.particle_encoder]
+        self.set_transformer = _SetTransformer(self, range(n_enc, self._n_model_vars))
+        self.integration_network = self.set_transformer
+
+    def _config(self, max_batch):
+        cfg = super()._config(max_batch)
+        self._c_pd = (ctypes.c_int32 * 1)(self.particle_feature_dimensions)
+        self._c_ff = (ctypes.c_int32 * len(self.ff_arch_per_block))(*self.ff_arch_per_block)
+        cfg.feature_dimensionalities = self._c_pd
+        cfg.integration_kind = _lib.INTEGRATION_KINDS["set_transformer"]
+        cfg.set_size = self.number_particles
+        cfg.number_attention_blocks = self.number_attention_blocks
+        cfg.number_heads, cfg.key_dim = self.number_heads, self.key_dim
+        cfg.number_ff_layers, cfg.ff_architecture = len(self.ff_arch_per_block), self._c_ff
+        cfg.ff_activation_fn = _lib.ACTIVATIONS[self.ff_activation_fn]
+        cfg.layer_norm_epsilon = 1e-3                                        # [KERAS] LayerNormalization default
+        return cfg
+
+    def param_specs(self):
+        """(name, Keras shape, init) of every trainable variable in flat order; see :func:`set_transformer_param_specs`."""
+        return set_transformer_param_specs(self.particle_feature_dimensions, self.feature_encoder_architecture,
+                                           self.feature_embedding_dimension, self.number_particles, self.number_heads,
+                                           self.key_dim, self.number_attention_blocks, self.ff_arch_per_block,
+                                           self.final_processing_arch, self.output_dimensionality,
+                                           self.number_positional_encoding_frequencies if self.use_positional_encoding else 1)
+
+    def _glorot_flat(self):
+        """[KERAS] glorot_uniform kernels with the fans of ``_compute_fans`` (3-D attention kernels included), zero biases,
+        LayerNorm gamma = 1 and beta = 0 (RNG stream is ours)."""
+        g = torch.Generator(device="cpu")
+        g.manual_seed(self.seed)
+        flat = torch.zeros(self._P, dtype=torch.float32)
+        for off, (_, shape, init) in zip(self._var_off, self.param_specs()):
+            size = int(np.prod(shape))
+            if init == "ones":
+                flat[off:off + size] = 1.0
+            elif init != "zeros":
+                lim = math.sqrt(6.0 / (init[1] + init[2]))
+                flat[off:off + size] = (torch.rand(size, generator=g) * 2 - 1) * lim
+        return flat
+
+    def _encode_feature(self, i, x_i):
+        """Particle rows [..., d] -> [rows, 2E]."""
+        t = self._to_device(x_i).reshape(-1, self.particle_feature_dimensions).contiguous()
+        n = t.shape[0]
+        self._ensure_handle(max(1, -(-n // self.number_particles)))
+        out = torch.empty(n, 2 * self.feature_embedding_dimension, dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.dib_encode_feature(self._handle, _lib.ptr(self._params), 0, _lib.ptr(t), n, _lib.ptr(out),
+                                                    _lib.ptr(self._workspace), _stream()))
+        return out
+
+    def compile(self, optimizer='adam', loss=None, metrics=None, **kw):
+        kind = resolve_loss(loss)
+        if kind in ("sparse_ce_logits", "infonce"):
+            raise ValueError("SetTransformerIBNet trains with BinaryCrossentropy (logits or probabilities), MSE or the external "
+                             f"loss, not {kind!r}")
+        super().compile(optimizer, loss, metrics, **kw)
+
+    def build(self, input_shape):
+        assert tuple(input_shape[-2:]) == (self.number_particles, self.particle_feature_dimensions)
+
+    def compression_matrices(self, *a, **k):
+        raise NotImplementedError("compression matrices of particles: run model.particle_encoder on the particle rows and "
+                                  "utils.bhattacharyya_dist_mat on its output")

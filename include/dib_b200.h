@@ -33,8 +33,9 @@
 extern "C" {
 #endif
 
-/* 3 appends the InfoNCE fields to dib_config; dib_create still accepts abi_version 2 structs and reads only their prefix. */
-#define DIB_ABI_VERSION 3
+/* 3 appended the InfoNCE fields to dib_config, 4 the integration-network fields; dib_create still accepts abi_version 2 and 3
+ * structs and reads only their prefix. */
+#define DIB_ABI_VERSION 4
 
 /* activation_fn strings accepted by tf.keras.layers.Dense in the reference's call sites
  * (train.py:37 'relu', nb-radial 'tanh', nb-bool LeakyReLU, None). */
@@ -85,6 +86,23 @@ enum dib_precision { DIB_PREC_FP32 = 0, DIB_PREC_TF32 = 1, DIB_PREC_BF16 = 2, DI
  * flat parameter order per feature: mu_scaling, logvar; feature_encoder_architecture is ignored). */
 enum dib_encoder_kind { DIB_ENCODER_MLP = 0, DIB_ENCODER_SIMPLE = 1 };
 
+/* integration networks: the Dense stack of models.py:81-84, or the per-particle set transformer of nb-particle cell 8.
+ * DIB_INTEGRATION_SET_TRANSFORMER: number_features == 1 and x is [n, set_size, d] -- n counts SETS of set_size particles,
+ * y is [n, out], max_batch counts sets (the workspace holds max_batch * set_size particle rows).  The one feature encoder runs
+ * with shared weights on every particle; its embeddings [n, L, E] pass number_attention_blocks blocks of
+ *   H = LayerNorm(x + MultiHeadAttention(number_heads, key_dim)(x, x, x)),  x' = LayerNorm(H + FF(H))
+ * (Keras 2 MultiHeadAttention without dropout or mask; FF = Dense(ff_architecture[j], ff_activation_fn) for every j, the
+ * last width equal to E; LayerNorm with layer_norm_epsilon, biased variance), then the mean over the particles feeds the Dense
+ * head integration_network_architecture (activation_fn) -> output_dimensionality (output_activation_fn).
+ * Flat parameter order: the encoder, then per block q kernel [E, h*dk], q bias [h*dk], k, k bias, v, v bias, output kernel
+ * [h*dk, E], output bias [E], LN1 gamma, LN1 beta, the FF kernels and biases, LN2 gamma, LN2 beta; then the head.
+ * Statistics: the KL slot sums over sets, particles and dims; inv_global_batch is 1 / (global number of sets); the noise of
+ * particle p of set s is keyed by the global particle row (sample_offset + s) * set_size + p.
+ * Needs set_size in [1, 64], key_dim in [1, 128], number_heads * key_dim and E multiples of 4, E <= 128, max_batch <= 65535,
+ * no dropout, and a loss other than DIB_LOSS_SPARSE_CE_LOGITS / DIB_LOSS_INFONCE.  The attention core and the LayerNorms are
+ * fp32 CUDA-core kernels in every precision; FP16 / BF16 run every dense layer on the TF32 kernels. */
+enum dib_integration_kind { DIB_INTEGRATION_MLP = 0, DIB_INTEGRATION_SET_TRANSFORMER = 1 };
+
 /* Mirrors the constructor of models.DistributedIBNet (models.py:56-66). */
 typedef struct dib_config {
   int32_t abi_version;               /* DIB_ABI_VERSION */
@@ -119,6 +137,16 @@ typedef struct dib_config {
   const int32_t* y_encoder_architecture; /* hidden widths (--infonce_y_encoder_architecture)  train.py:189-190 */
   int32_t infonce_similarity;        /* 0 'l2sq' | 1 'l2' | 2 'l1' | 3 'linf' | 4 'cosine' (dib_scaled_similarity kinds) */
   float   infonce_temperature;       /* > 0                                          train.py:204 */
+  /* ---- abi_version >= 4: the integration network (zero-initialised fields give models.py's Dense stack) ---- */
+  int32_t integration_kind;          /* enum dib_integration_kind */
+  int32_t set_size;                  /* L, particles per set (nb-particle clips every set to 50) */
+  int32_t number_attention_blocks;   /* 6 in nb-particle cell 8 */
+  int32_t number_heads;              /* 12 */
+  int32_t key_dim;                   /* 128 */
+  int32_t number_ff_layers;          /* len(ff_architecture) */
+  const int32_t* ff_architecture;    /* [128, E] */
+  int32_t ff_activation_fn;          /* enum dib_activation; relu on every FF layer in the notebook */
+  float   layer_norm_epsilon;        /* 0 -> 1e-3 (the Keras default) */
 } dib_config;
 
 typedef struct dib_model dib_model;
