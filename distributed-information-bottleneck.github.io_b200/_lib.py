@@ -73,6 +73,11 @@ SIGNATURES = {
     "dib_encode_feature": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
     "dib_train_step": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_float, c_void_p,
                                  c_uint64, c_uint32, c_uint64, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "dib_infonce_shard_forward": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_uint64, c_uint32,
+                                            c_uint64, c_void_p, c_int64, c_int64, c_void_p, c_void_p]),
+    "dib_infonce_shard_lse": (c_int32, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "dib_infonce_shard_backward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_uint64, c_uint32, c_uint64,
+                                             c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p]),
     "dib_set_noise_step_device": (c_int32, [c_void_p, c_void_p]),
     "dib_adam_step": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_float,
                                 c_float, c_float, c_void_p]),

@@ -101,6 +101,8 @@ struct dib_model {
   Buf ype, y_out, d_y_out;          // PE(y), e2 = output_encoder(y), d loss / d e2
   std::vector<Buf> y_act, d_yact;   // index 1..Ly
   long long nce_off = 0;            // 3 * max_batch floats of InfoNCE scratch
+  long long nce_stats_off = 0;      // F + 3 floats: the stats dib_infonce_shard_lse wrote, for the backward's IB weight
+  int nce_nblk_kl = 0;              // KL partials per feature dib_infonce_shard_forward left for dib_infonce_shard_lse
   std::vector<int> y_fwd, y_dgrad, y_wgrad;
   int* d_ycol_src = nullptr;
   int* d_ycol_freq = nullptr;
@@ -253,6 +255,7 @@ void plan(dib_model* h) {
     h->d_y_out = make_buf(c, B, h->out, 1);
     for (int j = 1; j <= h->Ly; ++j) h->d_yact[j] = make_buf(c, B, h->y_arch[j - 1], 1);
     h->nce_off = take(c, 3 * B);
+    h->nce_stats_off = take(c, h->F + 3);
   }
   if (h->st) {                          // per block what its backward reads; one set of backward scratch for all blocks
     const int E = h->E, nf = nff(h);
@@ -617,39 +620,80 @@ int forward_encoders(const Ctx& c, const float* x, const NoiseKey& nk, float* us
   return 0;
 }
 
-// DIB_LOSS_INFONCE with targets, after the integration network wrote e1 = pred: output encoder e2 = output_encoder(y), the
-// streaming InfoNCE loss into the stats row and, training, d loss / d e1 into d_pred (what the DIB_LOSS_EXTERNAL backward reads)
-// and d loss / d e2 into d_y_out (what backward_output_encoder reads)
-int forward_infonce(const Ctx& c, const float* y, bool training, float* user_pred, float* out_stats, int nblk_kl) {
+// e2 = output_encoder(y) into y_out (train.py:186-193)
+int forward_output_encoder(const Ctx& c, const float* y) {
   dib_model* h = c.h;
-  const int rnd = is_tc(h) ? 1 : 0;
   prof_begin(c, "y_pe");
-  DIB_CUDA_OK(dib_launch_pe(y, h->ydim, 0, h->d_ycol_src, h->d_ycol_freq, 0, h->ldype, c.ws + h->ype.off, h->ldype, 0, c.n, rnd, c.st));
+  DIB_CUDA_OK(dib_launch_pe(y, h->ydim, 0, h->d_ycol_src, h->d_ycol_freq, 0, h->ldype, c.ws + h->ype.off, h->ldype, 0, c.n,
+                            is_tc(h) ? 1 : 0, c.st));
   prof_end(c);
   for (int j = 0; j <= h->Ly; ++j) {
     prof_begin(c, "y_fwd_l", j);
     if (gemm(c, DIB_GEMM_FWD, h->y_fwd[j], 1, y_fan_out(h, j), 0, 1, 0)) return 1;
     prof_end(c);
   }
+  return 0;
+}
+
+// the streaming InfoNCE of the c.n own rows [row0, row0 + c.n) of e1 / e2 [n, d] against all n rows: r and c at lse_stride,
+// s_ii, the loss sum and the accuracy zero in the workspace; d loss / d e1 into d_pred (what the DIB_LOSS_EXTERNAL backward
+// reads) and d loss / d e2 into d_y_out (what backward_output_encoder reads), both at local row index
+DibInfonceStream infonce_args(const Ctx& c, const float* e1, int ld1, const float* e2, int ld2, long long n, long long row0,
+                              float* lse_r, float* lse_c, int lse_stride) {
+  const dib_model* h = c.h;
   DibInfonceStream a;
   a.kind = h->sim_kind; a.temperature = h->temperature;
-  a.e1 = c.ws + h->pred.off; a.ld1 = h->pred.ld;
-  a.e2 = c.ws + h->y_out.off; a.ld2 = h->y_out.ld;
-  a.n = c.n; a.d = h->out;
-  a.scratch = c.ws + h->nce_off;
+  a.e1 = e1; a.ld1 = ld1;
+  a.e2 = e2; a.ld2 = ld2;
+  a.n = n; a.d = h->out;
+  a.row0 = row0; a.rows = c.n;
+  a.lse_r = lse_r; a.lse_c = lse_c; a.lse_stride = lse_stride;
+  a.diag = c.ws + h->nce_off + 2 * (long long)c.n;
   a.loss_sum = c.ws + h->loss_part_off; a.acc_zero = c.ws + h->acc_part_off;
   a.d_e1 = c.ws + h->d_pred.off; a.ld_d1 = h->d_pred.ld;
   a.d_e2 = c.ws + h->d_y_out.off; a.ld_d2 = h->d_y_out.ld;
-  a.round_out = rnd;
+  a.round_out = is_tc(h) ? 1 : 0;
+  return a;
+}
+
+// the row / column sweeps and the loss sum of the own rows, then the stats row (KL sums of the forward, n = own rows)
+int infonce_loss_stats(const Ctx& c, const DibInfonceStream& a, float* out_stats, int nblk_kl) {
+  dib_model* h = c.h;
   prof_begin(c, "infonce_loss_stats");
   DIB_CUDA_OK(dib_launch_infonce_stream_loss(a, c.st));
   DIB_CUDA_OK(dib_launch_finalize_stats(c.ws + h->kl_part_off, h->kl_stride, nblk_kl, c.ws + h->loss_part_off, c.ws + h->acc_part_off,
                                         1, h->F, c.n, 1, out_stats, c.st));
   prof_end(c);
+  return 0;
+}
+
+int infonce_grads(const Ctx& c, const DibInfonceStream& a) {
+  prof_begin(c, "infonce_grads");
+  DIB_CUDA_OK(dib_launch_infonce_stream_grads(a, c.st));
+  prof_end(c);
+  return 0;
+}
+
+// DIB_LOSS_INFONCE with targets on one GPU, after the integration network wrote e1 = pred: output encoder e2 = output_encoder(y),
+// the streaming InfoNCE loss over all c.n rows into the stats row and, training, its gradients
+int forward_infonce(const Ctx& c, const float* y, bool training, float* user_pred, float* out_stats, int nblk_kl) {
+  dib_model* h = c.h;
+  if (forward_output_encoder(c, y)) return 1;
+  float* scratch = c.ws + h->nce_off;
+  const DibInfonceStream a = infonce_args(c, c.ws + h->pred.off, h->pred.ld, c.ws + h->y_out.off, h->y_out.ld, c.n, 0, scratch,
+                                          scratch + c.n, 1);
+  if (infonce_loss_stats(c, a, out_stats, nblk_kl)) return 1;
   if (user_pred) DIB_CUDA_OK(dib_launch_copy2d(c.ws + h->pred.off, h->pred.ld, user_pred, h->out, h->out, c.n, c.st));
-  if (training) {
-    prof_begin(c, "infonce_grads");
-    DIB_CUDA_OK(dib_launch_infonce_stream_grads(a, c.st));
+  if (training && infonce_grads(c, a)) return 1;
+  return 0;
+}
+
+// the integration layers on the per-layer GEMM route: emb -> pred
+int forward_int_gemms(const Ctx& c) {
+  dib_model* h = c.h;
+  for (int j = 0; j <= h->Li; ++j) {
+    prof_begin(c, "int_fwd_l", j);
+    if (gemm(c, DIB_GEMM_FWD, h->int_fwd[j], 1, int_fan_out(h, j), 0, 1, 0)) return 1;
     prof_end(c);
   }
   return 0;
@@ -665,11 +709,7 @@ int forward_integration(const Ctx& c, const float* y, float inv_batch, bool trai
                                      nblk_loss, h->F, c.n, y != nullptr, out_stats, c.st);
   };
   if (!h->route.int16) {
-    for (int j = 0; j <= h->Li; ++j) {
-      prof_begin(c, "int_fwd_l", j);
-      if (gemm(c, DIB_GEMM_FWD, h->int_fwd[j], 1, int_fan_out(h, j), 0, 1, 0)) return 1;
-      prof_end(c);
-    }
+    if (forward_int_gemms(c)) return 1;
     if (infonce(h) && y) return forward_infonce(c, y, training, user_pred, out_stats, nblk_kl);
     prof_begin(c, "loss_stats");
     DIB_CUDA_OK(dib_launch_loss(h->loss, h->out_act, h->alpha, c.ws + h->pred.off, h->pred.ld, y, h->out, c.n, inv_batch,
@@ -724,14 +764,21 @@ int forward_integration(const Ctx& c, const float* y, float inv_batch, bool trai
   return 0;
 }
 
-int run_forward(const Ctx& c, const float* x, const float* y, const NoiseKey& nk, float inv_batch, float* user_pred,
-                float* user_emb, float* out_stats, bool enc_only = false) {
+// TF32 GEMMs read the weights through a TF32-rounded copy
+int weights_shadow(const Ctx& c) {
   dib_model* h = c.h;
-  if (is_tc(h) && !h->route.int16) {      // TF32 GEMMs read the weights through a TF32-rounded copy
+  if (is_tc(h) && !h->route.int16) {
     prof_begin(c, "weights_tf32_shadow");
     DIB_CUDA_OK(dib_launch_round_copy(c.params, c.ws + h->wshadow_off, h->P, c.st));
     prof_end(c);
   }
+  return 0;
+}
+
+int run_forward(const Ctx& c, const float* x, const float* y, const NoiseKey& nk, float inv_batch, float* user_pred,
+                float* user_emb, float* out_stats, bool enc_only = false) {
+  dib_model* h = c.h;
+  if (weights_shadow(c)) return 1;
   int nblk_kl = 0;
   if (forward_encoders(c, x, nk, user_emb, enc_only, &nblk_kl)) return 1;
   if (enc_only) {
@@ -1082,6 +1129,58 @@ int train_step_set(const Ctx& cs, const float* x, const float* y, const NoiseKey
   DIB_CUDA_OK(dib_launch_reduce_partials(c.ws + h->part_off, h->Pp, nrows, h->intW[0], grads_flat, c.st));
   prof_end(c);
   return 0;
+}
+
+// the reverse mode of dib_train_step after its forward (and, with DIB_LOSS_INFONCE, the InfoNCE gradients) left the
+// workspace: the IB weight from the stats, the integration network's, the output encoder's and the encoders' backward and the
+// fixed-order reductions into grads_flat
+int backward_all(const Ctx& c, const float* x, const NoiseKey& nk, const float* beta_dev, const float* stats, float inv_global_batch,
+                 float* grads_flat) {
+  dib_model* h = c.h;
+  const float* beta_w = nullptr;           // weight of the per-sample KL gradients in the encoder backward
+  if (ib_weight(c, beta_dev, stats, inv_global_batch, &beta_w)) return 1;
+  const Split sp = batch_split(c.n);
+  std::vector<DibReduceSeg> segs;          // fixed-order reductions of the step, run as ONE launch at the end
+  if (backward_integration(c, inv_global_batch, sp, grads_flat, &segs)) return 1;
+  if (infonce(h) && backward_output_encoder(c, sp, grads_flat)) return 1;
+  int nrows = 0;
+  const bool d16 = h->route.int16;         // the 16-bit integration backward leaves d emb in fp16
+  if (backward_encoders(c, x, nk, d16 ? nullptr : c.ws + h->d_emb.off, d16 ? 0 : h->d_emb.ld, d16 ? c.ws + h->demb16_off : nullptr,
+                        beta_w, inv_global_batch, sp, &nrows))
+    return 1;
+  float* part = c.ws + h->part_off;
+  const long long p_enc = h->intW[0];      // encoder parameters occupy [0, p_enc)
+  prof_begin(c, "enc_split_reduce");
+  if (h->route.enc_fused) {
+    segs.push_back({part, h->Pp, nrows, p_enc, 1.f, grads_flat});
+    DIB_CUDA_OK(dib_launch_reduce_segments(segs.data(), (int)segs.size(), c.st));
+  } else {
+    DIB_CUDA_OK(dib_launch_reduce_partials(part, h->Pp, nrows, p_enc, grads_flat, c.st));
+  }
+  prof_end(c);
+  return 0;
+}
+
+// ---- DIB_LOSS_INFONCE across a data-parallel group (DESIGN section 7): the step split where rows of other ranks enter ----
+int check_shard(const dib_model* h, const char* fn, int64_t n, int64_t n_global, int64_t row_offset, const void* e_all,
+                const void* workspace) {
+  if (!h) return fail("null model handle");
+  if (!infonce(h)) return fail(std::string(fn) + ": the loss is not DIB_LOSS_INFONCE");
+  if (n < 1 || n > h->maxB)
+    return fail(std::string(fn) + ": n = " + std::to_string(n) + " must be in [1, config.max_batch = " + std::to_string(h->maxB) + "]");
+  if (row_offset < 0 || n_global > 0x7fffffffll || row_offset + n > n_global)
+    return fail(std::string(fn) + ": needs 0 <= row_offset and row_offset + n <= n_global < 2^31 (row_offset = " +
+                std::to_string(row_offset) + ", n = " + std::to_string(n) + ", n_global = " + std::to_string(n_global) + ")");
+  if (!e_all || (reinterpret_cast<uintptr_t>(e_all) & 15)) return fail(std::string(fn) + ": e_all must be 16-byte aligned");
+  if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255)) return fail(std::string(fn) + ": workspace must be 256-byte aligned");
+  return 0;
+}
+
+// [e1 | e2] of all n_global rows, row-major [n_global, 2d]
+DibInfonceStream shard_args(const Ctx& c, const float* e_all, int64_t n_global, int64_t row_offset, const float* lse_all) {
+  const int d = c.h->out;
+  float* lse = const_cast<float*>(lse_all);
+  return infonce_args(c, e_all, 2 * d, e_all + d, 2 * d, n_global, row_offset, lse, lse + 1, 2);
 }
 
 }  // namespace
@@ -1489,28 +1588,56 @@ int dib_train_step(dib_model* h, const float* params, const float* x, const floa
   const NoiseKey nk{eps, seed, step, sample_offset, true};
   if (h->st) return train_step_set(c, x, y, nk, beta_dev, inv_global_batch, grads_flat, out_stats);
   if (run_forward(c, x, y, nk, inv_global_batch, nullptr, nullptr, out_stats)) return 1;
-  const float* beta_w = nullptr;           // weight of the per-sample KL gradients in the encoder backward
-  if (ib_weight(c, beta_dev, out_stats, inv_global_batch, &beta_w)) return 1;
-  const Split sp = batch_split(n);
-  std::vector<DibReduceSeg> segs;          // fixed-order reductions of the step, run as ONE launch at the end
-  if (backward_integration(c, inv_global_batch, sp, grads_flat, &segs)) return 1;
-  if (infonce(h) && backward_output_encoder(c, sp, grads_flat)) return 1;
-  int nrows = 0;
-  const bool d16 = h->route.int16;         // the 16-bit integration backward leaves d emb in fp16
-  if (backward_encoders(c, x, nk, d16 ? nullptr : c.ws + h->d_emb.off, d16 ? 0 : h->d_emb.ld, d16 ? c.ws + h->demb16_off : nullptr,
-                        beta_w, inv_global_batch, sp, &nrows))
+  return backward_all(c, x, nk, beta_dev, out_stats, inv_global_batch, grads_flat);
+}
+
+int dib_infonce_shard_forward(dib_model* h, const float* params, const float* x, const float* y, int64_t n, int32_t training,
+                              const float* eps, uint64_t seed, uint32_t step, uint64_t sample_offset, float* e_all,
+                              int64_t n_global, int64_t row_offset, void* workspace, void* stream) {
+  if (check_call(h, params, x, n, workspace) ||
+      check_shard(h, "dib_infonce_shard_forward", n, n_global, row_offset, e_all, workspace))
     return 1;
-  float* part = c.ws + h->part_off;
-  const long long p_enc = h->intW[0];      // encoder parameters occupy [0, p_enc)
-  prof_begin(c, "enc_split_reduce");
-  if (h->route.enc_fused) {
-    segs.push_back({part, h->Pp, nrows, p_enc, 1.f, grads_flat});
-    DIB_CUDA_OK(dib_launch_reduce_segments(segs.data(), (int)segs.size(), c.st));
-  } else {
-    DIB_CUDA_OK(dib_launch_reduce_partials(part, h->Pp, nrows, p_enc, grads_flat, c.st));
-  }
-  prof_end(c);
+  if (!y) return fail("dib_infonce_shard_forward: y is required");
+  Ctx c{h, params, static_cast<float*>(workspace), static_cast<cudaStream_t>(stream), (int)n};
+  c.dev_step = training != 0;
+  const NoiseKey nk{eps, seed, step, sample_offset, training != 0};
+  if (weights_shadow(c)) return 1;
+  int nblk_kl = 0;
+  if (forward_encoders(c, x, nk, nullptr, false, &nblk_kl) || forward_int_gemms(c) || forward_output_encoder(c, y)) return 1;
+  h->nce_nblk_kl = nblk_kl;
+  const int d = h->out;
+  float* own = e_all + row_offset * 2 * d;
+  DIB_CUDA_OK(dib_launch_copy2d(c.ws + h->pred.off, h->pred.ld, own, 2 * d, d, n, c.st));
+  DIB_CUDA_OK(dib_launch_copy2d(c.ws + h->y_out.off, h->y_out.ld, own + d, 2 * d, d, n, c.st));
   return 0;
+}
+
+int dib_infonce_shard_lse(dib_model* h, const float* e_all, int64_t n_global, int64_t row_offset, int64_t n, float* lse_all,
+                          float* out_stats, void* workspace, void* stream) {
+  if (check_shard(h, "dib_infonce_shard_lse", n, n_global, row_offset, e_all, workspace)) return 1;
+  if (!lse_all || (reinterpret_cast<uintptr_t>(lse_all) & 15) || !out_stats)
+    return fail("dib_infonce_shard_lse: lse_all (16-byte aligned) and out_stats are required");
+  Ctx c{h, nullptr, static_cast<float*>(workspace), static_cast<cudaStream_t>(stream), (int)n};
+  if (infonce_loss_stats(c, shard_args(c, e_all, n_global, row_offset, lse_all), out_stats, h->nce_nblk_kl)) return 1;
+  if (h->kl_exp != 1.f || h->kl_scale != 1.f)      // the backward's IB weight reads the KL sums
+    DIB_CUDA_OK(cudaMemcpyAsync(c.ws + h->nce_stats_off, out_stats, sizeof(float) * (h->F + 3), cudaMemcpyDeviceToDevice, c.st));
+  return 0;
+}
+
+int dib_infonce_shard_backward(dib_model* h, const float* params, const float* x, int64_t n, const float* beta_dev, const float* eps,
+                               uint64_t seed, uint32_t step, uint64_t sample_offset, const float* e_all, const float* lse_all,
+                               int64_t n_global, int64_t row_offset, float* grads_flat, void* workspace, void* stream) {
+  if (check_call(h, params, x, n, workspace) ||
+      check_shard(h, "dib_infonce_shard_backward", n, n_global, row_offset, e_all, workspace))
+    return 1;
+  if (!lse_all || (reinterpret_cast<uintptr_t>(lse_all) & 15) || !beta_dev || !grads_flat)
+    return fail("dib_infonce_shard_backward: lse_all (16-byte aligned), beta_dev and grads_flat are required");
+  Ctx c{h, params, static_cast<float*>(workspace), static_cast<cudaStream_t>(stream), (int)n};
+  c.dev_step = true;
+  const NoiseKey nk{eps, seed, step, sample_offset, true};
+  if (infonce_grads(c, shard_args(c, e_all, n_global, row_offset, lse_all))) return 1;
+  // rounded from double like a caller's inv_global_batch: one rank's step is dib_train_step's bit for bit
+  return backward_all(c, x, nk, beta_dev, c.ws + h->nce_stats_off, (float)(1.0 / (double)n_global), grads_flat);
 }
 
 // Philox 'step' word from device memory (CUDA-Graph replay: a captured launch cannot carry a fresh by-value step):

@@ -9,6 +9,9 @@
 //      (a - b = -(b - a), fmaf(a, b) = fmaf(b, a)), so the column sweep is the row sweep with the operands swapped;
 //   3. loss: sum_i (r_i + c_i - 2 s_ii) in a fixed order (= n * loss, the stats slot);
 //   4. gradient sweeps, again once per side with the roles swapped.
+// Every sweep covers a range of own rows [row0, row0 + rows) of `self` against all n rows of `other`, with the diagonal test
+// and 1/n on global indices: a data-parallel rank sweeps its rows of the all-gathered embeddings, and each r_i, c_j, s_ii
+// and gradient row is bit-identical to the one a single GPU computes for that row.
 // Arithmetic is fp32 on CUDA cores in the difference form of dib_similarity_kernel (dib_infonce.cu): every s_ij is
 // accumulated over d in the same order, so it equals the value that kernel writes.  Nothing is accumulated with atomics:
 // every sum has a fixed order, so results are bit-identical run to run and under graph replay.  d <= 512.
@@ -78,13 +81,14 @@ __device__ __forceinline__ void tile_similarity(const float* sa, int i0, const f
   }
 }
 
-// lse[i] = log sum_j exp S(self_i, other_j) over all n rows of `other`; diag[i] = S(self_i, other_i) when diag != nullptr.
-// One block per 32 rows of `self`; each lane keeps an online (max, sum) over the columns j = lane (mod 32), merged across
-// the warp in a fixed tree at the end.
+// lse[i * lse_stride] = log sum_j exp S(self_i, other_j) over all n rows of `other`, for the own rows i in [self0, self_end);
+// diag[i - self0] = S(self_i, other_i) when diag != nullptr.  One block per 32 own rows; each lane keeps an online
+// (max, sum) over the columns j = lane (mod 32), merged across the warp in a fixed tree at the end.
 template <int KIND>
 __global__ void __launch_bounds__(kThreads)
 dib_infonce_lse_kernel(const float* __restrict__ self, int ld_self, const float* __restrict__ other, int ld_other, int n, int d,
-                       float inv_t, float* __restrict__ lse, float* __restrict__ diag) {
+                       float inv_t, long long self0, long long self_end, float* __restrict__ lse, int lse_stride,
+                       float* __restrict__ diag) {
   extern __shared__ float sm[];
   const int ld = smem_ld(d);
   float* sa = sm;
@@ -92,8 +96,8 @@ dib_infonce_lse_kernel(const float* __restrict__ self, int ld_self, const float*
   float* na = sb + kTile * ld;
   float* nb = na + kTile;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, i0 = warp * kRowsPerWarp;
-  const long long row0 = (long long)blockIdx.x * kTile;
-  stage_rows<KIND>(self, ld_self, n, row0, d, sa, na);
+  const long long row0 = self0 + (long long)blockIdx.x * kTile;
+  stage_rows<KIND>(self, ld_self, self_end, row0, d, sa, na);
   float mx[kRowsPerWarp], sum[kRowsPerWarp];
 #pragma unroll
   for (int r = 0; r < kRowsPerWarp; ++r) { mx[r] = -INFINITY; sum[r] = 0.f; }
@@ -109,7 +113,7 @@ dib_infonce_lse_kernel(const float* __restrict__ self, int ld_self, const float*
     for (int r = 0; r < kRowsPerWarp; ++r) {
       if (s[r] > mx[r]) { sum[r] = sum[r] * expf(mx[r] - s[r]) + 1.f; mx[r] = s[r]; }
       else sum[r] += expf(s[r] - mx[r]);
-      if (diag && row0 + i0 + r == j) diag[j] = s[r];
+      if (diag && row0 + i0 + r == j && j < self_end) diag[j - self0] = s[r];
     }
   }
 #pragma unroll
@@ -124,17 +128,18 @@ dib_infonce_lse_kernel(const float* __restrict__ self, int ld_self, const float*
       m = mm;
     }
     const long long i = row0 + i0 + r;
-    if (lane == 0 && i < n) lse[i] = m + logf(t);
+    if (lane == 0 && i < self_end) lse[i * lse_stride] = m + logf(t);
   }
 }
 
-// out[0] = sum_i (r_i + c_i - 2 s_ii) (= n * loss) and out_acc[0] = 0, one block, fixed order
+// out[0] = sum_i (r_i + c_i - 2 s_ii) over the `rows` own rows (r, c at element stride `stride`, all three at local index;
+// = n * loss on one GPU) and out_acc[0] = 0, one block, fixed order
 __global__ void __launch_bounds__(kThreads)
-dib_infonce_stream_loss_kernel(const float* __restrict__ r, const float* __restrict__ c, const float* __restrict__ diag, int n,
-                               float* __restrict__ out, float* __restrict__ out_acc) {
+dib_infonce_stream_loss_kernel(const float* __restrict__ r, const float* __restrict__ c, int stride, const float* __restrict__ diag,
+                               int rows, float* __restrict__ out, float* __restrict__ out_acc) {
   __shared__ float red[kThreads / 32];
   float v = 0.f;
-  for (int i = threadIdx.x; i < n; i += kThreads) v += r[i] + c[i] - 2.f * diag[i];
+  for (int i = threadIdx.x; i < rows; i += kThreads) v += r[(long long)i * stride] + c[(long long)i * stride] - 2.f * diag[i];
   v = dib_warp_sum(v);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
   __syncthreads();
@@ -147,14 +152,16 @@ dib_infonce_stream_loss_kernel(const float* __restrict__ r, const float* __restr
 }
 
 // d self_i = sum_o w_io d s_io / d self_i, w_io = (exp(s_io - lse_self_i) + exp(s_io - lse_other_o) - 2 delta_io) / n, with
-// s_io = S(self_i, other_o).  One block per 32 rows of `self`; per tile the weights and the per-pair factor go to shared
-// memory, then every thread adds the tile's contribution to its own (row, dim) elements of the accumulator.  Output rows are
-// written with leading dimension ld_out (pad columns zeroed) and rounded to TF32 when round_out.
+// s_io = S(self_i, other_o), for the own rows i in [self0, self_end) against all n rows of `other`; lse_self / lse_other at
+// element stride lse_stride, global index.  One block per 32 own rows; per tile the weights and the per-pair factor go to
+// shared memory, then every thread adds the tile's contribution to its own (row, dim) elements of the accumulator.  Output
+// row i is written at local index i - self0 with leading dimension ld_out (pad columns zeroed), rounded to TF32 when round_out.
 template <int KIND>
 __global__ void __launch_bounds__(kThreads)
 dib_infonce_grad_stream_kernel(const float* __restrict__ self, int ld_self, const float* __restrict__ other, int ld_other, int n,
-                               int d, float inv_t, const float* __restrict__ lse_self, const float* __restrict__ lse_other,
-                               float* __restrict__ d_self, int ld_out, int round_out) {
+                               int d, float inv_t, long long self0, long long self_end, const float* __restrict__ lse_self,
+                               const float* __restrict__ lse_other, int lse_stride, float* __restrict__ d_self, int ld_out,
+                               int round_out) {
   extern __shared__ float sm[];
   const int ld = smem_ld(d);
   float* sa = sm;
@@ -165,13 +172,13 @@ dib_infonce_grad_stream_kernel(const float* __restrict__ self, int ld_self, cons
   float* na = ex + kTile * (kTile + 1);
   float* nb = na + kTile;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, i0 = warp * kRowsPerWarp;
-  const long long row0 = (long long)blockIdx.x * kTile;
+  const long long row0 = self0 + (long long)blockIdx.x * kTile;
   const float inv_n = 1.f / (float)n;
-  stage_rows<KIND>(self, ld_self, n, row0, d, sa, na);
+  stage_rows<KIND>(self, ld_self, self_end, row0, d, sa, na);
   for (int idx = threadIdx.x; idx < kTile * d; idx += kThreads) acc[idx] = 0.f;
   float lr[kRowsPerWarp];
 #pragma unroll
-  for (int r = 0; r < kRowsPerWarp; ++r) lr[r] = row0 + i0 + r < n ? lse_self[row0 + i0 + r] : 0.f;
+  for (int r = 0; r < kRowsPerWarp; ++r) lr[r] = row0 + i0 + r < self_end ? lse_self[(row0 + i0 + r) * lse_stride] : 0.f;
   for (int j0 = 0; j0 < n; j0 += kTile) {
     __syncthreads();
     stage_rows<KIND>(other, ld_other, n, j0, d, sb, nb);
@@ -180,12 +187,12 @@ dib_infonce_grad_stream_kernel(const float* __restrict__ self, int ld_self, cons
       const int j = j0 + lane;
       float s[kRowsPerWarp]; int am[kRowsPerWarp];
       tile_similarity<KIND>(sa, i0, sb, lane, d, na, nb, inv_t, s, am);
-      const float lo = j < n ? lse_other[j] : 0.f;
+      const float lo = j < n ? lse_other[(long long)j * lse_stride] : 0.f;
 #pragma unroll
       for (int r = 0; r < kRowsPerWarp; ++r) {
         const long long i = row0 + i0 + r;
         float w = 0.f, e = 0.f;
-        if (i < n && j < n) {
+        if (i < self_end && j < n) {
           w = (expf(s[r] - lr[r]) + expf(s[r] - lo) - (i == j ? 2.f : 0.f)) * inv_n;
           if (KIND == SIM_L2) e = 1.f / (-s[r] / inv_t);        // sqrt(d2 + eps) = -S T
           else if (KIND == SIM_COS) e = s[r] / inv_t;           // cos(a, b) = S T
@@ -222,9 +229,9 @@ dib_infonce_grad_stream_kernel(const float* __restrict__ self, int ld_self, cons
 #pragma unroll
   for (int r = 0; r < kRowsPerWarp; ++r) {
     const long long i = row0 + i0 + r;
-    if (i >= n) continue;
+    if (i >= self_end) continue;
     for (int k = lane; k < ld_out; k += 32)
-      d_self[i * ld_out + k] = k < d ? dib_maybe_round(acc[(i0 + r) * d + k] * inv_t, round_out) : 0.f;
+      d_self[(i - self0) * ld_out + k] = k < d ? dib_maybe_round(acc[(i0 + r) * d + k] * inv_t, round_out) : 0.f;
   }
 }
 
@@ -239,11 +246,15 @@ cudaError_t launch_loss(const DibInfonceStream& a, cudaStream_t st) {
   const size_t smem = lse_smem(d);
   cudaError_t e = cudaFuncSetAttribute(dib_infonce_lse_kernel<KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  const unsigned blocks = (unsigned)DIB_CEIL_DIV(n, kTile);
-  float *r = a.scratch, *c = a.scratch + n, *diag = a.scratch + 2 * (long long)n;
-  dib_infonce_lse_kernel<KIND><<<blocks, kThreads, smem, st>>>(a.e1, a.ld1, a.e2, a.ld2, n, d, 1.f / a.temperature, r, diag);
-  dib_infonce_lse_kernel<KIND><<<blocks, kThreads, smem, st>>>(a.e2, a.ld2, a.e1, a.ld1, n, d, 1.f / a.temperature, c, nullptr);
-  dib_infonce_stream_loss_kernel<<<1, kThreads, 0, st>>>(r, c, diag, n, a.loss_sum, a.acc_zero);
+  const unsigned blocks = (unsigned)DIB_CEIL_DIV(a.rows, (int64_t)kTile);
+  const long long r0 = a.row0, r1 = a.row0 + a.rows;
+  const int ls = a.lse_stride;
+  dib_infonce_lse_kernel<KIND><<<blocks, kThreads, smem, st>>>(a.e1, a.ld1, a.e2, a.ld2, n, d, 1.f / a.temperature, r0, r1, a.lse_r,
+                                                                ls, a.diag);
+  dib_infonce_lse_kernel<KIND><<<blocks, kThreads, smem, st>>>(a.e2, a.ld2, a.e1, a.ld1, n, d, 1.f / a.temperature, r0, r1, a.lse_c,
+                                                                ls, nullptr);
+  dib_infonce_stream_loss_kernel<<<1, kThreads, 0, st>>>(a.lse_r + r0 * ls, a.lse_c + r0 * ls, ls, a.diag, (int)a.rows, a.loss_sum,
+                                                         a.acc_zero);
   dib_note_launch(3);
   return cudaGetLastError();
 }
@@ -254,16 +265,17 @@ cudaError_t launch_grads(const DibInfonceStream& a, cudaStream_t st) {
   const size_t smem = grad_smem(d);
   cudaError_t e = cudaFuncSetAttribute(dib_infonce_grad_stream_kernel<KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  const unsigned blocks = (unsigned)DIB_CEIL_DIV(n, kTile);
-  const float *r = a.scratch, *c = a.scratch + n;
+  const unsigned blocks = (unsigned)DIB_CEIL_DIV(a.rows, (int64_t)kTile);
+  const long long r0 = a.row0, r1 = a.row0 + a.rows;
+  const float *r = a.lse_r, *c = a.lse_c;
   if (a.d_e1) {
-    dib_infonce_grad_stream_kernel<KIND><<<blocks, kThreads, smem, st>>>(a.e1, a.ld1, a.e2, a.ld2, n, d, 1.f / a.temperature, r,
-                                                                         c, a.d_e1, a.ld_d1, a.round_out);
+    dib_infonce_grad_stream_kernel<KIND><<<blocks, kThreads, smem, st>>>(a.e1, a.ld1, a.e2, a.ld2, n, d, 1.f / a.temperature, r0, r1,
+                                                                         r, c, a.lse_stride, a.d_e1, a.ld_d1, a.round_out);
     dib_note_launch();
   }
   if (a.d_e2) {
-    dib_infonce_grad_stream_kernel<KIND><<<blocks, kThreads, smem, st>>>(a.e2, a.ld2, a.e1, a.ld1, n, d, 1.f / a.temperature, c,
-                                                                         r, a.d_e2, a.ld_d2, a.round_out);
+    dib_infonce_grad_stream_kernel<KIND><<<blocks, kThreads, smem, st>>>(a.e2, a.ld2, a.e1, a.ld1, n, d, 1.f / a.temperature, r0, r1,
+                                                                         c, r, a.lse_stride, a.d_e2, a.ld_d2, a.round_out);
     dib_note_launch();
   }
   return cudaGetLastError();
@@ -272,7 +284,7 @@ cudaError_t launch_grads(const DibInfonceStream& a, cudaStream_t st) {
 }  // namespace
 
 cudaError_t dib_launch_infonce_stream_loss(const DibInfonceStream& a, cudaStream_t st) {
-  if (a.n <= 0) return cudaSuccess;
+  if (a.n <= 0 || a.rows <= 0) return cudaSuccess;
   switch (a.kind) {
     case SIM_L2SQ: return launch_loss<SIM_L2SQ>(a, st);
     case SIM_L2: return launch_loss<SIM_L2>(a, st);
@@ -283,7 +295,7 @@ cudaError_t dib_launch_infonce_stream_loss(const DibInfonceStream& a, cudaStream
 }
 
 cudaError_t dib_launch_infonce_stream_grads(const DibInfonceStream& a, cudaStream_t st) {
-  if (a.n <= 0) return cudaSuccess;
+  if (a.n <= 0 || a.rows <= 0) return cudaSuccess;
   switch (a.kind) {
     case SIM_L2SQ: return launch_grads<SIM_L2SQ>(a, st);
     case SIM_L2: return launch_grads<SIM_L2>(a, st);

@@ -91,20 +91,26 @@ cudaError_t dib_launch_similarity(int kind, const float* e1, int64_t n, const fl
 cudaError_t dib_launch_infonce_head(int kind, const float* e1, const float* e2, int64_t n, int d, float temperature,
                                     float* scratch, float* out_loss, float* d_e1, float* d_e2, cudaStream_t st);
 
-// the InfoNCE loss of DIB_LOSS_INFONCE with memory linear in n (dib_infonce_stream.cu): e1 [n, d] (ld1), e2 [n, d] (ld2), d <= 512
+// the InfoNCE loss of DIB_LOSS_INFONCE with memory linear in n (dib_infonce_stream.cu): e1 [n, d] (ld1), e2 [n, d] (ld2), d <= 512.
+// The sweeps cover the own rows [row0, row0 + rows) of both sides against all n rows of the other side (one rank of a
+// data-parallel group; row0 = 0, rows = n on one GPU).  Every index below is global unless it says otherwise.
 struct DibInfonceStream {
   int kind; float temperature;
   const float* e1; int ld1;
   const float* e2; int ld2;
   int64_t n; int d;
-  float* scratch;                  // 3n floats: row log-sum-exps | column log-sum-exps | diagonal of S
-  float* loss_sum;                 // [1] = sum_i (r_i + c_i - 2 s_ii) = n * loss
+  int64_t row0, rows;
+  float* lse_r;                    // row log-sum-exps r_i at lse_r[i * lse_stride]: written for own i, read for all i
+  float* lse_c;                    // column log-sum-exps c_j at lse_c[j * lse_stride]: likewise
+  int lse_stride;
+  float* diag;                     // [rows] s_ii of the own rows, local index
+  float* loss_sum;                 // [1] = sum_{own i} (r_i + c_i - 2 s_ii) (= n * loss on one GPU)
   float* acc_zero;                 // [1] = 0 (the accuracy slot of the stats), nullable
-  float* d_e1; int ld_d1;          // d loss / d e1, d loss / d e2 (pad columns zeroed); each nullable
-  float* d_e2; int ld_d2;
+  float* d_e1; int ld_d1;          // d loss / d e1, d loss / d e2 of the own rows at local index (pad columns zeroed); each
+  float* d_e2; int ld_d2;          // nullable
   int round_out;                   // round the gradients to the TF32 grid (tensor-core operands)
 };
-// the row / column sweeps and the loss; then (after it, reading its scratch) the two gradient sweeps
+// the row / column sweeps and the loss; then (after it, reading r and c of all n rows) the two gradient sweeps
 cudaError_t dib_launch_infonce_stream_loss(const DibInfonceStream& a, cudaStream_t st);
 cudaError_t dib_launch_infonce_stream_grads(const DibInfonceStream& a, cudaStream_t st);
 

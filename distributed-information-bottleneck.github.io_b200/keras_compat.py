@@ -97,12 +97,21 @@ class InfoNCE(_Loss):
     activation_fn)`` for every width of ``y_encoder_architecture``, then a linear ``Dense(output_dimensionality)``
     (train.py:186-193) -- on the symmetric InfoNCE of train.py:201-213 between ``model(x)`` and ``output_encoder(y)``:
     ``mean_i CE(i, S[i,:]) + mean_i CE(i, S^T[i,:])`` with ``S = get_scaled_similarity(., ., similarity, temperature)``.
-    Defaults are train.py:55-62's.  ``y_dimensionality`` is the width of y (it sizes the output encoder)."""
+    Defaults are train.py:55-62's.  ``y_dimensionality`` is the width of y (it sizes the output encoder).
+
+    ``negatives`` says which rows are the negatives of a row when the model is data parallel, because that choice changes
+    the loss.  ``'global'``: all other rows of the global batch, so N processes compute exactly the one-process loss of that
+    batch (DESIGN.md section 7).  ``None`` (default): no choice made; one process trains as always, and a process group of
+    more than one rank is refused."""
     kind = "infonce"
 
-    def __init__(self, y_dimensionality, y_encoder_architecture=(128, 128), similarity="l2", temperature=1.0, name=None):
+    def __init__(self, y_dimensionality, y_encoder_architecture=(128, 128), similarity="l2", temperature=1.0, name=None,
+                 negatives=None):
         from .utils import SIMILARITY_TYPES
         super().__init__(from_logits=True, name=name)
+        if negatives not in (None, "global"):
+            raise ValueError(f"negatives must be None or 'global', got {negatives!r}")
+        self.negatives = negatives
         if similarity not in SIMILARITY_TYPES:
             raise ValueError(f"similarity must be one of {sorted(SIMILARITY_TYPES)}, got {similarity!r}")
         if not float(temperature) > 0:

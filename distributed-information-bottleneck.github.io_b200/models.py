@@ -542,17 +542,73 @@ class DistributedIBNet:
         self._step_dev_active = on
 
     def _backward(self, x, y, global_batch, eps=None, sample_offset=0, step=None, device_step=False):
-        """dib_train_step: forward + reverse mode into self._gradstats = [grads (P) || stats (F+3)]."""
+        """dib_train_step: forward + reverse mode into self._gradstats = [grads (P) || stats (F+3)].  InfoNCE with more than
+        one rank: the three shard phases with the two all-gathers between them (DESIGN.md section 7)."""
         n = x.shape[0]
         self._ensure_handle(n)
         P = self._P
         self._set_device_step(device_step)
         st = 0 if device_step else (self._train_step_count if step is None else step)
+        world, rank = parallel.world_and_rank(self.process_group)
+        if self._infonce is not None and world > 1:
+            n_global, row_offset = self._infonce_shard(n, global_batch, world, rank)
+            e_all, lse_all = self._infonce_buffers(n_global)
+            self._infonce_forward(x, y, e_all, n_global, row_offset, eps, st, sample_offset, training=True)
+            parallel.all_gather_rows_(e_all, self.process_group)
+            self._infonce_lse(n, e_all, lse_all, n_global, row_offset, self._gradstats[P:])
+            parallel.all_gather_rows_(lse_all, self.process_group)
+            self._infonce_backward(x, e_all, lse_all, n_global, row_offset, eps, st, sample_offset)
+            return
         _lib.check(self._lib.dib_train_step(
             self._handle, _lib.ptr(self._params), _lib.ptr(x), _lib.ptr(y), n, _lib.ptr(self.beta._dev),
             1.0 / float(global_batch), _lib.ptr(eps), self.noise_seed, int(st) & 0xFFFFFFFF,
             int(sample_offset), _lib.ptr(self._gradstats), _lib.ptr(self._gradstats[P:]), _lib.ptr(self._workspace),
             _stream()))
+
+    # ------------------------------------------------------------------ InfoNCE with global negatives on several ranks
+    def _check_infonce_world(self, nce, batch_size=None):
+        """Refuse, before any device work or collective, what data-parallel InfoNCE cannot do."""
+        world, _ = parallel.world_and_rank(self.process_group)
+        if world == 1:
+            return
+        if nce.negatives is None:
+            raise NotImplementedError(
+                "losses.InfoNCE couples every row of the global batch, so with more than one rank the negatives of a row must "
+                "be chosen: compile with losses.InfoNCE(..., negatives='global') to all-gather the embeddings of the global "
+                "batch and train on exactly the one-process loss")
+        if batch_size is not None and int(batch_size) % world:
+            raise ValueError(f"InfoNCE with negatives='global' needs equal shards: batch_size {batch_size} is not a multiple "
+                             f"of the {world} ranks")
+
+    def _infonce_shard(self, n, global_batch, world, rank):
+        """(n_global, row_offset) of this rank's n rows: equal shards, rank r owns rows [r n, (r + 1) n)."""
+        self._check_infonce_world(self._infonce)
+        if global_batch is not None and int(global_batch) != world * n:
+            raise ValueError(f"InfoNCE with negatives='global' needs equal shards: global_batch {global_batch} != "
+                             f"{world} ranks x {n} rows")
+        return world * n, rank * n
+
+    def _infonce_buffers(self, n_global):
+        """e_all [n_global, 2 d] = (e1 || e2) per row and lse_all [n_global, 2] = (r, c) per row."""
+        d = self.output_dimensionality
+        return (torch.empty(n_global, 2 * d, dtype=torch.float32, device=self.device),
+                torch.empty(n_global, 2, dtype=torch.float32, device=self.device))
+
+    def _infonce_forward(self, x, y, e_all, n_global, row_offset, eps, step, sample_offset, training):
+        _lib.check(self._lib.dib_infonce_shard_forward(
+            self._handle, _lib.ptr(self._params), _lib.ptr(x), _lib.ptr(y), x.shape[0], int(training), _lib.ptr(eps),
+            self.noise_seed, int(step) & 0xFFFFFFFF, int(sample_offset), _lib.ptr(e_all), n_global, row_offset,
+            _lib.ptr(self._workspace), _stream()))
+
+    def _infonce_lse(self, n, e_all, lse_all, n_global, row_offset, stats_out):
+        _lib.check(self._lib.dib_infonce_shard_lse(self._handle, _lib.ptr(e_all), n_global, row_offset, n, _lib.ptr(lse_all),
+                                                   _lib.ptr(stats_out), _lib.ptr(self._workspace), _stream()))
+
+    def _infonce_backward(self, x, e_all, lse_all, n_global, row_offset, eps, step, sample_offset):
+        _lib.check(self._lib.dib_infonce_shard_backward(
+            self._handle, _lib.ptr(self._params), _lib.ptr(x), x.shape[0], _lib.ptr(self.beta._dev), _lib.ptr(eps),
+            self.noise_seed, int(step) & 0xFFFFFFFF, int(sample_offset), _lib.ptr(e_all), _lib.ptr(lse_all), n_global,
+            row_offset, _lib.ptr(self._gradstats), _lib.ptr(self._workspace), _stream()))
 
     def apply_gradients(self, flat_grads):
         """optimizer.apply_gradients(zip(grads, model.trainable_variables)) of the custom loops (train.py:217-219,
@@ -607,7 +663,8 @@ class DistributedIBNet:
     def _capture_step(self, key):
         """Capture the step for one (n, global_batch, sample_offset, world) into CUDA graphs.  Single GPU: ONE graph
         (forward + backward + Adam + noise-step increment).  Data parallel: two graphs (backward | Adam) with the NCCL all-reduce
-        issued eagerly between them.  Inputs are copied into static buffers before each replay; beta,
+        issued eagerly between them; InfoNCE: four graphs (the three shard phases | Adam) with the two all-gathers and the
+        all-reduce issued eagerly between them, and e_all / lse_all kept with the graphs.  Inputs are copied into static buffers before each replay; beta,
         learning rate, the Adam step and the Philox step are device scalars, so nothing by-value changes between replays."""
         n, global_batch, sample_offset, world = key
         D = sum(self.feature_dimensionalities)
@@ -633,8 +690,18 @@ class DistributedIBNet:
                     self._adam()
                     self._noise_step_dev.add_(1)
 
+                nce = None
                 if world == 1:
                     cap(lambda: (self._backward(gx, gy, global_batch, None, sample_offset, device_step=True), tail()))
+                elif self._infonce is not None:     # phase 1 | all-gather | phase 2 | all-gather | phase 3 | all-reduce | tail
+                    _, rank = parallel.world_and_rank(self.process_group)
+                    n_global, row_offset = self._infonce_shard(n, global_batch, world, rank)
+                    e_all, lse_all = self._infonce_buffers(n_global)
+                    nce = dict(e_all=e_all, lse_all=lse_all)
+                    cap(lambda: self._infonce_forward(gx, gy, e_all, n_global, row_offset, None, 0, sample_offset, True))
+                    cap(lambda: self._infonce_lse(n, e_all, lse_all, n_global, row_offset, self._gradstats[self._P:]))
+                    cap(lambda: self._infonce_backward(gx, e_all, lse_all, n_global, row_offset, None, 0, sample_offset))
+                    cap(tail)
                 else:        # one all-reduce between backward and optimizer: two graphs
                     cap(lambda: self._backward(gx, gy, global_batch, None, sample_offset, device_step=True))
                     cap(tail)
@@ -648,7 +715,7 @@ class DistributedIBNet:
             self._graph_failed = True
             self._set_device_step(False)
             return None
-        g = dict(graphs=graphs, x=gx, y=gy, launches=int(self._lib.dib_launch_count()) - launches0)
+        g = dict(graphs=graphs, x=gx, y=gy, launches=int(self._lib.dib_launch_count()) - launches0, nce=nce)
         self._graphs[key] = g
         return g
 
@@ -661,6 +728,14 @@ class DistributedIBNet:
         g["y"].copy_(y.reshape(g["y"].shape), non_blocking=True)
         if world == 1:
             g["graphs"][0].replay()
+        elif g["nce"] is not None:
+            g["graphs"][0].replay()
+            parallel.all_gather_rows_(g["nce"]["e_all"], self.process_group)
+            g["graphs"][1].replay()
+            parallel.all_gather_rows_(g["nce"]["lse_all"], self.process_group)
+            g["graphs"][2].replay()
+            parallel.allreduce_sum_(self._gradstats, self.process_group)
+            g["graphs"][3].replay()
         else:
             g["graphs"][0].replay()
             parallel.allreduce_sum_(self._gradstats, self.process_group)
@@ -675,7 +750,10 @@ class DistributedIBNet:
             xd = self._to_device(x, sum(self.feature_dimensionalities))
             yd = self._targets(y)
             e = self._to_device(eps) if eps is not None else None
-            self._backward(xd, yd, global_batch or max(xd.shape[0], 1), e, sample_offset, step)
+            if not global_batch:            # InfoNCE on several ranks: every rank passes its equal shard of the global batch
+                nce_world = parallel.world_and_rank(self.process_group)[0] if self._infonce is not None else 1
+                global_batch = max(xd.shape[0] * nce_world, 1)
+            self._backward(xd, yd, global_batch, e, sample_offset, step)
             return self._gradstats[:self._P].clone(), self._gradstats[self._P:].clone()
 
     # ------------------------------------------------------------------ encoder-only custom steps (SURVEY 8f3)
@@ -785,7 +863,7 @@ class DistributedIBNet:
             if self.output_activation_fn is not None:
                 raise ValueError("losses.InfoNCE needs output_activation_fn=None: the prediction is the InfoNCE embedding "
                                  "(train.py:117)")
-            self._check_single_rank()
+            self._check_infonce_world(loss)
         for m in (metrics or []):
             if m not in ("accuracy", "acc"):
                 raise ValueError(f"only metrics=['accuracy'] is implemented (reference data.py:67), got {m!r}")
@@ -795,12 +873,6 @@ class DistributedIBNet:
         self.compiled_metrics_names = ["accuracy" for _ in (metrics or [])]
         self._lr_host = None
         self._sync_lr()
-
-    def _check_single_rank(self):
-        if parallel.world_and_rank(self.process_group)[0] > 1:
-            raise NotImplementedError(
-                "losses.InfoNCE couples every row of the global batch; data-parallel InfoNCE needs an all-gather of both "
-                "embeddings and is not implemented: train it in a process group of one rank")
 
     def _sync_lr(self):
         """Device copy of optimizer.learning_rate (the step kernels read it from memory so that a schedule needs no re-capture);
@@ -891,7 +963,9 @@ class DistributedIBNet:
         error) and validation takes floor(Nv / batch_size) + 1 full batches from the repeated validation permutation.
         History keys are loss (= InfoNCE + beta * sum KL, so ``loss - beta * sum KL`` is the InfoNCE term), KL{i}, beta and
         their val_ twins.  beta follows the annealing callback's on_epoch_begin, i.e. it is set before an epoch's first
-        step; the reference's custom loop assigns it after that step (train.py:245-250), one step late.  One process only."""
+        step; the reference's custom loop assigns it after that step (train.py:245-250), one step late.  With more than one
+        rank it needs ``losses.InfoNCE(..., negatives='global')`` and a batch_size that is a multiple of the number of ranks:
+        every rank then trains on its equal shard of the same global batches and the result is the one-process result."""
         if self.optimizer is None:
             raise RuntimeError("call compile() first")
         batch_size = 32 if batch_size is None else int(batch_size)
@@ -899,7 +973,7 @@ class DistributedIBNet:
         D = sum(self.feature_dimensionalities)
         nce = self._infonce is not None
         if nce:
-            self._check_single_rank()
+            self._check_infonce_world(self._infonce, batch_size)
         with torch.cuda.device(self.device):
             xd, yd = self._to_device(x, D), self._targets(y)
             N = xd.shape[0]
@@ -922,10 +996,11 @@ class DistributedIBNet:
                 if shuffle:
                     perm = self.epoch_permutation(epoch, N)
                 self._epoch_acc.zero_()
-                if nce:                                                      # full batches only, one process
+                if nce:                                                      # full batches only, equal shards
                     for b0, b1 in plan:
-                        idx = perm[b0:b1] if shuffle else slice(b0, b1)
-                        self._metrics_update(self._train_step(xd[idx], yd[idx], global_batch=b1 - b0))
+                        lo, hi = parallel.shard_range(b1 - b0, rank, world)
+                        idx = perm[b0 + lo:b0 + hi] if shuffle else slice(b0 + lo, b0 + hi)
+                        self._metrics_update(self._train_step(xd[idx], yd[idx], global_batch=b1 - b0, sample_offset=lo))
                 else:
                     for b0 in range(0, N, batch_size):
                         b1 = min(b0 + batch_size, N)
@@ -939,7 +1014,7 @@ class DistributedIBNet:
                         self._metrics_update(stats)
                 logs = self._read_epoch_logs()
                 if xv is not None and nce:
-                    logs.update(self._evaluate_infonce_into_logs(xv, yv, batch_size, epoch, (2 ** 31 + epoch)))
+                    logs.update(self._evaluate_infonce_into_logs(xv, yv, batch_size, epoch, (2 ** 31 + epoch), world, rank))
                 elif xv is not None:
                     logs.update(self._evaluate_into_logs(xv, yv, batch_size, epoch, world, rank))
                 if verbose not in (False, 0) and rank == 0:          # 'auto' -> 1 like Keras outside notebooks
@@ -966,18 +1041,30 @@ class DistributedIBNet:
             self._metrics_update(stats)
         return self._read_epoch_logs(prefix="val_")
 
-    def _evaluate_infonce_into_logs(self, xv, yv, batch_size, perm_key, step):
+    def _evaluate_infonce_into_logs(self, xv, yv, batch_size, perm_key, step, world=1, rank=0):
         """InfoNCE validation (train.py:233-234, 264-270): floor(Nv / B) + 1 full batches drawn from the repeated validation
-        permutation (:func:`infonce_validation_batches`), noise keyed by (step, position in the repeated stream)."""
-        Nv = xv.shape[0]
-        pos = torch.from_numpy(infonce_validation_batches(Nv, batch_size)).to(self.device)
+        permutation (:func:`infonce_validation_batches`), noise keyed by (step, position in the repeated stream).  With more
+        than one rank each rank runs its equal shard of every batch through the first two shard phases and the statistics are
+        summed over the ranks."""
+        Nv, B = xv.shape[0], int(batch_size)
+        pos = torch.from_numpy(infonce_validation_batches(Nv, B)).to(self.device)
         idx_all = self.validation_permutation(perm_key, Nv)[pos]
         self._epoch_acc.zero_()
         stats = torch.empty(self.number_features + 3, dtype=torch.float32, device=self.device)
+        lo, hi = parallel.shard_range(B, rank, world)
         for k in range(idx_all.shape[0]):
             idx = idx_all[k]
-            self._forward(xv.index_select(0, idx), yv.index_select(0, idx), None, step, k * int(batch_size), want_pred=False,
-                          stats_out=stats)
+            if world == 1:
+                self._forward(xv.index_select(0, idx), yv.index_select(0, idx), None, step, k * B, want_pred=False,
+                              stats_out=stats)
+            else:
+                xs, ys = xv.index_select(0, idx[lo:hi]), yv.index_select(0, idx[lo:hi])
+                self._ensure_handle(hi - lo)
+                e_all, lse_all = self._infonce_buffers(B)
+                self._infonce_forward(xs, ys, e_all, B, lo, None, step, k * B + lo, training=False)
+                parallel.all_gather_rows_(e_all, self.process_group)
+                self._infonce_lse(hi - lo, e_all, lse_all, B, lo, stats)
+                parallel.allreduce_sum_(stats, self.process_group)
             self._metrics_update(stats)
         return self._read_epoch_logs(prefix="val_")
 
@@ -994,8 +1081,9 @@ class DistributedIBNet:
             self._inference_calls += 1           # a fresh noise draw per evaluate() call
             key = (1 << 29) | (self._inference_calls & 0x1FFFFFFF)
             if self._infonce is not None:
-                self._check_single_rank()
-                logs = self._evaluate_infonce_into_logs(self._to_device(x, D), self._targets(y), int(batch_size), key, key)
+                self._check_infonce_world(self._infonce, batch_size)
+                logs = self._evaluate_infonce_into_logs(self._to_device(x, D), self._targets(y), int(batch_size), key, key,
+                                                        world, rank)
             else:
                 logs = self._evaluate_into_logs(self._to_device(x, D), self._to_device(y, self._y_cols()), int(batch_size),
                                                 key, world, rank)

@@ -23,6 +23,22 @@ def shard_range(n, rank, world):
     return lo, hi
 
 
+def all_gather_rows_(buf: torch.Tensor, group=None):
+    """In-place all-gather of a rank-contiguous buffer: ``buf`` holds world equal row blocks, rank r has filled block r, and
+    afterwards every rank holds all of them.  No-op for a single process."""
+    if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
+        return buf
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    if buf.shape[0] % world:
+        raise ValueError(f"all_gather_rows_: {buf.shape[0]} rows do not split into {world} equal blocks")
+    blocks = list(buf.chunk(world))
+    if dist.get_backend(group) == "nccl":
+        dist.all_gather_into_tensor(buf, blocks[rank], group=group)
+    else:                                    # gloo: list all-gather; the own block goes in as a copy
+        dist.all_gather(blocks, blocks[rank].clone(), group=group)
+    return buf
+
+
 def allreduce_sum_(flat: torch.Tensor, group=None):
     """In-place sum over the data-parallel group on the current stream; no-op for a single process."""
     if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:

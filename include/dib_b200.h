@@ -196,6 +196,36 @@ int dib_train_step(dib_model* h, const float* params, const float* x, const floa
                    const float* eps, uint64_t seed, uint32_t step, uint64_t sample_offset,
                    float* grads_flat, float* out_stats, void* workspace, void* stream);
 
+/* dib_train_step of a DIB_LOSS_INFONCE model on one rank of a data-parallel group whose negatives are all rows of the GLOBAL
+ * batch (train.py:203-219 on that batch: every rank computes the one-GPU loss and gradient).  The rank owns the n global rows
+ * [row_offset, row_offset + n) of an n_global-row batch; the step runs as three phases with two exchanges between them that
+ * the caller does (DESIGN.md section 7):
+ *   1. dib_infonce_shard_forward (train.py:201-202, 209-210: model(x), output_encoder(y)): writes
+ *      e_all[row_offset + i] = (e1_i || e2_i), e_all [n_global, 2 * output_dimensionality] row-major.
+ *      -> the caller all-gathers e_all.
+ *   2. dib_infonce_shard_lse (train.py:203-213): from all rows of e_all, the row log-sum-exps r_i of the own e1 rows and the
+ *      column log-sum-exps c_j of the own e2 rows into lse_all[row_offset + i] = (r_i, c_i), lse_all [n_global, 2];
+ *      out_stats [dib_stats_count] = KL sums of the own rows | sum_own (r_i + c_i - 2 s_ii) | 0 | n.
+ *      -> the caller all-gathers lse_all.
+ *   3. dib_infonce_shard_backward (train.py:216-220): d e1 of the own rows against all columns and d e2 of the own rows against
+ *      all rows (weights (...) / n_global), the model's and the output encoder's backward, KL means over n_global:
+ *      grads_flat [P] = this rank's share; the sum over ranks is the one-GPU gradient of the global batch.
+ *      -> the caller all-reduces [grads || stats], then runs the optimizer.
+ * Noise is keyed by sample_offset as in dib_train_step; dib_set_noise_step_device applies to phase 1 with training != 0 and to
+ * phase 3 (phase 1 with training == 0 is the validation forward of dib_forward).  Phases 2 and 3 read what the phases before
+ * them left in the workspace: run them in order on the same handle, workspace and inputs, with no other call on the handle in
+ * between.  With row_offset = 0 and n = n_global the three phases are dib_train_step bit for bit.  Caller-owned buffers, the
+ * caller's stream, no host sync.  Needs 1 <= n <= max_batch, row_offset + n <= n_global < 2^31, e_all and lse_all 16-byte
+ * aligned. */
+int dib_infonce_shard_forward(dib_model* h, const float* params, const float* x, const float* y, int64_t n, int32_t training,
+                              const float* eps, uint64_t seed, uint32_t step, uint64_t sample_offset, float* e_all,
+                              int64_t n_global, int64_t row_offset, void* workspace, void* stream);
+int dib_infonce_shard_lse(dib_model* h, const float* e_all, int64_t n_global, int64_t row_offset, int64_t n, float* lse_all,
+                          float* out_stats, void* workspace, void* stream);
+int dib_infonce_shard_backward(dib_model* h, const float* params, const float* x, int64_t n, const float* beta_dev, const float* eps,
+                               uint64_t seed, uint32_t step, uint64_t sample_offset, const float* e_all, const float* lse_all,
+                               int64_t n_global, int64_t row_offset, float* grads_flat, void* workspace, void* stream);
+
 /* NEXT ROW f3 -- encoder-only custom steps (nb-particle cell 8: a shared particle encoder feeding the caller's own
  * network, e.g. a set transformer; nb-chaos cell 10): the model's integration network is not used.
  *   dib_encoders_forward : x [n, sum d_i] -> out_emb [n, F*E] (u = mu + exp(logvar/2) eps) and out_stats (KL sums; loss = acc = 0).
