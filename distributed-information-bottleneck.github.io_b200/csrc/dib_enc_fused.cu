@@ -6,8 +6,9 @@
 //     x column -> positional encoding -> Dense(128,act) -> Dense(128,act) -> Dense(2E) -> split (mu, logvar)
 //     -> u = mu + exp(logvar/2) eps -> KL partial sums -> emb[:, f*E:(f+1)*E]
 // runs on chip: the three contractions are wgmma instructions (16-bit operands with an 11-bit significand = TF32's, fp32
-// accumulation in registers), the activations travel registers -> shared memory (as the next MMA's swizzled A operand)
-// and never touch HBM.  Only x (4 B/sample/feature) is read and emb is written.
+// accumulation in registers), the activations stay in registers (forward: the next MMA's register A operand) or travel
+// registers -> shared memory (backward: swizzled operand tiles) and never touch HBM.  Only x (4 B/sample/feature) is read
+// and emb is written.
 //
 // Two warpgroups per CTA; warpgroup g owns rows [64 g, 64 g + 64) of a tile (wgmma M = 64).  Every contraction whose
 // reduction runs over the hidden features (forward, dgrad) reads only the warpgroup's own rows, so the two warpgroups
@@ -49,14 +50,17 @@ constexpr int kOffW2 = kOffW1 + 2 * kPanel;        // 32 KB
 constexpr int kOffW0 = kOffW2 + kPanel;            // 16 KB
 constexpr int kOffBb1 = kOffW0 + 2 * K0 * 128;     // 4 KB : W0p = 2 panels x 16 rows x 128 B
 constexpr int kOffBb2 = kOffBb1 + 2 * K0 * 128;    // 4 KB : Bb1 likewise
+constexpr int kA0Bytes = 2 * TM * 16;              // A0 = [2 k-halves][128 rows][16 B] (no swizzle)
 constexpr int kOffA0 = kOffBb2 + K0 * 128;         // 2 KB : Bb2 = 1 panel x 16 rows x 128 B
-constexpr int kOffH1 = kOffA0 + 2 * TM * 16 + 2048;// 4 KB : A0 = [2 k-halves][128 rows][16 B] (no swizzle); +2 KB keeps 1024-alignment
-constexpr int kOffFwdEnd = kOffH1 + 2 * kPanel;    // forward: h2 overwrites h1 (the layer-1 MMA that read it has retired)
-// backward-only tiles
+constexpr int kOffX = kOffA0 + 2 * kA0Bytes;       // 8 KB : two A0 buffers (the backward alternates them; the forward uses one)
+constexpr int kOffFwdEnd = kOffX + kThreads * 16;  // 4 KB : x ring, one 16-byte slot per thread (see prefetch_x)
+// backward-only tiles (the forward keeps h1 / h2 in registers)
+constexpr int kOffH1 = kOffFwdEnd;
 constexpr int kOffH2 = kOffH1 + 2 * kPanel;        // h2, later dz1
 constexpr int kOffDO = kOffH2 + 2 * kPanel;        // [128 x 64] d(mu | logvar), one panel
 constexpr int kOffDZ2 = kOffDO + kPanel;           // [128 x 128]
-constexpr int kOffBwdEnd = kOffDZ2 + 2 * kPanel;
+constexpr int kOffG = kOffDZ2 + 2 * kPanel;        // [128 rows][32] 16-bit d_emb16 of the next tile (TMA, no swizzle)
+constexpr int kOffBwdEnd = kOffG + TM * 64;
 static_assert(kOffH1 % 1024 == 0 && kOffDZ2 % 1024 == 0, "operand tiles must be 1024-byte aligned");
 
 struct EncFusedParams {
@@ -142,6 +146,20 @@ __device__ __forceinline__ void frag_to_tile(const float (&d)[N / 2], uint32_t t
   }
 }
 
+// the same activation, kept in registers as the next MMA's A operand: the accumulator fragment of 8-column block j is the
+// A fragment half i = j % 2 of k step j / 2, so a[4 kk .. 4 kk + 3] is the A operand of k step kk (see wgmma_m64n128k16_rs)
+template <bool BF16, bool RELU, int N>
+__device__ __forceinline__ void frag_to_a(const float (&d)[N / 2], uint32_t (&a)[N / 4], int act, float alpha) {
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const float v0 = d[4 * j + 2 * h], v1 = d[4 * j + 2 * h + 1];
+      a[2 * j + h] = RELU ? pack2_relu<BF16>(v0, v1) : pack2<BF16>(dib_act16(act, v0, alpha), dib_act16(act, v1, alpha));
+    }
+  }
+}
+
 // packed 16-bit pair p * (h > 0): relu' applied to two gradients at once (exact: multiplication by 1.0 / 0.0)
 template <bool BF16>
 __device__ __forceinline__ uint32_t relu_gate2(uint32_t p, uint32_t h) {
@@ -192,10 +210,6 @@ __device__ __forceinline__ float dib_sin_pe(float a) {
   return __sinf(6.283185307179586f * t);
 }
 constexpr int kMaxFeatDim = 3;     // d * nfreq + 1 <= 16 and nfreq >= 1
-__device__ __forceinline__ void load_x(const float* xrow, int d, float (&xv)[kMaxFeatDim]) {
-#pragma unroll
-  for (int j = 0; j < kMaxFeatDim; ++j) xv[j] = (xrow && j < d) ? xrow[j] : 0.f;
-}
 template <bool BF16>
 __device__ __forceinline__ void write_a0_row(uint32_t a0, int r, int khalf, bool valid, const float (&xv)[kMaxFeatDim], int d,
                                              int nfreq) {
@@ -222,12 +236,32 @@ __device__ __forceinline__ void write_a0_row(uint32_t a0, int r, int khalf, bool
 }
 
 // the [pe|1] operand of one tile: thread t of the CTA stages (row 64 g + t % 64, k-half (t / 64) % 2) of its own warpgroup g
+__device__ __forceinline__ int a0_row(int tid) { return 64 * (tid >> 7) + (tid & 63); }
+
+// The x values a thread stages for the tile at row0 are copied into its own 16-byte slot `xs` of the x ring by cp.async
+// one tile ahead, so no global-load latency sits in front of stage_a0.  Rows past the batch end copy nothing.  (A TMA
+// box cannot do this: the row pitch ldx * 4 B need not be a multiple of 16.)
+__device__ __forceinline__ void prefetch_x(const EncFusedParams& P, uint32_t xs, int tid, long long row0, int d, int xo) {
+  const long long grow = row0 + a0_row(tid);
+  if (grow < P.n) {
+    const float* src = P.x + grow * P.ldx + xo;
+#pragma unroll
+    for (int j = 0; j < kMaxFeatDim; ++j)
+      if (j < d) cp_async_4(xs + 4 * j, src + j);
+  }
+  cp_async_commit();
+}
+// Waits for this thread's prefetch_x of the tile (slot xslot) and writes its part of [pe|1].  The slot may be refilled
+// (prefetch_x of the next tile) as soon as this returns: its values have been consumed by the shared-memory stores.
 template <bool BF16>
-__device__ __forceinline__ void stage_a0(const EncFusedParams& P, uint32_t a0, int tid, long long row0, int d, int xo) {
-  const int ar = 64 * (tid >> 7) + (tid & 63), khalf = (tid >> 6) & 1;
+__device__ __forceinline__ void stage_a0(const EncFusedParams& P, uint32_t a0, const float* xslot, int tid, long long row0,
+                                         int d) {
+  const int ar = a0_row(tid), khalf = (tid >> 6) & 1;
   const long long grow = row0 + ar;
+  cp_async_wait_all();
   float xv[kMaxFeatDim];
-  load_x(grow < P.n ? P.x + grow * P.ldx + xo : nullptr, d, xv);
+#pragma unroll
+  for (int j = 0; j < kMaxFeatDim; ++j) xv[j] = (grow < P.n && j < d) ? xslot[j] : 0.f;
   write_a0_row<BF16>(a0, ar, khalf, grow < P.n, xv, d, P.nfreq);
 }
 
@@ -311,6 +345,25 @@ __device__ __forceinline__ void mma_layer2(float (&d)[32], uint32_t sb, uint32_t
   for (int kk = 0; kk < HID / 16; ++kk)
     wgmma_m64n64k16<BF16, 0, 1>(d, desc_act_as_a(h2, wg, kk), gmma_desc(sb + kOffW2 + kk * 2048, kPanel, 1024), 1u);
 }
+// the same with h1 / h2 as register A operands (frag_to_a); same operands, same k order into the accumulator
+template <bool BF16>
+__device__ __forceinline__ void mma_layer1_rs(float (&d)[64], uint32_t sb, const uint32_t (&h1)[32], uint32_t a0, int wg) {
+  wgmma_m64n128k16<BF16, 0, 1>(d, desc_a0_as_a(a0, wg), gmma_desc(sb + kOffBb1, K0 * 128, 1024), 0u);
+#pragma unroll
+  for (int kk = 0; kk < HID / 16; ++kk) {
+    const uint32_t a[4] = {h1[4 * kk], h1[4 * kk + 1], h1[4 * kk + 2], h1[4 * kk + 3]};
+    wgmma_m64n128k16_rs<BF16, 1>(d, a, gmma_desc(sb + kOffW1 + kk * 2048, kPanel, 1024), 1u);
+  }
+}
+template <bool BF16>
+__device__ __forceinline__ void mma_layer2_rs(float (&d)[32], uint32_t sb, const uint32_t (&h2)[32], uint32_t a0, int wg) {
+  wgmma_m64n64k16<BF16, 0, 1>(d, desc_a0_as_a(a0, wg), gmma_desc(sb + kOffBb2, K0 * 128, 1024), 0u);
+#pragma unroll
+  for (int kk = 0; kk < HID / 16; ++kk) {
+    const uint32_t a[4] = {h2[4 * kk], h2[4 * kk + 1], h2[4 * kk + 2], h2[4 * kk + 3]};
+    wgmma_m64n64k16_rs<BF16, 1>(d, a, gmma_desc(sb + kOffW2 + kk * 2048, kPanel, 1024), 1u);
+  }
+}
 
 // shared tile written by this warpgroup -> visible to its MMAs
 __device__ __forceinline__ void wg_publish(int wg) {
@@ -332,8 +385,8 @@ __device__ __forceinline__ Sched sched_of(int c, int G, int F) {
 }
 
 // ====================================================================================================
-// forward: x -> emb, KL partial sums.  96 KB of shared memory -> two CTAs per SM, so one CTA's epilogue overlaps the
-// other's MMAs.
+// forward: x -> emb, KL partial sums.  71 KB of shared memory, at most 128 registers -> two CTAs per SM, so one CTA's
+// epilogue overlaps the other's MMAs.  h1 and h2 never leave registers: each is the register A operand of the next layer.
 // ====================================================================================================
 template <bool BF16, bool RELU>
 __global__ void __launch_bounds__(kThreads, 2)
@@ -349,7 +402,8 @@ dib_enc_fused_fwd_kernel(const __grid_constant__ WeightMaps maps, const EncFused
   const int F = P.F;
   const int ntiles = (int)((P.n + TM - 1) / TM);
   const unsigned int nstep = P.step + (P.step_dev ? P.step_dev[0] : 0u);
-  const uint32_t a0 = sb + kOffA0, hbuf = sb + kOffH1;
+  const uint32_t a0 = sb + kOffA0, xs = sb + kOffX + tid * 16;
+  const float* xslot = reinterpret_cast<const float*>(sg + kOffX + tid * 16);
 
   if (tid == 0) {
     tma_prefetch_desc(&maps.w0); tma_prefetch_desc(&maps.w1); tma_prefetch_desc(&maps.w2);
@@ -364,30 +418,31 @@ dib_enc_fused_fwd_kernel(const __grid_constant__ WeightMaps maps, const EncFused
   for (int f = s.f_first; f < F; f += s.f_step, ++fit) {
     if (tid == 0) load_weights(sb, maps, bar_w, f);
     const int d = P.fdim[f], xo = P.x_off[f];
+    prefetch_x(P, xs, tid, (long long)s.slot * TM, d, xo);
     float kl_acc = 0.f;
     mbar_wait(bar_w, fit & 1);
     for (int t = s.slot; t < ntiles; t += s.nslots) {
       const long long row0 = (long long)t * TM;
-      stage_a0<BF16>(P, a0, tid, row0, d, xo);
-      wg_publish(wg);
+      stage_a0<BF16>(P, a0, xslot, tid, row0, d);
+      prefetch_x(P, xs, tid, row0 + (long long)s.nslots * TM, d, xo);
+      wg_publish(wg);       // a0 rows of this warpgroup are read only by its own MMAs, which retired in the previous tile
       float acc[64];
+      uint32_t ha[32];
       wgmma_fence();
       mma_layer0<BF16>(acc, sb, a0, wg);
       wgmma_commit();
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
-      frag_to_tile<BF16, RELU, 128>(acc, hbuf, fr, P.act, P.alpha);
-      wg_publish(wg);
+      frag_to_a<BF16, RELU, 128>(acc, ha, P.act, P.alpha);
       wgmma_fence();
-      mma_layer1<BF16>(acc, sb, hbuf, a0, wg);
+      mma_layer1_rs<BF16>(acc, sb, ha, a0, wg);
       wgmma_commit();
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
-      frag_to_tile<BF16, RELU, 128>(acc, hbuf, fr, P.act, P.alpha);      // h2 over h1
-      wg_publish(wg);
+      frag_to_a<BF16, RELU, 128>(acc, ha, P.act, P.alpha);               // h2 over h1
       float acc2[32];
       wgmma_fence();
-      mma_layer2<BF16>(acc2, sb, hbuf, a0, wg);
+      mma_layer2_rs<BF16>(acc2, sb, ha, a0, wg);
       wgmma_commit();
       // the noise of this thread's 2 rows x 8 embedding dims while layer 2 runs
       const long long grow_lo = row0 + fr.rb;
@@ -443,69 +498,94 @@ dib_enc_fused_fwd_kernel(const __grid_constant__ WeightMaps maps, const EncFused
 //   (bias gradients = the ones column of [pe|1] used as the B operand: column sums for free)
 // S is a power-of-two loss scale that keeps the 16-bit gradient operands in range (fp16); the fp32 accumulators are
 // multiplied by 1/S when they are flushed.  The weight-gradient accumulators live in registers for the whole feature:
-// warpgroup g owns rows [64 g, 64 g + 64) of dW1, dW2 (and of dW0^T, db1); warpgroup 0 stores db2.  176 KB of shared
+// warpgroup g owns rows [64 g, 64 g + 64) of dW1, dW2 (and of dW0^T, db1); warpgroup 0 stores db2.  190 KB of shared
 // memory: one CTA per SM.
+//
+// The tensor pipe is kept busy across the epilogues of the serial chain:
+//   * in each backward layer the dgrad MMAs and the weight-gradient MMAs are two commit groups; the dz epilogue waits only
+//     for the first, and the wait for the second sits just before the CTA barrier that follows (dz1 is written over h2,
+//     which the other warpgroup's dW2 reads; that wait keeps the write behind every dW2 of the tile);
+//   * dW0 of tile t retires under the start of tile t + 1: [pe|1] is double-buffered, and the barrier after the layer-0
+//     epilogue is a CTA barrier, so both warpgroups' dW0 (retired by their layer-0 wait) are done before h2 is rewritten;
+//   * x (prefetch_x) and the 16-bit gradient d_emb16 (TMA, one 8 KB buffer) of the next tile are loaded a tile ahead.
 // ====================================================================================================
 struct EncFusedBwdParams {
   EncFusedParams f;
   const float* d_emb; int ldd;              // [n, ldd] gradient w.r.t. emb (already scaled by 1/B_global)
-  const uint16_t* d_emb16; int ldd16;       // or: 16-bit gradient already multiplied by the loss scale S
+  const uint16_t* d_emb16;                  // or: 16-bit gradient already multiplied by the loss scale S (read through gmap)
   const float* beta_dev; float inv_batch; float gscale;
   float* part; long long split_stride;      // weight-gradient partials [slot][P]
   const long long* w0_off; const long long* b0_off; const long long* w1_off; const long long* w2_off;
 };
 
+// one thread: the [128 rows x 32] block of d_emb16 (feature f, rows from row0) -> shared memory; rows past n read as 0
+__device__ __forceinline__ void load_demb16(uint32_t dst, const CUtensorMap* gmap, uint32_t bar, int f, long long row0) {
+  mbar_expect_tx(bar, TM * 64);
+  tma_load_2d(dst, gmap, bar, f * 32, (int)row0);
+}
+
 template <bool BF16, bool RELU>
 __global__ void __launch_bounds__(kThreads, 1)
-dib_enc_fused_bwd_kernel(const __grid_constant__ WeightMaps maps, const EncFusedBwdParams Q) {
+dib_enc_fused_bwd_kernel(const __grid_constant__ WeightMaps maps, const __grid_constant__ CUtensorMap gmap,
+                         const EncFusedBwdParams Q) {
   const EncFusedParams& P = Q.f;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sb = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar_w = sb + kOffBwdEnd;
+  const uint8_t* sg = smem_raw + (sb - smem_u32(smem_raw));
+  const uint32_t bar_w = sb + kOffBwdEnd, bar_g = bar_w + 8;
 
   const int tid = threadIdx.x, lane = tid & 31, wg = tid >> 7;
   const Frag fr = frag_of(tid);
   const int F = P.F;
   const int ntiles = (int)((P.n + TM - 1) / TM);
   const unsigned int nstep = P.step + (P.step_dev ? P.step_dev[0] : 0u);
-  const uint32_t a0 = sb + kOffA0, h1 = sb + kOffH1, h2 = sb + kOffH2, dO = sb + kOffDO, dz2 = sb + kOffDZ2;
+  const uint32_t h1 = sb + kOffH1, h2 = sb + kOffH2, dO = sb + kOffDO, dz2 = sb + kOffDZ2, gbuf = sb + kOffG;
+  const uint32_t xs = sb + kOffX + tid * 16;
+  const float* xslot = reinterpret_cast<const float*>(sg + kOffX + tid * 16);
+  const uint32_t* gsm = reinterpret_cast<const uint32_t*>(sg + kOffG);    // [128 rows][16 pairs] d_emb16 of this tile
   const float S = Q.gscale, invS = 1.f / Q.gscale;
 
   if (tid == 0) {
     tma_prefetch_desc(&maps.w0); tma_prefetch_desc(&maps.w1); tma_prefetch_desc(&maps.w2);
     tma_prefetch_desc(&maps.b1); tma_prefetch_desc(&maps.b2);
+    if (Q.d_emb16) tma_prefetch_desc(&gmap);
     mbar_init(bar_w, 1);
+    mbar_init(bar_g, 1);
     fence_barrier_init();
   }
   __syncthreads();
 
   const Sched s = sched_of(blockIdx.x, gridDim.x, F);
-  uint32_t fit = 0;
+  uint32_t fit = 0, tpar = 0;   // tpar: parity of the tiles run so far = this tile's [pe|1] buffer and d_emb16-load phase
   for (int f = s.f_first; f < F; f += s.f_step, ++fit) {
-    if (tid == 0) load_weights(sb, maps, bar_w, f);
+    if (tid == 0) {
+      load_weights(sb, maps, bar_w, f);
+      if (Q.d_emb16 && s.slot < ntiles) load_demb16(gbuf, &gmap, bar_g, f, (long long)s.slot * TM);
+    }
     const int d = P.fdim[f], xo = P.x_off[f];
+    prefetch_x(P, xs, tid, (long long)s.slot * TM, d, xo);
     const float bs = Q.beta_dev[0] * Q.inv_batch * S;
+    // The weight-gradient accumulators are started by the first tile's MMAs (scale-d = 0), not by register writes: no
+    // instruction but a wgmma may define them while dW0 is in flight across tiles.  A CTA without a tile of the feature
+    // flushes zeros.
     float accW1[64], accW2[32], accW0[8], accB1[8], accB2[8];
-#pragma unroll
-    for (int i = 0; i < 64; ++i) accW1[i] = 0.f;
-#pragma unroll
-    for (int i = 0; i < 32; ++i) accW2[i] = 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) { accW0[i] = 0.f; accB1[i] = 0.f; accB2[i] = 0.f; }
     mbar_wait(bar_w, fit & 1);
     for (int t = s.slot; t < ntiles; t += s.nslots) {
       const long long row0 = (long long)t * TM;
+      const uint32_t wacc = t != s.slot;   // accumulate into the weight gradients (all but the feature's first tile)
+      const uint32_t a0 = sb + kOffA0 + tpar * kA0Bytes;
       // ---- recompute the forward of this warpgroup's rows
-      stage_a0<BF16>(P, a0, tid, row0, d, xo);
+      stage_a0<BF16>(P, a0, xslot, tid, row0, d);
+      prefetch_x(P, xs, tid, row0 + (long long)s.nslots * TM, d, xo);
       wg_publish(wg);
       float acc[64];
       wgmma_fence();
       mma_layer0<BF16>(acc, sb, a0, wg);
       wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs(acc);
+      wgmma_wait<0>();                     // also retires this warpgroup's dW0 of the previous tile
+      wgmma_fence_regs(acc); wgmma_fence_regs(accW0);
       frag_to_tile<BF16, RELU, 128>(acc, h1, fr, P.act, P.alpha);
-      wg_publish(wg);
+      cta_publish();                       // h1; and both warpgroups' dW0 of the previous tile (it read all of h2) are done
       wgmma_fence();
       mma_layer1<BF16>(acc, sb, h1, a0, wg);
       wgmma_commit();
@@ -521,6 +601,7 @@ dib_enc_fused_bwd_kernel(const __grid_constant__ WeightMaps maps, const EncFused
       float nz[4][2][2];
 #pragma unroll
       for (int j = 0; j < 4; ++j) noise_pair(P, nstep, grow_lo, f, j, fr.q, lane, nz[j]);
+      if (Q.d_emb16) mbar_wait(bar_g, tpar);
       wgmma_wait<0>();
       wgmma_fence_regs(acc2);
       // ---- (mu, logvar) -> d(mu), d(logvar) -> dO tile.  Rows past the batch end contribute nothing.
@@ -535,7 +616,7 @@ dib_enc_fused_bwd_kernel(const __grid_constant__ WeightMaps maps, const EncFused
           const int e = 8 * j + 2 * fr.q;
           float g[2] = {0.f, 0.f};
           if (valid) {
-            if (Q.d_emb16) unpack2<BF16>(*reinterpret_cast<const uint32_t*>(Q.d_emb16 + grow * Q.ldd16 + f * 32 + e), g[0], g[1]);
+            if (Q.d_emb16) unpack2<BF16>(gsm[r * 16 + e / 2], g[0], g[1]);
             else {
               const float2 g2 = *reinterpret_cast<const float2*>(Q.d_emb + grow * Q.ldd + f * 32 + e);
               g[0] = g2.x * S; g[1] = g2.y * S;
@@ -553,80 +634,89 @@ dib_enc_fused_bwd_kernel(const __grid_constant__ WeightMaps maps, const EncFused
           st_shared_b32(tile_chunk_addr(dO, r, 32 + e) + 4 * fr.q, pack2<BF16>(dl[0], dl[1]));
         }
       }
-      cta_publish();                       // dO, h2, h1, [pe|1] of all 128 rows
-      // ---- layer 2 backward: G2 = dO W2^T (own rows); dW2 += h2^T dO; db2 += dO^T [pe|1]
+      cta_publish();                       // dO, h2, h1, [pe|1] of all 128 rows; the d_emb16 buffer has been read
+      if (tid == 0 && Q.d_emb16 && t + s.nslots < ntiles) load_demb16(gbuf, &gmap, bar_g, f, row0 + (long long)s.nslots * TM);
+      // ---- layer 2 backward: G2 = dO W2^T (own rows) | dW2 += h2^T dO; db2 += dO^T [pe|1]
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < EO / 16; ++kk)
         wgmma_m64n128k16<BF16, 0, 0>(acc, gmma_desc(dO + wg * 64 * 128 + kk * 32, 16, 1024),
                                      gmma_desc(sb + kOffW2 + kk * 32, 16, 1024), kk > 0 ? 1u : 0u);
+      wgmma_commit();
 #pragma unroll
       for (int kk = 0; kk < TM / 16; ++kk)
-        wgmma_m64n64k16<BF16, 1, 1>(accW2, desc_act_t_as_a(h2, wg, kk), desc_act_as_b(dO, kk), 1u);
+        wgmma_m64n64k16<BF16, 1, 1>(accW2, desc_act_t_as_a(h2, wg, kk), desc_act_as_b(dO, kk), kk > 0 ? 1u : wacc);
       // (both warpgroups run the small db2 contraction -- uniform issue keeps the MMAs unserialised; warpgroup 0 stores it)
 #pragma unroll
       for (int kk = 0; kk < TM / 16; ++kk)
-        wgmma_m64n16k16<BF16, 1, 1>(accB2, desc_act_t_as_a(dO, 0, kk), desc_a0_as_b(a0, kk), 1u);
+        wgmma_m64n16k16<BF16, 1, 1>(accB2, desc_act_t_as_a(dO, 0, kk), desc_a0_as_b(a0, kk), kk > 0 ? 1u : wacc);
       wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs(acc); wgmma_fence_regs(accW2); wgmma_fence_regs(accB2);
-      // ---- dz2 = G2 * act'(h2)
+      wgmma_wait<1>();
+      wgmma_fence_regs(acc);
+      // ---- dz2 = G2 * act'(h2), while dW2 / db2 run
       frag_dgrad_to_tile<BF16, RELU>(acc, h2, dz2, fr, P.act, P.alpha);
+      wgmma_wait<0>();
+      wgmma_fence_regs(accW2); wgmma_fence_regs(accB2);
       cta_publish();
-      // ---- layer 1 backward: G1 = dz2 W1^T (own rows); dW1 += h1^T dz2; db1 += dz2^T [pe|1]
+      // ---- layer 1 backward: G1 = dz2 W1^T (own rows) | dW1 += h1^T dz2; db1 += dz2^T [pe|1]
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < HID / 16; ++kk)
         wgmma_m64n128k16<BF16, 0, 0>(acc, desc_act_as_a(dz2, wg, kk),
                                      gmma_desc(sb + kOffW1 + (kk >> 2) * kPanel + (kk & 3) * 32, 16, 1024), kk > 0 ? 1u : 0u);
-#pragma unroll
-      for (int kk = 0; kk < TM / 16; ++kk)
-        wgmma_m64n128k16<BF16, 1, 1>(accW1, desc_act_t_as_a(h1, wg, kk), desc_act_as_b(dz2, kk), 1u);
-#pragma unroll
-      for (int kk = 0; kk < TM / 16; ++kk)
-        wgmma_m64n16k16<BF16, 1, 1>(accB1, desc_act_t_as_a(dz2, wg, kk), desc_a0_as_b(a0, kk), 1u);
       wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs(acc); wgmma_fence_regs(accW1); wgmma_fence_regs(accB1);
-      // ---- dz1 = G1 * act'(h1) -> the h2 buffer (its last readers, the dz2 epilogue and dW2, are done)
+#pragma unroll
+      for (int kk = 0; kk < TM / 16; ++kk)
+        wgmma_m64n128k16<BF16, 1, 1>(accW1, desc_act_t_as_a(h1, wg, kk), desc_act_as_b(dz2, kk), kk > 0 ? 1u : wacc);
+#pragma unroll
+      for (int kk = 0; kk < TM / 16; ++kk)
+        wgmma_m64n16k16<BF16, 1, 1>(accB1, desc_act_t_as_a(dz2, wg, kk), desc_a0_as_b(a0, kk), kk > 0 ? 1u : wacc);
+      wgmma_commit();
+      wgmma_wait<1>();
+      wgmma_fence_regs(acc);
+      // ---- dz1 = G1 * act'(h1) -> the h2 buffer, while dW1 / db1 run (they read h1, dz2, [pe|1]; every dW2 is done)
       frag_dgrad_to_tile<BF16, RELU>(acc, h1, h2, fr, P.act, P.alpha);
+      wgmma_wait<0>();
+      wgmma_fence_regs(accW1); wgmma_fence_regs(accB1);
       cta_publish();
-      // ---- layer 0 backward: [dW0;db0]^T += dz1^T [pe|1]
+      // ---- layer 0 backward: [dW0;db0]^T += dz1^T [pe|1], retired by the next tile's layer-0 wait (or after the loop)
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < TM / 16; ++kk)
-        wgmma_m64n16k16<BF16, 1, 1>(accW0, desc_act_t_as_a(h2, wg, kk), desc_a0_as_b(a0, kk), 1u);
+        wgmma_m64n16k16<BF16, 1, 1>(accW0, desc_act_t_as_a(h2, wg, kk), desc_a0_as_b(a0, kk), kk > 0 ? 1u : wacc);
       wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs(accW0);
-      __syncthreads();                     // every MMA of this tile has read its operands: the next tile may overwrite them
+      tpar ^= 1u;
     }
+    wgmma_wait<0>();
+    wgmma_fence_regs(accW0);
     // ================= flush this (feature, slot)'s weight-gradient partials (scaled back by 1/S)
     float* part = Q.part + (long long)s.slot * Q.split_stride;
     const int w_in = d * P.nfreq;
+    const bool ran = s.slot < ntiles;
+    auto out = [&](float v) { return ran ? v * invS : 0.f; };
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int m = fr.rb + 8 * h;                       // this thread's rows of the warpgroup-owned accumulators
 #pragma unroll
       for (int j = 0; j < 16; ++j)                       // dW1[h1 = m][h2 = 8 j + 2 q ..]
         *reinterpret_cast<float2*>(part + Q.w1_off[f] + (long long)m * HID + 8 * j + 2 * fr.q) =
-            make_float2(accW1[4 * j + 2 * h] * invS, accW1[4 * j + 2 * h + 1] * invS);
+            make_float2(out(accW1[4 * j + 2 * h]), out(accW1[4 * j + 2 * h + 1]));
 #pragma unroll
       for (int j = 0; j < 8; ++j)                        // dW2[h2 = m][o = 8 j + 2 q ..]
         *reinterpret_cast<float2*>(part + Q.w2_off[f] + (long long)m * EO + 8 * j + 2 * fr.q) =
-            make_float2(accW2[4 * j + 2 * h] * invS, accW2[4 * j + 2 * h + 1] * invS);
+            make_float2(out(accW2[4 * j + 2 * h]), out(accW2[4 * j + 2 * h + 1]));
       // dW0[k][h1 = m] (k < w_in) and db0[m] = column w_in of dW0p^T; db1[h2 = m], db2[o = m] = column w_in
 #pragma unroll
       for (int j = 0; j < 2; ++j) {
 #pragma unroll
         for (int k = 0; k < 2; ++k) {
           const int col = 8 * j + 2 * fr.q + k;
-          const float v0 = accW0[4 * j + 2 * h + k] * invS;
+          const float v0 = out(accW0[4 * j + 2 * h + k]);
           if (col < w_in) part[Q.w0_off[f] + (long long)col * HID + m] = v0;
           else if (col == w_in) {
             part[Q.b0_off[f] + m] = v0;
-            part[P.b1_off[f] + m] = accB1[4 * j + 2 * h + k] * invS;
-            if (wg == 0) part[P.b2_off[f] + m] = accB2[4 * j + 2 * h + k] * invS;
+            part[P.b1_off[f] + m] = out(accB1[4 * j + 2 * h + k]);
+            if (wg == 0) part[P.b2_off[f] + m] = out(accB2[4 * j + 2 * h + k]);
           }
         }
       }
@@ -702,6 +792,19 @@ bool make_wmap(CUtensorMap* m, const uint16_t* base, int cols, int rows, int nfe
                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
+// d_emb16 [n rows, pitch ld] 16-bit, columns [0, cols) -> 2D map, box 32 cols x 128 rows (one feature's block of a tile),
+// no swizzle; rows past n are filled with zeros
+bool make_gmap(CUtensorMap* m, const void* base, int cols, long long n, int ld, bool bf16) {
+  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)n};
+  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
+  cuuint32_t box[2] = {32, TM};
+  cuuint32_t es[2] = {1, 1};
+  return encode_fn2()(m, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2,
+                      const_cast<void*>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                      CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
 bool make_all_maps(WeightMaps* m, const void* packed, int F, bool bf16) {
   const uint16_t* pk = static_cast<const uint16_t*>(packed);
   return make_wmap(&m->w0, pk, HID, K0, F, bf16) && make_wmap(&m->w1, pk + kW0Elems, HID, HID, F, bf16) &&
@@ -718,11 +821,11 @@ void fill_params(EncFusedParams& P, const DibEncFusedDesc& d, const DibEncFusedI
   P.round_emb = 1; P.emb16 = static_cast<uint16_t*>(io.emb16); P.ldemb16 = io.ldemb16;
 }
 
-template <typename K, typename A>
-cudaError_t launch_fused(K kern, int smem, int grid, const WeightMaps& m, const A& args, cudaStream_t st) {
+template <typename K, typename... A>
+cudaError_t launch_fused(K kern, int smem, int grid, cudaStream_t st, const A&... args) {
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e != cudaSuccess) return e;
-  kern<<<grid, kThreads, smem, st>>>(m, args);
+  kern<<<grid, kThreads, smem, st>>>(args...);
   dib_note_launch();
   return cudaGetLastError();
 }
@@ -754,10 +857,10 @@ cudaError_t dib_enc_fused_forward(const DibEncFusedDesc& d, const DibEncFusedIO&
   fill_params(P, d, io);
   constexpr int smem = kOffFwdEnd + 128 + 1024;
   const bool relu = d.act == DIB_ACT_RELU;
-  if (d.bf16) return relu ? launch_fused(dib_enc_fused_fwd_kernel<true, true>, smem, d.grid, m, P, st)
-                          : launch_fused(dib_enc_fused_fwd_kernel<true, false>, smem, d.grid, m, P, st);
-  return relu ? launch_fused(dib_enc_fused_fwd_kernel<false, true>, smem, d.grid, m, P, st)
-              : launch_fused(dib_enc_fused_fwd_kernel<false, false>, smem, d.grid, m, P, st);
+  if (d.bf16) return relu ? launch_fused(dib_enc_fused_fwd_kernel<true, true>, smem, d.grid, st, m, P)
+                          : launch_fused(dib_enc_fused_fwd_kernel<true, false>, smem, d.grid, st, m, P);
+  return relu ? launch_fused(dib_enc_fused_fwd_kernel<false, true>, smem, d.grid, st, m, P)
+              : launch_fused(dib_enc_fused_fwd_kernel<false, false>, smem, d.grid, st, m, P);
 }
 
 cudaError_t dib_enc_fused_backward(const DibEncFusedDesc& d, const DibEncFusedIO& io, const DibEncFusedBwdIO& b,
@@ -768,14 +871,16 @@ cudaError_t dib_enc_fused_backward(const DibEncFusedDesc& d, const DibEncFusedIO
   EncFusedBwdParams Q;
   fill_params(Q.f, d, io);
   Q.f.round_emb = 0;
-  Q.d_emb16 = static_cast<const uint16_t*>(b.d_emb16); Q.ldd16 = b.ldd16;
+  Q.d_emb16 = static_cast<const uint16_t*>(b.d_emb16);
+  CUtensorMap gmap = {};                  // unused without d_emb16
+  if (b.d_emb16 && !make_gmap(&gmap, b.d_emb16, d.F * 32, io.n, b.ldd16, d.bf16)) return cudaErrorInvalidValue;
   Q.d_emb = b.d_emb; Q.ldd = b.ldd; Q.beta_dev = b.beta_dev; Q.inv_batch = b.inv_batch; Q.gscale = b.gscale;
   Q.part = b.part; Q.split_stride = b.split_stride;
   Q.w0_off = d.w0_off; Q.b0_off = d.b0_off; Q.w1_off = d.w1_off; Q.w2_off = d.w2_off;
   constexpr int smem = kOffBwdEnd + 128 + 1024;
   const bool relu = d.act == DIB_ACT_RELU;
-  if (d.bf16) return relu ? launch_fused(dib_enc_fused_bwd_kernel<true, true>, smem, d.grid, m, Q, st)
-                          : launch_fused(dib_enc_fused_bwd_kernel<true, false>, smem, d.grid, m, Q, st);
-  return relu ? launch_fused(dib_enc_fused_bwd_kernel<false, true>, smem, d.grid, m, Q, st)
-              : launch_fused(dib_enc_fused_bwd_kernel<false, false>, smem, d.grid, m, Q, st);
+  if (d.bf16) return relu ? launch_fused(dib_enc_fused_bwd_kernel<true, true>, smem, d.grid, st, m, gmap, Q)
+                          : launch_fused(dib_enc_fused_bwd_kernel<true, false>, smem, d.grid, st, m, gmap, Q);
+  return relu ? launch_fused(dib_enc_fused_bwd_kernel<false, true>, smem, d.grid, st, m, gmap, Q)
+              : launch_fused(dib_enc_fused_bwd_kernel<false, false>, smem, d.grid, st, m, gmap, Q);
 }
