@@ -89,6 +89,8 @@ struct dib_model {
     bool enc_fused = false;         // fused per-feature encoder kernels (else PE + grouped GEMMs + reparam kernels)
     bool int16 = false;             // 16-bit integration network (else per-layer TF32 GEMMs + dib_launch_loss)
     bool tail_fused = false;        // int16: last two hidden layers + head + loss as one kernel (dib_int16_fwd2_head)
+    bool tail_bwd = false;          // tail_fused, training: the same kernel also runs the dgrad of its second layer (and of
+                                    // its first when the embedding lies below), which the backward then does not launch
     bool head1 = false;             // int16, no fused tail: the out = 1 head kernel instead of the generic one
   } route;
   // DIB_LOSS_INFONCE (train.py:180-289): the output encoder y -> [PE] -> Dense(y_arch[j], act)... -> Dense(out), its variables
@@ -156,13 +158,15 @@ int nff(const dib_model* h) { return (int)h->ff_arch.size(); }
 
 // the one place the kernel path is chosen.  fused_ok / int16_ok are what dib_create found the shapes to support; the bits of
 // `unfused` (dib_debug_force_unfused) turn paths off: 1 = fused encoders, 2 = 16-bit integration network (it reads the fp16
-// embedding only the fused encoders write), 4 = fused integration tail, 8 = out = 1 head kernel.
+// embedding only the fused encoders write), 4 = fused integration tail, 8 = out = 1 head kernel, 16 = the dgrad stages of
+// the fused tail (separate dgrad launches instead).
 void set_route(dib_model* h, int unfused) {
   dib_model::Route& r = h->route;
   r.enc_fused = h->fused_ok && !(unfused & 1);
   r.int16 = r.enc_fused && h->int16_ok && !(unfused & 2);
   r.tail_fused = r.int16 && !(unfused & 4) && h->Li >= 2 &&
                  dib_int16_fwd2_ok(int_fan_in(h, h->Li - 2), int_fan_out(h, h->Li - 2), int_fan_out(h, h->Li - 1), h->out);
+  r.tail_bwd = r.tail_fused && !(unfused & 16);
   r.head1 = r.int16 && !r.tail_fused && h->out == 1 && !(unfused & 8);
 }
 
@@ -741,14 +745,19 @@ int forward_integration(const Ctx& c, const float* y, float inv_batch, bool trai
     prof_end(c);
   }
   if (h->route.tail_fused) {
-    // the last two hidden layers and the head run as ONE kernel (g2 stays on chip)
+    // the last two hidden layers and the head run as ONE kernel (g2 stays on chip); in training on the tail_bwd route it
+    // continues with the dgrad chain (dg1 -> dg16_off[j1], its column sums -> the dbpart row of layer j1, and d emb when
+    // j0 == 0) that backward_integration then skips
     const int j0 = h->Li - 2, j1 = h->Li - 1;
-    prof_begin(c, "int16_fwd2_head");
+    const bool bwd = training && h->route.tail_bwd;
+    prof_begin(c, bwd ? "int16_fwd2_head_dgrad" : "int16_fwd2_head");
     DIB_CUDA_OK(dib_int16_fwd2_head(int16_in(c, j0), int_fan_in(h, j0), int_fan_in(h, j0), c.ws + h->w16_off[j0], c.params + h->intB[j0],
                                     c.ws + h->w16_off[j1], c.params + h->intB[j1], c.ws + h->g16_off[j1], c.params + h->intW[h->Li],
                                     c.params + h->intB[h->Li], h->act, h->out_act, h->alpha, h->loss, y, c.n, inv_batch, gscale, dg,
-                                    user_pred, c.ws + h->headpart_off, h->head_stride, c.ws + h->loss_part_off, c.ws + h->acc_part_off,
-                                    &h->head_used, bf, c.st));
+                                    bwd ? (void*)(c.ws + h->dg16_off[j1]) : nullptr,
+                                    bwd ? c.ws + h->dbpart_off + (long long)j1 * h->dbpart_layer : nullptr,
+                                    bwd && j0 == 0 ? (void*)(c.ws + h->demb16_off) : nullptr, user_pred, c.ws + h->headpart_off,
+                                    h->head_stride, c.ws + h->loss_part_off, c.ws + h->acc_part_off, &h->head_used, bf, c.st));
     DIB_CUDA_OK(finalize(h->head_used));
     prof_end(c);
     return 0;
@@ -917,16 +926,20 @@ int backward_integration(const Ctx& c, float inv_batch, const Split& sp, float* 
   segs->push_back({c.ws + h->headpart_off + (long long)Kh * h->out + h->out, h->head_stride, h->head_used, Kh, 1.f / gscale,
                    grads_flat + h->intB[h->Li - 1]});
   // the dgrad chain first (layer j's dgrad produces the gradient layer j-1's wgrad consumes), then the weight gradients in PAIRS of
-  // layers per launch: one layer's [K/128 x N/128 x splits] tiles do not fill the 2 x SMs CTA slots, two layers' tiles do
+  // layers per launch: one layer's [K/128 x N/128 x splits] tiles do not fill the 2 x SMs CTA slots, two layers' tiles do.
+  // On the tail_bwd route the training forward already ran the dgrads of layer j1 = Li-1 and, when j0 = Li-2 is 0, of j0.
+  const int j_top = h->route.tail_bwd ? (h->Li == 2 ? -1 : h->Li - 2) : h->Li - 1;
   for (int j = h->Li - 1; j >= 0; --j) {
     const int K = int_fan_in(h, j), N = int_fan_out(h, j);
-    prof_begin(c, "int16_dgrad_l", j);
-    DIB_CUDA_OK(dib_int16_dgrad(c.ws + h->dg16_off[j + 1], N, c.ws + h->w16_off[j], j > 0 ? (const void*)(c.ws + h->g16_off[j]) : nullptr,
-                                K, j > 0 ? (void*)(c.ws + h->dg16_off[j]) : (void*)(c.ws + h->demb16_off), K, c.n, K, N, h->act,
-                                h->alpha, j > 0 ? c.ws + h->dbpart_off + (long long)j * h->dbpart_layer : nullptr, bf, c.st));
-    if (j > 0)   // bias gradient of layer j-1 = column sums of the gradient this dgrad just produced
+    if (j <= j_top) {
+      prof_begin(c, "int16_dgrad_l", j);
+      DIB_CUDA_OK(dib_int16_dgrad(c.ws + h->dg16_off[j + 1], N, c.ws + h->w16_off[j], j > 0 ? (const void*)(c.ws + h->g16_off[j]) : nullptr,
+                                  K, j > 0 ? (void*)(c.ws + h->dg16_off[j]) : (void*)(c.ws + h->demb16_off), K, c.n, K, N, h->act,
+                                  h->alpha, j > 0 ? c.ws + h->dbpart_off + (long long)j * h->dbpart_layer : nullptr, bf, c.st));
+      prof_end(c);
+    }
+    if (j > 0)   // bias gradient of layer j-1 = column sums of the gradient layer j's dgrad produced
       segs->push_back({c.ws + h->dbpart_off + (long long)j * h->dbpart_layer, K, row_tiles, K, 1.f / gscale, grads_flat + h->intB[j - 1]});
-    prof_end(c);
   }
   std::vector<int> nsplit_of(h->Li, sp.nsplit);
   auto tiles_of = [&](int j) { return DIB_CEIL_DIV(int_fan_in(h, j), 128) * DIB_CEIL_DIV(int_fan_out(h, j), 128); };
@@ -1271,6 +1284,7 @@ int32_t dib_model_info(const dib_model* h, char* out, size_t out_bytes) {
     s += fused ? std::string(" operands=") + (h->precision == DIB_PREC_BF16 ? "bf16" : "fp16") : std::string(" operands=tf32");
     s += " accumulate=fp32";
   }
+  if (h->route.tail_fused) s += h->route.tail_bwd ? " integration_tail=fwd2-head-dgrad" : " integration_tail=fwd2-head";
   if (h->st)
     s += std::string(" set_transformer=attention-simt-fp32,layernorm-simt-fp32,dense-") + (is_tc(h) ? "wgmma-tf32" : "simt-fp32");
   if (infonce(h))

@@ -8,7 +8,9 @@
 //   * dib_int16_head_kernel: the narrow output layer (out <= 16) fused with everything around it -- logits, compiled
 //     loss + accuracy, d loss / d logits, the dgrad into the last hidden layer (incl. its act') and the output layer's
 //     own weight/bias gradients -- one pass over the last hidden activation.  dib_int16_head1_kernel: the same for out = 1.
-//   * dib_int16_fwd2_kernel: the last two 256-wide hidden layers and the single-output head of models with out = 1.
+//   * dib_int16_fwd2_kernel: the last two 256-wide hidden layers and the single-output head of models with out = 1, and in
+//     training the dgrad chain below the head: down to the 16-bit embedding gradient, or to the first fused layer's
+//     pre-activation gradient when another hidden layer lies below it.
 // Which tail and which head kernel run is the caller's choice (the model handle's route in dib_api.cu); nothing here
 // reads process-wide state.
 // Gradient operands are scaled by the power-of-two loss scale S (see dib_enc_fused.cu) to stay inside fp16 range.
@@ -19,6 +21,8 @@
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+
+#include <type_traits>
 
 #include "dib_common.cuh"
 #include "dib_kernels.h"
@@ -59,6 +63,11 @@ __device__ __forceinline__ void unpack_h2(uint32_t u, float& a, float& b) {
 
 __device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) {
   asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint32_t ld_shared_b32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+  return v;
 }
 
 // 16-bit operand tiles of one pipeline stage (TMA SWIZZLE_128B boxes, see map_k / map_mn):
@@ -249,11 +258,25 @@ dib_int16_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
 //                      e1  g2 = act(D1 + b1) kept PACKED IN REGISTERS, logit = g2 . w + b, compiled loss / metric,
 //                          d loss / d logit, dg2 = dz w act'(g2) -> HBM, output-layer weight / bias gradients and the bias gradient
 //                          of the last hidden layer as per-CTA partials.
-// g2 never reaches HBM, and the head's re-read of it (and its launch) disappears.  A warp owns 16 whole rows of the
-// accumulator, so each row's logit is complete after a reduction over the 4 lanes that share the row.
+//   training, backward stages on (dg1 != null), the dgrad chain of the same rows:
+//                      D1  acc = dg2 W1^T  (dg2 packed in registers = the wgmma A fragment; W1 K-major through the ring;
+//                          two 128-column chunks)
+//                      e2  dg1 = acc act'(g1) (g1 read back from the shared tile) -> HBM, packed into registers; its column
+//                          sums per tile (bias gradient of the first fused layer) -> dbpart, in the order of the DGRAD epilogue
+//                      D0  (only when the layer below is the embedding, which has no act') d emb = dg1 W0^T over 128-column
+//                          chunks (W0 K-major through the ring)
+//                      e3  16-bit d emb -> the g1 tile (free by then) -> TMA tensor store (no partial-sector writes)
+// g2 never reaches HBM, and the head's re-read of it (and its launch) disappears; with the backward stages, neither do
+// the two dgrad launches nor their re-reads of dg2, dg1 and g1.  A warp owns 16 whole rows of the accumulator, so each
+// row's logit is complete after a reduction over the 4 lanes that share the row.  Every MMA keeps the operands and the
+// k order of dib_int16_dgrad, and every sum its order: the results are those of the separate launches, bit for bit.
+// Ring stages of a tile: nk0 x (A, W0 MN-major), 4 x W1 MN-major; then 2 x 2 x W1 K-major and K0 / 128 x 2 x W0 K-major
+// (B only: 128 output columns x 128 k each).  Shared memory: the 2-stage ring (2 x 48 KB), the g1 tile (4 swizzled
+// 64-column panels of 128 rows, 64 KB), the barriers, and statically the bias / head-weight rows and the column-sum scratch.
 // ====================================================================================================
 constexpr int kF2N = 256, kF2Stages = 2;
 constexpr int kF2AB = kBM * 128, kF2BB = kF2N * 128, kF2Stage = kF2AB + kF2BB;      // 16 KB + 32 KB
+constexpr int kF2BtN = 128, kF2BtB = kF2BtN * 128;   // backward stages: B only, two k-blocks of 128 K-major rows (2 x 16 KB)
 constexpr int kF2G1Off = kF2Stages * kF2Stage;
 constexpr int kF2BarOff = kF2G1Off + kBM * kF2N * 2;
 constexpr int kF2Smem = kF2BarOff + 64 + 1024;
@@ -262,6 +285,10 @@ struct Fwd2Args {
   const float *b0, *b1, *wout, *bout;
   uint16_t* g1; int ldg1;             // out: first fused layer's activation [M x 256]
   uint16_t* dg2; int lddg;            // out (training) or null: gradient w.r.t. the second fused layer's pre-activation, x gscale
+  uint16_t* dg1;                      // out (training, backward stages) or null: gradient w.r.t. the first fused layer's
+                                      // pre-activation [M x 256], x gscale
+  float* dbpart;                      // with dg1: column sums of dg1 per 128-row tile [tiles][256]
+  int demb_cols;                      // with dg1, > 0: the layer below is the embedding; d emb [M x demb_cols] via mapDemb
   const float* y; float* user_pred;
   float* wpart; int wpart_stride; float *loss_part, *acc_part;
   int M, nk0, act, out_act, loss;
@@ -274,7 +301,8 @@ constexpr int kF2Threads = kConsumers + 128;      // + a producer warpgroup, so 
 template <bool BF16, int ACT>
 __global__ void __launch_bounds__(kF2Threads, 1)
 dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapW0,
-                      const __grid_constant__ CUtensorMap mapW1, const Fwd2Args a) {
+                      const __grid_constant__ CUtensorMap mapW1, const __grid_constant__ CUtensorMap mapW1t,
+                      const __grid_constant__ CUtensorMap mapW0t, const __grid_constant__ CUtensorMap mapDemb, const Fwd2Args a) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sb = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bar_base = sb + kF2BarOff;
@@ -287,6 +315,7 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
   __shared__ float s_red[3][kConsumers / 32];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int ntile = DIB_CEIL_DIV(a.M, kBM);
+  const bool bwd = a.dg1 != nullptr;
 
   for (int i = tid; i < kF2N; i += blockDim.x) { s_b0[i] = a.b0[i]; s_b1[i] = a.b1[i]; s_w[i] = a.wout[i]; }
   if (tid == 0) {
@@ -299,7 +328,15 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (warp == kProducerWarp && lane == 0) {
       tma_prefetch_desc(&mapA); tma_prefetch_desc(&mapW0); tma_prefetch_desc(&mapW1);
+      if (bwd) { tma_prefetch_desc(&mapW1t); if (a.demb_cols > 0) tma_prefetch_desc(&mapW0t); }
       uint32_t s = 0, ph = 0;
+      auto b_stage = [&](const CUtensorMap* m, int k0, int c0) {     // a B-only stage: 128 K-major rows x 128 k
+        mbar_wait(empty_bar(s), ph ^ 1);
+        mbar_expect_tx(full_bar(s), 2 * kF2BtB);
+        tma_load_2d(sb + s * kF2Stage + kF2AB, m, full_bar(s), k0, c0);
+        tma_load_2d(sb + s * kF2Stage + kF2AB + kF2BtB, m, full_bar(s), k0 + kBK, c0);
+        if (++s == kF2Stages) { s = 0; ph ^= 1; }
+      };
       for (int tile = blockIdx.x; tile < ntile; tile += gridDim.x) {
         for (int k = 0; k < a.nk0; ++k) {
           mbar_wait(empty_bar(s), ph ^ 1);
@@ -314,6 +351,12 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
           mbar_expect_tx(full_bar(s), kF2BB);
           tma_load_3d(sb + s * kF2Stage + kF2AB, &mapW1, full_bar(s), 0, k * kBK, 0);
           if (++s == kF2Stages) { s = 0; ph ^= 1; }
+        }
+        if (bwd) {
+          for (int c0 = 0; c0 < kF2N; c0 += kF2BtN)
+            for (int k = 0; k < kF2N; k += 2 * kBK) b_stage(&mapW1t, k, c0);
+          for (int c0 = 0; c0 < a.demb_cols; c0 += kF2BtN)
+            for (int k = 0; k < kF2N; k += 2 * kBK) b_stage(&mapW0t, k, c0);
         }
       }
     }
@@ -348,6 +391,39 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
     if (lane == 0) mbar_arrive(empty_bar(prev));
     wgmma_fence_regs(acc);
   };
+  // acc = A[64 x 256] B[256 x 128] over 2 B-only ring stages of two k-blocks; A packed in registers (ap[4 t .. 4 t + 3]: the
+  // fragment of k16 step t).  128-column chunks: a 256-column accumulator next to the 64 A registers does not fit the
+  // register budget.  Stages of 128 k: the ring is 2 deep, and half as many stages halves the exposed load latencies.
+  auto mainloop_rs = [&](float (&acc)[64], const uint32_t (&ap)[64]) {
+    uint32_t prev = 0;
+#pragma unroll
+    for (int k = 0; k < kF2N / (2 * kBK); ++k) {
+      mbar_wait(full_bar(s), ph);
+      const uint32_t bt = sb + s * kF2Stage + kF2AB;
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 2 * kBK / 16; ++kk) {
+        const int t = 8 * k + kk;
+        const uint32_t af[4] = {ap[4 * t], ap[4 * t + 1], ap[4 * t + 2], ap[4 * t + 3]};
+        wgmma_m64n128k16_rs<BF16, 0>(acc, af, desc_kmaj(bt + (kk >> 2) * kF2BtB, kk & 3), t > 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (k > 0 && lane == 0) mbar_arrive(empty_bar(prev));
+      prev = s;
+      if (++s == kF2Stages) { s = 0; ph ^= 1; }
+    }
+    wgmma_wait<0>();
+    if (lane == 0) mbar_arrive(empty_bar(prev));
+    wgmma_fence_regs(acc);
+  };
+  // this thread's word (columns c, c + 1 of row r) in the swizzled g1 tile; every thread reads back only words it wrote
+  auto g1_word = [&](int c, int r) { return g1s + (c >> 6) * kF2AB + r * 128 + ((((c & 63) >> 3) ^ (r & 7)) << 4) + 4 * q; };
+  // the warpgroup's d emb stores, all (N = 0) or all but the last group (N = 1), have read its rows of the g1 tile
+  auto stores_drained = [&](auto n_pending) {
+    if ((tid & 127) == 0) bulk_wait_read<decltype(n_pending)::value>();
+    named_bar_sync(2 + wg, 128);
+  };
 
   for (int tile = blockIdx.x; tile < ntile; tile += gridDim.x) {
     const long long row_lo = (long long)tile * kBM + rb;
@@ -356,6 +432,7 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
     for (int i = 0; i < 128; ++i) acc[i] = 0.f;
     // ---------------- L0, e0: g1 = act(D0 + b0) -> shared tile (L1's A operand) and HBM
     mainloop(acc, a.nk0, true);
+    if (a.demb_cols > 0) stores_drained(std::integral_constant<int, 0>());
 #pragma unroll
     for (int j = 0; j < kF2N / 8; ++j) {
       const int c = 8 * j + 2 * q;
@@ -364,7 +441,7 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
       for (int h = 0; h < 2; ++h) {
         const int r = rb + 8 * h;
         const uint32_t w = pack_h2<BF16>(dib_act16(ACT, acc[4 * j + 2 * h] + bv.x, a.alpha), dib_act16(ACT, acc[4 * j + 2 * h + 1] + bv.y, a.alpha));
-        st_shared_b32(g1s + (c >> 6) * kF2AB + r * 128 + ((((c & 63) >> 3) ^ (r & 7)) << 4) + 4 * q, w);
+        st_shared_b32(g1_word(c, r), w);
         if (row_lo + 8 * h < a.M) *reinterpret_cast<uint32_t*>(a.g1 + (row_lo + 8 * h) * a.ldg1 + c) = w;
       }
     }
@@ -384,8 +461,12 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
       for (int h = 0; h < 2; ++h) {
         const uint32_t p = pack_h2<BF16>(dib_act16(ACT, acc[4 * j + 2 * h] + bv.x, a.alpha), dib_act16(ACT, acc[4 * j + 2 * h + 1] + bv.y, a.alpha));
         g2p[2 * j + h] = p;
+        // an opaque copy: else the compiler keeps these unpacked floats (twice the registers of g2p) alive for pass 2 instead
+        // of unpacking g2p again there, and spills once pass 2 feeds the backward stages
+        uint32_t pc;
+        asm("mov.b32 %0, %1;" : "=r"(pc) : "r"(p));
         float h0, h1;
-        unpack_h2<BF16>(p, h0, h1);
+        unpack_h2<BF16>(pc, h0, h1);
         zp[h] = fmaf(h0, wv.x, zp[h]); zp[h] = fmaf(h1, wv.y, zp[h]);
       }
     }
@@ -412,7 +493,8 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
       if (q == 0) dbo += dzs[h];
     }
     if (train) {
-      // ---------------- e1, pass 2: dg2 = ds w act'(g2) -> HBM; column sums of g2 dz (output-layer dW) and of dg2 (bias gradient)
+      // ---------------- e1, pass 2: dg2 = ds w act'(g2) -> HBM and packed into g2p (A of D1); column sums of g2 dz (output-layer
+      // dW) and of dg2 (bias gradient)
 #pragma unroll
       for (int j = 0; j < kF2N / 8; ++j) {
         const int c = 8 * j + 2 * q;
@@ -425,7 +507,9 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
           const float d0 = ds[h] * wv.x * dib_act_grad(ACT, h0, a.alpha), d1 = ds[h] * wv.y * dib_act_grad(ACT, h1, a.alpha);
           cw[0] += h0 * dzs[h]; cw[1] += h1 * dzs[h];
           cb[0] += d0; cb[1] += d1;
-          if (row_lo + 8 * h < a.M) *reinterpret_cast<uint32_t*>(a.dg2 + (row_lo + 8 * h) * a.lddg + c) = pack_h2<BF16>(d0, d1);
+          const uint32_t dp = pack_h2<BF16>(d0, d1);
+          g2p[2 * j + h] = dp;
+          if (row_lo + 8 * h < a.M) *reinterpret_cast<uint32_t*>(a.dg2 + (row_lo + 8 * h) * a.lddg + c) = dp;
         }
 #pragma unroll
         for (int k = 0; k < 2; ++k) {
@@ -443,7 +527,71 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
       for (int w = 0; w < kConsumers / 32; ++w) { acc_dw += s_colw[w][tid]; acc_dbh += s_colb[w][tid]; }
       named_bar_sync(1, kConsumers);
     }
+    if (bwd) {
+      // ---------------- D1, e2 per 128-column chunk: dg1 = (dg2 W1^T) act'(g1) -> HBM and packed into dg1p (A of D0);
+      // column sums -> dbpart row of the tile
+      uint32_t dg1p[64];
+      float acc2[64];
+#pragma unroll
+      for (int cc = 0; cc < kF2N / kF2BtN; ++cc) {
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc2[i] = 0.f;
+        mainloop_rs(acc2, g2p);
+#pragma unroll
+        for (int j = 0; j < kF2BtN / 8; ++j) {
+          const int c = kF2BtN * cc + 8 * j + 2 * q;
+          float cs[2] = {0.f, 0.f};
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float x0, x1;
+            unpack_h2<BF16>(ld_shared_b32(g1_word(c, rb + 8 * h)), x0, x1);
+            const float v0 = acc2[4 * j + 2 * h] * dib_act_grad(ACT, x0, a.alpha);
+            const float v1 = acc2[4 * j + 2 * h + 1] * dib_act_grad(ACT, x1, a.alpha);
+            const uint32_t p = pack_h2<BF16>(v0, v1);
+            dg1p[2 * (kF2BtN / 8 * cc + j) + h] = p;
+            if (row_lo + 8 * h < a.M) {                   // rows outside the matrix add nothing
+              *reinterpret_cast<uint32_t*>(a.dg1 + (row_lo + 8 * h) * kF2N + c) = p;
+              cs[0] += v0; cs[1] += v1;
+            }
+          }
+          cs[0] = quad_col_sum(cs[0]); cs[1] = quad_col_sum(cs[1]);
+          if (lane < 4) { s_colb[warp][c] = cs[0]; s_colb[warp][c + 1] = cs[1]; }
+        }
+      }
+      named_bar_sync(1, kConsumers);
+      {
+        float sum = 0.f;
+#pragma unroll
+        for (int w = 0; w < kConsumers / 32; ++w) sum += s_colb[w][tid];
+        a.dbpart[(long long)tile * kF2N + tid] = sum;
+      }
+      named_bar_sync(1, kConsumers);
+      // ---------------- D0, e3: d emb = dg1 W0^T per 128-column chunk -> two 64-column panels of the warpgroup's rows of the
+      // g1 tile (chunks alternate between panels 0-1 and 2-3, so a chunk waits only for the stores of the chunk before last)
+      // -> TMA store
+      for (int c0 = 0, cc = 0; c0 < a.demb_cols; c0 += kF2BtN, ++cc) {
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc2[i] = 0.f;
+        mainloop_rs(acc2, dg1p);
+        if (cc >= 2) stores_drained(std::integral_constant<int, 1>());
+        const int tc = (cc & 1) * kF2BtN;                 // shared-tile columns of this chunk
+#pragma unroll
+        for (int j = 0; j < kF2BtN / 8; ++j) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            st_shared_b32(g1_word(tc + 8 * j + 2 * q, rb + 8 * h), pack_h2<BF16>(acc2[4 * j + 2 * h], acc2[4 * j + 2 * h + 1]));
+        }
+        fence_proxy_async_smem();
+        named_bar_sync(2 + wg, 128);
+        if ((tid & 127) == 0) {
+          for (int p = 0; p < kF2BtN / 64 && c0 + 64 * p < a.demb_cols; ++p)
+            tma_store_2d(&mapDemb, g1s + (tc / 64 + p) * kF2AB + wg * 64 * 128, c0 + 64 * p, tile * kBM + 64 * wg);
+          bulk_commit();
+        }
+      }
+    }
   }
+  if (a.demb_cols > 0 && (tid & 127) == 0) bulk_wait_all();
   // ---------------- per-CTA partials, layout of the head kernels: [dWc (K) | dbc (1) | column sums of dg2 (K)], loss, accuracy
   if (train) {
     a.wpart[(long long)blockIdx.x * a.wpart_stride + tid] = acc_dw;
@@ -898,19 +1046,27 @@ bool dib_int16_fwd2_ok(int K0, int N1, int N2, int out_dim) {
 }
 
 // g1 = act(g_in W0 + b0) -> HBM;  g2 = act(g1 W1 + b1) (on chip);  logit = g2 . wout + bout;  compiled loss / metric;
-// training (dg2 != null): dg2, per-CTA partials of the output layer's gradients and of the last hidden layer's bias gradient.
-// *nblocks = CTAs launched = rows of wpart / loss_part / acc_part written.
+// training (dg2 != null): dg2, per-CTA partials of the output layer's gradients and of the last hidden layer's bias gradient;
+// and with dg1 != null the dgrad of the second layer, dg1 = (dg2 W1^T) act'(g1) with its per-tile column sums in dbpart
+// [ceil(M/128)][256] (as dib_int16_dgrad), and with demb != null (g_in has no activation: the embedding) also
+// demb [M x K0] = dg1 W0^T.  *nblocks = CTAs launched = rows of wpart / loss_part / acc_part written.
 cudaError_t dib_int16_fwd2_head(const void* g_in, int ld_in, int K0, const void* w16_0, const float* b0, const void* w16_1, const float* b1,
                                 void* g1, const float* wout, const float* bout, int act, int out_act, float alpha, int loss, const float* y,
-                                int M, float inv_batch, float gscale, void* dg2, float* user_pred, float* wpart, int wpart_stride,
-                                float* loss_part, float* acc_part, int* nblocks, int bf16, cudaStream_t st) {
+                                int M, float inv_batch, float gscale, void* dg2, void* dg1, float* dbpart, void* demb, float* user_pred,
+                                float* wpart, int wpart_stride, float* loss_part, float* acc_part, int* nblocks, int bf16, cudaStream_t st) {
   if (!encode_fn3()) return cudaErrorNotSupported;
+  if ((dg1 && (!dg2 || !dbpart)) || (demb && !dg1)) return cudaErrorInvalidValue;
   CUtensorMap mA, mW0, mW1;
   if (!map_k(&mA, g_in, K0, M, ld_in, kBM) || !map_mn(&mW0, w16_0, kF2N, K0, kF2N, kF2N / 64) || !map_mn(&mW1, w16_1, kF2N, kF2N, kF2N, kF2N / 64))
     return cudaErrorInvalidValue;
+  // backward stages: W1 and W0 K-major (box 64 x 128, as dib_int16_dgrad reads them), the d emb store map (box 64 x 64)
+  CUtensorMap mW1t = mA, mW0t = mA, mDemb = mA;
+  if (dg1 && !map_k(&mW1t, w16_1, kF2N, kF2N, kF2N, kF2BtN)) return cudaErrorInvalidValue;
+  if (demb && (!map_k(&mW0t, w16_0, kF2N, K0, kF2N, kF2BtN) || !map_k(&mDemb, demb, K0, M, K0, 64))) return cudaErrorInvalidValue;
   Fwd2Args a{};
   a.b0 = b0; a.b1 = b1; a.wout = wout; a.bout = bout; a.g1 = static_cast<uint16_t*>(g1); a.ldg1 = kF2N;
   a.dg2 = static_cast<uint16_t*>(dg2); a.lddg = kF2N; a.y = y; a.user_pred = user_pred; a.wpart = wpart; a.wpart_stride = wpart_stride;
+  a.dg1 = static_cast<uint16_t*>(dg1); a.dbpart = dbpart; a.demb_cols = demb ? K0 : 0;
   a.loss_part = loss_part; a.acc_part = acc_part; a.M = M; a.nk0 = K0 / kBK; a.act = act; a.out_act = out_act; a.loss = loss;
   a.alpha = alpha; a.inv_batch = inv_batch; a.gscale = gscale;
   const int tiles = DIB_CEIL_DIV(M, kBM);
@@ -924,7 +1080,7 @@ cudaError_t dib_int16_fwd2_head(const void* g_in, int ld_in, int K0, const void*
     e = attr ? cudaSuccess : cudaFuncSetAttribute(dib_int16_fwd2_kernel<BF, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, kF2Smem); \
     if (e != cudaSuccess) return e;                                                                                                  \
     attr = true;                                                                                                                     \
-    dib_int16_fwd2_kernel<BF, ACT><<<grid, kF2Threads, kF2Smem, st>>>(mA, mW0, mW1, a);                                               \
+    dib_int16_fwd2_kernel<BF, ACT><<<grid, kF2Threads, kF2Smem, st>>>(mA, mW0, mW1, mW1t, mW0t, mDemb, a);                           \
   } while (0)
 #define DIB_F2_ACT(ACT) do { if (bf16) DIB_F2_LAUNCH(true, ACT); else DIB_F2_LAUNCH(false, ACT); } while (0)
   switch (act) {

@@ -196,8 +196,8 @@ int dib_int16_head_blocks(int num_sms);
 bool dib_int16_fwd2_ok(int K0, int N1, int N2, int out_dim);
 cudaError_t dib_int16_fwd2_head(const void* g_in, int ld_in, int K0, const void* w16_0, const float* b0, const void* w16_1, const float* b1,
                                 void* g1, const float* wout, const float* bout, int act, int out_act, float alpha, int loss, const float* y,
-                                int M, float inv_batch, float gscale, void* dg2, float* user_pred, float* wpart, int wpart_stride,
-                                float* loss_part, float* acc_part, int* nblocks, int bf16, cudaStream_t st);
+                                int M, float inv_batch, float gscale, void* dg2, void* dg1, float* dbpart, void* demb, float* user_pred,
+                                float* wpart, int wpart_stride, float* loss_part, float* acc_part, int* nblocks, int bf16, cudaStream_t st);
 // head1: the out = 1 kernel (8 rows per pass) instead of the generic one
 cudaError_t dib_int16_head(const void* g, int ldg, int K, const float* Wc, const float* bc, int out_dim, int out_act, int hid_act,
                            float alpha, int loss, const float* y, long long n, float inv_batch, float gscale, void* dg, int lddg,

@@ -59,6 +59,16 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const void* map, uint3
       "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
+// shared -> global tile store (bulk async group of the issuing thread; out-of-range rows / columns of the box are not written)
+__device__ __forceinline__ void tma_store_2d(const void* map, uint32_t src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(map), "r"(src), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of the issuing thread's committed store groups have not yet read their shared-memory source / all are complete
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 // ------------------------------------------------------------------------------------------------ cp.async
 // 4-byte global -> shared copy of this thread; cp_async_wait_all returns once every copy this thread committed has landed
 __device__ __forceinline__ void cp_async_4(uint32_t dst, const void* src) {

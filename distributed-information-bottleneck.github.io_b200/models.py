@@ -797,7 +797,8 @@ class DistributedIBNet:
         """Bring-up switch: keep the tensor-core mode on the reference kernels (fused-vs-unfused comparisons).
 
         ``on`` is a bit mask (``True`` = 1): 1 = unfused encoders, 2 = fp32-storage TF32 integration network, 4 = no fused
-        integration tail (per-layer 16-bit GEMMs plus a head kernel), 8 = the generic head kernel even when out = 1."""
+        integration tail (per-layer 16-bit GEMMs plus a head kernel), 8 = the generic head kernel even when out = 1, 16 = the
+        fused tail without its dgrad stages (separate dgrad launches in the backward)."""
         self._force_unfused = int(on)
         if self._handle is not None:
             _lib.check(self._lib.dib_debug_force_unfused(self._handle, int(on)))

@@ -362,7 +362,8 @@ int dib_debug_gemm_tc(int32_t mode, const float* A, int32_t lda, const float* B,
 
 /* bring-up switch for THIS handle (bit mask, 0 = the default kernels): 1 = unfused encoder kernels, 2 = integration network on
  * fp32-storage TF32 kernels, 4 = no fused integration tail (per-layer 16-bit GEMMs plus a head kernel), 8 = the generic head
- * kernel even when output_dimensionality == 1.  dib_model_info reports the resulting path. */
+ * kernel even when output_dimensionality == 1, 16 = the fused tail without its dgrad stages (the backward launches those
+ * dgrads separately).  dib_model_info reports the resulting path. */
 int dib_debug_force_unfused(dib_model* h, int32_t on);
 
 /* text of the last error raised on this thread ("" if none). */
