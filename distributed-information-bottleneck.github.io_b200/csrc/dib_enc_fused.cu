@@ -759,10 +759,8 @@ __global__ void dib_enc_pack_weights_kernel(const float* __restrict__ params, co
     const int k = i / EO, n = i - k * EO;
     v = k == w_in ? params[b2_off[f] + n] + (n >= EO / 2 ? logvar_offset : 0.f) : 0.f;
   }
-  uint16_t h;
-  if constexpr (BF16) { __nv_bfloat16 b = __float2bfloat16_rn(v); h = *reinterpret_cast<uint16_t*>(&b); }
-  else { __half b = __float2half_rn(v); h = *reinterpret_cast<uint16_t*>(&b); }
-  out[(long long)f * kPackElems + idx] = h;
+  // saturating like every activation operand: a weight beyond fp16's 65 504 packs as +-65 504, not inf
+  out[(long long)f * kPackElems + idx] = (uint16_t)(pack2<BF16>(v, 0.f) & 0xffffu);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,

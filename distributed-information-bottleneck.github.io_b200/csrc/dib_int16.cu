@@ -962,11 +962,8 @@ __global__ void dib_f32_to_16_segs_kernel(const ConvSegs A) {
   int k = 0;
 #pragma unroll
   for (int q = 1; q < 8; ++q) if (q < A.nseg && i >= A.first[q]) k = q;
-  const float v = A.src[k][i - A.first[k]];
-  uint16_t o;
-  if constexpr (BF16) { const __nv_bfloat16 b = __float2bfloat16_rn(v); o = *reinterpret_cast<const uint16_t*>(&b); }
-  else { const __half b = __float2half_rn(v); o = *reinterpret_cast<const uint16_t*>(&b); }
-  A.dst[k][i - A.first[k]] = o;
+  // saturating like every activation operand: a weight beyond fp16's 65 504 converts to +-65 504, not inf
+  A.dst[k][i - A.first[k]] = (uint16_t)(pack_h2<BF16>(A.src[k][i - A.first[k]], 0.f) & 0xffffu);
 }
 }  // namespace
 
