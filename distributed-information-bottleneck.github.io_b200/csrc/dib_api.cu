@@ -33,6 +33,18 @@ struct Buf {
   long long feat_stride = 0;  // distance between consecutive features (0 for single matrices)
 };
 
+// a stack of Dense layers 0..L on the per-layer grouped GEMMs (dib_gemm_simt.cu in fp32, dib_gemm_tc.cu otherwise): every
+// layer is one launch per GEMM mode over G groups -- the F feature encoders, Q / K / V, else one.  build_stack emits its
+// problems, stack_forward / stack_backward run them.
+struct Stack {
+  int G = 1;
+  std::vector<int> fwd, dgrad, wgrad;   // [j]: first of layer j's G problems in d_probs (dgrad[0] = -1 without dgrad0)
+  std::vector<int> fan_in, fan_out;     // [j]: largest fan-in over the groups (DGRAD maxC, WGRAD maxR), fan-out
+  bool dgrad0 = false;                  // layer 0 has a DGRAD: the gradient of the stack's input is wanted
+  float drop = 0.f;                     // Keras Dropout after every hidden layer (the feature encoders only)
+  const char* label = nullptr;          // profile ranges <label>_fwd_l<j> ...; none: the stack runs inside its caller's range
+};
+
 constexpr int kMaxSplits = 32;
 constexpr int kRowsPerBlock = 256;
 
@@ -67,9 +79,7 @@ struct dib_model {
   int* d_col_src = nullptr;
   int* d_col_freq = nullptr;
   int* d_col_feat = nullptr;   // feature owning each first-layer operand column (row gather of dib_compression_matrices)
-  std::vector<int> enc_fwd, enc_dgrad, enc_wgrad;  // start index into d_probs per layer j
-  std::vector<int> int_fwd, int_dgrad, int_wgrad;
-  std::vector<int> enc_maxK;                        // max over features of fan-in of layer j
+  Stack enc_stack, int_stack;  // the feature encoders (not the SimpleEncoder), the integration network / set-transformer head
   // fused per-feature encoder kernels (tensor-core mode; dib_enc_fused.cu)
   bool fused_ok = false;
   DibEncFusedDesc fdesc;
@@ -105,7 +115,7 @@ struct dib_model {
   long long nce_off = 0;            // 3 * max_batch floats of InfoNCE scratch
   long long nce_stats_off = 0;      // F + 3 floats: the stats dib_infonce_shard_lse wrote, for the backward's IB weight
   int nce_nblk_kl = 0;              // KL partials per feature dib_infonce_shard_forward left for dib_infonce_shard_lse
-  std::vector<int> y_fwd, y_dgrad, y_wgrad;
+  Stack y_stack;
   int* d_ycol_src = nullptr;
   int* d_ycol_freq = nullptr;
   // DIB_INTEGRATION_SET_TRANSFORMER (nb-particle cell 8, dib_set_attn.cu): the encoder and the attention blocks run on
@@ -121,8 +131,7 @@ struct dib_model {
     Buf q, k, v, o, a, hh, xout;                      // Q, K, V, attention output (heads concatenated), its projection, LN1, LN2
     std::vector<Buf> ff;                              // index 1..nff: output of FF layer j-1
     long long lse = 0, mean1 = 0, rstd1 = 0, mean2 = 0, rstd2 = 0;
-    int qkv_fwd = -1, o_fwd = -1, qkv_dgrad = -1, o_dgrad = -1, qkv_wgrad = -1, o_wgrad = -1;
-    std::vector<int> ff_fwd, ff_dgrad, ff_wgrad;
+    Stack qkv_stack, o_stack, ff_stack;               // Q / K / V (G = 3), the output projection, the FF stack
   };
   std::vector<StBlock> blk;
   Buf dq, dk, dv, d_o, dz1, dz2, dh_ff, dxq, dxk, dxv, pooled, d_pooled;   // backward scratch shared by the blocks
@@ -287,18 +296,84 @@ void plan(dib_model* h) {
   h->ws_floats = c;
 }
 
-// the dense layers of the attention blocks, all on n * Ls particle rows: Q / K / V as one group of three problems (same
-// input, kernels [E, h*dk]), the output projection [h*dk, E], the FF stack; each in the three GEMM modes
-void build_set_problems(dib_model* h, std::vector<DibGemmProblem>& v) {
-  auto zero = [] { DibGemmProblem p; memset(&p, 0, sizeof(p)); return p; };
-  const int E = h->E, hdk = h->hdk, nf = nff(h);
-  auto prob = [&](const Buf& a, long long b_off, int ldb, long long c_off, int ldc, long long x_off, int ldx, int T, int C, int R,
-                  int act) {
-    DibGemmProblem p = zero();
-    p.a_off = a.off; p.lda = a.ld; p.b_off = b_off; p.ldb = ldb; p.c_off = c_off; p.ldc = ldc; p.x_off = x_off; p.ldx = ldx;
-    p.T = T; p.C = C; p.R = R; p.act = act;
-    v.push_back(p);
-  };
+// a float offset and leading dimension inside the workspace
+struct Operand { long long off = 0; int ld = 0; };
+Operand opnd(const Buf& b, int g = 0) { return {b.off + g * b.feat_stride, b.ld}; }
+
+// what build_stack asks of group g at boundary k = 0..L+1 of a stack: the input of layer k, the output of layer k-1
+struct StackPoint {
+  int width = 0;            // columns: layer k's fan-in, layer k-1's fan-out
+  Operand in;               // what layer k reads (Dropout's output when there is one)
+  Operand act;              // what layer k-1 writes, after its activation and before Dropout: layer k's DGRAD takes act' of it
+  Operand grad;             // d (layer k-1's pre-activation output), which layer k's DGRAD writes; k = 0: d (the stack's input)
+  long long W = 0, b = 0;   // layer k's kernel [width, next width] and bias
+};
+
+// the FWD, DGRAD and WGRAD problems of layers 0..L: the hidden layers apply act, layer L out_act; the DGRAD of layer 0
+// (dgrad0) differentiates no activation
+template <class At>
+Stack build_stack(std::vector<DibGemmProblem>& v, int G, int L, int act, int out_act, bool dgrad0, At at) {
+  Stack s;
+  s.G = G; s.dgrad0 = dgrad0;
+  s.fwd.assign(L + 1, -1); s.dgrad.assign(L + 1, -1); s.wgrad.assign(L + 1, -1);
+  s.fan_in.assign(L + 1, 0); s.fan_out.assign(L + 1, 0);
+  for (int j = 0; j <= L; ++j) {
+    s.fan_out[j] = at(0, j + 1).width;
+    for (int g = 0; g < G; ++g)
+      if (at(g, j).width > s.fan_in[j]) s.fan_in[j] = at(g, j).width;
+  }
+  std::vector<int>* first[3] = {&s.fwd, &s.dgrad, &s.wgrad};
+  for (int mode = DIB_GEMM_FWD; mode <= DIB_GEMM_WGRAD; ++mode)
+    for (int j = mode == DIB_GEMM_DGRAD && !dgrad0 ? 1 : 0; j <= L; ++j) {
+      (*first[mode])[j] = (int)v.size();
+      for (int g = 0; g < G; ++g) {
+        const StackPoint x = at(g, j), y = at(g, j + 1);
+        DibGemmProblem p;
+        memset(&p, 0, sizeof(p));
+        if (mode == DIB_GEMM_FWD) {            // y.act = act(x.in W + b)
+          p.a_off = x.in.off; p.lda = x.in.ld; p.b_off = x.W; p.ldb = y.width; p.c_off = y.act.off; p.ldc = y.act.ld;
+          p.x_off = x.b; p.T = x.width; p.C = y.width; p.act = j < L ? act : out_act;
+        } else if (mode == DIB_GEMM_DGRAD) {   // x.grad = y.grad W^T * act'(x.act)
+          p.a_off = y.grad.off; p.lda = y.grad.ld; p.b_off = x.W; p.ldb = y.width; p.c_off = x.grad.off; p.ldc = x.grad.ld;
+          if (j > 0) { p.x_off = x.act.off; p.ldx = x.act.ld; }
+          p.T = y.width; p.C = x.width; p.act = j > 0 ? act : DIB_ACT_LINEAR;
+        } else {                               // dW = x.in^T y.grad, db = column sums of y.grad
+          p.a_off = x.in.off; p.lda = x.in.ld; p.b_off = y.grad.off; p.ldb = y.grad.ld; p.c_off = x.W; p.ldc = y.width;
+          p.x_off = x.b; p.R = x.width; p.C = y.width;
+        }
+        v.push_back(p);
+      }
+    }
+  return s;
+}
+
+void build_problems(dib_model* h, std::vector<DibGemmProblem>& v) {
+  const int L = h->L, Li = h->Li, Ly = h->Ly, E = h->E, hdk = h->hdk, nf = nff(h);
+  if (!h->simple) {
+    h->enc_stack = build_stack(v, h->F, L, h->act, DIB_ACT_LINEAR, false, [&](int f, int k) {
+      StackPoint p;
+      if (k > L) { p.width = 2 * E; p.act = opnd(h->enc_out, f); p.grad = opnd(h->d_out, f); return p; }
+      p.width = enc_fan_in(h, f, k);
+      p.in = k == 0 ? Operand{h->pe.off + h->pe_off[f], h->ldpe} : opnd(h->drop > 0.f ? h->enc_drop[k] : h->enc_act[k], f);
+      p.act = opnd(h->enc_act[k], f); p.grad = opnd(h->d_enc[k], f);
+      p.W = h->encW[f][k]; p.b = h->encB[f][k];
+      return p;
+    });
+    h->enc_stack.drop = h->drop;
+    h->enc_stack.label = "enc";
+  }
+  h->int_stack = build_stack(v, 1, Li, h->act, h->out_act, true, [&](int, int k) {   // the set transformer's head reads the set means
+    StackPoint p;
+    if (k > Li) { p.width = h->out; p.act = opnd(h->pred); p.grad = opnd(h->d_pred); return p; }
+    p.width = int_fan_in(h, k);
+    if (k == 0) { p.in = opnd(h->st ? h->pooled : h->emb); p.grad = opnd(h->st ? h->d_pooled : h->d_emb); }
+    else { p.in = p.act = opnd(h->int_act[k]); p.grad = opnd(h->d_int[k]); }
+    p.W = h->intW[k]; p.b = h->intB[k];
+    return p;
+  });
+  h->int_stack.label = "int";
+  // the dense layers of the attention blocks, all on n * Ls particle rows: Q / K / V as one group of three (same input,
+  // kernels [E, h*dk]), the output projection [h*dk, E], the FF stack on LN1's output
   for (int b = 0; b < h->nblk; ++b) {
     dib_model::StBlock& k = h->blk[b];
     const Buf& x = b == 0 ? h->emb : h->blk[b - 1].xout;
@@ -306,188 +381,38 @@ void build_set_problems(dib_model* h, std::vector<DibGemmProblem>& v) {
     const Buf* qkv[3] = {&k.q, &k.k, &k.v};
     const Buf* dqkv[3] = {&h->dq, &h->dk, &h->dv};
     const Buf* dx[3] = {&h->dxq, &h->dxk, &h->dxv};
-    k.qkv_fwd = (int)v.size();
-    for (int i = 0; i < 3; ++i) prob(x, W[i], hdk, qkv[i]->off, qkv[i]->ld, bias[i], 0, E, hdk, 0, DIB_ACT_LINEAR);
-    k.o_fwd = (int)v.size();
-    prob(k.o, k.Wo, E, k.a.off, k.a.ld, k.bo, 0, hdk, E, 0, DIB_ACT_LINEAR);
-    k.ff_fwd.assign(nf, -1); k.ff_dgrad.assign(nf, -1); k.ff_wgrad.assign(nf, -1);
-    for (int j = 0; j < nf; ++j) {
-      k.ff_fwd[j] = (int)v.size();
-      prob(j == 0 ? k.hh : k.ff[j], k.ffW[j], h->ff_arch[j], k.ff[j + 1].off, k.ff[j + 1].ld, k.ffB[j], 0, ff_fan_in(h, j), h->ff_arch[j], 0,
-           h->ff_act);
-    }
-    for (int j = 0; j < nf; ++j) {       // d (pre-activation of FF layer j) -> d (its input); layer 0's input is H (no activation)
-      k.ff_dgrad[j] = (int)v.size();
-      const Buf& o = j == 0 ? h->dh_ff : h->d_ff[j];
-      prob(h->d_ff[j + 1], k.ffW[j], h->ff_arch[j], o.off, o.ld, j == 0 ? 0 : k.ff[j].off, j == 0 ? 0 : k.ff[j].ld, h->ff_arch[j],
-           ff_fan_in(h, j), 0, j == 0 ? DIB_ACT_LINEAR : h->ff_act);
-      k.ff_wgrad[j] = (int)v.size();
-      DibGemmProblem p = zero();
-      const Buf& a = j == 0 ? k.hh : k.ff[j];
-      p.a_off = a.off; p.lda = a.ld; p.b_off = h->d_ff[j + 1].off; p.ldb = h->d_ff[j + 1].ld;
-      p.c_off = k.ffW[j]; p.ldc = h->ff_arch[j]; p.x_off = k.ffB[j]; p.R = ff_fan_in(h, j); p.C = h->ff_arch[j];
-      v.push_back(p);
-    }
-    k.o_dgrad = (int)v.size();
-    prob(h->dz1, k.Wo, E, h->d_o.off, h->d_o.ld, 0, 0, E, hdk, 0, DIB_ACT_LINEAR);
-    k.o_wgrad = (int)v.size();
-    {
-      DibGemmProblem p = zero();
-      p.a_off = k.o.off; p.lda = k.o.ld; p.b_off = h->dz1.off; p.ldb = h->dz1.ld;
-      p.c_off = k.Wo; p.ldc = E; p.x_off = k.bo; p.R = hdk; p.C = E;
-      v.push_back(p);
-    }
-    k.qkv_dgrad = (int)v.size();
-    for (int i = 0; i < 3; ++i) prob(*dqkv[i], W[i], hdk, dx[i]->off, dx[i]->ld, 0, 0, hdk, E, 0, DIB_ACT_LINEAR);
-    k.qkv_wgrad = (int)v.size();
-    for (int i = 0; i < 3; ++i) {
-      DibGemmProblem p = zero();
-      p.a_off = x.off; p.lda = x.ld; p.b_off = dqkv[i]->off; p.ldb = dqkv[i]->ld;
-      p.c_off = W[i]; p.ldc = hdk; p.x_off = bias[i]; p.R = E; p.C = hdk;
-      v.push_back(p);
-    }
+    k.qkv_stack = build_stack(v, 3, 0, DIB_ACT_LINEAR, DIB_ACT_LINEAR, true, [&](int i, int q) {
+      StackPoint p;
+      if (q == 0) { p.width = E; p.in = opnd(x); p.grad = opnd(*dx[i]); p.W = W[i]; p.b = bias[i]; }
+      else { p.width = hdk; p.act = opnd(*qkv[i]); p.grad = opnd(*dqkv[i]); }
+      return p;
+    });
+    k.o_stack = build_stack(v, 1, 0, DIB_ACT_LINEAR, DIB_ACT_LINEAR, true, [&](int, int q) {
+      StackPoint p;
+      if (q == 0) { p.width = hdk; p.in = opnd(k.o); p.grad = opnd(h->d_o); p.W = k.Wo; p.b = k.bo; }
+      else { p.width = E; p.act = opnd(k.a); p.grad = opnd(h->dz1); }
+      return p;
+    });
+    k.ff_stack = build_stack(v, 1, nf - 1, h->ff_act, h->ff_act, true, [&](int, int q) {
+      StackPoint p;
+      p.width = ff_fan_in(h, q);
+      p.in = opnd(q == 0 ? k.hh : k.ff[q]); p.act = opnd(k.ff[q]); p.grad = opnd(q == 0 ? h->dh_ff : h->d_ff[q]);
+      if (q < nf) { p.W = k.ffW[q]; p.b = k.ffB[q]; }
+      return p;
+    });
   }
-}
-
-void build_problems(dib_model* h, std::vector<DibGemmProblem>& v) {
-  auto zero = [] { DibGemmProblem p; memset(&p, 0, sizeof(p)); return p; };
-  const int F = h->F, L = h->L, Li = h->Li;
-  h->enc_fwd.assign(L + 1, -1); h->enc_dgrad.assign(L + 1, -1); h->enc_wgrad.assign(L + 1, -1);
-  h->int_fwd.assign(Li + 1, -1); h->int_dgrad.assign(Li + 1, -1); h->int_wgrad.assign(Li + 1, -1);
-  h->enc_maxK.assign(L + 1, 0);
-  auto encA = [&](int f, int j, long long& off, int& ld) {   // input of encoder layer j (after Dropout when there is one)
-    if (j == 0) { off = h->pe.off + h->pe_off[f]; ld = h->ldpe; }
-    else {
-      const Buf& b = h->drop > 0.f ? h->enc_drop[j] : h->enc_act[j];
-      off = b.off + f * b.feat_stride; ld = b.ld;
-    }
-  };
-  auto encDZ = [&](int f, int j, long long& off, int& ld) {  // grad wrt pre-activation output of layer j
-    const Buf& b = j == L ? h->d_out : h->d_enc[j + 1];
-    off = b.off + f * b.feat_stride; ld = b.ld;
-  };
-  for (int j = 0; j <= L && !h->simple; ++j) {
-    h->enc_fwd[j] = (int)v.size();
-    for (int f = 0; f < F; ++f) {
-      DibGemmProblem p = zero();
-      encA(f, j, p.a_off, p.lda);
-      p.b_off = h->encW[f][j]; p.ldb = enc_fan_out(h, j);
-      const Buf& o = j < L ? h->enc_act[j + 1] : h->enc_out;
-      p.c_off = o.off + f * o.feat_stride; p.ldc = o.ld;
-      p.x_off = h->encB[f][j];
-      p.T = enc_fan_in(h, f, j); p.C = enc_fan_out(h, j); p.act = j < L ? h->act : DIB_ACT_LINEAR;
-      if (p.T > h->enc_maxK[j]) h->enc_maxK[j] = p.T;
-      v.push_back(p);
-    }
-  }
-  for (int j = 1; j <= L && !h->simple; ++j) {
-    h->enc_dgrad[j] = (int)v.size();
-    for (int f = 0; f < F; ++f) {
-      DibGemmProblem p = zero();
-      encDZ(f, j, p.a_off, p.lda);
-      p.b_off = h->encW[f][j]; p.ldb = enc_fan_out(h, j);
-      p.c_off = h->d_enc[j].off + f * h->d_enc[j].feat_stride; p.ldc = h->d_enc[j].ld;
-      p.x_off = h->enc_act[j].off + f * h->enc_act[j].feat_stride; p.ldx = h->enc_act[j].ld;
-      p.T = enc_fan_out(h, j); p.C = enc_fan_in(h, f, j); p.act = h->act;
-      v.push_back(p);
-    }
-  }
-  for (int j = 0; j <= L && !h->simple; ++j) {
-    h->enc_wgrad[j] = (int)v.size();
-    for (int f = 0; f < F; ++f) {
-      DibGemmProblem p = zero();
-      encA(f, j, p.a_off, p.lda);
-      encDZ(f, j, p.b_off, p.ldb);
-      p.c_off = h->encW[f][j]; p.ldc = enc_fan_out(h, j);
-      p.x_off = h->encB[f][j];
-      p.R = enc_fan_in(h, f, j); p.C = enc_fan_out(h, j);
-      v.push_back(p);
-    }
-  }
-  const Buf& int_in = h->st ? h->pooled : h->emb;     // the set transformer's head reads the set means
-  auto intA = [&](int j, long long& off, int& ld) {
-    if (j == 0) { off = int_in.off; ld = int_in.ld; } else { off = h->int_act[j].off; ld = h->int_act[j].ld; }
-  };
-  auto intDZ = [&](int j, long long& off, int& ld) {
-    const Buf& b = j == Li ? h->d_pred : h->d_int[j + 1];
-    off = b.off; ld = b.ld;
-  };
-  for (int j = 0; j <= Li; ++j) {
-    h->int_fwd[j] = (int)v.size();
-    DibGemmProblem p = zero();
-    intA(j, p.a_off, p.lda);
-    p.b_off = h->intW[j]; p.ldb = int_fan_out(h, j);
-    const Buf& o = j < Li ? h->int_act[j + 1] : h->pred;
-    p.c_off = o.off; p.ldc = o.ld;
-    p.x_off = h->intB[j];
-    p.T = int_fan_in(h, j); p.C = int_fan_out(h, j); p.act = j < Li ? h->act : h->out_act;
-    v.push_back(p);
-  }
-  for (int j = 0; j <= Li; ++j) {
-    h->int_dgrad[j] = (int)v.size();
-    DibGemmProblem p = zero();
-    intDZ(j, p.a_off, p.lda);
-    p.b_off = h->intW[j]; p.ldb = int_fan_out(h, j);
-    const Buf& o = j == 0 ? (h->st ? h->d_pooled : h->d_emb) : h->d_int[j];
-    p.c_off = o.off; p.ldc = o.ld;
-    if (j > 0) { p.x_off = h->int_act[j].off; p.ldx = h->int_act[j].ld; p.act = h->act; }
-    else { p.act = DIB_ACT_LINEAR; }
-    p.T = int_fan_out(h, j); p.C = int_fan_in(h, j);
-    v.push_back(p);
-  }
-  for (int j = 0; j <= Li; ++j) {
-    h->int_wgrad[j] = (int)v.size();
-    DibGemmProblem p = zero();
-    intA(j, p.a_off, p.lda);
-    intDZ(j, p.b_off, p.ldb);
-    p.c_off = h->intW[j]; p.ldc = int_fan_out(h, j);
-    p.x_off = h->intB[j];
-    p.R = int_fan_in(h, j); p.C = int_fan_out(h, j);
-    v.push_back(p);
-  }
-  if (h->st) build_set_problems(h, v);
   if (!infonce(h)) return;
-  // the output encoder: the same three modes on its own buffers (train.py:186-193)
-  const int Ly = h->Ly;
-  h->y_fwd.assign(Ly + 1, -1); h->y_dgrad.assign(Ly + 1, -1); h->y_wgrad.assign(Ly + 1, -1);
-  auto yA = [&](int j, long long& off, int& ld) {
-    if (j == 0) { off = h->ype.off; ld = h->ldype; } else { off = h->y_act[j].off; ld = h->y_act[j].ld; }
-  };
-  auto yDZ = [&](int j, long long& off, int& ld) {
-    const Buf& b = j == Ly ? h->d_y_out : h->d_yact[j + 1];
-    off = b.off; ld = b.ld;
-  };
-  for (int j = 0; j <= Ly; ++j) {
-    h->y_fwd[j] = (int)v.size();
-    DibGemmProblem p = zero();
-    yA(j, p.a_off, p.lda);
-    p.b_off = h->yW[j]; p.ldb = y_fan_out(h, j);
-    const Buf& o = j < Ly ? h->y_act[j + 1] : h->y_out;
-    p.c_off = o.off; p.ldc = o.ld;
-    p.x_off = h->yB[j];
-    p.T = y_fan_in(h, j); p.C = y_fan_out(h, j); p.act = j < Ly ? h->act : DIB_ACT_LINEAR;
-    v.push_back(p);
-  }
-  for (int j = 1; j <= Ly; ++j) {         // no gradient is taken with respect to y itself
-    h->y_dgrad[j] = (int)v.size();
-    DibGemmProblem p = zero();
-    yDZ(j, p.a_off, p.lda);
-    p.b_off = h->yW[j]; p.ldb = y_fan_out(h, j);
-    p.c_off = h->d_yact[j].off; p.ldc = h->d_yact[j].ld;
-    p.x_off = h->y_act[j].off; p.ldx = h->y_act[j].ld; p.act = h->act;
-    p.T = y_fan_out(h, j); p.C = y_fan_in(h, j);
-    v.push_back(p);
-  }
-  for (int j = 0; j <= Ly; ++j) {
-    h->y_wgrad[j] = (int)v.size();
-    DibGemmProblem p = zero();
-    yA(j, p.a_off, p.lda);
-    yDZ(j, p.b_off, p.ldb);
-    p.c_off = h->yW[j]; p.ldc = y_fan_out(h, j);
-    p.x_off = h->yB[j];
-    p.R = y_fan_in(h, j); p.C = y_fan_out(h, j);
-    v.push_back(p);
-  }
+  // the output encoder on its own buffers (train.py:186-193); no gradient is taken with respect to y itself
+  h->y_stack = build_stack(v, 1, Ly, h->act, DIB_ACT_LINEAR, false, [&](int, int k) {
+    StackPoint p;
+    if (k > Ly) { p.width = h->out; p.act = opnd(h->y_out); p.grad = opnd(h->d_y_out); return p; }
+    p.width = y_fan_in(h, k);
+    p.in = k == 0 ? Operand{h->ype.off, h->ldype} : opnd(h->y_act[k]);
+    p.act = opnd(h->y_act[k]); p.grad = opnd(h->d_yact[k]);
+    p.W = h->yW[k]; p.b = h->yB[k];
+    return p;
+  });
+  h->y_stack.label = "y";
 }
 
 struct Ctx {
@@ -557,7 +482,57 @@ int check_sets(const dib_model* h, int64_t n) {
 
 // noise of one forward: the caller's eps, or Philox (seed, step, sample_offset); training turns Dropout on
 struct NoiseKey { const float* eps; uint64_t seed; uint32_t step; uint64_t sample_offset; bool training; };
-int encode_all(const Ctx& c, const float* x, int ldx, int rnd, const int* row_index, int64_t n_src, const NoiseKey* key = nullptr);
+int encode_all(const Ctx& c, const float* x, int ldx, int feature, const int* row_index, int64_t n_src, const NoiseKey* key = nullptr);
+
+// TF32 GEMMs read the weights through a TF32-rounded copy
+int tf32_shadow(const Ctx& c) {
+  if (!is_tc(c.h)) return 0;
+  prof_begin(c, "weights_tf32_shadow");
+  DIB_CUDA_OK(dib_launch_round_copy(c.params, c.ws + c.h->wshadow_off, c.h->P, c.st));
+  prof_end(c);
+  return 0;
+}
+
+// FWD of layers 0..L of `groups` groups from `first` (all, or one feature of the encoders).  Dropout (the encoders) runs after
+// each hidden layer: keyed by `key` in training, the identity copy otherwise.
+int stack_forward(const Ctx& c, const Stack& s, int first, int groups, const NoiseKey* key = nullptr) {
+  dib_model* h = c.h;
+  const int L = (int)s.fwd.size() - 1;
+  const bool tr = key && key->training;
+  for (int j = 0; j <= L; ++j) {
+    if (s.label) prof_begin(c, (std::string(s.label) + "_fwd_l").c_str(), j);
+    if (gemm(c, DIB_GEMM_FWD, s.fwd[j] + first, groups, s.fan_out[j], 0, 1, 0)) return 1;
+    if (j < L && s.drop > 0.f) {
+      const Buf& a = h->enc_act[j + 1];
+      DIB_CUDA_OK(dib_launch_dropout(c.ws + a.off, c.ws + h->enc_drop[j + 1].off, a.feat_stride, a.ld, s.fan_out[j], s.G, c.n,
+                                     tr ? s.drop : 0.f, key ? key->seed : 0, key ? key->step : 0, tr ? c.step_dev() : nullptr,
+                                     key ? key->sample_offset : 0, j + 1, groups < s.G ? first : -1, 0, is_tc(h) ? 1 : 0, c.st));
+    }
+    if (s.label) prof_end(c);
+  }
+  return 0;
+}
+
+// for j = L..0: WGRAD of layer j into the split-partial table, then its DGRAD (layer 0: with dgrad0) and Dropout's backward
+// (the same keep mask as the training forward keyed by `key`, scaled)
+int stack_backward(const Ctx& c, const Stack& s, const Split& sp, const NoiseKey* key = nullptr) {
+  dib_model* h = c.h;
+  for (int j = (int)s.fwd.size() - 1; j >= 0; --j) {
+    if (s.label) prof_begin(c, (std::string(s.label) + "_wgrad_l").c_str(), j);
+    if (gemm(c, DIB_GEMM_WGRAD, s.wgrad[j], s.G, s.fan_out[j], s.fan_in[j], sp.nsplit, (int)sp.rps)) return 1;
+    if (s.label) prof_end(c);
+    if (j == 0 && !s.dgrad0) continue;
+    if (s.label) prof_begin(c, (std::string(s.label) + "_dgrad_l").c_str(), j);
+    if (gemm(c, DIB_GEMM_DGRAD, s.dgrad[j], s.G, s.fan_in[j], 0, 1, 0)) return 1;
+    if (s.drop > 0.f) {
+      const Buf& d = h->d_enc[j];
+      DIB_CUDA_OK(dib_launch_dropout(nullptr, c.ws + d.off, d.feat_stride, d.ld, s.fan_in[j], s.G, c.n, s.drop, key->seed, key->step,
+                                     c.step_dev(), key->sample_offset, j, -1, 1, is_tc(h) ? 1 : 0, c.st));
+    }
+    if (s.label) prof_end(c);
+  }
+  return 0;
+}
 
 DibReparamArgs reparam_args(const Ctx& c, const NoiseKey& nk) {
   const dib_model* h = c.h;
@@ -588,7 +563,7 @@ const void* int16_in(const Ctx& c, int j) {
 int forward_encoders(const Ctx& c, const float* x, const NoiseKey& nk, float* user_emb, bool enc_only, int* nblk_kl) {
   dib_model* h = c.h;
   if (!h->route.enc_fused) {
-    if (encode_all(c, x, h->D, is_tc(h) ? 1 : 0, nullptr, 0, &nk)) return 1;
+    if (encode_all(c, x, h->D, -1, nullptr, 0, &nk)) return 1;
     prof_begin(c, "reparam_kl_fwd");
     DIB_CUDA_OK(dib_launch_reparam_fwd(reparam_args(c, nk), c.ws + h->emb.off, h->emb.ld, user_emb, c.ws + h->kl_part_off,
                                        h->kl_stride, c.st));
@@ -631,12 +606,7 @@ int forward_output_encoder(const Ctx& c, const float* y) {
   DIB_CUDA_OK(dib_launch_pe(y, h->ydim, 0, h->d_ycol_src, h->d_ycol_freq, 0, h->ldype, c.ws + h->ype.off, h->ldype, 0, c.n,
                             is_tc(h) ? 1 : 0, c.st));
   prof_end(c);
-  for (int j = 0; j <= h->Ly; ++j) {
-    prof_begin(c, "y_fwd_l", j);
-    if (gemm(c, DIB_GEMM_FWD, h->y_fwd[j], 1, y_fan_out(h, j), 0, 1, 0)) return 1;
-    prof_end(c);
-  }
-  return 0;
+  return stack_forward(c, h->y_stack, 0, 1);
 }
 
 // the streaming InfoNCE of the c.n own rows [row0, row0 + c.n) of e1 / e2 [n, d] against all n rows: r and c at lse_stride,
@@ -692,17 +662,6 @@ int forward_infonce(const Ctx& c, const float* y, bool training, float* user_pre
   return 0;
 }
 
-// the integration layers on the per-layer GEMM route: emb -> pred
-int forward_int_gemms(const Ctx& c) {
-  dib_model* h = c.h;
-  for (int j = 0; j <= h->Li; ++j) {
-    prof_begin(c, "int_fwd_l", j);
-    if (gemm(c, DIB_GEMM_FWD, h->int_fwd[j], 1, int_fan_out(h, j), 0, 1, 0)) return 1;
-    prof_end(c);
-  }
-  return 0;
-}
-
 // integration half of the forward: integration layers -> prediction, compiled loss / metrics, d loss / d prediction
 // (training) -> the stats row
 int forward_integration(const Ctx& c, const float* y, float inv_batch, bool training, float* user_pred, float* out_stats,
@@ -713,7 +672,7 @@ int forward_integration(const Ctx& c, const float* y, float inv_batch, bool trai
                                      nblk_loss, h->F, c.n, y != nullptr, out_stats, c.st);
   };
   if (!h->route.int16) {
-    if (forward_int_gemms(c)) return 1;
+    if (stack_forward(c, h->int_stack, 0, 1)) return 1;
     if (infonce(h) && y) return forward_infonce(c, y, training, user_pred, out_stats, nblk_kl);
     prof_begin(c, "loss_stats");
     DIB_CUDA_OK(dib_launch_loss(h->loss, h->out_act, h->alpha, c.ws + h->pred.off, h->pred.ld, y, h->out, c.n, inv_batch,
@@ -773,21 +732,10 @@ int forward_integration(const Ctx& c, const float* y, float inv_batch, bool trai
   return 0;
 }
 
-// TF32 GEMMs read the weights through a TF32-rounded copy
-int weights_shadow(const Ctx& c) {
-  dib_model* h = c.h;
-  if (is_tc(h) && !h->route.int16) {
-    prof_begin(c, "weights_tf32_shadow");
-    DIB_CUDA_OK(dib_launch_round_copy(c.params, c.ws + h->wshadow_off, h->P, c.st));
-    prof_end(c);
-  }
-  return 0;
-}
-
 int run_forward(const Ctx& c, const float* x, const float* y, const NoiseKey& nk, float inv_batch, float* user_pred,
                 float* user_emb, float* out_stats, bool enc_only = false) {
   dib_model* h = c.h;
-  if (weights_shadow(c)) return 1;
+  if (!h->route.int16 && tf32_shadow(c)) return 1;     // the 16-bit route runs no TF32 GEMM
   int nblk_kl = 0;
   if (forward_encoders(c, x, nk, user_emb, enc_only, &nblk_kl)) return 1;
   if (enc_only) {
@@ -798,35 +746,27 @@ int run_forward(const Ctx& c, const float* x, const float* y, const NoiseKey& nk
   return forward_integration(c, y, inv_batch, nk.training, user_pred, out_stats, nblk_kl);
 }
 
-// every feature encoder on n rows of x (deterministic part: mu | logvar incl. the offset) into the enc_out workspace
-// buffer: positional encoding + grouped GEMMs (models.py:72-78,106), or nb-bool's SimpleEncoder constants
-int encode_all(const Ctx& c, const float* x, int ldx, int rnd, const int* row_index, int64_t n_src, const NoiseKey* key) {
+// every feature encoder (feature = -1), or feature `feature` alone reading only its columns of x, on n rows of x
+// (deterministic part: mu | logvar incl. the offset) into the enc_out workspace buffer: positional encoding + grouped GEMMs
+// (models.py:72-78,106), or nb-bool's SimpleEncoder constants
+int encode_all(const Ctx& c, const float* x, int ldx, int feature, const int* row_index, int64_t n_src, const NoiseKey* key) {
   dib_model* h = c.h;
+  const int f = feature;
   if (h->simple) {
     prof_begin(c, "simple_enc_fwd");
     DIB_CUDA_OK(dib_launch_simple_enc_fwd(x, ldx, h->d_xoff, c.params, c.ws + h->enc_out.off, h->enc_out.feat_stride,
-                                          h->enc_out.ld, h->F, h->E, c.n, -1, 0, row_index, n_src, c.st));
+                                          h->enc_out.ld, h->F, h->E, c.n, f, f >= 0 ? 1 : 0, row_index, n_src, c.st));
     prof_end(c);
   } else {
     prof_begin(c, "pe");
-    DIB_CUDA_OK(dib_launch_pe(x, ldx, 0, h->d_col_src, h->d_col_freq, 0, h->ldpe, c.ws + h->pe.off, h->ldpe, 0, c.n, rnd, c.st,
-                              row_index, row_index ? h->d_col_feat : nullptr, n_src));
+    DIB_CUDA_OK(dib_launch_pe(x, ldx, f >= 0 ? h->x_off[f] : 0, h->d_col_src, h->d_col_freq, f >= 0 ? h->pe_off[f] : 0,
+                              f >= 0 ? h->pe_off[f] + DIB_ROUND_UP(h->w_in[f], 4) : h->ldpe, c.ws + h->pe.off, h->ldpe, 0, c.n,
+                              is_tc(h) ? 1 : 0, c.st, row_index, row_index ? h->d_col_feat : nullptr, n_src));
     prof_end(c);
-    for (int j = 0; j <= h->L; ++j) {
-      prof_begin(c, "enc_fwd_l", j);
-      if (gemm(c, DIB_GEMM_FWD, h->enc_fwd[j], h->F, enc_fan_out(h, j), 0, 1, 0)) return 1;
-      if (j < h->L && h->drop > 0.f) {     // Keras Dropout after the hidden Dense (training) / identity copy (inference)
-        const bool tr = key && key->training;
-        DIB_CUDA_OK(dib_launch_dropout(c.ws + h->enc_act[j + 1].off, c.ws + h->enc_drop[j + 1].off, h->enc_act[j + 1].feat_stride,
-                                       h->enc_act[j + 1].ld, h->enc_arch[j], h->F, c.n, tr ? h->drop : 0.f, key ? key->seed : 0,
-                                       key ? key->step : 0, tr ? c.step_dev() : nullptr, key ? key->sample_offset : 0, j + 1, -1, 0,
-                                       rnd, c.st));
-      }
-      prof_end(c);
-    }
+    if (stack_forward(c, h->enc_stack, f >= 0 ? f : 0, f >= 0 ? 1 : h->F, key)) return 1;
   }
   DIB_CUDA_OK(dib_launch_add_logvar_offset(c.ws + h->enc_out.off, h->enc_out.feat_stride, h->enc_out.ld, h->F, h->E, c.n,
-                                           h->lv_off, -1, c.st));
+                                           h->lv_off, f, c.st));
   return 0;
 }
 
@@ -875,20 +815,8 @@ int backward_encoders(const Ctx& c, const float* x, const NoiseKey& nk, const fl
     DIB_CUDA_OK(dib_launch_simple_enc_wgrad(x, h->D, h->d_xoff, c.ws + h->d_out.off, h->d_out.feat_stride, h->d_out.ld, h->F, h->E,
                                             c.n, sp.nsplit, (int)sp.rps, part, h->Pp, c.st));
     prof_end(c);
-  }
-  for (int j = h->L; j >= 0 && !h->simple; --j) {
-    prof_begin(c, "enc_wgrad_l", j);
-    if (gemm(c, DIB_GEMM_WGRAD, h->enc_wgrad[j], h->F, enc_fan_out(h, j), h->enc_maxK[j], sp.nsplit, (int)sp.rps)) return 1;
-    prof_end(c);
-    if (j >= 1) {
-      prof_begin(c, "enc_dgrad_l", j);
-      if (gemm(c, DIB_GEMM_DGRAD, h->enc_dgrad[j], h->F, h->enc_arch[j - 1], 0, 1, 0)) return 1;
-      if (h->drop > 0.f)                   // Dropout backward: the same keep mask, scaled
-        DIB_CUDA_OK(dib_launch_dropout(nullptr, c.ws + h->d_enc[j].off, h->d_enc[j].feat_stride, h->d_enc[j].ld, h->enc_arch[j - 1],
-                                       h->F, c.n, h->drop, nk.seed, nk.step, c.step_dev(), nk.sample_offset, j, -1, 1,
-                                       is_tc(h) ? 1 : 0, c.st));
-      prof_end(c);
-    }
+  } else if (stack_backward(c, h->enc_stack, sp, &nk)) {
+    return 1;
   }
   *nrows = sp.nsplit;
   return 0;
@@ -904,14 +832,7 @@ int backward_integration(const Ctx& c, float inv_batch, const Split& sp, float* 
   float* part = c.ws + h->part_off;
   if (!h->route.int16) {
     const long long p_enc = h->intW[0];
-    for (int j = h->Li; j >= 0; --j) {
-      prof_begin(c, "int_wgrad_l", j);
-      if (gemm(c, DIB_GEMM_WGRAD, h->int_wgrad[j], 1, int_fan_out(h, j), int_fan_in(h, j), sp.nsplit, (int)sp.rps)) return 1;
-      prof_end(c);
-      prof_begin(c, "int_dgrad_l", j);
-      if (gemm(c, DIB_GEMM_DGRAD, h->int_dgrad[j], 1, int_fan_in(h, j), 0, 1, 0)) return 1;
-      prof_end(c);
-    }
+    if (stack_backward(c, h->int_stack, sp)) return 1;
     prof_begin(c, "int_split_reduce");
     DIB_CUDA_OK(dib_launch_reduce_partials(part + p_enc, h->Pp, sp.nsplit, h->Px - p_enc, grads_flat + p_enc, c.st));
     prof_end(c);
@@ -978,16 +899,7 @@ int backward_integration(const Ctx& c, float inv_batch, const Split& sp, float* 
 // the output encoder's backward from the d loss / d e2 forward_infonce left, into grads_flat[Px, P)
 int backward_output_encoder(const Ctx& c, const Split& sp, float* grads_flat) {
   dib_model* h = c.h;
-  for (int j = h->Ly; j >= 0; --j) {
-    prof_begin(c, "y_wgrad_l", j);
-    if (gemm(c, DIB_GEMM_WGRAD, h->y_wgrad[j], 1, y_fan_out(h, j), y_fan_in(h, j), sp.nsplit, (int)sp.rps)) return 1;
-    prof_end(c);
-    if (j >= 1) {
-      prof_begin(c, "y_dgrad_l", j);
-      if (gemm(c, DIB_GEMM_DGRAD, h->y_dgrad[j], 1, y_fan_in(h, j), 0, 1, 0)) return 1;
-      prof_end(c);
-    }
-  }
+  if (stack_backward(c, h->y_stack, sp)) return 1;
   prof_begin(c, "y_split_reduce");
   DIB_CUDA_OK(dib_launch_reduce_partials(c.ws + h->part_off + h->Px, h->Pp, sp.nsplit, h->P - h->Px, grads_flat + h->Px, c.st));
   prof_end(c);
@@ -1023,18 +935,17 @@ int forward_set_blocks(const Ctx& c) {
     const dib_model::StBlock& k = h->blk[b];
     const Buf& x = b == 0 ? h->emb : h->blk[b - 1].xout;
     prof_begin(c, "st_qkv_fwd_b", b);
-    if (gemm(c, DIB_GEMM_FWD, k.qkv_fwd, 3, h->hdk, 0, 1, 0)) return 1;
+    if (stack_forward(c, k.qkv_stack, 0, 3)) return 1;
     prof_end(c);
     prof_begin(c, "st_attn_fwd_b", b);
     DIB_CUDA_OK(dib_launch_attn_fwd(attn_args(c, k), c.st));
     prof_end(c);
     prof_begin(c, "st_out_proj_ln1_fwd_b", b);
-    if (gemm(c, DIB_GEMM_FWD, k.o_fwd, 1, h->E, 0, 1, 0)) return 1;
+    if (stack_forward(c, k.o_stack, 0, 1)) return 1;
     DIB_CUDA_OK(dib_launch_ln_fwd(ln_args(c, x, k.a, k.g1, k.be1, k.hh, k.mean1, k.rstd1), c.st));
     prof_end(c);
     prof_begin(c, "st_ff_ln2_fwd_b", b);
-    for (int j = 0; j < nff(h); ++j)
-      if (gemm(c, DIB_GEMM_FWD, k.ff_fwd[j], 1, h->ff_arch[j], 0, 1, 0)) return 1;
+    if (stack_forward(c, k.ff_stack, 0, 1)) return 1;
     DIB_CUDA_OK(dib_launch_ln_fwd(ln_args(c, k.hh, k.ff[nff(h)], k.g2, k.be2, k.xout, k.mean2, k.rstd2), c.st));
     prof_end(c);
   }
@@ -1072,25 +983,20 @@ int backward_set_blocks(const Ctx& c, const Split& sp) {
       DIB_CUDA_OK(ln_bwd(ln_args(c, k.hh, k.ff[nf], k.g2, k.be2, k.xout, k.mean2, k.rstd2), dy, last ? c.ws + h->d_pooled.off : nullptr,
                          h->dz2, &h->d_ff[nf], k.g2, k.be2));
     }
-    for (int j = nf - 1; j >= 0; --j) {
-      if (gemm(c, DIB_GEMM_WGRAD, k.ff_wgrad[j], 1, h->ff_arch[j], ff_fan_in(h, j), sp.nsplit, (int)sp.rps)) return 1;
-      if (gemm(c, DIB_GEMM_DGRAD, k.ff_dgrad[j], 1, ff_fan_in(h, j), 0, 1, 0)) return 1;
-    }
+    if (stack_backward(c, k.ff_stack, sp)) return 1;
     prof_end(c);
     prof_begin(c, "st_ln1_out_proj_bwd_b", b);
     {
       const float* dy[4] = {c.ws + h->dz2.off, c.ws + h->dh_ff.off, nullptr, nullptr};
       DIB_CUDA_OK(ln_bwd(ln_args(c, x, k.a, k.g1, k.be1, k.hh, k.mean1, k.rstd1), dy, nullptr, h->dz1, nullptr, k.g1, k.be1));
     }
-    if (gemm(c, DIB_GEMM_WGRAD, k.o_wgrad, 1, h->E, h->hdk, sp.nsplit, (int)sp.rps)) return 1;
-    if (gemm(c, DIB_GEMM_DGRAD, k.o_dgrad, 1, h->hdk, 0, 1, 0)) return 1;
+    if (stack_backward(c, k.o_stack, sp)) return 1;
     prof_end(c);
     prof_begin(c, "st_attn_bwd_b", b);
     DIB_CUDA_OK(dib_launch_attn_bwd(attn_args(c, k), c.st));
     prof_end(c);
     prof_begin(c, "st_qkv_bwd_b", b);
-    if (gemm(c, DIB_GEMM_WGRAD, k.qkv_wgrad, 3, h->hdk, h->E, sp.nsplit, (int)sp.rps)) return 1;
-    if (gemm(c, DIB_GEMM_DGRAD, k.qkv_dgrad, 3, h->E, 0, 1, 0)) return 1;
+    if (stack_backward(c, k.qkv_stack, sp)) return 1;
     prof_end(c);
   }
   // d emb = block 0's residual-path gradient + its Q / K / V input gradients (dib_create requires at least one block)
@@ -1111,11 +1017,7 @@ int run_forward_set(const Ctx& cs, const float* x, const float* y, const NoiseKe
   c.n = cs.n * h->Ls;
   NoiseKey nr = nk;
   nr.sample_offset = nk.sample_offset * (uint64_t)h->Ls;     // noise keyed by the global particle row
-  if (is_tc(h)) {
-    prof_begin(c, "weights_tf32_shadow");
-    DIB_CUDA_OK(dib_launch_round_copy(c.params, c.ws + h->wshadow_off, h->P, c.st));
-    prof_end(c);
-  }
+  if (tf32_shadow(c)) return 1;
   int nblk_kl = 0;
   if (forward_encoders(c, x, nr, user_emb, false, &nblk_kl)) return 1;
   if (forward_set_blocks(c)) return 1;
@@ -1563,24 +1465,9 @@ int dib_encode_feature(dib_model* h, const float* params, int32_t feature, const
   if (!out_mu_logvar) return fail("dib_encode_feature: null output");
   if (n == 0) return 0;
   Ctx c{h, params, static_cast<float*>(workspace), static_cast<cudaStream_t>(stream), (int)n};
-  const int f = feature, wpad = DIB_ROUND_UP(h->w_in[f], 4);
-  const int rnd = is_tc(h) ? 1 : 0;
-  if (h->simple) {
-    DIB_CUDA_OK(dib_launch_simple_enc_fwd(x_i, h->fdims[f], h->d_xoff, c.params, c.ws + h->enc_out.off, h->enc_out.feat_stride,
-                                          h->enc_out.ld, h->F, h->E, n, f, 1, nullptr, 0, c.st));
-  } else {
-    if (rnd) DIB_CUDA_OK(dib_launch_round_copy(c.params, c.ws + h->wshadow_off, h->P, c.st));
-    DIB_CUDA_OK(dib_launch_pe(x_i, h->fdims[f], h->x_off[f], h->d_col_src, h->d_col_freq, h->pe_off[f], h->pe_off[f] + wpad,
-                              c.ws + h->pe.off, h->ldpe, 0, n, rnd, c.st));
-    for (int j = 0; j <= h->L; ++j) {
-      if (gemm(c, DIB_GEMM_FWD, h->enc_fwd[j] + f, 1, enc_fan_out(h, j), 0, 1, 0)) return 1;
-      if (j < h->L && h->drop > 0.f)       // inference: Dropout is the identity
-        DIB_CUDA_OK(dib_launch_dropout(c.ws + h->enc_act[j + 1].off, c.ws + h->enc_drop[j + 1].off, h->enc_act[j + 1].feat_stride,
-                                       h->enc_act[j + 1].ld, h->enc_arch[j], h->F, n, 0.f, 0, 0, nullptr, 0, j + 1, f, 0, rnd, c.st));
-    }
-  }
-  DIB_CUDA_OK(dib_launch_add_logvar_offset(c.ws + h->enc_out.off, h->enc_out.feat_stride, h->enc_out.ld, h->F, h->E, n,
-                                           h->lv_off, f, c.st));
+  const int f = feature;
+  if (!h->simple && tf32_shadow(c)) return 1;
+  if (encode_all(c, x_i, h->fdims[f], f, nullptr, 0)) return 1;
   DIB_CUDA_OK(dib_launch_copy2d(c.ws + h->enc_out.off + f * h->enc_out.feat_stride, h->enc_out.ld, out_mu_logvar,
                                 2 * h->E, 2 * h->E, n, c.st));
   return 0;
@@ -1615,9 +1502,10 @@ int dib_infonce_shard_forward(dib_model* h, const float* params, const float* x,
   Ctx c{h, params, static_cast<float*>(workspace), static_cast<cudaStream_t>(stream), (int)n};
   c.dev_step = training != 0;
   const NoiseKey nk{eps, seed, step, sample_offset, training != 0};
-  if (weights_shadow(c)) return 1;
+  if (!h->route.int16 && tf32_shadow(c)) return 1;
   int nblk_kl = 0;
-  if (forward_encoders(c, x, nk, nullptr, false, &nblk_kl) || forward_int_gemms(c) || forward_output_encoder(c, y)) return 1;
+  if (forward_encoders(c, x, nk, nullptr, false, &nblk_kl) || stack_forward(c, h->int_stack, 0, 1) || forward_output_encoder(c, y))
+    return 1;
   h->nce_nblk_kl = nblk_kl;
   const int d = h->out;
   float* own = e_all + row_offset * 2 * d;
@@ -1688,7 +1576,7 @@ int dib_integration_forward(dib_model* h, const float* params, const float* emb,
   if (n == 0) return 0;
   Ctx c{h, params, static_cast<float*>(workspace), static_cast<cudaStream_t>(stream), (int)n};
   const int FE = h->F * h->E;
-  if (is_tc(h)) DIB_CUDA_OK(dib_launch_round_copy(c.params, c.ws + h->wshadow_off, h->P, c.st));
+  if (tf32_shadow(c)) return 1;
   if (h->st) {                 // emb [n, Ls, E] (E is a multiple of 4: no padded columns) through the blocks and the mean
     Ctx cr = c;
     cr.n = (int)n * h->Ls;
@@ -1700,8 +1588,7 @@ int dib_integration_forward(dib_model* h, const float* params, const float* emb,
   }
   if (!h->st && h->emb.ld > FE)          // zero the padded operand columns
     DIB_CUDA_OK(cudaMemset2DAsync(c.ws + h->emb.off + FE, sizeof(float) * h->emb.ld, 0, sizeof(float) * (h->emb.ld - FE), (size_t)n, c.st));
-  for (int j = 0; j <= h->Li; ++j)
-    if (gemm(c, DIB_GEMM_FWD, h->int_fwd[j], 1, int_fan_out(h, j), 0, 1, 0)) return 1;
+  if (stack_forward(c, h->int_stack, 0, 1)) return 1;
   DIB_CUDA_OK(dib_launch_copy2d(c.ws + h->pred.off, h->pred.ld, out_pred, h->out, h->out, n, c.st));
   return 0;
 }
@@ -1712,11 +1599,7 @@ int dib_output_encoder_forward(dib_model* h, const float* params, const float* y
   if (!out) return fail("dib_output_encoder_forward: null output");
   if (n == 0) return 0;
   Ctx c{h, params, static_cast<float*>(workspace), static_cast<cudaStream_t>(stream), (int)n};
-  const int rnd = is_tc(h) ? 1 : 0;
-  if (rnd) DIB_CUDA_OK(dib_launch_round_copy(c.params, c.ws + h->wshadow_off, h->P, c.st));
-  DIB_CUDA_OK(dib_launch_pe(y, h->ydim, 0, h->d_ycol_src, h->d_ycol_freq, 0, h->ldype, c.ws + h->ype.off, h->ldype, 0, c.n, rnd, c.st));
-  for (int j = 0; j <= h->Ly; ++j)
-    if (gemm(c, DIB_GEMM_FWD, h->y_fwd[j], 1, y_fan_out(h, j), 0, 1, 0)) return 1;
+  if (tf32_shadow(c) || forward_output_encoder(c, y)) return 1;
   DIB_CUDA_OK(dib_launch_copy2d(c.ws + h->y_out.off, h->y_out.ld, out, h->out, h->out, n, c.st));
   return 0;
 }
@@ -1837,10 +1720,9 @@ int dib_compression_matrices(dib_model* h, const float* params, const float* x, 
     return fail("dib_compression_matrices: rows out of range");
   if (n == 0) return 0;
   Ctx c{h, params, static_cast<float*>(workspace), static_cast<cudaStream_t>(stream), (int)n};
-  const int rnd = is_tc(h) ? 1 : 0;
-  if (rnd) DIB_CUDA_OK(dib_launch_round_copy(c.params, c.ws + h->wshadow_off, h->P, c.st));
+  if (tf32_shadow(c)) return 1;
   // all F encoders as ONE grouped problem per layer (the reference loops over features in Python, visualization.py:14-35)
-  if (encode_all(c, x, h->D, rnd, row_index, n_total)) return 1;
+  if (encode_all(c, x, h->D, -1, row_index, n_total)) return 1;
   const float* eo = c.ws + h->enc_out.off;
   if (out_mu_logvar)
     for (int f = 0; f < h->F; ++f)
