@@ -37,6 +37,21 @@ def _as_numpy_like(ref, t):
     return t.detach().cpu().numpy()
 
 
+def _run_phases(phases, last_exchange=True):
+    """Run (launch, exchange) phases eagerly: each launch, then its exchange -- the last phase's only with ``last_exchange``."""
+    for k, (launch, exchange) in enumerate(phases):
+        launch()
+        if exchange is not None and (last_exchange or k < len(phases) - 1):
+            exchange()
+
+
+def _shard_rows(order, b0, b1, rank, world):
+    """This rank's rows of the batch [b0, b1) of ``order`` (a permutation, or None for the rows in order) as an index tensor
+    or a slice, and their offset in the batch (:func:`parallel.shard_range`)."""
+    lo, hi = parallel.shard_range(b1 - b0, rank, world)
+    return (order[b0 + lo:b0 + hi] if order is not None else slice(b0 + lo, b0 + hi)), lo
+
+
 class PositionalEncoding:
     """models.py:12-23.  Kept for API parity; inside DistributedIBNet the encoding is fused into the first-layer
     operand by the library.  Calling it directly is a convenience (plain torch ops, not the hot path)."""
@@ -132,13 +147,18 @@ class _FeatureEncoder(_Network):
 
 
 class _IntegrationNetwork(_Network):
-    """model.integration_network (models.py:84).  Direct calls are rare (the fused step never materialises this
-    boundary); they run dib_integration_forward on the model's precision path."""
+    """model.integration_network (models.py:84), or the set transformer of :class:`SetTransformerIBNet`: embeddings
+    [n, width] (width = F * E, or number_particles * E for the set transformer) -> [n, out].  Direct calls are rare (the fused
+    step never materialises this boundary); they run dib_integration_forward on the model's precision path."""
+
+    def __init__(self, model, var_slice, width):
+        super().__init__(model, var_slice)
+        self._width = width
 
     def __call__(self, emb, training=None):
         m = self._model
         with torch.cuda.device(m.device):
-            e = m._to_device(emb, m.number_features * m.feature_embedding_dimension)
+            e = m._to_device(emb, self._width)
             n = e.shape[0]
             m._ensure_handle(n)
             out = torch.empty(n, m.output_dimensionality, dtype=torch.float32, device=m.device)
@@ -288,7 +308,8 @@ class DistributedIBNet:
             _FeatureEncoder(self, i, range(i * n_enc_vars, (i + 1) * n_enc_vars)) for i in range(self.number_features)]
         self._n_model_vars = len(self._var_off)
         self.integration_network = _IntegrationNetwork(                      # models.py:84
-            self, range(self.number_features * n_enc_vars, self._n_model_vars))
+            self, range(self.number_features * n_enc_vars, self._n_model_vars),
+            self.number_features * self.feature_embedding_dimension)
         self.output_encoder = None                                           # losses.InfoNCE: train.py:186-193
         self._p_enc = int(self._var_off[self.number_features * n_enc_vars])  # first integration-network parameter
 
@@ -384,17 +405,30 @@ class DistributedIBNet:
         """Keras Dense defaults: kernel glorot_uniform, bias zeros (third-party behaviour; RNG stream is ours)."""
         self._params.copy_(self._glorot_flat())
 
+    def _param_inits(self):
+        """The initializer of every variable in flat order: ('glorot', fan_in, fan_out), 'zeros', 'ones' or a constant."""
+        n_simple = 2 * self.number_features if self.encoder_kind == "simple" else 0
+        inits = []
+        for k, (r, c) in enumerate(zip(self._var_rows, self._var_cols)):
+            if k < n_simple:                 # nb-bool cell 4: mu_scaling = ones, logvar = -3 * ones
+                inits.append(1.0 if k % 2 == 0 else -3.0)
+            else:
+                inits.append(("glorot", r, c) if r > 0 else "zeros")
+        return inits
+
     def _glorot_flat(self):
+        """The flat weights :meth:`_param_inits` describes; glorot_uniform draws one generator seeded by ``seed`` in flat
+        order (RNG stream is ours)."""
         g = torch.Generator(device="cpu")
         g.manual_seed(self.seed)
         flat = torch.zeros(self._P, dtype=torch.float32)
-        n_simple = 2 * self.number_features if self.encoder_kind == "simple" else 0
-        for k, (off, r, c) in enumerate(zip(self._var_off, self._var_rows, self._var_cols)):
-            if k < n_simple:                 # nb-bool cell 4: mu_scaling = ones, logvar = -3 * ones
-                flat[off] = 1.0 if k % 2 == 0 else -3.0
-            elif r > 0:
-                lim = math.sqrt(6.0 / (r + c))
-                flat[off:off + r * c] = (torch.rand(r * c, generator=g) * 2 - 1) * lim
+        for off, r, c, init in zip(self._var_off, self._var_rows, self._var_cols, self._param_inits()):
+            size = max(r, 1) * c
+            if isinstance(init, tuple):
+                lim = math.sqrt(6.0 / (init[1] + init[2]))
+                flat[off:off + size] = (torch.rand(size, generator=g) * 2 - 1) * lim
+            elif init != "zeros":
+                flat[off:off + size] = 1.0 if init == "ones" else init
         return flat
 
     def _set_output_encoder(self, nce):
@@ -489,10 +523,15 @@ class DistributedIBNet:
             _lib.ptr(self._workspace), _stream()))
         return pred, emb, stats
 
-    def _encode_feature(self, i, x_i):
+    def _encoder_rows(self, i, x_i):
+        """x_i on the device as encoder i's input rows [rows, d_i], and the batch size the handle needs for them."""
         t = self._to_device(x_i, self.feature_dimensionalities[i])
+        return t, t.shape[0]
+
+    def _encode_feature(self, i, x_i):
+        t, batch = self._encoder_rows(i, x_i)
         n = t.shape[0]
-        self._ensure_handle(n)
+        self._ensure_handle(batch)
         out = torch.empty(n, 2 * self.feature_embedding_dimension, dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
             _lib.check(self._lib.dib_encode_feature(self._handle, _lib.ptr(self._params), i, _lib.ptr(t), n,
@@ -541,29 +580,50 @@ class DistributedIBNet:
         _lib.check(self._lib.dib_set_noise_step_device(self._handle, _lib.ptr(self._noise_step_dev) if on else None))
         self._step_dev_active = on
 
-    def _backward(self, x, y, global_batch, eps=None, sample_offset=0, step=None, device_step=False):
-        """dib_train_step: forward + reverse mode into self._gradstats = [grads (P) || stats (F+3)].  InfoNCE with more than
-        one rank: the three shard phases with the two all-gathers between them (DESIGN.md section 7)."""
-        n = x.shape[0]
+    def _step_phases(self, x, y, global_batch, eps, sample_offset, step, device_step=False, training=True, stats=None):
+        """The train step of one batch as an ordered list of (launch, exchange): ``exchange`` is the collective that has to
+        follow ``launch`` -- the all-gather of e_all or lse_all, or the all-reduce of self._gradstats = [grads (P) || stats
+        (F+3)] -- and None where there is none, which is everywhere with one process.  ``step`` is the Philox step word.
+
+        dib_train_step, the all-reduce, the optimizer update; losses.InfoNCE(negatives='global') on more than one rank splits
+        dib_train_step into its three shard phases with the two all-gathers between them (DESIGN.md section 7).  With
+        ``device_step`` (graph capture) the optimizer phase also advances the device noise step; ``training`` and ``stats``
+        (default the stats of self._gradstats) go to the InfoNCE shard forward and lse."""
+        n, P, group = x.shape[0], self._P, self.process_group
         self._ensure_handle(n)
-        P = self._P
-        self._set_device_step(device_step)
-        st = 0 if device_step else (self._train_step_count if step is None else step)
-        world, rank = parallel.world_and_rank(self.process_group)
+        world, rank = parallel.world_and_rank(group)
+        stats = self._gradstats[P:] if stats is None else stats
+        gather = (lambda t: lambda: parallel.all_gather_rows_(t, group)) if world > 1 else (lambda t: None)
+        reduce = (lambda: parallel.allreduce_sum_(self._gradstats, group)) if world > 1 else None
+
+        def update():
+            self._adam()
+            if device_step:
+                self._noise_step_dev.add_(1)
+
         if self._infonce is not None and world > 1:
             n_global, row_offset = self._infonce_shard(n, global_batch, world, rank)
             e_all, lse_all = self._infonce_buffers(n_global)
-            self._infonce_forward(x, y, e_all, n_global, row_offset, eps, st, sample_offset, training=True)
-            parallel.all_gather_rows_(e_all, self.process_group)
-            self._infonce_lse(n, e_all, lse_all, n_global, row_offset, self._gradstats[P:])
-            parallel.all_gather_rows_(lse_all, self.process_group)
-            self._infonce_backward(x, e_all, lse_all, n_global, row_offset, eps, st, sample_offset)
-            return
-        _lib.check(self._lib.dib_train_step(
-            self._handle, _lib.ptr(self._params), _lib.ptr(x), _lib.ptr(y), n, _lib.ptr(self.beta._dev),
-            1.0 / float(global_batch), _lib.ptr(eps), self.noise_seed, int(st) & 0xFFFFFFFF,
-            int(sample_offset), _lib.ptr(self._gradstats), _lib.ptr(self._gradstats[P:]), _lib.ptr(self._workspace),
-            _stream()))
+            phases = [
+                (lambda: self._infonce_forward(x, y, e_all, n_global, row_offset, eps, step, sample_offset, training),
+                 gather(e_all)),
+                (lambda: self._infonce_lse(n, e_all, lse_all, n_global, row_offset, stats), gather(lse_all)),
+                (lambda: self._infonce_backward(x, e_all, lse_all, n_global, row_offset, eps, step, sample_offset), reduce)]
+        else:
+            phases = [(lambda: _lib.check(self._lib.dib_train_step(
+                self._handle, _lib.ptr(self._params), _lib.ptr(x), _lib.ptr(y), n, _lib.ptr(self.beta._dev),
+                1.0 / float(global_batch), _lib.ptr(eps), self.noise_seed, int(step) & 0xFFFFFFFF,
+                int(sample_offset), _lib.ptr(self._gradstats), _lib.ptr(self._gradstats[P:]), _lib.ptr(self._workspace),
+                _stream())), reduce)]
+        return phases + [(update, None)]
+
+    def _backward(self, x, y, global_batch, eps=None, sample_offset=0, step=None, device_step=False):
+        """Forward + reverse mode into self._gradstats = [grads (P) || stats (F+3)] of this rank: the step's phases up to
+        the all-reduce."""
+        st = 0 if device_step else (self._train_step_count if step is None else step)
+        phases = self._step_phases(x, y, global_batch, eps, sample_offset, st, device_step)
+        self._set_device_step(device_step)
+        _run_phases(phases[:-1], last_exchange=False)
 
     # ------------------------------------------------------------------ InfoNCE with global negatives on several ranks
     def _check_infonce_world(self, nce, batch_size=None):
@@ -650,22 +710,23 @@ class DistributedIBNet:
             if g is None and self._graph_seen.get(key, 0) >= 2:
                 g = self._capture_step(key)
             if g is not None:
-                return self._replay_step(g, x, y, world)
+                return self._replay_step(g, x, y)
             self._graph_seen[key] = self._graph_seen.get(key, 0) + 1
-        self._backward(x, y, global_batch, eps, sample_offset)
-        parallel.allreduce_sum_(self._gradstats, self.process_group)
-        self._adam()
+        phases = self._step_phases(x, y, global_batch, eps, sample_offset, self._train_step_count)
+        self._set_device_step(False)
+        _run_phases(phases)
         self._train_step_count += 1
         self._step_dev_dirty = True
         return self._gradstats[P:]
 
     # ------------------------------------------------------------------ CUDA-graph replay of the step
     def _capture_step(self, key):
-        """Capture the step for one (n, global_batch, sample_offset, world) into CUDA graphs.  Single GPU: ONE graph
-        (forward + backward + Adam + noise-step increment).  Data parallel: two graphs (backward | Adam) with the NCCL all-reduce
-        issued eagerly between them; InfoNCE: four graphs (the three shard phases | Adam) with the two all-gathers and the
-        all-reduce issued eagerly between them, and e_all / lse_all kept with the graphs.  Inputs are copied into static buffers before each replay; beta,
-        learning rate, the Adam step and the Philox step are device scalars, so nothing by-value changes between replays."""
+        """Capture the step for one (n, global_batch, sample_offset, world) into CUDA graphs: one graph per run of phases
+        between two collectives, each kept with the exchange that follows it.  Single GPU: ONE graph (forward + backward +
+        optimizer + noise-step increment); plain data parallel: two (backward | optimizer); InfoNCE with global negatives: four
+        (the three shard phases | optimizer), e_all / lse_all kept with the graphs.  Inputs are copied into static buffers
+        before each replay; beta, learning rate, the optimizer step and the Philox step are device scalars, so nothing by-value
+        changes between replays."""
         n, global_batch, sample_offset, world = key
         D = sum(self.feature_dimensionalities)
         yc = self._y_cols()
@@ -673,38 +734,21 @@ class DistributedIBNet:
             with torch.cuda.device(self.device):
                 gx = torch.zeros(n, D, dtype=torch.float32, device=self.device)
                 gy = torch.zeros((n, yc) if yc > 0 else (n,), dtype=torch.float32, device=self.device)
-                self._ensure_handle(n)
+                phases = self._step_phases(gx, gy, global_batch, None, sample_offset, 0, device_step=True)
                 self._set_device_step(True)
                 torch.cuda.synchronize(self.device)
                 keep = [t.clone() for t in (self._params, self._m, self._v, self._step_dev, self._noise_step_dev)]
-                graphs = []
+                graphs, run = [], []
                 launches0 = int(self._lib.dib_launch_count())
-
-                def cap(fn):
-                    g = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(g):
-                        fn()
-                    graphs.append(g)
-
-                def tail():
-                    self._adam()
-                    self._noise_step_dev.add_(1)
-
-                nce = None
-                if world == 1:
-                    cap(lambda: (self._backward(gx, gy, global_batch, None, sample_offset, device_step=True), tail()))
-                elif self._infonce is not None:     # phase 1 | all-gather | phase 2 | all-gather | phase 3 | all-reduce | tail
-                    _, rank = parallel.world_and_rank(self.process_group)
-                    n_global, row_offset = self._infonce_shard(n, global_batch, world, rank)
-                    e_all, lse_all = self._infonce_buffers(n_global)
-                    nce = dict(e_all=e_all, lse_all=lse_all)
-                    cap(lambda: self._infonce_forward(gx, gy, e_all, n_global, row_offset, None, 0, sample_offset, True))
-                    cap(lambda: self._infonce_lse(n, e_all, lse_all, n_global, row_offset, self._gradstats[self._P:]))
-                    cap(lambda: self._infonce_backward(gx, e_all, lse_all, n_global, row_offset, None, 0, sample_offset))
-                    cap(tail)
-                else:        # one all-reduce between backward and optimizer: two graphs
-                    cap(lambda: self._backward(gx, gy, global_batch, None, sample_offset, device_step=True))
-                    cap(tail)
+                for k, (launch, exchange) in enumerate(phases):
+                    run.append(launch)
+                    if exchange is not None or k == len(phases) - 1:
+                        g = torch.cuda.CUDAGraph()
+                        with torch.cuda.graph(g):
+                            for fn in run:
+                                fn()
+                        graphs.append((g, exchange))
+                        run = []
                 torch.cuda.synchronize(self.device)
                 # capture does not execute, but be safe against any eager side effect: restore the optimizer state
                 for t, k in zip((self._params, self._m, self._v, self._step_dev, self._noise_step_dev), keep):
@@ -715,31 +759,21 @@ class DistributedIBNet:
             self._graph_failed = True
             self._set_device_step(False)
             return None
-        g = dict(graphs=graphs, x=gx, y=gy, launches=int(self._lib.dib_launch_count()) - launches0, nce=nce)
+        g = dict(graphs=graphs, x=gx, y=gy, launches=int(self._lib.dib_launch_count()) - launches0)
         self._graphs[key] = g
         return g
 
-    def _replay_step(self, g, x, y, world):
+    def _replay_step(self, g, x, y):
         P = self._P
         if not self._step_dev_active or self._step_dev_dirty:
             self._set_device_step(True)
         self._replayed_launches += g["launches"]
         g["x"].copy_(x.reshape(g["x"].shape), non_blocking=True)
         g["y"].copy_(y.reshape(g["y"].shape), non_blocking=True)
-        if world == 1:
-            g["graphs"][0].replay()
-        elif g["nce"] is not None:
-            g["graphs"][0].replay()
-            parallel.all_gather_rows_(g["nce"]["e_all"], self.process_group)
-            g["graphs"][1].replay()
-            parallel.all_gather_rows_(g["nce"]["lse_all"], self.process_group)
-            g["graphs"][2].replay()
-            parallel.allreduce_sum_(self._gradstats, self.process_group)
-            g["graphs"][3].replay()
-        else:
-            g["graphs"][0].replay()
-            parallel.allreduce_sum_(self._gradstats, self.process_group)
-            g["graphs"][1].replay()
+        for graph, exchange in g["graphs"]:
+            graph.replay()
+            if exchange is not None:
+                exchange()
         self._train_step_count += 1
         return self._gradstats[P:]
 
@@ -972,13 +1006,12 @@ class DistributedIBNet:
         batch_size = 32 if batch_size is None else int(batch_size)
         world, rank = parallel.world_and_rank(self.process_group)
         D = sum(self.feature_dimensionalities)
-        nce = self._infonce is not None
-        if nce:
+        if self._infonce is not None:
             self._check_infonce_world(self._infonce, batch_size)
         with torch.cuda.device(self.device):
             xd, yd = self._to_device(x, D), self._targets(y)
             N = xd.shape[0]
-            plan = infonce_epoch_batches(N, batch_size) if nce else None
+            plan = self._batch_plan(N, batch_size)
             xv = yv = None
             if validation_data is not None:
                 xv, yv = self._to_device(validation_data[0], D), self._targets(validation_data[1])
@@ -994,30 +1027,15 @@ class DistributedIBNet:
                 for cb in cbs:
                     cb.on_epoch_begin(epoch, logs=None)                      # beta annealing lives here
                 self._sync_lr()
-                if shuffle:
-                    perm = self.epoch_permutation(epoch, N)
+                order = self.epoch_permutation(epoch, N) if shuffle else None
                 self._epoch_acc.zero_()
-                if nce:                                                      # full batches only, equal shards
-                    for b0, b1 in plan:
-                        lo, hi = parallel.shard_range(b1 - b0, rank, world)
-                        idx = perm[b0 + lo:b0 + hi] if shuffle else slice(b0 + lo, b0 + hi)
-                        self._metrics_update(self._train_step(xd[idx], yd[idx], global_batch=b1 - b0, sample_offset=lo))
-                else:
-                    for b0 in range(0, N, batch_size):
-                        b1 = min(b0 + batch_size, N)
-                        lo, hi = parallel.shard_range(b1 - b0, rank, world)
-                        if shuffle:
-                            idx = perm[b0 + lo:b0 + hi]
-                            xb, yb = xd.index_select(0, idx), yd.index_select(0, idx)
-                        else:
-                            xb, yb = xd[b0 + lo:b0 + hi], yd[b0 + lo:b0 + hi]
-                        stats = self._train_step(xb, yb, global_batch=b1 - b0, sample_offset=lo)
-                        self._metrics_update(stats)
+                for b0, b1 in plan:
+                    idx, lo = _shard_rows(order, b0, b1, rank, world)
+                    self._metrics_update(self._train_step(xd[idx], yd[idx], global_batch=b1 - b0, sample_offset=lo))
                 logs = self._read_epoch_logs()
-                if xv is not None and nce:
-                    logs.update(self._evaluate_infonce_into_logs(xv, yv, batch_size, epoch, (2 ** 31 + epoch), world, rank))
-                elif xv is not None:
-                    logs.update(self._evaluate_into_logs(xv, yv, batch_size, epoch, world, rank))
+                if xv is not None:
+                    logs.update(self._evaluate_into_logs(xv, yv, *self._validation_plan(xv.shape[0], batch_size, epoch),
+                                                         2 ** 31 + epoch))
                 if verbose not in (False, 0) and rank == 0:          # 'auto' -> 1 like Keras outside notebooks
                     print(f"Epoch {epoch + 1}/{epochs} - " + " - ".join(
                         f"{k}: {v:.4g}" for k, v in logs.items() if not k.removeprefix('val_').startswith('KL')))
@@ -1029,43 +1047,38 @@ class DistributedIBNet:
                 getattr(cb, "on_train_end", lambda logs=None: None)()
         return history
 
-    def _evaluate_into_logs(self, xv, yv, batch_size, epoch, world, rank):
-        Nv = xv.shape[0]
-        self._epoch_acc.zero_()
-        stats = torch.empty(self.number_features + 3, dtype=torch.float32, device=self.device)
-        for b0 in range(0, Nv, batch_size):
-            b1 = min(b0 + batch_size, Nv)
-            lo, hi = parallel.shard_range(b1 - b0, rank, world)
-            self._forward(xv[b0 + lo:b0 + hi], yv[b0 + lo:b0 + hi], None, (2 ** 31 + epoch), b0 + lo,
-                          want_pred=False, stats_out=stats)
-            parallel.allreduce_sum_(stats, self.process_group)
-            self._metrics_update(stats)
-        return self._read_epoch_logs(prefix="val_")
+    def _batch_plan(self, n, batch_size):
+        """The [b0, b1) batches of one pass over n rows: full ones for InfoNCE (:func:`infonce_epoch_batches`), otherwise
+        consecutive batches with a short last one."""
+        if self._infonce is not None:
+            return infonce_epoch_batches(n, batch_size)
+        return [(b0, min(b0 + batch_size, n)) for b0 in range(0, n, batch_size)]
 
-    def _evaluate_infonce_into_logs(self, xv, yv, batch_size, perm_key, step, world=1, rank=0):
-        """InfoNCE validation (train.py:233-234, 264-270): floor(Nv / B) + 1 full batches drawn from the repeated validation
-        permutation (:func:`infonce_validation_batches`), noise keyed by (step, position in the repeated stream).  With more
-        than one rank each rank runs its equal shard of every batch through the first two shard phases and the statistics are
-        summed over the ranks."""
-        Nv, B = xv.shape[0], int(batch_size)
-        pos = torch.from_numpy(infonce_validation_batches(Nv, B)).to(self.device)
-        idx_all = self.validation_permutation(perm_key, Nv)[pos]
+    def _validation_plan(self, n, batch_size, perm_key):
+        """(batches, row order) of a validation pass over n rows.  InfoNCE (train.py:233-234): floor(n / B) + 1 full batches
+        drawn from the repeated validation permutation of ``perm_key`` (:func:`infonce_validation_batches`); otherwise the
+        rows in order (order None)."""
+        if self._infonce is None:
+            return self._batch_plan(n, batch_size), None
+        pos = torch.from_numpy(infonce_validation_batches(n, batch_size)).to(self.device)
+        order = self.validation_permutation(perm_key, n)[pos].reshape(-1)
+        return self._batch_plan(order.shape[0], batch_size), order
+
+    def _evaluate_into_logs(self, xv, yv, plan, order, step):
+        """Validation logs of the batches ``plan`` of rows ``order`` (see :func:`_shard_rows`), noise keyed by (step, the
+        row's position in ``order``): every rank runs the forward of its shard of a batch -- InfoNCE with more than one rank
+        the first two phases of the step, without training -- and the statistics are summed over the ranks."""
+        world, rank = parallel.world_and_rank(self.process_group)
         self._epoch_acc.zero_()
         stats = torch.empty(self.number_features + 3, dtype=torch.float32, device=self.device)
-        lo, hi = parallel.shard_range(B, rank, world)
-        for k in range(idx_all.shape[0]):
-            idx = idx_all[k]
-            if world == 1:
-                self._forward(xv.index_select(0, idx), yv.index_select(0, idx), None, step, k * B, want_pred=False,
-                              stats_out=stats)
+        for b0, b1 in plan:
+            idx, lo = _shard_rows(order, b0, b1, rank, world)
+            if self._infonce is not None and world > 1:
+                phases = self._step_phases(xv[idx], yv[idx], b1 - b0, None, b0 + lo, step, training=False, stats=stats)
+                _run_phases(phases[:2], last_exchange=False)
             else:
-                xs, ys = xv.index_select(0, idx[lo:hi]), yv.index_select(0, idx[lo:hi])
-                self._ensure_handle(hi - lo)
-                e_all, lse_all = self._infonce_buffers(B)
-                self._infonce_forward(xs, ys, e_all, B, lo, None, step, k * B + lo, training=False)
-                parallel.all_gather_rows_(e_all, self.process_group)
-                self._infonce_lse(hi - lo, e_all, lse_all, B, lo, stats)
-                parallel.allreduce_sum_(stats, self.process_group)
+                self._forward(xv[idx], yv[idx], None, step, b0 + lo, want_pred=False, stats_out=stats)
+            parallel.allreduce_sum_(stats, self.process_group)
             self._metrics_update(stats)
         return self._read_epoch_logs(prefix="val_")
 
@@ -1077,17 +1090,14 @@ class DistributedIBNet:
 
     def evaluate(self, x, y, batch_size=32, return_dict=True, **_):
         with torch.cuda.device(self.device):
-            world, rank = parallel.world_and_rank(self.process_group)
             D = sum(self.feature_dimensionalities)
             self._inference_calls += 1           # a fresh noise draw per evaluate() call
             key = (1 << 29) | (self._inference_calls & 0x1FFFFFFF)
             if self._infonce is not None:
                 self._check_infonce_world(self._infonce, batch_size)
-                logs = self._evaluate_infonce_into_logs(self._to_device(x, D), self._targets(y), int(batch_size), key, key,
-                                                        world, rank)
-            else:
-                logs = self._evaluate_into_logs(self._to_device(x, D), self._to_device(y, self._y_cols()), int(batch_size),
-                                                key, world, rank)
+            xv, yv = self._to_device(x, D), self._targets(y)
+            step = key if self._infonce is not None else 2 ** 31 + key
+            logs = self._evaluate_into_logs(xv, yv, *self._validation_plan(xv.shape[0], int(batch_size), key), step)
         logs = {k[len("val_"):]: v for k, v in logs.items()}
         return logs if return_dict else [logs["loss"]] + [logs[m] for m in self.compiled_metrics_names]
 
@@ -1380,22 +1390,6 @@ class _ParticleEncoder(_FeatureEncoder):
         return _as_numpy_like(x, out.reshape(*t.shape[:-1], out.shape[-1]))
 
 
-class _SetTransformer(_Network):
-    """model.set_transformer: embeddings [n, L, E] -> [n, out] through the attention blocks, the mean over the particles and
-    the head (dib_integration_forward), deterministic, on the model's precision path."""
-
-    def __call__(self, embs, training=None):
-        m = self._model
-        with torch.cuda.device(m.device):
-            e = m._to_device(embs, m.number_particles * m.feature_embedding_dimension)
-            n = e.shape[0]
-            m._ensure_handle(n)
-            out = torch.empty(n, m.output_dimensionality, dtype=torch.float32, device=m.device)
-            _lib.check(m._lib.dib_integration_forward(m._handle, _lib.ptr(m._params), _lib.ptr(e), n, _lib.ptr(out),
-                                                      _lib.ptr(m._workspace), _stream()))
-        return _as_numpy_like(embs, out)
-
-
 class SetTransformerIBNet(DistributedIBNet):
     """nb-particle cell 8 (BASELINE config 5): a shared particle encoder (positional encoding -> Dense stack -> (mu, logvar),
     logvar + ``logvar_initialization``, reparameterised per particle) feeding a set transformer -- ``number_attention_blocks``
@@ -1435,7 +1429,8 @@ class SetTransformerIBNet(DistributedIBNet):
         n_enc = 2 * (len(self.feature_encoder_architecture) + 1)
         self.particle_encoder = _ParticleEncoder(self, 0, range(n_enc))
         self.feature_encoders = [self.particle_encoder]
-        self.set_transformer = _SetTransformer(self, range(n_enc, self._n_model_vars))
+        # embeddings [n, L, E] -> [n, out] through the attention blocks, the mean over the particles and the head
+        self.set_transformer = _IntegrationNetwork(self, range(n_enc, self._n_model_vars), self.number_particles * E)
         self.integration_network = self.set_transformer
 
     def _config(self, max_batch):
@@ -1460,31 +1455,15 @@ class SetTransformerIBNet(DistributedIBNet):
                                            self.final_processing_arch, self.output_dimensionality,
                                            self.number_positional_encoding_frequencies if self.use_positional_encoding else 1)
 
-    def _glorot_flat(self):
+    def _param_inits(self):
         """[KERAS] glorot_uniform kernels with the fans of ``_compute_fans`` (3-D attention kernels included), zero biases,
-        LayerNorm gamma = 1 and beta = 0 (RNG stream is ours)."""
-        g = torch.Generator(device="cpu")
-        g.manual_seed(self.seed)
-        flat = torch.zeros(self._P, dtype=torch.float32)
-        for off, (_, shape, init) in zip(self._var_off, self.param_specs()):
-            size = int(np.prod(shape))
-            if init == "ones":
-                flat[off:off + size] = 1.0
-            elif init != "zeros":
-                lim = math.sqrt(6.0 / (init[1] + init[2]))
-                flat[off:off + size] = (torch.rand(size, generator=g) * 2 - 1) * lim
-        return flat
+        LayerNorm gamma = 1 and beta = 0."""
+        return [init for _, _, init in self.param_specs()]
 
-    def _encode_feature(self, i, x_i):
-        """Particle rows [..., d] -> [rows, 2E]."""
+    def _encoder_rows(self, i, x_i):
+        """Particle rows [..., d] -> [rows, d]; the handle is sized in sets of number_particles rows."""
         t = self._to_device(x_i).reshape(-1, self.particle_feature_dimensions).contiguous()
-        n = t.shape[0]
-        self._ensure_handle(max(1, -(-n // self.number_particles)))
-        out = torch.empty(n, 2 * self.feature_embedding_dimension, dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self._lib.dib_encode_feature(self._handle, _lib.ptr(self._params), 0, _lib.ptr(t), n, _lib.ptr(out),
-                                                    _lib.ptr(self._workspace), _stream()))
-        return out
+        return t, max(1, -(-t.shape[0] // self.number_particles))
 
     def compile(self, optimizer='adam', loss=None, metrics=None, **kw):
         kind = resolve_loss(loss)
