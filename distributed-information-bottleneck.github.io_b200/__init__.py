@@ -8,10 +8,10 @@ from . import ctw, keras_compat, models, parallel, utils                        
 from .keras_compat import Adam, SGD, RMSprop, Callback, History, losses, optimizers           # noqa: F401
 from .models import (DistributedIBNet, InfoBottleneckAnnealingCallback, PositionalEncoding,   # noqa: F401
                      SaveCompressionMatricesCallback, StashEmbeddingsCallback, InfoPerFeatureCallback,
-                     SimpleEncoder, SharedParticleEncoder, SetTransformerIBNet)
+                     SimpleEncoder, SharedParticleEncoder, SetTransformerIBNet, pad_sets)
 from ._lib import DibError, library_path                                         # noqa: F401
 
 __all__ = ["DistributedIBNet", "PositionalEncoding", "InfoBottleneckAnnealingCallback",
            "SaveCompressionMatricesCallback", "StashEmbeddingsCallback", "InfoPerFeatureCallback", "SimpleEncoder",
-           "SharedParticleEncoder", "SetTransformerIBNet", "Adam", "SGD", "RMSprop", "optimizers", "losses",
+           "SharedParticleEncoder", "SetTransformerIBNet", "pad_sets", "Adam", "SGD", "RMSprop", "optimizers", "losses",
            "Callback", "History", "models", "utils", "parallel", "keras_compat", "DibError", "library_path"]

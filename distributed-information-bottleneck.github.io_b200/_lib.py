@@ -6,7 +6,7 @@ from ctypes import POINTER, c_char_p, c_float, c_int32, c_int64, c_size_t, c_uin
 
 from . import build as _build
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 
 ACTIVATIONS = {None: 0, "linear": 0, "relu": 1, "tanh": 2, "leaky_relu": 3, "sigmoid": 4, "elu": 5}
 LOSSES = {"bce_logits": 0, "sparse_ce_logits": 1, "mse": 2, "external": 3, "bce_probs": 4, "infonce": 5}
@@ -57,6 +57,8 @@ class DibConfig(ctypes.Structure):
         ("ff_architecture", POINTER(c_int32)),
         ("ff_activation_fn", c_int32),
         ("layer_norm_epsilon", c_float),
+        # abi_version 5: sets of different sizes padded to set_size (dib_set_set_sizes_device)
+        ("variable_set_sizes", c_int32),
     ]
 
 
@@ -79,6 +81,7 @@ SIGNATURES = {
     "dib_infonce_shard_backward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_uint64, c_uint32, c_uint64,
                                              c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p]),
     "dib_set_noise_step_device": (c_int32, [c_void_p, c_void_p]),
+    "dib_set_set_sizes_device": (c_int32, [c_void_p, c_void_p]),
     "dib_adam_step": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_float,
                                 c_float, c_float, c_void_p]),
     "dib_optimizer_step": (c_int32, [c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_float,

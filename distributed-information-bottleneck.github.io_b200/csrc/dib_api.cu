@@ -122,6 +122,12 @@ struct dib_model {
   // n * Ls particle rows (maxB counts rows, maxSets sets), the head on the n set means
   bool st = false;
   int Ls = 1, nblk = 0, heads = 0, dkey = 0, hdk = 0, ff_act = 0;
+  // variable set sizes (dib_config.variable_set_sizes): Ls is the padded size Lmax and the caller binds the int32 sizes of the
+  // n sets of the following calls (dib_set_set_sizes_device); the attention runs on the key-tiled kernels of
+  // dib_set_attn_varlen.cu, which keep rowsum(dO o O) at dsum between their two backward passes
+  bool varlen = false;
+  const int32_t* set_sizes_dev = nullptr;
+  long long dsum = 0;
   float ln_eps = 1e-3f;
   long long maxSets = 0;
   std::vector<int> ff_arch;
@@ -292,6 +298,7 @@ void plan(dib_model* h) {
     for (int j = 1; j <= nf; ++j) h->d_ff[j] = make_buf(c, B, h->ff_arch[j - 1], 1);
     h->pooled = make_buf(c, h->maxSets, E, 1);
     h->d_pooled = make_buf(c, h->maxSets, E, 1);
+    if (h->varlen) h->dsum = take(c, h->maxSets * h->heads * h->Ls);
   }
   h->ws_floats = c;
 }
@@ -423,6 +430,7 @@ struct Ctx {
   int n;
   bool dev_step = false;     // dib_train_step only: add *h->step_dev to the Philox step word (dib_set_noise_step_device)
   const uint32_t* step_dev() const { return dev_step ? h->step_dev : nullptr; }
+  const int* sizes = nullptr;   // particle-row contexts of a variable-size set transformer: the bound set sizes
 };
 
 void prof_begin(const Ctx& c, const char* label, int j = -1) {
@@ -477,6 +485,8 @@ int check_call(const dib_model* h, const void* params, const void* x, int64_t n,
 int check_sets(const dib_model* h, int64_t n) {
   if (h->st && n > h->maxSets)
     return fail("n = " + std::to_string(n) + " sets exceeds config.max_batch = " + std::to_string(h->maxSets));
+  if (h->varlen && n > 0 && !h->set_sizes_dev)
+    return fail("variable set sizes: bind the sizes of the n sets with dib_set_set_sizes_device before this call");
   return 0;
 }
 
@@ -540,6 +550,7 @@ DibReparamArgs reparam_args(const Ctx& c, const NoiseKey& nk) {
   ra.enc_out = c.ws + h->enc_out.off; ra.feat_stride = h->enc_out.feat_stride; ra.ldo = h->enc_out.ld;
   ra.eps = nk.eps; ra.seed = nk.seed; ra.step = nk.step; ra.step_dev = c.step_dev(); ra.sample_offset = nk.sample_offset;
   ra.F = h->F; ra.E = h->E; ra.n = c.n; ra.round_out = is_tc(h) ? 1 : 0;
+  ra.set_sizes = c.sizes; ra.set_len = h->Ls;
   return ra;
 }
 
@@ -762,6 +773,8 @@ int encode_all(const Ctx& c, const float* x, int ldx, int feature, const int* ro
     DIB_CUDA_OK(dib_launch_pe(x, ldx, f >= 0 ? h->x_off[f] : 0, h->d_col_src, h->d_col_freq, f >= 0 ? h->pe_off[f] : 0,
                               f >= 0 ? h->pe_off[f] + DIB_ROUND_UP(h->w_in[f], 4) : h->ldpe, c.ws + h->pe.off, h->ldpe, 0, c.n,
                               is_tc(h) ? 1 : 0, c.st, row_index, row_index ? h->d_col_feat : nullptr, n_src));
+    // padding particles enter the first layer as zeros: whatever x holds there, every activation of theirs stays finite
+    if (c.sizes) DIB_CUDA_OK(dib_launch_zero_pad_rows(c.ws + h->pe.off, h->ldpe, c.n, h->Ls, c.sizes, c.st));
     prof_end(c);
     if (stack_forward(c, h->enc_stack, f >= 0 ? f : 0, f >= 0 ? 1 : h->F, key)) return 1;
   }
@@ -915,6 +928,7 @@ DibAttnArgs attn_args(const Ctx& c, const dib_model::StBlock& k) {
   a.sets = c.n / h->Ls; a.heads = h->heads; a.L = h->Ls; a.dk = h->dkey;
   a.round_out = is_tc(h) ? 1 : 0;
   a.dout = c.ws + h->d_o.off; a.dq = c.ws + h->dq.off; a.dk_ = c.ws + h->dk.off; a.dv = c.ws + h->dv.off;
+  a.set_sizes = c.sizes; a.dsum = h->varlen ? c.ws + h->dsum : nullptr;
   return a;
 }
 
@@ -938,7 +952,7 @@ int forward_set_blocks(const Ctx& c) {
     if (stack_forward(c, k.qkv_stack, 0, 3)) return 1;
     prof_end(c);
     prof_begin(c, "st_attn_fwd_b", b);
-    DIB_CUDA_OK(dib_launch_attn_fwd(attn_args(c, k), c.st));
+    DIB_CUDA_OK(h->varlen ? dib_launch_attn_varlen_fwd(attn_args(c, k), c.st) : dib_launch_attn_fwd(attn_args(c, k), c.st));
     prof_end(c);
     prof_begin(c, "st_out_proj_ln1_fwd_b", b);
     if (stack_forward(c, k.o_stack, 0, 1)) return 1;
@@ -951,8 +965,12 @@ int forward_set_blocks(const Ctx& c) {
   }
   const Buf& last = h->nblk ? h->blk[h->nblk - 1].xout : h->emb;
   prof_begin(c, "st_pool_fwd");
-  DIB_CUDA_OK(dib_launch_pool_fwd(c.ws + last.off, last.ld, h->E, h->Ls, c.n / h->Ls, c.ws + h->pooled.off, h->pooled.ld,
-                                  is_tc(h) ? 1 : 0, c.st));
+  if (h->varlen)
+    DIB_CUDA_OK(dib_launch_pool_varlen_fwd(c.ws + last.off, last.ld, h->E, h->Ls, c.n / h->Ls, c.sizes, c.ws + h->pooled.off,
+                                           h->pooled.ld, is_tc(h) ? 1 : 0, c.st));
+  else
+    DIB_CUDA_OK(dib_launch_pool_fwd(c.ws + last.off, last.ld, h->E, h->Ls, c.n / h->Ls, c.ws + h->pooled.off, h->pooled.ld,
+                                    is_tc(h) ? 1 : 0, c.st));
   prof_end(c);
   return 0;
 }
@@ -967,7 +985,7 @@ int backward_set_blocks(const Ctx& c, const Split& sp) {
                     long long g, long long be) {
     DibLayerNormBwd b;
     for (int q = 0; q < 4; ++q) b.dy[q] = dy[q];
-    b.dy_pool = dy_pool; b.pool_rows = h->Ls; b.pool_scale = 1.f / (float)h->Ls;
+    b.dy_pool = dy_pool; b.pool_rows = h->Ls; b.pool_scale = 1.f / (float)h->Ls; b.set_sizes = c.sizes;
     b.d_res = c.ws + d_res.off; b.d_branch = d_branch ? c.ws + d_branch->off : nullptr; b.branch_act = h->ff_act; b.alpha = h->alpha;
     b.part = part; b.split_stride = h->Pp; b.gamma_off = g; b.beta_off = be; b.nsplit = sp.nsplit; b.rows_per_split = sp.rps;
     return dib_launch_ln_bwd(l, b, c.st);
@@ -993,7 +1011,7 @@ int backward_set_blocks(const Ctx& c, const Split& sp) {
     if (stack_backward(c, k.o_stack, sp)) return 1;
     prof_end(c);
     prof_begin(c, "st_attn_bwd_b", b);
-    DIB_CUDA_OK(dib_launch_attn_bwd(attn_args(c, k), c.st));
+    DIB_CUDA_OK(h->varlen ? dib_launch_attn_varlen_bwd(attn_args(c, k), c.st) : dib_launch_attn_bwd(attn_args(c, k), c.st));
     prof_end(c);
     prof_begin(c, "st_qkv_bwd_b", b);
     if (stack_backward(c, k.qkv_stack, sp)) return 1;
@@ -1015,6 +1033,7 @@ int run_forward_set(const Ctx& cs, const float* x, const float* y, const NoiseKe
   dib_model* h = cs.h;
   Ctx c = cs;
   c.n = cs.n * h->Ls;
+  c.sizes = h->varlen ? h->set_sizes_dev : nullptr;
   NoiseKey nr = nk;
   nr.sample_offset = nk.sample_offset * (uint64_t)h->Ls;     // noise keyed by the global particle row
   if (tf32_shadow(c)) return 1;
@@ -1034,6 +1053,7 @@ int train_step_set(const Ctx& cs, const float* x, const float* y, const NoiseKey
   if (backward_integration(cs, inv_global_batch, batch_split(cs.n), grads_flat, &segs)) return 1;
   Ctx c = cs;
   c.n = cs.n * h->Ls;
+  c.sizes = h->varlen ? h->set_sizes_dev : nullptr;
   NoiseKey nr = nk;
   nr.sample_offset = nk.sample_offset * (uint64_t)h->Ls;
   const Split sp = batch_split(c.n);
@@ -1170,7 +1190,7 @@ int dib_debug_gemm_tc(int32_t mode, const float* A, int32_t lda, const float* B,
 const char* dib_last_error(void) { return g_last_error.c_str(); }
 
 const char* dib_build_info(void) {
-  return "dib_b200 abi=4 arch=sm_90a paths=fp32-simt,tf32-wgmma,fp16-fused-wgmma,bf16-fused-wgmma";
+  return "dib_b200 abi=5 arch=sm_90a paths=fp32-simt,tf32-wgmma,fp16-fused-wgmma,bf16-fused-wgmma";
 }
 
 int32_t dib_model_info(const dib_model* h, char* out, size_t out_bytes) {
@@ -1188,7 +1208,8 @@ int32_t dib_model_info(const dib_model* h, char* out, size_t out_bytes) {
   }
   if (h->route.tail_fused) s += h->route.tail_bwd ? " integration_tail=fwd2-head-dgrad" : " integration_tail=fwd2-head";
   if (h->st)
-    s += std::string(" set_transformer=attention-simt-fp32,layernorm-simt-fp32,dense-") + (is_tc(h) ? "wgmma-tf32" : "simt-fp32");
+    s += std::string(" set_transformer=") + (h->varlen ? "attention-varlen-simt-fp32" : "attention-simt-fp32") +
+         ",layernorm-simt-fp32,dense-" + (is_tc(h) ? "wgmma-tf32" : "simt-fp32");
   if (infonce(h))
     s += std::string(" output_encoder=") + (is_tc(h) ? "wgmma-tf32" : "simt-fp32") + " loss=infonce-stream-fp32";
   const size_t k = s.size() < out_bytes - 1 ? s.size() : out_bytes - 1;
@@ -1203,9 +1224,16 @@ int dib_create(const dib_config* cfg, dib_model** out) {
   if (cfg->abi_version < 2 || cfg->abi_version > DIB_ABI_VERSION) return fail("dib_create: abi_version mismatch");
   const int kind = cfg->abi_version >= 4 ? cfg->integration_kind : DIB_INTEGRATION_MLP;
   if (kind != DIB_INTEGRATION_MLP && kind != DIB_INTEGRATION_SET_TRANSFORMER) return fail("dib_create: unknown integration_kind");
+  const bool varlen = cfg->abi_version >= 5 && cfg->variable_set_sizes != 0;
+  if (varlen && kind != DIB_INTEGRATION_SET_TRANSFORMER) return fail("dib_create: variable_set_sizes needs the set transformer");
   if (kind == DIB_INTEGRATION_SET_TRANSFORMER) {
     const int E = cfg->feature_embedding_dimension;
-    if (cfg->set_size < 1 || cfg->set_size > 64) return fail("dib_create: set transformer needs set_size in [1, 64]");
+    if (varlen && (cfg->set_size < 1 || cfg->set_size > DIB_MAX_VARIABLE_SET_SIZE))
+      return fail("dib_create: set transformer with variable set sizes needs set_size (the largest set) in [1, " +
+                  std::to_string(DIB_MAX_VARIABLE_SET_SIZE) + "]");
+    if (!varlen && (cfg->set_size < 1 || cfg->set_size > 64))
+      return fail("dib_create: set transformer needs set_size in [1, 64] (up to " + std::to_string(DIB_MAX_VARIABLE_SET_SIZE) +
+                  " with variable_set_sizes)");
     if (cfg->number_features != 1) return fail("dib_create: set transformer needs number_features == 1 (one shared particle encoder)");
     if (cfg->number_attention_blocks < 1 || cfg->number_heads < 1 || cfg->key_dim < 1 || cfg->key_dim > 128)
       return fail("dib_create: set transformer needs >= 1 attention block, >= 1 head and key_dim in [1, 128]");
@@ -1263,6 +1291,7 @@ int dib_create(const dib_config* cfg, dib_model** out) {
   }
   if (kind == DIB_INTEGRATION_SET_TRANSFORMER) {
     h->st = true;
+    h->varlen = varlen;
     h->Ls = cfg->set_size; h->nblk = cfg->number_attention_blocks; h->heads = cfg->number_heads; h->dkey = cfg->key_dim;
     h->hdk = h->heads * h->dkey;
     h->ff_arch.assign(cfg->ff_architecture, cfg->ff_architecture + cfg->number_ff_layers);
@@ -1372,7 +1401,7 @@ int dib_create(const dib_config* cfg, dib_model** out) {
     if (e == cudaSuccess) e = cudaMemcpy(h->d_ycol_src, ycol_src.data(), ycol_src.size() * sizeof(int), cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMemcpy(h->d_ycol_freq, ycol_freq.data(), ycol_freq.size() * sizeof(int), cudaMemcpyHostToDevice);
   }
-  if (e == cudaSuccess && h->st) e = dib_attn_prepare();
+  if (e == cudaSuccess && h->st) e = h->varlen ? dib_attn_varlen_prepare() : dib_attn_prepare();
   if (e != cudaSuccess) {
     std::string msg = std::string("dib_create: CUDA error: ") + cudaGetErrorString(e);
     dib_destroy(h);
@@ -1550,6 +1579,16 @@ int dib_set_noise_step_device(dib_model* h, const uint32_t* step_dev) {
   return 0;
 }
 
+// the int32 sizes of the n sets of the following calls, read by the kernels from device memory: a captured graph reads
+// whatever the buffer holds at replay
+int dib_set_set_sizes_device(dib_model* h, const int32_t* set_sizes_dev) {
+  if (!h) return fail("null model handle");
+  if (!h->varlen && set_sizes_dev) return fail("dib_set_set_sizes_device: the model was not created with variable_set_sizes");
+  if (reinterpret_cast<uintptr_t>(set_sizes_dev) & 3) return fail("dib_set_set_sizes_device: sizes must be 4-byte aligned");
+  h->set_sizes_dev = set_sizes_dev;
+  return 0;
+}
+
 int dib_adam_step(float* params, const float* grads, float* m, float* v, int64_t count, const float* lr_dev,
                   int32_t* step_dev, float beta_1, float beta_2, float epsilon, void* stream) {
   if (!params || !grads || !m || !v || !lr_dev || !step_dev) return fail("dib_adam_step: null pointer");
@@ -1580,8 +1619,10 @@ int dib_integration_forward(dib_model* h, const float* params, const float* emb,
   if (h->st) {                 // emb [n, Ls, E] (E is a multiple of 4: no padded columns) through the blocks and the mean
     Ctx cr = c;
     cr.n = (int)n * h->Ls;
+    cr.sizes = h->varlen ? h->set_sizes_dev : nullptr;
     if (is_tc(h)) DIB_CUDA_OK(dib_launch_round_copy(emb, c.ws + h->emb.off, (int64_t)cr.n * FE, c.st));
     else DIB_CUDA_OK(dib_launch_copy2d(emb, FE, c.ws + h->emb.off, h->emb.ld, FE, cr.n, c.st));
+    if (cr.sizes) DIB_CUDA_OK(dib_launch_zero_pad_rows(c.ws + h->emb.off, h->emb.ld, cr.n, h->Ls, cr.sizes, c.st));
     if (forward_set_blocks(cr)) return 1;
   } else {
     DIB_CUDA_OK(dib_launch_copy2d(emb, FE, c.ws + h->emb.off, h->emb.ld, FE, n, c.st));

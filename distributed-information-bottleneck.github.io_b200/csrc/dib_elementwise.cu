@@ -60,7 +60,15 @@ dib_reparam_fwd_kernel(DibReparamArgs a, float* __restrict__ emb, int ldemb, flo
   const long long row = (long long)blockIdx.x * kRowsPerBlock + threadIdx.x;
   const int f = blockIdx.y, E = a.E;
   float kl = 0.f;
-  if (row < a.n) {
+  const bool pad = a.set_sizes && row < a.n && (int)(row % a.set_len) >= a.set_sizes[row / a.set_len];
+  if (pad) {                       // a padding particle of a padded set: u = 0, outside the KL
+    for (int e = 0; e < E; ++e) {
+      emb[row * ldemb + f * E + e] = 0.f;
+      if (user_emb) user_emb[row * ((long long)a.F * E) + f * E + e] = 0.f;
+    }
+    if (f == a.F - 1)
+      for (int c = a.F * E; c < ldemb; ++c) emb[row * ldemb + c] = 0.f;
+  } else if (row < a.n) {
     const float* o = a.enc_out + (long long)f * a.feat_stride + row * a.ldo;
     float* dst = emb + row * ldemb + f * E;
     float* udst = user_emb ? user_emb + row * ((long long)a.F * E) + f * E : nullptr;
@@ -99,6 +107,10 @@ dib_reparam_bwd_kernel(DibReparamArgs a, const float* __restrict__ d_emb, int ld
   const float bs = beta_dev[0] * inv_batch;
   const float* o = a.enc_out + (long long)f * a.feat_stride + row * a.ldo;
   float* dq = d_out + (long long)f * a.feat_stride + row * a.ldo;
+  if (a.set_sizes && (int)(row % a.set_len) >= a.set_sizes[row / a.set_len]) {   // padding particle: no gradient
+    for (int c = 0; c < a.ldo; ++c) dq[c] = 0.f;
+    return;
+  }
   const float* du = d_emb + row * ldemb + f * E;
   const float* ep = a.eps ? a.eps + (row * a.F + f) * E : nullptr;
   for (int e0 = 0; e0 < E; e0 += 4) {

@@ -48,6 +48,9 @@ struct DibReparamArgs {
   int F, E;
   int64_t n;
   int round_out = 0;
+  // variable set sizes: rows are sets of set_len padded particle rows, set s has set_sizes[s] real ones; a padding row gets
+  // u = 0, no KL and d(mu, logvar) = 0.  nullptr: every row is real
+  const int* set_sizes = nullptr; int set_len = 1;
 };
 // u = mu + exp(logvar/2) eps (models.py:108); per-(block,feature) partial sums of the KL (models.py:111-112).
 cudaError_t dib_launch_reparam_fwd(const DibReparamArgs& a, float* emb, int ldemb, float* user_emb,
@@ -213,11 +216,18 @@ struct DibAttnArgs {
   long long sets; int heads, L, dk;
   int round_out;
   const float* dout; float* dq; float* dk_; float* dv;
+  // the key-tiled kernels of sets of different sizes (dib_set_attn_varlen.cu): L is the padded size Lmax, set s has
+  // set_sizes[s] real rows; dsum [sets, heads, L] = rowsum(dO o O), written by the query pass of the backward
+  const int* set_sizes = nullptr; float* dsum = nullptr;
 };
 size_t dib_attn_smem_bytes(int L, int dk, bool backward);
 cudaError_t dib_attn_prepare();   // once per model: the kernels' shared-memory opt-in
 cudaError_t dib_launch_attn_fwd(const DibAttnArgs& a, cudaStream_t st);
 cudaError_t dib_launch_attn_bwd(const DibAttnArgs& a, cudaStream_t st);
+// masked, key-tiled attention of padded sets (shared memory independent of L, dk <= 128); the backward is two launches
+cudaError_t dib_attn_varlen_prepare();
+cudaError_t dib_launch_attn_varlen_fwd(const DibAttnArgs& a, cudaStream_t st);
+cudaError_t dib_launch_attn_varlen_bwd(const DibAttnArgs& a, cudaStream_t st);
 // LayerNorm(a + b) over the last axis of [rows, E] (E <= 128, leading dimension ld); mean / rstd [rows] are kept
 struct DibLayerNorm {
   const float* a; const float* b; int ld; long long rows; int E;
@@ -232,12 +242,20 @@ struct DibLayerNormBwd {
   const float* dy[4]; const float* dy_pool; int pool_rows; float pool_scale;
   float* d_res; float* d_branch; int branch_act; float alpha;
   float* part; long long split_stride; long long gamma_off, beta_off; int nsplit; long long rows_per_split;
+  // variable set sizes: the pooled source reaches row p of set s as dy_pool[s] / set_sizes[s] for p < set_sizes[s] and not at
+  // all for the padding rows (pool_scale is then unused)
+  const int* set_sizes = nullptr;
 };
 cudaError_t dib_launch_ln_fwd(const DibLayerNorm& a, cudaStream_t st);
 cudaError_t dib_launch_ln_bwd(const DibLayerNorm& a, const DibLayerNormBwd& b, cudaStream_t st);
 // out[s] = mean over the L rows of set s of x [sets * L, ld] (E live columns), out [sets, ldo]
 cudaError_t dib_launch_pool_fwd(const float* x, int ld, int E, int L, int64_t sets, float* out, int ldo, int round_out,
                                 cudaStream_t st);
+// the same over the l_s = sizes[s] real rows of each padded set: out[s] = (sum_{p < l_s} x[s L + p]) / l_s
+cudaError_t dib_launch_pool_varlen_fwd(const float* x, int ld, int E, int L, int64_t sets, const int* sizes, float* out, int ldo,
+                                       int round_out, cudaStream_t st);
+// zero every column of the padding rows p >= sizes[s] of a [rows = sets * L, ld] buffer
+cudaError_t dib_launch_zero_pad_rows(float* buf, int ld, int64_t rows, int L, const int* sizes, cudaStream_t st);
 // dst[i] = sum of the non-null src[q][i], i < count
 struct DibSumRows { const float* src[4]; float* dst; long long count; };
 cudaError_t dib_launch_sum_rows(const DibSumRows& a, cudaStream_t st);

@@ -189,7 +189,13 @@ ln_bwd_kernel(DibLayerNorm a, DibLayerNormBwd b) {
       if (e >= E) continue;
       xh[k] = (a.a[r * a.ld + e] + a.b[r * a.ld + e] - mean) * rstd;
       float dy = 0.f;
-      if (b.dy_pool) dy = b.dy_pool[(r / b.pool_rows) * a.ld + e] * b.pool_scale;
+      if (b.dy_pool && b.set_sizes) {          // padded sets of different sizes: the mean over the l real rows
+        const long long s = r / b.pool_rows;
+        const int l = b.set_sizes[s];
+        if (r - s * b.pool_rows < l) dy = b.dy_pool[s * a.ld + e] * (1.f / (float)l);
+      } else if (b.dy_pool) {
+        dy = b.dy_pool[(r / b.pool_rows) * a.ld + e] * b.pool_scale;
+      }
       for (int q = 0; q < 4; ++q)
         if (b.dy[q]) dy += b.dy[q][r * a.ld + e];
       dg[k] = fmaf(dy, xh[k], dg[k]);

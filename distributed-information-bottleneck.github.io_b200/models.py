@@ -155,16 +155,17 @@ class _IntegrationNetwork(_Network):
         super().__init__(model, var_slice)
         self._width = width
 
-    def __call__(self, emb, training=None):
+    def __call__(self, emb, training=None, set_sizes=None):
         m = self._model
         with torch.cuda.device(m.device):
-            e = m._to_device(emb, self._width)
+            e, sd = m._integration_inputs(emb, set_sizes, self._width)
             n = e.shape[0]
             m._ensure_handle(n)
+            m._bind_set_sizes(sd)
             out = torch.empty(n, m.output_dimensionality, dtype=torch.float32, device=m.device)
             _lib.check(m._lib.dib_integration_forward(m._handle, _lib.ptr(m._params), _lib.ptr(e), n, _lib.ptr(out),
                                                       _lib.ptr(m._workspace), _stream()))
-        return _as_numpy_like(emb, out)
+        return _as_numpy_like(emb[0] if isinstance(emb, list) and emb else emb, out)
 
 
 class _OutputEncoder(_Network):
@@ -220,6 +221,8 @@ class DistributedIBNet:
     wgmma kernels with fp32 accumulation; ``model.kernel_info()`` says what a handle actually runs), ``process_group``
     (data-parallel group; defaults to the WORLD group when torch.distributed is initialised), ``leaky_alpha``.
     """
+
+    variable_set_sizes = False         # SetTransformerIBNet(variable_set_sizes=True): inputs carry per-set sizes
 
     def __init__(self,
                  feature_dimensionalities: Sequence[int],
@@ -508,10 +511,25 @@ class DistributedIBNet:
                 raise ValueError(f"y has shape {shape}; the InfoNCE output encoder takes [n, {self._infonce.y_dimensionality}]")
         return self._to_device(y, self._y_cols())
 
+    def _inputs(self, x):
+        """Model inputs on the device: (x [n, sum d_i], per-set sizes or None -- see SetTransformerIBNet)."""
+        return self._to_device(x, sum(self.feature_dimensionalities)), None
+
+    def _integration_inputs(self, emb, set_sizes, width):
+        if set_sizes is not None:
+            raise ValueError("set_sizes is for SetTransformerIBNet(variable_set_sizes=True)")
+        return self._to_device(emb, width), None
+
+    def _bind_set_sizes(self, sizes):
+        """Point the handle at the int32 device sizes of the sets of the following library calls (variable set sizes)."""
+        if sizes is not None:
+            _lib.check(self._lib.dib_set_set_sizes_device(self._handle, _lib.ptr(sizes)))
+
     # ------------------------------------------------------------------ compute entry points
-    def _forward(self, x, y, eps, step, sample_offset, want_pred=True, want_emb=False, stats_out=None):
+    def _forward(self, x, y, eps, step, sample_offset, want_pred=True, want_emb=False, stats_out=None, sizes=None):
         n = x.shape[0]
         self._ensure_handle(n)
+        self._bind_set_sizes(sizes)
         pred = torch.empty(n, self.output_dimensionality, dtype=torch.float32, device=self.device) if want_pred else None
         emb = torch.empty(n, self.number_features * self.feature_embedding_dimension, dtype=torch.float32,
                           device=self.device) if want_emb else None
@@ -580,7 +598,8 @@ class DistributedIBNet:
         _lib.check(self._lib.dib_set_noise_step_device(self._handle, _lib.ptr(self._noise_step_dev) if on else None))
         self._step_dev_active = on
 
-    def _step_phases(self, x, y, global_batch, eps, sample_offset, step, device_step=False, training=True, stats=None):
+    def _step_phases(self, x, y, global_batch, eps, sample_offset, step, device_step=False, training=True, stats=None,
+                     sizes=None):
         """The train step of one batch as an ordered list of (launch, exchange): ``exchange`` is the collective that has to
         follow ``launch`` -- the all-gather of e_all or lse_all, or the all-reduce of self._gradstats = [grads (P) || stats
         (F+3)] -- and None where there is none, which is everywhere with one process.  ``step`` is the Philox step word.
@@ -588,7 +607,8 @@ class DistributedIBNet:
         dib_train_step, the all-reduce, the optimizer update; losses.InfoNCE(negatives='global') on more than one rank splits
         dib_train_step into its three shard phases with the two all-gathers between them (DESIGN.md section 7).  With
         ``device_step`` (graph capture) the optimizer phase also advances the device noise step; ``training`` and ``stats``
-        (default the stats of self._gradstats) go to the InfoNCE shard forward and lse."""
+        (default the stats of self._gradstats) go to the InfoNCE shard forward and lse; ``sizes`` are the set sizes of a
+        variable-size set transformer, bound to the handle right before its train step."""
         n, P, group = x.shape[0], self._P, self.process_group
         self._ensure_handle(n)
         world, rank = parallel.world_and_rank(group)
@@ -610,18 +630,21 @@ class DistributedIBNet:
                 (lambda: self._infonce_lse(n, e_all, lse_all, n_global, row_offset, stats), gather(lse_all)),
                 (lambda: self._infonce_backward(x, e_all, lse_all, n_global, row_offset, eps, step, sample_offset), reduce)]
         else:
-            phases = [(lambda: _lib.check(self._lib.dib_train_step(
-                self._handle, _lib.ptr(self._params), _lib.ptr(x), _lib.ptr(y), n, _lib.ptr(self.beta._dev),
-                1.0 / float(global_batch), _lib.ptr(eps), self.noise_seed, int(step) & 0xFFFFFFFF,
-                int(sample_offset), _lib.ptr(self._gradstats), _lib.ptr(self._gradstats[P:]), _lib.ptr(self._workspace),
-                _stream())), reduce)]
+            def train_step():
+                self._bind_set_sizes(sizes)
+                _lib.check(self._lib.dib_train_step(
+                    self._handle, _lib.ptr(self._params), _lib.ptr(x), _lib.ptr(y), n, _lib.ptr(self.beta._dev),
+                    1.0 / float(global_batch), _lib.ptr(eps), self.noise_seed, int(step) & 0xFFFFFFFF,
+                    int(sample_offset), _lib.ptr(self._gradstats), _lib.ptr(self._gradstats[P:]), _lib.ptr(self._workspace),
+                    _stream()))
+            phases = [(train_step, reduce)]
         return phases + [(update, None)]
 
-    def _backward(self, x, y, global_batch, eps=None, sample_offset=0, step=None, device_step=False):
+    def _backward(self, x, y, global_batch, eps=None, sample_offset=0, step=None, device_step=False, sizes=None):
         """Forward + reverse mode into self._gradstats = [grads (P) || stats (F+3)] of this rank: the step's phases up to
         the all-reduce."""
         st = 0 if device_step else (self._train_step_count if step is None else step)
-        phases = self._step_phases(x, y, global_batch, eps, sample_offset, st, device_step)
+        phases = self._step_phases(x, y, global_batch, eps, sample_offset, st, device_step, sizes=sizes)
         self._set_device_step(device_step)
         _run_phases(phases[:-1], last_exchange=False)
 
@@ -699,20 +722,21 @@ class DistributedIBNet:
     def _adam(self):
         self._optimizer_update(self._gradstats)
 
-    def _train_step(self, x, y, global_batch, eps=None, sample_offset=0):
+    def _train_step(self, x, y, global_batch, eps=None, sample_offset=0, sizes=None):
         """backward, one flat all-reduce of [grads || stats] over the data-parallel group, Keras-Adam.  Replayed from
-        CUDA graphs once a (batch size, offset) combination has run eagerly twice."""
+        CUDA graphs once a (batch size, offset) combination has run eagerly twice; the set sizes of a variable-size set
+        transformer are data, not part of that key."""
         P = self._P
         world, _ = parallel.world_and_rank(self.process_group)
         key = (int(x.shape[0]), int(global_batch), int(sample_offset), world)
         if self.use_cuda_graph and not self._graph_failed and eps is None and x.shape[0] > 0:
             g = self._graphs.get(key)
             if g is None and self._graph_seen.get(key, 0) >= 2:
-                g = self._capture_step(key)
+                g = self._capture_step(key, with_sizes=sizes is not None)
             if g is not None:
-                return self._replay_step(g, x, y)
+                return self._replay_step(g, x, y, sizes)
             self._graph_seen[key] = self._graph_seen.get(key, 0) + 1
-        phases = self._step_phases(x, y, global_batch, eps, sample_offset, self._train_step_count)
+        phases = self._step_phases(x, y, global_batch, eps, sample_offset, self._train_step_count, sizes=sizes)
         self._set_device_step(False)
         _run_phases(phases)
         self._train_step_count += 1
@@ -720,13 +744,13 @@ class DistributedIBNet:
         return self._gradstats[P:]
 
     # ------------------------------------------------------------------ CUDA-graph replay of the step
-    def _capture_step(self, key):
+    def _capture_step(self, key, with_sizes=False):
         """Capture the step for one (n, global_batch, sample_offset, world) into CUDA graphs: one graph per run of phases
         between two collectives, each kept with the exchange that follows it.  Single GPU: ONE graph (forward + backward +
         optimizer + noise-step increment); plain data parallel: two (backward | optimizer); InfoNCE with global negatives: four
         (the three shard phases | optimizer), e_all / lse_all kept with the graphs.  Inputs are copied into static buffers
-        before each replay; beta, learning rate, the optimizer step and the Philox step are device scalars, so nothing by-value
-        changes between replays."""
+        before each replay (and, ``with_sizes``, the set sizes into a third one); beta, learning rate, the optimizer step and
+        the Philox step are device scalars, so nothing by-value changes between replays."""
         n, global_batch, sample_offset, world = key
         D = sum(self.feature_dimensionalities)
         yc = self._y_cols()
@@ -734,7 +758,8 @@ class DistributedIBNet:
             with torch.cuda.device(self.device):
                 gx = torch.zeros(n, D, dtype=torch.float32, device=self.device)
                 gy = torch.zeros((n, yc) if yc > 0 else (n,), dtype=torch.float32, device=self.device)
-                phases = self._step_phases(gx, gy, global_batch, None, sample_offset, 0, device_step=True)
+                gs = torch.ones(n, dtype=torch.int32, device=self.device) if with_sizes else None
+                phases = self._step_phases(gx, gy, global_batch, None, sample_offset, 0, device_step=True, sizes=gs)
                 self._set_device_step(True)
                 torch.cuda.synchronize(self.device)
                 keep = [t.clone() for t in (self._params, self._m, self._v, self._step_dev, self._noise_step_dev)]
@@ -759,17 +784,19 @@ class DistributedIBNet:
             self._graph_failed = True
             self._set_device_step(False)
             return None
-        g = dict(graphs=graphs, x=gx, y=gy, launches=int(self._lib.dib_launch_count()) - launches0)
+        g = dict(graphs=graphs, x=gx, y=gy, sizes=gs, launches=int(self._lib.dib_launch_count()) - launches0)
         self._graphs[key] = g
         return g
 
-    def _replay_step(self, g, x, y):
+    def _replay_step(self, g, x, y, sizes=None):
         P = self._P
         if not self._step_dev_active or self._step_dev_dirty:
             self._set_device_step(True)
         self._replayed_launches += g["launches"]
         g["x"].copy_(x.reshape(g["x"].shape), non_blocking=True)
         g["y"].copy_(y.reshape(g["y"].shape), non_blocking=True)
+        if g["sizes"] is not None:
+            g["sizes"].copy_(sizes, non_blocking=True)
         for graph, exchange in g["graphs"]:
             graph.replay()
             if exchange is not None:
@@ -781,13 +808,13 @@ class DistributedIBNet:
         """GradientTape-style access (nb-bool cell 6 / train.py:201-220 custom loops): returns
         (flat gradient of task + beta*sum KL w.r.t. trainable_variables, statistics vector) as device tensors."""
         with torch.cuda.device(self.device):
-            xd = self._to_device(x, sum(self.feature_dimensionalities))
+            xd, sd = self._inputs(x)
             yd = self._targets(y)
             e = self._to_device(eps) if eps is not None else None
             if not global_batch:            # InfoNCE on several ranks: every rank passes its equal shard of the global batch
                 nce_world = parallel.world_and_rank(self.process_group)[0] if self._infonce is not None else 1
                 global_batch = max(xd.shape[0] * nce_world, 1)
-            self._backward(xd, yd, global_batch, e, sample_offset, step)
+            self._backward(xd, yd, global_batch, e, sample_offset, step, sizes=sd)
             return self._gradstats[:self._P].clone(), self._gradstats[self._P:].clone()
 
     # ------------------------------------------------------------------ encoder-only custom steps (SURVEY 8f3)
@@ -873,16 +900,16 @@ class DistributedIBNet:
         Noise: explicit ``eps`` [n, F, E], or Philox keyed by ``step`` (reproducible), or -- default -- a fresh draw
         on every call."""
         with torch.cuda.device(self.device):
-            x = self._to_device(inputs, sum(self.feature_dimensionalities))
+            x, sd = self._inputs(inputs)
             e = self._to_device(eps) if eps is not None else None
             st = self._inference_step() if step is None else step
-            pred, _, stats = self._forward(x, None, e, st, sample_offset)
+            pred, _, stats = self._forward(x, None, e, st, sample_offset, sizes=sd)
             n = x.shape[0]
             kl = stats[:self.number_features] / max(n, 1)
             self.losses = [self.beta._dev[0] * self.kl_loss_scale * kl.sum() ** self.kl_loss_exponent]
             self._last_kl = kl
             self.metrics_values = {"beta": self.beta.value()}
-        return _as_numpy_like(inputs, pred)
+        return _as_numpy_like(inputs[0] if isinstance(inputs, (list, tuple)) and inputs else inputs, pred)
 
     call = __call__
 
@@ -931,10 +958,10 @@ class DistributedIBNet:
             D = sum(self.feature_dimensionalities)
             world, rank = parallel.world_and_rank(self.process_group)
             host_x = not (isinstance(x, torch.Tensor) and x.is_cuda)
-            if sync or not host_x:
-                xd, yd = self._to_device(x, D), self._targets(y)
+            if sync or not host_x or self.variable_set_sizes:      # sized sets are not staged through the copy stream
+                (xd, sd), yd = self._inputs(x), self._targets(y)
                 n = xd.shape[0]
-                stats = self._train_step(xd, yd, global_batch=n * world, sample_offset=rank * n)
+                stats = self._train_step(xd, yd, global_batch=n * world, sample_offset=rank * n, sizes=sd)
                 res = PendingBatchResult(self, stats.detach().clone() if not sync else stats, None, None)
             else:
                 xd, yd, slot = self._stage_async(x, y, D)
@@ -1005,16 +1032,15 @@ class DistributedIBNet:
             raise RuntimeError("call compile() first")
         batch_size = 32 if batch_size is None else int(batch_size)
         world, rank = parallel.world_and_rank(self.process_group)
-        D = sum(self.feature_dimensionalities)
         if self._infonce is not None:
             self._check_infonce_world(self._infonce, batch_size)
         with torch.cuda.device(self.device):
-            xd, yd = self._to_device(x, D), self._targets(y)
+            (xd, sd), yd = self._inputs(x), self._targets(y)
             N = xd.shape[0]
             plan = self._batch_plan(N, batch_size)
-            xv = yv = None
+            xv = yv = sv = None
             if validation_data is not None:
-                xv, yv = self._to_device(validation_data[0], D), self._targets(validation_data[1])
+                (xv, sv), yv = self._inputs(validation_data[0]), self._targets(validation_data[1])
             history = History()
             cbs = list(callbacks or []) + [history]
             for cb in cbs:
@@ -1031,11 +1057,12 @@ class DistributedIBNet:
                 self._epoch_acc.zero_()
                 for b0, b1 in plan:
                     idx, lo = _shard_rows(order, b0, b1, rank, world)
-                    self._metrics_update(self._train_step(xd[idx], yd[idx], global_batch=b1 - b0, sample_offset=lo))
+                    self._metrics_update(self._train_step(xd[idx], yd[idx], global_batch=b1 - b0, sample_offset=lo,
+                                                          sizes=None if sd is None else sd[idx]))
                 logs = self._read_epoch_logs()
                 if xv is not None:
                     logs.update(self._evaluate_into_logs(xv, yv, *self._validation_plan(xv.shape[0], batch_size, epoch),
-                                                         2 ** 31 + epoch))
+                                                         2 ** 31 + epoch, sv))
                 if verbose not in (False, 0) and rank == 0:          # 'auto' -> 1 like Keras outside notebooks
                     print(f"Epoch {epoch + 1}/{epochs} - " + " - ".join(
                         f"{k}: {v:.4g}" for k, v in logs.items() if not k.removeprefix('val_').startswith('KL')))
@@ -1064,7 +1091,7 @@ class DistributedIBNet:
         order = self.validation_permutation(perm_key, n)[pos].reshape(-1)
         return self._batch_plan(order.shape[0], batch_size), order
 
-    def _evaluate_into_logs(self, xv, yv, plan, order, step):
+    def _evaluate_into_logs(self, xv, yv, plan, order, step, sv=None):
         """Validation logs of the batches ``plan`` of rows ``order`` (see :func:`_shard_rows`), noise keyed by (step, the
         row's position in ``order``): every rank runs the forward of its shard of a batch -- InfoNCE with more than one rank
         the first two phases of the step, without training -- and the statistics are summed over the ranks."""
@@ -1077,7 +1104,8 @@ class DistributedIBNet:
                 phases = self._step_phases(xv[idx], yv[idx], b1 - b0, None, b0 + lo, step, training=False, stats=stats)
                 _run_phases(phases[:2], last_exchange=False)
             else:
-                self._forward(xv[idx], yv[idx], None, step, b0 + lo, want_pred=False, stats_out=stats)
+                self._forward(xv[idx], yv[idx], None, step, b0 + lo, want_pred=False, stats_out=stats,
+                              sizes=None if sv is None else sv[idx])
             parallel.allreduce_sum_(stats, self.process_group)
             self._metrics_update(stats)
         return self._read_epoch_logs(prefix="val_")
@@ -1090,14 +1118,13 @@ class DistributedIBNet:
 
     def evaluate(self, x, y, batch_size=32, return_dict=True, **_):
         with torch.cuda.device(self.device):
-            D = sum(self.feature_dimensionalities)
             self._inference_calls += 1           # a fresh noise draw per evaluate() call
             key = (1 << 29) | (self._inference_calls & 0x1FFFFFFF)
             if self._infonce is not None:
                 self._check_infonce_world(self._infonce, batch_size)
-            xv, yv = self._to_device(x, D), self._targets(y)
+            (xv, sv), yv = self._inputs(x), self._targets(y)
             step = key if self._infonce is not None else 2 ** 31 + key
-            logs = self._evaluate_into_logs(xv, yv, *self._validation_plan(xv.shape[0], int(batch_size), key), step)
+            logs = self._evaluate_into_logs(xv, yv, *self._validation_plan(xv.shape[0], int(batch_size), key), step, sv)
         logs = {k[len("val_"):]: v for k, v in logs.items()}
         return logs if return_dict else [logs["loss"]] + [logs[m] for m in self.compiled_metrics_names]
 
@@ -1356,17 +1383,25 @@ def set_transformer_param_specs(d, encoder_arch, E, L, number_heads, key_dim, nu
     return specs
 
 
+# largest number_particles with variable_set_sizes (include/dib_b200.h: DIB_MAX_VARIABLE_SET_SIZE)
+MAX_VARIABLE_SET_SIZE = 256
+
+
 def check_set_transformer_args(particle_feature_dimensions, particle_encoder_arch_spec, bottleneck_dimension, number_particles,
                                key_dim, number_heads, number_attention_blocks, ff_arch_per_block, ff_activation_fn,
-                               final_processing_arch, activation_fn, output_dimensionality, precision):
+                               final_processing_arch, activation_fn, output_dimensionality, precision, variable_set_sizes=False):
     """The constructor checks of :class:`SetTransformerIBNet` (host only: they run before any device call)."""
     E, L = int(bottleneck_dimension), int(number_particles)
     if int(particle_feature_dimensions) < 1 or int(output_dimensionality) < 1:
         raise ValueError("particle_feature_dimensions and output_dimensionality must be >= 1")
     if any(int(w) < 1 for w in list(particle_encoder_arch_spec) + list(final_processing_arch) + list(ff_arch_per_block)):
         raise ValueError("layer widths must be >= 1")
-    if not 1 <= L <= 64:
-        raise ValueError(f"number_particles must be in [1, 64] (one attention problem per set and head in shared memory), got {L}")
+    if variable_set_sizes and not 1 <= L <= MAX_VARIABLE_SET_SIZE:
+        raise ValueError(f"number_particles (the largest set) must be in [1, {MAX_VARIABLE_SET_SIZE}] with variable_set_sizes, "
+                         f"got {L}")
+    if not variable_set_sizes and not 1 <= L <= 64:
+        raise ValueError(f"number_particles must be in [1, 64] (one attention problem per set and head in shared memory; up to "
+                         f"{MAX_VARIABLE_SET_SIZE} with variable_set_sizes=True), got {L}")
     if not 1 <= int(key_dim) <= 128 or int(number_heads) < 1 or int(number_attention_blocks) < 1:
         raise ValueError("the attention needs key_dim in [1, 128], number_heads >= 1 and number_attention_blocks >= 1")
     if (int(number_heads) * int(key_dim)) % 4 or E % 4 or E > 128:
@@ -1380,13 +1415,57 @@ def check_set_transformer_args(particle_feature_dimensions, particle_encoder_arc
         raise ValueError(f"precision must be one of {sorted(_lib.PRECISIONS)}, got {precision!r}")
 
 
+def pad_sets(sets, max_set_size):
+    """Sets of different sizes -- a list of N arrays [l_i, d], e.g. nb-particle's neighbourhoods before ``np.stack`` -- as
+    (x [N, max_set_size, d] float32 with zero padding rows, set_sizes [N] int32), the pair a variable-size
+    :class:`SetTransformerIBNet` takes."""
+    arrs = [np.asarray(a, dtype=np.float32) for a in sets]
+    if not arrs:
+        raise ValueError("pad_sets needs at least one set")
+    L = int(max_set_size)
+    d = arrs[0].shape[-1] if arrs[0].ndim == 2 else -1
+    for i, a in enumerate(arrs):
+        if a.ndim != 2 or a.shape[1] != d:
+            raise ValueError(f"set {i} has shape {a.shape}; every set must be [particles, {d}]")
+    sizes = np.array([a.shape[0] for a in arrs], dtype=np.int32)
+    check_set_sizes(sizes, len(arrs), L)
+    x = np.zeros((len(arrs), L, d), dtype=np.float32)
+    for i, a in enumerate(arrs):
+        x[i, :a.shape[0]] = a
+    return x, sizes
+
+
+def check_set_sizes(sizes, n, max_set_size):
+    """Host check of the sizes of n padded sets: an int array [n] with 1 <= size <= max_set_size."""
+    s = np.asarray(sizes)
+    if s.shape != (int(n),):
+        raise ValueError(f"set_sizes has shape {s.shape}; expected one size per set, ({int(n)},)")
+    if s.size and (s.min() < 1 or s.max() > int(max_set_size)):
+        bad = s[(s < 1) | (s > int(max_set_size))][0]
+        raise ValueError(f"set sizes must be in [1, {int(max_set_size)}], got {int(bad)}")
+
+
 class _ParticleEncoder(_FeatureEncoder):
     """model.particle_encoder: [..., d] -> [..., 2E] = (mu || logvar), logvar offset applied (dib_encode_feature on particle
-    rows).  ``utils.estimate_mi_sandwich_bounds(model.particle_encoder, particles [N, d])`` works on it."""
+    rows).  ``utils.estimate_mi_sandwich_bounds(model.particle_encoder, particles [N, d])`` works on it.  A variable-size model
+    also takes a list of [l_i, d] sets (-> a list of [l_i, 2E]) or a pair (x [N, Lmax, d], set_sizes [N]) (-> [N, Lmax, 2E],
+    padding rows zero); only the real particles are encoded."""
 
     def __call__(self, x, training=None):
+        m = self._model
+        if m.variable_set_sizes and isinstance(x, (list, tuple)):
+            if isinstance(x, list):
+                rows = np.concatenate([np.asarray(a, dtype=np.float32).reshape(-1, m.particle_feature_dimensions) for a in x])
+                out = m._encode_feature(0, torch.from_numpy(rows)).cpu().numpy()
+                return np.split(out, np.cumsum([len(a) for a in x])[:-1])
+            xd, sd = m._inputs(x)
+            L = m.number_particles
+            real = (torch.arange(L, device=m.device)[None, :] < sd[:, None].long()).reshape(-1)
+            out = torch.zeros(xd.shape[0] * L, 2 * m.feature_embedding_dimension, dtype=torch.float32, device=m.device)
+            out[real] = m._encode_feature(0, xd.reshape(-1, m.particle_feature_dimensions)[real])
+            return _as_numpy_like(x[0], out.reshape(xd.shape[0], L, -1))
         t = x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32))
-        out = self._model._encode_feature(0, t)
+        out = m._encode_feature(0, t)
         return _as_numpy_like(x, out.reshape(*t.shape[:-1], out.shape[-1]))
 
 
@@ -1402,17 +1481,28 @@ class SetTransformerIBNet(DistributedIBNet):
     ``x`` is [N, number_particles, particle_feature_dimensions] and ``y`` [N, output_dimensionality]; batches count sets.
     ``model.particle_encoder(x)`` returns mu || logvar per particle and ``model.set_transformer(embs)`` runs the network
     after the encoder.  History keys: loss, accuracy (with metrics=['accuracy']), KL0 (per set), beta and their val_ twins.
-    ``fp16`` / ``bf16`` run every dense layer on the TF32 kernels; the attention and LayerNorm kernels are fp32 in every mode."""
+    ``fp16`` / ``bf16`` run every dense layer on the TF32 kernels; the attention and LayerNorm kernels are fp32 in every mode.
+
+    ``variable_set_sizes=True`` takes sets of different sizes, up to ``number_particles`` (at most 256) particles each -- the
+    notebook's ragged neighbourhoods without clipping them to one size.  Wherever ``x`` goes (``fit`` and its
+    ``validation_data``, ``evaluate``, ``predict``, ``train_on_batch``, ``compute_gradients``, calling the model), pass either a
+    list of N arrays [l_i, d] or a pair (x_padded [N, number_particles, d], set_sizes [N]) (see :func:`pad_sets`).  Each set's
+    loss, KL, prediction and gradient are the fixed-size model's with number_particles = l_i on its real particles: padding keys
+    are masked out of the attention (Keras' attention_mask), the mean runs over the real particles, the KL sums over them, and
+    what the padding rows hold is ignored.  ``model.set_transformer(embs, set_sizes=...)`` takes the sizes of padded
+    embeddings [N, number_particles, E] (or a list of [l_i, E])."""
 
     def __init__(self, particle_feature_dimensions, particle_encoder_arch_spec, bottleneck_dimension=32, number_particles=50,
                  key_dim=128, number_heads=12, number_attention_blocks=6, ff_arch_per_block=None, ff_activation_fn='relu',
                  final_processing_arch=(256,), activation_fn='leaky_relu', leaky_alpha=0.1, output_dimensionality=1,
-                 logvar_initialization=-3., number_positional_encoding_frequencies=5, precision='fp32', **kw):
+                 logvar_initialization=-3., number_positional_encoding_frequencies=5, precision='fp32', variable_set_sizes=False,
+                 **kw):
         E = int(bottleneck_dimension)
         ff = [128, E] if ff_arch_per_block is None else [int(w) for w in ff_arch_per_block]
         check_set_transformer_args(particle_feature_dimensions, particle_encoder_arch_spec, E, number_particles, key_dim,
                                    number_heads, number_attention_blocks, ff, ff_activation_fn, final_processing_arch,
-                                   activation_fn, output_dimensionality, precision)
+                                   activation_fn, output_dimensionality, precision, bool(variable_set_sizes))
+        self.variable_set_sizes = bool(variable_set_sizes)
         self.particle_feature_dimensions = int(particle_feature_dimensions)
         self.number_particles = int(number_particles)
         self.key_dim, self.number_heads = int(key_dim), int(number_heads)
@@ -1445,7 +1535,65 @@ class SetTransformerIBNet(DistributedIBNet):
         cfg.number_ff_layers, cfg.ff_architecture = len(self.ff_arch_per_block), self._c_ff
         cfg.ff_activation_fn = _lib.ACTIVATIONS[self.ff_activation_fn]
         cfg.layer_norm_epsilon = 1e-3                                        # [KERAS] LayerNormalization default
+        cfg.variable_set_sizes = int(self.variable_set_sizes)
         return cfg
+
+    def _device_sizes(self, sizes, n):
+        """Set sizes checked on the host (one read of a device tensor), then as int32 on the device."""
+        host = sizes.detach().cpu().numpy() if isinstance(sizes, torch.Tensor) else np.asarray(sizes)
+        if host.dtype.kind not in "iu":
+            raise ValueError(f"set_sizes must be integers, got {host.dtype}")
+        check_set_sizes(host, n, self.number_particles)
+        if isinstance(sizes, torch.Tensor):
+            return sizes.to(device=self.device, dtype=torch.int32).contiguous()
+        return torch.from_numpy(np.ascontiguousarray(host, dtype=np.int32)).to(self.device)
+
+    def _inputs(self, x):
+        """Variable set sizes: a list of [l_i, d] sets or a pair (x [N, Lmax, d], set_sizes [N]) -> (x [N, Lmax * d] on the
+        device, int32 sizes on the device), the sizes checked before any device work."""
+        if not self.variable_set_sizes:
+            return super()._inputs(x)
+        L, d = self.number_particles, self.particle_feature_dimensions
+        if isinstance(x, list):
+            x = pad_sets(x, L)
+        if not (isinstance(x, tuple) and len(x) == 2):
+            raise ValueError("a SetTransformerIBNet with variable_set_sizes takes a list of [particles, d] arrays or a pair "
+                             "(x_padded [N, number_particles, d], set_sizes [N])")
+        xp, sizes = x
+        shape = tuple(xp.shape)
+        if len(shape) != 3 or shape[1:] != (L, d):
+            raise ValueError(f"padded x has shape {shape}; expected [N, {L}, {d}]")
+        sd = self._device_sizes(sizes, shape[0])
+        return self._to_device(xp, L * d), sd
+
+    def _integration_inputs(self, emb, set_sizes, width):
+        if not self.variable_set_sizes:
+            return super()._integration_inputs(emb, set_sizes, width)
+        E = self.feature_embedding_dimension
+        if isinstance(emb, list):
+            if set_sizes is not None:
+                raise ValueError("a list of embeddings carries its own set sizes")
+            emb, set_sizes = pad_sets(emb, self.number_particles)
+        if set_sizes is None:
+            raise ValueError("model.set_transformer of a variable-size model needs set_sizes (or a list of [l_i, E] embeddings)")
+        if len(emb.shape) != 3 or tuple(emb.shape[1:]) != (self.number_particles, E):
+            raise ValueError(f"embeddings have shape {tuple(emb.shape)}; expected [N, {self.number_particles}, {E}]")
+        sd = self._device_sizes(set_sizes, emb.shape[0])
+        return self._to_device(emb, width), sd
+
+    def predict(self, x, batch_size=32, **_):
+        if not self.variable_set_sizes:
+            return super().predict(x, batch_size)
+        if isinstance(x, list):
+            x = pad_sets(x, self.number_particles)
+        xp, sizes = x
+        self._device_sizes(sizes, xp.shape[0])                  # checked once, before any device work
+        outs, n = [], xp.shape[0]
+        st = self._inference_step()
+        for b0 in range(0, n, int(batch_size)):
+            o = self((xp[b0:b0 + int(batch_size)], sizes[b0:b0 + int(batch_size)]), training=False, step=st, sample_offset=b0)
+            outs.append(o if isinstance(xp, torch.Tensor) else np.asarray(o))
+        return torch.cat(outs) if isinstance(xp, torch.Tensor) else np.concatenate(outs)
 
     def param_specs(self):
         """(name, Keras shape, init) of every trainable variable in flat order; see :func:`set_transformer_param_specs`."""

@@ -33,9 +33,12 @@
 extern "C" {
 #endif
 
-/* 3 appended the InfoNCE fields to dib_config, 4 the integration-network fields; dib_create still accepts abi_version 2 and 3
- * structs and reads only their prefix. */
-#define DIB_ABI_VERSION 4
+/* 3 appended the InfoNCE fields to dib_config, 4 the integration-network fields, 5 variable_set_sizes; dib_create still accepts
+ * abi_version 2, 3 and 4 structs and reads only their prefix. */
+#define DIB_ABI_VERSION 5
+
+/* largest set_size of a set transformer with variable_set_sizes (fixed-size sets: 64) */
+#define DIB_MAX_VARIABLE_SET_SIZE 256
 
 /* activation_fn strings accepted by tf.keras.layers.Dense in the reference's call sites
  * (train.py:37 'relu', nb-radial 'tanh', nb-bool LeakyReLU, None). */
@@ -100,7 +103,16 @@ enum dib_encoder_kind { DIB_ENCODER_MLP = 0, DIB_ENCODER_SIMPLE = 1 };
  * particle p of set s is keyed by the global particle row (sample_offset + s) * set_size + p.
  * Needs set_size in [1, 64], key_dim in [1, 128], number_heads * key_dim and E multiples of 4, E <= 128, max_batch <= 65535,
  * no dropout, and a loss other than DIB_LOSS_SPARSE_CE_LOGITS / DIB_LOSS_INFONCE.  The attention core and the LayerNorms are
- * fp32 CUDA-core kernels in every precision; FP16 / BF16 run every dense layer on the TF32 kernels. */
+ * fp32 CUDA-core kernels in every precision; FP16 / BF16 run every dense layer on the TF32 kernels.
+ * Variable set sizes (abi_version >= 5, variable_set_sizes = 1; nb-particle's ragged neighbourhoods): set_size is the largest
+ * set Lmax, in [1, DIB_MAX_VARIABLE_SET_SIZE].  x stays [n, Lmax, d], each set padded to Lmax rows, and set s has l_s real
+ * particles, 1 <= l_s <= Lmax, given by dib_set_set_sizes_device.  Per set, loss, KL, prediction and gradients are those of the
+ * fixed-size model with set_size = l_s on the real particles: keys p >= l_s are masked out of every softmax (Keras 2
+ * MultiHeadAttention with attention_mask), the mean runs over the l_s real rows, and the KL slot sums over real particles only.
+ * Padding rows are zeroed before the encoder and get u = 0 and zero gradients: their content, NaN included, changes nothing.
+ * Noise stays keyed by the padded row (sample_offset + s) * set_size + p.  The attention runs on key-tiled kernels whose
+ * shared memory does not depend on Lmax and whose work follows sum_s l_s^2; the dense layers still run on all n * Lmax rows.
+ * The workspace stays linear in max_batch * set_size. */
 enum dib_integration_kind { DIB_INTEGRATION_MLP = 0, DIB_INTEGRATION_SET_TRANSFORMER = 1 };
 
 /* Mirrors the constructor of models.DistributedIBNet (models.py:56-66). */
@@ -147,6 +159,8 @@ typedef struct dib_config {
   const int32_t* ff_architecture;    /* [128, E] */
   int32_t ff_activation_fn;          /* enum dib_activation; relu on every FF layer in the notebook */
   float   layer_norm_epsilon;        /* 0 -> 1e-3 (the Keras default) */
+  /* ---- abi_version >= 5 ---- */
+  int32_t variable_set_sizes;        /* set transformer: 1 = sets of l_s <= set_size particles (dib_set_set_sizes_device) */
 } dib_config;
 
 typedef struct dib_model dib_model;
@@ -245,6 +259,13 @@ int dib_encoders_backward(dib_model* h, const float* params, const float* x, con
  * and the encoder-only entry points keep the by-value step).  The caller owns the counter and advances it (on the stream)
  * between steps.  NULL restores the by-value behaviour. */
 int dib_set_noise_step_device(dib_model* h, const uint32_t* step_dev);
+
+/* Variable set sizes: set_sizes_dev is DEVICE memory holding the int32 sizes of the n local sets of the following dib_forward,
+ * dib_train_step and dib_integration_forward calls of this handle (data parallel: the sizes of this rank's shard).  The kernels
+ * read it on the stream, so one captured graph serves every size vector written into the buffer.  The caller checks
+ * 1 <= size <= set_size: out-of-range sizes keep every access in bounds but give meaningless results.  A variable-size handle
+ * without bound sizes fails those calls; NULL unbinds.  Fails on a fixed-size handle. */
+int dib_set_set_sizes_device(dib_model* h, const int32_t* set_sizes_dev);
 
 /* tf.keras.optimizers.Adam dense update over the flat buffer (train.py:128-129, nb-radial Adam(lr)):
  *   t = *step_dev + 1 (the kernel increments *step_dev);  lr_t = lr*sqrt(1-b2^t)/(1-b1^t);
