@@ -253,7 +253,8 @@ dib_int16_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
 // Fused tail of the integration network for single-output models (C0, nb-radial): the last two hidden layers
 // (256 wide each) and the output head in ONE persistent kernel -- models.py:81-84,122 + the compiled loss.
 //   per 128-row tile:  L0  D0 = A W0   (A, W0 k-blocks streamed through a TMA ring; N = 256, fp32 in registers)
-//                      e0  g1 = act(D0 + b0) -> 16-bit -> swizzled shared tile (= L1's A operand) and -> HBM (the backward needs it)
+//                      e0  g1 = act(D0 + b0) -> 16-bit -> swizzled shared tile (= L1's A operand) -> TMA tensor store to HBM
+//                          (the weight gradients need it) while L1 reads the same tile
 //                      L1  D1 = g1 W1  (W1 k-blocks through the same ring)
 //                      e1  g2 = act(D1 + b1) kept PACKED IN REGISTERS, logit = g2 . w + b, compiled loss / metric,
 //                          d loss / d logit, dg2 = dz w act'(g2) -> HBM, output-layer weight / bias gradients and the bias gradient
@@ -261,32 +262,42 @@ dib_int16_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
 //   training, backward stages on (dg1 != null), the dgrad chain of the same rows:
 //                      D1  acc = dg2 W1^T  (dg2 packed in registers = the wgmma A fragment; W1 K-major through the ring;
 //                          two 128-column chunks)
-//                      e2  dg1 = acc act'(g1) (g1 read back from the shared tile) -> HBM, packed into registers; its column
-//                          sums per tile (bias gradient of the first fused layer) -> dbpart, in the order of the DGRAD epilogue
+//                      e2  dg1 = acc act'(g1) (g1 read back from the shared tile) -> over g1 in the shared tile -> TMA tensor
+//                          store, and packed into registers; its column sums per tile (bias gradient of the first fused layer)
+//                          -> dbpart, in the order of the DGRAD epilogue
 //                      D0  (only when the layer below is the embedding, which has no act') d emb = dg1 W0^T over 128-column
 //                          chunks (W0 K-major through the ring)
-//                      e3  16-bit d emb -> the g1 tile (free by then) -> TMA tensor store (no partial-sector writes)
+//                      e3  16-bit d emb -> the g1 tile (free by then) -> TMA tensor store
+// The tensor stores leave no partial-sector writes behind and run while the MMAs go on; 4-byte fragment stores straight
+// from the accumulators stall the epilogue that issues them.  Only dg2, produced while the g1 tile still holds g1 (needed
+// by e2's act'), leaves as fragment stores.
 // g2 never reaches HBM, and the head's re-read of it (and its launch) disappears; with the backward stages, neither do
 // the two dgrad launches nor their re-reads of dg2, dg1 and g1.  A warp owns 16 whole rows of the accumulator, so each
 // row's logit is complete after a reduction over the 4 lanes that share the row.  Every MMA keeps the operands and the
 // k order of dib_int16_dgrad, and every sum its order: the results are those of the separate launches, bit for bit.
 // Ring stages of a tile: nk0 x (A, W0 MN-major), 4 x W1 MN-major; then 2 x 2 x W1 K-major and K0 / 128 x 2 x W0 K-major
-// (B only: 128 output columns x 128 k each).  Shared memory: the 2-stage ring (2 x 48 KB), the g1 tile (4 swizzled
-// 64-column panels of 128 rows, 64 KB), the barriers, and statically the bias / head-weight rows and the column-sum scratch.
+// (B only: 128 output columns x 128 k each).  The ring is 3 deep, so two loads are in flight while the consumers run a
+// stage's MMAs, and during each epilogue the producer fills the first stages of the next phase (or of the next tile).
+// Shared memory: the 3-stage ring (3 x 48 KB), the g1 tile (4 swizzled 64-column panels of 128 rows, 64 KB), the barriers,
+// and statically the bias / head-weight rows and one [8][256] column-sum scratch (used in turn by the output layer's dW,
+// the bias gradient of the last hidden layer and that of the first fused layer).
 // ====================================================================================================
-constexpr int kF2N = 256, kF2Stages = 2;
+constexpr int kF2N = 256, kF2Stages = 3;
 constexpr int kF2AB = kBM * 128, kF2BB = kF2N * 128, kF2Stage = kF2AB + kF2BB;      // 16 KB + 32 KB
 constexpr int kF2BtN = 128, kF2BtB = kF2BtN * 128;   // backward stages: B only, two k-blocks of 128 K-major rows (2 x 16 KB)
 constexpr int kF2G1Off = kF2Stages * kF2Stage;
 constexpr int kF2BarOff = kF2G1Off + kBM * kF2N * 2;
 constexpr int kF2Smem = kF2BarOff + 64 + 1024;
+// static shared memory of the kernel: s_b0, s_b1, s_w; s_col; s_red
+constexpr int kF2StaticSmem = (3 * kF2N + (kConsumers / 32) * kF2N + 3 * (kConsumers / 32)) * (int)sizeof(float);
+static_assert(2 * 8 * kF2Stages <= 64, "the ring's full and empty barriers fit their 64 bytes");
+static_assert(kF2Smem + kF2StaticSmem <= 232448, "fused tail: shared memory above the sm_90 227 KB per-block opt-in");
 
 struct Fwd2Args {
   const float *b0, *b1, *wout, *bout;
-  uint16_t* g1; int ldg1;             // out: first fused layer's activation [M x 256]
   uint16_t* dg2; int lddg;            // out (training) or null: gradient w.r.t. the second fused layer's pre-activation, x gscale
-  uint16_t* dg1;                      // out (training, backward stages) or null: gradient w.r.t. the first fused layer's
-                                      // pre-activation [M x 256], x gscale
+  bool bwd;                           // training, backward stages: dg1, the gradient w.r.t. the first fused layer's
+                                      // pre-activation [M x 256] x gscale, via mapDg1
   float* dbpart;                      // with dg1: column sums of dg1 per 128-row tile [tiles][256]
   int demb_cols;                      // with dg1, > 0: the layer below is the embedding; d emb [M x demb_cols] via mapDemb
   const float* y; float* user_pred;
@@ -302,7 +313,8 @@ template <bool BF16, int ACT>
 __global__ void __launch_bounds__(kF2Threads, 1)
 dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapW0,
                       const __grid_constant__ CUtensorMap mapW1, const __grid_constant__ CUtensorMap mapW1t,
-                      const __grid_constant__ CUtensorMap mapW0t, const __grid_constant__ CUtensorMap mapDemb, const Fwd2Args a) {
+                      const __grid_constant__ CUtensorMap mapW0t, const __grid_constant__ CUtensorMap mapDemb,
+                      const __grid_constant__ CUtensorMap mapG1, const __grid_constant__ CUtensorMap mapDg1, const Fwd2Args a) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sb = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bar_base = sb + kF2BarOff;
@@ -311,11 +323,11 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
   const uint32_t g1s = sb + kF2G1Off;
 
   __shared__ __align__(16) float s_b0[kF2N], s_b1[kF2N], s_w[kF2N];
-  __shared__ float s_colw[kConsumers / 32][kF2N], s_colb[kConsumers / 32][kF2N];
+  __shared__ float s_col[kConsumers / 32][kF2N];     // per-warp column sums of one quantity at a time
   __shared__ float s_red[3][kConsumers / 32];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int ntile = DIB_CEIL_DIV(a.M, kBM);
-  const bool bwd = a.dg1 != nullptr;
+  const bool bwd = a.bwd;
 
   for (int i = tid; i < kF2N; i += blockDim.x) { s_b0[i] = a.b0[i]; s_b1[i] = a.b1[i]; s_w[i] = a.wout[i]; }
   if (tid == 0) {
@@ -393,7 +405,7 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
   };
   // acc = A[64 x 256] B[256 x 128] over 2 B-only ring stages of two k-blocks; A packed in registers (ap[4 t .. 4 t + 3]: the
   // fragment of k16 step t).  128-column chunks: a 256-column accumulator next to the 64 A registers does not fit the
-  // register budget.  Stages of 128 k: the ring is 2 deep, and half as many stages halves the exposed load latencies.
+  // register budget.  Stages of 128 k: half as many stages as 64-deep ones, so half as many load latencies to hide.
   auto mainloop_rs = [&](float (&acc)[64], const uint32_t (&ap)[64]) {
     uint32_t prev = 0;
 #pragma unroll
@@ -419,10 +431,18 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
   };
   // this thread's word (columns c, c + 1 of row r) in the swizzled g1 tile; every thread reads back only words it wrote
   auto g1_word = [&](int c, int r) { return g1s + (c >> 6) * kF2AB + r * 128 + ((((c & 63) >> 3) ^ (r & 7)) << 4) + 4 * q; };
-  // the warpgroup's d emb stores, all (N = 0) or all but the last group (N = 1), have read its rows of the g1 tile
+  // the warpgroup's tensor stores, all (N = 0) or all but the last group (N = 1), have read its rows of the g1 tile
   auto stores_drained = [&](auto n_pending) {
     if ((tid & 127) == 0) bulk_wait_read<decltype(n_pending)::value>();
     named_bar_sync(2 + wg, 128);
+  };
+  // the warpgroup's rows of g1-tile panels [p0, p0 + n) -> columns [c0, c0 + 64 n) of a 16-bit [M x *] tensor as one store
+  // group (rows past M are not written); the caller has fenced its shared writes and synchronised the warpgroup
+  auto store_panels = [&](const CUtensorMap* m, int tile, int p0, int n, int c0) {
+    if ((tid & 127) == 0) {
+      for (int p = 0; p < n; ++p) tma_store_2d(m, g1s + (p0 + p) * kF2AB + wg * 64 * 128, c0 + 64 * p, tile * kBM + 64 * wg);
+      bulk_commit();
+    }
   };
 
   for (int tile = blockIdx.x; tile < ntile; tile += gridDim.x) {
@@ -430,23 +450,22 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
     float acc[128];
 #pragma unroll
     for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-    // ---------------- L0, e0: g1 = act(D0 + b0) -> shared tile (L1's A operand) and HBM
+    // ---------------- L0, e0: g1 = act(D0 + b0) -> shared tile (L1's A operand) -> HBM
     mainloop(acc, a.nk0, true);
-    if (a.demb_cols > 0) stores_drained(std::integral_constant<int, 0>());
+    stores_drained(std::integral_constant<int, 0>());   // the previous tile's stores have read the g1 tile
 #pragma unroll
     for (int j = 0; j < kF2N / 8; ++j) {
       const int c = 8 * j + 2 * q;
       const float2 bv = *reinterpret_cast<const float2*>(&s_b0[c]);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int r = rb + 8 * h;
         const uint32_t w = pack_h2<BF16>(dib_act16(ACT, acc[4 * j + 2 * h] + bv.x, a.alpha), dib_act16(ACT, acc[4 * j + 2 * h + 1] + bv.y, a.alpha));
-        st_shared_b32(g1_word(c, r), w);
-        if (row_lo + 8 * h < a.M) *reinterpret_cast<uint32_t*>(a.g1 + (row_lo + 8 * h) * a.ldg1 + c) = w;
+        st_shared_b32(g1_word(c, rb + 8 * h), w);
       }
     }
     fence_proxy_async_smem();
     named_bar_sync(2 + wg, 128);                     // this warpgroup's rows of g1 are complete
+    store_panels(&mapG1, tile, 0, kF2N / 64, 0);
     // ---------------- L1, e1 pass 1: g2 = act(D1 + b1) packed into registers, partial logits
 #pragma unroll
     for (int i = 0; i < 128; ++i) acc[i] = 0.f;
@@ -493,43 +512,52 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
       if (q == 0) dbo += dzs[h];
     }
     if (train) {
-      // ---------------- e1, pass 2: dg2 = ds w act'(g2) -> HBM and packed into g2p (A of D1); column sums of g2 dz (output-layer
-      // dW) and of dg2 (bias gradient)
+      // ---------------- e1, pass 2: column sums of g2 dz (output-layer dW).  The 8 warps cover the tile's 128 rows: fixed-order
+      // combine into the thread-owned column
+#pragma unroll
+      for (int j = 0; j < kF2N / 8; ++j) {
+        const int c = 8 * j + 2 * q;
+        float cw[2] = {0.f, 0.f};
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float h0, h1;
+          unpack_h2<BF16>(g2p[2 * j + h], h0, h1);
+          cw[0] += h0 * dzs[h]; cw[1] += h1 * dzs[h];
+        }
+        cw[0] = quad_col_sum(cw[0]); cw[1] = quad_col_sum(cw[1]);
+        if (lane < 4) { s_col[warp][c] = cw[0]; s_col[warp][c + 1] = cw[1]; }
+      }
+      named_bar_sync(1, kConsumers);
+#pragma unroll
+      for (int w = 0; w < kConsumers / 32; ++w) acc_dw += s_col[w][tid];
+      named_bar_sync(1, kConsumers);
+      // ---------------- e1, pass 3: dg2 = ds w act'(g2) -> HBM and packed into g2p (A of D1); its column sums (bias gradient)
 #pragma unroll
       for (int j = 0; j < kF2N / 8; ++j) {
         const int c = 8 * j + 2 * q;
         const float2 wv = *reinterpret_cast<const float2*>(&s_w[c]);
-        float cw[2] = {0.f, 0.f}, cb[2] = {0.f, 0.f};
+        float cb[2] = {0.f, 0.f};
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           float h0, h1;
           unpack_h2<BF16>(g2p[2 * j + h], h0, h1);
           const float d0 = ds[h] * wv.x * dib_act_grad(ACT, h0, a.alpha), d1 = ds[h] * wv.y * dib_act_grad(ACT, h1, a.alpha);
-          cw[0] += h0 * dzs[h]; cw[1] += h1 * dzs[h];
           cb[0] += d0; cb[1] += d1;
           const uint32_t dp = pack_h2<BF16>(d0, d1);
           g2p[2 * j + h] = dp;
           if (row_lo + 8 * h < a.M) *reinterpret_cast<uint32_t*>(a.dg2 + (row_lo + 8 * h) * a.lddg + c) = dp;
         }
-#pragma unroll
-        for (int k = 0; k < 2; ++k) {
-          cw[k] = quad_col_sum(cw[k]);
-          cb[k] = quad_col_sum(cb[k]);
-        }
-        if (lane < 4) {
-          s_colw[warp][c] = cw[0]; s_colw[warp][c + 1] = cw[1];
-          s_colb[warp][c] = cb[0]; s_colb[warp][c + 1] = cb[1];
-        }
+        cb[0] = quad_col_sum(cb[0]); cb[1] = quad_col_sum(cb[1]);
+        if (lane < 4) { s_col[warp][c] = cb[0]; s_col[warp][c + 1] = cb[1]; }
       }
-      // the 8 warps cover the tile's 128 rows: fixed-order combine into the thread-owned column
       named_bar_sync(1, kConsumers);
 #pragma unroll
-      for (int w = 0; w < kConsumers / 32; ++w) { acc_dw += s_colw[w][tid]; acc_dbh += s_colb[w][tid]; }
+      for (int w = 0; w < kConsumers / 32; ++w) acc_dbh += s_col[w][tid];
       named_bar_sync(1, kConsumers);
     }
     if (bwd) {
-      // ---------------- D1, e2 per 128-column chunk: dg1 = (dg2 W1^T) act'(g1) -> HBM and packed into dg1p (A of D0);
-      // column sums -> dbpart row of the tile
+      // ---------------- D1, e2 per 128-column chunk: dg1 = (dg2 W1^T) act'(g1) -> over the chunk's g1 in the shared tile (each
+      // thread overwrites the words it reads) -> HBM, and packed into dg1p (A of D0); column sums -> dbpart row of the tile
       uint32_t dg1p[64];
       float acc2[64];
 #pragma unroll
@@ -537,6 +565,7 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
 #pragma unroll
         for (int i = 0; i < 64; ++i) acc2[i] = 0.f;
         mainloop_rs(acc2, g2p);
+        if (cc == 0) stores_drained(std::integral_constant<int, 0>());   // the g1 store has read the tile
 #pragma unroll
         for (int j = 0; j < kF2BtN / 8; ++j) {
           const int c = kF2BtN * cc + 8 * j + 2 * q;
@@ -544,36 +573,38 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             float x0, x1;
-            unpack_h2<BF16>(ld_shared_b32(g1_word(c, rb + 8 * h)), x0, x1);
+            const uint32_t wa = g1_word(c, rb + 8 * h);
+            unpack_h2<BF16>(ld_shared_b32(wa), x0, x1);
             const float v0 = acc2[4 * j + 2 * h] * dib_act_grad(ACT, x0, a.alpha);
             const float v1 = acc2[4 * j + 2 * h + 1] * dib_act_grad(ACT, x1, a.alpha);
             const uint32_t p = pack_h2<BF16>(v0, v1);
             dg1p[2 * (kF2BtN / 8 * cc + j) + h] = p;
-            if (row_lo + 8 * h < a.M) {                   // rows outside the matrix add nothing
-              *reinterpret_cast<uint32_t*>(a.dg1 + (row_lo + 8 * h) * kF2N + c) = p;
-              cs[0] += v0; cs[1] += v1;
-            }
+            st_shared_b32(wa, p);
+            if (row_lo + 8 * h < a.M) { cs[0] += v0; cs[1] += v1; }   // rows outside the matrix add nothing
           }
           cs[0] = quad_col_sum(cs[0]); cs[1] = quad_col_sum(cs[1]);
-          if (lane < 4) { s_colb[warp][c] = cs[0]; s_colb[warp][c + 1] = cs[1]; }
+          if (lane < 4) { s_col[warp][c] = cs[0]; s_col[warp][c + 1] = cs[1]; }
         }
+        fence_proxy_async_smem();
+        named_bar_sync(2 + wg, 128);
+        store_panels(&mapDg1, tile, 2 * cc, kF2BtN / 64, kF2BtN * cc);
       }
       named_bar_sync(1, kConsumers);
       {
         float sum = 0.f;
 #pragma unroll
-        for (int w = 0; w < kConsumers / 32; ++w) sum += s_colb[w][tid];
+        for (int w = 0; w < kConsumers / 32; ++w) sum += s_col[w][tid];
         a.dbpart[(long long)tile * kF2N + tid] = sum;
       }
       named_bar_sync(1, kConsumers);
       // ---------------- D0, e3: d emb = dg1 W0^T per 128-column chunk -> two 64-column panels of the warpgroup's rows of the
-      // g1 tile (chunks alternate between panels 0-1 and 2-3, so a chunk waits only for the stores of the chunk before last)
-      // -> TMA store
+      // g1 tile (chunks alternate between panels 0-1 and 2-3, as the dg1 stores did, so a chunk waits only for the store
+      // group before last) -> TMA store
       for (int c0 = 0, cc = 0; c0 < a.demb_cols; c0 += kF2BtN, ++cc) {
 #pragma unroll
         for (int i = 0; i < 64; ++i) acc2[i] = 0.f;
         mainloop_rs(acc2, dg1p);
-        if (cc >= 2) stores_drained(std::integral_constant<int, 1>());
+        stores_drained(std::integral_constant<int, 1>());
         const int tc = (cc & 1) * kF2BtN;                 // shared-tile columns of this chunk
 #pragma unroll
         for (int j = 0; j < kF2BtN / 8; ++j) {
@@ -583,15 +614,11 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
         }
         fence_proxy_async_smem();
         named_bar_sync(2 + wg, 128);
-        if ((tid & 127) == 0) {
-          for (int p = 0; p < kF2BtN / 64 && c0 + 64 * p < a.demb_cols; ++p)
-            tma_store_2d(&mapDemb, g1s + (tc / 64 + p) * kF2AB + wg * 64 * 128, c0 + 64 * p, tile * kBM + 64 * wg);
-          bulk_commit();
-        }
+        store_panels(&mapDemb, tile, tc / 64, min(kF2BtN, a.demb_cols - c0) / 64, c0);
       }
     }
   }
-  if (a.demb_cols > 0 && (tid & 127) == 0) bulk_wait_all();
+  if ((tid & 127) == 0) bulk_wait_all();
   // ---------------- per-CTA partials, layout of the head kernels: [dWc (K) | dbc (1) | column sums of dg2 (K)], loss, accuracy
   if (train) {
     a.wpart[(long long)blockIdx.x * a.wpart_stride + tid] = acc_dw;
@@ -1056,14 +1083,16 @@ cudaError_t dib_int16_fwd2_head(const void* g_in, int ld_in, int K0, const void*
   CUtensorMap mA, mW0, mW1;
   if (!map_k(&mA, g_in, K0, M, ld_in, kBM) || !map_mn(&mW0, w16_0, kF2N, K0, kF2N, kF2N / 64) || !map_mn(&mW1, w16_1, kF2N, kF2N, kF2N, kF2N / 64))
     return cudaErrorInvalidValue;
-  // backward stages: W1 and W0 K-major (box 64 x 128, as dib_int16_dgrad reads them), the d emb store map (box 64 x 64)
-  CUtensorMap mW1t = mA, mW0t = mA, mDemb = mA;
-  if (dg1 && !map_k(&mW1t, w16_1, kF2N, kF2N, kF2N, kF2BtN)) return cudaErrorInvalidValue;
+  // the store maps of g1, dg1 and d emb (box 64 x 64: one panel of a warpgroup's rows); backward stages: W1 and W0 K-major
+  // (box 64 x 128, as dib_int16_dgrad reads them)
+  CUtensorMap mG1, mW1t = mA, mW0t = mA, mDg1 = mA, mDemb = mA;
+  if (!map_k(&mG1, g1, kF2N, M, kF2N, 64)) return cudaErrorInvalidValue;
+  if (dg1 && (!map_k(&mW1t, w16_1, kF2N, kF2N, kF2N, kF2BtN) || !map_k(&mDg1, dg1, kF2N, M, kF2N, 64))) return cudaErrorInvalidValue;
   if (demb && (!map_k(&mW0t, w16_0, kF2N, K0, kF2N, kF2BtN) || !map_k(&mDemb, demb, K0, M, K0, 64))) return cudaErrorInvalidValue;
   Fwd2Args a{};
-  a.b0 = b0; a.b1 = b1; a.wout = wout; a.bout = bout; a.g1 = static_cast<uint16_t*>(g1); a.ldg1 = kF2N;
+  a.b0 = b0; a.b1 = b1; a.wout = wout; a.bout = bout;
   a.dg2 = static_cast<uint16_t*>(dg2); a.lddg = kF2N; a.y = y; a.user_pred = user_pred; a.wpart = wpart; a.wpart_stride = wpart_stride;
-  a.dg1 = static_cast<uint16_t*>(dg1); a.dbpart = dbpart; a.demb_cols = demb ? K0 : 0;
+  a.bwd = dg1 != nullptr; a.dbpart = dbpart; a.demb_cols = demb ? K0 : 0;
   a.loss_part = loss_part; a.acc_part = acc_part; a.M = M; a.nk0 = K0 / kBK; a.act = act; a.out_act = out_act; a.loss = loss;
   a.alpha = alpha; a.inv_batch = inv_batch; a.gscale = gscale;
   const int tiles = DIB_CEIL_DIV(M, kBM);
@@ -1077,7 +1106,7 @@ cudaError_t dib_int16_fwd2_head(const void* g_in, int ld_in, int K0, const void*
     e = attr ? cudaSuccess : cudaFuncSetAttribute(dib_int16_fwd2_kernel<BF, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, kF2Smem); \
     if (e != cudaSuccess) return e;                                                                                                  \
     attr = true;                                                                                                                     \
-    dib_int16_fwd2_kernel<BF, ACT><<<grid, kF2Threads, kF2Smem, st>>>(mA, mW0, mW1, mW1t, mW0t, mDemb, a);                           \
+    dib_int16_fwd2_kernel<BF, ACT><<<grid, kF2Threads, kF2Smem, st>>>(mA, mW0, mW1, mW1t, mW0t, mDemb, mG1, mDg1, a);               \
   } while (0)
 #define DIB_F2_ACT(ACT) do { if (bf16) DIB_F2_LAUNCH(true, ACT); else DIB_F2_LAUNCH(false, ACT); } while (0)
   switch (act) {
