@@ -109,6 +109,9 @@ SIGNATURES = {
     "dib_mi_sandwich_bounds": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_uint64, c_uint32, c_void_p, c_void_p, c_void_p]),
     "dib_mi_sandwich_bounds_batched": (c_int32, [c_void_p, c_int32, c_int64, c_int32, c_void_p, c_uint64, c_int32, c_void_p,
                                                  c_void_p, c_void_p]),
+    "dib_mi_bounds_at_probes": (c_int32, [c_void_p, c_int64, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_uint64,
+                                          c_void_p, c_void_p, c_void_p]),
+    "dib_mi_bounds_at_probes_scratch_bytes": (c_size_t, [c_int64, c_int64, c_int32, c_int32]),
     "dib_launch_count": (c_uint64, []),
     "dib_profile_enable": (c_int32, [c_void_p, c_int32]),
     "dib_profile_read": (c_int32, [c_void_p, c_char_p, c_size_t, POINTER(c_float), c_int32]),

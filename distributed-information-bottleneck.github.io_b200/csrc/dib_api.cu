@@ -1715,6 +1715,24 @@ int dib_mi_sandwich_bounds_batched(const float* mu_logvar, int32_t groups, int64
   return 0;
 }
 
+int dib_mi_bounds_at_probes(const float* probe_mu_logvar, int64_t m, const float* data_mu_logvar,
+                            const int64_t* batch_offsets, int32_t batches, int32_t embedding_dimension, const float* eps,
+                            uint64_t seed, void* scratch, double* out_lower_upper, void* stream) {
+  if (!probe_mu_logvar || !data_mu_logvar || !batch_offsets || !scratch || !out_lower_upper)
+    return fail("dib_mi_bounds_at_probes: null pointer");
+  if (m < 1 || m > 0x7fffffffll || batches < 1 || batches > 65535 || embedding_dimension < 1 || embedding_dimension > 128)
+    return fail("dib_mi_bounds_at_probes: bad arguments (1 <= m < 2^31, 1 <= batches <= 65535, 1 <= E <= 128)");
+  if (reinterpret_cast<uintptr_t>(scratch) % 256 != 0) return fail("dib_mi_bounds_at_probes: scratch must be 256-byte aligned");
+  DIB_CUDA_OK(dib_launch_mi_probes(probe_mu_logvar, m, data_mu_logvar, batch_offsets, batches, embedding_dimension, eps, seed,
+                                   scratch, out_lower_upper, static_cast<cudaStream_t>(stream)));
+  return 0;
+}
+
+size_t dib_mi_bounds_at_probes_scratch_bytes(int64_t m, int64_t data_rows, int32_t batches, int32_t embedding_dimension) {
+  if (m < 0 || data_rows < 0 || batches < 0 || embedding_dimension < 1) return 0;
+  return dib_mi_probes_scratch_bytes(m, data_rows, batches, embedding_dimension);
+}
+
 int dib_bhattacharyya(const float* mu_logvar, int64_t n, int32_t embedding_dimension, float* out_dist,
                       float* out_compression, void* stream) {
   if (!mu_logvar || n < 0 || embedding_dimension < 1) return fail("dib_bhattacharyya: bad arguments");

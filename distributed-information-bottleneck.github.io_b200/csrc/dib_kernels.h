@@ -266,3 +266,7 @@ cudaError_t dib_launch_mi_sandwich(const float* mu_logvar, int64_t n, int E, con
 // (seed << 8) + g / batches_per_feature at step g % batches_per_feature
 cudaError_t dib_launch_mi_sandwich_batched(const float* mu_logvar, int groups, int64_t n, int E, const float* eps, uint64_t seed,
                                            int batches_per_feature, double* row_scratch, double* out, cudaStream_t st);
+// per-probe bounds against B batches of data rows [offsets[b], offsets[b+1]) (dib_mi_probes.cu); 1 <= E <= 128, B <= 65535
+size_t dib_mi_probes_scratch_bytes(int64_t m, int64_t data_rows, int B, int E);
+cudaError_t dib_launch_mi_probes(const float* probes, int64_t m, const float* data, const int64_t* offsets, int B, int E,
+                                 const float* eps, uint64_t seed, void* scratch, double* out, cudaStream_t st);

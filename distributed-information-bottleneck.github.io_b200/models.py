@@ -9,6 +9,7 @@ unchanged with ``import dib_b200.models as models``.  PyTorch is used for device
 from __future__ import annotations
 
 import ctypes
+import gc
 import math
 import os
 from typing import Optional, Sequence
@@ -765,15 +766,23 @@ class DistributedIBNet:
                 keep = [t.clone() for t in (self._params, self._m, self._v, self._step_dev, self._noise_step_dev)]
                 graphs, run = [], []
                 launches0 = int(self._lib.dib_launch_count())
-                for k, (launch, exchange) in enumerate(phases):
-                    run.append(launch)
-                    if exchange is not None or k == len(phases) - 1:
-                        g = torch.cuda.CUDAGraph()
-                        with torch.cuda.graph(g):
-                            for fn in run:
-                                fn()
-                        graphs.append((g, exchange))
-                        run = []
+                # a garbage collection inside the capture could finalize a dead model, whose synchronize and dib_destroy
+                # would invalidate the capture
+                gc_on = gc.isenabled()
+                gc.disable()
+                try:
+                    for k, (launch, exchange) in enumerate(phases):
+                        run.append(launch)
+                        if exchange is not None or k == len(phases) - 1:
+                            g = torch.cuda.CUDAGraph()
+                            with torch.cuda.graph(g):
+                                for fn in run:
+                                    fn()
+                            graphs.append((g, exchange))
+                            run = []
+                finally:
+                    if gc_on:
+                        gc.enable()
                 torch.cuda.synchronize(self.device)
                 # capture does not execute, but be safe against any eager side effect: restore the optimizer state
                 for t, k in zip((self._params, self._m, self._v, self._step_dev, self._noise_step_dev), keep):
@@ -1285,6 +1294,49 @@ class InfoPerFeatureCallback(Callback):
                                                                seed=self.seed + epoch)
         for i in range(m.number_features):
             self.bounds.append([float(lo_up[i, 0]), float(lo_up[i, 1])])
+
+
+class ParticleInformationCallback(Callback):
+    """nb-particle's information plane and per-particle maps during ``fit`` of a SetTransformerIBNet.  Every
+    ``save_frequency`` epochs it appends ``utils.estimate_set_information`` ([lower, upper] nats per set, on
+    ``x_validation``: sets as the model takes them) to ``self.bounds``, and with ``probes`` [M, d] also
+    ``{epoch, beta, bounds [M, 2]}`` from ``utils.estimate_mi_bounds_at_probes(model.particle_encoder, probes, x_validation)``
+    to ``self.probe_bounds``, saved as ``probe_information_log10beta_{log10 beta:.3f}.npz`` under ``outdir`` when given.
+    The epoch's draws use ``seed + epoch``.  Neither estimate changes the training run."""
+
+    def __init__(self, save_frequency, x_validation, probes=None, evaluation_batch_size=32, number_evaluation_batches=16,
+                 probe_evaluation_batch_size=512, probe_number_evaluation_batches=16, outdir=None, seed=0):
+        super().__init__()
+        self.save_frequency = save_frequency
+        self.x_validation = x_validation
+        self.probes = probes
+        self.evaluation_batch_size, self.number_evaluation_batches = evaluation_batch_size, number_evaluation_batches
+        self.probe_evaluation_batch_size = probe_evaluation_batch_size
+        self.probe_number_evaluation_batches = probe_number_evaluation_batches
+        self.outdir = outdir
+        self.seed = seed
+        self.bounds = []
+        self.probe_bounds = []
+
+    def on_epoch_end(self, epoch, logs=None):
+        if (epoch % self.save_frequency) != 0:
+            return
+        from . import utils
+        m = self.model
+        lo_up = utils.estimate_set_information(m, self.x_validation, self.evaluation_batch_size, self.number_evaluation_batches,
+                                               seed=self.seed + epoch)
+        self.bounds.append([float(lo_up[0]), float(lo_up[1])])
+        if self.probes is None:
+            return
+        beta_value = float(m.beta.value())
+        rec = dict(epoch=epoch, beta=beta_value,
+                   bounds=utils.estimate_mi_bounds_at_probes(m.particle_encoder, self.probes, self.x_validation,
+                                                             self.probe_evaluation_batch_size,
+                                                             self.probe_number_evaluation_batches, seed=self.seed + epoch))
+        self.probe_bounds.append(rec)
+        if self.outdir:
+            os.makedirs(self.outdir, exist_ok=True)
+            np.savez(os.path.join(self.outdir, f'probe_information_log10beta_{np.log10(beta_value):.3f}.npz'), **rec)
 
 
 class SimpleEncoder:

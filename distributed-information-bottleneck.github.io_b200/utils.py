@@ -140,6 +140,171 @@ def estimate_mi_sandwich_bounds_all_features(model, x, evaluation_batch_size=102
     return out.view(F, nb, 2).mean(1).cpu().numpy()
 
 
+def mi_bounds_at_probes(probe_mu_logvar, data_mu_logvar, batch_offsets, eps=None, seed=0):
+    """nb-particle cell 8 (:549-570) on the GPU (dib_mi_bounds_at_probes): per-probe (InfoNCE lower, leave-one-out upper)
+    bounds in nats, float64 [M, 2], of probe encodings ``probe_mu_logvar`` [M, 2E] against the batches of encoded data
+    rows ``data_mu_logvar`` [R, 2E], batch b being rows ``batch_offsets[b] .. batch_offsets[b + 1]`` (B + 1 nondecreasing
+    int64 offsets, every batch at least one row).  ``eps`` [B, M, E] or None (Philox keyed by seed, batch and probe)."""
+    lib = _lib.load()
+    dev = data_mu_logvar.device
+    P = probe_mu_logvar.to(device=dev, dtype=torch.float32).contiguous()
+    D = data_mu_logvar.to(dtype=torch.float32).contiguous()
+    if P.dim() != 2 or D.dim() != 2 or P.shape[1] != D.shape[1] or P.shape[1] % 2:
+        raise ValueError(f"probe and data encodings must be [rows, 2E] of one E, got {tuple(P.shape)} and {tuple(D.shape)}")
+    M, R, E = P.shape[0], D.shape[0], P.shape[1] // 2
+    if not (isinstance(batch_offsets, torch.Tensor) and batch_offsets.is_cuda):
+        o = np.asarray(batch_offsets.cpu() if isinstance(batch_offsets, torch.Tensor) else batch_offsets, dtype=np.int64)
+        if o.ndim != 1 or o.size < 2 or o[0] < 0 or o[-1] > R or np.any(np.diff(o) < 1):
+            raise ValueError("batch_offsets must be B + 1 increasing offsets in [0, rows]: every batch needs a row")
+    off = torch.as_tensor(batch_offsets).to(device=dev, dtype=torch.int64).contiguous()
+    B = off.numel() - 1
+    e = None
+    if eps is not None:
+        e = _dev(eps, dev)
+        if tuple(e.shape) != (B, M, E):
+            raise ValueError(f"eps has shape {tuple(e.shape)}; expected {(B, M, E)}")
+    scratch = torch.empty(int(lib.dib_mi_bounds_at_probes_scratch_bytes(M, R, B, E)), dtype=torch.uint8, device=dev)
+    out = torch.empty(M, 2, dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.dib_mi_bounds_at_probes(_lib.ptr(P), M, _lib.ptr(D), _lib.ptr(off), B, E, _lib.ptr(e), int(seed),
+                                               _lib.ptr(scratch), _lib.ptr(out),
+                                               ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
+    return out
+
+
+def draw_evaluation_batches(number_items, evaluation_batch_size, number_evaluation_batches, seed, device):
+    """The evaluation draws of :func:`estimate_mi_bounds_at_probes` and :func:`estimate_set_information`: a
+    ``torch.Generator(device)`` seeded with ``seed``, then for b = 0, 1, ... in order
+    ``torch.randint(0, number_items, (evaluation_batch_size,), generator=gen, device=device)``.  Returns [B, bs] int64."""
+    gen = torch.Generator(device=device)
+    gen.manual_seed(int(seed))
+    return torch.stack([torch.randint(0, int(number_items), (int(evaluation_batch_size),), generator=gen, device=device)
+                        for _ in range(int(number_evaluation_batches))])
+
+
+def set_batch_rows(set_index, set_sizes, set_length):
+    """Particle rows of drawn sets: ``set_index`` [B, bs] set numbers, ``set_sizes`` [N] real particles per set (None: all
+    ``set_length``).  Returns (rows, offsets): the indices into the [N * set_length] particle rows of every real particle,
+    batch by batch, set by set, particle by particle, and the B + 1 batch offsets into ``rows``.  Works on any device."""
+    L = int(set_length)
+    idx = set_index.to(torch.int64)
+    ar = torch.arange(L, device=idx.device)
+    if set_sizes is None:
+        sz = torch.full_like(idx, L)
+    else:
+        sz = torch.as_tensor(set_sizes).to(device=idx.device, dtype=torch.int64)[idx]
+    rows = (idx[..., None] * L + ar)[ar < sz[..., None]]
+    offsets = torch.cat([torch.zeros(1, dtype=torch.int64, device=idx.device), torch.cumsum(sz.sum(1), 0)])
+    return rows, offsets
+
+
+def _particle_sets(model, dataset):
+    """Sets for a SetTransformerIBNet: [N, L, d] (a fixed-size model also takes an (x, y) pair), or for a variable-size
+    model a list of [l_i, d] or a pair (x_padded, set_sizes).  Returns (particle rows [N * L, d] on the device, set count
+    N, int64 device sizes or None)."""
+    from .models import pad_sets
+    L, d = model.number_particles, model.particle_feature_dimensions
+    sizes = None
+    if model.variable_set_sizes and isinstance(dataset, list):
+        dataset = pad_sets(dataset, L)
+    if isinstance(dataset, tuple):
+        if model.variable_set_sizes:
+            dataset, sizes = dataset
+        else:
+            dataset = dataset[0]
+    N = dataset.shape[0]
+    x = model._to_device(dataset, L * d).reshape(N * L, d)
+    if sizes is not None:
+        sizes = model._device_sizes(sizes, N).to(torch.int64)
+    return x, N, sizes
+
+
+def _encode_within_handle(model, i, rows):
+    """Encoder i (no noise, logvar offset applied) on ``rows`` in chunks that fit the model's handle, so that encoding
+    never re-creates it (that would re-allocate the training workspace and drop the captured CUDA graphs); a model without
+    a handle gets the smallest one."""
+    if model._handle is None:
+        model._ensure_handle(1)
+    per = model._max_batch * getattr(model, "number_particles", 1)
+    out = torch.empty(rows.shape[0], 2 * model.feature_embedding_dimension, dtype=torch.float32, device=model.device)
+    for a in range(0, rows.shape[0], per):
+        out[a:a + per] = model._encode_feature(i, rows[a:a + per])
+    return out
+
+
+def estimate_mi_bounds_at_probes(encoder, probes, dataset, evaluation_batch_size=512, number_evaluation_batches=16, seed=0):
+    """Per-probe information map (nb-particle cell 8, :521-570): for every probe input, the InfoNCE lower and the
+    leave-one-out upper bound (nats) of the information its encoding carries, against ``number_evaluation_batches``
+    batches of data.  Returns float64 [M, 2] (lower, upper); the notebook plots mean(lower, upper) / ln 2.
+
+    ``encoder`` is ``model.particle_encoder`` of a SetTransformerIBNet -- ``probes`` [M, d] particle rows, ``dataset`` sets
+    ([N, L, d]; for a variable-size model also a list of [l_i, d] or a pair (x_padded, set_sizes)); a batch draws
+    ``evaluation_batch_size`` sets and holds all their real particles, padding rows never enter -- or
+    ``model.feature_encoders[i]`` -- ``probes`` [M, d_i], ``dataset`` rows [N, d_i] (an (x, y) pair: x); a batch draws
+    ``evaluation_batch_size`` rows.  Draws: :func:`draw_evaluation_batches` (``seed``) over the sets or rows, then for sets
+    :func:`set_batch_rows`.  Probes and data rows are encoded without noise (logvar offset included) within the model's
+    current handle; training state (handle, graphs, step counters, noise streams) is left as it was.  The sample noise is
+    Philox keyed (seed, batch, probe), so a probe's result does not depend on the other probes.
+
+    The notebook draws fresh batches for every chunk of 100 probes; here the batches are drawn once and every probe is
+    scored against them.  Each probe's estimator has the same distribution either way, only the correlation between
+    probes changes, and the data rows are encoded once instead of once per chunk."""
+    from .models import _ParticleEncoder
+    model = encoder._model
+    dev = model.device
+    bs, nb = int(evaluation_batch_size), int(number_evaluation_batches)
+    if isinstance(encoder, _ParticleEncoder):
+        x, N, sizes = _particle_sets(model, dataset)
+        rows, off = set_batch_rows(draw_evaluation_batches(N, bs, nb, seed, dev), sizes, model.number_particles)
+        d = model.particle_feature_dimensions
+    else:
+        if isinstance(dataset, (tuple, list)):
+            dataset = dataset[0]
+        d = model.feature_dimensionalities[encoder.index]
+        x = _dev(dataset, dev).reshape(-1, d)
+        rows = draw_evaluation_batches(x.shape[0], bs, nb, seed, dev).reshape(-1)
+        off = torch.arange(nb + 1, dtype=torch.int64, device=dev) * bs
+    p = _dev(probes, dev).reshape(-1, d)
+    data = _encode_within_handle(model, encoder.index, x.index_select(0, rows))
+    ml_probes = _encode_within_handle(model, encoder.index, p)
+    return mi_bounds_at_probes(ml_probes, data, off, None, seed).cpu().numpy()
+
+
+def estimate_set_information(model, x, evaluation_batch_size=32, number_evaluation_batches=16, seed=0):
+    """nb-particle's ``info_bounds`` (:502-517), the x-axis of its information plane: [lower, upper] in nats per set of a
+    SetTransformerIBNet.  Sets are drawn with :func:`draw_evaluation_batches` (``seed``); the batch bounds of all the real
+    particles of a batch come from dib_mi_sandwich_bounds_batched (float64, E <= 64) and are multiplied by the particles
+    per set: number_particles, or for variable sizes the batch's mean drawn size.  Fixed sizes: one launch, batch b on the
+    noise stream (seed << 8) at step b; variable sizes: one launch per batch, on stream ((seed << 16) + b) << 8."""
+    lib = _lib.load()
+    xr, N, sizes = _particle_sets(model, x)
+    L, E = model.number_particles, model.feature_embedding_dimension
+    bs, nb = int(evaluation_batch_size), int(number_evaluation_batches)
+    rows, off = set_batch_rows(draw_evaluation_batches(N, bs, nb, seed, model.device), sizes, L)
+    ml = _encode_within_handle(model, 0, xr.index_select(0, rows))
+    stream = ctypes.c_void_p(torch.cuda.current_stream(model.device).cuda_stream)
+    with torch.cuda.device(model.device):
+        if sizes is None:
+            n = bs * L
+            scratch = torch.empty(nb * n * 2, dtype=torch.float64, device=model.device)
+            out = torch.empty(nb, 2, dtype=torch.float64, device=model.device)
+            _lib.check(lib.dib_mi_sandwich_bounds_batched(_lib.ptr(ml), nb, n, E, None, int(seed), nb, _lib.ptr(scratch),
+                                                          _lib.ptr(out), stream))
+            per_set = out * L
+        else:
+            oh = off.cpu().tolist()
+            per_set = torch.empty(nb, 2, dtype=torch.float64, device=model.device)
+            scratch = torch.empty(2 * max(b1 - b0 for b0, b1 in zip(oh[:-1], oh[1:])), dtype=torch.float64,
+                                  device=model.device)
+            for b in range(nb):
+                n = oh[b + 1] - oh[b]
+                _lib.check(lib.dib_mi_sandwich_bounds_batched(_lib.ptr(ml[oh[b]:oh[b + 1]]), 1, n, E, None,
+                                                              (int(seed) << 16) + b, 1, _lib.ptr(scratch),
+                                                              _lib.ptr(per_set[b]), stream))
+                per_set[b] *= n / bs
+    return per_set.mean(0).cpu().numpy()
+
+
 SIMILARITY_TYPES = {"l2sq": 0, "l2": 1, "l1": 2, "linf": 3, "cosine": 4}
 
 

@@ -355,6 +355,21 @@ int dib_mi_sandwich_bounds_batched(const float* mu_logvar, int32_t groups, int64
                                    const float* eps, uint64_t seed, int32_t batches_per_feature, double* row_scratch,
                                    double* out_lower_upper, void* stream);
 
+/* nb-particle cell 8 (:521-570): per-probe InfoNCE lower / leave-one-out upper bounds (nats), float64, of m probe encodings
+ * against `batches` batches of encoded data rows, in one launch of the main kernel.  probe_mu_logvar [m, 2E] and
+ * data_mu_logvar [data_rows, 2E] are (mu || logvar) rows (dib_encode_feature output); batch b is rows
+ * [batch_offsets[b], batch_offsets[b+1]) with batch_offsets a nondecreasing DEVICE int64 array of batches + 1 entries in
+ * [0, data_rows], every batch at least one row.  For probe p and batch b, u = mu_p + exp(lv_p / 2) eps_pb and
+ *   lower_pb = log p(u|x_p) - log( (p(u|x_p) + sum_j p(u|x_j)) / (N_b + 1) ),  upper_pb = log p(u|x_p) - log( sum_j p(u|x_j) / N_b )
+ * evaluated in log space (finite where the linear-space upper bound underflows to log(x/0)); out [m, 2] = the means over b.
+ * eps [batches, m, E] or NULL -> Philox keyed (seed, step b, row p, feature 0, dim), so a probe's result does not depend on
+ * m.  scratch: dib_mi_bounds_at_probes_scratch_bytes(m, data_rows, batches, E), 256-byte aligned.  1 <= E <= 128,
+ * 1 <= batches <= 65535, m < 2^31.  Deterministic: no atomics, repeated calls are bit-identical. */
+int dib_mi_bounds_at_probes(const float* probe_mu_logvar, int64_t m, const float* data_mu_logvar,
+                            const int64_t* batch_offsets, int32_t batches, int32_t embedding_dimension, const float* eps,
+                            uint64_t seed, void* scratch, double* out_lower_upper, void* stream);
+size_t dib_mi_bounds_at_probes_scratch_bytes(int64_t m, int64_t data_rows, int32_t batches, int32_t embedding_dimension);
+
 /* NEXT ROW f4 -- ctw.estimate_entropy(seq, alphabet_size) (chaos/ctw.pyx:2-3 -> chaos/cppctw.cpp:163-171): infinite-depth
  * Context-Tree-Weighting entropy-rate estimate in bits/symbol.  HOST functions on HOST memory (the suffix-tree build is
  * irregular pointer chasing; SURVEY 8f keeps it on the CPU): symbols are int8 in [0, alphabet_size), alphabet_size <= 127.
