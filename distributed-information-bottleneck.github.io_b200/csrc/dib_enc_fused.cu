@@ -116,12 +116,6 @@ __device__ __forceinline__ uint32_t ld_shared_b32(uint32_t addr) {
   return v;
 }
 
-// address of the 16-byte chunk holding columns [8c, 8c+8) of row r in a [128 x 64k] swizzled tile
-__device__ __forceinline__ uint32_t tile_chunk_addr(uint32_t tile, int r, int col) {
-  const int panel = col >> 6, c = (col & 63) >> 3;
-  return tile + panel * kPanel + r * 128 + ((c ^ (r & 7)) << 4);
-}
-
 // Position of this thread's accumulator elements in the tile: rows rb and rb + 8, columns 8 j + 2 q (+1).
 struct Frag {
   int rb, q;
@@ -131,23 +125,29 @@ __device__ __forceinline__ Frag frag_of(int tid) {
   return Frag{64 * wg + 16 * wq + (lane >> 2), lane & 3};
 }
 
-// accumulator of a 64 x N tile -> activation -> 16-bit -> the swizzled shared tile (the next MMA's A operand).  The bias is
-// already in the accumulator.  Each quad of lanes writes one 16-byte chunk of a row: conflict-free under the swizzle.
-template <bool BF16, bool RELU, int N>
-__device__ __forceinline__ void frag_to_tile(const float (&d)[N / 2], uint32_t tile, Frag fr, int act, float alpha) {
-#pragma unroll
-  for (int j = 0; j < N / 8; ++j) {
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const float v0 = d[4 * j + 2 * h], v1 = d[4 * j + 2 * h + 1];
-      const uint32_t w = RELU ? pack2_relu<BF16>(v0, v1) : pack2<BF16>(dib_act16(act, v0, alpha), dib_act16(act, v1, alpha));
-      st_shared_b32(tile_chunk_addr(tile, fr.rb + 8 * h, 8 * j) + 4 * fr.q, w);
-    }
-  }
+// v, as a value the compiler cannot precompute.  The backward kernel runs at the 255-register limit; addresses and operand
+// descriptors derived from such a value are formed where they are used instead of being kept in registers across the tile.
+__device__ __forceinline__ uint32_t opaque(uint32_t v) {
+  asm volatile("" : "+r"(v));
+  return v;
 }
 
-// the same activation, kept in registers as the next MMA's A operand: the accumulator fragment of 8-column block j is the
-// A fragment half i = j % 2 of k step j / 2, so a[4 kk .. 4 kk + 3] is the A operand of k step kk (see wgmma_m64n128k16_rs)
+// Shared-memory places of a thread's accumulator words in a [128 x 64k] swizzled tile (16-byte chunk index XORed with
+// row % 8): word 2 j + h (columns 8 j + 2 q (+1), row rb + 8 h) is at fw.base + (j / 8) * kPanel + h * 1024 +
+// ((j % 8) * 16 ^ fw.sw).  The j-th offset is one LOP3 from fw.sw rather than one of eight registers held through the tile.
+struct FragWords {
+  uint32_t base, sw;
+};
+__device__ __forceinline__ FragWords frag_words(uint32_t tile, Frag fr) {
+  return FragWords{opaque(tile + fr.rb * 128 + 4 * fr.q), opaque((fr.rb & 7) << 4)};
+}
+__device__ __forceinline__ uint32_t frag_word_addr(FragWords fw, int j, int h) {
+  return fw.base + (j >> 3) * kPanel + h * 1024 + (((j & 7) << 4) ^ fw.sw);
+}
+
+// accumulator of a 64 x N tile -> activation -> 16-bit, kept in registers as the next MMA's A operand (the bias is already
+// in the accumulator): the accumulator fragment of 8-column block j is the A fragment half i = j % 2 of k step j / 2, so
+// a[4 kk .. 4 kk + 3] is the A operand of k step kk (see wgmma_m64n128k16_rs)
 template <bool BF16, bool RELU, int N>
 __device__ __forceinline__ void frag_to_a(const float (&d)[N / 2], uint32_t (&a)[N / 4], int act, float alpha) {
 #pragma unroll
@@ -157,6 +157,19 @@ __device__ __forceinline__ void frag_to_a(const float (&d)[N / 2], uint32_t (&a)
       const float v0 = d[4 * j + 2 * h], v1 = d[4 * j + 2 * h + 1];
       a[2 * j + h] = RELU ? pack2_relu<BF16>(v0, v1) : pack2<BF16>(dib_act16(act, v0, alpha), dib_act16(act, v1, alpha));
     }
+  }
+}
+
+// the packed words of such a fragment -> this thread's places in the swizzled shared tile of the warpgroup's 64 x N rows
+// (the backward's weight-gradient operands and act').  Each quad of lanes writes one 16-byte chunk of a row: conflict-free
+// under the swizzle.
+template <int N>
+__device__ __forceinline__ void a_to_tile(const uint32_t (&a)[N / 4], uint32_t tile, Frag fr) {
+  const FragWords fw = frag_words(tile, fr);
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) st_shared_b32(frag_word_addr(fw, j, h), a[2 * j + h]);
   }
 }
 
@@ -174,27 +187,26 @@ __device__ __forceinline__ uint32_t relu_gate2(uint32_t p, uint32_t h) {
   }
 }
 
-// gradient accumulator (64 x 128) * act'(h) -> 16-bit -> shared tile `dtile`; h is read back from the shared tile `htile`
-// that the recomputed forward wrote (relu: as a packed comparison, other activations through act'(h)).  dtile may be htile.
+// gradient accumulator (64 x 128) * act'(h) -> 16-bit, packed as the next dgrad MMA's A fragment (layout of frag_to_a); h
+// is read back from this thread's own words of the shared tile `htile` that the recomputed forward wrote (relu: as a packed
+// comparison, other activations through act'(h)).  a_to_tile stores the result for the weight gradients.
 template <bool BF16, bool RELU>
-__device__ __forceinline__ void frag_dgrad_to_tile(const float (&d)[64], uint32_t htile, uint32_t dtile, Frag fr, int act,
-                                                   float alpha) {
+__device__ __forceinline__ void frag_dgrad_to_a(const float (&d)[64], uint32_t htile, uint32_t (&a)[32], Frag fr, int act,
+                                                float alpha) {
+  const FragWords fw = frag_words(htile, fr);
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const uint32_t off = tile_chunk_addr(0u, fr.rb + 8 * h, 8 * j) + 4 * fr.q;
-      const uint32_t hv = ld_shared_b32(htile + off);
+      const uint32_t hv = ld_shared_b32(frag_word_addr(fw, j, h));
       const float g0 = d[4 * j + 2 * h], g1 = d[4 * j + 2 * h + 1];
-      uint32_t o;
       if constexpr (RELU) {
-        o = relu_gate2<BF16>(pack2<BF16>(g0, g1), hv);
+        a[2 * j + h] = relu_gate2<BF16>(pack2<BF16>(g0, g1), hv);
       } else {
         float h0, h1;
         unpack2<BF16>(hv, h0, h1);
-        o = pack2<BF16>(g0 * dib_act_grad(act, h0, alpha), g1 * dib_act_grad(act, h1, alpha));
+        a[2 * j + h] = pack2<BF16>(g0 * dib_act_grad(act, h0, alpha), g1 * dib_act_grad(act, h1, alpha));
       }
-      st_shared_b32(dtile + off, o);
     }
   }
 }
@@ -317,7 +329,7 @@ __device__ __forceinline__ void load_weights(uint32_t sb, const WeightMaps& m, u
 __device__ __forceinline__ uint64_t desc_a0_as_a(uint32_t a0, int wg) { return gmma_desc(a0 + wg * 64 * 16, TM * 16, 128, kLayoutNone); }
 // [pe|1] as B over 16 samples from sample 16 kk (MN-major, no swizzle): 8 columns per k-half plane, 8 samples per 128 B
 __device__ __forceinline__ uint64_t desc_a0_as_b(uint32_t a0, int kk) { return gmma_desc(a0 + kk * 256, 128, TM * 16, kLayoutNone); }
-// activation tile as A (K-major): k step kk of 16 features
+// activation tile as A (K-major): k step kk of 16 features of the warpgroup's rows
 __device__ __forceinline__ uint64_t desc_act_as_a(uint32_t tile, int wg, int kk) {
   return gmma_desc(tile + (kk >> 2) * kPanel + wg * 64 * 128 + (kk & 3) * 32, 16, 1024);
 }
@@ -331,21 +343,7 @@ template <bool BF16>
 __device__ __forceinline__ void mma_layer0(float (&d)[64], uint32_t sb, uint32_t a0, int wg) {
   wgmma_m64n128k16<BF16, 0, 1>(d, desc_a0_as_a(a0, wg), gmma_desc(sb + kOffW0, K0 * 128, 1024), 0u);
 }
-template <bool BF16>
-__device__ __forceinline__ void mma_layer1(float (&d)[64], uint32_t sb, uint32_t h1, uint32_t a0, int wg) {
-  wgmma_m64n128k16<BF16, 0, 1>(d, desc_a0_as_a(a0, wg), gmma_desc(sb + kOffBb1, K0 * 128, 1024), 0u);
-#pragma unroll
-  for (int kk = 0; kk < HID / 16; ++kk)
-    wgmma_m64n128k16<BF16, 0, 1>(d, desc_act_as_a(h1, wg, kk), gmma_desc(sb + kOffW1 + kk * 2048, kPanel, 1024), 1u);
-}
-template <bool BF16>
-__device__ __forceinline__ void mma_layer2(float (&d)[32], uint32_t sb, uint32_t h2, uint32_t a0, int wg) {
-  wgmma_m64n64k16<BF16, 0, 1>(d, desc_a0_as_a(a0, wg), gmma_desc(sb + kOffBb2, K0 * 128, 1024), 0u);
-#pragma unroll
-  for (int kk = 0; kk < HID / 16; ++kk)
-    wgmma_m64n64k16<BF16, 0, 1>(d, desc_act_as_a(h2, wg, kk), gmma_desc(sb + kOffW2 + kk * 2048, kPanel, 1024), 1u);
-}
-// the same with h1 / h2 as register A operands (frag_to_a); same operands, same k order into the accumulator
+// layers 1 and 2 take h1 / h2 as register A operands (frag_to_a); only their bias-carrier step reads [pe|1] from shared memory
 template <bool BF16>
 __device__ __forceinline__ void mma_layer1_rs(float (&d)[64], uint32_t sb, const uint32_t (&h1)[32], uint32_t a0, int wg) {
   wgmma_m64n128k16<BF16, 0, 1>(d, desc_a0_as_a(a0, wg), gmma_desc(sb + kOffBb1, K0 * 128, 1024), 0u);
@@ -370,11 +368,17 @@ __device__ __forceinline__ void wg_publish(int wg) {
   fence_proxy_async_smem();
   named_bar_sync(1 + wg, 128);
 }
-// ... to the MMAs of both warpgroups
-__device__ __forceinline__ void cta_publish() {
+// Split-phase hand-off between the backward's two warpgroups: xwg_arrive(e, wg) signals this warpgroup's side of event e
+// and does not wait; xwg_wait(e, wg) blocks until the other warpgroup has signalled e.  Named barrier e + g carries
+// warpgroup g's signal (128 arriving + 128 waiting threads).  Every event is signalled and waited once per tile, and a
+// warpgroup cannot signal an event again before the other has waited for it (each tile ends in a two-sided wait).  The
+// fence makes this warpgroup's shared-memory stores visible to the other warpgroup's MMAs.
+constexpr uint32_t kEvL0 = 3, kEvDO = 5, kEvDZ2 = 7, kEvDW2 = 9, kEvDZ1 = 11;   // 1, 2: wg_publish
+__device__ __forceinline__ void xwg_arrive(uint32_t e, int wg) {
   fence_proxy_async_smem();
-  __syncthreads();
+  named_bar_arrive(e + wg, 256);
 }
+__device__ __forceinline__ void xwg_wait(uint32_t e, int wg) { named_bar_sync(e + (wg ^ 1), 256); }
 
 // feature / tile assignment of a persistent CTA: with at least as many CTAs as features, CTA c serves feature c % F and
 // its tiles slot, slot + nslots, ...; otherwise it walks features c, c + G, ... with all of their tiles
@@ -501,12 +505,16 @@ dib_enc_fused_fwd_kernel(const __grid_constant__ WeightMaps maps, const EncFused
 // warpgroup g owns rows [64 g, 64 g + 64) of dW1, dW2 (and of dW0^T, db1); warpgroup 0 stores db2.  190 KB of shared
 // memory: one CTA per SM.
 //
-// The tensor pipe is kept busy across the epilogues of the serial chain:
-//   * in each backward layer the dgrad MMAs and the weight-gradient MMAs are two commit groups; the dz epilogue waits only
-//     for the first, and the wait for the second sits just before the CTA barrier that follows (dz1 is written over h2,
-//     which the other warpgroup's dW2 reads; that wait keeps the write behind every dW2 of the tile);
-//   * dW0 of tile t retires under the start of tile t + 1: [pe|1] is double-buffered, and the barrier after the layer-0
-//     epilogue is a CTA barrier, so both warpgroups' dW0 (retired by their layer-0 wait) are done before h2 is rewritten;
+// The chain of a warpgroup's rows waits for nothing but its own MMAs (and its own warpgroup):
+//   * every MMA that reduces over features (recomputed L1, L2; dgrad G2, G1) reads only the warpgroup's rows.  L1, L2 and
+//     G2 take them as register A fragments (h1, h2, dO packed once); the same words are stored to the shared tiles, where
+//     only the weight-gradient MMAs (and act') read them.  G1 reads dz2 from its tile (registers are short there);
+//   * only the weight-gradient MMAs read the other warpgroup's rows, so they are the only MMAs behind a wait for the other
+//     warpgroup.  That wait is split-phase (xwg_arrive / xwg_wait): a warpgroup signals once its rows are stored, issues its
+//     dgrad MMAs, and only then waits;
+//   * in each backward layer the dgrad MMAs and the weight-gradient MMAs are separate commit groups; the dz epilogue waits
+//     only for the dgrad, so the weight-gradient MMAs run under it;
+//   * dW0 of tile t retires under the start of tile t + 1 ([pe|1] is double-buffered);
 //   * x (prefetch_x) and the 16-bit gradient d_emb16 (TMA, one 8 KB buffer) of the next tile are loaded a tile ahead.
 // ====================================================================================================
 struct EncFusedBwdParams {
@@ -542,7 +550,6 @@ dib_enc_fused_bwd_kernel(const __grid_constant__ WeightMaps maps, const __grid_c
   const uint32_t h1 = sb + kOffH1, h2 = sb + kOffH2, dO = sb + kOffDO, dz2 = sb + kOffDZ2, gbuf = sb + kOffG;
   const uint32_t xs = sb + kOffX + tid * 16;
   const float* xslot = reinterpret_cast<const float*>(sg + kOffX + tid * 16);
-  const uint32_t* gsm = reinterpret_cast<const uint32_t*>(sg + kOffG);    // [128 rows][16 pairs] d_emb16 of this tile
   const float S = Q.gscale, invS = 1.f / Q.gscale;
 
   if (tid == 0) {
@@ -584,18 +591,27 @@ dib_enc_fused_bwd_kernel(const __grid_constant__ WeightMaps maps, const __grid_c
       wgmma_commit();
       wgmma_wait<0>();                     // also retires this warpgroup's dW0 of the previous tile
       wgmma_fence_regs(acc); wgmma_fence_regs(accW0);
-      frag_to_tile<BF16, RELU, 128>(acc, h1, fr, P.act, P.alpha);
-      cta_publish();                       // h1; and both warpgroups' dW0 of the previous tile (it read all of h2) are done
+      xwg_arrive(kEvL0, wg);               // this warpgroup's dW0 of the previous tile (it read all of h2) is done
+      uint32_t ha[32];
+      frag_to_a<BF16, RELU, 128>(acc, ha, P.act, P.alpha);
+      // h1 for dW1 and act'(h1).  The previous tile's dW1 of both warpgroups retired before its kEvDZ1 hand-off.
+      a_to_tile<128>(ha, h1, fr);
+      // (each MMA chain that starts with scale-d = 0 gets a fresh accumulator: then the values that the previous epilogue
+      // consumed are not kept live up to the next MMA's issue, next to its register A fragment)
+      float acc1[64];
       wgmma_fence();
-      mma_layer1<BF16>(acc, sb, h1, a0, wg);
+      mma_layer1_rs<BF16>(acc1, sb, ha, a0, wg);
       wgmma_commit();
       wgmma_wait<0>();
-      wgmma_fence_regs(acc);
-      frag_to_tile<BF16, RELU, 128>(acc, h2, fr, P.act, P.alpha);
-      wg_publish(wg);
+      wgmma_fence_regs(acc1);
+      frag_to_a<BF16, RELU, 128>(acc1, ha, P.act, P.alpha);              // h2 over h1
+      // h2 for dW2 and act'(h2), over the previous tile's dz1: behind both warpgroups' dW0 of the previous tile.  (The
+      // stores come before the MMA: the A registers of an MMA in flight are not read.)
+      xwg_wait(kEvL0, wg);
+      a_to_tile<128>(ha, h2, fr);
       float acc2[32];
       wgmma_fence();
-      mma_layer2<BF16>(acc2, sb, h2, a0, wg);
+      mma_layer2_rs<BF16>(acc2, sb, ha, a0, wg);
       wgmma_commit();
       const long long grow_lo = row0 + fr.rb;
       float nz[4][2][2];
@@ -604,7 +620,9 @@ dib_enc_fused_bwd_kernel(const __grid_constant__ WeightMaps maps, const __grid_c
       if (Q.d_emb16) mbar_wait(bar_g, tpar);
       wgmma_wait<0>();
       wgmma_fence_regs(acc2);
-      // ---- (mu, logvar) -> d(mu), d(logvar) -> dO tile.  Rows past the batch end contribute nothing.
+      // ---- (mu, logvar) -> d(mu), d(logvar) = dO, packed as the A fragment of G2 (column e of dO is word 2 (e / 8) + h of
+      // the fragment, 32 + e is 8 + 2 (e / 8) + h).  Rows past the batch end contribute nothing.
+      uint32_t ao[16];
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const long long grow = grow_lo + 8 * h;
@@ -616,7 +634,7 @@ dib_enc_fused_bwd_kernel(const __grid_constant__ WeightMaps maps, const __grid_c
           const int e = 8 * j + 2 * fr.q;
           float g[2] = {0.f, 0.f};
           if (valid) {
-            if (Q.d_emb16) unpack2<BF16>(gsm[r * 16 + e / 2], g[0], g[1]);
+            if (Q.d_emb16) unpack2<BF16>(ld_shared_b32(gbuf + 4 * (r * 16 + e / 2)), g[0], g[1]);   // [128 rows][16 pairs]
             else {
               const float2 g2 = *reinterpret_cast<const float2*>(Q.d_emb + grow * Q.ldd + f * 32 + e);
               g[0] = g2.x * S; g[1] = g2.y * S;
@@ -630,60 +648,90 @@ dib_enc_fused_bwd_kernel(const __grid_constant__ WeightMaps maps, const __grid_c
             dm[k] = fmaf(bsv, mu, g[k]);
             dl[k] = valid ? fmaf(g[k] * nz[j][h][k], 0.5f * sgm, bsv * 0.5f * (sgm * sgm - 1.f)) : 0.f;
           }
-          st_shared_b32(tile_chunk_addr(dO, r, e) + 4 * fr.q, pack2<BF16>(dm[0], dm[1]));
-          st_shared_b32(tile_chunk_addr(dO, r, 32 + e) + 4 * fr.q, pack2<BF16>(dl[0], dl[1]));
+          ao[2 * j + h] = pack2<BF16>(dm[0], dm[1]);
+          ao[8 + 2 * j + h] = pack2<BF16>(dl[0], dl[1]);
         }
       }
-      cta_publish();                       // dO, h2, h1, [pe|1] of all 128 rows; the d_emb16 buffer has been read
-      if (tid == 0 && Q.d_emb16 && t + s.nslots < ntiles) load_demb16(gbuf, &gmap, bar_g, f, row0 + (long long)s.nslots * TM);
-      // ---- layer 2 backward: G2 = dO W2^T (own rows) | dW2 += h2^T dO; db2 += dO^T [pe|1]
+      // dO for dW2 / db2.  The previous tile's dW2 / db2 of both warpgroups retired before its kEvDZ1 hand-off.
+      a_to_tile<64>(ao, dO, fr);
+      xwg_arrive(kEvDO, wg);               // this warpgroup's rows of h1, h2, dO, [pe|1] are stored; its d_emb16 rows read
+      // ---- layer 2 backward: G2 = dO W2^T (own rows, A from registers) | dW2 += h2^T dO; db2 += dO^T [pe|1]
+      float accd[64];
       wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < EO / 16; ++kk)
-        wgmma_m64n128k16<BF16, 0, 0>(acc, gmma_desc(dO + wg * 64 * 128 + kk * 32, 16, 1024),
-                                     gmma_desc(sb + kOffW2 + kk * 32, 16, 1024), kk > 0 ? 1u : 0u);
+      for (int kk = 0; kk < EO / 16; ++kk) {
+        const uint32_t a[4] = {ao[4 * kk], ao[4 * kk + 1], ao[4 * kk + 2], ao[4 * kk + 3]};
+        wgmma_m64n128k16_rs<BF16, 0>(accd, a, gmma_desc(sb + kOffW2 + kk * 32, 16, 1024), kk > 0 ? 1u : 0u);
+      }
       wgmma_commit();
+      xwg_wait(kEvDO, wg);                 // dW2 / db2 read both warpgroups' rows of h2, dO and [pe|1]
+      if (tid == 0 && Q.d_emb16 && t + s.nslots < ntiles) load_demb16(gbuf, &gmap, bar_g, f, row0 + (long long)s.nslots * TM);
+      {
+        const uint32_t h2o = opaque(h2), dOo = opaque(dO), a0o = opaque(a0);
+        wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < TM / 16; ++kk)
-        wgmma_m64n64k16<BF16, 1, 1>(accW2, desc_act_t_as_a(h2, wg, kk), desc_act_as_b(dO, kk), kk > 0 ? 1u : wacc);
-      // (both warpgroups run the small db2 contraction -- uniform issue keeps the MMAs unserialised; warpgroup 0 stores it)
+        for (int kk = 0; kk < TM / 16; ++kk)
+          wgmma_m64n64k16<BF16, 1, 1>(accW2, desc_act_t_as_a(h2o, wg, kk), desc_act_as_b(dOo, kk), kk > 0 ? 1u : wacc);
+        // (both warpgroups run the small db2 contraction -- uniform issue keeps the MMAs unserialised; warpgroup 0 stores it)
 #pragma unroll
-      for (int kk = 0; kk < TM / 16; ++kk)
-        wgmma_m64n16k16<BF16, 1, 1>(accB2, desc_act_t_as_a(dO, 0, kk), desc_a0_as_b(a0, kk), kk > 0 ? 1u : wacc);
+        for (int kk = 0; kk < TM / 16; ++kk)
+          wgmma_m64n16k16<BF16, 1, 1>(accB2, desc_act_t_as_a(dOo, 0, kk), desc_a0_as_b(a0o, kk), kk > 0 ? 1u : wacc);
+      }
       wgmma_commit();
       wgmma_wait<1>();
-      wgmma_fence_regs(acc);
-      // ---- dz2 = G2 * act'(h2), while dW2 / db2 run
-      frag_dgrad_to_tile<BF16, RELU>(acc, h2, dz2, fr, P.act, P.alpha);
-      wgmma_wait<0>();
-      wgmma_fence_regs(accW2); wgmma_fence_regs(accB2);
-      cta_publish();
+      wgmma_fence_regs(accd);
+      // ---- dz2 = G2 * act'(h2), while dW2 / db2 run -> the dz2 tile (the previous tile's dW1 / db1 of both warpgroups
+      // retired before its kEvDZ1 hand-off)
+      {
+        uint32_t az[32];
+        frag_dgrad_to_a<BF16, RELU>(accd, h2, az, fr, P.act, P.alpha);
+        a_to_tile<128>(az, dz2, fr);
+      }
+      xwg_arrive(kEvDZ2, wg);
       // ---- layer 1 backward: G1 = dz2 W1^T (own rows) | dW1 += h1^T dz2; db1 += dz2^T [pe|1]
+      // G1 reads dz2 from the tile, behind a barrier of this warpgroup only.  As a register A fragment it would hold 32
+      // registers through the issue of dW1 / db1, next to G1's accumulator and the weight gradients: more than 255.
+      float accg[64];
+      wg_publish(wg);
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < HID / 16; ++kk)
-        wgmma_m64n128k16<BF16, 0, 0>(acc, desc_act_as_a(dz2, wg, kk),
+        wgmma_m64n128k16<BF16, 0, 0>(accg, desc_act_as_a(dz2, wg, kk),
                                      gmma_desc(sb + kOffW1 + (kk >> 2) * kPanel + (kk & 3) * 32, 16, 1024), kk > 0 ? 1u : 0u);
       wgmma_commit();
+      xwg_wait(kEvDZ2, wg);                // dW1 / db1 read both warpgroups' rows of dz2
+      {
+        const uint32_t h1o = opaque(h1), dz2o = opaque(dz2), a0o = opaque(a0);
+        wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < TM / 16; ++kk)
-        wgmma_m64n128k16<BF16, 1, 1>(accW1, desc_act_t_as_a(h1, wg, kk), desc_act_as_b(dz2, kk), kk > 0 ? 1u : wacc);
+        for (int kk = 0; kk < TM / 16; ++kk)
+          wgmma_m64n128k16<BF16, 1, 1>(accW1, desc_act_t_as_a(h1o, wg, kk), desc_act_as_b(dz2o, kk), kk > 0 ? 1u : wacc);
 #pragma unroll
-      for (int kk = 0; kk < TM / 16; ++kk)
-        wgmma_m64n16k16<BF16, 1, 1>(accB1, desc_act_t_as_a(dz2, wg, kk), desc_a0_as_b(a0, kk), kk > 0 ? 1u : wacc);
+        for (int kk = 0; kk < TM / 16; ++kk)
+          wgmma_m64n16k16<BF16, 1, 1>(accB1, desc_act_t_as_a(dz2o, wg, kk), desc_a0_as_b(a0o, kk), kk > 0 ? 1u : wacc);
+      }
       wgmma_commit();
-      wgmma_wait<1>();
-      wgmma_fence_regs(acc);
-      // ---- dz1 = G1 * act'(h1) -> the h2 buffer, while dW1 / db1 run (they read h1, dz2, [pe|1]; every dW2 is done)
-      frag_dgrad_to_tile<BF16, RELU>(acc, h1, h2, fr, P.act, P.alpha);
+      wgmma_wait<1>();                     // G1, and dW2 / db2 before it
+      wgmma_fence_regs(accg); wgmma_fence_regs(accW2); wgmma_fence_regs(accB2);
+      xwg_arrive(kEvDW2, wg);              // this warpgroup's dW2 (it read all of h2) is done
+      // ---- dz1 = G1 * act'(h1) -> the h2 buffer, while dW1 / db1 run (they read h1, dz2, [pe|1])
+      uint32_t az[32];
+      frag_dgrad_to_a<BF16, RELU>(accg, h1, az, fr, P.act, P.alpha);
+      xwg_wait(kEvDW2, wg);                // dz1 is written over h2 only after every dW2 of the tile
+      a_to_tile<128>(az, h2, fr);
       wgmma_wait<0>();
       wgmma_fence_regs(accW1); wgmma_fence_regs(accB1);
-      cta_publish();
+      // dz1 stored, and this warpgroup's dW1 / db1 (they read all of h1, dz2) done: h1, dz2 and dO may be rewritten
+      xwg_arrive(kEvDZ1, wg);
+      xwg_wait(kEvDZ1, wg);                // dW0 reads both warpgroups' rows of dz1
       // ---- layer 0 backward: [dW0;db0]^T += dz1^T [pe|1], retired by the next tile's layer-0 wait (or after the loop)
-      wgmma_fence();
+      {
+        const uint32_t h2o = opaque(h2), a0o = opaque(a0);
+        wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < TM / 16; ++kk)
-        wgmma_m64n16k16<BF16, 1, 1>(accW0, desc_act_t_as_a(h2, wg, kk), desc_a0_as_b(a0, kk), kk > 0 ? 1u : wacc);
+        for (int kk = 0; kk < TM / 16; ++kk)
+          wgmma_m64n16k16<BF16, 1, 1>(accW0, desc_act_t_as_a(h2o, wg, kk), desc_a0_as_b(a0o, kk), kk > 0 ? 1u : wacc);
+      }
       wgmma_commit();
       tpar ^= 1u;
     }

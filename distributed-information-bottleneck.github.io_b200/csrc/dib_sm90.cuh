@@ -44,6 +44,10 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
+// the non-blocking half: counts this warp's threads towards the barrier's `count` and does not wait for the others
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 
 // ------------------------------------------------------------------------------------------------ TMA
 __device__ __forceinline__ void tma_prefetch_desc(const void* map) {
