@@ -10,10 +10,10 @@
 // registers -> shared memory (backward: swizzled operand tiles) and never touch HBM.  Only x (4 B/sample/feature) is read
 // and emb is written.
 //
-// Two warpgroups per CTA; warpgroup g owns rows [64 g, 64 g + 64) of a tile (wgmma M = 64).  Every contraction whose
+// Two MMA warpgroups per CTA; warpgroup g owns rows [64 g, 64 g + 64) of a tile (wgmma M = 64).  Every contraction whose
 // reduction runs over the hidden features (forward, dgrad) reads only the warpgroup's own rows, so the two warpgroups
 // proceed independently; the weight-gradient contractions of the backward reduce over all 128 samples of the tile and
-// meet at CTA barriers.
+// meet at barriers of the two.  The backward has a third, producer warpgroup that stages each tile's inputs and noise.
 //
 // Operand layouts (16-bit): every activation/weight tile is [rows][64-element panels of 128 B] with the 16-byte chunk
 // index XORed with (row % 8) -- the SWIZZLE_128B pattern, which for 16-bit types is simultaneously a valid K-major operand
@@ -60,8 +60,12 @@ constexpr int kOffH2 = kOffH1 + 2 * kPanel;        // h2, later dz1
 constexpr int kOffDO = kOffH2 + 2 * kPanel;        // [128 x 64] d(mu | logvar), one panel
 constexpr int kOffDZ2 = kOffDO + kPanel;           // [128 x 128]
 constexpr int kOffG = kOffDZ2 + 2 * kPanel;        // [128 rows][32] 16-bit d_emb16 of the next tile (TMA, no swizzle)
-constexpr int kOffBwdEnd = kOffG + TM * 64;
+constexpr int kNzBytes = TM * 32 * 4;              // one tile's noise: [128 rows][32 dims] fp32 (see nz_chunk)
+constexpr int kOffNz = kOffG + TM * 64;            // two noise buffers, alternating with the [pe|1] buffers
+constexpr int kOffBwdEnd = kOffNz + 2 * kNzBytes;
+constexpr int kBwdThreads = kThreads + 128;        // + a producer warpgroup (inputs and noise of the next tile)
 static_assert(kOffH1 % 1024 == 0 && kOffDZ2 % 1024 == 0, "operand tiles must be 1024-byte aligned");
+static_assert(kOffBwdEnd + 128 + 1024 <= 232448, "backward shared memory exceeds the 227 KB per-block opt-in");
 
 struct EncFusedParams {
   const float* x; int ldx;                 // [n, D]
@@ -115,6 +119,11 @@ __device__ __forceinline__ uint32_t ld_shared_b32(uint32_t addr) {
   asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
   return v;
 }
+__device__ __forceinline__ float2 ld_shared_v2f(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
+  return v;
+}
 
 // Position of this thread's accumulator elements in the tile: rows rb and rb + 8, columns 8 j + 2 q (+1).
 struct Frag {
@@ -133,16 +142,18 @@ __device__ __forceinline__ uint32_t opaque(uint32_t v) {
 }
 
 // Shared-memory places of a thread's accumulator words in a [128 x 64k] swizzled tile (16-byte chunk index XORed with
-// row % 8): word 2 j + h (columns 8 j + 2 q (+1), row rb + 8 h) is at fw.base + (j / 8) * kPanel + h * 1024 +
-// ((j % 8) * 16 ^ fw.sw).  The j-th offset is one LOP3 from fw.sw rather than one of eight registers held through the tile.
+// row % 8): word 2 j + h (columns 8 j + 2 q (+1), row rb + 8 h) is at tile + rb * 128 + 4 q + (j / 8) * kPanel + h * 1024
+// + ((j % 8) * 16 ^ (rb % 8) * 16).  Bits 4..6 of tile + rb * 128 + 4 q are zero (1024-aligned tile), so the swizzle folds
+// into one per-tile word fw.bsw = (tile + rb * 128 + 4 q) ^ (rb % 8) * 16, and the j-th place is one LOP3 with an immediate
+// from it: no swizzle term is shared between tiles, where the compiler would keep it in a register through the tile.
 struct FragWords {
-  uint32_t base, sw;
+  uint32_t bsw;
 };
 __device__ __forceinline__ FragWords frag_words(uint32_t tile, Frag fr) {
-  return FragWords{opaque(tile + fr.rb * 128 + 4 * fr.q), opaque((fr.rb & 7) << 4)};
+  return FragWords{opaque((tile + fr.rb * 128 + 4 * fr.q) ^ ((fr.rb & 7) << 4))};
 }
 __device__ __forceinline__ uint32_t frag_word_addr(FragWords fw, int j, int h) {
-  return fw.base + (j >> 3) * kPanel + h * 1024 + (((j & 7) << 4) ^ fw.sw);
+  return (fw.bsw ^ ((j & 7) << 4)) + (j >> 3) * kPanel + h * 1024;
 }
 
 // accumulator of a 64 x N tile -> activation -> 16-bit, kept in registers as the next MMA's A operand (the bias is already
@@ -353,6 +364,16 @@ __device__ __forceinline__ void mma_layer1_rs(float (&d)[64], uint32_t sb, const
     wgmma_m64n128k16_rs<BF16, 1>(d, a, gmma_desc(sb + kOffW1 + kk * 2048, kPanel, 1024), 1u);
   }
 }
+// The backward's recomputed layer 1 reads h1 from its shared tile (after wg_publish): a register A fragment would keep 32
+// registers live through the issue, next to the accumulator and the 120 weight-gradient registers, and the backward's MMA
+// warpgroups have 240 registers (the producer warpgroup has the rest).
+template <bool BF16>
+__device__ __forceinline__ void mma_layer1_ss(float (&d)[64], uint32_t sb, uint32_t h1, uint32_t a0, int wg) {
+  wgmma_m64n128k16<BF16, 0, 1>(d, desc_a0_as_a(a0, wg), gmma_desc(sb + kOffBb1, K0 * 128, 1024), 0u);
+#pragma unroll
+  for (int kk = 0; kk < HID / 16; ++kk)
+    wgmma_m64n128k16<BF16, 0, 1>(d, desc_act_as_a(h1, wg, kk), gmma_desc(sb + kOffW1 + kk * 2048, kPanel, 1024), 1u);
+}
 template <bool BF16>
 __device__ __forceinline__ void mma_layer2_rs(float (&d)[32], uint32_t sb, const uint32_t (&h2)[32], uint32_t a0, int wg) {
   wgmma_m64n64k16<BF16, 0, 1>(d, desc_a0_as_a(a0, wg), gmma_desc(sb + kOffBb2, K0 * 128, 1024), 0u);
@@ -502,7 +523,7 @@ dib_enc_fused_fwd_kernel(const __grid_constant__ WeightMaps maps, const EncFused
 //   (bias gradients = the ones column of [pe|1] used as the B operand: column sums for free)
 // S is a power-of-two loss scale that keeps the 16-bit gradient operands in range (fp16); the fp32 accumulators are
 // multiplied by 1/S when they are flushed.  The weight-gradient accumulators live in registers for the whole feature:
-// warpgroup g owns rows [64 g, 64 g + 64) of dW1, dW2 (and of dW0^T, db1); warpgroup 0 stores db2.  190 KB of shared
+// warpgroup g owns rows [64 g, 64 g + 64) of dW1, dW2 (and of dW0^T, db1); warpgroup 0 stores db2.  222 KB of shared
 // memory: one CTA per SM.
 //
 // The chain of a warpgroup's rows waits for nothing but its own MMAs (and its own warpgroup):
@@ -515,7 +536,18 @@ dib_enc_fused_fwd_kernel(const __grid_constant__ WeightMaps maps, const EncFused
 //   * in each backward layer the dgrad MMAs and the weight-gradient MMAs are separate commit groups; the dz epilogue waits
 //     only for the dgrad, so the weight-gradient MMAs run under it;
 //   * dW0 of tile t retires under the start of tile t + 1 ([pe|1] is double-buffered);
-//   * x (prefetch_x) and the 16-bit gradient d_emb16 (TMA, one 8 KB buffer) of the next tile are loaded a tile ahead.
+//   * nothing on the chain stages inputs: a third, producer warpgroup writes [pe|1] and the noise of tile t + 1 and issues
+//     its d_emb16 TMA (one 8 KB buffer) while the two MMA warpgroups run tile t (see the hand-offs below).
+//
+// Producer -> consumer hand-offs are mbarriers (the named barriers are taken by the consumers' events).  Each tile k of the
+// CTA's sequence (all features' tiles in sched_of order, which both sides walk) uses slot k % 2: a [pe|1] buffer and a noise
+// buffer.  Full barriers: a0_full / nz_full[slot] (128 producer threads), bar_g (d_emb16 TMA bytes), bar_w (weights).
+// Empty barriers, one arrival per consumer warp (8):
+//   * slot_empty[slot]: both warpgroups' dW0 of the tile retired (at the next tile's layer-0 wait, or after the feature's
+//     last tile); the noise was read before that, in the tile's dO epilogue;
+//   * g_empty: both warpgroups' dO epilogues read d_emb16;
+//   * w_empty: both warpgroups' last MMAs of the feature retired: the next feature's weights may be loaded.
+// A wait for use u of a buffer is for phase parity u & 1 (full) or (u & 1) ^ 1 (empty: the first use passes at once).
 // ====================================================================================================
 struct EncFusedBwdParams {
   EncFusedParams f;
@@ -526,65 +558,152 @@ struct EncFusedBwdParams {
   const long long* w0_off; const long long* b0_off; const long long* w1_off; const long long* w2_off;
 };
 
+// The backward's feature loop forms the schedule where it is used: both warpgroup roles are at their register limits across
+// the tile loop, so what sched_of derives from the CTA index is recomputed per feature instead of kept.  feature_iter = how
+// many features this CTA has run before f.
+__device__ __forceinline__ Sched sched_here(int F) {
+  uint32_t c, G;
+  asm volatile("mov.u32 %0, %%ctaid.x;" : "=r"(c));
+  asm volatile("mov.u32 %0, %%nctaid.x;" : "=r"(G));
+  return sched_of((int)c, (int)G, F);
+}
+__device__ __forceinline__ uint32_t feature_iter(int f, const Sched& s) { return (uint32_t)((f - s.f_first) / s.f_step); }
+
 // one thread: the [128 rows x 32] block of d_emb16 (feature f, rows from row0) -> shared memory; rows past n read as 0
 __device__ __forceinline__ void load_demb16(uint32_t dst, const CUtensorMap* gmap, uint32_t bar, int f, long long row0) {
   mbar_expect_tx(bar, TM * 64);
   tma_load_2d(dst, gmap, bar, f * 32, (int)row0);
 }
 
+// Noise buffer of a tile: the 16-byte chunk c (dims 4 c .. 4 c + 3, one Philox quad) of row r sits at r * 128 + (c ^ r % 8) * 16.
+// The producer's float4 stores (a warp: 4 rows x 8 chunks) and the consumers' float2 reads of a fragment's pairs (a warp:
+// 8 rows x 2 chunks) are both conflict-free; a plain [128][32] layout would make the reads 8-way conflicted.
+__device__ __forceinline__ uint32_t nz_chunk(uint32_t nzb, int r, int c) { return nzb + r * 128 + ((c ^ (r & 7)) << 4); }
+
+// the producer's share of tile row0's noise: thread p (of 128) writes the chunks p, p + 128, ... of the [128 x 8] chunks.
+// Rows past the batch end are written as zeros (the dO epilogue does not use them).
+__device__ __forceinline__ void produce_noise(const EncFusedParams& P, unsigned int nstep, uint32_t nzb, int p, long long row0,
+                                              int f) {
+#pragma unroll 1
+  for (int i = p; i < TM * 8; i += 128) {
+    const int r = i >> 3, c = i & 7;
+    const long long grow = row0 + r;
+    float n4[4] = {0.f, 0.f, 0.f, 0.f};
+    if (grow < P.n) {
+      if (P.eps) {
+        const float* e = P.eps + (grow * P.F + f) * 32 + 4 * c;
+        const float2 lo = *reinterpret_cast<const float2*>(e), hi = *reinterpret_cast<const float2*>(e + 2);
+        n4[0] = lo.x; n4[1] = lo.y; n4[2] = hi.x; n4[3] = hi.y;
+      } else {
+        dib_philox_normal4(P.seed, nstep, P.sample_offset + (unsigned long long)grow, (uint32_t)f, (uint32_t)c, n4);
+      }
+    }
+    st_shared_v4(nz_chunk(nzb, r, c), __float_as_uint(n4[0]), __float_as_uint(n4[1]), __float_as_uint(n4[2]),
+                 __float_as_uint(n4[3]));
+  }
+}
+
+// a consumer warp's arrival on an empty barrier, once all its lanes are past their reads
+__device__ __forceinline__ void warp_arrive(uint32_t bar) {
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
+}
+
 template <bool BF16, bool RELU>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(kBwdThreads, 1)
 dib_enc_fused_bwd_kernel(const __grid_constant__ WeightMaps maps, const __grid_constant__ CUtensorMap gmap,
                          const EncFusedBwdParams Q) {
   const EncFusedParams& P = Q.f;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sb = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint8_t* sg = smem_raw + (sb - smem_u32(smem_raw));
-  const uint32_t bar_w = sb + kOffBwdEnd, bar_g = bar_w + 8;
+  const uint32_t bar_w = sb + kOffBwdEnd, w_empty = bar_w + 8, bar_g = bar_w + 16, g_empty = bar_w + 24;
+  auto a0_full = [&](uint32_t b) { return bar_w + 32 + 8 * b; };
+  auto nz_full = [&](uint32_t b) { return bar_w + 48 + 8 * b; };
+  auto slot_empty = [&](uint32_t b) { return bar_w + 64 + 8 * b; };
+  // a slot's tile, written by the producer with its [pe|1]: rows inside the batch (<= 128), and whether the weight-gradient
+  // MMAs accumulate (all but the feature's first tile; the first one starts them with scale-d = 0)
+  auto rows_of = [&](uint32_t b) { return bar_w + 80 + 4 * b; };
+  auto wacc_of = [&](uint32_t b) { return bar_w + 88 + 4 * b; };
 
-  const int tid = threadIdx.x, lane = tid & 31, wg = tid >> 7;
-  const Frag fr = frag_of(tid);
+  const int tid = threadIdx.x, wg = tid >> 7;
   const int F = P.F;
-  const int ntiles = (int)((P.n + TM - 1) / TM);
-  const unsigned int nstep = P.step + (P.step_dev ? P.step_dev[0] : 0u);
   const uint32_t h1 = sb + kOffH1, h2 = sb + kOffH2, dO = sb + kOffDO, dz2 = sb + kOffDZ2, gbuf = sb + kOffG;
-  const uint32_t xs = sb + kOffX + tid * 16;
-  const float* xslot = reinterpret_cast<const float*>(sg + kOffX + tid * 16);
-  const float S = Q.gscale, invS = 1.f / Q.gscale;
+  const float S = Q.gscale;
 
   if (tid == 0) {
     tma_prefetch_desc(&maps.w0); tma_prefetch_desc(&maps.w1); tma_prefetch_desc(&maps.w2);
     tma_prefetch_desc(&maps.b1); tma_prefetch_desc(&maps.b2);
     if (Q.d_emb16) tma_prefetch_desc(&gmap);
     mbar_init(bar_w, 1);
+    mbar_init(w_empty, 8);
     mbar_init(bar_g, 1);
+    mbar_init(g_empty, 8);
+    for (uint32_t b = 0; b < 2; ++b) { mbar_init(a0_full(b), 128); mbar_init(nz_full(b), 128); mbar_init(slot_empty(b), 8); }
     fence_barrier_init();
   }
   __syncthreads();
 
-  const Sched s = sched_of(blockIdx.x, gridDim.x, F);
-  uint32_t fit = 0, tpar = 0;   // tpar: parity of the tiles run so far = this tile's [pe|1] buffer and d_emb16-load phase
-  for (int f = s.f_first; f < F; f += s.f_step, ++fit) {
-    if (tid == 0) {
-      load_weights(sb, maps, bar_w, f);
-      if (Q.d_emb16 && s.slot < ntiles) load_demb16(gbuf, &gmap, bar_g, f, (long long)s.slot * TM);
+  if (wg == 2) {
+    // ================= producer: weights, [pe|1], noise and d_emb16 of each tile, one tile ahead of the consumers
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");
+    // (24 registers: what depends only on the feature or the step is loaded again per tile rather than kept)
+    const int p = tid - kThreads;
+    uint32_t tk = 0;
+    for (int f = sched_here(F).f_first; f < F; f += sched_here(F).f_step) {
+      const Sched s = sched_here(F);
+      // (the producer's waits are made by all of its threads and only the TMA issue by one: its control flow stays
+      // warp-uniform, so that the loop state can live in uniform registers)
+      mbar_wait(w_empty, (feature_iter(f, s) & 1) ^ 1);
+      if (p == 0) load_weights(sb, maps, bar_w, f);
+      for (int t = s.slot; (long long)t * TM < P.n; t += s.nslots, ++tk) {
+        const long long row0 = (long long)t * TM;
+        const uint32_t b = tk & 1;
+        mbar_wait(slot_empty(b), ((tk >> 1) & 1) ^ 1);
+        {   // [pe|1]: thread p writes both k-halves of row p
+          const int dt = P.fdim[f], xo = P.x_off[f];
+          const long long grow = row0 + p;
+          float xv[kMaxFeatDim];
+#pragma unroll
+          for (int j = 0; j < kMaxFeatDim; ++j) xv[j] = (grow < P.n && j < dt) ? P.x[grow * P.ldx + xo + j] : 0.f;
+          const uint32_t a0 = sb + kOffA0 + b * kA0Bytes;
+          if (p == 0) {
+            st_shared_b32(rows_of(b), (uint32_t)min((long long)TM, P.n - row0));
+            st_shared_b32(wacc_of(b), t != s.slot);
+          }
+#pragma unroll 1
+          for (int kh = 0; kh < 2; ++kh) write_a0_row<BF16>(a0, p, kh, grow < P.n, xv, dt, P.nfreq);
+          fence_proxy_async_smem();        // the consumers' MMAs read it
+          mbar_arrive(a0_full(b));
+        }
+        produce_noise(P, P.step + (P.step_dev ? P.step_dev[0] : 0u), sb + kOffNz + b * kNzBytes, p, row0, f);
+        mbar_arrive(nz_full(b));
+        if (Q.d_emb16) {
+          mbar_wait(g_empty, (tk & 1) ^ 1);
+          if (p == 0) load_demb16(gbuf, &gmap, bar_g, f, row0);
+        }
+      }
     }
-    const int d = P.fdim[f], xo = P.x_off[f];
-    prefetch_x(P, xs, tid, (long long)s.slot * TM, d, xo);
-    const float bs = Q.beta_dev[0] * Q.inv_batch * S;
+    return;
+  }
+  // ================= consumers: warpgroups 0 and 1
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 240;");   // 128 x 24 + 256 x 240 = 384 x 168, what the CTA holds at launch
+  const Frag fr = frag_of(tid);
+  uint32_t tk = 0;   // tiles run so far; tile tk uses slot tk % 2 and the d_emb16 phase tk % 2
+  for (int f = sched_here(F).f_first; f < F; f += sched_here(F).f_step) {
+    const Sched s = sched_here(F);
     // The weight-gradient accumulators are started by the first tile's MMAs (scale-d = 0), not by register writes: no
     // instruction but a wgmma may define them while dW0 is in flight across tiles.  A CTA without a tile of the feature
     // flushes zeros.
     float accW1[64], accW2[32], accW0[8], accB1[8], accB2[8];
-    mbar_wait(bar_w, fit & 1);
-    for (int t = s.slot; t < ntiles; t += s.nslots) {
+    mbar_wait(bar_w, feature_iter(f, s) & 1);
+    // (the tile count, the schedule and the loss-scaled beta are formed where they are used, and the tile's row count and
+    // accumulate flag read from its slot: the consumers' registers are full across the feature loop)
+    for (int t = s.slot; (long long)t * TM < P.n; t += sched_here(F).nslots, ++tk) {
       const long long row0 = (long long)t * TM;
-      const uint32_t wacc = t != s.slot;   // accumulate into the weight gradients (all but the feature's first tile)
-      const uint32_t a0 = sb + kOffA0 + tpar * kA0Bytes;
+      const uint32_t b = tk & 1, bpar = (tk >> 1) & 1;
+      const uint32_t a0 = sb + kOffA0 + b * kA0Bytes;
       // ---- recompute the forward of this warpgroup's rows
-      stage_a0<BF16>(P, a0, xslot, tid, row0, d);
-      prefetch_x(P, xs, tid, row0 + (long long)s.nslots * TM, d, xo);
-      wg_publish(wg);
+      mbar_wait(a0_full(b), bpar);
       float acc[64];
       wgmma_fence();
       mma_layer0<BF16>(acc, sb, a0, wg);
@@ -592,15 +711,17 @@ dib_enc_fused_bwd_kernel(const __grid_constant__ WeightMaps maps, const __grid_c
       wgmma_wait<0>();                     // also retires this warpgroup's dW0 of the previous tile
       wgmma_fence_regs(acc); wgmma_fence_regs(accW0);
       xwg_arrive(kEvL0, wg);               // this warpgroup's dW0 of the previous tile (it read all of h2) is done
+      if (ld_shared_b32(wacc_of(b))) warp_arrive(slot_empty(b ^ 1));   // ... and with it every read of the previous tile's slot
       uint32_t ha[32];
       frag_to_a<BF16, RELU, 128>(acc, ha, P.act, P.alpha);
       // h1 for dW1 and act'(h1).  The previous tile's dW1 of both warpgroups retired before its kEvDZ1 hand-off.
       a_to_tile<128>(ha, h1, fr);
       // (each MMA chain that starts with scale-d = 0 gets a fresh accumulator: then the values that the previous epilogue
-      // consumed are not kept live up to the next MMA's issue, next to its register A fragment)
+      // consumed are not kept live up to the next MMA's issue)
       float acc1[64];
+      wg_publish(wg);
       wgmma_fence();
-      mma_layer1_rs<BF16>(acc1, sb, ha, a0, wg);
+      mma_layer1_ss<BF16>(acc1, sb, h1, a0, wg);
       wgmma_commit();
       wgmma_wait<0>();
       wgmma_fence_regs(acc1);
@@ -614,24 +735,30 @@ dib_enc_fused_bwd_kernel(const __grid_constant__ WeightMaps maps, const __grid_c
       mma_layer2_rs<BF16>(acc2, sb, ha, a0, wg);
       wgmma_commit();
       const long long grow_lo = row0 + fr.rb;
-      float nz[4][2][2];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) noise_pair(P, nstep, grow_lo, f, j, fr.q, lane, nz[j]);
-      if (Q.d_emb16) mbar_wait(bar_g, tpar);
+      const float bs = Q.beta_dev[0] * Q.inv_batch * S;
+      const int rows = (int)ld_shared_b32(rows_of(b));   // rows of the tile inside the batch
+      mbar_wait(nz_full(b), bpar);
+      if (Q.d_emb16) mbar_wait(bar_g, tk & 1);
       wgmma_wait<0>();
       wgmma_fence_regs(acc2);
       // ---- (mu, logvar) -> d(mu), d(logvar) = dO, packed as the A fragment of G2 (column e of dO is word 2 (e / 8) + h of
       // the fragment, 32 + e is 8 + 2 (e / 8) + h).  Rows past the batch end contribute nothing.
+      // this thread's eps pairs: dims 8 j + 2 q (+1) of row rb + 8 h are at nzo + h * 1024 + (32 j ^ nzs) (nz_chunk with
+      // chunk 2 j + q / 2), formed where they are read
+      const uint32_t nzo = opaque(sb + kOffNz + b * kNzBytes + fr.rb * 128 + 8 * (fr.q & 1));
+      const uint32_t nzs = opaque((((fr.rb & 7) ^ (fr.q >> 1)) << 4));
       uint32_t ao[16];
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const long long grow = grow_lo + 8 * h;
-        const bool valid = grow < P.n;
+        const bool valid = fr.rb + 8 * h < rows;
         const float bsv = valid ? bs : 0.f;
         const int r = fr.rb + 8 * h;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           const int e = 8 * j + 2 * fr.q;
+          const float2 ez = ld_shared_v2f(nzo + h * 1024 + ((32 * j) ^ nzs));   // eps of dims e, e + 1
+          const float nz[2] = {ez.x, ez.y};
           float g[2] = {0.f, 0.f};
           if (valid) {
             if (Q.d_emb16) unpack2<BF16>(ld_shared_b32(gbuf + 4 * (r * 16 + e / 2)), g[0], g[1]);   // [128 rows][16 pairs]
@@ -646,12 +773,13 @@ dib_enc_fused_bwd_kernel(const __grid_constant__ WeightMaps maps, const __grid_c
             const float mu = acc2[4 * j + 2 * h + k], lv = acc2[4 * (j + 4) + 2 * h + k];
             const float sgm = expf(0.5f * lv);
             dm[k] = fmaf(bsv, mu, g[k]);
-            dl[k] = valid ? fmaf(g[k] * nz[j][h][k], 0.5f * sgm, bsv * 0.5f * (sgm * sgm - 1.f)) : 0.f;
+            dl[k] = valid ? fmaf(g[k] * nz[k], 0.5f * sgm, bsv * 0.5f * (sgm * sgm - 1.f)) : 0.f;
           }
           ao[2 * j + h] = pack2<BF16>(dm[0], dm[1]);
           ao[8 + 2 * j + h] = pack2<BF16>(dl[0], dl[1]);
         }
       }
+      if (Q.d_emb16) warp_arrive(g_empty);   // this warp's d_emb16 rows are read: the producer may load the next tile's
       // dO for dW2 / db2.  The previous tile's dW2 / db2 of both warpgroups retired before its kEvDZ1 hand-off.
       a_to_tile<64>(ao, dO, fr);
       xwg_arrive(kEvDO, wg);               // this warpgroup's rows of h1, h2, dO, [pe|1] are stored; its d_emb16 rows read
@@ -665,9 +793,8 @@ dib_enc_fused_bwd_kernel(const __grid_constant__ WeightMaps maps, const __grid_c
       }
       wgmma_commit();
       xwg_wait(kEvDO, wg);                 // dW2 / db2 read both warpgroups' rows of h2, dO and [pe|1]
-      if (tid == 0 && Q.d_emb16 && t + s.nslots < ntiles) load_demb16(gbuf, &gmap, bar_g, f, row0 + (long long)s.nslots * TM);
       {
-        const uint32_t h2o = opaque(h2), dOo = opaque(dO), a0o = opaque(a0);
+        const uint32_t h2o = opaque(h2), dOo = opaque(dO), a0o = opaque(a0), wacc = ld_shared_b32(wacc_of(b));
         wgmma_fence();
 #pragma unroll
         for (int kk = 0; kk < TM / 16; ++kk)
@@ -701,7 +828,7 @@ dib_enc_fused_bwd_kernel(const __grid_constant__ WeightMaps maps, const __grid_c
       wgmma_commit();
       xwg_wait(kEvDZ2, wg);                // dW1 / db1 read both warpgroups' rows of dz2
       {
-        const uint32_t h1o = opaque(h1), dz2o = opaque(dz2), a0o = opaque(a0);
+        const uint32_t h1o = opaque(h1), dz2o = opaque(dz2), a0o = opaque(a0), wacc = ld_shared_b32(wacc_of(b));
         wgmma_fence();
 #pragma unroll
         for (int kk = 0; kk < TM / 16; ++kk)
@@ -726,21 +853,23 @@ dib_enc_fused_bwd_kernel(const __grid_constant__ WeightMaps maps, const __grid_c
       xwg_wait(kEvDZ1, wg);                // dW0 reads both warpgroups' rows of dz1
       // ---- layer 0 backward: [dW0;db0]^T += dz1^T [pe|1], retired by the next tile's layer-0 wait (or after the loop)
       {
-        const uint32_t h2o = opaque(h2), a0o = opaque(a0);
+        const uint32_t h2o = opaque(h2), a0o = opaque(a0), wacc = ld_shared_b32(wacc_of(b));
         wgmma_fence();
 #pragma unroll
         for (int kk = 0; kk < TM / 16; ++kk)
           wgmma_m64n16k16<BF16, 1, 1>(accW0, desc_act_t_as_a(h2o, wg, kk), desc_a0_as_b(a0o, kk), kk > 0 ? 1u : wacc);
       }
       wgmma_commit();
-      tpar ^= 1u;
     }
     wgmma_wait<0>();
     wgmma_fence_regs(accW0);
+    warp_arrive(w_empty);                  // this warp's MMAs of the feature (the weights' last readers) retired
+    const bool ran = (long long)sched_here(F).slot * TM < P.n;
+    if (ran) warp_arrive(slot_empty((tk - 1) & 1));   // the last tile's dW0 retired
     // ================= flush this (feature, slot)'s weight-gradient partials (scaled back by 1/S)
-    float* part = Q.part + (long long)s.slot * Q.split_stride;
-    const int w_in = d * P.nfreq;
-    const bool ran = s.slot < ntiles;
+    float* part = Q.part + (long long)sched_here(F).slot * Q.split_stride;
+    const int w_in = P.fdim[f] * P.nfreq;
+    const float invS = 1.f / __uint_as_float(opaque(__float_as_uint(S)));
     auto out = [&](float v) { return ran ? v * invS : 0.f; };
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -769,7 +898,6 @@ dib_enc_fused_bwd_kernel(const __grid_constant__ WeightMaps maps, const __grid_c
         }
       }
     }
-    __syncthreads();                       // both warpgroups are done with this feature's weights
   }
 }
 
@@ -868,10 +996,10 @@ void fill_params(EncFusedParams& P, const DibEncFusedDesc& d, const DibEncFusedI
 }
 
 template <typename K, typename... A>
-cudaError_t launch_fused(K kern, int smem, int grid, cudaStream_t st, const A&... args) {
+cudaError_t launch_fused(K kern, int threads, int smem, int grid, cudaStream_t st, const A&... args) {
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e != cudaSuccess) return e;
-  kern<<<grid, kThreads, smem, st>>>(args...);
+  kern<<<grid, threads, smem, st>>>(args...);
   dib_note_launch();
   return cudaGetLastError();
 }
@@ -903,10 +1031,10 @@ cudaError_t dib_enc_fused_forward(const DibEncFusedDesc& d, const DibEncFusedIO&
   fill_params(P, d, io);
   constexpr int smem = kOffFwdEnd + 128 + 1024;
   const bool relu = d.act == DIB_ACT_RELU;
-  if (d.bf16) return relu ? launch_fused(dib_enc_fused_fwd_kernel<true, true>, smem, d.grid, st, m, P)
-                          : launch_fused(dib_enc_fused_fwd_kernel<true, false>, smem, d.grid, st, m, P);
-  return relu ? launch_fused(dib_enc_fused_fwd_kernel<false, true>, smem, d.grid, st, m, P)
-              : launch_fused(dib_enc_fused_fwd_kernel<false, false>, smem, d.grid, st, m, P);
+  if (d.bf16) return relu ? launch_fused(dib_enc_fused_fwd_kernel<true, true>, kThreads, smem, d.grid, st, m, P)
+                          : launch_fused(dib_enc_fused_fwd_kernel<true, false>, kThreads, smem, d.grid, st, m, P);
+  return relu ? launch_fused(dib_enc_fused_fwd_kernel<false, true>, kThreads, smem, d.grid, st, m, P)
+              : launch_fused(dib_enc_fused_fwd_kernel<false, false>, kThreads, smem, d.grid, st, m, P);
 }
 
 cudaError_t dib_enc_fused_backward(const DibEncFusedDesc& d, const DibEncFusedIO& io, const DibEncFusedBwdIO& b,
@@ -925,8 +1053,8 @@ cudaError_t dib_enc_fused_backward(const DibEncFusedDesc& d, const DibEncFusedIO
   Q.w0_off = d.w0_off; Q.b0_off = d.b0_off; Q.w1_off = d.w1_off; Q.w2_off = d.w2_off;
   constexpr int smem = kOffBwdEnd + 128 + 1024;
   const bool relu = d.act == DIB_ACT_RELU;
-  if (d.bf16) return relu ? launch_fused(dib_enc_fused_bwd_kernel<true, true>, smem, d.grid, st, m, gmap, Q)
-                          : launch_fused(dib_enc_fused_bwd_kernel<true, false>, smem, d.grid, st, m, gmap, Q);
-  return relu ? launch_fused(dib_enc_fused_bwd_kernel<false, true>, smem, d.grid, st, m, gmap, Q)
-              : launch_fused(dib_enc_fused_bwd_kernel<false, false>, smem, d.grid, st, m, gmap, Q);
+  if (d.bf16) return relu ? launch_fused(dib_enc_fused_bwd_kernel<true, true>, kBwdThreads, smem, d.grid, st, m, gmap, Q)
+                          : launch_fused(dib_enc_fused_bwd_kernel<true, false>, kBwdThreads, smem, d.grid, st, m, gmap, Q);
+  return relu ? launch_fused(dib_enc_fused_bwd_kernel<false, true>, kBwdThreads, smem, d.grid, st, m, gmap, Q)
+              : launch_fused(dib_enc_fused_bwd_kernel<false, false>, kBwdThreads, smem, d.grid, st, m, gmap, Q);
 }
