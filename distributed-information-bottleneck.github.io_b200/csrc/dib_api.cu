@@ -492,6 +492,20 @@ int check_sets(const dib_model* h, int64_t n) {
 
 // noise of one forward: the caller's eps, or Philox (seed, step, sample_offset); training turns Dropout on
 struct NoiseKey { const float* eps; uint64_t seed; uint32_t step; uint64_t sample_offset; bool training; };
+
+// the encoder side of a call on n sets: the encoders and the attention blocks run on its n * Ls particle rows (with the bound
+// sizes of a variable-size model), their noise keyed by the global particle row.  An MLP model (Ls = 1, no sizes) gets the call
+// unchanged.
+struct RowView { Ctx c; NoiseKey nk; };
+RowView particle_rows(const Ctx& c, const NoiseKey& nk) {
+  const dib_model* h = c.h;
+  RowView r{c, nk};
+  r.c.n = c.n * h->Ls;
+  r.c.sizes = h->varlen ? h->set_sizes_dev : nullptr;
+  r.nk.sample_offset = nk.sample_offset * (uint64_t)h->Ls;
+  return r;
+}
+
 int encode_all(const Ctx& c, const float* x, int ldx, int feature, const int* row_index, int64_t n_src, const NoiseKey* key = nullptr);
 
 // TF32 GEMMs read the weights through a TF32-rounded copy
@@ -741,20 +755,6 @@ int forward_integration(const Ctx& c, const float* y, float inv_batch, bool trai
   DIB_CUDA_OK(finalize(h->head_blocks));
   prof_end(c);
   return 0;
-}
-
-int run_forward(const Ctx& c, const float* x, const float* y, const NoiseKey& nk, float inv_batch, float* user_pred,
-                float* user_emb, float* out_stats, bool enc_only = false) {
-  dib_model* h = c.h;
-  if (!h->route.int16 && tf32_shadow(c)) return 1;     // the 16-bit route runs no TF32 GEMM
-  int nblk_kl = 0;
-  if (forward_encoders(c, x, nk, user_emb, enc_only, &nblk_kl)) return 1;
-  if (enc_only) {
-    DIB_CUDA_OK(dib_launch_finalize_stats(c.ws + h->kl_part_off, h->kl_stride, nblk_kl, c.ws + h->loss_part_off,
-                                          c.ws + h->acc_part_off, 0, h->F, c.n, 0, out_stats, c.st));
-    return 0;
-  }
-  return forward_integration(c, y, inv_batch, nk.training, user_pred, out_stats, nblk_kl);
 }
 
 // every feature encoder (feature = -1), or feature `feature` alone reading only its columns of x, on n rows of x
@@ -1027,64 +1027,45 @@ int backward_set_blocks(const Ctx& c, const Split& sp) {
   return 0;
 }
 
-// dib_forward / dib_train_step's forward for the set transformer: cs.n counts sets
-int run_forward_set(const Ctx& cs, const float* x, const float* y, const NoiseKey& nk, float inv_batch, float* user_pred,
-                    float* user_emb, float* out_stats) {
-  dib_model* h = cs.h;
-  Ctx c = cs;
-  c.n = cs.n * h->Ls;
-  c.sizes = h->varlen ? h->set_sizes_dev : nullptr;
-  NoiseKey nr = nk;
-  nr.sample_offset = nk.sample_offset * (uint64_t)h->Ls;     // noise keyed by the global particle row
-  if (tf32_shadow(c)) return 1;
+// the forward of a call: the encoders (and a set transformer's attention blocks) on its particle rows, the integration network
+// on its own rows
+int run_forward(const Ctx& c, const float* x, const float* y, const NoiseKey& nk, float inv_batch, float* user_pred,
+                float* user_emb, float* out_stats, bool enc_only = false) {
+  dib_model* h = c.h;
+  const RowView r = particle_rows(c, nk);
+  if (!h->route.int16 && tf32_shadow(c)) return 1;     // the 16-bit route runs no TF32 GEMM
   int nblk_kl = 0;
-  if (forward_encoders(c, x, nr, user_emb, false, &nblk_kl)) return 1;
-  if (forward_set_blocks(c)) return 1;
-  return forward_integration(cs, y, inv_batch, nk.training, user_pred, out_stats, nblk_kl);
-}
-
-int train_step_set(const Ctx& cs, const float* x, const float* y, const NoiseKey& nk, const float* beta_dev, float inv_global_batch,
-                   float* grads_flat, float* out_stats) {
-  dib_model* h = cs.h;
-  if (run_forward_set(cs, x, y, nk, inv_global_batch, nullptr, nullptr, out_stats)) return 1;
-  const float* beta_w = nullptr;
-  if (ib_weight(cs, beta_dev, out_stats, inv_global_batch, &beta_w)) return 1;
-  std::vector<DibReduceSeg> segs;          // unused: the head runs on the per-layer GEMM route, which reduces its own range
-  if (backward_integration(cs, inv_global_batch, batch_split(cs.n), grads_flat, &segs)) return 1;
-  Ctx c = cs;
-  c.n = cs.n * h->Ls;
-  c.sizes = h->varlen ? h->set_sizes_dev : nullptr;
-  NoiseKey nr = nk;
-  nr.sample_offset = nk.sample_offset * (uint64_t)h->Ls;
-  const Split sp = batch_split(c.n);
-  if (backward_set_blocks(c, sp)) return 1;
-  int nrows = 0;
-  if (backward_encoders(c, x, nr, c.ws + h->d_emb.off, h->d_emb.ld, nullptr, beta_w, inv_global_batch, sp, &nrows)) return 1;
-  prof_begin(c, "enc_blocks_split_reduce");   // the encoder and the blocks: [0, first head parameter)
-  DIB_CUDA_OK(dib_launch_reduce_partials(c.ws + h->part_off, h->Pp, nrows, h->intW[0], grads_flat, c.st));
-  prof_end(c);
-  return 0;
+  if (forward_encoders(r.c, x, r.nk, user_emb, enc_only, &nblk_kl)) return 1;
+  if (enc_only) {
+    DIB_CUDA_OK(dib_launch_finalize_stats(c.ws + h->kl_part_off, h->kl_stride, nblk_kl, c.ws + h->loss_part_off,
+                                          c.ws + h->acc_part_off, 0, h->F, c.n, 0, out_stats, c.st));
+    return 0;
+  }
+  if (h->st && forward_set_blocks(r.c)) return 1;
+  return forward_integration(c, y, inv_batch, nk.training, user_pred, out_stats, nblk_kl);
 }
 
 // the reverse mode of dib_train_step after its forward (and, with DIB_LOSS_INFONCE, the InfoNCE gradients) left the
-// workspace: the IB weight from the stats, the integration network's, the output encoder's and the encoders' backward and the
-// fixed-order reductions into grads_flat
+// workspace: the IB weight from the stats, the integration network's, the output encoder's, the attention blocks' and the
+// encoders' backward and the fixed-order reductions into grads_flat
 int backward_all(const Ctx& c, const float* x, const NoiseKey& nk, const float* beta_dev, const float* stats, float inv_global_batch,
                  float* grads_flat) {
   dib_model* h = c.h;
+  const RowView r = particle_rows(c, nk);
   const float* beta_w = nullptr;           // weight of the per-sample KL gradients in the encoder backward
   if (ib_weight(c, beta_dev, stats, inv_global_batch, &beta_w)) return 1;
-  const Split sp = batch_split(c.n);
+  const Split sp = batch_split(c.n), sp_rows = batch_split(r.c.n);
   std::vector<DibReduceSeg> segs;          // fixed-order reductions of the step, run as ONE launch at the end
   if (backward_integration(c, inv_global_batch, sp, grads_flat, &segs)) return 1;
   if (infonce(h) && backward_output_encoder(c, sp, grads_flat)) return 1;
+  if (h->st && backward_set_blocks(r.c, sp_rows)) return 1;
   int nrows = 0;
   const bool d16 = h->route.int16;         // the 16-bit integration backward leaves d emb in fp16
-  if (backward_encoders(c, x, nk, d16 ? nullptr : c.ws + h->d_emb.off, d16 ? 0 : h->d_emb.ld, d16 ? c.ws + h->demb16_off : nullptr,
-                        beta_w, inv_global_batch, sp, &nrows))
+  if (backward_encoders(r.c, x, r.nk, d16 ? nullptr : c.ws + h->d_emb.off, d16 ? 0 : h->d_emb.ld, d16 ? c.ws + h->demb16_off : nullptr,
+                        beta_w, inv_global_batch, sp_rows, &nrows))
     return 1;
   float* part = c.ws + h->part_off;
-  const long long p_enc = h->intW[0];      // encoder parameters occupy [0, p_enc)
+  const long long p_enc = h->intW[0];      // encoder (and attention block) parameters occupy [0, p_enc)
   prof_begin(c, "enc_split_reduce");
   if (h->route.enc_fused) {
     segs.push_back({part, h->Pp, nrows, p_enc, 1.f, grads_flat});
@@ -1483,7 +1464,6 @@ int dib_forward(dib_model* h, const float* params, const float* x, const float* 
   if (!out_stats) return fail("dib_forward: out_stats is required");
   Ctx c{h, params, static_cast<float*>(workspace), static_cast<cudaStream_t>(stream), (int)n};
   if (n == 0) { DIB_CUDA_OK(cudaMemsetAsync(out_stats, 0, sizeof(float) * (h->F + 3), c.st)); return 0; }
-  if (h->st) return run_forward_set(c, x, y, NoiseKey{eps, seed, step, sample_offset, false}, 0.f, out_pred, out_emb, out_stats);
   return run_forward(c, x, y, NoiseKey{eps, seed, step, sample_offset, false}, 0.f, out_pred, out_emb, out_stats);
 }
 
@@ -1516,7 +1496,6 @@ int dib_train_step(dib_model* h, const float* params, const float* x, const floa
     return 0;
   }
   const NoiseKey nk{eps, seed, step, sample_offset, true};
-  if (h->st) return train_step_set(c, x, y, nk, beta_dev, inv_global_batch, grads_flat, out_stats);
   if (run_forward(c, x, y, nk, inv_global_batch, nullptr, nullptr, out_stats)) return 1;
   return backward_all(c, x, nk, beta_dev, out_stats, inv_global_batch, grads_flat);
 }
@@ -1617,18 +1596,16 @@ int dib_integration_forward(dib_model* h, const float* params, const float* emb,
   const int FE = h->F * h->E;
   if (tf32_shadow(c)) return 1;
   if (h->st) {                 // emb [n, Ls, E] (E is a multiple of 4: no padded columns) through the blocks and the mean
-    Ctx cr = c;
-    cr.n = (int)n * h->Ls;
-    cr.sizes = h->varlen ? h->set_sizes_dev : nullptr;
+    const Ctx cr = particle_rows(c, NoiseKey{}).c;
     if (is_tc(h)) DIB_CUDA_OK(dib_launch_round_copy(emb, c.ws + h->emb.off, (int64_t)cr.n * FE, c.st));
     else DIB_CUDA_OK(dib_launch_copy2d(emb, FE, c.ws + h->emb.off, h->emb.ld, FE, cr.n, c.st));
     if (cr.sizes) DIB_CUDA_OK(dib_launch_zero_pad_rows(c.ws + h->emb.off, h->emb.ld, cr.n, h->Ls, cr.sizes, c.st));
     if (forward_set_blocks(cr)) return 1;
   } else {
     DIB_CUDA_OK(dib_launch_copy2d(emb, FE, c.ws + h->emb.off, h->emb.ld, FE, n, c.st));
+    if (h->emb.ld > FE)          // zero the padded operand columns
+      DIB_CUDA_OK(cudaMemset2DAsync(c.ws + h->emb.off + FE, sizeof(float) * h->emb.ld, 0, sizeof(float) * (h->emb.ld - FE), (size_t)n, c.st));
   }
-  if (!h->st && h->emb.ld > FE)          // zero the padded operand columns
-    DIB_CUDA_OK(cudaMemset2DAsync(c.ws + h->emb.off + FE, sizeof(float) * h->emb.ld, 0, sizeof(float) * (h->emb.ld - FE), (size_t)n, c.st));
   if (stack_forward(c, h->int_stack, 0, 1)) return 1;
   DIB_CUDA_OK(dib_launch_copy2d(c.ws + h->pred.off, h->pred.ld, out_pred, h->out, h->out, n, c.st));
   return 0;
