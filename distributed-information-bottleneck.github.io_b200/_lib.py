@@ -82,6 +82,8 @@ SIGNATURES = {
                                              c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p]),
     "dib_set_noise_step_device": (c_int32, [c_void_p, c_void_p]),
     "dib_set_set_sizes_device": (c_int32, [c_void_p, c_void_p]),
+    "dib_set_sample_weights_device": (c_int32, [c_void_p, c_void_p]),
+    "dib_class_weight_rows": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_int32, c_void_p, c_void_p, c_void_p]),
     "dib_adam_step": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_float,
                                 c_float, c_float, c_void_p]),
     "dib_optimizer_step": (c_int32, [c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_float,

@@ -128,6 +128,8 @@ struct dib_model {
   bool varlen = false;
   const int32_t* set_sizes_dev = nullptr;
   long long dsum = 0;
+  // per-row sample weights of the following dib_forward / dib_train_step calls (dib_set_sample_weights_device), or null
+  const float* sample_weights_dev = nullptr;
   float ln_eps = 1e-3f;
   long long maxSets = 0;
   std::vector<int> ff_arch;
@@ -692,6 +694,7 @@ int forward_infonce(const Ctx& c, const float* y, bool training, float* user_pre
 int forward_integration(const Ctx& c, const float* y, float inv_batch, bool training, float* user_pred, float* out_stats,
                         int nblk_kl) {
   dib_model* h = c.h;
+  const float* weights = y ? h->sample_weights_dev : nullptr;
   auto finalize = [&](int nblk_loss) {
     return dib_launch_finalize_stats(c.ws + h->kl_part_off, h->kl_stride, nblk_kl, c.ws + h->loss_part_off, c.ws + h->acc_part_off,
                                      nblk_loss, h->F, c.n, y != nullptr, out_stats, c.st);
@@ -702,7 +705,7 @@ int forward_integration(const Ctx& c, const float* y, float inv_batch, bool trai
     prof_begin(c, "loss_stats");
     DIB_CUDA_OK(dib_launch_loss(h->loss, h->out_act, h->alpha, c.ws + h->pred.off, h->pred.ld, y, h->out, c.n, inv_batch,
                                 training ? c.ws + h->d_pred.off : nullptr, user_pred, c.ws + h->loss_part_off,
-                                c.ws + h->acc_part_off, is_tc(h) ? 1 : 0, c.st));
+                                c.ws + h->acc_part_off, is_tc(h) ? 1 : 0, weights, c.st));
     DIB_CUDA_OK(finalize((int)DIB_CEIL_DIV((long long)c.n, (long long)kRowsPerBlock)));
     prof_end(c);
     return 0;
@@ -741,7 +744,8 @@ int forward_integration(const Ctx& c, const float* y, float inv_batch, bool trai
                                     bwd ? (void*)(c.ws + h->dg16_off[j1]) : nullptr,
                                     bwd ? c.ws + h->dbpart_off + (long long)j1 * h->dbpart_layer : nullptr,
                                     bwd && j0 == 0 ? (void*)(c.ws + h->demb16_off) : nullptr, user_pred, c.ws + h->headpart_off,
-                                    h->head_stride, c.ws + h->loss_part_off, c.ws + h->acc_part_off, &h->head_used, bf, c.st));
+                                    h->head_stride, c.ws + h->loss_part_off, c.ws + h->acc_part_off, &h->head_used, weights, bf,
+                                    c.st));
     DIB_CUDA_OK(finalize(h->head_used));
     prof_end(c);
     return 0;
@@ -751,7 +755,8 @@ int forward_integration(const Ctx& c, const float* y, float inv_batch, bool trai
   prof_begin(c, "int16_head_loss");
   DIB_CUDA_OK(dib_int16_head(c.ws + h->g16_off[h->Li], Kh, Kh, c.params + h->intW[h->Li], c.params + h->intB[h->Li], h->out,
                              h->out_act, h->act, h->alpha, h->loss, y, c.n, inv_batch, gscale, dg, Kh, user_pred, c.ws + h->headpart_off,
-                             h->head_stride, c.ws + h->loss_part_off, c.ws + h->acc_part_off, h->head_blocks, h->route.head1, bf, c.st));
+                             h->head_stride, c.ws + h->loss_part_off, c.ws + h->acc_part_off, h->head_blocks, h->route.head1, weights,
+                             bf, c.st));
   DIB_CUDA_OK(finalize(h->head_blocks));
   prof_end(c);
   return 0;
@@ -1565,6 +1570,26 @@ int dib_set_set_sizes_device(dib_model* h, const int32_t* set_sizes_dev) {
   if (!h->varlen && set_sizes_dev) return fail("dib_set_set_sizes_device: the model was not created with variable_set_sizes");
   if (reinterpret_cast<uintptr_t>(set_sizes_dev) & 3) return fail("dib_set_set_sizes_device: sizes must be 4-byte aligned");
   h->set_sizes_dev = set_sizes_dev;
+  return 0;
+}
+
+// the fp32 sample weights of the n rows of the following dib_forward / dib_train_step calls, read by the loss kernels from
+// device memory (a captured graph reads whatever the buffer holds at replay); null: unweighted
+int dib_set_sample_weights_device(dib_model* h, const float* w_dev) {
+  if (!h) return fail("null model handle");
+  if (w_dev && (h->loss == DIB_LOSS_EXTERNAL || h->loss == DIB_LOSS_INFONCE))
+    return fail("dib_set_sample_weights_device: the external and InfoNCE losses take no sample weights");
+  if (reinterpret_cast<uintptr_t>(w_dev) & 3) return fail("dib_set_sample_weights_device: weights must be 4-byte aligned");
+  h->sample_weights_dev = w_dev;
+  return 0;
+}
+
+int dib_class_weight_rows(const float* y, int64_t n, int32_t y_cols, const float* class_table, int32_t classes,
+                          const float* sample_weight_or_null, float* out, void* stream) {
+  if (n < 0 || classes < 1 || y_cols < 0) return fail("dib_class_weight_rows: n >= 0, classes >= 1 and y_cols >= 0 are required");
+  if (n > 0 && (!y || !class_table || !out)) return fail("dib_class_weight_rows: null y / class_table / out");
+  DIB_CUDA_OK(dib_launch_class_weight_rows(y, n, y_cols, class_table, classes, sample_weight_or_null, out,
+                                           static_cast<cudaStream_t>(stream)));
   return 0;
 }
 

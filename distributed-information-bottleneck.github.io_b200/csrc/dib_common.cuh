@@ -64,6 +64,29 @@ __device__ __forceinline__ float dib_loss_add(int loss, float z, float t, float&
   return g;
 }
 
+// The same with the loss term weighted by the row's sample weight w (Keras SUM_OVER_BATCH_SIZE: sum_i w_i l_i / n); the
+// accuracy hit and d loss / d z stay unweighted (the callers weight d loss / d z through their 1/batch factor).  w enters
+// as the last factor of a product term (MSE: d * (d * w)), so that with w = 1 every sum contracts as in dib_loss_add and
+// all-ones weights give the unweighted bits.
+__device__ __forceinline__ float dib_loss_add_w(int loss, float z, float t, float w, float& l, float& acc) {
+  float g;
+  if (loss == DIB_LOSS_BCE_LOGITS) { l += (fmaxf(z, 0.f) - z * t + log1pf(expf(-fabsf(z)))) * w; g = 1.f / (1.f + expf(-z)) - t; }
+  else if (loss == DIB_LOSS_BCE_PROBS) {
+    const float ep = 1e-7f, pc = fminf(fmaxf(z, ep), 1.f - ep);
+    l -= (t * logf(pc + ep) + (1.f - t) * logf(1.f - pc + ep)) * w;
+    g = (z > ep && z < 1.f - ep) ? -t / (pc + ep) + (1.f - t) / (1.f - pc + ep) : 0.f;
+  } else { const float d = z - t; l += d * (d * w); g = 2.f * d; }
+  acc += ((z > 0.5f ? 1.f : 0.f) == t) ? 1.f : 0.f;
+  return g;
+}
+
+// dib_loss_add, weighted (W) or not: the one switch the loss epilogues of the WEIGHTED kernel instantiations go through
+template <bool W>
+__device__ __forceinline__ float dib_loss_add_t(int loss, float z, float t, float w, float& l, float& acc) {
+  if constexpr (W) return dib_loss_add_w(loss, z, t, w, l, acc);
+  else return dib_loss_add(loss, z, t, l, acc);
+}
+
 // ---------------------------------------------------------------------------------------------
 // Philox4x32-10 noise; contract documented in oracle/philox.py (the CPU restatement used by tests).
 // ---------------------------------------------------------------------------------------------

@@ -133,16 +133,19 @@ dib_reparam_bwd_kernel(DibReparamArgs a, const float* __restrict__ d_emb, int ld
 
 // ------------------------------------------------------------------------------------------------
 // compiled loss (Keras, data.py:65 / :343 / MSE), metrics=['accuracy'] (data.py:67) and d loss / d z_out.
-// One thread per row.
+// One thread per row.  WEIGHTED: row i's loss and d loss / d z carry its sample weight wts[i] (the accuracy does not).
 // ------------------------------------------------------------------------------------------------
+template <bool WEIGHTED>
 __global__ void __launch_bounds__(kRowsPerBlock)
 dib_loss_kernel(int loss, int out_act, float alpha, const float* __restrict__ pred, int ldp, const float* __restrict__ y,
                 int out_dim, long long n, float inv_batch, float* __restrict__ d_pred, float* __restrict__ user_pred,
-                float* __restrict__ loss_part, float* __restrict__ acc_part, int round_out) {
+                float* __restrict__ loss_part, float* __restrict__ acc_part, int round_out, const float* __restrict__ wts) {
   __shared__ float red[8];
   const long long row = (long long)blockIdx.x * kRowsPerBlock + threadIdx.x;
   float l = 0.f, acc = 0.f;
   if (row < n) {
+    float w = 1.f;
+    if constexpr (WEIGHTED) { w = wts[row]; inv_batch *= w; }
     const float* z = pred + row * ldp;
     float* dz = d_pred ? d_pred + row * ldp : nullptr;
     if (user_pred)
@@ -161,6 +164,7 @@ dib_loss_kernel(int loss, int out_act, float alpha, const float* __restrict__ pr
         float se = 0.f;
         for (int j = 0; j < out_dim; ++j) se += expf(z[j] - m);
         l = m + logf(se) - z[label];
+        if constexpr (WEIGHTED) l *= w;
         acc = (am == label) ? 1.f : 0.f;
         if (dz) {
           const float inv_se = 1.f / se;
@@ -173,7 +177,7 @@ dib_loss_kernel(int loss, int out_act, float alpha, const float* __restrict__ pr
         const float* yy = y + row * out_dim;
         for (int j = 0; j < out_dim; ++j) {
           const float zz = z[j];
-          const float g = dib_loss_add(loss, zz, yy[j], l, acc);
+          const float g = dib_loss_add_t<WEIGHTED>(loss, zz, yy[j], w, l, acc);
           if (dz) dz[j] = dib_maybe_round(g * inv_out * inv_batch * dib_act_grad(out_act, zz, alpha), round_out);
         }
         l *= inv_out;
@@ -432,11 +436,45 @@ cudaError_t dib_launch_reparam_bwd(const DibReparamArgs& a, const float* d_emb, 
 
 cudaError_t dib_launch_loss(int loss, int out_act, float alpha, const float* pred, int ldp, const float* y, int out_dim,
                             int64_t n, float inv_batch, float* d_pred, float* user_pred, float* loss_part,
-                            float* acc_part, int round_out, cudaStream_t st) {
+                            float* acc_part, int round_out, const float* weights, cudaStream_t st) {
   if (n <= 0) return cudaSuccess;
-  dib_loss_kernel<<<nblocks(n, kRowsPerBlock), kRowsPerBlock, 0, st>>>(loss, out_act, alpha, pred, ldp, y, out_dim, n,
-                                                                      inv_batch, d_pred, user_pred, loss_part, acc_part,
-                                                                      round_out);
+  if (weights)
+    dib_loss_kernel<true><<<nblocks(n, kRowsPerBlock), kRowsPerBlock, 0, st>>>(loss, out_act, alpha, pred, ldp, y, out_dim, n,
+                                                                              inv_batch, d_pred, user_pred, loss_part, acc_part,
+                                                                              round_out, weights);
+  else
+    dib_loss_kernel<false><<<nblocks(n, kRowsPerBlock), kRowsPerBlock, 0, st>>>(loss, out_act, alpha, pred, ldp, y, out_dim, n,
+                                                                               inv_batch, d_pred, user_pred, loss_part, acc_part,
+                                                                               round_out, nullptr);
+  dib_note_launch();
+  return cudaGetLastError();
+}
+
+// Keras' class_weight map (_make_class_weight_map_fn): the class of row i is argmax y[i, :] when y has more than one
+// column, else y[i] cast to an integer (truncating); out[i] = table[class] (NaN for a class outside [0, classes)), times
+// sample_weight[i] when given.  One thread per row.
+__global__ void dib_class_weight_rows_kernel(const float* __restrict__ y, long long n, int y_cols, const float* __restrict__ table,
+                                             int classes, const float* __restrict__ sw, float* __restrict__ out) {
+  const long long row = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (row >= n) return;
+  int c = -1;
+  if (y_cols > 1) {
+    const float* yr = y + row * y_cols;
+    float m = yr[0]; c = 0;
+    for (int j = 1; j < y_cols; ++j) if (yr[j] > m) { m = yr[j]; c = j; }
+  } else {
+    const float v = y[row];
+    if (v > -1.f && v < (float)classes) c = (int)v;           // truncation toward zero; NaN and out-of-range stay -1
+  }
+  float w = (c >= 0 && c < classes) ? table[c] : __int_as_float(0x7fc00000);
+  if (sw) w = sw[row] * w;
+  out[row] = w;
+}
+
+cudaError_t dib_launch_class_weight_rows(const float* y, int64_t n, int y_cols, const float* table, int classes, const float* sw,
+                                         float* out, cudaStream_t st) {
+  if (n <= 0) return cudaSuccess;
+  dib_class_weight_rows_kernel<<<nblocks(n, kRowsPerBlock), kRowsPerBlock, 0, st>>>(y, n, y_cols, table, classes, sw, out);
   dib_note_launch();
   return cudaGetLastError();
 }

@@ -301,15 +301,17 @@ struct Fwd2Args {
   float* dbpart;                      // with dg1: column sums of dg1 per 128-row tile [tiles][256]
   int demb_cols;                      // with dg1, > 0: the layer below is the embedding; d emb [M x demb_cols] via mapDemb
   const float* y; float* user_pred;
+  const float* wts;                   // WEIGHTED: the rows' sample weights
   float* wpart; int wpart_stride; float *loss_part, *acc_part;
   int M, nk0, act, out_act, loss;
   float alpha, inv_batch, gscale;
 };
 
 // ACT is a template parameter: the activation switch inside the fully unrolled register-resident passes would otherwise be
-// evaluated per element.
+// evaluated per element.  WEIGHTED: row i's loss and d loss / d logit carry its sample weight a.wts[i] (in e1's loss block,
+// before any 16-bit rounding); the unweighted instantiations do not read it.
 constexpr int kF2Threads = kConsumers + 128;      // + a producer warpgroup, so that setmaxnreg can move its registers to the consumers
-template <bool BF16, int ACT>
+template <bool BF16, int ACT, bool WEIGHTED>
 __global__ void __launch_bounds__(kF2Threads, 1)
 dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapW0,
                       const __grid_constant__ CUtensorMap mapW1, const __grid_constant__ CUtensorMap mapW1t,
@@ -498,16 +500,18 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
       const long long row = row_lo + 8 * h;
       const bool live = row < a.M;
       const float z = dib_act(a.out_act, zp[h] + bout, a.alpha);
-      float dz = 0.f;
+      float dz = 0.f, ib = a.inv_batch;
       if (live && a.y) {
         const float t = a.y[row];
+        float wr = 1.f;
+        if constexpr (WEIGHTED) { wr = a.wts[row]; ib *= wr; }
         float l = -0.f, acc1 = -0.f;
         if (a.loss == DIB_LOSS_SPARSE_CE_LOGITS) { l = 0.f; acc1 = (int)t == 0 ? 1.f : 0.f; }   // one class: the softmax is constant
-        else dz = dib_loss_add(a.loss, z, t, l, acc1);
+        else dz = dib_loss_add_t<WEIGHTED>(a.loss, z, t, wr, l, acc1);
         if (q == 0) { lsum += l; asum += acc1; }
       }
       if (a.user_pred && live && q == 0) a.user_pred[row] = z;
-      dzs[h] = live ? dz * a.inv_batch * dib_act_grad(a.out_act, z, a.alpha) : 0.f;
+      dzs[h] = live ? dz * ib * dib_act_grad(a.out_act, z, a.alpha) : 0.f;
       ds[h] = dzs[h] * a.gscale;
       if (q == 0) dbo += dzs[h];
     }
@@ -641,12 +645,14 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
 // ----------------------------------------------------------------------------------------------------
 constexpr int kHeadMaxOut = 16, kHeadWarps = 8;
 
-template <int KPT, int OUT, int ROWS, bool BF16>   // hidden units per lane (K / 32); bound of the output width; rows in flight per warp
+// WEIGHTED: row i's loss and d loss / d z carry its sample weight wts[i]
+template <int KPT, int OUT, int ROWS, bool BF16, bool WEIGHTED>   // hidden units per lane (K / 32); bound of the output width; rows in flight per warp
 __global__ void __launch_bounds__(kHeadWarps * 32)
 dib_int16_head_kernel(const uint16_t* __restrict__ g, int ldg, int K, const float* __restrict__ Wc, const float* __restrict__ bc,
                       int out_dim, int out_act, int hid_act, float alpha, int loss, const float* __restrict__ y, long long n,
                       float inv_batch, float gscale, uint16_t* __restrict__ dg, int lddg, float* __restrict__ user_pred,
-                      float* __restrict__ wpart, int wpart_stride, float* __restrict__ loss_part, float* __restrict__ acc_part) {
+                      float* __restrict__ wpart, int wpart_stride, float* __restrict__ loss_part, float* __restrict__ acc_part,
+                      const float* __restrict__ wts) {
   __shared__ float red[kHeadWarps][KPT * 32];
   __shared__ float sred[kHeadWarps];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -696,6 +702,8 @@ dib_int16_head_kernel(const uint16_t* __restrict__ g, int ldg, int K, const floa
         dz[o] = 0.f;
       }
       // ---- compiled loss / metric / d loss / d z  (identical on all lanes)
+      float wr = 1.f, ib = inv_batch;
+      if constexpr (WEIGHTED) { wr = wts[row]; ib *= wr; }
       if (y) {
         float l = 0.f, acc = 0.f;
         const float inv_out = 1.f / (float)out_dim;
@@ -707,13 +715,14 @@ dib_int16_head_kernel(const uint16_t* __restrict__ g, int ldg, int K, const floa
 #pragma unroll
           for (int o = 0; o < OUT; ++o) if (o < out_dim) { se += expf(z[o] - m); if (o == label) zl = z[o]; }
           l = m + logf(se) - zl;
+          if constexpr (WEIGHTED) l *= wr;
           acc = am == label ? 1.f : 0.f;
 #pragma unroll
           for (int o = 0; o < OUT; ++o) if (o < out_dim) dz[o] = expf(z[o] - m) / se - (o == label ? 1.f : 0.f);
         } else {
 #pragma unroll
           for (int o = 0; o < OUT; ++o) if (o < out_dim) {
-            dz[o] = dib_loss_add(loss, z[o], y[row * out_dim + o], l, acc) * inv_out;
+            dz[o] = dib_loss_add_t<WEIGHTED>(loss, z[o], y[row * out_dim + o], wr, l, acc) * inv_out;
           }
           l *= inv_out; acc *= inv_out;
         }
@@ -725,7 +734,7 @@ dib_int16_head_kernel(const uint16_t* __restrict__ g, int ldg, int K, const floa
       }
       if (train) {
 #pragma unroll
-        for (int o = 0; o < OUT; ++o) { dz[o] *= inv_batch * dib_act_grad(out_act, z[o], alpha); db[o] += dz[o]; }
+        for (int o = 0; o < OUT; ++o) { dz[o] *= ib * dib_act_grad(out_act, z[o], alpha); db[o] += dz[o]; }
         float d[KPT];
 #pragma unroll
         for (int i = 0; i < KPT; ++i) {
@@ -803,12 +812,13 @@ dib_int16_head_kernel(const uint16_t* __restrict__ g, int ldg, int K, const floa
 // instead of 40), after which lane L holds the logit of row L & 7 and the loss / metric / d loss / d z arithmetic runs once
 // per pass, lane-parallel, instead of once per row on every lane (ncu: the generic kernel was issue-bound at 45 %).
 // ----------------------------------------------------------------------------------------------------
-template <bool BF16>
+template <bool BF16, bool WEIGHTED>       // WEIGHTED: as the generic kernel
 __global__ void __launch_bounds__(kHeadWarps * 32)
 dib_int16_head1_kernel(const uint16_t* __restrict__ g, int ldg, int K, const float* __restrict__ Wc, const float* __restrict__ bc,
                        int out_act, int hid_act, float alpha, int loss, const float* __restrict__ y, long long n,
                        float inv_batch, float gscale, uint16_t* __restrict__ dg, int lddg, float* __restrict__ user_pred,
-                       float* __restrict__ wpart, int wpart_stride, float* __restrict__ loss_part, float* __restrict__ acc_part) {
+                       float* __restrict__ wpart, int wpart_stride, float* __restrict__ loss_part, float* __restrict__ acc_part,
+                       const float* __restrict__ wts) {
   constexpr int KPT = 8, ROWS = 8;
   __shared__ float red[kHeadWarps][KPT * 32];
   __shared__ float sred[kHeadWarps];
@@ -852,17 +862,19 @@ dib_int16_head1_kernel(const uint16_t* __restrict__ g, int ldg, int K, const flo
     const long long mrow = row0 + myr;
     const bool live = mrow < n;
     z = dib_act(out_act, z + bias, alpha);
-    float dz = 0.f;
+    float dz = 0.f, ib = inv_batch;
     if (live && y) {
       const float t = y[mrow];
+      float wr = 1.f;
+      if constexpr (WEIGHTED) { wr = wts[mrow]; ib *= wr; }
       float l = -0.f, acc = -0.f;
       if (loss == DIB_LOSS_SPARSE_CE_LOGITS) { l = 0.f; acc = (int)t == 0 ? 1.f : 0.f; }        // one class: the softmax is constant
-      else dz = dib_loss_add(loss, z, t, l, acc);
+      else dz = dib_loss_add_t<WEIGHTED>(loss, z, t, wr, l, acc);
       if (lane < ROWS) { lsum += l; asum += acc; }
     }
     if (user_pred && live && lane < ROWS) user_pred[mrow] = z;
     if (train) {
-      dz = live ? dz * inv_batch * dib_act_grad(out_act, z, alpha) : 0.f;
+      dz = live ? dz * ib * dib_act_grad(out_act, z, alpha) : 0.f;
       if (lane < ROWS) db += dz;
 #pragma unroll
       for (int rr = 0; rr < ROWS; ++rr) {
@@ -1077,7 +1089,8 @@ bool dib_int16_fwd2_ok(int K0, int N1, int N2, int out_dim) {
 cudaError_t dib_int16_fwd2_head(const void* g_in, int ld_in, int K0, const void* w16_0, const float* b0, const void* w16_1, const float* b1,
                                 void* g1, const float* wout, const float* bout, int act, int out_act, float alpha, int loss, const float* y,
                                 int M, float inv_batch, float gscale, void* dg2, void* dg1, float* dbpart, void* demb, float* user_pred,
-                                float* wpart, int wpart_stride, float* loss_part, float* acc_part, int* nblocks, int bf16, cudaStream_t st) {
+                                float* wpart, int wpart_stride, float* loss_part, float* acc_part, int* nblocks, const float* weights,
+                                int bf16, cudaStream_t st) {
   if (!encode_fn3()) return cudaErrorNotSupported;
   if ((dg1 && (!dg2 || !dbpart)) || (demb && !dg1)) return cudaErrorInvalidValue;
   CUtensorMap mA, mW0, mW1;
@@ -1091,7 +1104,7 @@ cudaError_t dib_int16_fwd2_head(const void* g_in, int ld_in, int K0, const void*
   if (demb && (!map_k(&mW0t, w16_0, kF2N, K0, kF2N, kF2BtN) || !map_k(&mDemb, demb, K0, M, K0, 64))) return cudaErrorInvalidValue;
   Fwd2Args a{};
   a.b0 = b0; a.b1 = b1; a.wout = wout; a.bout = bout;
-  a.dg2 = static_cast<uint16_t*>(dg2); a.lddg = kF2N; a.y = y; a.user_pred = user_pred; a.wpart = wpart; a.wpart_stride = wpart_stride;
+  a.dg2 = static_cast<uint16_t*>(dg2); a.lddg = kF2N; a.y = y; a.user_pred = user_pred; a.wts = weights; a.wpart = wpart; a.wpart_stride = wpart_stride;
   a.bwd = dg1 != nullptr; a.dbpart = dbpart; a.demb_cols = demb ? K0 : 0;
   a.loss_part = loss_part; a.acc_part = acc_part; a.M = M; a.nk0 = K0 / kBK; a.act = act; a.out_act = out_act; a.loss = loss;
   a.alpha = alpha; a.inv_batch = inv_batch; a.gscale = gscale;
@@ -1100,15 +1113,16 @@ cudaError_t dib_int16_fwd2_head(const void* g_in, int ld_in, int K0, const void*
   *nblocks = grid;
   if (grid <= 0) return cudaSuccess;
   cudaError_t e = cudaErrorInvalidValue;
-#define DIB_F2_LAUNCH(BF, ACT)                                                                                                       \
+#define DIB_F2_LAUNCH(BF, ACT, W)                                                                                                    \
   do {                                                                                                                               \
     static bool attr = false;                                                                                                        \
-    e = attr ? cudaSuccess : cudaFuncSetAttribute(dib_int16_fwd2_kernel<BF, ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, kF2Smem); \
+    e = attr ? cudaSuccess : cudaFuncSetAttribute(dib_int16_fwd2_kernel<BF, ACT, W>, cudaFuncAttributeMaxDynamicSharedMemorySize, kF2Smem); \
     if (e != cudaSuccess) return e;                                                                                                  \
     attr = true;                                                                                                                     \
-    dib_int16_fwd2_kernel<BF, ACT><<<grid, kF2Threads, kF2Smem, st>>>(mA, mW0, mW1, mW1t, mW0t, mDemb, mG1, mDg1, a);               \
+    dib_int16_fwd2_kernel<BF, ACT, W><<<grid, kF2Threads, kF2Smem, st>>>(mA, mW0, mW1, mW1t, mW0t, mDemb, mG1, mDg1, a);            \
   } while (0)
-#define DIB_F2_ACT(ACT) do { if (bf16) DIB_F2_LAUNCH(true, ACT); else DIB_F2_LAUNCH(false, ACT); } while (0)
+#define DIB_F2_BF(ACT, W) do { if (bf16) DIB_F2_LAUNCH(true, ACT, W); else DIB_F2_LAUNCH(false, ACT, W); } while (0)
+#define DIB_F2_ACT(ACT) do { if (weights) DIB_F2_BF(ACT, true); else DIB_F2_BF(ACT, false); } while (0)
   switch (act) {
     case DIB_ACT_LINEAR: DIB_F2_ACT(DIB_ACT_LINEAR); break;
     case DIB_ACT_RELU: DIB_F2_ACT(DIB_ACT_RELU); break;
@@ -1119,6 +1133,7 @@ cudaError_t dib_int16_fwd2_head(const void* g_in, int ld_in, int K0, const void*
     default: return cudaErrorInvalidValue;
   }
 #undef DIB_F2_ACT
+#undef DIB_F2_BF
 #undef DIB_F2_LAUNCH
   dib_note_launch();
   return cudaGetLastError();
@@ -1129,24 +1144,28 @@ int dib_int16_head_blocks(int num_sms) { return num_sms * 2; }
 cudaError_t dib_int16_head(const void* g, int ldg, int K, const float* Wc, const float* bc, int out_dim, int out_act, int hid_act,
                            float alpha, int loss, const float* y, long long n, float inv_batch, float gscale, void* dg, int lddg,
                            float* user_pred, float* wpart, int wpart_stride, float* loss_part, float* acc_part, int nblocks,
-                           bool head1, int bf16, cudaStream_t st) {
+                           bool head1, const float* weights, int bf16, cudaStream_t st) {
   if (out_dim > kHeadMaxOut || out_dim < 1 || K != 256 || (head1 && out_dim != 1)) return cudaErrorInvalidValue;
-#define DIB_HEAD_T(OUT, BF)                                                                                             \
-  dib_int16_head_kernel<8, OUT, (OUT <= 2 ? 4 : 1), BF><<<nblocks, kHeadWarps * 32, 0, st>>>(static_cast<const uint16_t*>(g), ldg, K, Wc, bc, out_dim,  \
+#define DIB_HEAD_T(OUT, BF, W)                                                                                          \
+  dib_int16_head_kernel<8, OUT, (OUT <= 2 ? 4 : 1), BF, W><<<nblocks, kHeadWarps * 32, 0, st>>>(static_cast<const uint16_t*>(g), ldg, K, Wc, bc, out_dim,  \
       out_act, hid_act, alpha, loss, y, n, inv_batch, gscale, static_cast<uint16_t*>(dg), lddg, user_pred, wpart, wpart_stride, \
-      loss_part, acc_part)
-#define DIB_HEAD(OUT) do { if (bf16) DIB_HEAD_T(OUT, true); else DIB_HEAD_T(OUT, false); } while (0)
+      loss_part, acc_part, weights)
+#define DIB_HEAD_W(OUT, W) do { if (bf16) DIB_HEAD_T(OUT, true, W); else DIB_HEAD_T(OUT, false, W); } while (0)
+#define DIB_HEAD(OUT) do { if (weights) DIB_HEAD_W(OUT, true); else DIB_HEAD_W(OUT, false); } while (0)
+#define DIB_HEAD1(BF, W)                                                                                                \
+  dib_int16_head1_kernel<BF, W><<<nblocks, kHeadWarps * 32, 0, st>>>(static_cast<const uint16_t*>(g), ldg, K, Wc, bc, out_act, hid_act,  \
+      alpha, loss, y, n, inv_batch, gscale, static_cast<uint16_t*>(dg), lddg, user_pred, wpart, wpart_stride, loss_part, acc_part, weights)
   if (head1) {
-    if (bf16) dib_int16_head1_kernel<true><<<nblocks, kHeadWarps * 32, 0, st>>>(static_cast<const uint16_t*>(g), ldg, K, Wc, bc, out_act,
-        hid_act, alpha, loss, y, n, inv_batch, gscale, static_cast<uint16_t*>(dg), lddg, user_pred, wpart, wpart_stride, loss_part, acc_part);
-    else dib_int16_head1_kernel<false><<<nblocks, kHeadWarps * 32, 0, st>>>(static_cast<const uint16_t*>(g), ldg, K, Wc, bc, out_act,
-        hid_act, alpha, loss, y, n, inv_batch, gscale, static_cast<uint16_t*>(dg), lddg, user_pred, wpart, wpart_stride, loss_part, acc_part);
+    if (bf16) { if (weights) DIB_HEAD1(true, true); else DIB_HEAD1(true, false); }
+    else { if (weights) DIB_HEAD1(false, true); else DIB_HEAD1(false, false); }
   } else if (out_dim == 1) DIB_HEAD(1);
   else if (out_dim == 2) DIB_HEAD(2);
   else if (out_dim <= 4) DIB_HEAD(4);
   else if (out_dim <= 8) DIB_HEAD(8);
   else DIB_HEAD(16);
+#undef DIB_HEAD1
 #undef DIB_HEAD
+#undef DIB_HEAD_W
 #undef DIB_HEAD_T
   dib_note_launch();
   return cudaGetLastError();

@@ -59,10 +59,13 @@ cudaError_t dib_launch_reparam_fwd(const DibReparamArgs& a, float* emb, int ldem
 cudaError_t dib_launch_reparam_bwd(const DibReparamArgs& a, const float* d_emb, int ldemb, const float* beta_dev,
                                    float inv_batch, float* d_out, cudaStream_t st);
 
-// compiled loss + metrics=['accuracy'] + d(loss)/d(pre-activation output).
+// compiled loss + metrics=['accuracy'] + d(loss)/d(pre-activation output); weights: the n rows' sample weights or null.
 cudaError_t dib_launch_loss(int loss, int out_act, float alpha, const float* pred, int ldp, const float* y, int out_dim,
                             int64_t n, float inv_batch, float* d_pred /*nullable*/, float* user_pred /*nullable*/,
-                            float* loss_part, float* acc_part, int round_out, cudaStream_t st);
+                            float* loss_part, float* acc_part, int round_out, const float* weights /*nullable*/, cudaStream_t st);
+// Keras' class_weight map of n rows: out[i] = table[class of y row i] (* sw[i]); see dib_class_weight_rows
+cudaError_t dib_launch_class_weight_rows(const float* y, int64_t n, int y_cols, const float* table, int classes, const float* sw,
+                                         float* out, cudaStream_t st);
 
 cudaError_t dib_launch_round_copy(const float* src, float* dst, int64_t count, cudaStream_t st);
 
@@ -200,12 +203,13 @@ bool dib_int16_fwd2_ok(int K0, int N1, int N2, int out_dim);
 cudaError_t dib_int16_fwd2_head(const void* g_in, int ld_in, int K0, const void* w16_0, const float* b0, const void* w16_1, const float* b1,
                                 void* g1, const float* wout, const float* bout, int act, int out_act, float alpha, int loss, const float* y,
                                 int M, float inv_batch, float gscale, void* dg2, void* dg1, float* dbpart, void* demb, float* user_pred,
-                                float* wpart, int wpart_stride, float* loss_part, float* acc_part, int* nblocks, int bf16, cudaStream_t st);
+                                float* wpart, int wpart_stride, float* loss_part, float* acc_part, int* nblocks, const float* weights,
+                                int bf16, cudaStream_t st);
 // head1: the out = 1 kernel (8 rows per pass) instead of the generic one
 cudaError_t dib_int16_head(const void* g, int ldg, int K, const float* Wc, const float* bc, int out_dim, int out_act, int hid_act,
                            float alpha, int loss, const float* y, long long n, float inv_batch, float gscale, void* dg, int lddg,
                            float* user_pred, float* wpart, int wpart_stride, float* loss_part, float* acc_part, int nblocks,
-                           bool head1, int bf16, cudaStream_t st);
+                           bool head1, const float* weights, int bf16, cudaStream_t st);
 
 // ---- the set-attention integration network (dib_set_attn.cu; integration_kind 1) ----
 // attention core of one block: q, k, v, o (and dout, dq, dk, dv) are [sets * L, heads * dk] with leading dimension ld; lse

@@ -53,6 +53,72 @@ def _shard_rows(order, b0, b1, rank, world):
     return (order[b0 + lo:b0 + hi] if order is not None else slice(b0 + lo, b0 + hi)), lo
 
 
+def check_sample_weights(w, n, what="sample_weight"):
+    """Host check of the per-sample weights of n rows (sets, for a set transformer): [n] or [n, 1], finite and >= 0.  Returns
+    them as a float32 array [n]."""
+    a = np.asarray(w)
+    if a.dtype.kind not in "biuf":
+        raise ValueError(f"{what} must be numeric, got {a.dtype}")
+    if a.shape not in ((int(n),), (int(n), 1)):
+        raise ValueError(f"{what} has shape {a.shape}; expected one weight per sample, ({int(n)},) or ({int(n)}, 1)")
+    a = a.reshape(-1).astype(np.float32)
+    if not np.all(np.isfinite(a)) or (a.size and a.min() < 0):
+        raise ValueError(f"{what} must be finite and >= 0")
+    return a
+
+
+def check_class_weight(class_weight):
+    """[KERAS] ``_make_class_weight_map_fn``: a dict whose keys are exactly 0..C-1.  Returns the float32 table [C]."""
+    if not isinstance(class_weight, dict) or not class_weight:
+        raise ValueError("class_weight must be a non-empty dict {class index: weight}")
+    keys = sorted(class_weight.keys())
+    if keys != list(range(len(keys))):
+        raise ValueError(f"Expected `class_weight` to be a dict with keys from 0 to one less than the number of classes, "
+                         f"found {class_weight}")
+    table = np.asarray([float(class_weight[k]) for k in keys], dtype=np.float32)
+    if not np.all(np.isfinite(table)) or table.min() < 0:
+        raise ValueError("class_weight values must be finite and >= 0")
+    return table
+
+
+def class_weight_classes(y):
+    """[KERAS] the class of each row in ``_make_class_weight_map_fn``: argmax over the columns of y [n, k > 1], otherwise y
+    reshaped to [n] and cast to an integer, truncating (float labels 1.7 -> 1).  Non-finite labels map to -1."""
+    a = np.asarray(y)
+    if a.ndim > 2:
+        raise ValueError("class_weight is not supported for 3+ dimensional targets")
+    if a.ndim == 2 and a.shape[1] > 1:
+        return a.argmax(axis=1).astype(np.int64)
+    v = a.reshape(-1).astype(np.float64)
+    return np.where(np.isfinite(v), np.trunc(np.where(np.isfinite(v), v, 0.0)), -1).astype(np.int64)
+
+
+def class_weight_rows(y, class_weight, sample_weight=None):
+    """Host statement of the row weights ``fit(..., class_weight=, sample_weight=)`` trains with (dib_class_weight_rows
+    computes them on the device): table[class of row i], times sample_weight[i] when given, in float32.  Labels outside
+    0..C-1 raise ValueError."""
+    table = check_class_weight(class_weight)
+    cls = class_weight_classes(y)
+    bad = (cls < 0) | (cls >= table.size)
+    if bad.any():
+        raise ValueError(f"class_weight: label {np.asarray(y).reshape(len(cls), -1)[bad][0].tolist()} of row "
+                         f"{int(np.flatnonzero(bad)[0])} has no class in 0..{table.size - 1}")
+    w = table[cls]
+    if sample_weight is not None:
+        w = check_sample_weights(sample_weight, len(cls)) * w
+    return w
+
+
+def check_weighted_loss(loss_kind, output_dimensionality, class_weight=False):
+    """Refuse sample / class weights where the compiled loss cannot take them: losses.InfoNCE and the external loss (the
+    caller owns the loss), and class_weight with MSE or a multi-output BCE (no class label to map)."""
+    if loss_kind in ("infonce", "external"):
+        raise ValueError(f"the {loss_kind!r} loss takes no sample_weight / class_weight")
+    if class_weight and (loss_kind == "mse" or (loss_kind != "sparse_ce_logits" and int(output_dimensionality) != 1)):
+        raise ValueError("class_weight needs a class label per row: sparse categorical cross-entropy, or binary "
+                         f"cross-entropy with one output (compiled loss {loss_kind!r}, {int(output_dimensionality)} outputs)")
+
+
 class PositionalEncoding:
     """models.py:12-23.  Kept for API parity; inside DistributedIBNet the encoding is fused into the first-layer
     operand by the library.  Calling it directly is a convenience (plain torch ops, not the hot path)."""
@@ -526,11 +592,45 @@ class DistributedIBNet:
         if sizes is not None:
             _lib.check(self._lib.dib_set_set_sizes_device(self._handle, _lib.ptr(sizes)))
 
+    def _bind_sample_weights(self, weights):
+        """Point the handle at the fp32 device weights of the rows of the following library calls (None: unweighted)."""
+        _lib.check(self._lib.dib_set_sample_weights_device(self._handle, _lib.ptr(weights)))
+
+    def _sample_weights(self, sample_weight, n, what="sample_weight"):
+        """sample_weight checked on the host (one read of a device tensor), then as float32 [n] on the device; None stays
+        None."""
+        if sample_weight is None:
+            return None
+        check_weighted_loss(self._loss_kind, self.output_dimensionality)
+        t = sample_weight if isinstance(sample_weight, torch.Tensor) else None
+        host = check_sample_weights(t.detach().cpu().numpy() if t is not None else sample_weight, n, what)
+        if t is not None:
+            return t.to(device=self.device, dtype=torch.float32).reshape(-1).contiguous()
+        return torch.from_numpy(host).to(self.device)
+
+    def _row_weights(self, y, yd, sample_weight, class_weight, n):
+        """The training weights of n rows: sample_weight, or with class_weight the Keras class map of y (labels checked on
+        the host, the rows mapped on the device by dib_class_weight_rows) times sample_weight.  None when neither is given."""
+        wd = self._sample_weights(sample_weight, n)
+        if class_weight is None:
+            return wd
+        check_weighted_loss(self._loss_kind, self.output_dimensionality, class_weight=True)
+        yh = y.detach().cpu().numpy() if isinstance(y, torch.Tensor) else np.asarray(y)
+        table = check_class_weight(class_weight)
+        class_weight_rows(yh, class_weight)                     # the label check, before any device work
+        td = torch.from_numpy(table).to(self.device)
+        out = torch.empty(n, dtype=torch.float32, device=self.device)
+        _lib.check(self._lib.dib_class_weight_rows(_lib.ptr(yd), n, yd.shape[1] if yd.dim() == 2 else 0, _lib.ptr(td),
+                                                   table.size, _lib.ptr(wd), _lib.ptr(out), _stream()))
+        return out
+
     # ------------------------------------------------------------------ compute entry points
-    def _forward(self, x, y, eps, step, sample_offset, want_pred=True, want_emb=False, stats_out=None, sizes=None):
+    def _forward(self, x, y, eps, step, sample_offset, want_pred=True, want_emb=False, stats_out=None, sizes=None,
+                 weights=None):
         n = x.shape[0]
         self._ensure_handle(n)
         self._bind_set_sizes(sizes)
+        self._bind_sample_weights(weights)
         pred = torch.empty(n, self.output_dimensionality, dtype=torch.float32, device=self.device) if want_pred else None
         emb = torch.empty(n, self.number_features * self.feature_embedding_dimension, dtype=torch.float32,
                           device=self.device) if want_emb else None
@@ -600,7 +700,7 @@ class DistributedIBNet:
         self._step_dev_active = on
 
     def _step_phases(self, x, y, global_batch, eps, sample_offset, step, device_step=False, training=True, stats=None,
-                     sizes=None):
+                     sizes=None, weights=None):
         """The train step of one batch as an ordered list of (launch, exchange): ``exchange`` is the collective that has to
         follow ``launch`` -- the all-gather of e_all or lse_all, or the all-reduce of self._gradstats = [grads (P) || stats
         (F+3)] -- and None where there is none, which is everywhere with one process.  ``step`` is the Philox step word.
@@ -609,7 +709,8 @@ class DistributedIBNet:
         dib_train_step into its three shard phases with the two all-gathers between them (DESIGN.md section 7).  With
         ``device_step`` (graph capture) the optimizer phase also advances the device noise step; ``training`` and ``stats``
         (default the stats of self._gradstats) go to the InfoNCE shard forward and lse; ``sizes`` are the set sizes of a
-        variable-size set transformer, bound to the handle right before its train step."""
+        variable-size set transformer, and ``weights`` the rows' sample weights (or None), bound to the handle right before
+        its train step."""
         n, P, group = x.shape[0], self._P, self.process_group
         self._ensure_handle(n)
         world, rank = parallel.world_and_rank(group)
@@ -633,6 +734,7 @@ class DistributedIBNet:
         else:
             def train_step():
                 self._bind_set_sizes(sizes)
+                self._bind_sample_weights(weights)
                 _lib.check(self._lib.dib_train_step(
                     self._handle, _lib.ptr(self._params), _lib.ptr(x), _lib.ptr(y), n, _lib.ptr(self.beta._dev),
                     1.0 / float(global_batch), _lib.ptr(eps), self.noise_seed, int(step) & 0xFFFFFFFF,
@@ -641,11 +743,11 @@ class DistributedIBNet:
             phases = [(train_step, reduce)]
         return phases + [(update, None)]
 
-    def _backward(self, x, y, global_batch, eps=None, sample_offset=0, step=None, device_step=False, sizes=None):
+    def _backward(self, x, y, global_batch, eps=None, sample_offset=0, step=None, device_step=False, sizes=None, weights=None):
         """Forward + reverse mode into self._gradstats = [grads (P) || stats (F+3)] of this rank: the step's phases up to
         the all-reduce."""
         st = 0 if device_step else (self._train_step_count if step is None else step)
-        phases = self._step_phases(x, y, global_batch, eps, sample_offset, st, device_step, sizes=sizes)
+        phases = self._step_phases(x, y, global_batch, eps, sample_offset, st, device_step, sizes=sizes, weights=weights)
         self._set_device_step(device_step)
         _run_phases(phases[:-1], last_exchange=False)
 
@@ -723,21 +825,22 @@ class DistributedIBNet:
     def _adam(self):
         self._optimizer_update(self._gradstats)
 
-    def _train_step(self, x, y, global_batch, eps=None, sample_offset=0, sizes=None):
+    def _train_step(self, x, y, global_batch, eps=None, sample_offset=0, sizes=None, weights=None):
         """backward, one flat all-reduce of [grads || stats] over the data-parallel group, Keras-Adam.  Replayed from
-        CUDA graphs once a (batch size, offset) combination has run eagerly twice; the set sizes of a variable-size set
-        transformer are data, not part of that key."""
+        CUDA graphs once a (batch size, offset, weighted or not) combination has run eagerly twice; the set sizes of a
+        variable-size set transformer and the sample weights are data, not part of that key."""
         P = self._P
         world, _ = parallel.world_and_rank(self.process_group)
-        key = (int(x.shape[0]), int(global_batch), int(sample_offset), world)
+        key = (int(x.shape[0]), int(global_batch), int(sample_offset), world, weights is not None)
         if self.use_cuda_graph and not self._graph_failed and eps is None and x.shape[0] > 0:
             g = self._graphs.get(key)
             if g is None and self._graph_seen.get(key, 0) >= 2:
                 g = self._capture_step(key, with_sizes=sizes is not None)
             if g is not None:
-                return self._replay_step(g, x, y, sizes)
+                return self._replay_step(g, x, y, sizes, weights)
             self._graph_seen[key] = self._graph_seen.get(key, 0) + 1
-        phases = self._step_phases(x, y, global_batch, eps, sample_offset, self._train_step_count, sizes=sizes)
+        phases = self._step_phases(x, y, global_batch, eps, sample_offset, self._train_step_count, sizes=sizes,
+                                   weights=weights)
         self._set_device_step(False)
         _run_phases(phases)
         self._train_step_count += 1
@@ -746,13 +849,13 @@ class DistributedIBNet:
 
     # ------------------------------------------------------------------ CUDA-graph replay of the step
     def _capture_step(self, key, with_sizes=False):
-        """Capture the step for one (n, global_batch, sample_offset, world) into CUDA graphs: one graph per run of phases
+        """Capture the step for one (n, global_batch, sample_offset, world, weighted) into CUDA graphs: one graph per run of phases
         between two collectives, each kept with the exchange that follows it.  Single GPU: ONE graph (forward + backward +
         optimizer + noise-step increment); plain data parallel: two (backward | optimizer); InfoNCE with global negatives: four
         (the three shard phases | optimizer), e_all / lse_all kept with the graphs.  Inputs are copied into static buffers
-        before each replay (and, ``with_sizes``, the set sizes into a third one); beta, learning rate, the optimizer step and
+        before each replay (and, ``with_sizes``, the set sizes into a third one; weighted, the sample weights into a fourth); beta, learning rate, the optimizer step and
         the Philox step are device scalars, so nothing by-value changes between replays."""
-        n, global_batch, sample_offset, world = key
+        n, global_batch, sample_offset, world, weighted = key
         D = sum(self.feature_dimensionalities)
         yc = self._y_cols()
         try:
@@ -760,7 +863,9 @@ class DistributedIBNet:
                 gx = torch.zeros(n, D, dtype=torch.float32, device=self.device)
                 gy = torch.zeros((n, yc) if yc > 0 else (n,), dtype=torch.float32, device=self.device)
                 gs = torch.ones(n, dtype=torch.int32, device=self.device) if with_sizes else None
-                phases = self._step_phases(gx, gy, global_batch, None, sample_offset, 0, device_step=True, sizes=gs)
+                gw = torch.ones(n, dtype=torch.float32, device=self.device) if weighted else None
+                phases = self._step_phases(gx, gy, global_batch, None, sample_offset, 0, device_step=True, sizes=gs,
+                                           weights=gw)
                 self._set_device_step(True)
                 torch.cuda.synchronize(self.device)
                 keep = [t.clone() for t in (self._params, self._m, self._v, self._step_dev, self._noise_step_dev)]
@@ -793,11 +898,11 @@ class DistributedIBNet:
             self._graph_failed = True
             self._set_device_step(False)
             return None
-        g = dict(graphs=graphs, x=gx, y=gy, sizes=gs, launches=int(self._lib.dib_launch_count()) - launches0)
+        g = dict(graphs=graphs, x=gx, y=gy, sizes=gs, weights=gw, launches=int(self._lib.dib_launch_count()) - launches0)
         self._graphs[key] = g
         return g
 
-    def _replay_step(self, g, x, y, sizes=None):
+    def _replay_step(self, g, x, y, sizes=None, weights=None):
         P = self._P
         if not self._step_dev_active or self._step_dev_dirty:
             self._set_device_step(True)
@@ -806,6 +911,8 @@ class DistributedIBNet:
         g["y"].copy_(y.reshape(g["y"].shape), non_blocking=True)
         if g["sizes"] is not None:
             g["sizes"].copy_(sizes, non_blocking=True)
+        if g["weights"] is not None:
+            g["weights"].copy_(weights, non_blocking=True)
         for graph, exchange in g["graphs"]:
             graph.replay()
             if exchange is not None:
@@ -813,17 +920,19 @@ class DistributedIBNet:
         self._train_step_count += 1
         return self._gradstats[P:]
 
-    def compute_gradients(self, x, y, eps=None, global_batch=None, sample_offset=0, step=None):
+    def compute_gradients(self, x, y, eps=None, global_batch=None, sample_offset=0, step=None, sample_weight=None):
         """GradientTape-style access (nb-bool cell 6 / train.py:201-220 custom loops): returns
-        (flat gradient of task + beta*sum KL w.r.t. trainable_variables, statistics vector) as device tensors."""
+        (flat gradient of task + beta*sum KL w.r.t. trainable_variables, statistics vector) as device tensors.
+        ``sample_weight`` [n] weights each row's task loss (Keras SUM_OVER_BATCH_SIZE: sum_i w_i l_i / global_batch)."""
         with torch.cuda.device(self.device):
             xd, sd = self._inputs(x)
             yd = self._targets(y)
+            wd = self._sample_weights(sample_weight, xd.shape[0])
             e = self._to_device(eps) if eps is not None else None
             if not global_batch:            # InfoNCE on several ranks: every rank passes its equal shard of the global batch
                 nce_world = parallel.world_and_rank(self.process_group)[0] if self._infonce is not None else 1
                 global_batch = max(xd.shape[0] * nce_world, 1)
-            self._backward(xd, yd, global_batch, e, sample_offset, step, sizes=sd)
+            self._backward(xd, yd, global_batch, e, sample_offset, step, sizes=sd, weights=wd)
             return self._gradstats[:self._P].clone(), self._gradstats[self._P:].clone()
 
     # ------------------------------------------------------------------ encoder-only custom steps (SURVEY 8f3)
@@ -953,8 +1062,9 @@ class DistributedIBNet:
             self._lr_dev.fill_(lr)
             self._lr_host = lr
 
-    def train_on_batch(self, x, y, return_dict=True, sync=True):
-        """One optimizer step on a (host or device) batch.
+    def train_on_batch(self, x, y, sample_weight=None, class_weight=None, return_dict=True, sync=True):
+        """One optimizer step on a (host or device) batch; ``sample_weight`` / ``class_weight`` weight the rows' task loss
+        as in :meth:`fit`.
 
         ``sync=True`` (Keras behaviour): returns the batch metrics (dict, or the scalar loss) -- forces the D2H read.
         ``sync=False``: returns a :class:`PendingBatchResult`; host batches are staged through a copy stream with two
@@ -970,12 +1080,20 @@ class DistributedIBNet:
             if sync or not host_x or self.variable_set_sizes:      # sized sets are not staged through the copy stream
                 (xd, sd), yd = self._inputs(x), self._targets(y)
                 n = xd.shape[0]
-                stats = self._train_step(xd, yd, global_batch=n * world, sample_offset=rank * n, sizes=sd)
+                wd = self._row_weights(y, yd, sample_weight, class_weight, n)
+                stats = self._train_step(xd, yd, global_batch=n * world, sample_offset=rank * n, sizes=sd, weights=wd)
                 res = PendingBatchResult(self, stats.detach().clone() if not sync else stats, None, None)
             else:
-                xd, yd, slot = self._stage_async(x, y, D)
+                w = None
+                if sample_weight is not None or class_weight is not None:      # checked and mapped on the host, staged as x, y
+                    n = len(x)
+                    check_weighted_loss(self._loss_kind, self.output_dimensionality, class_weight is not None)
+                    w = (class_weight_rows(np.asarray(y), class_weight, sample_weight) if class_weight is not None
+                         else check_sample_weights(sample_weight.detach().cpu().numpy()
+                                                   if isinstance(sample_weight, torch.Tensor) else sample_weight, n))
+                xd, yd, wd, slot = self._stage_async(x, y, D, w)
                 n = xd.shape[0]
-                stats = self._train_step(xd, yd, global_batch=n * world, sample_offset=rank * n)
+                stats = self._train_step(xd, yd, global_batch=n * world, sample_offset=rank * n, weights=wd)
                 st = self._staging
                 st["done"][slot].record(torch.cuda.current_stream())          # slot may be overwritten after this
                 hi = (st["k"] - 1) % len(st["stats_host"])
@@ -992,8 +1110,9 @@ class DistributedIBNet:
         out = res.get()
         return out if return_dict else out["loss"]
 
-    def _stage_async(self, x, y, D):
-        """H2D of a host batch on the copy stream into one of two device slots; the compute stream waits on it."""
+    def _stage_async(self, x, y, D, w=None):
+        """H2D of a host batch (and its float32 row weights w, or None) on the copy stream into one of two device slots; the
+        compute stream waits on it."""
         xt = x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32))
         yt = y if isinstance(y, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(y, dtype=np.float32))
         n, yc = xt.shape[0], self._y_cols()
@@ -1002,6 +1121,7 @@ class DistributedIBNet:
             st = dict(n=n, k=0, stream=torch.cuda.Stream(device=self.device),
                       x=[torch.empty(n, D, dtype=torch.float32, device=self.device) for _ in range(2)],
                       y=[torch.empty((n, yc) if yc > 0 else (n,), dtype=torch.float32, device=self.device) for _ in range(2)],
+                      w=[torch.empty(n, dtype=torch.float32, device=self.device) for _ in range(2)],
                       done=[torch.cuda.Event() for _ in range(2)], copied=[torch.cuda.Event() for _ in range(2)],
                       stats_host=[torch.empty(self.number_features + 3, dtype=torch.float32).pin_memory() for _ in range(8)],
                       pending=[None] * 8, used=[False, False])
@@ -1014,13 +1134,15 @@ class DistributedIBNet:
         with torch.cuda.stream(cs):
             st["x"][slot].copy_(xt.reshape(n, D), non_blocking=True)
             st["y"][slot].copy_(yt.reshape(st["y"][slot].shape), non_blocking=True)
+            if w is not None:
+                st["w"][slot].copy_(torch.from_numpy(w), non_blocking=True)
             st["copied"][slot].record(cs)
         torch.cuda.current_stream().wait_event(st["copied"][slot])
         st["used"][slot] = True
-        return st["x"][slot], st["y"][slot], slot
+        return st["x"][slot], st["y"][slot], (st["w"][slot] if w is not None else None), slot
 
     def fit(self, x=None, y=None, batch_size=None, epochs=1, verbose='auto', callbacks=None, validation_data=None,
-            shuffle=True, initial_epoch=0, **_):
+            shuffle=True, initial_epoch=0, class_weight=None, sample_weight=None, **_):
         """Keras ``Model.fit`` mechanics around the fused step (train.py:157-166, nb-radial cell 10): per epoch
         on_epoch_begin -> shuffled consecutive batches incl. a short last one -> running means -> validation pass
         (noise sampled, train.py:264-265) -> on_epoch_end; returns a History whose ``.history`` has the keys
@@ -1028,6 +1150,12 @@ class DistributedIBNet:
 
         Data-parallel: with torch.distributed initialised every rank passes the SAME x, y; each global batch is
         split into contiguous row ranges per rank, so the result does not depend on the number of GPUs.
+
+        ``sample_weight`` [N] and ``class_weight`` {0: w_0, ..., C-1: w_{C-1}} weight each row's task loss as Keras does
+        [KERAS]: loss = sum_i w_i l_i / batch size + beta * sum KL (the KL term and ``accuracy`` are unweighted); class_weight
+        maps a row to its class by argmax of a one-hot y or by the truncated integer label, and multiplies sample_weight
+        when both are given.  ``validation_data=(x_val, y_val, w_val)`` weights the validation loss by w_val; class_weight
+        applies to training only.
 
         Compiled with ``losses.InfoNCE`` this runs train.py:180-289's InfoNCE training, which needs full, equal batches:
         an epoch is floor(N / batch_size) batches of the epoch permutation (the remainder is dropped; N < batch_size is an
@@ -1047,9 +1175,12 @@ class DistributedIBNet:
             (xd, sd), yd = self._inputs(x), self._targets(y)
             N = xd.shape[0]
             plan = self._batch_plan(N, batch_size)
-            xv = yv = sv = None
+            xv = yv = sv = wv = None
             if validation_data is not None:
                 (xv, sv), yv = self._inputs(validation_data[0]), self._targets(validation_data[1])
+                if len(validation_data) > 2:
+                    wv = self._sample_weights(validation_data[2], xv.shape[0], "validation sample_weight")
+            wd = self._row_weights(y, yd, sample_weight, class_weight, N)
             history = History()
             cbs = list(callbacks or []) + [history]
             for cb in cbs:
@@ -1067,11 +1198,12 @@ class DistributedIBNet:
                 for b0, b1 in plan:
                     idx, lo = _shard_rows(order, b0, b1, rank, world)
                     self._metrics_update(self._train_step(xd[idx], yd[idx], global_batch=b1 - b0, sample_offset=lo,
-                                                          sizes=None if sd is None else sd[idx]))
+                                                          sizes=None if sd is None else sd[idx],
+                                                          weights=None if wd is None else wd[idx]))
                 logs = self._read_epoch_logs()
                 if xv is not None:
                     logs.update(self._evaluate_into_logs(xv, yv, *self._validation_plan(xv.shape[0], batch_size, epoch),
-                                                         2 ** 31 + epoch, sv))
+                                                         2 ** 31 + epoch, sv, wv))
                 if verbose not in (False, 0) and rank == 0:          # 'auto' -> 1 like Keras outside notebooks
                     print(f"Epoch {epoch + 1}/{epochs} - " + " - ".join(
                         f"{k}: {v:.4g}" for k, v in logs.items() if not k.removeprefix('val_').startswith('KL')))
@@ -1100,7 +1232,7 @@ class DistributedIBNet:
         order = self.validation_permutation(perm_key, n)[pos].reshape(-1)
         return self._batch_plan(order.shape[0], batch_size), order
 
-    def _evaluate_into_logs(self, xv, yv, plan, order, step, sv=None):
+    def _evaluate_into_logs(self, xv, yv, plan, order, step, sv=None, wv=None):
         """Validation logs of the batches ``plan`` of rows ``order`` (see :func:`_shard_rows`), noise keyed by (step, the
         row's position in ``order``): every rank runs the forward of its shard of a batch -- InfoNCE with more than one rank
         the first two phases of the step, without training -- and the statistics are summed over the ranks."""
@@ -1114,7 +1246,7 @@ class DistributedIBNet:
                 _run_phases(phases[:2], last_exchange=False)
             else:
                 self._forward(xv[idx], yv[idx], None, step, b0 + lo, want_pred=False, stats_out=stats,
-                              sizes=None if sv is None else sv[idx])
+                              sizes=None if sv is None else sv[idx], weights=None if wv is None else wv[idx])
             parallel.allreduce_sum_(stats, self.process_group)
             self._metrics_update(stats)
         return self._read_epoch_logs(prefix="val_")
@@ -1125,15 +1257,17 @@ class DistributedIBNet:
         gen.manual_seed((self.seed << 20) + (1 << 19) + int(key))
         return torch.randperm(n, generator=gen, device=self.device)
 
-    def evaluate(self, x, y, batch_size=32, return_dict=True, **_):
+    def evaluate(self, x, y, batch_size=32, return_dict=True, sample_weight=None, **_):
+        """Loss (task weighted by ``sample_weight`` [n] when given, as in :meth:`fit`), accuracy and KL of one pass over x."""
         with torch.cuda.device(self.device):
             self._inference_calls += 1           # a fresh noise draw per evaluate() call
             key = (1 << 29) | (self._inference_calls & 0x1FFFFFFF)
             if self._infonce is not None:
                 self._check_infonce_world(self._infonce, batch_size)
             (xv, sv), yv = self._inputs(x), self._targets(y)
+            wv = self._sample_weights(sample_weight, xv.shape[0])
             step = key if self._infonce is not None else 2 ** 31 + key
-            logs = self._evaluate_into_logs(xv, yv, *self._validation_plan(xv.shape[0], int(batch_size), key), step, sv)
+            logs = self._evaluate_into_logs(xv, yv, *self._validation_plan(xv.shape[0], int(batch_size), key), step, sv, wv)
         logs = {k[len("val_"):]: v for k, v in logs.items()}
         return logs if return_dict else [logs["loss"]] + [logs[m] for m in self.compiled_metrics_names]
 

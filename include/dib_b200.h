@@ -72,6 +72,24 @@ enum dib_loss {
   DIB_LOSS_INFONCE = 5
 };
 
+/* Per-sample weights of the compiled loss (Keras fit / evaluate / train_on_batch sample_weight=, class_weight=), reduction
+ * SUM_OVER_BATCH_SIZE: task loss = sum_i w_i l_i / n with n the (global) batch size, not sum w; d loss / d z_i is w_i times
+ * the unweighted value; the beta*KL term and the accuracy statistic are not weighted.  The task-loss slot of the stats holds
+ * sum_i w_i l_i.  Declared after dib_model below:
+ *
+ *   int dib_set_sample_weights_device(dib_model* h, const float* w_dev);
+ *     binds w_dev (DEVICE memory, 4-byte aligned): the fp32 weights of the n rows (sets, for a set transformer) of the following
+ *     dib_forward and dib_train_step calls of this handle (data parallel: this rank's shard).  The loss kernels read it on the
+ *     stream, so one captured graph serves every weight vector written into the buffer.  NULL (the default) = unweighted.  The
+ *     caller checks that the weights are finite and >= 0.  Fails on DIB_LOSS_EXTERNAL and DIB_LOSS_INFONCE handles.
+ *
+ *   int dib_class_weight_rows(const float* y, int64_t n, int32_t y_cols, const float* class_table, int32_t classes,
+ *                             const float* sample_weight_or_null, float* out, void* stream);
+ *     Keras' class_weight map (_make_class_weight_map_fn) on the device: the class of row i is argmax_j y[i, j] when
+ *     y_cols > 1, else y[i] cast to an integer (truncating); out[i] = class_table[class] * sample_weight[i] (the product only
+ *     when sample_weight_or_null is given).  A class outside [0, classes) gives NaN, which the caller must not bind.  y, the
+ *     table, the sample weights and out are DEVICE memory; y_cols = 0 or 1 reads y as [n]. */
+
 /* arithmetic of the dense contractions; everything else (PE, exp, KL, loss, Adam, reductions) is fp32 in every mode
  * and all tensor-core modes accumulate in fp32 (wgmma register accumulators).
  *   FP32: CUDA-core FMA -- the exact parity path (the reference's tf.keras fp32 graph on a CPU).
@@ -266,6 +284,11 @@ int dib_set_noise_step_device(dib_model* h, const uint32_t* step_dev);
  * 1 <= size <= set_size: out-of-range sizes keep every access in bounds but give meaningless results.  A variable-size handle
  * without bound sizes fails those calls; NULL unbinds.  Fails on a fixed-size handle. */
 int dib_set_set_sizes_device(dib_model* h, const int32_t* set_sizes_dev);
+
+/* per-sample weights of the compiled loss and Keras' class_weight map: see the comment after enum dib_loss */
+int dib_set_sample_weights_device(dib_model* h, const float* w_dev);
+int dib_class_weight_rows(const float* y, int64_t n, int32_t y_cols, const float* class_table, int32_t classes,
+                          const float* sample_weight_or_null, float* out, void* stream);
 
 /* tf.keras.optimizers.Adam dense update over the flat buffer (train.py:128-129, nb-radial Adam(lr)):
  *   t = *step_dev + 1 (the kernel increments *step_dev);  lr_t = lr*sqrt(1-b2^t)/(1-b1^t);
