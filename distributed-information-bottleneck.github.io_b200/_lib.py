@@ -62,6 +62,16 @@ class DibConfig(ctypes.Structure):
     ]
 
 
+# compiled metrics (dib_set_metrics): enum dib_metric_kind and struct dib_metric_spec
+METRIC_KINDS = {"mse": 0, "mae": 1, "binary_accuracy": 2, "sparse_categorical_accuracy": 3, "binary_crossentropy": 4,
+                "sparse_categorical_crossentropy": 5, "confusion": 6}
+
+
+class DibMetricSpec(ctypes.Structure):
+    _fields_ = [("kind", c_int32), ("weighted", c_int32), ("from_logits", c_int32), ("num_thresholds", c_int32),
+                ("threshold", c_float)]
+
+
 # name -> (restype, argtypes); mirrors include/dib_b200.h one to one
 SIGNATURES = {
     "dib_create": (c_int32, [POINTER(DibConfig), POINTER(c_void_p)]),
@@ -84,6 +94,8 @@ SIGNATURES = {
     "dib_set_set_sizes_device": (c_int32, [c_void_p, c_void_p]),
     "dib_set_sample_weights_device": (c_int32, [c_void_p, c_void_p]),
     "dib_class_weight_rows": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_int32, c_void_p, c_void_p, c_void_p]),
+    "dib_set_metrics": (c_int32, [c_void_p, c_void_p, c_int32]),
+    "dib_metrics_update_tail": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p]),
     "dib_adam_step": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_float,
                                 c_float, c_float, c_void_p]),
     "dib_optimizer_step": (c_int32, [c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_float,

@@ -130,6 +130,11 @@ struct dib_model {
   long long dsum = 0;
   // per-row sample weights of the following dib_forward / dib_train_step calls (dib_set_sample_weights_device), or null
   const float* sample_weights_dev = nullptr;
+  // compiled metrics (dib_set_metrics): their table and, behind the planned workspace (plan_floats), the prediction
+  // [rows, out] the loss kernels write for them and the metric kernel's CTA partials; the last CTA's counter
+  DibMetricTable metrics;
+  long long plan_floats = 0, metric_z_off = 0, metric_part_off = 0;
+  unsigned int* d_metric_counter = nullptr;
   float ln_eps = 1e-3f;
   long long maxSets = 0;
   std::vector<int> ff_arch;
@@ -302,8 +307,20 @@ void plan(dib_model* h) {
     h->d_pooled = make_buf(c, h->maxSets, E, 1);
     if (h->varlen) h->dsum = take(c, h->maxSets * h->heads * h->Ls);
   }
+  h->ws_floats = h->plan_floats = c;
+}
+
+// the compiled metrics' workspace behind the plan: nothing without metrics
+void plan_metrics(dib_model* h) {
+  long long c = h->plan_floats;
+  if (h->metrics.count > 0) {
+    h->metric_z_off = take(c, (h->st ? h->maxSets : h->maxB) * h->out);
+    h->metric_part_off = take(c, (long long)kDibMetricMaxCtas * h->metrics.tail);
+  }
   h->ws_floats = c;
 }
+
+int32_t stats_count(const dib_model* h) { return h->F + 3 + (h->metrics.count > 0 ? h->metrics.tail : 0); }
 
 // a float offset and leading dimension inside the workspace
 struct Operand { long long off = 0; int ld = 0; };
@@ -691,8 +708,8 @@ int forward_infonce(const Ctx& c, const float* y, bool training, float* user_pre
 
 // integration half of the forward: integration layers -> prediction, compiled loss / metrics, d loss / d prediction
 // (training) -> the stats row
-int forward_integration(const Ctx& c, const float* y, float inv_batch, bool training, float* user_pred, float* out_stats,
-                        int nblk_kl) {
+int forward_loss(const Ctx& c, const float* y, float inv_batch, bool training, float* user_pred, float* out_stats,
+                 int nblk_kl) {
   dib_model* h = c.h;
   const float* weights = y ? h->sample_weights_dev : nullptr;
   auto finalize = [&](int nblk_loss) {
@@ -1034,6 +1051,21 @@ int backward_set_blocks(const Ctx& c, const Split& sp) {
 
 // the forward of a call: the encoders (and a set transformer's attention blocks) on its particle rows, the integration network
 // on its own rows
+// forward_loss and, with compiled metrics and targets, the metric tail behind the stats row from the prediction the loss
+// kernels wrote (into user_pred when the caller wants it, else into the workspace)
+int forward_integration(const Ctx& c, const float* y, float inv_batch, bool training, float* user_pred, float* out_stats,
+                        int nblk_kl) {
+  dib_model* h = c.h;
+  if (h->metrics.count == 0 || !y) return forward_loss(c, y, inv_batch, training, user_pred, out_stats, nblk_kl);
+  float* z = user_pred ? user_pred : c.ws + h->metric_z_off;
+  if (forward_loss(c, y, inv_batch, training, z, out_stats, nblk_kl)) return 1;
+  prof_begin(c, "metrics");
+  DIB_CUDA_OK(dib_launch_metrics(h->metrics, z, y, h->out, c.n, h->sample_weights_dev, c.ws + h->metric_part_off,
+                                 h->d_metric_counter, out_stats + h->F + 3, c.st));
+  prof_end(c);
+  return 0;
+}
+
 int run_forward(const Ctx& c, const float* x, const float* y, const NoiseKey& nk, float inv_batch, float* user_pred,
                 float* user_emb, float* out_stats, bool enc_only = false) {
   dib_model* h = c.h;
@@ -1442,6 +1474,7 @@ void dib_destroy(dib_model* h) {
   if (h->d_fused_tables) cudaFree(h->d_fused_tables);
   if (h->d_ycol_src) cudaFree(h->d_ycol_src);
   if (h->d_ycol_freq) cudaFree(h->d_ycol_freq);
+  if (h->d_metric_counter) cudaFree(h->d_metric_counter);
   for (auto& r : h->prof) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
   delete h;
 }
@@ -1459,7 +1492,7 @@ int dib_param_layout(const dib_model* h, int64_t* offsets, int32_t* rows, int32_
 
 size_t dib_workspace_bytes(const dib_model* h) { return h ? (size_t)h->ws_floats * sizeof(float) : 0; }
 
-int32_t dib_stats_count(const dib_model* h) { return h ? h->F + 3 : -1; }
+int32_t dib_stats_count(const dib_model* h) { return h ? stats_count(h) : -1; }
 
 int dib_forward(dib_model* h, const float* params, const float* x, const float* y, int64_t n, const float* beta_dev,
                 const float* eps, uint64_t seed, uint32_t step, uint64_t sample_offset, float* out_pred, float* out_emb,
@@ -1468,7 +1501,7 @@ int dib_forward(dib_model* h, const float* params, const float* x, const float* 
   if (check_call(h, params, x, n, workspace) || check_sets(h, n)) return 1;
   if (!out_stats) return fail("dib_forward: out_stats is required");
   Ctx c{h, params, static_cast<float*>(workspace), static_cast<cudaStream_t>(stream), (int)n};
-  if (n == 0) { DIB_CUDA_OK(cudaMemsetAsync(out_stats, 0, sizeof(float) * (h->F + 3), c.st)); return 0; }
+  if (n == 0) { DIB_CUDA_OK(cudaMemsetAsync(out_stats, 0, sizeof(float) * stats_count(h), c.st)); return 0; }
   return run_forward(c, x, y, NoiseKey{eps, seed, step, sample_offset, false}, 0.f, out_pred, out_emb, out_stats);
 }
 
@@ -1497,7 +1530,7 @@ int dib_train_step(dib_model* h, const float* params, const float* x, const floa
   c.dev_step = true;
   if (n == 0) {
     DIB_CUDA_OK(cudaMemsetAsync(grads_flat, 0, sizeof(float) * h->P, c.st));
-    DIB_CUDA_OK(cudaMemsetAsync(out_stats, 0, sizeof(float) * (h->F + 3), c.st));
+    DIB_CUDA_OK(cudaMemsetAsync(out_stats, 0, sizeof(float) * stats_count(h), c.st));
     return 0;
   }
   const NoiseKey nk{eps, seed, step, sample_offset, true};
@@ -1581,6 +1614,54 @@ int dib_set_sample_weights_device(dib_model* h, const float* w_dev) {
     return fail("dib_set_sample_weights_device: the external and InfoNCE losses take no sample weights");
   if (reinterpret_cast<uintptr_t>(w_dev) & 3) return fail("dib_set_sample_weights_device: weights must be 4-byte aligned");
   h->sample_weights_dev = w_dev;
+  return 0;
+}
+
+int dib_set_metrics(dib_model* h, const dib_metric_spec* specs, int32_t count) {
+  if (!h) return fail("null model handle");
+  if (count < 0 || count > DIB_MAX_METRICS || (count > 0 && !specs))
+    return fail("dib_set_metrics: 0 <= count <= DIB_MAX_METRICS specs are required");
+  if (count > 0 && (h->loss == DIB_LOSS_EXTERNAL || h->loss == DIB_LOSS_INFONCE))
+    return fail("dib_set_metrics: the external and InfoNCE losses take no compiled metrics");
+  DibMetricTable t;
+  const bool sparse = h->loss == DIB_LOSS_SPARSE_CE_LOGITS;
+  for (int k = 0; k < count; ++k) {
+    const dib_metric_spec& m = specs[k];
+    const std::string at = "dib_set_metrics: metric " + std::to_string(k) + ": ";
+    if (m.kind < DIB_METRIC_MSE || m.kind > DIB_METRIC_CONFUSION) return fail(at + "unknown kind");
+    const bool label_kind = m.kind == DIB_METRIC_SPARSE_CATEGORICAL_ACCURACY || m.kind == DIB_METRIC_SPARSE_CATEGORICAL_CROSSENTROPY;
+    if (label_kind != sparse)
+      return fail(at + (sparse ? "the sparse categorical loss's targets are class labels: only the sparse kinds read them"
+                               : "the sparse kinds need the sparse categorical loss's class-label targets"));
+    t.kind[k] = m.kind; t.weighted[k] = m.weighted ? 1 : 0; t.from_logits[k] = m.from_logits ? 1 : 0;
+    t.threshold[k] = m.threshold; t.off[k] = t.tail; t.boff[k] = 0; t.nthr[k] = 0;
+    if (m.kind == DIB_METRIC_CONFUSION) {
+      if (h->out != 1) return fail(at + "confusion metrics need output_dimensionality 1");
+      if (m.num_thresholds < 1 || t.buckets + m.num_thresholds + 1 > DIB_MAX_METRIC_BUCKETS)
+        return fail(at + "num_thresholds must be >= 1, with at most DIB_MAX_METRIC_BUCKETS buckets over all confusion metrics");
+      t.nthr[k] = m.num_thresholds; t.boff[k] = t.buckets;
+      t.buckets += m.num_thresholds + 1;
+      t.tail += 2 * (m.num_thresholds + 1);
+      if (m.from_logits) t.sigmoid = true;
+    } else {
+      t.tail += 2;
+    }
+  }
+  t.count = count;
+  DIB_CUDA_OK(dib_metrics_prepare(t));
+  if (count > 0 && !h->d_metric_counter) {
+    DIB_CUDA_OK(cudaMalloc(&h->d_metric_counter, sizeof(unsigned int)));
+    DIB_CUDA_OK(cudaMemset(h->d_metric_counter, 0, sizeof(unsigned int)));
+    DIB_CUDA_OK(cudaDeviceSynchronize());
+  }
+  h->metrics = t;
+  plan_metrics(h);
+  return 0;
+}
+
+int dib_metrics_update_tail(const float* tail, double* acc, int32_t count, void* stream) {
+  if (count < 0 || (count > 0 && (!tail || !acc))) return fail("dib_metrics_update_tail: bad arguments");
+  DIB_CUDA_OK(dib_launch_metrics_update_tail(tail, acc, count, static_cast<cudaStream_t>(stream)));
   return 0;
 }
 

@@ -67,6 +67,27 @@ cudaError_t dib_launch_loss(int loss, int out_act, float alpha, const float* pre
 cudaError_t dib_launch_class_weight_rows(const float* y, int64_t n, int y_cols, const float* table, int classes, const float* sw,
                                          float* out, cudaStream_t st);
 
+// ---- compiled metrics (dib_metrics.cu; dib_set_metrics) -----------------------------------------------------------
+constexpr int kDibMaxMetrics = 16;                 // DIB_MAX_METRICS
+constexpr int kDibMetricMaxCtas = 128;             // CTA partials in the workspace: kDibMetricMaxCtas * tail floats
+struct DibMetricTable {
+  int count = 0;                                   // metrics
+  int tail = 0;                                    // floats of the metric tail
+  int buckets = 0;                                 // sum over the confusion metrics of (T + 1)
+  bool sigmoid = false;                            // some confusion metric reads sigmoid(z)
+  int kind[kDibMaxMetrics], weighted[kDibMaxMetrics], from_logits[kDibMaxMetrics], nthr[kDibMaxMetrics];
+  int off[kDibMaxMetrics];                         // first tail float of metric k
+  int boff[kDibMaxMetrics];                        // confusion: first entry of its threshold table / bucket row
+  float threshold[kDibMaxMetrics];
+};
+// z [n, out_dim] and y ([n] labels or [n, out_dim]) -> tail [t.tail]; w: the rows' sample weights or null; part: the
+// workspace's CTA partials, counter: a zeroed device word the last CTA resets
+cudaError_t dib_launch_metrics(const DibMetricTable& t, const float* z, const float* y, int out_dim, int64_t n, const float* w,
+                               float* part, unsigned int* counter, float* tail, cudaStream_t st);
+// host-side set-up of a table's launches (the shared-memory opt-in); call before the first launch and outside graph capture
+cudaError_t dib_metrics_prepare(const DibMetricTable& t);
+cudaError_t dib_launch_metrics_update_tail(const float* tail, double* acc, int count, cudaStream_t st);
+
 cudaError_t dib_launch_round_copy(const float* src, float* dst, int64_t count, cudaStream_t st);
 
 cudaError_t dib_launch_finalize_stats(const float* kl_part, int nblk_stride, int nblk_kl, const float* loss_part,

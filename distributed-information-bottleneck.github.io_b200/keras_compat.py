@@ -159,6 +159,9 @@ def resolve_loss(loss):
     raise ValueError(f"unsupported loss {loss!r}")
 
 
+from .metrics import metrics  # noqa: E402,F401 -- keras.metrics: the compiled metrics' objects
+
+
 class Callback:
     """tf.keras.callbacks.Callback protocol (models.py:125,152,188): the trainer sets ``.model``."""
     model = None

@@ -18,6 +18,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from . import metrics as _metrics
 from . import parallel
 from .keras_compat import Adam, InfoNCE, RMSprop, SGD, Callback, History, optimizers, resolve_loss
 
@@ -357,6 +358,7 @@ class DistributedIBNet:
             self._lr_dev = torch.full((1,), 1e-3, dtype=torch.float32, device=self.device)
             self._step_dev = torch.zeros(1, dtype=torch.int32, device=self.device)
             self._epoch_acc = torch.zeros(self.number_features + 4, dtype=torch.float32, device=self.device)
+            self._epoch_tail = torch.zeros(0, dtype=torch.float64, device=self.device)    # compiled metrics' epoch sums
         self._train_step_count = 0
         # ---- CUDA-graph replay of the train step (launch-bound small batches; fewer host calls per step at any size)
         env = os.environ.get("DIB_CUDA_GRAPH", "auto").lower()
@@ -371,6 +373,8 @@ class DistributedIBNet:
         self._inference_calls = 0          # fresh noise per un-seeded inference call (tf.random.normal, models.py:108)
         self.optimizer = None
         self.compiled_metrics_names = []
+        self._metric_entries = []          # metrics.CompiledMetric per compiled metric, in history order
+        self._tail_len = 0                 # floats of the metric tail behind the F + 3 statistics
         self.losses = []
         self.metrics_values = {}
         n_enc_vars = 2 if self.encoder_kind == "simple" else 2 * (len(self.feature_encoder_architecture) + 1)
@@ -426,7 +430,8 @@ class DistributedIBNet:
                 self._lib.dib_destroy(h)
 
     def _ensure_handle(self, n):
-        key = (self._loss_kind, self.precision, self._infonce.spec() if self._infonce is not None else None)
+        key = (self._loss_kind, self.precision, self._infonce.spec() if self._infonce is not None else None,
+               _metrics.signature(self._metric_entries))
         if self._handle is not None and self._handle_key == key and n <= self._max_batch:
             return
         self._release_handle()
@@ -440,6 +445,10 @@ class DistributedIBNet:
             self._step_dev_active = False
             if getattr(self, "_force_unfused", 0):
                 _lib.check(self._lib.dib_debug_force_unfused(h, int(self._force_unfused)))
+            if self._tail_len:
+                specs, count = _metrics.library_specs(self._metric_entries)
+                _lib.check(self._lib.dib_set_metrics(h, specs, count))
+            assert int(self._lib.dib_stats_count(h)) == self._stats_count()
             nbytes = int(self._lib.dib_workspace_bytes(h))
             self._workspace = None
             self._workspace = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
@@ -520,7 +529,7 @@ class DistributedIBNet:
             m, v = torch.zeros_like(params), torch.zeros_like(params)
             m[:keep], v[:keep] = self._m[:keep], self._v[:keep]
             self._params, self._m, self._v = params, m, v
-            self._gradstats = torch.zeros(self._P + self.number_features + 3, dtype=torch.float32, device=self.device)
+            self._gradstats = torch.zeros(self._P + self._stats_count(), dtype=torch.float32, device=self.device)
         self._staging = None
         self.output_encoder = (_OutputEncoder(self, range(self._n_model_vars, len(self._var_off)))
                                if nce is not None else None)
@@ -554,6 +563,10 @@ class DistributedIBNet:
 
     def build(self, input_shape):
         assert input_shape[-1] == sum(self.feature_dimensionalities)       # models.py:89
+
+    def _stats_count(self):
+        """Floats of the statistics vector: [KL sums (F) | task loss | accuracy | n] and the compiled metrics' tail."""
+        return self.number_features + 3 + self._tail_len
 
     # ------------------------------------------------------------------ data helpers
     def _to_device(self, a, cols=None):
@@ -634,7 +647,7 @@ class DistributedIBNet:
         pred = torch.empty(n, self.output_dimensionality, dtype=torch.float32, device=self.device) if want_pred else None
         emb = torch.empty(n, self.number_features * self.feature_embedding_dimension, dtype=torch.float32,
                           device=self.device) if want_emb else None
-        stats = stats_out if stats_out is not None else torch.empty(self.number_features + 3, dtype=torch.float32,
+        stats = stats_out if stats_out is not None else torch.empty(self._stats_count(), dtype=torch.float32,
                                                                     device=self.device)
         _lib.check(self._lib.dib_forward(
             self._handle, _lib.ptr(self._params), _lib.ptr(x), _lib.ptr(y), n, _lib.ptr(self.beta._dev), _lib.ptr(eps),
@@ -827,11 +840,12 @@ class DistributedIBNet:
 
     def _train_step(self, x, y, global_batch, eps=None, sample_offset=0, sizes=None, weights=None):
         """backward, one flat all-reduce of [grads || stats] over the data-parallel group, Keras-Adam.  Replayed from
-        CUDA graphs once a (batch size, offset, weighted or not) combination has run eagerly twice; the set sizes of a
+        CUDA graphs once a (batch size, offset, weighted or not, compiled metrics) combination has run eagerly twice; the set sizes of a
         variable-size set transformer and the sample weights are data, not part of that key."""
         P = self._P
         world, _ = parallel.world_and_rank(self.process_group)
-        key = (int(x.shape[0]), int(global_batch), int(sample_offset), world, weights is not None)
+        key = (int(x.shape[0]), int(global_batch), int(sample_offset), world, _metrics.signature(self._metric_entries),
+               weights is not None)
         if self.use_cuda_graph and not self._graph_failed and eps is None and x.shape[0] > 0:
             g = self._graphs.get(key)
             if g is None and self._graph_seen.get(key, 0) >= 2:
@@ -849,13 +863,13 @@ class DistributedIBNet:
 
     # ------------------------------------------------------------------ CUDA-graph replay of the step
     def _capture_step(self, key, with_sizes=False):
-        """Capture the step for one (n, global_batch, sample_offset, world, weighted) into CUDA graphs: one graph per run of phases
+        """Capture the step for one (n, global_batch, sample_offset, world, compiled metrics, weighted) into CUDA graphs: one graph per run of phases
         between two collectives, each kept with the exchange that follows it.  Single GPU: ONE graph (forward + backward +
         optimizer + noise-step increment); plain data parallel: two (backward | optimizer); InfoNCE with global negatives: four
         (the three shard phases | optimizer), e_all / lse_all kept with the graphs.  Inputs are copied into static buffers
         before each replay (and, ``with_sizes``, the set sizes into a third one; weighted, the sample weights into a fourth); beta, learning rate, the optimizer step and
         the Philox step are device scalars, so nothing by-value changes between replays."""
-        n, global_batch, sample_offset, world, weighted = key
+        n, global_batch, sample_offset, world, _, weighted = key
         D = sum(self.feature_dimensionalities)
         yc = self._y_cols()
         try:
@@ -940,6 +954,7 @@ class DistributedIBNet:
         """Every feature encoder + reparameterisation, without the integration network (nb-particle cell 8's
         ``particle_encoder`` front end): returns (emb [n, F*E] = mu + exp(logvar/2) eps, KL_i batch means [F]) as device
         tensors.  Noise as in ``__call__``: explicit ``eps``, Philox keyed by ``step``, or a fresh draw."""
+        self._refuse_tail_metrics("encode")
         with torch.cuda.device(self.device):
             xd = self._to_device(x, sum(self.feature_dimensionalities))
             e = self._to_device(eps) if eps is not None else None
@@ -958,6 +973,7 @@ class DistributedIBNet:
         (already carrying the caller's batch scaling); the IB term beta * scale * (sum KL)^p, with KL means over
         ``global_batch`` rows (default n), is added here.  Returns (flat gradient [P] -- integration entries are zero --,
         statistics vector).  Pass the same ``eps`` / ``step`` as the ``encode`` call it differentiates."""
+        self._refuse_tail_metrics("encoder_gradients")
         with torch.cuda.device(self.device):
             xd = self._to_device(x, sum(self.feature_dimensionalities))
             gd = self._to_device(d_emb, self.number_features * self.feature_embedding_dimension)
@@ -988,17 +1004,30 @@ class DistributedIBNet:
         gen.manual_seed((self.seed << 20) + epoch)
         return torch.randperm(n, generator=gen, device=self.device)
 
+    def _zero_epoch(self):
+        self._epoch_acc.zero_()
+        self._epoch_tail.zero_()
+
     def _metrics_update(self, stats):
         _lib.check(self._lib.dib_metrics_update_ex(_lib.ptr(stats), _lib.ptr(self.beta._dev), _lib.ptr(self._epoch_acc),
                                                    self.number_features, self.kl_loss_exponent, self.kl_loss_scale, _stream()))
+        if self._tail_len:
+            F = self.number_features
+            _lib.check(self._lib.dib_metrics_update_tail(_lib.ptr(stats[F + 3:]), _lib.ptr(self._epoch_tail), self._tail_len,
+                                                         _stream()))
+
+    def _metric_logs(self, acc_sum, n, tail, prefix=""):
+        """{prefix + name: value} of the compiled metrics in history order: the accuracy slot (acc_sum / n) and the tail's."""
+        vals = _metrics.metric_values(self._metric_entries, tail) if self._tail_len else {}
+        return {prefix + e.name: (float(acc_sum / n) if not e.in_tail else vals[e.name]) for e in self._metric_entries}
 
     def _read_epoch_logs(self, prefix=""):
         F = self.number_features
         a = self._epoch_acc.detach().cpu().numpy().astype(np.float64)       # one D2H per epoch
+        tail = self._epoch_tail.detach().cpu().numpy() if self._tail_len else None
         n, nb = max(a[F + 2], 1.0), max(a[F + 3], 1.0)
         logs = {prefix + "loss": float(a[F] / n)}
-        for m in self.compiled_metrics_names:
-            logs[prefix + m] = float(a[F + 1] / n)
+        logs.update(self._metric_logs(a[F + 1], n, tail, prefix))
         for i in range(F):
             logs[f"{prefix}KL{i}"] = float(a[i] / nb)                        # add_metric mean over batches (models.py:115)
         logs[prefix + "beta"] = float(self.beta.value())                     # models.py:121
@@ -1031,28 +1060,49 @@ class DistributedIBNet:
 
     call = __call__
 
-    def compile(self, optimizer='adam', loss=None, metrics=None, **_):
-        """train.py:138-142."""
+    def compile(self, optimizer='adam', loss=None, metrics=None, weighted_metrics=None, **_):
+        """train.py:138-142, and Keras' compiled metrics: ``metrics`` / ``weighted_metrics`` take 'accuracy' (its own
+        statistics slot, as before), the strings 'binary_accuracy', 'sparse_categorical_accuracy', 'mse' /
+        'mean_squared_error', 'mae' / 'mean_absolute_error', 'binary_crossentropy', 'sparse_categorical_crossentropy'
+        (Keras' functions as written: from_logits=False) and the objects of :mod:`dib_b200.metrics` (AUC, Precision,
+        Recall with one output).  ``weighted_metrics`` weight each row by the step's sample weight; a metric in both lists
+        gets the ``weighted_`` prefix on its weighted copy.  History keys are the names as written (objects: ``name``) and
+        their ``val_`` twins; see :mod:`dib_b200.metrics` for the semantics and the refusals."""
         new_opt = optimizers.get(optimizer)
-        if new_opt is not self.optimizer:        # a fresh Keras optimizer has fresh slots and iteration count
-            self._m.zero_(); self._v.zero_(); self._step_dev.zero_()
         kind = resolve_loss(loss)
         if kind == "infonce":
-            if metrics:
+            if metrics or weighted_metrics:
                 raise ValueError("losses.InfoNCE has no accuracy: compile it without metrics (train.py:180-289 tracks none)")
             if self.output_activation_fn is not None:
                 raise ValueError("losses.InfoNCE needs output_activation_fn=None: the prediction is the InfoNCE embedding "
                                  "(train.py:117)")
             self._check_infonce_world(loss)
-        for m in (metrics or []):
-            if m not in ("accuracy", "acc"):
-                raise ValueError(f"only metrics=['accuracy'] is implemented (reference data.py:67), got {m!r}")
+        entries = _metrics.compile_metrics(metrics, weighted_metrics, kind, self.output_dimensionality,
+                                           self.output_activation_fn)
+        if new_opt is not self.optimizer:        # a fresh Keras optimizer has fresh slots and iteration count
+            self._m.zero_(); self._v.zero_(); self._step_dev.zero_()
         self.optimizer = new_opt
         self._loss_kind = kind
         self._set_output_encoder(loss if kind == "infonce" else None)
-        self.compiled_metrics_names = ["accuracy" for _ in (metrics or [])]
+        self._set_metric_entries(entries)
         self._lr_host = None
         self._sync_lr()
+
+    def _set_metric_entries(self, entries):
+        """The compiled metrics: history names, the tail length, and the device buffers whose size depends on it."""
+        self._metric_entries = entries
+        self.compiled_metrics_names = [e.name for e in entries]
+        tail = _metrics.tail_length(entries)
+        if tail != self._tail_len:
+            self._tail_len = tail
+            with torch.cuda.device(self.device):
+                self._gradstats = torch.zeros(self._P + self._stats_count(), dtype=torch.float32, device=self.device)
+                self._epoch_tail = torch.zeros(tail, dtype=torch.float64, device=self.device)
+
+    def _refuse_tail_metrics(self, what):
+        if self._tail_len:
+            raise ValueError(f"{what} is an encoder-only step and computes no compiled metrics: compile the model without "
+                             "metrics other than 'accuracy' to use it")
 
     def _sync_lr(self):
         """Device copy of optimizer.learning_rate (the step kernels read it from memory so that a schedule needs no re-capture);
@@ -1117,13 +1167,13 @@ class DistributedIBNet:
         yt = y if isinstance(y, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(y, dtype=np.float32))
         n, yc = xt.shape[0], self._y_cols()
         st = getattr(self, "_staging", None)
-        if st is None or st["n"] != n:
+        if st is None or st["n"] != n or st["stats_host"][0].numel() != self._stats_count():
             st = dict(n=n, k=0, stream=torch.cuda.Stream(device=self.device),
                       x=[torch.empty(n, D, dtype=torch.float32, device=self.device) for _ in range(2)],
                       y=[torch.empty((n, yc) if yc > 0 else (n,), dtype=torch.float32, device=self.device) for _ in range(2)],
                       w=[torch.empty(n, dtype=torch.float32, device=self.device) for _ in range(2)],
                       done=[torch.cuda.Event() for _ in range(2)], copied=[torch.cuda.Event() for _ in range(2)],
-                      stats_host=[torch.empty(self.number_features + 3, dtype=torch.float32).pin_memory() for _ in range(8)],
+                      stats_host=[torch.empty(self._stats_count(), dtype=torch.float32).pin_memory() for _ in range(8)],
                       pending=[None] * 8, used=[False, False])
             self._staging = st
         slot = st["k"] % 2
@@ -1194,7 +1244,7 @@ class DistributedIBNet:
                     cb.on_epoch_begin(epoch, logs=None)                      # beta annealing lives here
                 self._sync_lr()
                 order = self.epoch_permutation(epoch, N) if shuffle else None
-                self._epoch_acc.zero_()
+                self._zero_epoch()
                 for b0, b1 in plan:
                     idx, lo = _shard_rows(order, b0, b1, rank, world)
                     self._metrics_update(self._train_step(xd[idx], yd[idx], global_batch=b1 - b0, sample_offset=lo,
@@ -1237,8 +1287,8 @@ class DistributedIBNet:
         row's position in ``order``): every rank runs the forward of its shard of a batch -- InfoNCE with more than one rank
         the first two phases of the step, without training -- and the statistics are summed over the ranks."""
         world, rank = parallel.world_and_rank(self.process_group)
-        self._epoch_acc.zero_()
-        stats = torch.empty(self.number_features + 3, dtype=torch.float32, device=self.device)
+        self._zero_epoch()
+        stats = torch.empty(self._stats_count(), dtype=torch.float32, device=self.device)
         for b0, b1 in plan:
             idx, lo = _shard_rows(order, b0, b1, rank, world)
             if self._infonce is not None and world > 1:
@@ -1302,6 +1352,8 @@ class PendingBatchResult:
             m = self._m
             ib = self._beta * m.kl_loss_scale * (s[:F].sum() / nn) ** m.kl_loss_exponent      # models.py:118 / nb-chaos
             out = {"loss": float(s[F] / nn + ib), "accuracy": float(s[F + 1] / nn)}
+            if m._tail_len:                              # the batch's compiled metrics (Keras reset_metrics=True)
+                out.update(_metrics.metric_values(m._metric_entries, s[F + 3:F + 3 + m._tail_len]))
             for i in range(F):
                 out[f"KL{i}"] = float(s[i] / nn)
             self._out = out

@@ -90,6 +90,40 @@ enum dib_loss {
  *     when sample_weight_or_null is given).  A class outside [0, classes) gives NaN, which the caller must not bind.  y, the
  *     table, the sample weights and out are DEVICE memory; y_cols = 0 or 1 reads y as [n]. */
 
+/* Compiled Keras metrics beyond metrics=['accuracy'] (Keras 2 semantics; see dib_set_metrics below).  Each metric adds sums
+ * to a METRIC TAIL behind the F + 3 statistics, so dib_stats_count = F + 3 + M; every entry is a sum over rows, so the
+ * all-reduce of [grads || stats] that data parallelism already does also sums the tail.  m_i is the row's value averaged over
+ * the outputs, w_i its sample weight (1 unless the metric is weighted and weights are bound):
+ *   mean metrics, 2 floats: [ sum_i w_i m_i | sum_i w_i ]   (epoch value = sum w m / sum w)
+ *     DIB_METRIC_MSE (z - y)^2;  DIB_METRIC_MAE |z - y|;  DIB_METRIC_BINARY_ACCURACY [(z > threshold) == y];
+ *     DIB_METRIC_SPARSE_CATEGORICAL_ACCURACY [argmax z == y];  DIB_METRIC_BINARY_CROSSENTROPY (from_logits: the logistic
+ *     loss of z; else keras.backend.binary_crossentropy: p clipped to [1e-7, 1 - 1e-7], -(y log(p + 1e-7) + (1-y) log(1 - p
+ *     + 1e-7)));  DIB_METRIC_SPARSE_CATEGORICAL_CROSSENTROPY (from_logits: logsumexp z - z_y; else -log(p~_y / sum_j p~_j),
+ *     p~ = p clipped to [1e-7, 1 - 1e-7]).  The two sparse kinds need y [n] class labels, the others y [n, out].
+ *   DIB_METRIC_CONFUSION (out = 1), 2 (T + 1) floats: [ neg[0..T] | pos[0..T] ], the summed w of the rows with y == 0 (neg)
+ *     and y != 0 (pos) whose p (sigmoid(z) with from_logits, else z) exceeds exactly b of the T float32 thresholds
+ *     (p > t strictly).  T >= 2: Keras' AUC table {-1e-7, 1/(T-1), ..., (T-2)/(T-1), 1 + 1e-7}; T == 1: {threshold}
+ *     (Precision / Recall).  TP(t_j) = sum_{b > j} pos[b], FP(t_j) = sum_{b > j} neg[b], FN and TN the rest. */
+enum dib_metric_kind {
+  DIB_METRIC_MSE = 0,
+  DIB_METRIC_MAE = 1,
+  DIB_METRIC_BINARY_ACCURACY = 2,
+  DIB_METRIC_SPARSE_CATEGORICAL_ACCURACY = 3,
+  DIB_METRIC_BINARY_CROSSENTROPY = 4,
+  DIB_METRIC_SPARSE_CATEGORICAL_CROSSENTROPY = 5,
+  DIB_METRIC_CONFUSION = 6
+};
+#define DIB_MAX_METRICS 16
+#define DIB_MAX_METRIC_BUCKETS 2048      /* sum over the confusion metrics of (num_thresholds + 1) */
+
+typedef struct dib_metric_spec {
+  int32_t kind;             /* dib_metric_kind */
+  int32_t weighted;         /* 1: w_i = the bound sample weight (dib_set_sample_weights_device), 0: w_i = 1 */
+  int32_t from_logits;      /* crossentropy and confusion metrics: z is a logit */
+  int32_t num_thresholds;   /* DIB_METRIC_CONFUSION: T (1 .. DIB_MAX_METRIC_BUCKETS - 1); otherwise 0 */
+  float threshold;          /* DIB_METRIC_BINARY_ACCURACY, and DIB_METRIC_CONFUSION with T == 1 */
+} dib_metric_spec;
+
 /* arithmetic of the dense contractions; everything else (PE, exp, KL, loss, Adam, reductions) is fp32 in every mode
  * and all tensor-core modes accumulate in fp32 (wgmma register accumulators).
  *   FP32: CUDA-core FMA -- the exact parity path (the reference's tf.keras fp32 graph on a CPU).
@@ -200,7 +234,8 @@ int dib_param_layout(const dib_model* h, int64_t* offsets, int32_t* rows, int32_
  * aligned and `params` 16-byte aligned (checked; cudaMalloc / torch allocations are). */
 size_t dib_workspace_bytes(const dib_model* h);
 
-/* number of floats in the statistics vector: [ sum_b KL_i (F) | sum_b task loss | sum_b accuracy | n ] */
+/* number of floats in the statistics vector: [ sum_b KL_i (F) | sum_b task loss | sum_b accuracy | n ], followed by the
+ * metric tail (M floats) when dib_set_metrics configured one: F + 3 + M, else F + 3 */
 int32_t dib_stats_count(const dib_model* h);
 
 /* DistributedIBNet.call (models.py:96-123) + compiled loss/metrics, no gradient: the validation pass of
@@ -289,6 +324,20 @@ int dib_set_set_sizes_device(dib_model* h, const int32_t* set_sizes_dev);
 int dib_set_sample_weights_device(dib_model* h, const float* w_dev);
 int dib_class_weight_rows(const float* y, int64_t n, int32_t y_cols, const float* class_table, int32_t classes,
                           const float* sample_weight_or_null, float* out, void* stream);
+
+/* Compiled metrics (see dib_metric_spec after enum dib_loss): specs[0 .. count) in order define the metric tail, which
+ * dib_forward (with y) and dib_train_step write behind the F + 3 statistics.  The prediction is written to the workspace
+ * (or to out_pred when given) and one launch after the loss reduces it with y and the weights into the tail, in a fixed
+ * order (no float atomics: repeated calls and graph replays are bit-identical).  count = 0 removes the tail, and the calls
+ * run exactly the launches they ran before.  Changes dib_stats_count and dib_workspace_bytes: query both after this call.
+ * Fails (and changes nothing) on DIB_LOSS_EXTERNAL / DIB_LOSS_INFONCE handles, on a confusion metric with
+ * output_dimensionality != 1, on the sparse kinds without DIB_LOSS_SPARSE_CE_LOGITS, on the other kinds with it, and
+ * beyond DIB_MAX_METRICS / DIB_MAX_METRIC_BUCKETS.  The encoder-only entry points write the F + 3 statistics only. */
+int dib_set_metrics(dib_model* h, const dib_metric_spec* specs, int32_t count);
+
+/* epoch accumulation of a metric tail: acc[i] += (double)tail[i] for i < count (tail: the all-reduced floats behind the
+ * F + 3 statistics; acc: float64 DEVICE memory the caller zeroes at the start of an epoch). */
+int dib_metrics_update_tail(const float* tail, double* acc, int32_t count, void* stream);
 
 /* tf.keras.optimizers.Adam dense update over the flat buffer (train.py:128-129, nb-radial Adam(lr)):
  *   t = *step_dev + 1 (the kernel increments *step_dev);  lr_t = lr*sqrt(1-b2^t)/(1-b1^t);
