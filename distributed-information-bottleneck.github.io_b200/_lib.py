@@ -72,6 +72,17 @@ class DibMetricSpec(ctypes.Structure):
                 ("threshold", c_float)]
 
 
+# grouped GEMM problem descriptor of dib_debug_gemm (struct dib_gemm_problem); offsets in floats
+class DibGemmProblem(ctypes.Structure):
+    _fields_ = [("a_off", c_int64), ("b_off", c_int64), ("c_off", c_int64), ("x_off", c_int64),
+                ("lda", c_int32), ("ldb", c_int32), ("ldc", c_int32), ("ldx", c_int32),
+                ("T", c_int32), ("C", c_int32), ("R", c_int32), ("act", c_int32)]
+
+
+GEMM_KERNELS = {"simt": 0, "tc": 1}
+GEMM_MODES = {"fwd": 0, "dgrad": 1, "wgrad": 2}
+
+
 # name -> (restype, argtypes); mirrors include/dib_b200.h one to one
 SIGNATURES = {
     "dib_create": (c_int32, [POINTER(DibConfig), POINTER(c_void_p)]),
@@ -129,9 +140,8 @@ SIGNATURES = {
     "dib_launch_count": (c_uint64, []),
     "dib_profile_enable": (c_int32, [c_void_p, c_int32]),
     "dib_profile_read": (c_int32, [c_void_p, c_char_p, c_size_t, POINTER(c_float), c_int32]),
-    "dib_debug_gemm_tc": (c_int32, [c_int32, c_void_p, c_int32, c_void_p, c_int32, c_void_p, c_int32, c_void_p, c_int32,
-                                    c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int64, c_int32,
-                                    c_void_p]),
+    "dib_debug_gemm": (c_int32, [c_int32, c_int32, c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                 c_int32, c_int32, c_int32, c_int32, c_int32, c_int64, c_float, c_int32, c_void_p]),
     "dib_debug_force_unfused": (c_int32, [c_void_p, c_int32]),
     "dib_last_error": (c_char_p, []),
     "dib_build_info": (c_char_p, []),

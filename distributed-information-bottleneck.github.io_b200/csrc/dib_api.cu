@@ -1,6 +1,7 @@
 // dib_api.cu -- the C ABI declared in include/dib_b200.h: model description, workspace plan, and the
 // orchestration of one forward / train step as a fixed sequence of asynchronous launches on the caller's stream.
 #include <atomic>
+#include <cstddef>
 #include <cstdio>
 #include <cstring>
 #include <new>
@@ -1179,26 +1180,41 @@ int32_t dib_profile_read(dib_model* h, char* labels, size_t labels_bytes, float*
   return n;
 }
 
-// single-problem GEMM through the tensor-core kernel (bring-up / unit tests): see DibGemmProblem for the modes
-int dib_debug_gemm_tc(int32_t mode, const float* A, int32_t lda, const float* B, int32_t ldb, float* Cout, int32_t ldc,
-                      float* X, int32_t ldx, int32_t M, int32_t T, int32_t Ccols, int32_t R, int32_t act,
-                      int32_t nsplit, int32_t rows_per_split, int64_t split_stride, int32_t use_simt, void* stream) {
-  DibGemmProblem p;
-  memset(&p, 0, sizeof(p));
-  p.lda = lda; p.ldb = ldb; p.ldc = ldc; p.ldx = ldx; p.T = T; p.C = Ccols; p.R = R; p.act = act;
-  p.x_off = 0;
+// the header's C mirror of the kernels' problem descriptor: the test hook hands its array to the kernels as it is
+static_assert(sizeof(dib_gemm_problem) == sizeof(DibGemmProblem), "dib_gemm_problem size");
+static_assert(offsetof(dib_gemm_problem, a_off) == offsetof(DibGemmProblem, a_off) &&
+              offsetof(dib_gemm_problem, x_off) == offsetof(DibGemmProblem, x_off) &&
+              offsetof(dib_gemm_problem, lda) == offsetof(DibGemmProblem, lda) &&
+              offsetof(dib_gemm_problem, ldx) == offsetof(DibGemmProblem, ldx) &&
+              offsetof(dib_gemm_problem, T) == offsetof(DibGemmProblem, T) &&
+              offsetof(dib_gemm_problem, C) == offsetof(DibGemmProblem, C) &&
+              offsetof(dib_gemm_problem, R) == offsetof(DibGemmProblem, R) &&
+              offsetof(dib_gemm_problem, act) == offsetof(DibGemmProblem, act), "dib_gemm_problem layout");
+
+// one grouped GEMM launch of the simt or tc kernel, set up as gemm() sets up its launches (unit tests)
+int dib_debug_gemm(int32_t kernel, int32_t mode, const dib_gemm_problem* problems, int32_t nprob, const float* A,
+                   const float* B, float* C, float* X, const float* bias, int32_t M, int32_t maxC, int32_t maxR, int32_t nsplit,
+                   int32_t rows_per_split, int64_t split_stride, float alpha, int32_t round_out, void* stream) {
+  if (kernel != DIB_GEMM_KERNEL_SIMT && kernel != DIB_GEMM_KERNEL_TC) return fail("dib_debug_gemm: unknown kernel");
+  if (mode < DIB_GEMM_FWD || mode > DIB_GEMM_WGRAD) return fail("dib_debug_gemm: unknown mode");
+  if (!problems || nprob < 1 || M < 0 || nsplit < 1) return fail("dib_debug_gemm: needs nprob >= 1, M >= 0 and nsplit >= 1");
+  if (kernel == DIB_GEMM_KERNEL_SIMT && mode == DIB_GEMM_FWD && bias && bias != B)
+    return fail("dib_debug_gemm: the simt kernel reads FWD biases from B's base (bias must be B or null)");
+  const DibGemmProblem* hp = reinterpret_cast<const DibGemmProblem*>(problems);
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (kernel == DIB_GEMM_KERNEL_TC && !dib_gemm_tc_eligible(mode, hp, nprob, nullptr))
+    return fail("dib_debug_gemm: the tensor-core kernel cannot run this group");
   DibGemmProblem* dp = nullptr;
-  DIB_CUDA_OK(cudaMalloc(&dp, sizeof(p)));
-  DIB_CUDA_OK(cudaMemcpy(dp, &p, sizeof(p), cudaMemcpyHostToDevice));
+  DIB_CUDA_OK(cudaMalloc(&dp, (size_t)nprob * sizeof(DibGemmProblem)));
+  cudaError_t e = cudaMemcpy(dp, hp, (size_t)nprob * sizeof(DibGemmProblem), cudaMemcpyHostToDevice);
   DibGemmLaunch L;
-  L.probs = dp; L.nprob = 1; L.baseA = A; L.baseB = B; L.baseC = Cout; L.baseX = X; L.M = M;
-  L.maxC = Ccols; L.maxR = R; L.nsplit = nsplit < 1 ? 1 : nsplit; L.rows_per_split = rows_per_split;
-  L.split_stride = split_stride; L.alpha = 0.2f;
-  cudaError_t e;
-  if (use_simt) e = dib_launch_gemm_simt(mode, L, static_cast<cudaStream_t>(stream));
-  else if (!dib_gemm_tc_eligible(mode, &p, 1, nullptr)) { cudaFree(dp); return fail("dib_debug_gemm_tc: not eligible"); }
-  else e = dib_launch_gemm_tc(mode, L, &p, static_cast<cudaStream_t>(stream));
-  cudaError_t e2 = cudaStreamSynchronize(static_cast<cudaStream_t>(stream));
+  L.probs = dp; L.nprob = nprob; L.baseA = A; L.baseB = B; L.baseC = C; L.baseX = X; L.M = M;
+  L.maxC = maxC; L.maxR = maxR; L.nsplit = nsplit; L.rows_per_split = rows_per_split;
+  L.split_stride = split_stride; L.alpha = alpha; L.round_out = round_out ? 1 : 0;
+  if (mode == DIB_GEMM_FWD) L.baseBias = bias;
+  if (e == cudaSuccess)
+    e = kernel == DIB_GEMM_KERNEL_TC ? dib_launch_gemm_tc(mode, L, hp, st) : dib_launch_gemm_simt(mode, L, st);
+  cudaError_t e2 = cudaStreamSynchronize(st);
   cudaFree(dp);
   if (e != cudaSuccess) return fail(std::string("launch: ") + cudaGetErrorString(e));
   if (e2 != cudaSuccess) return fail(std::string("sync: ") + cudaGetErrorString(e2));
@@ -1273,6 +1289,9 @@ int dib_create(const dib_config* cfg, dib_model** out) {
       cfg->max_batch < 1 || cfg->number_encoder_layers < 0 || cfg->number_integration_layers < 0)
     return fail("dib_create: invalid sizes");
   if (cfg->max_batch > 0x7fffffffll) return fail("dib_create: max_batch too large");
+  // the reparametrisation and KL kernels index the feature by gridDim.y, whose hardware limit is 65 535
+  if (cfg->number_features > 65535)
+    return fail("dib_create: number_features = " + std::to_string(cfg->number_features) + " exceeds 65535");
   if (cfg->precision < DIB_PREC_FP32 || cfg->precision > DIB_PREC_FP16)
     return fail("dib_create: unknown precision");
   if (cfg->activation_fn < 0 || cfg->activation_fn > DIB_ACT_ELU || cfg->output_activation_fn < 0 ||

@@ -244,16 +244,26 @@ dib_gemm_simt_kernel(const DibGemmProblem* __restrict__ probs, const float* __re
 template <int MODE, int BR, int BC, int BT, int TM, int TN>
 cudaError_t launch_cfg(const DibGemmLaunch& L, cudaStream_t st) {
   constexpr int NT = (BR / TM) * (BC / TN);
-  dim3 grid;
-  if (MODE == DIB_GEMM_WGRAD)
-    grid = dim3(DIB_CEIL_DIV(L.maxC, BC), DIB_CEIL_DIV(L.maxR, BR), L.nprob * L.nsplit);
-  else
-    grid = dim3(DIB_CEIL_DIV(L.M, BR), DIB_CEIL_DIV(L.maxC, BC), L.nprob);
-  if (grid.x == 0 || grid.y == 0 || grid.z == 0) return cudaSuccess;
-  dib_gemm_simt_kernel<MODE, BR, BC, BT, TM, TN><<<grid, NT, 0, st>>>(
-      L.probs, L.baseA, L.baseB, L.baseC, L.baseX, L.M, L.nsplit, L.rows_per_split, L.split_stride, L.alpha, L.round_out);
-  dib_note_launch();
-  return cudaGetLastError();
+  // gridDim.z holds (problem, split): a group with more than 65 535 of them runs as consecutive launches over its problems
+  const int zper = MODE == DIB_GEMM_WGRAD ? L.nsplit : 1;
+  const int chunk = dib_gemm_chunk_problems(L.nprob, zper);
+  if (L.nprob > 0 && chunk < 1) return cudaErrorInvalidConfiguration;
+  for (int first = 0; first < L.nprob; first += chunk) {
+    const int np = L.nprob - first < chunk ? L.nprob - first : chunk;
+    dim3 grid;
+    if (MODE == DIB_GEMM_WGRAD)
+      grid = dim3(DIB_CEIL_DIV(L.maxC, BC), DIB_CEIL_DIV(L.maxR, BR), np * L.nsplit);
+    else
+      grid = dim3(DIB_CEIL_DIV(L.M, BR), DIB_CEIL_DIV(L.maxC, BC), np);
+    if (grid.x == 0 || grid.y == 0 || grid.z == 0) return cudaSuccess;
+    dib_gemm_simt_kernel<MODE, BR, BC, BT, TM, TN><<<grid, NT, 0, st>>>(
+        L.probs + first, L.baseA, L.baseB, L.baseC, L.baseX, L.M, L.nsplit, L.rows_per_split, L.split_stride, L.alpha,
+        L.round_out);
+    dib_note_launch();
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
 }
 
 template <int MODE>

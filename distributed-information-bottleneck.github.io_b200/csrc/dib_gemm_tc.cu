@@ -289,7 +289,10 @@ bool dib_gemm_tc_eligible(int mode, const DibGemmProblem* hp, int nprob, const f
   return false;
 }
 
-cudaError_t dib_launch_gemm_tc(int mode, const DibGemmLaunch& L, const DibGemmProblem* hp, cudaStream_t st) {
+namespace {
+
+// one launch over problems hp[0 .. L.nprob) (L.probs: their device copies); the TMA maps start at hp[0]
+cudaError_t launch_group(int mode, const DibGemmLaunch& L, const DibGemmProblem* hp, cudaStream_t st) {
   const DibGemmProblem& p0 = hp[0];
   const int nf = L.nprob;
   const long long sa = nf > 1 ? hp[1].a_off - hp[0].a_off : 0, sb = nf > 1 ? hp[1].b_off - hp[0].b_off : 0;
@@ -323,4 +326,21 @@ cudaError_t dib_launch_gemm_tc(int mode, const DibGemmLaunch& L, const DibGemmPr
   }
 #undef DIB_TC_CASE
   return cudaErrorInvalidValue;
+}
+
+}  // namespace
+
+cudaError_t dib_launch_gemm_tc(int mode, const DibGemmLaunch& L, const DibGemmProblem* hp, cudaStream_t st) {
+  // gridDim.z holds (problem, split): a group with more than 65 535 of them runs as consecutive launches over its problems,
+  // each with TMA maps built from its own first descriptor (the kernel's problem index is relative to the launch)
+  const int chunk = dib_gemm_chunk_problems(L.nprob, mode == DIB_GEMM_WGRAD ? L.nsplit : 1);
+  if (L.nprob > 0 && chunk < 1) return cudaErrorInvalidConfiguration;
+  for (int first = 0; first < L.nprob; first += chunk) {
+    DibGemmLaunch part = L;
+    part.probs = L.probs + first;
+    part.nprob = L.nprob - first < chunk ? L.nprob - first : chunk;
+    const cudaError_t e = launch_group(mode, part, hp + first, st);
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
 }

@@ -25,6 +25,13 @@ struct DibGemmLaunch {
   const float* baseBias = nullptr; // FWD bias base when baseB points at the TF32-rounded weight shadow
 };
 
+// problems per launch of a group whose every problem takes `z_per_problem` grid slices along z (WGRAD: nsplit, else 1):
+// gridDim.z is at most 65 535, so larger groups run as several launches of this many problems (0: one problem does not fit)
+inline int dib_gemm_chunk_problems(int nprob, int z_per_problem) {
+  const int cap = 65535 / (z_per_problem > 0 ? z_per_problem : 1);
+  return nprob < cap ? nprob : cap;
+}
+
 cudaError_t dib_launch_gemm_simt(int mode, const DibGemmLaunch& L, cudaStream_t st);
 
 // TF32 wgmma path (dib_gemm_tc.cu); `hp` = host copies of the group's problem descriptors

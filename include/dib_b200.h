@@ -461,12 +461,27 @@ uint64_t dib_launch_count(void);
 int dib_profile_enable(dib_model* h, int32_t on);
 int32_t dib_profile_read(dib_model* h, char* labels, size_t labels_bytes, float* ms, int32_t capacity);
 
-/* bring-up / unit-test hook: ONE GEMM problem through the tensor-core kernel (use_simt=0) or the fp32 SIMT kernel
- * (use_simt=1); mode 0 FWD (bias = X, act), 1 DGRAD (X = activation source), 2 WGRAD (X = bias-grad partials).
- * Synchronises the stream. */
-int dib_debug_gemm_tc(int32_t mode, const float* A, int32_t lda, const float* B, int32_t ldb, float* Cout, int32_t ldc,
-                      float* X, int32_t ldx, int32_t M, int32_t T, int32_t Ccols, int32_t R, int32_t act,
-                      int32_t nsplit, int32_t rows_per_split, int64_t split_stride, int32_t use_simt, void* stream);
+/* unit-test hook: one grouped GEMM launch of the dense-layer kernels, as the library's own steps issue it.
+ * A group is `nprob` problem descriptors (host memory; the C mirror of the kernels' descriptor) whose offsets, in floats,
+ * are relative to the base pointers: a_off / b_off / c_off to A / B / C, x_off to `bias` (FWD bias), X (DGRAD activation
+ * source) or X (WGRAD bias-gradient partials; x_off < 0: none).  Canonical form Out[R x C] = sum_t Aop[R x T] Bop[T x C]:
+ *   mode 0 FWD    C = act(A[M x T] B[T x C] + bias)      (T = fan-in,  C = fan-out)
+ *   mode 1 DGRAD  C = (A[M x T] B[C x T]^T) * act'(X)    (T = fan-out, C = fan-in; X is the activation output)
+ *   mode 2 WGRAD  for each split s: C + s * split_stride = A[rows of s]^T B[rows of s], X + x_off + s * split_stride = the
+ *                 column sums of B[rows of s]; split s holds batch rows [s * rows_per_split, min(M, (s + 1) * rows_per_split))
+ * maxC / maxR: the largest C / R of the group (grid size).  round_out: round FWD / DGRAD outputs to TF32 (cvt.rna).
+ * kernel: DIB_GEMM_KERNEL_SIMT (exact fp32 FMA) or DIB_GEMM_KERNEL_TC (tf32 wgmma); the tensor-core kernel fails with a message
+ * on a group it cannot run, it never runs another.  The SIMT kernel reads FWD biases from B's base, so it needs bias == B
+ * (or null).  Synchronises the stream. */
+typedef struct dib_gemm_problem {
+  int64_t a_off, b_off, c_off, x_off;
+  int32_t lda, ldb, ldc, ldx;
+  int32_t T, C, R, act;
+} dib_gemm_problem;
+enum { DIB_GEMM_KERNEL_SIMT = 0, DIB_GEMM_KERNEL_TC = 1 };
+int dib_debug_gemm(int32_t kernel, int32_t mode, const dib_gemm_problem* problems, int32_t nprob, const float* A,
+                   const float* B, float* C, float* X, const float* bias, int32_t M, int32_t maxC, int32_t maxR, int32_t nsplit,
+                   int32_t rows_per_split, int64_t split_stride, float alpha, int32_t round_out, void* stream);
 
 /* bring-up switch for THIS handle (bit mask, 0 = the default kernels): 1 = unfused encoder kernels, 2 = integration network on
  * fp32-storage TF32 kernels, 4 = no fused integration tail (per-layer 16-bit GEMMs plus a head kernel), 8 = the generic head
