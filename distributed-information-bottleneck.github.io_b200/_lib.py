@@ -142,6 +142,9 @@ SIGNATURES = {
     "dib_profile_read": (c_int32, [c_void_p, c_char_p, c_size_t, POINTER(c_float), c_int32]),
     "dib_debug_gemm": (c_int32, [c_int32, c_int32, c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                  c_int32, c_int32, c_int32, c_int32, c_int32, c_int64, c_float, c_int32, c_void_p]),
+    "dib_debug_infonce_stream": (c_int32, [c_int32, c_float, c_void_p, c_int32, c_void_p, c_int32, c_int64, c_int32, c_int64,
+                                           c_int64, c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_int32,
+                                           c_void_p, c_int32, c_int32, c_int32, c_void_p]),
     "dib_debug_force_unfused": (c_int32, [c_void_p, c_int32]),
     "dib_last_error": (c_char_p, []),
     "dib_build_info": (c_char_p, []),

@@ -1,6 +1,7 @@
 // dib_api.cu -- the C ABI declared in include/dib_b200.h: model description, workspace plan, and the
 // orchestration of one forward / train step as a fixed sequence of asynchronous launches on the caller's stream.
 #include <atomic>
+#include <cmath>
 #include <cstddef>
 #include <cstdio>
 #include <cstring>
@@ -1218,6 +1219,46 @@ int dib_debug_gemm(int32_t kernel, int32_t mode, const dib_gemm_problem* problem
   cudaFree(dp);
   if (e != cudaSuccess) return fail(std::string("launch: ") + cudaGetErrorString(e));
   if (e2 != cudaSuccess) return fail(std::string("sync: ") + cudaGetErrorString(e2));
+  return 0;
+}
+
+// the streaming InfoNCE sweeps with the arguments infonce_args fills, through the launchers the steps use (unit tests)
+int dib_debug_infonce_stream(int32_t kind, float temperature, const float* e1, int32_t ld1, const float* e2, int32_t ld2,
+                             int64_t n, int32_t d, int64_t row0, int64_t rows, float* lse_r, float* lse_c, int32_t lse_stride,
+                             float* diag, float* loss_sum, float* d_e1, int32_t ld_d1, float* d_e2, int32_t ld_d2,
+                             int32_t round_out, int32_t phases, void* stream) {
+  const char* fn = "dib_debug_infonce_stream: ";
+  if (kind < 0 || kind > 4) return fail(std::string(fn) + "unknown similarity kind " + std::to_string(kind));
+  if (!(temperature > 0.f) || !std::isfinite(temperature)) return fail(std::string(fn) + "needs 0 < temperature < inf");
+  if (d < 1 || d > 512) return fail(std::string(fn) + "needs 1 <= d <= 512 (d = " + std::to_string(d) + ")");
+  if (ld1 < d || ld2 < d) return fail(std::string(fn) + "needs ld1, ld2 >= d");
+  if (n < 1 || n > 0x7fffffffll) return fail(std::string(fn) + "needs 1 <= n < 2^31 (n = " + std::to_string(n) + ")");
+  if (row0 < 0 || rows < 1 || row0 + rows > n)
+    return fail(std::string(fn) + "the own rows [row0, row0 + rows) must be a nonempty range inside [0, n) (row0 = " +
+                std::to_string(row0) + ", rows = " + std::to_string(rows) + ", n = " + std::to_string(n) + ")");
+  if (lse_stride < 1) return fail(std::string(fn) + "needs lse_stride >= 1");
+  if (phases < 1 || phases > 3) return fail(std::string(fn) + "phases is a mask of 1 (loss sweeps) and 2 (gradient sweeps)");
+  if (!e1 || !e2 || !lse_r || !lse_c) return fail(std::string(fn) + "e1, e2, lse_r and lse_c must not be null");
+  if ((phases & 1) && (!diag || !loss_sum)) return fail(std::string(fn) + "the loss sweeps need diag and loss_sum");
+  if ((phases & 2) && ((d_e1 && ld_d1 < d) || (d_e2 && ld_d2 < d))) return fail(std::string(fn) + "needs ld_d1, ld_d2 >= d");
+  DibInfonceStream a;
+  a.kind = kind; a.temperature = temperature;
+  a.e1 = e1; a.ld1 = ld1;
+  a.e2 = e2; a.ld2 = ld2;
+  a.n = n; a.d = d;
+  a.row0 = row0; a.rows = rows;
+  a.lse_r = lse_r; a.lse_c = lse_c; a.lse_stride = lse_stride;
+  a.diag = diag; a.loss_sum = loss_sum; a.acc_zero = nullptr;
+  a.d_e1 = d_e1; a.ld_d1 = ld_d1;
+  a.d_e2 = d_e2; a.ld_d2 = ld_d2;
+  a.round_out = round_out ? 1 : 0;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaError_t e = cudaSuccess;
+  if (phases & 1) e = dib_launch_infonce_stream_loss(a, st);
+  if (e == cudaSuccess && (phases & 2)) e = dib_launch_infonce_stream_grads(a, st);
+  const cudaError_t es = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return fail(std::string("launch: ") + cudaGetErrorString(e));
+  if (es != cudaSuccess) return fail(std::string("sync: ") + cudaGetErrorString(es));
   return 0;
 }
 

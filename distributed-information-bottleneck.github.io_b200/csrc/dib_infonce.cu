@@ -135,7 +135,7 @@ dib_infonce_grad_kernel(int kind, const float* __restrict__ self, const float* _
   extern __shared__ float sm[];
   float* a = sm;                         // [d] this row
   float* w = sm + d;                     // [kGradThreads] dS for the chunk
-  float* ex = w + kGradThreads;          // [kGradThreads] per-pair extra (l2: 1/dist, cosine: c, linf: argmax as float bits)
+  float* ex = w + kGradThreads;          // [kGradThreads] per-pair extra (l2: 1/dist, cosine: c, linf: max_k |a_k - b_k|)
   const int r = blockIdx.x, tid = threadIdx.x;
   for (int k = tid; k < d; k += kGradThreads) a[k] = self[(long long)r * d + k];
   const float lse_r = lse[TRANSPOSED ? n + r : r];
@@ -154,11 +154,16 @@ dib_infonce_grad_kernel(int kind, const float* __restrict__ self, const float* _
       float e = 0.f;
       if (kind == SIM_L2) e = 1.f / (-s / inv_t);                 // sqrt(d2 + eps) = -S T
       else if (kind == SIM_COS) e = s / inv_t;                    // cos(a, b) = S T
-      else if (kind == SIM_LINF) {
+      else if (kind == SIM_LINF) {              // the gradient is split evenly between tied maxima (TF _MinOrMaxGrad)
         const float* b = other + (long long)o * d;
-        float best = -1.f; int bi = 0;
-        for (int k = 0; k < d; ++k) { const float v = fabsf(a[k] - b[k]); if (v > best) { best = v; bi = k; } }
-        e = __int_as_float(bi);
+        float best = -1.f; int ties = 0;
+        for (int k = 0; k < d; ++k) {
+          const float v = fabsf(a[k] - b[k]);
+          if (v > best) { best = v; ties = 1; }
+          else if (v == best) ++ties;
+        }
+        e = best;
+        w[tid] *= 1.f / (float)ties;             // unchanged for one maximum
       }
       ex[tid] = e;
     }
@@ -177,7 +182,7 @@ dib_infonce_grad_kernel(int kind, const float* __restrict__ self, const float* _
             case SIM_L2SQ: t = fmaf(wq, -2.f * df, t); break;
             case SIM_L2: t = fmaf(wq * ex[q], -df, t); break;
             case SIM_L1: t = fmaf(wq, -signf(df), t); break;
-            case SIM_LINF: if (__float_as_int(ex[q]) == k) t = fmaf(wq, -signf(df), t); break;
+            case SIM_LINF: if (fabsf(df) == ex[q]) t = fmaf(wq, -signf(df), t); break;
             default: t = fmaf(wq, (bk / norm_o[o0 + q] - ex[q] * ak * inv_na) * inv_na, t); break;
           }
         }

@@ -50,14 +50,16 @@ __device__ __forceinline__ void stage_rows(const float* __restrict__ m, int ldm,
   }
 }
 
-// the similarities of rows (i0 .. i0+3) of sa with row j of sb, scaled by inv_t; am[] = argmax_k |a_k - b_k| (LINF)
+// the similarities of rows (i0 .. i0+3) of sa with row j of sb, scaled by inv_t.  LINF also gives mx[] = max_k |a_k - b_k|
+// and ties[] = the number of k attaining it: reduce_max's gradient is split evenly between tied maxima (TF _MinOrMaxGrad)
 template <int KIND>
 __device__ __forceinline__ void tile_similarity(const float* sa, int i0, const float* sb, int j, int d, const float* na,
-                                                const float* nb, float inv_t, float (&s)[kRowsPerWarp], int (&am)[kRowsPerWarp]) {
+                                                const float* nb, float inv_t, float (&s)[kRowsPerWarp], float (&mx)[kRowsPerWarp],
+                                                int (&ties)[kRowsPerWarp]) {
   const int ld = smem_ld(d);
   float acc[kRowsPerWarp];
 #pragma unroll
-  for (int r = 0; r < kRowsPerWarp; ++r) { acc[r] = 0.f; am[r] = 0; }
+  for (int r = 0; r < kRowsPerWarp; ++r) { acc[r] = 0.f; ties[r] = 0; }
   const float* b = sb + j * ld;
   for (int k = 0; k < d; ++k) {
     const float bk = b[k];
@@ -66,12 +68,17 @@ __device__ __forceinline__ void tile_similarity(const float* sa, int i0, const f
       const float a = sa[(i0 + r) * ld + k];
       if (KIND == SIM_L2SQ || KIND == SIM_L2) { const float df = a - bk; acc[r] = fmaf(df, df, acc[r]); }
       else if (KIND == SIM_L1) acc[r] += fabsf(a - bk);
-      else if (KIND == SIM_LINF) { const float v = fabsf(a - bk); if (v > acc[r]) { acc[r] = v; am[r] = k; } }
+      else if (KIND == SIM_LINF) {
+        const float v = fabsf(a - bk);
+        if (v > acc[r]) { acc[r] = v; ties[r] = 1; }
+        else if (v == acc[r]) ++ties[r];
+      }
       else acc[r] = fmaf(a, bk, acc[r]);
     }
   }
 #pragma unroll
   for (int r = 0; r < kRowsPerWarp; ++r) {
+    mx[r] = acc[r];
     float v;
     if (KIND == SIM_L2SQ) v = -acc[r];
     else if (KIND == SIM_L2) v = -sqrtf(acc[r] + kL2Eps);
@@ -107,8 +114,8 @@ dib_infonce_lse_kernel(const float* __restrict__ self, int ld_self, const float*
     __syncthreads();
     const int j = j0 + lane;
     if (j >= n) continue;
-    float s[kRowsPerWarp]; int am[kRowsPerWarp];
-    tile_similarity<KIND>(sa, i0, sb, lane, d, na, nb, inv_t, s, am);
+    float s[kRowsPerWarp], dmax[kRowsPerWarp]; int ties[kRowsPerWarp];
+    tile_similarity<KIND>(sa, i0, sb, lane, d, na, nb, inv_t, s, dmax, ties);
 #pragma unroll
     for (int r = 0; r < kRowsPerWarp; ++r) {
       if (s[r] > mx[r]) { sum[r] = sum[r] * expf(mx[r] - s[r]) + 1.f; mx[r] = s[r]; }
@@ -168,7 +175,7 @@ dib_infonce_grad_stream_kernel(const float* __restrict__ self, int ld_self, cons
   float* sb = sa + kTile * ld;
   float* acc = sb + kTile * ld;                       // [kTile][d]
   float* wt = acc + kTile * d;                        // [kTile][kTile + 1]
-  float* ex = wt + kTile * (kTile + 1);               // [kTile][kTile + 1]: l2 1/distance, cosine cos, linf argmax bits
+  float* ex = wt + kTile * (kTile + 1);               // [kTile][kTile + 1]: l2 1/distance, cosine cos, linf max |a_k - b_k|
   float* na = ex + kTile * (kTile + 1);
   float* nb = na + kTile;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, i0 = warp * kRowsPerWarp;
@@ -185,8 +192,8 @@ dib_infonce_grad_stream_kernel(const float* __restrict__ self, int ld_self, cons
     __syncthreads();
     {
       const int j = j0 + lane;
-      float s[kRowsPerWarp]; int am[kRowsPerWarp];
-      tile_similarity<KIND>(sa, i0, sb, lane, d, na, nb, inv_t, s, am);
+      float s[kRowsPerWarp], dmax[kRowsPerWarp]; int ties[kRowsPerWarp];
+      tile_similarity<KIND>(sa, i0, sb, lane, d, na, nb, inv_t, s, dmax, ties);
       const float lo = j < n ? lse_other[(long long)j * lse_stride] : 0.f;
 #pragma unroll
       for (int r = 0; r < kRowsPerWarp; ++r) {
@@ -196,7 +203,7 @@ dib_infonce_grad_stream_kernel(const float* __restrict__ self, int ld_self, cons
           w = (expf(s[r] - lr[r]) + expf(s[r] - lo) - (i == j ? 2.f : 0.f)) * inv_n;
           if (KIND == SIM_L2) e = 1.f / (-s[r] / inv_t);        // sqrt(d2 + eps) = -S T
           else if (KIND == SIM_COS) e = s[r] / inv_t;           // cos(a, b) = S T
-          else if (KIND == SIM_LINF) e = __int_as_float(am[r]);
+          else if (KIND == SIM_LINF) { e = dmax[r]; w *= 1.f / (float)ties[r]; }   // w unchanged for one maximum
         }
         wt[(i0 + r) * (kTile + 1) + lane] = w;
         ex[(i0 + r) * (kTile + 1) + lane] = e;
@@ -218,7 +225,7 @@ dib_infonce_grad_stream_kernel(const float* __restrict__ self, int ld_self, cons
           if (KIND == SIM_L2SQ) t = fmaf(wq, -2.f * df, t);
           else if (KIND == SIM_L2) t = fmaf(wq * er[q], -df, t);
           else if (KIND == SIM_L1) t = fmaf(wq, -((df > 0.f) - (df < 0.f)), t);
-          else if (KIND == SIM_LINF) { if (__float_as_int(er[q]) == k) t = fmaf(wq, -(float)((df > 0.f) - (df < 0.f)), t); }
+          else if (KIND == SIM_LINF) { if (fabsf(df) == er[q]) t = fmaf(wq, -(float)((df > 0.f) - (df < 0.f)), t); }
           else t = fmaf(wq, (bk / nb[q] - er[q] * ak * inv_na) * inv_na, t);
         }
         acc[il * d + k] += t;

@@ -400,14 +400,18 @@ int dib_compression_matrices(dib_model* h, const float* params, const float* x, 
                              float* out_compression, void* workspace, void* stream);
 
 /* NEXT ROW f3 -- utils.get_scaled_similarity (utils.py:127-175; distances utils.py:75-125):
- * kind 0 'l2sq' | 1 'l2' | 2 'l1' | 3 'linf' | 4 'cosine';  e1 [n, d], e2 [m, d] -> out [n, m] = similarity / temperature. */
+ * kind 0 'l2sq' | 1 'l2' | 2 'l1' | 3 'linf' | 4 'cosine';  e1 [n, d], e2 [m, d] -> out [n, m] = similarity / temperature.
+ * Every entry equals, bit for bit, the s_ij the streaming InfoNCE sweeps compute (dib_debug_infonce_stream runs those). */
 int dib_scaled_similarity(int32_t kind, const float* e1, int64_t n, const float* e2, int64_t m, int32_t d,
                           float temperature, float* out, void* stream);
 
 /* NEXT ROW f3 -- the InfoNCE head of the custom training loop (train.py:203-213) and its reverse mode (train.py:216-219):
  *   S = get_scaled_similarity(e1, e2);  out_loss[0] = mean_i CE(i, S[i,:]) + mean_i CE(i, S^T[i,:])   (nats)
  *   d_e1, d_e2 [n, d] = d loss / d e1, d e2 (either may be NULL).  e1 = model(x) (feed d_e1 to dib_train_step of a
- *   DIB_LOSS_EXTERNAL model), e2 = the caller's output encoder.  scratch: n*n + 4n floats.  n <= 32768, d <= 512. */
+ *   DIB_LOSS_EXTERNAL model), e2 = the caller's output encoder.  scratch: n*n + 4n floats.  n <= 32768, d <= 512.
+ *   'linf': the gradient of max_k |a_k - b_k| is split evenly between tied maximal coordinates, as TF's reduce_max does.
+ *   tests/test_gpu_infonce_stream.py checks this head and the streaming sweeps (dib_debug_infonce_stream) element by
+ *   element against float64 with per-element error bounds. */
 int dib_infonce_head(int32_t kind, const float* e1, const float* e2, int64_t n, int32_t d, float temperature,
                      float* scratch, float* out_loss, float* d_e1, float* d_e2, void* stream);
 
@@ -482,6 +486,20 @@ enum { DIB_GEMM_KERNEL_SIMT = 0, DIB_GEMM_KERNEL_TC = 1 };
 int dib_debug_gemm(int32_t kernel, int32_t mode, const dib_gemm_problem* problems, int32_t nprob, const float* A,
                    const float* B, float* C, float* X, const float* bias, int32_t M, int32_t maxC, int32_t maxR, int32_t nsplit,
                    int32_t rows_per_split, int64_t split_stride, float alpha, int32_t round_out, void* stream);
+
+/* unit-test hook: the streaming InfoNCE sweeps of DIB_LOSS_INFONCE, launched as the library's own steps launch them.
+ * kind as dib_scaled_similarity; e1 [n, d] (leading dimension ld1), e2 [n, d] (ld2); the own rows [row0, row0 + rows) of
+ * both sides are swept against all n rows of the other side, and rows past n are never read.  phases: 1 = loss sweeps
+ * (lse_r[i * lse_stride] = r_i and lse_c[i * lse_stride] = c_i for the own i, diag[i - row0] = s_ii, loss_sum[0] =
+ * sum_{own i} (r_i + c_i - 2 s_ii)), 2 = gradient sweeps (read r and c of all n rows from lse_r / lse_c; write d loss / d e1
+ * and d loss / d e2 of the own rows at local index, leading dimensions ld_d1 / ld_d2, pad columns zeroed, rounded to TF32
+ * when round_out; either may be NULL), 3 = both.  Fails with a message unless 1 <= d <= 512, ld1, ld2 >= d,
+ * 0 < temperature < inf, 1 <= n < 2^31, 0 <= row0, 1 <= rows, row0 + rows <= n and lse_stride >= 1.  Synchronises the
+ * stream. */
+int dib_debug_infonce_stream(int32_t kind, float temperature, const float* e1, int32_t ld1, const float* e2, int32_t ld2,
+                             int64_t n, int32_t d, int64_t row0, int64_t rows, float* lse_r, float* lse_c, int32_t lse_stride,
+                             float* diag, float* loss_sum, float* d_e1, int32_t ld_d1, float* d_e2, int32_t ld_d2,
+                             int32_t round_out, int32_t phases, void* stream);
 
 /* bring-up switch for THIS handle (bit mask, 0 = the default kernels): 1 = unfused encoder kernels, 2 = integration network on
  * fp32-storage TF32 kernels, 4 = no fused integration tail (per-layer 16-bit GEMMs plus a head kernel), 8 = the generic head

@@ -629,6 +629,14 @@ def _logsumexp(s, axis):
     return (m + np.log(np.exp(s - m).sum(axis=axis, keepdims=True))).squeeze(axis)
 
 
+def linf_tie_weights(diff):
+    """d max_k |diff_k| / d |diff_k| as TF's reduce_max gradient (_MinOrMaxGrad) takes it: 1 / (number of tied maxima) at
+    every coordinate attaining the maximum, 0 elsewhere.  torch.amax splits it the same way."""
+    ad = np.abs(diff)
+    tied = ad == ad.max(-1, keepdims=True)
+    return tied / tied.sum(-1, keepdims=True)
+
+
 def infonce_loss_and_grads(embeddings1, embeddings2, similarity_type, temperature):
     """train.py:203-213: S = get_scaled_similarity(e1, e2); loss = mean_i CE(i, S[i,:]) + mean_i CE(i, S^T[i,:]).
     Returns (loss, d loss/d e1, d loss/d e2, S) with the analytic reverse mode GradientTape would produce."""
@@ -649,10 +657,7 @@ def infonce_loss_and_grads(embeddings1, embeddings2, similarity_type, temperatur
     elif similarity_type == "l1":
         g = -np.sign(diff) / T
     elif similarity_type == "linf":
-        k = np.abs(diff).argmax(-1)
-        g = np.zeros_like(diff)
-        ii, jj = np.meshgrid(np.arange(n), np.arange(n), indexing="ij")
-        g[ii, jj, k] = -np.sign(diff[ii, jj, k]) / T
+        g = -np.sign(diff) * linf_tie_weights(diff) / T
     if similarity_type == "cosine":
         na, nb = np.linalg.norm(a, axis=-1), np.linalg.norm(b, axis=-1)
         ah, bh = a / na[:, None], b / nb[:, None]

@@ -79,10 +79,7 @@ def infonce_loss_and_grads(e1, e2, similarity_type, temperature, chunk=64, want_
         elif similarity_type == "l1":
             ga = -np.sign(diff) / T
         elif similarity_type == "linf":
-            k = np.abs(diff).argmax(-1)
-            ga = np.zeros_like(diff)
-            ii, jj = np.meshgrid(np.arange(i1 - i0), np.arange(n), indexing="ij")
-            ga[ii, jj, k] = -np.sign(diff[ii, jj, k]) / T
+            ga = -np.sign(diff) * O.linf_tie_weights(diff) / T
         if similarity_type == "cosine":
             ah, bh = a[i0:i1] / na[i0:i1, None], b / nb[:, None]
             c = ah @ bh.T

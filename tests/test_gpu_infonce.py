@@ -263,3 +263,81 @@ def test_rejections_and_abi_2_configs(monkeypatch):
         assert lib.dib_param_count(h) == p_model
     finally:
         lib.dib_destroy(h)
+
+
+def _edge_model(d, similarity, T, precision="fp32"):
+    import dib_b200
+    cfg = O.DIBConfig([2, 1, 2, 1], [128, 128], [256, 256], d)
+    m = dib_b200.DistributedIBNet(cfg.feature_dimensionalities, cfg.feature_encoder_architecture,
+                                  cfg.integration_network_architecture, d, output_activation_fn=None, precision=precision, seed=0)
+    m.compile(optimizer=dib_b200.Adam(1e-3), loss=dib_b200.losses.InfoNCE(YD, YARCH, similarity=similarity, temperature=T))
+    p = IO.glorot(IO.infonce_param_shapes(cfg, YD, YARCH), np.random.default_rng(21)).astype(np.float32)
+    return cfg, m, p
+
+
+def _check_edge(cfg, m, p, n, similarity, T, seed):
+    m.set_flat_weights(p)
+    m.beta.assign(0.01)
+    x, y, eps = data(n, seed)
+    g, st = m.compute_gradients(x, y, eps=eps)
+    g = g.cpu().numpy()
+    g_ref, loss_ref, _ = IO.infonce_train_grads(cfg, p, x, y, eps, 0.01, y_dimensionality=YD, y_encoder_architecture=YARCH,
+                                                similarity=similarity, temperature=T)
+    assert rel_err(g, g_ref) < 5e-5, (similarity, n, rel_err(g, g_ref))
+    for i, v in enumerate(m.trainable_variables):
+        sl = slice(m._var_off[i], m._var_off[i] + v.numel())
+        assert rel_err(g[sl], g_ref[sl]) < 2e-4, (similarity, n, i, rel_err(g[sl], g_ref[sl]))
+    F = cfg.number_features
+    assert abs(st[F].item() / n - loss_ref) < 2e-5 * max(1.0, abs(loss_ref))
+    return g
+
+
+@pytest.mark.parametrize("similarity,n,d", [("l2", 1000, 1), ("l2sq", 1000, 3), ("cosine", 1000, 33), ("l1", 1000, 512),
+                                            ("linf", 1000, 33), ("l2", 1, 64)])
+def test_fp32_step_at_width_and_batch_edges(similarity, n, d):
+    """Embedding widths below, across and at the top of the sweeps' range, a batch that is not a multiple of their 32-row
+    tiles, and n = 1 (loss 0, InfoNCE gradient 0)."""
+    T = temperature_of(similarity)
+    cfg, m, p = _edge_model(d, similarity, T)
+    _check_edge(cfg, m, p, n, similarity, T, 22)
+
+
+def test_linf_step_splits_the_gradient_between_tied_coordinates():
+    """The last Dense of the model and of the output encoder get pairwise equal columns, so e1_i and e2_j repeat every
+    coordinate and max_k |e1_ik - e2_jk| is attained at least twice in every pair: the gradient is split between the tied
+    coordinates as reduce_max's is.  The targets are quantised as well (repeated e2 rows)."""
+    d, n, T = 8, 500, 1.0
+    cfg, m, p = _edge_model(d, "linf", T)
+    shapes = IO.infonce_param_shapes(cfg, YD, YARCH)
+    offs = np.cumsum([0] + [int(np.prod(s)) for s in shapes])
+    for wi in (len(cfg.param_shapes()) - 2, len(shapes) - 2):        # the two last Dense kernels [fan_in, d] and biases [d]
+        W = p[offs[wi]:offs[wi + 1]].reshape(shapes[wi])
+        W[:, 1::2] = W[:, 0::2]
+        b = p[offs[wi + 1]:offs[wi + 2]]
+        b[1::2] = b[0::2]
+    m.set_flat_weights(p)
+    m.beta.assign(0.01)
+    x, y, eps = data(n, 23)
+    y = np.round(y * 2) / 2
+    g, _ = m.compute_gradients(x, y, eps=eps)
+    g = g.cpu().numpy()
+    e1 = m(torch.from_numpy(x).cuda(), eps=eps).cpu().numpy()
+    assert np.array_equal(e1[:, 0::2], e1[:, 1::2])
+    g_ref, _, _ = IO.infonce_train_grads(cfg, p, x, y, eps, 0.01, y_dimensionality=YD, y_encoder_architecture=YARCH,
+                                         similarity="linf", temperature=T)
+    assert rel_err(g, g_ref) < 5e-5, rel_err(g, g_ref)
+
+
+def test_tf32_step_at_a_padded_width():
+    """d = 3: the tensor-core path pads the embedding buffers and rounds the sweeps' gradients to TF32 (round_out)."""
+    out = {}
+    for prec in ("fp32", "tf32"):
+        cfg, m, p = _edge_model(3, "l2", 1.0, precision=prec)
+        m.set_flat_weights(p)
+        m.beta.assign(0.01)
+        x, y, eps = data(1000, 24)
+        g, st = m.compute_gradients(x, y, eps=eps)
+        out[prec] = (g.cpu().numpy(), st.cpu().numpy())
+    F = cfg.number_features
+    assert rel_err(out["tf32"][0], out["fp32"][0]) < 3e-2, rel_err(out["tf32"][0], out["fp32"][0])
+    assert abs(out["tf32"][1][F] - out["fp32"][1][F]) < 5e-3 * abs(out["fp32"][1][F])

@@ -97,3 +97,23 @@ def test_infonce_string_loss_points_to_the_loss_object():
     assert resolve_loss(InfoNCE(6)) == "infonce"
     with pytest.raises(ValueError):
         InfoNCE(6, similarity="hamming")
+
+
+@pytest.mark.parametrize("similarity", O.SIMILARITY_TYPES)
+def test_oracle_head_matches_autograd_on_integer_embeddings(similarity):
+    """Integer-valued embeddings tie max_k |a_k - b_k| in many pairs: the 'linf' gradient is split evenly between the tied
+    coordinates, as TF's reduce_max gradient and torch.amax split it."""
+    import torch
+    rng = np.random.default_rng(7)
+    a, b = rng.integers(-3, 4, (6, 4)).astype(np.float64), rng.integers(-3, 4, (6, 4)).astype(np.float64)
+    b[np.linalg.norm(b, axis=1) == 0, 0] = 1.0
+    a[np.linalg.norm(a, axis=1) == 0, 0] = 1.0
+    ta, tb = torch.tensor(a, requires_grad=True), torch.tensor(b, requires_grad=True)
+    loss_t = IO.torch_infonce(ta, tb, similarity, 1.0)
+    loss_t.backward()
+    for loss, da, db in (O.infonce_loss_and_grads(a, b, similarity, 1.0)[:3], IO.infonce_loss_and_grads(a, b, similarity, 1.0, chunk=4)):
+        assert abs(loss - loss_t.item()) < 1e-12
+        if similarity in ("l2", "l2sq"):
+            continue        # equal rows sit at the reference's clamp of |a|^2 + |b|^2 - 2ab, whose gradient the forms do not share
+        np.testing.assert_allclose(da, ta.grad.numpy(), rtol=0, atol=1e-12)
+        np.testing.assert_allclose(db, tb.grad.numpy(), rtol=0, atol=1e-12)
