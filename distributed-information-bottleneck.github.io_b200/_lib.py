@@ -145,6 +145,15 @@ SIGNATURES = {
     "dib_debug_infonce_stream": (c_int32, [c_int32, c_float, c_void_p, c_int32, c_void_p, c_int32, c_int64, c_int32, c_int64,
                                            c_int64, c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_int32,
                                            c_void_p, c_int32, c_int32, c_int32, c_void_p]),
+    "dib_debug_set_attention": (c_int32, [c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int64, c_int32,
+                                          c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                          c_int32, c_void_p]),
+    "dib_debug_layer_norm": (c_int32, [c_int32, c_void_p, c_void_p, c_int32, c_int64, c_int32, c_void_p, c_void_p, c_float,
+                                       c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32,
+                                       c_void_p, c_void_p, c_void_p, c_int32, c_float, c_void_p, c_int64, c_int64, c_int64,
+                                       c_int32, c_int64, c_int32, c_void_p]),
+    "dib_debug_set_pool": (c_int32, [c_int32, c_void_p, c_int32, c_int32, c_int32, c_int64, c_void_p, c_void_p, c_int32, c_int32,
+                                     c_void_p]),
     "dib_debug_force_unfused": (c_int32, [c_void_p, c_int32]),
     "dib_last_error": (c_char_p, []),
     "dib_build_info": (c_char_p, []),

@@ -1262,6 +1262,115 @@ int dib_debug_infonce_stream(int32_t kind, float temperature, const float* e1, i
   return 0;
 }
 
+// the attention core of a set-transformer block, fixed-size or key-tiled, through the launchers the steps use (unit tests)
+int dib_debug_set_attention(int32_t variable_sizes, int32_t phases, const float* q, const float* k, const float* v,
+                            const float* dout, int32_t ld, int64_t sets, int32_t heads, int32_t L, int32_t dk,
+                            const int32_t* set_sizes, float* o, float* lse, float* dq, float* dk_, float* dv, float* dsum,
+                            int32_t round_out, void* stream) {
+  const std::string fn = "dib_debug_set_attention: ";
+  if (variable_sizes != 0 && variable_sizes != 1) return fail(fn + "variable_sizes is 0 (fixed-size kernels) or 1 (key-tiled)");
+  if (phases < 1 || phases > 3) return fail(fn + "phases is a mask of 1 (forward) and 2 (backward)");
+  const int maxL = variable_sizes ? DIB_MAX_VARIABLE_SET_SIZE : 64;
+  if (L < 1 || L > maxL) return fail(fn + "needs 1 <= L <= " + std::to_string(maxL) + " (L = " + std::to_string(L) + ")");
+  if (dk < 1 || dk > 128) return fail(fn + "needs 1 <= dk <= 128 (dk = " + std::to_string(dk) + ")");
+  if (heads < 1) return fail(fn + "needs heads >= 1");
+  if ((heads * dk) % 4) return fail(fn + "needs heads * dk to be a multiple of 4 (heads * dk = " + std::to_string(heads * dk) + ")");
+  if ((int64_t)ld < (int64_t)heads * dk) return fail(fn + "needs ld >= heads * dk (ld = " + std::to_string(ld) + ")");
+  if (sets < 0 || sets > 65535) return fail(fn + "needs 0 <= sets <= 65535 (sets = " + std::to_string(sets) + ")");
+  if (!q || !k || !v || !o || !lse) return fail(fn + "q, k, v, o and lse must not be null");
+  if ((phases & 2) && (!dout || !dq || !dk_ || !dv)) return fail(fn + "the backward needs dout, dq, dk and dv");
+  if (variable_sizes && !set_sizes) return fail(fn + "the key-tiled kernels need set_sizes");
+  if (variable_sizes && (phases & 2) && !dsum) return fail(fn + "the key-tiled backward needs dsum");
+  DibAttnArgs a;
+  a.q = q; a.k = k; a.v = v; a.ld = ld;
+  a.o = o; a.lse = lse;
+  a.sets = sets; a.heads = heads; a.L = L; a.dk = dk;
+  a.round_out = round_out ? 1 : 0;
+  a.dout = dout; a.dq = dq; a.dk_ = dk_; a.dv = dv;
+  a.set_sizes = variable_sizes ? set_sizes : nullptr; a.dsum = variable_sizes ? dsum : nullptr;
+  DIB_CUDA_OK(variable_sizes ? dib_attn_varlen_prepare() : dib_attn_prepare());
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaError_t e = cudaSuccess;
+  if (phases & 1) e = variable_sizes ? dib_launch_attn_varlen_fwd(a, st) : dib_launch_attn_fwd(a, st);
+  if (e == cudaSuccess && (phases & 2)) e = variable_sizes ? dib_launch_attn_varlen_bwd(a, st) : dib_launch_attn_bwd(a, st);
+  const cudaError_t es = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return fail(std::string("launch: ") + cudaGetErrorString(e));
+  if (es != cudaSuccess) return fail(std::string("sync: ") + cudaGetErrorString(es));
+  return 0;
+}
+
+// LayerNorm(a + b) forward and / or backward of a set-transformer block, set up as forward_set_blocks / backward_set_blocks
+// set them up (unit tests)
+int dib_debug_layer_norm(int32_t phases, const float* a, const float* b, int32_t ld, int64_t rows, int32_t E, const float* gamma,
+                         const float* beta, float epsilon, float* y, float* mean, float* rstd, const float* dy0,
+                         const float* dy1, const float* dy2, const float* dy3, const float* dy_pool, int32_t pool_rows,
+                         const int32_t* set_sizes, float* d_res, float* d_branch, int32_t branch_act, float alpha, float* part,
+                         int64_t split_stride, int64_t gamma_off, int64_t beta_off, int32_t nsplit, int64_t rows_per_split,
+                         int32_t round_out, void* stream) {
+  const std::string fn = "dib_debug_layer_norm: ";
+  if (phases < 1 || phases > 3) return fail(fn + "phases is a mask of 1 (forward) and 2 (backward)");
+  if (E < 1 || E > 128 || E % 4) return fail(fn + "needs 1 <= E <= 128, a multiple of 4 (E = " + std::to_string(E) + ")");
+  if (ld < E) return fail(fn + "needs ld >= E (ld = " + std::to_string(ld) + ")");
+  if (rows < 0) return fail(fn + "needs rows >= 0");
+  if (!(epsilon >= 0.f) || !std::isfinite(epsilon)) return fail(fn + "needs 0 <= epsilon < inf");
+  if (!a || !b || !gamma || !mean || !rstd) return fail(fn + "a, b, gamma, mean and rstd must not be null");
+  if ((phases & 1) && (!beta || !y)) return fail(fn + "the forward needs beta and y");
+  DibLayerNorm l;
+  l.a = a; l.b = b; l.ld = ld; l.rows = rows; l.E = E;
+  l.gamma = gamma; l.beta = beta; l.epsilon = epsilon;
+  l.y = y; l.mean = mean; l.rstd = rstd;
+  l.round_out = round_out ? 1 : 0;
+  DibLayerNormBwd g;
+  if (phases & 2) {
+    if (!d_res || !part) return fail(fn + "the backward needs d_res and part");
+    if (nsplit < 1 || rows_per_split < 1 || (int64_t)nsplit * rows_per_split < rows)
+      return fail(fn + "needs nsplit >= 1, rows_per_split >= 1 and nsplit * rows_per_split >= rows");
+    if (gamma_off < 0 || beta_off < 0 || gamma_off + E > split_stride || beta_off + E > split_stride)
+      return fail(fn + "the d gamma / d beta partial ranges [gamma_off, gamma_off + E), [beta_off, beta_off + E) must lie "
+                       "inside [0, split_stride)");
+    if (dy_pool && pool_rows < 1) return fail(fn + "dy_pool needs pool_rows >= 1");
+    if (set_sizes && !dy_pool) return fail(fn + "set_sizes needs dy_pool");
+    if (d_branch && (branch_act < DIB_ACT_LINEAR || branch_act > DIB_ACT_ELU)) return fail(fn + "unknown branch_act");
+    g.dy[0] = dy0; g.dy[1] = dy1; g.dy[2] = dy2; g.dy[3] = dy3;
+    g.dy_pool = dy_pool; g.pool_rows = pool_rows; g.pool_scale = dy_pool ? 1.f / (float)pool_rows : 0.f; g.set_sizes = set_sizes;
+    g.d_res = d_res; g.d_branch = d_branch; g.branch_act = branch_act; g.alpha = alpha;
+    g.part = part; g.split_stride = split_stride; g.gamma_off = gamma_off; g.beta_off = beta_off;
+    g.nsplit = nsplit; g.rows_per_split = rows_per_split;
+  }
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaError_t e = cudaSuccess;
+  if (phases & 1) e = dib_launch_ln_fwd(l, st);
+  if (e == cudaSuccess && (phases & 2)) e = dib_launch_ln_bwd(l, g, st);
+  const cudaError_t es = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return fail(std::string("launch: ") + cudaGetErrorString(e));
+  if (es != cudaSuccess) return fail(std::string("sync: ") + cudaGetErrorString(es));
+  return 0;
+}
+
+// the mean over each set's rows (fixed or variable sizes) or zero_pad_rows, through the launchers the steps use (unit tests)
+int dib_debug_set_pool(int32_t zero_pad, float* x, int32_t ld, int32_t E, int32_t L, int64_t sets, const int32_t* set_sizes,
+                       float* out, int32_t ldo, int32_t round_out, void* stream) {
+  const std::string fn = "dib_debug_set_pool: ";
+  const int maxL = set_sizes ? DIB_MAX_VARIABLE_SET_SIZE : 64;
+  if (zero_pad != 0 && zero_pad != 1) return fail(fn + "zero_pad is 0 (mean pooling) or 1 (zero_pad_rows)");
+  if (zero_pad && !set_sizes) return fail(fn + "zero_pad_rows needs set_sizes");
+  if (L < 1 || L > maxL) return fail(fn + "needs 1 <= L <= " + std::to_string(maxL) + " (L = " + std::to_string(L) + ")");
+  if (sets < 0 || sets > 65535) return fail(fn + "needs 0 <= sets <= 65535 (sets = " + std::to_string(sets) + ")");
+  if (!x) return fail(fn + "x must not be null");
+  if (!zero_pad && (E < 1 || E > 128 || E % 4 || ld < E || ldo < E || !out))
+    return fail(fn + "mean pooling needs 1 <= E <= 128 a multiple of 4, ld >= E, ldo >= E and out");
+  if (zero_pad && ld < 1) return fail(fn + "needs ld >= 1");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaError_t e;
+  if (zero_pad) e = dib_launch_zero_pad_rows(x, ld, sets * L, L, set_sizes, st);
+  else if (set_sizes) e = dib_launch_pool_varlen_fwd(x, ld, E, L, sets, set_sizes, out, ldo, round_out ? 1 : 0, st);
+  else e = dib_launch_pool_fwd(x, ld, E, L, sets, out, ldo, round_out ? 1 : 0, st);
+  const cudaError_t es = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return fail(std::string("launch: ") + cudaGetErrorString(e));
+  if (es != cudaSuccess) return fail(std::string("sync: ") + cudaGetErrorString(es));
+  return 0;
+}
+
 const char* dib_last_error(void) { return g_last_error.c_str(); }
 
 const char* dib_build_info(void) {

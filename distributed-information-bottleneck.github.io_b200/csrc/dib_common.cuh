@@ -160,6 +160,13 @@ __device__ __forceinline__ float dib_warp_sum(float v) {
   return v;
 }
 
+// the real rows l_s of padded set s.  The sizes live in the caller's device memory and cannot be checked without a sync, so
+// every kernel that reads one treats a size outside [1, Lmax] as the nearest bound: forward and backward then agree.
+__device__ __forceinline__ int dib_set_len(const int* sizes, long long s, int Lmax) {
+  const int l = sizes[s];
+  return l < 1 ? 1 : (l > Lmax ? Lmax : l);
+}
+
 // ---------------------------------------------------------------------------------------------
 // grouped GEMM problem descriptor (one per feature encoder / one for an integration layer).
 // Canonical form  Out[R x C] = sum_t Aop[R x T] * Bop[T x C]; see dib_gemm_simt.cu for the three modes.

@@ -60,7 +60,7 @@ dib_reparam_fwd_kernel(DibReparamArgs a, float* __restrict__ emb, int ldemb, flo
   const long long row = (long long)blockIdx.x * kRowsPerBlock + threadIdx.x;
   const int f = blockIdx.y, E = a.E;
   float kl = 0.f;
-  const bool pad = a.set_sizes && row < a.n && (int)(row % a.set_len) >= a.set_sizes[row / a.set_len];
+  const bool pad = a.set_sizes && row < a.n && (int)(row % a.set_len) >= dib_set_len(a.set_sizes, row / a.set_len, a.set_len);
   if (pad) {                       // a padding particle of a padded set: u = 0, outside the KL
     for (int e = 0; e < E; ++e) {
       emb[row * ldemb + f * E + e] = 0.f;
@@ -107,7 +107,7 @@ dib_reparam_bwd_kernel(DibReparamArgs a, const float* __restrict__ d_emb, int ld
   const float bs = beta_dev[0] * inv_batch;
   const float* o = a.enc_out + (long long)f * a.feat_stride + row * a.ldo;
   float* dq = d_out + (long long)f * a.feat_stride + row * a.ldo;
-  if (a.set_sizes && (int)(row % a.set_len) >= a.set_sizes[row / a.set_len]) {   // padding particle: no gradient
+  if (a.set_sizes && (int)(row % a.set_len) >= dib_set_len(a.set_sizes, row / a.set_len, a.set_len)) {   // padding particle: no gradient
     for (int c = 0; c < a.ldo; ++c) dq[c] = 0.f;
     return;
   }

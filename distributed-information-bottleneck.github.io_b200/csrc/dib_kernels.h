@@ -56,7 +56,7 @@ struct DibReparamArgs {
   int64_t n;
   int round_out = 0;
   // variable set sizes: rows are sets of set_len padded particle rows, set s has set_sizes[s] real ones; a padding row gets
-  // u = 0, no KL and d(mu, logvar) = 0.  nullptr: every row is real
+  // u = 0, no KL and d(mu, logvar) = 0 (set_sizes[s] clamped into [1, set_len], dib_set_len).  nullptr: every row is real
   const int* set_sizes = nullptr; int set_len = 1;
 };
 // u = mu + exp(logvar/2) eps (models.py:108); per-(block,feature) partial sums of the KL (models.py:111-112).
@@ -249,7 +249,8 @@ struct DibAttnArgs {
   int round_out;
   const float* dout; float* dq; float* dk_; float* dv;
   // the key-tiled kernels of sets of different sizes (dib_set_attn_varlen.cu): L is the padded size Lmax, set s has
-  // set_sizes[s] real rows; dsum [sets, heads, L] = rowsum(dO o O), written by the query pass of the backward
+  // set_sizes[s] real rows; dsum [sets, heads, L] = rowsum(dO o O), written by the query pass of the backward.  Every kernel
+  // that reads set sizes takes one outside [1, L] as the nearest bound (dib_set_len)
   const int* set_sizes = nullptr; float* dsum = nullptr;
 };
 size_t dib_attn_smem_bytes(int L, int dk, bool backward);
@@ -275,7 +276,7 @@ struct DibLayerNormBwd {
   float* d_res; float* d_branch; int branch_act; float alpha;
   float* part; long long split_stride; long long gamma_off, beta_off; int nsplit; long long rows_per_split;
   // variable set sizes: the pooled source reaches row p of set s as dy_pool[s] / set_sizes[s] for p < set_sizes[s] and not at
-  // all for the padding rows (pool_scale is then unused)
+  // all for the padding rows (pool_scale is then unused); set_sizes[s] clamped into [1, pool_rows]
   const int* set_sizes = nullptr;
 };
 cudaError_t dib_launch_ln_fwd(const DibLayerNorm& a, cudaStream_t st);

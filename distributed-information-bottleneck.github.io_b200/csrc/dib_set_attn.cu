@@ -191,7 +191,7 @@ ln_bwd_kernel(DibLayerNorm a, DibLayerNormBwd b) {
       float dy = 0.f;
       if (b.dy_pool && b.set_sizes) {          // padded sets of different sizes: the mean over the l real rows
         const long long s = r / b.pool_rows;
-        const int l = b.set_sizes[s];
+        const int l = dib_set_len(b.set_sizes, s, b.pool_rows);
         if (r - s * b.pool_rows < l) dy = b.dy_pool[s * a.ld + e] * (1.f / (float)l);
       } else if (b.dy_pool) {
         dy = b.dy_pool[(r / b.pool_rows) * a.ld + e] * b.pool_scale;

@@ -20,10 +20,7 @@ constexpr int kMaxDk = 128;
 constexpr int kOC = kMaxDk / 16;  // output columns per thread
 constexpr int kSP = kT + 1;       // pitch of the 64 x 64 score tiles
 
-__device__ __forceinline__ int set_len(const DibAttnArgs& a, long long set) {
-  const int l = a.set_sizes[set];
-  return l < 1 ? 1 : (l > a.L ? a.L : l);
-}
+__device__ __forceinline__ int set_len(const DibAttnArgs& a, long long set) { return dib_set_len(a.set_sizes, set, a.L); }
 
 // rows [r0, r0 + kT) of one head of a set into a [kT, dk + 1] tile; rows >= lim are zero
 __device__ __forceinline__ void load_tile(float* dst, const float* src, int ld, long long row0, int col0, int r0, int lim, int dk,
@@ -326,8 +323,7 @@ __global__ void pool_varlen_fwd_kernel(const float* x, int ld, int E, int Lmax, 
   if (i >= sets * ldo) return;
   const long long s = i / ldo;
   const int e = (int)(i % ldo);
-  int l = sizes[s];
-  l = l < 1 ? 1 : (l > Lmax ? Lmax : l);
+  const int l = dib_set_len(sizes, s, Lmax);
   float acc = 0.f;
   if (e < E)
     for (int p = 0; p < l; ++p) acc += x[(s * Lmax + p) * ld + e];
@@ -339,7 +335,7 @@ __global__ void zero_pad_rows_kernel(float* buf, int ld, long long rows, int Lma
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= rows * ld) return;
   const long long r = i / ld, s = r / Lmax;
-  if ((int)(r - s * Lmax) >= sizes[s]) buf[i] = 0.f;
+  if ((int)(r - s * Lmax) >= dib_set_len(sizes, s, Lmax)) buf[i] = 0.f;
 }
 
 size_t smem_fwd(int dk) { return sizeof(float) * (3 * kT * (dk + 1) + kT * kSP); }

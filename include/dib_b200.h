@@ -316,7 +316,8 @@ int dib_set_noise_step_device(dib_model* h, const uint32_t* step_dev);
 /* Variable set sizes: set_sizes_dev is DEVICE memory holding the int32 sizes of the n local sets of the following dib_forward,
  * dib_train_step and dib_integration_forward calls of this handle (data parallel: the sizes of this rank's shard).  The kernels
  * read it on the stream, so one captured graph serves every size vector written into the buffer.  The caller checks
- * 1 <= size <= set_size: out-of-range sizes keep every access in bounds but give meaningless results.  A variable-size handle
+ * 1 <= size <= set_size (the library cannot without a sync): every kernel treats a size outside [1, set_size] as the nearest
+ * bound, so such a set is computed, forward and backward alike, as a set of 1 or of set_size particles.  A variable-size handle
  * without bound sizes fails those calls; NULL unbinds.  Fails on a fixed-size handle. */
 int dib_set_set_sizes_device(dib_model* h, const int32_t* set_sizes_dev);
 
@@ -500,6 +501,48 @@ int dib_debug_infonce_stream(int32_t kind, float temperature, const float* e1, i
                              int64_t n, int32_t d, int64_t row0, int64_t rows, float* lse_r, float* lse_c, int32_t lse_stride,
                              float* diag, float* loss_sum, float* d_e1, int32_t ld_d1, float* d_e2, int32_t ld_d2,
                              int32_t round_out, int32_t phases, void* stream);
+
+/* unit-test hooks of the set-transformer kernels (DIB_INTEGRATION_SET_TRANSFORMER), launched as the library's own steps launch
+ * them; each checks its arguments against the limits dib_create enforces, fails with a message naming the one it rejects, and
+ * synchronises the stream.  tests/test_gpu_set_attention_kernels.py checks them element by element against float64.
+ *
+ * dib_debug_set_attention: the attention core of one block.  variable_sizes 0: the fixed-size kernels (1 <= L <= 64);
+ * 1: the key-tiled masked kernels of padded sets (1 <= L <= DIB_MAX_VARIABLE_SET_SIZE, device int32 set_sizes[sets], each
+ * clamped into [1, L]).  q, k, v, dout, o, dq, dk, dv are [sets * L, heads * dk] with leading dimension ld >= heads * dk;
+ * lse and dsum are [sets, heads, L].  phases: 1 = forward (o, lse), 2 = backward (dq, dk, dv and, key-tiled, dsum =
+ * rowsum(dout o o)) from the o and lse in those buffers, 3 = both.  The key-tiled kernels write zeros to the padding rows of
+ * o / dq / dk / dv and to their lse / dsum slots, and never read the padding rows of q / k / v / dout / o.  round_out rounds
+ * o / dq / dk / dv to TF32.  Needs 1 <= dk <= 128, heads >= 1, heads * dk a multiple of 4, 0 <= sets <= 65535 (0: nothing
+ * is launched). */
+int dib_debug_set_attention(int32_t variable_sizes, int32_t phases, const float* q, const float* k, const float* v,
+                            const float* dout, int32_t ld, int64_t sets, int32_t heads, int32_t L, int32_t dk,
+                            const int32_t* set_sizes, float* o, float* lse, float* dq, float* dk_grad, float* dv, float* dsum,
+                            int32_t round_out, void* stream);
+
+/* dib_debug_layer_norm: y = LayerNorm(a + b) over the E live columns of [rows, ld] rows (biased variance; mean / rstd [rows]
+ * kept), and / or its backward from caller-supplied mean / rstd.  phases: 1 = forward, 2 = backward, 3 = both.  The backward's
+ * dy = dy0 + dy1 + dy2 + dy3 (each nullable, [rows, ld]) + the pooled source: dy_pool [rows / pool_rows, ld] times
+ * fl(1 / pool_rows) on every row, or, with set_sizes, times 1 / l_s on the l_s real rows of each set of pool_rows rows and
+ * nothing on its padding rows.  d_res = d(a + b); d_branch (nullable) = d_res * act'(b) for the activation branch_act
+ * (derivative from the output b, leaky slope alpha).  Split s covers rows [s * rows_per_split, (s + 1) * rows_per_split)
+ * and writes its d gamma / d beta partials (zero for a split past the rows) to part + s * split_stride + gamma_off / beta_off.
+ * y, d_res and d_branch get zeros in their columns E <= e < min(ld, 128).  Needs 1 <= E <= 128 a multiple of 4, ld >= E,
+ * 0 <= epsilon < inf,
+ * and for the backward nsplit * rows_per_split >= rows with both partial ranges inside [0, split_stride). */
+int dib_debug_layer_norm(int32_t phases, const float* a, const float* b, int32_t ld, int64_t rows, int32_t E, const float* gamma,
+                         const float* beta, float epsilon, float* y, float* mean, float* rstd, const float* dy0,
+                         const float* dy1, const float* dy2, const float* dy3, const float* dy_pool, int32_t pool_rows,
+                         const int32_t* set_sizes, float* d_res, float* d_branch, int32_t branch_act, float alpha, float* part,
+                         int64_t split_stride, int64_t gamma_off, int64_t beta_off, int32_t nsplit, int64_t rows_per_split,
+                         int32_t round_out, void* stream);
+
+/* dib_debug_set_pool: zero_pad 0 = out [sets, ldo] = the mean over the L rows of each set of x [sets * L, ld] (E live
+ * columns; out's columns E <= e < ldo zeroed), or with set_sizes over its l_s real rows; zero_pad 1 = zero every column of
+ * the padding rows p >= l_s of x (out unused).  l_s = set_sizes[s] clamped into [1, L].  Needs 1 <= L <= 64 (fixed) or
+ * DIB_MAX_VARIABLE_SET_SIZE (with set_sizes), 0 <= sets <= 65535, and for the mean 1 <= E <= 128 a multiple of 4, ld >= E,
+ * ldo >= E. */
+int dib_debug_set_pool(int32_t zero_pad, float* x, int32_t ld, int32_t E, int32_t L, int64_t sets, const int32_t* set_sizes,
+                       float* out, int32_t ldo, int32_t round_out, void* stream);
 
 /* bring-up switch for THIS handle (bit mask, 0 = the default kernels): 1 = unfused encoder kernels, 2 = integration network on
  * fp32-storage TF32 kernels, 4 = no fused integration tail (per-layer 16-bit GEMMs plus a head kernel), 8 = the generic head
