@@ -79,6 +79,12 @@ class DibGemmProblem(ctypes.Structure):
                 ("T", c_int32), ("C", c_int32), ("R", c_int32), ("act", c_int32)]
 
 
+# one segment of dib_debug_reduce's fixed-order reduction list (struct dib_reduce_seg)
+class DibReduceSeg(ctypes.Structure):
+    _fields_ = [("src", c_void_p), ("row_stride", c_int64), ("nrows", c_int32), ("count", c_int64), ("scale", c_float),
+                ("dst", c_void_p)]
+
+
 GEMM_KERNELS = {"simt": 0, "tc": 1}
 GEMM_MODES = {"fwd": 0, "dgrad": 1, "wgrad": 2}
 
@@ -154,6 +160,17 @@ SIGNATURES = {
                                        c_int32, c_int64, c_int32, c_void_p]),
     "dib_debug_set_pool": (c_int32, [c_int32, c_void_p, c_int32, c_int32, c_int32, c_int64, c_void_p, c_void_p, c_int32, c_int32,
                                      c_void_p]),
+    "dib_debug_reparam": (c_int32, [c_int32, c_void_p, c_int64, c_int32, c_int32, c_int32, c_int64, c_void_p, c_uint64, c_uint32,
+                                    c_void_p, c_uint64, c_void_p, c_int32, c_void_p, c_int32, c_void_p, c_void_p, c_int32,
+                                    c_void_p, c_void_p, c_float, c_void_p, c_int32, c_void_p]),
+    "dib_debug_loss": (c_int32, [c_int32, c_int32, c_float, c_void_p, c_int32, c_void_p, c_int32, c_int64, c_float, c_void_p,
+                                 c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_void_p]),
+    "dib_debug_reduce": (c_int32, [c_int32, c_void_p, c_int64, c_int32, c_int64, c_void_p, c_void_p, c_int32, c_void_p, c_void_p,
+                                   c_int32, c_int64, c_int32, c_void_p]),
+    "dib_debug_pe": (c_int32, [c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int32, c_int32,
+                               c_int64, c_void_p, c_void_p, c_int64, c_int32, c_void_p]),
+    "dib_debug_dropout": (c_int32, [c_void_p, c_void_p, c_int64, c_int32, c_int32, c_int32, c_int64, c_float, c_uint64, c_uint32,
+                                    c_void_p, c_uint64, c_int32, c_int32, c_int32, c_int32, c_void_p]),
     "dib_debug_force_unfused": (c_int32, [c_void_p, c_int32]),
     "dib_last_error": (c_char_p, []),
     "dib_build_info": (c_char_p, []),

@@ -1371,6 +1371,167 @@ int dib_debug_set_pool(int32_t zero_pad, float* x, int32_t ld, int32_t E, int32_
   return 0;
 }
 
+// the reparameterisation forward and / or backward, set up as reparam_args sets them up (unit tests)
+int dib_debug_reparam(int32_t phases, const float* enc_out, int64_t feat_stride, int32_t ldo, int32_t F, int32_t E, int64_t n,
+                      const float* eps, uint64_t seed, uint32_t step, const uint32_t* step_dev, uint64_t sample_offset,
+                      const int32_t* set_sizes, int32_t set_len, float* emb, int32_t ldemb, float* user_emb, float* kl_part,
+                      int32_t nblk_stride, const float* d_emb, const float* beta_dev, float inv_batch, float* d_out,
+                      int32_t round_out, void* stream) {
+  const std::string fn = "dib_debug_reparam: ";
+  if (phases < 1 || phases > 3) return fail(fn + "phases is a mask of 1 (forward) and 2 (backward)");
+  if (F < 1 || F > 65535) return fail(fn + "needs 1 <= F <= 65535 (F = " + std::to_string(F) + ")");
+  if (E < 1) return fail(fn + "needs E >= 1");
+  if ((int64_t)ldo < 2 * (int64_t)E) return fail(fn + "needs ldo >= 2E (ldo = " + std::to_string(ldo) + ")");
+  if (n < 0 || n > 0x7fffffffll) return fail(fn + "needs 0 <= n < 2^31 (n = " + std::to_string(n) + ")");
+  if (feat_stride < n * ldo) return fail(fn + "needs feat_stride >= n * ldo");
+  if (!enc_out) return fail(fn + "enc_out must not be null");
+  if (set_sizes && (set_len < 1 || set_len > DIB_MAX_VARIABLE_SET_SIZE || n % set_len))
+    return fail(fn + "set_sizes needs 1 <= set_len <= " + std::to_string(DIB_MAX_VARIABLE_SET_SIZE) + " dividing n (set_len = " +
+                std::to_string(set_len) + ")");
+  if ((int64_t)ldemb < (int64_t)F * E) return fail(fn + "needs ldemb >= F * E (ldemb = " + std::to_string(ldemb) + ")");
+  if ((phases & 1) && (!emb || !kl_part)) return fail(fn + "the forward needs emb and kl_part");
+  if ((phases & 1) && (int64_t)nblk_stride < (n + 255) / 256) return fail(fn + "needs nblk_stride >= ceil(n / 256)");
+  if ((phases & 2) && (!d_emb || !beta_dev || !d_out)) return fail(fn + "the backward needs d_emb, beta_dev and d_out");
+  DibReparamArgs a;
+  a.enc_out = enc_out; a.feat_stride = feat_stride; a.ldo = ldo;
+  a.eps = eps; a.seed = seed; a.step = step; a.step_dev = step_dev; a.sample_offset = sample_offset;
+  a.F = F; a.E = E; a.n = n; a.round_out = round_out ? 1 : 0;
+  a.set_sizes = set_sizes; a.set_len = set_sizes ? set_len : 1;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaError_t e = cudaSuccess;
+  if (phases & 1) e = dib_launch_reparam_fwd(a, emb, ldemb, user_emb, kl_part, nblk_stride, st);
+  if (e == cudaSuccess && (phases & 2)) e = dib_launch_reparam_bwd(a, d_emb, ldemb, beta_dev, inv_batch, d_out, st);
+  const cudaError_t es = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return fail(std::string("launch: ") + cudaGetErrorString(e));
+  if (es != cudaSuccess) return fail(std::string("sync: ") + cudaGetErrorString(es));
+  return 0;
+}
+
+// the compiled loss, its accuracy and d loss / d z of n rows, as the step's loss phase launches it (unit tests)
+int dib_debug_loss(int32_t loss, int32_t out_act, float alpha, const float* pred, int32_t ldp, const float* y, int32_t out_dim,
+                   int64_t n, float inv_batch, const float* weights, float* d_pred, float* user_pred, float* loss_part,
+                   float* acc_part, int32_t round_out, void* stream) {
+  const std::string fn = "dib_debug_loss: ";
+  if (loss < DIB_LOSS_BCE_LOGITS || loss > DIB_LOSS_BCE_PROBS) return fail(fn + "unknown loss " + std::to_string(loss));
+  if (out_act < DIB_ACT_LINEAR || out_act > DIB_ACT_ELU) return fail(fn + "unknown out_act " + std::to_string(out_act));
+  if (out_dim < 1) return fail(fn + "needs out_dim >= 1");
+  if (ldp < out_dim) return fail(fn + "needs ldp >= out_dim (ldp = " + std::to_string(ldp) + ")");
+  if (n < 0 || n > 0x7fffffffll) return fail(fn + "needs 0 <= n < 2^31 (n = " + std::to_string(n) + ")");
+  if (weights && loss == DIB_LOSS_EXTERNAL) return fail(fn + "the external loss takes no sample weights");
+  if (!pred || !loss_part || !acc_part) return fail(fn + "pred, loss_part and acc_part must not be null");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const cudaError_t e = dib_launch_loss(loss, out_act, alpha, pred, ldp, y, out_dim, n, inv_batch, d_pred, user_pred, loss_part,
+                                        acc_part, round_out ? 1 : 0, weights, st);
+  const cudaError_t es = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return fail(std::string("launch: ") + cudaGetErrorString(e));
+  if (es != cudaSuccess) return fail(std::string("sync: ") + cudaGetErrorString(es));
+  return 0;
+}
+
+// the header's C mirror of a reduction segment: the test hook hands its array to the launcher as it is
+static_assert(sizeof(dib_reduce_seg) == sizeof(DibReduceSeg), "dib_reduce_seg size");
+static_assert(offsetof(dib_reduce_seg, src) == offsetof(DibReduceSeg, src) &&
+              offsetof(dib_reduce_seg, row_stride) == offsetof(DibReduceSeg, row_stride) &&
+              offsetof(dib_reduce_seg, nrows) == offsetof(DibReduceSeg, nrows) &&
+              offsetof(dib_reduce_seg, count) == offsetof(DibReduceSeg, count) &&
+              offsetof(dib_reduce_seg, scale) == offsetof(DibReduceSeg, scale) &&
+              offsetof(dib_reduce_seg, dst) == offsetof(DibReduceSeg, dst), "dib_reduce_seg layout");
+
+// the step's fixed-order reductions: reduce_partials, reduce_segments or finalize_stats (unit tests)
+int dib_debug_reduce(int32_t kind, const float* src, int64_t row_stride, int32_t nrows, int64_t count, float* dst,
+                     const dib_reduce_seg* segs, int32_t nseg, const float* loss_part, const float* acc_part, int32_t nblk_loss,
+                     int64_t n, int32_t has_y, void* stream) {
+  const std::string fn = "dib_debug_reduce: ";
+  auto shape_ok = [&](const std::string& what, int64_t rs, int64_t nr, int64_t cnt) -> bool {
+    if (cnt < 0 || cnt > 0x7fffffffll || nr < 0 || (nr > 1 && rs < cnt)) {
+      fail(fn + what + " needs 0 <= count < 2^31, nrows >= 0 and row_stride >= count (count = " + std::to_string(cnt) +
+           ", nrows = " + std::to_string(nr) + ", row_stride = " + std::to_string(rs) + ")");
+      return false;
+    }
+    return true;
+  };
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaError_t e;
+  if (kind == 0) {
+    if (!shape_ok("reduce_partials", row_stride, nrows, count)) return 1;
+    if (count > 0 && (!src || !dst)) return fail(fn + "src and dst must not be null");
+    e = dib_launch_reduce_partials(src, row_stride, nrows, count, dst, st);
+  } else if (kind == 1) {
+    if (nseg < 0 || (nseg > 0 && !segs)) return fail(fn + "needs nseg >= 0 segments");
+    for (int s = 0; s < nseg; ++s) {
+      if (segs[s].count <= 0) continue;
+      if (!shape_ok("segment " + std::to_string(s), segs[s].row_stride, segs[s].nrows, segs[s].count)) return 1;
+      if (!segs[s].src || !segs[s].dst) return fail(fn + "segment " + std::to_string(s) + ": src and dst must not be null");
+    }
+    e = dib_launch_reduce_segments(reinterpret_cast<const DibReduceSeg*>(segs), nseg, st);
+  } else if (kind == 2) {
+    if (nrows < 1) return fail(fn + "finalize_stats needs nrows = F >= 1");
+    if (!shape_ok("finalize_stats", row_stride, nrows, count)) return 1;
+    if (nblk_loss < 0 || n < 0) return fail(fn + "finalize_stats needs nblk_loss >= 0 and n >= 0");
+    if (!src || !dst || (has_y && nblk_loss > 0 && (!loss_part || !acc_part)))
+      return fail(fn + "finalize_stats needs src, dst and, with has_y, loss_part and acc_part");
+    e = dib_launch_finalize_stats(src, (int)row_stride, (int)count, loss_part, acc_part, nblk_loss, nrows, n, has_y ? 1 : 0, dst, st);
+  } else {
+    return fail(fn + "kind is 0 (reduce_partials), 1 (reduce_segments) or 2 (finalize_stats)");
+  }
+  const cudaError_t es = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return fail(std::string("launch: ") + cudaGetErrorString(e));
+  if (es != cudaSuccess) return fail(std::string("sync: ") + cudaGetErrorString(es));
+  return 0;
+}
+
+// the step's positional encoding (dib_launch_pe) with caller tables; the hook reads the tables to check them (unit tests)
+int dib_debug_pe(const float* x, int32_t ldx, int32_t x_col_shift, const int32_t* col_src, const int32_t* col_freq,
+                 int32_t col_begin, int32_t col_end, float* pe, int32_t ldpe, int32_t pe_col_shift, int64_t n,
+                 const int32_t* row_index, const int32_t* col_feat, int64_t n_src, int32_t round_out, void* stream) {
+  const std::string fn = "dib_debug_pe: ";
+  if (col_begin < 0 || col_end < col_begin) return fail(fn + "needs 0 <= col_begin <= col_end");
+  if (n < 0 || n > 0x7fffffffll) return fail(fn + "needs 0 <= n < 2^31 (n = " + std::to_string(n) + ")");
+  if (!x || !col_src || !col_freq || !pe) return fail(fn + "x, col_src, col_freq and pe must not be null");
+  if (row_index && (!col_feat || n_src < 1)) return fail(fn + "row_index needs col_feat and n_src >= 1");
+  std::vector<int32_t> src(col_end), feat(row_index ? col_end : 0);
+  if (col_end > 0) {
+    DIB_CUDA_OK(cudaMemcpy(src.data(), col_src, col_end * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    if (row_index) DIB_CUDA_OK(cudaMemcpy(feat.data(), col_feat, col_end * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  }
+  for (int c = col_begin; c < col_end; ++c) {
+    if (c - pe_col_shift < 0 || c - pe_col_shift >= ldpe)
+      return fail(fn + "column " + std::to_string(c) + " lands outside [0, ldpe) after pe_col_shift");
+    if (src[c] >= 0 && (src[c] - x_col_shift < 0 || src[c] - x_col_shift >= ldx))
+      return fail(fn + "col_src[" + std::to_string(c) + "] reads outside [0, ldx) after x_col_shift");
+    if (row_index && src[c] >= 0 && feat[c] < 0) return fail(fn + "col_feat[" + std::to_string(c) + "] < 0");
+  }
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const cudaError_t e = dib_launch_pe(x, ldx, x_col_shift, col_src, col_freq, col_begin, col_end, pe, ldpe, pe_col_shift, n,
+                                      round_out ? 1 : 0, st, row_index, col_feat, n_src);
+  const cudaError_t es = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return fail(std::string("launch: ") + cudaGetErrorString(e));
+  if (es != cudaSuccess) return fail(std::string("sync: ") + cudaGetErrorString(es));
+  return 0;
+}
+
+// the encoders' Keras Dropout, forward or backward in place, as the step launches it (unit tests)
+int dib_debug_dropout(const float* src, float* dst, int64_t feat_stride, int32_t ld, int32_t width, int32_t F, int64_t n,
+                      float rate, uint64_t seed, uint32_t step, const uint32_t* step_dev, uint64_t sample_offset, int32_t layer,
+                      int32_t feature, int32_t backward, int32_t round_out, void* stream) {
+  const std::string fn = "dib_debug_dropout: ";
+  if (!(rate >= 0.f && rate < 1.f)) return fail(fn + "needs 0 <= rate < 1");
+  if (width < 1 || ld < width) return fail(fn + "needs width >= 1 and ld >= width (width = " + std::to_string(width) + ")");
+  if (F < 1 || F > 65535) return fail(fn + "needs 1 <= F <= 65535 (F = " + std::to_string(F) + ")");
+  if (feature < -1 || feature >= F) return fail(fn + "needs -1 <= feature < F (feature = " + std::to_string(feature) + ")");
+  if (layer < 0 || layer > 127) return fail(fn + "needs 0 <= layer < 128 (layer = " + std::to_string(layer) + ")");
+  if (n < 0 || n > 0x7fffffffll) return fail(fn + "needs 0 <= n < 2^31 (n = " + std::to_string(n) + ")");
+  if (feat_stride < n * ld) return fail(fn + "needs feat_stride >= n * ld");
+  if (!dst || (!backward && !src)) return fail(fn + "needs dst, and src for the forward");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const cudaError_t e = dib_launch_dropout(backward ? nullptr : src, dst, feat_stride, ld, width, F, n, rate, seed, step, step_dev,
+                                           sample_offset, layer, feature, backward ? 1 : 0, round_out ? 1 : 0, st);
+  const cudaError_t es = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return fail(std::string("launch: ") + cudaGetErrorString(e));
+  if (es != cudaSuccess) return fail(std::string("sync: ") + cudaGetErrorString(es));
+  return 0;
+}
+
 const char* dib_last_error(void) { return g_last_error.c_str(); }
 
 const char* dib_build_info(void) {

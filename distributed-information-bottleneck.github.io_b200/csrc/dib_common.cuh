@@ -80,6 +80,20 @@ __device__ __forceinline__ float dib_loss_add_w(int loss, float z, float t, floa
   return g;
 }
 
+// The class a sparse label t names among C, as Keras on a GPU reads it: t is cast to an integer by truncation and is valid
+// when -1 < t < C; any other t (NaN included) gives -1, and the callers then return a NaN loss, a NaN d loss / d z for the
+// whole row and no accuracy hit.  An accuracy hit is (float)argmax == t, so a label of 2.7 names class 2 but never hits.
+__device__ __forceinline__ int dib_sparse_label(float t, int C) { return (t > -1.f && t < (float)C) ? (int)t : -1; }
+
+// 2 KL(N(mu, e^lv) || N(0, 1)) = mu^2 + (e^lv - 1 - lv).  e^lv - 1 - lv = lv^2/2 + lv^3/6 + ... is formed from terms near 1
+// and loses all relative accuracy as lv -> 0, which is where high beta drives the unused features; expm1f keeps it above
+// |lv| = 1/16 and a short series takes over below (its first dropped term is lv^4/360 relative, under 2^-24), in the way
+// dib_neg_log treats -ln(u) near 1.
+__device__ __forceinline__ float dib_kl_term(float mu, float lv) {
+  const float series = lv * lv * (0.5f + lv * (0.16666667f + lv * (0.041666668f + lv * 0.008333334f)));
+  return fmaf(mu, mu, fabsf(lv) < 0.0625f ? series : expm1f(lv) - lv);
+}
+
 // dib_loss_add, weighted (W) or not: the one switch the loss epilogues of the WEIGHTED kernel instantiations go through
 template <bool W>
 __device__ __forceinline__ float dib_loss_add_t(int loss, float z, float t, float w, float& l, float& acc) {

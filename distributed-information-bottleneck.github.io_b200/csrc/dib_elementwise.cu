@@ -84,7 +84,7 @@ dib_reparam_fwd_kernel(DibReparamArgs a, float* __restrict__ emb, int ldemb, flo
           const float s = expf(0.5f * lv);
           const float z = ep ? ep[e] : nrm[j];
           const float u = fmaf(s, z, mu);
-          kl += 0.5f * (mu * mu + expf(lv) - lv - 1.f);
+          kl += 0.5f * dib_kl_term(mu, lv);
           dst[e] = dib_maybe_round(u, a.round_out);
           if (udst) udst[e] = u;
         }
@@ -97,7 +97,7 @@ dib_reparam_fwd_kernel(DibReparamArgs a, float* __restrict__ emb, int ldemb, flo
   if (threadIdx.x == 0) kl_part[(long long)f * nblk_stride + blockIdx.x] = s;
 }
 
-// d mu = du + beta*mu/B ; d logvar = du*eps*0.5*sigma + beta*0.5*(exp(logvar)-1)/B
+// d mu = du + beta*mu/B ; d logvar = du*eps*0.5*sigma + beta*0.5*expm1(logvar)/B
 __global__ void __launch_bounds__(kRowsPerBlock)
 dib_reparam_bwd_kernel(DibReparamArgs a, const float* __restrict__ d_emb, int ldemb, const float* __restrict__ beta_dev,
                        float inv_batch, float* __restrict__ d_out) {
@@ -124,7 +124,7 @@ dib_reparam_bwd_kernel(DibReparamArgs a, const float* __restrict__ d_emb, int ld
         const float s = expf(0.5f * lv);
         const float z = ep ? ep[e] : nrm[j];
         dq[e] = dib_maybe_round(fmaf(bs, mu, g), a.round_out);
-        dq[E + e] = dib_maybe_round(fmaf(g * z, 0.5f * s, bs * 0.5f * (expf(lv) - 1.f)), a.round_out);
+        dq[E + e] = dib_maybe_round(fmaf(g * z, 0.5f * s, bs * 0.5f * expm1f(lv)), a.round_out);
       }
     }
   }
@@ -158,18 +158,20 @@ dib_loss_kernel(int loss, int out_act, float alpha, const float* __restrict__ pr
     } else if (y) {
       const float inv_out = 1.f / (float)out_dim;
       if (loss == DIB_LOSS_SPARSE_CE_LOGITS) {
-        const int label = (int)y[row];
+        const float t = y[row];
+        const int label = dib_sparse_label(t, out_dim);
+        const float bad = label < 0 ? __int_as_float(0x7fc00000) : 0.f;     // NaN loss and gradient for an invalid label
         float m = z[0]; int am = 0;
         for (int j = 1; j < out_dim; ++j) if (z[j] > m) { m = z[j]; am = j; }
         float se = 0.f;
         for (int j = 0; j < out_dim; ++j) se += expf(z[j] - m);
-        l = m + logf(se) - z[label];
+        l = m + logf(se) - z[label < 0 ? 0 : label] + bad;
         if constexpr (WEIGHTED) l *= w;
-        acc = (am == label) ? 1.f : 0.f;
+        acc = ((float)am == t) ? 1.f : 0.f;
         if (dz) {
           const float inv_se = 1.f / se;
           for (int j = 0; j < out_dim; ++j) {
-            const float g = expf(z[j] - m) * inv_se - (j == label ? 1.f : 0.f);
+            const float g = expf(z[j] - m) * inv_se - (j == label ? 1.f : 0.f) + bad;
             dz[j] = dib_maybe_round(g * inv_batch * dib_act_grad(out_act, z[j], alpha), round_out);
           }
         }
@@ -505,9 +507,10 @@ cudaError_t dib_launch_copy2d(const float* src, int lds, float* dst, int ldd, in
 
 cudaError_t dib_launch_adam(float* params, const float* grads, float* m, float* v, int64_t count, const float* lr_dev,
                             int32_t* step_dev, float b1, float b2, float eps, cudaStream_t st) {
-  if (count > 0)
+  if (count > 0) {
     dib_adam_kernel<<<nblocks(count, 256), 256, 0, st>>>(params, grads, m, v, count, lr_dev, step_dev, b1, b2, eps);
-  dib_note_launch();
+    dib_note_launch();
+  }
   dib_inc_step_kernel<<<1, 1, 0, st>>>(step_dev);
   dib_note_launch();
   return cudaGetLastError();
@@ -591,10 +594,11 @@ dib_reduce_segments_kernel(const ReduceSegsArg A) {
 }  // namespace
 
 cudaError_t dib_launch_reduce_segments(const DibReduceSeg* segs, int nseg, cudaStream_t st) {
-  for (int base = 0; base < nseg; base += kDibMaxReduceSegs) {
+  for (int base = 0; base < nseg;) {            // each launch takes up to kDibMaxReduceSegs live segments from where the last stopped
     ReduceSegsArg A{};
     int nb = 0, n = 0;
-    for (int k = base; k < nseg && n < kDibMaxReduceSegs; ++k) {
+    for (; base < nseg && n < kDibMaxReduceSegs; ++base) {
+      const int k = base;
       if (segs[k].count <= 0) continue;
       A.seg[n] = segs[k]; A.first_block[n] = nb;
       A.flat[n] = (segs[k].nrows <= 64 && segs[k].count >= 4096) ? 1 : 0;

@@ -506,7 +506,10 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
         float wr = 1.f;
         if constexpr (WEIGHTED) { wr = a.wts[row]; ib *= wr; }
         float l = -0.f, acc1 = -0.f;
-        if (a.loss == DIB_LOSS_SPARSE_CE_LOGITS) { l = 0.f; acc1 = (int)t == 0 ? 1.f : 0.f; }   // one class: the softmax is constant
+        if (a.loss == DIB_LOSS_SPARSE_CE_LOGITS) {   // one class: the softmax is constant; an invalid label gives NaN
+          l = dz = dib_sparse_label(t, 1) < 0 ? __int_as_float(0x7fc00000) : 0.f;
+          acc1 = t == 0.f ? 1.f : 0.f;
+        }
         else dz = dib_loss_add_t<WEIGHTED>(a.loss, z, t, wr, l, acc1);
         if (q == 0) { lsum += l; asum += acc1; }
       }
@@ -708,17 +711,18 @@ dib_int16_head_kernel(const uint16_t* __restrict__ g, int ldg, int K, const floa
         float l = 0.f, acc = 0.f;
         const float inv_out = 1.f / (float)out_dim;
         if (loss == DIB_LOSS_SPARSE_CE_LOGITS) {
-          const int label = (int)y[row];
-          float m = z[0], zl = 0.f, se = 0.f; int am = 0;
+          const int label = dib_sparse_label(y[row], out_dim);     // < 0: NaN loss and gradient (an invalid label)
+          float m = z[0], zl = __int_as_float(0x7fc00000), se = 0.f; int am = 0;
 #pragma unroll
           for (int o = 1; o < OUT; ++o) if (o < out_dim && z[o] > m) { m = z[o]; am = o; }
 #pragma unroll
           for (int o = 0; o < OUT; ++o) if (o < out_dim) { se += expf(z[o] - m); if (o == label) zl = z[o]; }
           l = m + logf(se) - zl;
           if constexpr (WEIGHTED) l *= wr;
-          acc = am == label ? 1.f : 0.f;
+          acc = (float)am == y[row] ? 1.f : 0.f;
 #pragma unroll
-          for (int o = 0; o < OUT; ++o) if (o < out_dim) dz[o] = expf(z[o] - m) / se - (o == label ? 1.f : 0.f);
+          for (int o = 0; o < OUT; ++o)
+            if (o < out_dim) dz[o] = label < 0 ? __int_as_float(0x7fc00000) : expf(z[o] - m) / se - (o == label ? 1.f : 0.f);
         } else {
 #pragma unroll
           for (int o = 0; o < OUT; ++o) if (o < out_dim) {
@@ -868,7 +872,10 @@ dib_int16_head1_kernel(const uint16_t* __restrict__ g, int ldg, int K, const flo
       float wr = 1.f;
       if constexpr (WEIGHTED) { wr = wts[mrow]; ib *= wr; }
       float l = -0.f, acc = -0.f;
-      if (loss == DIB_LOSS_SPARSE_CE_LOGITS) { l = 0.f; acc = (int)t == 0 ? 1.f : 0.f; }        // one class: the softmax is constant
+      if (loss == DIB_LOSS_SPARSE_CE_LOGITS) {     // one class: the softmax is constant; an invalid label gives NaN
+        l = dz = dib_sparse_label(t, 1) < 0 ? __int_as_float(0x7fc00000) : 0.f;
+        acc = t == 0.f ? 1.f : 0.f;
+      }
       else dz = dib_loss_add_t<WEIGHTED>(loss, z, t, wr, l, acc);
       if (lane < ROWS) { lsum += l; asum += acc; }
     }

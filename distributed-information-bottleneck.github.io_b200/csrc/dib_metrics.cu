@@ -30,7 +30,7 @@ __device__ __forceinline__ float mean_metric(int kind, int from_logits, float th
       for (int j = 1; j < out_dim; ++j) if (zr[j] > m) { m = zr[j]; am = j; }
       return (float)am == t ? 1.f : 0.f;
     }
-    const int label = (t > -1.f && t < (float)out_dim) ? (int)t : -1;     // truncation, as Keras' int64 cast
+    const int label = dib_sparse_label(t, out_dim);
     if (label < 0) return __int_as_float(0x7fc00000);
     if (from_logits) {
       float m = zr[0];

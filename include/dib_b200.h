@@ -50,7 +50,10 @@ enum dib_activation {
 /* compiled losses used by the reference's datasets (data.py:65, data.py:343, data.py:129). */
 enum dib_loss {
   DIB_LOSS_BCE_LOGITS = 0,       /* tf.keras.losses.BinaryCrossentropy(from_logits=True)            */
-  DIB_LOSS_SPARSE_CE_LOGITS = 1, /* tf.keras.losses.SparseCategoricalCrossentropy(from_logits=True) */
+  /* tf.keras.losses.SparseCategoricalCrossentropy(from_logits=True).  As TensorFlow on a GPU: a label t names class (int)t
+   * (truncation) when -1 < t < output_dimensionality; any other label (NaN included) gives a NaN loss and a NaN d loss / d z
+   * for its row, and no accuracy hit.  An accuracy hit is float(argmax z) == t. */
+  DIB_LOSS_SPARSE_CE_LOGITS = 1,
   DIB_LOSS_MSE = 2,
   /* NEXT ROW f3 -- custom training steps (GradientTape loops: train.py:201-220 InfoNCE, nb-bool cell 6, nb-particle
    * cell 7): the CALLER owns the task loss.  dib_forward returns the predictions; in dib_train_step the `y` argument
@@ -543,6 +546,71 @@ int dib_debug_layer_norm(int32_t phases, const float* a, const float* b, int32_t
  * ldo >= E. */
 int dib_debug_set_pool(int32_t zero_pad, float* x, int32_t ld, int32_t E, int32_t L, int64_t sets, const int32_t* set_sizes,
                        float* out, int32_t ldo, int32_t round_out, void* stream);
+
+/* unit-test hooks of the elementwise kernels of every training step (csrc/dib_elementwise.cu), launched through the launchers
+ * the step uses; each checks its arguments against the limits dib_create enforces, fails with a message naming the one it
+ * rejects, and synchronises the stream.  tests/test_gpu_elementwise_kernels.py checks them element by element against float64.
+ *
+ * dib_debug_reparam: phases 1 = forward: emb[row, f E + e] = u = mu + exp(lv / 2) z (TF32-rounded when round_out; columns
+ * F E <= c < ldemb zeroed), user_emb [n, F E] (nullable) = u unrounded, kl_part[f * nblk_stride + b] = the KL of feature f summed
+ * over the 256 rows of block b; 2 = backward: d_out (enc_out's layout) = (du + beta inv_batch mu | du z sigma / 2 + beta inv_batch
+ * expm1(lv) / 2 | zeros up to ldo) from d_emb [n, ldemb] and beta_dev[0]; 3 = both.  enc_out: feature f's row r is
+ * (mu[E] | lv[E] | pad) at f * feat_stride + r * ldo.  z = eps[(r F + f) E + e] when eps is given, else the Philox normal of
+ * (seed, step + *step_dev, sample_offset + r, f).  With set_sizes (device int32, n / set_len sets, each clamped into
+ * [1, set_len]) a padding row gets u = 0, no KL and a zero gradient.  Needs 1 <= F <= 65535, E >= 1, ldo >= 2E,
+ * feat_stride >= n ldo, ldemb >= F E, 0 <= n < 2^31, nblk_stride >= ceil(n / 256) and 1 <= set_len <= DIB_MAX_VARIABLE_SET_SIZE
+ * dividing n. */
+int dib_debug_reparam(int32_t phases, const float* enc_out, int64_t feat_stride, int32_t ldo, int32_t F, int32_t E, int64_t n,
+                      const float* eps, uint64_t seed, uint32_t step, const uint32_t* step_dev, uint64_t sample_offset,
+                      const int32_t* set_sizes, int32_t set_len, float* emb, int32_t ldemb, float* user_emb, float* kl_part,
+                      int32_t nblk_stride, const float* d_emb, const float* beta_dev, float inv_batch, float* d_out,
+                      int32_t round_out, void* stream);
+
+/* dib_debug_loss: the compiled loss of n rows of pred [n, ldp] (out_dim live columns) against y (sparse CE: [n] labels, the
+ * external loss: d task loss / d pred [n, out_dim], else [n, out_dim]; NULL: no loss) with the output activation out_act
+ * (derivative from the output): d_pred [n, ldp] (nullable; columns out_dim <= c < ldp zeroed), user_pred [n, out_dim]
+ * (nullable), and per 256-row block b loss_part[b] / acc_part[b] = the block's sums of the rows' loss and accuracy.  weights
+ * (nullable, not with DIB_LOSS_EXTERNAL): the rows' sample weights.  Needs loss != DIB_LOSS_INFONCE, a known out_act,
+ * out_dim >= 1, ldp >= out_dim and 0 <= n < 2^31. */
+int dib_debug_loss(int32_t loss, int32_t out_act, float alpha, const float* pred, int32_t ldp, const float* y, int32_t out_dim,
+                   int64_t n, float inv_batch, const float* weights, float* d_pred, float* user_pred, float* loss_part,
+                   float* acc_part, int32_t round_out, void* stream);
+
+/* dib_debug_reduce: kind 0 = the batch-split partial sum: dst[i] = sum_{k < nrows} src[k row_stride + i], i < count;
+ * kind 1 = the nseg segments (host array) of one fixed-order reduction list, as the training step hands it over: segment s
+ * writes dst[i] = scale sum_{k < nrows} src[k row_stride + i] for i < count, and a segment with count <= 0 is skipped; the
+ * list runs as ceil(live segments / 8) launches; kind 2 = the step statistics: dst[f] = sum_{b < count} src[f row_stride + b]
+ * for f < nrows = F, dst[F] / dst[F + 1] = the sums of loss_part / acc_part [nblk_loss] (0 unless has_y), dst[F + 2] = n.
+ * Needs count >= 0, nrows >= 0 (kind 2: >= 1), row_stride >= count and count < 2^31 in every reduction. */
+typedef struct dib_reduce_seg {
+  const float* src;
+  int64_t row_stride;
+  int32_t nrows;
+  int64_t count;
+  float scale;
+  float* dst;
+} dib_reduce_seg;
+int dib_debug_reduce(int32_t kind, const float* src, int64_t row_stride, int32_t nrows, int64_t count, float* dst,
+                     const dib_reduce_seg* segs, int32_t nseg, const float* loss_part, const float* acc_part, int32_t nblk_loss,
+                     int64_t n, int32_t has_y, void* stream);
+
+/* dib_debug_pe: the positional encoding of the step into pe [n, ldpe]: for every column col in [col_begin, col_end) of the
+ * device tables col_src / col_freq (/ col_feat), pe[r, col - pe_col_shift] = 0 when col_src[col] < 0, else with
+ * x~ = x[r', col_src[col] - x_col_shift] (r' = r, or with row_index the row row_index[col_feat[col] n + r] clamped into
+ * [0, n_src)) x~ itself when col_freq[col] = 0 and sinf(col_freq[col] x~) otherwise; TF32-rounded when round_out.  The hook reads
+ * the tables and needs every column to land inside [0, ldpe) and every source inside [0, ldx), n >= 0 and, with row_index,
+ * col_feat and n_src >= 1 (row_index holds (max col_feat + 1) n entries). */
+int dib_debug_pe(const float* x, int32_t ldx, int32_t x_col_shift, const int32_t* col_src, const int32_t* col_freq,
+                 int32_t col_begin, int32_t col_end, float* pe, int32_t ldpe, int32_t pe_col_shift, int64_t n,
+                 const int32_t* row_index, const int32_t* col_feat, int64_t n_src, int32_t round_out, void* stream);
+
+/* dib_debug_dropout: Keras Dropout of the encoder activations: dst = src keep / (1 - rate) (backward: dst *= the same mask,
+ * in place; src unused) over the width live columns of row r of feature f at f feat_stride + r ld, for every feature
+ * (feature = -1) or one; the keep mask of (seed, step + *step_dev, sample_offset + r, f, layer) is oracle/philox.dropout_keep.
+ * Needs 0 <= rate < 1, width >= 1, ld >= width, feat_stride >= n ld, 1 <= F <= 65535, -1 <= feature < F, 0 <= layer < 128. */
+int dib_debug_dropout(const float* src, float* dst, int64_t feat_stride, int32_t ld, int32_t width, int32_t F, int64_t n,
+                      float rate, uint64_t seed, uint32_t step, const uint32_t* step_dev, uint64_t sample_offset, int32_t layer,
+                      int32_t feature, int32_t backward, int32_t round_out, void* stream);
 
 /* bring-up switch for THIS handle (bit mask, 0 = the default kernels): 1 = unfused encoder kernels, 2 = integration network on
  * fp32-storage TF32 kernels, 4 = no fused integration tail (per-layer 16-bit GEMMs plus a head kernel), 8 = the generic head

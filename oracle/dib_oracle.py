@@ -226,6 +226,15 @@ def encoder_forward(cfg: DIBConfig, layers, x_i, keep=False, drop=None):
     return (h, acts, pres, masks) if keep else h
 
 
+def sparse_labels(y, C):
+    """[KERAS] the class of each sparse label as TensorFlow on a GPU reads it: y cast to an integer by truncation when
+    -1 < y < C, else -1 (NaN included), which gives a NaN loss and a NaN gradient row.  An accuracy hit is argmax == y
+    compared as floats, so a label of 2.7 names class 2 but never hits."""
+    y = np.asarray(y, np.float64).ravel()
+    ok = (y > -1.0) & (y < C)
+    return np.where(ok, np.trunc(np.where(ok, y, 0.0)), -1).astype(np.int64)
+
+
 def task_loss_per_sample(loss, pred, y):
     """[KERAS] per-sample loss value; the compiled loss is its mean over the batch."""
     if loss == LOSS_BCE_LOGITS:
@@ -235,7 +244,8 @@ def task_loss_per_sample(loss, pred, y):
     if loss == LOSS_SPARSE_CE_LOGITS:
         m = pred.max(axis=-1, keepdims=True)
         lse = (m + np.log(np.exp(pred - m).sum(axis=-1, keepdims=True)))[:, 0]
-        return lse - pred[np.arange(pred.shape[0]), y.astype(np.int64).ravel()]
+        lab = sparse_labels(y, pred.shape[-1])
+        return np.where(lab >= 0, lse - pred[np.arange(pred.shape[0]), np.maximum(lab, 0)], np.nan)
     if loss == LOSS_MSE:
         yy = y.reshape(pred.shape).astype(pred.dtype)
         return ((pred - yy) ** 2).mean(axis=-1)
@@ -255,7 +265,9 @@ def task_loss_grad(loss, pred, y):
         m = pred.max(axis=-1, keepdims=True)
         p = np.exp(pred - m)
         p /= p.sum(axis=-1, keepdims=True)
-        p[np.arange(pred.shape[0]), y.astype(np.int64).ravel()] -= 1.0
+        lab = sparse_labels(y, pred.shape[-1])
+        p[np.arange(pred.shape[0]), np.maximum(lab, 0)] -= (lab >= 0)
+        p[lab < 0] = np.nan
         return p
     if loss == LOSS_MSE:
         yy = y.reshape(pred.shape).astype(pred.dtype)
@@ -273,7 +285,7 @@ def accuracy_count(loss, pred, y):
     model output, logits included) for a BCE loss; sparse_categorical_accuracy for sparse CE.
     Returns the SUM over the batch of per-sample accuracies."""
     if loss == LOSS_SPARSE_CE_LOGITS:
-        return float((pred.argmax(axis=-1) == y.astype(np.int64).ravel()).sum())
+        return float((pred.argmax(axis=-1).astype(np.float64) == np.asarray(y, np.float64).ravel()).sum())
     yy = y.reshape(pred.shape)
     return float(((pred > 0.5).astype(np.float64) == yy).mean(axis=-1).sum())
 
@@ -318,7 +330,7 @@ def forward(cfg: DIBConfig, flat_params, x, eps, beta, y=None, loss=None, keep=F
             o, acts, pres, masks = encoder_forward(cfg, encoders[i], xs[i], keep=True, drop=drop)
         mu, lv = o[:, :E], o[:, E:] + cfg.logvar_offset               # models.py:106 tf.split(.,2,-1); nb-particle offset
         u = mu + np.exp(lv / 2.0) * eps[:, i, :]                      # models.py:108
-        kl = (0.5 * (mu ** 2 + np.exp(lv) - lv - 1.0)).sum(axis=-1).mean()   # models.py:111-112
+        kl = (0.5 * (mu ** 2 + (np.expm1(lv) - lv))).sum(axis=-1).mean()    # models.py:111-112
         embs.append(u)
         kls.append(kl)
         if cfg.encoder_kind == "simple":
@@ -396,7 +408,7 @@ def train_grads(cfg: DIBConfig, flat_params, x, y, eps, beta, loss, dtype=np.flo
         du = d_emb[:, i * E:(i + 1) * E]
         sig = np.exp(lv / 2.0)
         dmu = du + beta * mu / B
-        dlv = du * eps[:, i, :] * 0.5 * sig + beta * 0.5 * (np.exp(lv) - 1.0) / B
+        dlv = du * eps[:, i, :] * 0.5 * sig + beta * 0.5 * np.expm1(lv) / B
         dz = np.concatenate([dmu, dlv], axis=-1)
         if cfg.encoder_kind == "simple":
             enc_grads.append([(np.sum(dmu * acts[0]).reshape(1, 1), np.sum(dlv).reshape(1, 1))])

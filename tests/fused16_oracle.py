@@ -111,7 +111,7 @@ def forward(cfg, flat, x, eps, beta, y=None, loss=None, fmt=None, keep=False):
         a0, h1, h2, mu, lv = _encoder_forward(cfg, encoders[i], xs[i], fmt)
         sig = np.exp(lv / 2.0)
         embs.append(mu + sig * eps[:, i, :])                            # :466-467
-        kls.append((0.5 * (mu ** 2 + sig * sig - lv - 1.0)).sum(axis=-1).mean())   # :468 (sv * sv, not exp(lv))
+        kls.append((0.5 * (mu ** 2 + (np.expm1(lv) - lv))).sum(axis=-1).mean())   # :493 (sv * sv - lv - 1)
         enc.append((a0, h1, h2, mu, lv))
     emb = np.concatenate(embs, axis=-1)
     g = R(emb)                                                          # emb16 :471

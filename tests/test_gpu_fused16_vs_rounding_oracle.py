@@ -393,3 +393,31 @@ def test_weight_beyond_fp16_range_saturates():
     encs[0][2][0][3, 5] = 1e5
     integ[0][0][7, 11] = -1e5
     _grad_case(cfg, "fp16", "bce_logits", 128 * 12 + 5, 0.05, seed=17, p=p, label="weight 1e5")
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# sparse labels outside [0, C): one rule on every loss kernel (dib_sparse_label)
+# ---------------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("prec", ["fp32", "fp16", "bf16"])
+@pytest.mark.parametrize("out,mask", [(3, 0), (1, 0), (1, 4)])
+def test_out_of_range_sparse_label_gives_nan_loss_and_gradient(prec, out, mask):
+    """An invalid label (here C, or NaN) makes the row's loss and d loss / d z NaN, as TensorFlow on a GPU does; the accuracy
+    slot stays finite.  out = 3: the generic head; out = 1: the fused tail (mask 0) or the out = 1 head kernel (mask 4).
+    The same batch with its labels in range stays finite."""
+    if prec == "fp32" and mask:
+        pytest.skip("the fp32 path has one loss kernel")
+    cfg = _c(F=4, out=out)
+    n = 300
+    x, y, eps = _data(cfg, O.LOSS_SPARSE_CE_LOGITS, n, seed=5)
+    m = _model(cfg, prec, "sparse_ce_logits", mask=mask)
+    m.set_flat_weights(_params(cfg, 5))
+    g, st = (t.cpu().numpy() for t in m.compute_gradients(x, y, eps=eps))
+    assert np.isfinite(g).all() and np.isfinite(st).all()
+    F = cfg.number_features
+    for bad in (float(out), np.nan, -1.0):
+        yb = y.copy()
+        yb[17] = bad
+        g, st = (t.cpu().numpy() for t in m.compute_gradients(x, yb, eps=eps))
+        assert np.isnan(st[F]), (bad, st[F])
+        assert np.isfinite(st[F + 1]) and np.isfinite(st[:F]).all(), st
+        assert np.isnan(g).any(), bad
