@@ -85,6 +85,12 @@ class DibReduceSeg(ctypes.Structure):
                 ("dst", c_void_p)]
 
 
+# one layer of dib_debug_int16_gemm's weight-gradient launch (struct dib_int16_wgrad_layer)
+class DibInt16WgradLayer(ctypes.Structure):
+    _fields_ = [("g_in", c_void_p), ("K", c_int32), ("dz", c_void_p), ("N", c_int32), ("dW_part", c_void_p),
+                ("nsplit", c_int32), ("rows_per_split", c_int32)]
+
+
 GEMM_KERNELS = {"simt": 0, "tc": 1}
 GEMM_MODES = {"fwd": 0, "dgrad": 1, "wgrad": 2}
 
@@ -171,6 +177,16 @@ SIGNATURES = {
                                c_int64, c_void_p, c_void_p, c_int64, c_int32, c_void_p]),
     "dib_debug_dropout": (c_int32, [c_void_p, c_void_p, c_int64, c_int32, c_int32, c_int32, c_int64, c_float, c_uint64, c_uint32,
                                     c_void_p, c_uint64, c_int32, c_int32, c_int32, c_int32, c_void_p]),
+    "dib_debug_int16_gemm": (c_int32, [c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_int32, c_void_p, c_void_p,
+                                       c_void_p, c_int32, c_void_p, c_int32, c_int32, c_float, c_void_p, c_void_p, c_int32,
+                                       c_int64, c_float, c_void_p]),
+    "dib_debug_int16_head": (c_int32, [c_int32, c_int32, c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_int32, c_int32,
+                                       c_int32, c_float, c_int32, c_void_p, c_int64, c_float, c_float, c_void_p, c_int32,
+                                       c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_void_p, c_void_p]),
+    "dib_debug_int16_fwd2": (c_int32, [c_int32, c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                       c_void_p, c_void_p, c_int32, c_int32, c_float, c_int32, c_void_p, c_int32, c_float,
+                                       c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_void_p,
+                                       c_void_p, c_void_p, POINTER(c_int32), c_void_p]),
     "dib_debug_force_unfused": (c_int32, [c_void_p, c_int32]),
     "dib_last_error": (c_char_p, []),
     "dib_build_info": (c_char_p, []),

@@ -1140,6 +1140,30 @@ DibInfonceStream shard_args(const Ctx& c, const float* e_all, int64_t n_global, 
 
 }  // namespace
 
+namespace {
+// the memory contracts of the 16-bit kernels: TMA descriptors need 16-byte bases and row pitches, and the epilogues store and
+// load whole column pairs (4 bytes) or 8-column vectors (16 bytes)
+std::string int16_base_error(const char* name, const void* p) {
+  return p && reinterpret_cast<uintptr_t>(p) % 16 ? std::string(name) + " must be 16-byte aligned" : std::string();
+}
+std::string int16_ld_error(const char* name, int64_t ld, int64_t width) {
+  if (ld % 8 || ld < width)
+    return std::string(name) + " must be a multiple of 8 and >= " + std::to_string(width) + " (" + name + " = " +
+           std::to_string(ld) + ")";
+  return std::string();
+}
+std::string int16_bias_error(const char* name, const float* p) {
+  return p && reinterpret_cast<uintptr_t>(p) % 8 ? std::string(name) + " must be 8-byte aligned" : std::string();
+}
+bool known_act(int32_t act) { return act >= DIB_ACT_LINEAR && act <= DIB_ACT_ELU; }
+int sync_result(const std::string& fn, cudaError_t e, cudaStream_t st) {
+  const cudaError_t es = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return fail(fn + "launch: " + cudaGetErrorString(e));
+  if (es != cudaSuccess) return fail(fn + "sync: " + cudaGetErrorString(es));
+  return 0;
+}
+}  // namespace
+
 // =================================================================================================
 void dib_note_launch(int n) { g_launches.fetch_add((unsigned long long)n, std::memory_order_relaxed); }
 
@@ -1532,6 +1556,155 @@ int dib_debug_dropout(const float* src, float* dst, int64_t feat_stride, int32_t
   return 0;
 }
 
+// the header's C mirror of a weight-gradient layer: the test hook hands its array to the launcher as it is
+static_assert(sizeof(dib_int16_wgrad_layer) == sizeof(DibInt16Wgrad), "dib_int16_wgrad_layer size");
+static_assert(offsetof(dib_int16_wgrad_layer, g_in) == offsetof(DibInt16Wgrad, g_in) &&
+              offsetof(dib_int16_wgrad_layer, K) == offsetof(DibInt16Wgrad, K) &&
+              offsetof(dib_int16_wgrad_layer, dz) == offsetof(DibInt16Wgrad, dz) &&
+              offsetof(dib_int16_wgrad_layer, N) == offsetof(DibInt16Wgrad, N) &&
+              offsetof(dib_int16_wgrad_layer, dW_part) == offsetof(DibInt16Wgrad, dW_part) &&
+              offsetof(dib_int16_wgrad_layer, nsplit) == offsetof(DibInt16Wgrad, nsplit) &&
+              offsetof(dib_int16_wgrad_layer, rows_per_split) == offsetof(DibInt16Wgrad, rows_per_split),
+              "dib_int16_wgrad_layer layout");
+
+
+#define DIB_HOOK_CHECK(msg)                          \
+  do {                                               \
+    const std::string _m = (msg);                    \
+    if (!_m.empty()) return fail(fn + _m);           \
+  } while (0)
+
+// one dib_int16_fwd / dib_int16_dgrad / dib_int16_wgrad launch, as the 16-bit integration forward and backward issue them
+// (unit tests)
+int dib_debug_int16_gemm(int32_t mode, int32_t bf16, int32_t M, int32_t K, int32_t N, const void* a, int32_t lda,
+                         const void* w16, const float* bias, const void* x, int32_t ldx, void* out, int32_t ldc, int32_t act,
+                         float alpha, float* colsum, const dib_int16_wgrad_layer* layers, int32_t count, int64_t split_stride,
+                         float out_scale, void* stream) {
+  const std::string fn = "dib_debug_int16_gemm: ";
+  if (mode < DIB_GEMM_FWD || mode > DIB_GEMM_WGRAD) return fail(fn + "unknown mode " + std::to_string(mode));
+  if (bf16 != 0 && bf16 != 1) return fail(fn + "bf16 is 0 (fp16) or 1 (bf16)");
+  if (M < 1) return fail(fn + "needs M >= 1 (M = " + std::to_string(M) + ")");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (mode == DIB_GEMM_WGRAD) {
+    if (count < 1 || count > 2 || !layers) return fail(fn + "WGRAD takes 1 or 2 layers (count = " + std::to_string(count) + ")");
+    for (int q = 0; q < count; ++q) {
+      const dib_int16_wgrad_layer& l = layers[q];
+      const std::string lq = "layer " + std::to_string(q) + ": ";
+      if (l.K < 64 || l.K % 64) return fail(fn + lq + "needs K a positive multiple of 64 (K = " + std::to_string(l.K) + ")");
+      if (l.N < 128 || l.N % 128) return fail(fn + lq + "needs N a positive multiple of 128 (N = " + std::to_string(l.N) + ")");
+      if (!l.g_in || !l.dz || !l.dW_part) return fail(fn + lq + "g_in, dz and dW_part must not be null");
+      DIB_HOOK_CHECK(int16_base_error("g_in", l.g_in));
+      DIB_HOOK_CHECK(int16_base_error("dz", l.dz));
+      if (reinterpret_cast<uintptr_t>(l.dW_part) % 8) return fail(fn + lq + "dW_part must be 8-byte aligned");
+      if (l.nsplit < 1) return fail(fn + lq + "needs nsplit >= 1");
+      if (l.rows_per_split < 64 || l.rows_per_split % 64)
+        return fail(fn + lq + "needs rows_per_split a positive multiple of 64 (rows_per_split = " +
+                    std::to_string(l.rows_per_split) + ")");
+      const int64_t span = (int64_t)l.nsplit * l.rows_per_split;
+      if (span < M) return fail(fn + lq + "needs nsplit * rows_per_split >= M (" + std::to_string(span) + " < " + std::to_string(M) + ")");
+      if (span > 0x7fffffffll) return fail(fn + lq + "needs nsplit * rows_per_split < 2^31");
+      if ((int64_t)l.K * l.N > split_stride || split_stride % 2)
+        return fail(fn + lq + "every [K x N] partial slice must lie inside split_stride, an even count (split_stride = " +
+                    std::to_string(split_stride) + ")");
+    }
+    return sync_result(fn, dib_int16_wgrad(reinterpret_cast<const DibInt16Wgrad*>(layers), count, M, split_stride, out_scale,
+                                           bf16, st), st);
+  }
+  if (K < 64 || K % 64) return fail(fn + "needs K a positive multiple of 64 (K = " + std::to_string(K) + ")");
+  if (N < 128 || N % 128) return fail(fn + "needs N a positive multiple of 128 (N = " + std::to_string(N) + ")");
+  if (!known_act(act)) return fail(fn + "unknown act " + std::to_string(act));
+  if (!a || !w16 || !out) return fail(fn + "a, w16 and out must not be null");
+  const int in_w = mode == DIB_GEMM_FWD ? K : N, out_w = mode == DIB_GEMM_FWD ? N : K;
+  DIB_HOOK_CHECK(int16_base_error("a", a));
+  DIB_HOOK_CHECK(int16_base_error("w16", w16));
+  DIB_HOOK_CHECK(int16_base_error("out", out));
+  DIB_HOOK_CHECK(int16_ld_error("lda", lda, in_w));
+  DIB_HOOK_CHECK(int16_ld_error("ldc", ldc, out_w));
+  if (mode == DIB_GEMM_FWD) {
+    if (!bias) return fail(fn + "FWD needs bias");
+    DIB_HOOK_CHECK(int16_bias_error("bias", bias));
+    return sync_result(fn, dib_int16_fwd(a, lda, w16, bias, out, ldc, M, K, N, act, alpha, bf16, st), st);
+  }
+  if (x) {
+    DIB_HOOK_CHECK(int16_base_error("x", x));
+    DIB_HOOK_CHECK(int16_ld_error("ldx", ldx, K));
+  }
+  return sync_result(fn, dib_int16_dgrad(a, lda, w16, x, ldx, out, ldc, M, K, N, act, alpha, colsum, bf16, st), st);
+}
+
+// the output head of the 16-bit integration network, generic or out = 1, as the step's forward launches it (unit tests)
+int dib_debug_int16_head(int32_t head1, int32_t bf16, const void* g, int32_t ldg, int32_t K, const float* Wc, const float* bc,
+                         int32_t out_dim, int32_t out_act, int32_t hid_act, float alpha, int32_t loss, const float* y, int64_t n,
+                         float inv_batch, float gscale, void* dg, int32_t lddg, float* user_pred, float* wpart,
+                         int32_t wpart_stride, float* loss_part, float* acc_part, int32_t nblocks, const float* weights,
+                         void* stream) {
+  const std::string fn = "dib_debug_int16_head: ";
+  if (head1 != 0 && head1 != 1) return fail(fn + "head1 is 0 (generic kernel) or 1 (the out = 1 kernel)");
+  if (bf16 != 0 && bf16 != 1) return fail(fn + "bf16 is 0 (fp16) or 1 (bf16)");
+  if (K != 256) return fail(fn + "needs K == 256 (K = " + std::to_string(K) + ")");
+  if (out_dim < 1 || out_dim > 16) return fail(fn + "needs 1 <= out_dim <= 16 (out_dim = " + std::to_string(out_dim) + ")");
+  if (head1 && out_dim != 1) return fail(fn + "head1 needs out_dim == 1");
+  if (!known_act(out_act) || !known_act(hid_act)) return fail(fn + "unknown out_act or hid_act");
+  if (loss < DIB_LOSS_BCE_LOGITS || loss > DIB_LOSS_BCE_PROBS || loss == DIB_LOSS_EXTERNAL)
+    return fail(fn + "unknown loss " + std::to_string(loss) + " (the head computes bce_logits, sparse CE, mse or bce_probs)");
+  if (n < 1 || n > 0x7fffffffll) return fail(fn + "needs 1 <= n < 2^31 (n = " + std::to_string(n) + ")");
+  if (nblocks < 1 || nblocks > 65535) return fail(fn + "needs 1 <= nblocks <= 65535 (nblocks = " + std::to_string(nblocks) + ")");
+  if (!g || !Wc || !bc || !loss_part || !acc_part) return fail(fn + "g, Wc, bc, loss_part and acc_part must not be null");
+  DIB_HOOK_CHECK(int16_base_error("g", g));
+  DIB_HOOK_CHECK(int16_ld_error("ldg", ldg, K));
+  if (weights && !y) return fail(fn + "weights need y");
+  if (dg) {
+    DIB_HOOK_CHECK(int16_base_error("dg", dg));
+    DIB_HOOK_CHECK(int16_ld_error("lddg", lddg, K));
+    if (!wpart) return fail(fn + "training (dg) needs wpart");
+    if (wpart_stride < K * out_dim + out_dim + K)
+      return fail(fn + "needs wpart_stride >= K * out_dim + out_dim + K (wpart_stride = " + std::to_string(wpart_stride) + ")");
+  }
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return sync_result(fn, dib_int16_head(g, ldg, K, Wc, bc, out_dim, out_act, hid_act, alpha, loss, y, n, inv_batch, gscale, dg,
+                                        lddg, user_pred, wpart, wpart_stride, loss_part, acc_part, nblocks, head1 != 0, weights,
+                                        bf16, st), st);
+}
+
+// the fused integration tail, forward only, with the training head, or with its dgrad stages, as the step's forward launches
+// it (unit tests)
+int dib_debug_int16_fwd2(int32_t bf16, const void* g_in, int32_t ld_in, int32_t K0, const void* w16_0, const float* b0,
+                         const void* w16_1, const float* b1, void* g1, const float* wout, const float* bout, int32_t act,
+                         int32_t out_act, float alpha, int32_t loss, const float* y, int32_t M, float inv_batch, float gscale,
+                         void* dg2, void* dg1, float* dbpart, void* demb, float* user_pred, float* wpart, int32_t wpart_stride,
+                         float* loss_part, float* acc_part, const float* weights, int32_t* nblocks, void* stream) {
+  const std::string fn = "dib_debug_int16_fwd2: ";
+  if (bf16 != 0 && bf16 != 1) return fail(fn + "bf16 is 0 (fp16) or 1 (bf16)");
+  if (!dib_int16_fwd2_ok(K0, 256, 256, 1)) return fail(fn + "needs K0 a positive multiple of 64 (K0 = " + std::to_string(K0) + ")");
+  if (M < 1) return fail(fn + "needs M >= 1 (M = " + std::to_string(M) + ")");
+  if (!known_act(act) || !known_act(out_act)) return fail(fn + "unknown act or out_act");
+  if (loss < DIB_LOSS_BCE_LOGITS || loss > DIB_LOSS_BCE_PROBS || loss == DIB_LOSS_EXTERNAL)
+    return fail(fn + "unknown loss " + std::to_string(loss) + " (the tail computes bce_logits, sparse CE, mse or bce_probs)");
+  if (!g_in || !w16_0 || !b0 || !w16_1 || !b1 || !g1 || !wout || !bout || !loss_part || !acc_part || !nblocks)
+    return fail(fn + "g_in, w16_0, b0, w16_1, b1, g1, wout, bout, loss_part, acc_part and nblocks must not be null");
+  DIB_HOOK_CHECK(int16_base_error("g_in", g_in));
+  DIB_HOOK_CHECK(int16_ld_error("ld_in", ld_in, K0));
+  DIB_HOOK_CHECK(int16_base_error("w16_0", w16_0));
+  DIB_HOOK_CHECK(int16_base_error("w16_1", w16_1));
+  DIB_HOOK_CHECK(int16_base_error("g1", g1));
+  DIB_HOOK_CHECK(int16_base_error("dg2", dg2));
+  DIB_HOOK_CHECK(int16_base_error("dg1", dg1));
+  DIB_HOOK_CHECK(int16_base_error("demb", demb));
+  if (reinterpret_cast<uintptr_t>(b0) % 16 || reinterpret_cast<uintptr_t>(b1) % 16 || reinterpret_cast<uintptr_t>(wout) % 16)
+    return fail(fn + "b0, b1 and wout must be 16-byte aligned");
+  if (weights && !y) return fail(fn + "weights need y");
+  if (dg1 && (!dg2 || !dbpart)) return fail(fn + "dg1 needs dg2 and dbpart");
+  if (demb && !dg1) return fail(fn + "demb needs dg1");
+  if (dg2 && !wpart) return fail(fn + "training (dg2) needs wpart");
+  if (dg2 && wpart_stride < 256 + 1 + 256)
+    return fail(fn + "needs wpart_stride >= 513 (wpart_stride = " + std::to_string(wpart_stride) + ")");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return sync_result(fn, dib_int16_fwd2_head(g_in, ld_in, K0, w16_0, b0, w16_1, b1, g1, wout, bout, act, out_act, alpha, loss, y,
+                                             M, inv_batch, gscale, dg2, dg1, dbpart, demb, user_pred, wpart, wpart_stride,
+                                             loss_part, acc_part, nblocks, weights, bf16, st), st);
+}
+#undef DIB_HOOK_CHECK
+
 const char* dib_last_error(void) { return g_last_error.c_str(); }
 
 const char* dib_build_info(void) {
@@ -1552,6 +1725,7 @@ int32_t dib_model_info(const dib_model* h, char* out, size_t out_bytes) {
     s += " accumulate=fp32";
   }
   if (h->route.tail_fused) s += h->route.tail_bwd ? " integration_tail=fwd2-head-dgrad" : " integration_tail=fwd2-head";
+  else if (h->route.int16) s += h->route.head1 ? " integration_head=head1" : " integration_head=generic";
   if (h->st)
     s += std::string(" set_transformer=") + (h->varlen ? "attention-varlen-simt-fp32" : "attention-simt-fp32") +
          ",layernorm-simt-fp32,dense-" + (is_tc(h) ? "wgmma-tf32" : "simt-fp32");

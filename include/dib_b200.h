@@ -612,6 +612,62 @@ int dib_debug_dropout(const float* src, float* dst, int64_t feat_stride, int32_t
                       float rate, uint64_t seed, uint32_t step, const uint32_t* step_dev, uint64_t sample_offset, int32_t layer,
                       int32_t feature, int32_t backward, int32_t round_out, void* stream);
 
+/* unit-test hooks of the 16-bit integration network kernels (csrc/dib_int16.cu: 'fp16' / 'bf16' precision), launched through the
+ * launchers the step uses.  Each checks every argument on the host before anything is launched, fails with a message naming
+ * the one it rejects, and synchronises the stream.  bf16: 0 = fp16 operands, 1 = bf16.  16-bit buffers hold raw fp16 / bf16
+ * bit patterns.  Every 16-bit base must be 16-byte aligned and every 16-bit leading dimension a multiple of 8 and no smaller
+ * than the width it holds (the TMA descriptors and the vector accesses need both); fp32 bias rows must be 8-byte aligned.
+ * Widths are what dib_create allows: the embedding width a multiple of 64, hidden widths multiples of 128.
+ * tests/test_gpu_int16_kernels.py checks them element by element against a float64 reference.
+ *
+ * dib_debug_int16_gemm: mode 0 FWD   out [M, N] (ldc) = r(act(a [M, K] (lda) w16 [K, N] + bias [N]))
+ *                       mode 1 DGRAD out [M, K] (ldc) = r((a [M, N] (lda) w16 [K, N]^T) act'(x [M, K] (ldx))), x nullable (no
+ *                              act'); colsum (nullable) [ceil(M / 128)][K] = the column sums of the unrounded result per
+ *                              128-row tile
+ *                       mode 2 WGRAD for each of the `count` (1 or 2) layers and split s < nsplit: layers[q].dW_part +
+ *                              s * split_stride = out_scale g_in[rows of s]^T dz[rows of s] [K x N], g_in [M, K] and dz [M, N]
+ *                              dense; split s holds batch rows [s rows_per_split, min(M, (s + 1) rows_per_split)), a split
+ *                              past M writes zeros.  Needs rows_per_split > 0 a multiple of 64 (a k-block of 64 rows must
+ *                              not reach into the next split), nsplit rows_per_split >= M, and K N <= split_stride.
+ * r() is cvt.rn.satfinite to the 16-bit format.  Needs K % 64 == 0, N % 128 == 0 and M >= 1. */
+typedef struct dib_int16_wgrad_layer {
+  const void* g_in;
+  int32_t K;
+  const void* dz;
+  int32_t N;
+  float* dW_part;
+  int32_t nsplit;
+  int32_t rows_per_split;
+} dib_int16_wgrad_layer;
+int dib_debug_int16_gemm(int32_t mode, int32_t bf16, int32_t M, int32_t K, int32_t N, const void* a, int32_t lda,
+                         const void* w16, const float* bias, const void* x, int32_t ldx, void* out, int32_t ldc, int32_t act,
+                         float alpha, float* colsum, const dib_int16_wgrad_layer* layers, int32_t count, int64_t split_stride,
+                         float out_scale, void* stream);
+
+/* dib_debug_int16_head: the output head over n rows of the last hidden activation g [n, K] (ldg), K = 256: z = out_act(g Wc +
+ * bc) (Wc [K, out_dim], bc [out_dim] fp32), the compiled loss against y (nullable), and in training (dg != NULL) dg [n, K]
+ * (lddg) = r(dz S Wc^T act'(g)) plus per-block partials wpart[b * wpart_stride + ...] = [dWc (K out) | dbc (out) | column sums
+ * of dg (K)]; loss_part[b] / acc_part[b] for each of the nblocks blocks; user_pred [n, out_dim] (nullable) = z.  head1: the
+ * out = 1 kernel.  weights (nullable): the rows' sample weights.  Needs 1 <= out_dim <= 16, head1 => out_dim == 1, n >= 1,
+ * nblocks >= 1 and, in training, wpart_stride >= K out + out + K. */
+int dib_debug_int16_head(int32_t head1, int32_t bf16, const void* g, int32_t ldg, int32_t K, const float* Wc, const float* bc,
+                         int32_t out_dim, int32_t out_act, int32_t hid_act, float alpha, int32_t loss, const float* y, int64_t n,
+                         float inv_batch, float gscale, void* dg, int32_t lddg, float* user_pred, float* wpart,
+                         int32_t wpart_stride, float* loss_part, float* acc_part, int32_t nblocks, const float* weights,
+                         void* stream);
+
+/* dib_debug_int16_fwd2: the fused tail of single-output models: g1 [M, 256] = r(act(g_in [M, K0] (ld_in) W0 + b0)),
+ * g2 = r(act(g1 W1 + b1)) on chip, the logit and compiled loss; training (dg2 != NULL): dg2 [M, 256] and the per-CTA
+ * partials wpart[b * wpart_stride + ...] = [dW out (256) | db out (1) | column sums of dg2 (256)]; with dg1 (needs dg2 and
+ * dbpart) the dgrad of the second layer dg1 [M, 256] with its column sums per 128-row tile in dbpart [ceil(M / 128)][256];
+ * with demb (needs dg1) demb [M, K0] = r(dg1 W0^T).  *nblocks = the CTAs launched (rows of wpart / loss_part / acc_part
+ * written).  Needs K0 % 64 == 0 (K0 >= 64), n >= 1 and, in training, wpart_stride >= 513. */
+int dib_debug_int16_fwd2(int32_t bf16, const void* g_in, int32_t ld_in, int32_t K0, const void* w16_0, const float* b0,
+                         const void* w16_1, const float* b1, void* g1, const float* wout, const float* bout, int32_t act,
+                         int32_t out_act, float alpha, int32_t loss, const float* y, int32_t M, float inv_batch, float gscale,
+                         void* dg2, void* dg1, float* dbpart, void* demb, float* user_pred, float* wpart, int32_t wpart_stride,
+                         float* loss_part, float* acc_part, const float* weights, int32_t* nblocks, void* stream);
+
 /* bring-up switch for THIS handle (bit mask, 0 = the default kernels): 1 = unfused encoder kernels, 2 = integration network on
  * fp32-storage TF32 kernels, 4 = no fused integration tail (per-layer 16-bit GEMMs plus a head kernel), 8 = the generic head
  * kernel even when output_dimensionality == 1, 16 = the fused tail without its dgrad stages (the backward launches those
@@ -625,7 +681,9 @@ const char* dib_last_error(void);
 const char* dib_build_info(void);
 
 /* one line describing what THIS handle runs, e.g.
- * "precision=fp16 encoders=fused-wgmma-f16 integration=int16-wgmma-f16 operands=fp16 accumulate=fp32".
+ * "precision=fp16 encoders=fused-wgmma-f16 integration=int16-wgmma-f16 operands=fp16 accumulate=fp32".  The 16-bit path adds
+ * its tail ("integration_tail=fwd2-head-dgrad" / "fwd2-head") or, without a fused tail, its head kernel
+ * ("integration_head=head1" / "generic").
  * Returns the number of bytes written (excluding the terminator), negative on error. */
 int32_t dib_model_info(const dib_model* h, char* out, size_t out_bytes);
 
