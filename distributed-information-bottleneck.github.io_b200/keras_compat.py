@@ -3,6 +3,11 @@ nb-radial cell 10): optimizer/loss objects handed to ``model.compile``, the ``Ca
 These are thin descriptions -- the arithmetic they name runs in the CUDA library."""
 from __future__ import annotations
 
+import os
+import warnings
+
+import numpy as np
+
 
 class Adam:
     """tf.keras.optimizers.Adam(learning_rate, beta_1, beta_2, epsilon) -- Keras defaults; epsilon is applied
@@ -177,10 +182,6 @@ class Callback:
     def on_train_batch_end(self, batch, logs=None): pass
 
 
-class callbacks:
-    Callback = Callback
-
-
 class History(Callback):
     """Return value of Model.fit: ``.history`` maps metric name -> list over epochs (train.py:169-172)."""
 
@@ -192,3 +193,112 @@ class History(Callback):
         self.epoch.append(epoch)
         for k, v in (logs or {}).items():
             self.history.setdefault(k, []).append(v)
+
+
+def _higher_is_better(monitor):
+    """mode='auto': accuracy-, AUC-, precision- and recall-like names are maximised, everything else minimised."""
+    name = monitor.removeprefix("val_")
+    return "acc" in name or "auc" in name or "precision" in name or "recall" in name or name.startswith("fmeasure")
+
+
+class ModelCheckpoint(Callback):
+    """tf.keras.callbacks.ModelCheckpoint (Keras 2): at every epoch end, save the model (``model.save``) or its weights
+    (``save_weights_only``) to ``filepath.format(epoch=epoch + 1, **logs)``.  With ``save_best_only`` the file is written
+    only when ``logs[monitor]`` improves on the best value so far (``initial_value_threshold`` is the starting best); an
+    epoch whose logs lack ``monitor`` is skipped with a warning.  ``mode`` is 'min', 'max' or 'auto' ('max' for accuracy /
+    AUC / precision / recall names).  Only ``save_freq='epoch'`` is implemented."""
+
+    def __init__(self, filepath, monitor="val_loss", verbose=0, save_best_only=False, save_weights_only=False, mode="auto",
+                 save_freq="epoch", options=None, initial_value_threshold=None):
+        super().__init__()
+        if save_freq != "epoch":
+            if isinstance(save_freq, int) and not isinstance(save_freq, bool):
+                raise ValueError(f"ModelCheckpoint(save_freq={save_freq}): saving every so many batches is not implemented; "
+                                 "use save_freq='epoch'")
+            raise ValueError(f"Unrecognized save_freq: {save_freq!r}")
+        if options is not None:
+            raise ValueError("ModelCheckpoint(options=...) is not implemented")
+        self.filepath = os.fspath(filepath)
+        self.monitor = monitor
+        self.verbose = verbose
+        self.save_best_only = bool(save_best_only)
+        self.save_weights_only = bool(save_weights_only)
+        self.save_freq = save_freq
+        if mode not in ("auto", "min", "max"):
+            warnings.warn(f"ModelCheckpoint mode {mode!r} is unknown, fallback to auto mode.")
+            mode = "auto"
+        self.mode = mode
+        self._maximize = mode == "max" or (mode == "auto" and _higher_is_better(monitor))
+        self.best = (float(initial_value_threshold) if initial_value_threshold is not None
+                     else (-np.inf if self._maximize else np.inf))
+
+    def _improved(self, current):
+        return current > self.best if self._maximize else current < self.best
+
+    def on_epoch_end(self, epoch, logs=None):
+        logs = logs or {}
+        path = self.filepath.format(epoch=epoch + 1, **logs)
+        if self.save_best_only:
+            current = logs.get(self.monitor)
+            if current is None:
+                warnings.warn(f"Can save best model only with {self.monitor} available, skipping.")
+                return
+            if not self._improved(current):
+                if self.verbose:
+                    print(f"\nEpoch {epoch + 1}: {self.monitor} did not improve from {self.best:.5f}")
+                return
+            if self.verbose:
+                print(f"\nEpoch {epoch + 1}: {self.monitor} improved from {self.best:.5f} to {current:.5f}, saving to {path}")
+            self.best = current
+        elif self.verbose:
+            print(f"\nEpoch {epoch + 1}: saving model to {path}")
+        if self.save_weights_only:
+            self.model.save_weights(path)
+        else:
+            self.model.save(path)
+
+
+class BackupAndRestore(Callback):
+    """tf.keras.callbacks.BackupAndRestore: the full training state (``model.save``) goes to ``backup_dir`` at every epoch
+    end.  ``on_train_begin`` restores it when a backup exists and makes ``fit`` continue with the epoch after the last
+    completed one, so a run killed between epochs and started again with the same ``fit`` call ends where the uninterrupted
+    run ends -- bit for bit, as every random draw is keyed by saved state.  ``on_train_end`` deletes the backup when
+    ``delete_checkpoint``; an exception that escapes ``fit`` skips it, so the backup survives."""
+
+    FILENAME = "backup.npz"
+
+    def __init__(self, backup_dir, save_freq="epoch", delete_checkpoint=True):
+        super().__init__()
+        if save_freq != "epoch":
+            raise ValueError(f"BackupAndRestore(save_freq={save_freq!r}): only backups at epoch ends are implemented")
+        if not backup_dir:
+            raise ValueError("BackupAndRestore needs a backup_dir")
+        self.backup_dir = os.fspath(backup_dir)
+        self.delete_checkpoint = bool(delete_checkpoint)
+        self.path = os.path.join(self.backup_dir, self.FILENAME)
+
+    def on_train_begin(self, logs=None):
+        epochs_done = self.model._restore_backup(self.path)
+        if epochs_done is not None:
+            self.model._resume_epoch = epochs_done
+
+    def on_epoch_end(self, epoch, logs=None):
+        if self.model._is_writer():
+            os.makedirs(self.backup_dir, exist_ok=True)
+        self.model.save(self.path)
+
+    def on_train_end(self, logs=None):
+        if self.delete_checkpoint and self.model._is_writer():
+            try:
+                os.remove(self.path)
+                os.rmdir(self.backup_dir)
+            except OSError:                    # already gone, or the directory holds other files
+                pass
+
+
+
+class callbacks:
+    Callback = Callback
+    History = History
+    ModelCheckpoint = ModelCheckpoint
+    BackupAndRestore = BackupAndRestore

@@ -38,6 +38,10 @@ class Metric:
     def __repr__(self):
         return f"<{type(self).__name__} {self.name!r}>"
 
+    def get_config(self):
+        """The constructor arguments that rebuild this metric (``type(m)(**m.get_config())``)."""
+        return {"name": self.name}
+
 
 class BinaryAccuracy(Metric):
     """keras.metrics.BinaryAccuracy: mean over the outputs of [(z > threshold) == y]."""
@@ -46,6 +50,9 @@ class BinaryAccuracy(Metric):
     def __init__(self, name=None, dtype=None, threshold=0.5):
         super().__init__(name, dtype)
         self.threshold = float(threshold)
+
+    def get_config(self):
+        return dict(super().get_config(), threshold=self.threshold)
 
 
 class SparseCategoricalAccuracy(Metric):
@@ -74,6 +81,9 @@ class BinaryCrossentropy(Metric):
             raise ValueError("BinaryCrossentropy(label_smoothing=...) is not implemented")
         self.from_logits = bool(from_logits)
 
+    def get_config(self):
+        return dict(super().get_config(), from_logits=self.from_logits)
+
 
 class SparseCategoricalCrossentropy(Metric):
     """keras.metrics.SparseCategoricalCrossentropy: keras.backend.sparse_categorical_crossentropy; from_logits=False clips p
@@ -85,6 +95,9 @@ class SparseCategoricalCrossentropy(Metric):
         if axis != -1:
             raise ValueError("SparseCategoricalCrossentropy(axis=...) other than -1 is not implemented")
         self.from_logits = bool(from_logits)
+
+    def get_config(self):
+        return dict(super().get_config(), from_logits=self.from_logits)
 
 
 class _Confusion(Metric):
@@ -114,6 +127,10 @@ class AUC(_Confusion):
         self.summation_method = str(summation_method).lower()
         self.from_logits = bool(from_logits)
 
+    def get_config(self):
+        return dict(super().get_config(), num_thresholds=self.num_thresholds, curve=self.curve,
+                    summation_method=self.summation_method, from_logits=self.from_logits)
+
 
 class _AtThreshold(_Confusion):
     def __init__(self, thresholds=None, top_k=None, class_id=None, name=None, dtype=None):
@@ -128,6 +145,9 @@ class _AtThreshold(_Confusion):
             raise ValueError(f"Threshold values must be in [0, 1]. Received: {t}")
         self.threshold = t
         self.num_thresholds = 1
+
+    def get_config(self):
+        return dict(super().get_config(), thresholds=self.threshold)
 
 
 class Precision(_AtThreshold):
@@ -151,6 +171,21 @@ class metrics:
     AUC = AUC
     Precision = Precision
     Recall = Recall
+
+
+def serialize(m):
+    """A compiled metric as JSON-able data: ``'accuracy'`` stays the string, an object becomes {class, config}."""
+    return m if isinstance(m, str) else {"class": type(m).__name__, "config": m.get_config()}
+
+
+def deserialize(spec):
+    """The inverse of :func:`serialize`."""
+    if isinstance(spec, str):
+        return spec
+    cls = getattr(metrics, spec["class"], None) if isinstance(spec, dict) else None
+    if not (isinstance(cls, type) and issubclass(cls, Metric)):
+        raise ValueError(f"unknown metric {spec!r}")
+    return cls(**spec["config"])
 
 
 ACCURACY = "accuracy"          # the statistics slot of metrics=['accuracy'] (a compiled entry, not a tail metric)

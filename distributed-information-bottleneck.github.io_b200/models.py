@@ -10,14 +10,17 @@ from __future__ import annotations
 
 import ctypes
 import gc
+import json
 import math
 import os
+import zlib
 from typing import Optional, Sequence
 
 import numpy as np
 import torch
 
 from . import _lib
+from . import checkpoint
 from . import metrics as _metrics
 from . import parallel
 from .keras_compat import Adam, InfoNCE, RMSprop, SGD, Callback, History, optimizers, resolve_loss
@@ -371,6 +374,8 @@ class DistributedIBNet:
         self._step_dev_dirty = False       # _train_step_count moved outside a graph replay: refill the device mirror
         self._replayed_launches = 0        # kernels launched by graph replays (dib_launch_count only sees eager launches)
         self._inference_calls = 0          # fresh noise per un-seeded inference call (tf.random.normal, models.py:108)
+        self._epochs_done = 0              # epochs fit has completed (checkpoints: where a restored run continues)
+        self._resume_epoch = None          # set by BackupAndRestore.on_train_begin: the epoch fit starts at
         self.optimizer = None
         self.compiled_metrics_names = []
         self._metric_entries = []          # metrics.CompiledMetric per compiled metric, in history order
@@ -1237,8 +1242,11 @@ class DistributedIBNet:
                 cb.set_model(self) if hasattr(cb, "set_model") else setattr(cb, "model", self)
             self.history = history
             self.stop_training = False
+            self._resume_epoch = None
             for cb in cbs:
                 getattr(cb, "on_train_begin", lambda logs=None: None)()
+            if self._resume_epoch is not None:                  # BackupAndRestore restored a backup
+                initial_epoch, self._resume_epoch = self._resume_epoch, None
             for epoch in range(initial_epoch, epochs):
                 for cb in cbs:
                     cb.on_epoch_begin(epoch, logs=None)                      # beta annealing lives here
@@ -1257,6 +1265,7 @@ class DistributedIBNet:
                 if verbose not in (False, 0) and rank == 0:          # 'auto' -> 1 like Keras outside notebooks
                     print(f"Epoch {epoch + 1}/{epochs} - " + " - ".join(
                         f"{k}: {v:.4g}" for k, v in logs.items() if not k.removeprefix('val_').startswith('KL')))
+                self._epochs_done = epoch + 1
                 for cb in cbs:
                     cb.on_epoch_end(epoch, logs)
                 if self.stop_training:
@@ -1330,6 +1339,190 @@ class DistributedIBNet:
             o = self(xb, training=False, step=st, sample_offset=b0)
             outs.append(o if isinstance(x, torch.Tensor) else np.asarray(o))
         return torch.cat(outs) if isinstance(x, torch.Tensor) else np.concatenate(outs)
+
+    # ------------------------------------------------------------------ checkpoints (file format: checkpoint.py)
+    def get_config(self):
+        """The constructor arguments that rebuild this model (Keras' ``get_config``); ``device`` and ``process_group`` are
+        the caller's."""
+        return dict(feature_dimensionalities=list(self.feature_dimensionalities),
+                    feature_encoder_architecture=("simple" if self.encoder_kind == "simple"
+                                                  else list(self.feature_encoder_architecture)),
+                    integration_network_architecture=list(self.integration_network_architecture),
+                    output_dimensionality=self.output_dimensionality, use_positional_encoding=self.use_positional_encoding,
+                    number_positional_encoding_frequencies=self.number_positional_encoding_frequencies,
+                    activation_fn=self.activation_fn, feature_embedding_dimension=self.feature_embedding_dimension,
+                    output_activation_fn=self.output_activation_fn, dropout_rate=self.dropout_rate, seed=self.seed,
+                    precision=self.precision, leaky_alpha=self.leaky_alpha, logvar_offset=self.logvar_offset,
+                    kl_loss_exponent=self.kl_loss_exponent, kl_loss_scale=self.kl_loss_scale)
+
+    def _model_variable_names(self):
+        """Names of the model's own variables (not the InfoNCE output encoder's) in flat order."""
+        F, n_model = self.number_features, self._n_model_vars
+        if self.encoder_kind == "simple":
+            names = [f"feature_encoder_{i}/{v}" for i in range(F) for v in ("mu_scaling", "logvar")]
+        else:
+            L = len(self.feature_encoder_architecture) + 1
+            names = [f"feature_encoder_{i}/dense_{k}/{v}" for i in range(F) for k in range(L) for v in ("kernel", "bias")]
+        return names + [f"integration_network/dense_{k}/{v}" for k in range((n_model - len(names)) // 2)
+                        for v in ("kernel", "bias")]
+
+    def _variable_specs(self):
+        """(names, Keras shapes) of every trainable variable in flat order, the InfoNCE output encoder's last
+        (``output_encoder/dense_{k}/{kernel|bias}``)."""
+        names = self._model_variable_names()
+        names += [f"output_encoder/dense_{k}/{v}" for k in range((len(self._var_off) - self._n_model_vars) // 2)
+                  for v in ("kernel", "bias")]
+        shapes = [(r, c) if r > 0 else (c,) for r, c in zip(self._var_rows, self._var_cols)]
+        return names, shapes
+
+    def _compile_config(self):
+        """optimizer (class and constructor arguments), loss and compiled metrics as JSON-able data."""
+        opt = self.optimizer
+        keys = {Adam: ("beta_1", "beta_2", "epsilon"), SGD: ("momentum", "nesterov"),
+                RMSprop: ("rho", "momentum", "epsilon")}[type(opt)]
+        optimizer = {"class": type(opt).__name__,
+                     "config": dict({k: getattr(opt, k) for k in keys}, learning_rate=float(opt.learning_rate))}
+        nce = self._infonce
+        loss = {"kind": self._loss_kind}
+        if nce is not None:
+            loss.update(y_dimensionality=nce.y_dimensionality, y_encoder_architecture=list(nce.y_encoder_architecture),
+                        similarity=nce.similarity, temperature=nce.temperature, negatives=nce.negatives)
+        spec = lambda e: _metrics.ACCURACY if not e.in_tail else _metrics.serialize(e.metric)
+        return dict(optimizer=optimizer, loss=loss,
+                    metrics=[spec(e) for e in self._metric_entries if not e.weighted],
+                    weighted_metrics=[spec(e) for e in self._metric_entries if e.weighted])
+
+    def _manifest(self, kind):
+        names, shapes = self._variable_specs()
+        return dict(version=checkpoint.FORMAT_VERSION, kind=kind,
+                    model={"class": type(self).__name__, "config": self.get_config()},
+                    variables=[[n, list(s)] for n, s in zip(names, shapes)])
+
+    def _is_writer(self):
+        """Rank 0 writes the checkpoints of a data-parallel model: every rank holds the same replicated state."""
+        return parallel.world_and_rank(self.process_group)[1] == 0
+
+    def _write_checkpoint(self, path, manifest, arrays):
+        """Rank 0 writes; the all-gather of its outcome is the barrier after which every rank may read the file."""
+        error = None
+        if self._is_writer():
+            try:
+                checkpoint.write(path, manifest, arrays)
+            except Exception as e:              # noqa: BLE001 -- re-raised below, after the other ranks learn of it
+                error = e
+        failed = parallel.all_gather_ints([error is not None], self.process_group, self.device)
+        if error is not None:
+            raise error
+        if failed.any():
+            raise RuntimeError(f"rank 0 could not write {path}")
+
+    def _check_replicas(self):
+        """After a load, every rank must hold the same state: refuse to continue if (train step count, epochs done, CRC of
+        the parameters) differs between ranks."""
+        if parallel.world_and_rank(self.process_group)[0] == 1:
+            return
+        crc = zlib.crc32(self.get_flat_weights().tobytes())
+        rows = parallel.all_gather_ints([self._train_step_count, self._epochs_done, crc], self.process_group, self.device)
+        if (rows != rows[0]).any():
+            raise RuntimeError(f"the ranks hold different states after the load (step count, epochs done, parameter CRC "
+                               f"per rank: {rows.tolist()})")
+
+    def save_weights(self, path):
+        """Keras ``save_weights``: every trainable variable (the InfoNCE output encoder's included), float32 in Keras
+        orientation, into one checkpoint file (:mod:`dib_b200.checkpoint`).  The fp32 master weights are saved, so the file
+        loads into a model of the same architecture at any precision."""
+        names, shapes = self._variable_specs()
+        self._write_checkpoint(path, self._manifest("weights"), checkpoint.split(self.get_flat_weights(), names, shapes))
+
+    def load_weights(self, path):
+        """Keras ``load_weights`` from a file of :meth:`save_weights` or :meth:`save`: the variables' names and shapes must
+        match this model's (ValueError naming the first that differs, weights untouched).  The values are copied into the
+        existing parameter buffer, so captured CUDA graphs stay valid."""
+        manifest, members = checkpoint.read(path)
+        checkpoint.check_variables(manifest, *self._variable_specs())
+        flat = torch.from_numpy(checkpoint.flatten(manifest, members))
+        with torch.cuda.device(self.device):
+            self._params.copy_(flat)
+        self._check_replicas()
+
+    def save(self, path, include_optimizer=True):
+        """Keras ``model.save``: the weights, the model's constructor arguments and -- ``include_optimizer`` on a compiled
+        model -- the compile configuration and the training state: both optimizer slot buffers, the optimizer step, beta,
+        the learning rate, the Philox step count, the noise and shuffle seeds, the inference-call count and the number of
+        completed epochs.  :func:`load_model` then continues exactly where this model stands.  Under torch.distributed
+        rank 0 writes and every rank returns once the file is complete."""
+        names, shapes = self._variable_specs()
+        manifest = self._manifest("model")
+        arrays = checkpoint.split(self.get_flat_weights(), names, shapes)
+        if include_optimizer and self.optimizer is not None:
+            manifest["compile"] = self._compile_config()
+            manifest["state"] = dict(
+                beta=float(self.beta.value()), optimizer_step=int(self._step_dev.item()),
+                train_step_count=int(self._train_step_count), noise_seed=int(self.noise_seed), seed=int(self.seed),
+                inference_calls=int(self._inference_calls), epochs_done=int(self._epochs_done))
+            arrays[checkpoint.SLOTS[0]] = self._m.detach().cpu().numpy()
+            arrays[checkpoint.SLOTS[1]] = self._v.detach().cpu().numpy()
+        self._write_checkpoint(path, manifest, arrays)
+
+    def _check_restorable(self, manifest):
+        """Refuse (ValueError, nothing changed) a training state this compiled model cannot continue from: another model
+        class or architecture, another optimizer class or hyperparameters (the learning rate is restored), another loss or
+        InfoNCE spec, or a file without a training state."""
+        if self.optimizer is None:
+            raise RuntimeError("call compile() before restoring a training state")
+        if "state" not in manifest:
+            raise ValueError(f"the file has no training state (a {manifest['kind']!r} file saved without the optimizer)")
+        if manifest["model"]["class"] != type(self).__name__:
+            raise ValueError(f"the file holds a {manifest['model']['class']}, the model is a {type(self).__name__}")
+        mine, theirs = json.loads(json.dumps(self.get_config())), manifest["model"]["config"]
+        for k in sorted(set(mine) | set(theirs)):
+            if k not in ("precision", "seed") and mine.get(k) != theirs.get(k):
+                raise ValueError(f"architecture differs in {k!r}: the file has {theirs.get(k)!r}, the model {mine.get(k)!r}")
+        checkpoint.check_variables(manifest, *self._variable_specs())
+        mine, theirs = json.loads(json.dumps(self._compile_config())), manifest["compile"]
+        if mine["optimizer"]["class"] != theirs["optimizer"]["class"]:
+            raise ValueError(f"the file was trained with {theirs['optimizer']['class']}, the model is compiled with "
+                             f"{mine['optimizer']['class']}")
+        hyper = lambda c: {k: v for k, v in c["optimizer"]["config"].items() if k != "learning_rate"}
+        if hyper(mine) != hyper(theirs):
+            raise ValueError(f"optimizer hyperparameters differ: the file has {hyper(theirs)}, the model {hyper(mine)}")
+        if mine["loss"] != theirs["loss"]:
+            raise ValueError(f"the loss differs: the file has {theirs['loss']}, the model {mine['loss']}")
+
+    def _restore(self, manifest, members):
+        """Continue from the training state of a :meth:`save` file, in place: parameters, slots and counters are copied into
+        the existing buffers, so captured CUDA graphs stay valid; the next replay reloads the Philox step and the learning
+        rate from the restored values."""
+        self._check_restorable(manifest)
+        st = manifest["state"]
+        with torch.cuda.device(self.device):
+            self._params.copy_(torch.from_numpy(checkpoint.flatten(manifest, members)))
+            self._m.copy_(torch.from_numpy(members[checkpoint.SLOTS[0]]))
+            self._v.copy_(torch.from_numpy(members[checkpoint.SLOTS[1]]))
+            self._step_dev.fill_(int(st["optimizer_step"]))
+            self.beta.assign(np.float32(st["beta"]))
+            self.optimizer.learning_rate = manifest["compile"]["optimizer"]["config"]["learning_rate"]
+            self._lr_host = None
+            self._sync_lr()
+        if int(st["noise_seed"]) != self.noise_seed:       # captured steps pass the noise seed by value
+            self._graphs.clear(); self._graph_seen.clear()
+        self.noise_seed, self.seed = int(st["noise_seed"]), int(st["seed"])
+        self._train_step_count = int(st["train_step_count"])
+        self._step_dev_dirty = True
+        self._inference_calls = int(st["inference_calls"])
+        self._epochs_done = int(st["epochs_done"])
+        self._check_replicas()
+
+    def _restore_backup(self, path):
+        """BackupAndRestore: restore the training state at ``path`` if the file exists (on every rank, or on none) and
+        return the number of completed epochs; None when there is no backup."""
+        exists = os.path.exists(path)
+        if len(set(parallel.all_gather_ints([exists], self.process_group, self.device)[:, 0])) > 1:
+            raise RuntimeError(f"the backup {path} exists on some ranks only")
+        if not exists:
+            return None
+        self._restore(*checkpoint.read(path))
+        return self._epochs_done
 
 
 class PendingBatchResult:
@@ -1841,6 +2034,23 @@ class SetTransformerIBNet(DistributedIBNet):
                                            self.final_processing_arch, self.output_dimensionality,
                                            self.number_positional_encoding_frequencies if self.use_positional_encoding else 1)
 
+    def get_config(self):
+        return dict(particle_feature_dimensions=self.particle_feature_dimensions,
+                    particle_encoder_arch_spec=list(self.feature_encoder_architecture),
+                    bottleneck_dimension=self.feature_embedding_dimension, number_particles=self.number_particles,
+                    key_dim=self.key_dim, number_heads=self.number_heads, number_attention_blocks=self.number_attention_blocks,
+                    ff_arch_per_block=list(self.ff_arch_per_block), ff_activation_fn=self.ff_activation_fn,
+                    final_processing_arch=list(self.final_processing_arch), activation_fn=self.activation_fn,
+                    leaky_alpha=self.leaky_alpha, output_dimensionality=self.output_dimensionality,
+                    logvar_initialization=self.logvar_offset,
+                    number_positional_encoding_frequencies=self.number_positional_encoding_frequencies,
+                    precision=self.precision, variable_set_sizes=self.variable_set_sizes, seed=self.seed,
+                    dropout_rate=self.dropout_rate, kl_loss_exponent=self.kl_loss_exponent, kl_loss_scale=self.kl_loss_scale)
+
+    def _variable_specs(self):
+        specs = self.param_specs()
+        return [n for n, _, _ in specs], [tuple(s) for _, s, _ in specs]
+
     def _param_inits(self):
         """[KERAS] glorot_uniform kernels with the fans of ``_compute_fans`` (3-D attention kernels included), zero biases,
         LayerNorm gamma = 1 and beta = 0."""
@@ -1864,3 +2074,32 @@ class SetTransformerIBNet(DistributedIBNet):
     def compression_matrices(self, *a, **k):
         raise NotImplementedError("compression matrices of particles: run model.particle_encoder on the particle rows and "
                                   "utils.bhattacharyya_dist_mat on its output")
+
+
+_MODEL_CLASSES = {"DistributedIBNet": DistributedIBNet, "SetTransformerIBNet": SetTransformerIBNet}
+
+
+def load_model(path, device=None, process_group=None):
+    """Keras ``load_model`` of a :meth:`DistributedIBNet.save` file: rebuild the model from its constructor arguments on
+    ``device`` (default: the current CUDA device) in ``process_group``, compile it as it was compiled and restore its training
+    state, so ``fit`` / ``train_on_batch`` / ``evaluate`` continue exactly as in the process that saved it.  A file saved
+    with ``include_optimizer=False`` gives an uncompiled model with the saved weights."""
+    manifest, members = checkpoint.read(path)
+    if manifest["kind"] != "model":
+        raise ValueError(f"{path} is a {manifest['kind']!r} file: build the model and call load_weights")
+    cls = _MODEL_CLASSES.get(manifest["model"]["class"])
+    if cls is None:
+        raise ValueError(f"{path}: unknown model class {manifest['model']['class']!r}")
+    model = cls(**manifest["model"]["config"], device=device, process_group=process_group)
+    if "state" not in manifest:
+        model.load_weights(path)
+        return model
+    comp = manifest["compile"]
+    opt_cls = {"Adam": Adam, "SGD": SGD, "RMSprop": RMSprop}[comp["optimizer"]["class"]]
+    loss = dict(comp["loss"])
+    kind = loss.pop("kind")
+    model.compile(optimizer=opt_cls(**comp["optimizer"]["config"]), loss=InfoNCE(**loss) if kind == "infonce" else kind,
+                  metrics=[_metrics.deserialize(m) for m in comp["metrics"]] or None,
+                  weighted_metrics=[_metrics.deserialize(m) for m in comp["weighted_metrics"]] or None)
+    model._restore(manifest, members)
+    return model

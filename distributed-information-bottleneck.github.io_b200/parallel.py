@@ -44,3 +44,16 @@ def allreduce_sum_(flat: torch.Tensor, group=None):
     if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
         dist.all_reduce(flat, op=dist.ReduceOp.SUM, group=group)
     return flat
+
+
+def all_gather_ints(values, group=None, device=None):
+    """Every rank's int64 ``values`` as an array [world, len(values)] (rows in rank order); one row for a single process.  A
+    collective: every rank of the group must call it.  ``device`` is where NCCL exchanges (gloo exchanges host tensors)."""
+    own = torch.tensor([int(v) for v in values], dtype=torch.int64)
+    if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
+        return own[None].numpy()
+    if dist.get_backend(group) == "nccl":
+        own = own.to(device)
+    rows = [torch.empty_like(own) for _ in range(dist.get_world_size(group))]
+    dist.all_gather(rows, own, group=group)
+    return torch.stack(rows).cpu().numpy()
