@@ -187,6 +187,11 @@ SIGNATURES = {
                                        c_void_p, c_void_p, c_int32, c_int32, c_float, c_int32, c_void_p, c_int32, c_float,
                                        c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_void_p,
                                        c_void_p, c_void_p, POINTER(c_int32), c_void_p]),
+    "dib_debug_enc_fused": (c_int32, [c_int32, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_float, c_int32, c_float,
+                                      c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32,
+                                      c_int64, c_void_p, c_int32, c_void_p, c_uint64, c_uint32, c_void_p, c_uint64, c_void_p,
+                                      c_int32, c_void_p, c_void_p, c_int32, c_void_p, c_int32, c_void_p, c_int32, c_void_p,
+                                      c_int32, c_void_p, c_float, c_float, c_void_p, c_int64, c_void_p, c_void_p]),
     "dib_debug_force_unfused": (c_int32, [c_void_p, c_int32]),
     "dib_last_error": (c_char_p, []),
     "dib_build_info": (c_char_p, []),

@@ -1,5 +1,6 @@
 // dib_api.cu -- the C ABI declared in include/dib_b200.h: model description, workspace plan, and the
 // orchestration of one forward / train step as a fixed sequence of asynchronous launches on the caller's stream.
+#include <algorithm>
 #include <atomic>
 #include <cmath>
 #include <cstddef>
@@ -1702,6 +1703,134 @@ int dib_debug_int16_fwd2(int32_t bf16, const void* g_in, int32_t ld_in, int32_t 
   return sync_result(fn, dib_int16_fwd2_head(g_in, ld_in, K0, w16_0, b0, w16_1, b1, g1, wout, bout, act, out_act, alpha, loss, y,
                                              M, inv_batch, gscale, dg2, dg1, dbpart, demb, user_pred, wpart, wpart_stride,
                                              loss_part, acc_part, nblocks, weights, bf16, st), st);
+}
+
+// the fused encoder kernels (dib_enc_fused.cu): the weight pack, the forward and the backward, as forward_encoders and
+// backward_encoders launch them, on a grid the caller picks (unit tests)
+int dib_debug_enc_fused(int32_t phases, int32_t F, const int32_t* fdim, const int32_t* x_off, int32_t nfreq, int32_t act,
+                        float alpha, int32_t bf16, float logvar_offset, const float* params, int64_t param_count,
+                        const int64_t* w0_off, const int64_t* b0_off, const int64_t* w1_off, const int64_t* b1_off,
+                        const int64_t* w2_off, const int64_t* b2_off, int32_t grid, int64_t n, const float* x, int32_t ldx,
+                        const float* eps, uint64_t seed, uint32_t step, const uint32_t* step_dev, uint64_t sample_offset,
+                        float* emb, int32_t ldemb, float* user_emb, void* emb16, int32_t ldemb16, float* kl_part,
+                        int32_t kl_stride, const float* d_emb, int32_t ldd, const void* d_emb16, int32_t ldd16,
+                        const float* beta_dev, float inv_batch, float gscale, float* part, int64_t split_stride, void* packed,
+                        void* stream) {
+  const std::string fn = "dib_debug_enc_fused: ";
+  auto str = [](long long v) { return std::to_string(v); };
+  auto misaligned = [](const void* p, uintptr_t a) { return reinterpret_cast<uintptr_t>(p) % a != 0; };
+  if (phases < 1 || phases > 7) return fail(fn + "phases is a mask of 1 (pack), 2 (forward) and 4 (backward) (phases = " + str(phases) + ")");
+  if (F < 1 || F > 65535) return fail(fn + "needs 1 <= F <= 65535 (F = " + str(F) + ")");
+  if (!fdim || !x_off) return fail(fn + "fdim and x_off must not be null");
+  if (nfreq < 1) return fail(fn + "needs nfreq >= 1 (nfreq = " + str(nfreq) + ")");
+  if (!known_act(act)) return fail(fn + "unknown act " + str(act));
+  if (bf16 != 0 && bf16 != 1) return fail(fn + "bf16 is 0 (fp16) or 1 (bf16)");
+  if (!w0_off || !b0_off || !w1_off || !b1_off || !w2_off || !b2_off) return fail(fn + "the six offset tables must not be null");
+  if (!params || param_count < 1) return fail(fn + "needs params and param_count >= 1");
+  if (!packed || misaligned(packed, 16)) return fail(fn + "packed must be a 16-byte aligned buffer of the 16-bit image");
+  const bool fwd = phases & 2, bwd = phases & 4;
+  // every feature's x columns and parameter blocks (w_in = fdim nfreq first-layer inputs, hidden 128, 2E = 64 outputs)
+  const int64_t span = bwd ? std::min<int64_t>(param_count, split_stride) : param_count;
+  for (int f = 0; f < F; ++f) {
+    const std::string at = " of feature " + str(f);
+    if (fdim[f] < 1 || fdim[f] > 3) return fail(fn + "needs 1 <= fdim <= 3 (fdim" + at + " = " + str(fdim[f]) + ")");
+    if (fdim[f] * nfreq + 1 > 16)
+      return fail(fn + "needs fdim nfreq + 1 <= 16 (fdim" + at + " = " + str(fdim[f]) + ", nfreq = " + str(nfreq) + ")");
+    if ((fwd || bwd) && (x_off[f] < 0 || (int64_t)x_off[f] + fdim[f] > ldx))
+      return fail(fn + "the x columns" + at + " must lie inside [0, ldx) (x_off = " + str(x_off[f]) + ", ldx = " + str(ldx) + ")");
+    const int64_t off[6] = {w0_off[f], b0_off[f], w1_off[f], b1_off[f], w2_off[f], b2_off[f]};
+    const int64_t size[6] = {(int64_t)fdim[f] * nfreq * 128, 128, 128 * 128, 128, 128 * 64, 64};
+    static const char* names[6] = {"w0_off", "b0_off", "w1_off", "b1_off", "w2_off", "b2_off"};
+    for (int k = 0; k < 6; ++k)
+      if (off[k] < 0 || off[k] + size[k] > span)
+        return fail(fn + "the parameter block " + names[k] + at + " must lie inside params" + (bwd ? " and split_stride" : "") +
+                    " (offset " + str(off[k]) + ", size " + str(size[k]) + ")");
+    if (bwd && (w1_off[f] % 2 || w2_off[f] % 2)) return fail(fn + "w1_off and w2_off" + at + " must be even (float2 stores)");
+  }
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const long long tiles = (n + 127) / 128, want = (long long)F * tiles;
+  if ((fwd || bwd) && (n < 1 || n > 0x7fffffffll)) return fail(fn + "needs 1 <= n < 2^31 (n = " + str(n) + ")");
+  int sms = 0, dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+    return fail(fn + "cannot read the multiprocessor count");
+  // grid 0: the library's choice for the phase (forward: two CTAs per SM, backward: one)
+  const long long cap_fwd = (long long)sms * dib_enc_fused_fwd_ctas_per_sm(), cap_bwd = sms;
+  const int grid_fwd = grid ? grid : (int)std::min(want, cap_fwd), grid_bwd = grid ? grid : (int)std::min(want, cap_bwd);
+  if ((fwd || bwd) && (grid < 0 || grid > want))
+    return fail(fn + "needs 0 <= grid <= F ceil(n / 128) = " + str(want) + " (grid = " + str(grid) + ")");
+  if (fwd) {
+    if (!x) return fail(fn + "the forward needs x");
+    if (!emb && !emb16 && !user_emb) return fail(fn + "the forward needs emb, user_emb or emb16");
+    if (emb && (misaligned(emb, 8) || ldemb % 2 || ldemb < F * 32))
+      return fail(fn + "emb must be 8-byte aligned with ldemb even and >= F * 32 (ldemb = " + str(ldemb) + ")");
+    if (user_emb && misaligned(user_emb, 8)) return fail(fn + "user_emb must be 8-byte aligned");
+    if (emb16 && (misaligned(emb16, 4) || ldemb16 % 2 || ldemb16 < F * 32))
+      return fail(fn + "emb16 must be 4-byte aligned with ldemb16 even and >= F * 32 (ldemb16 = " + str(ldemb16) + ")");
+    if (!kl_part) return fail(fn + "the forward needs kl_part");
+    if (kl_stride < (grid_fwd + F - 1) / F)
+      return fail(fn + "needs kl_stride >= ceil(grid / F) = " + str((grid_fwd + F - 1) / F) + " (kl_stride = " + str(kl_stride) + ")");
+  }
+  if (bwd) {
+    if (!x) return fail(fn + "the backward needs x");
+    if (!d_emb == !d_emb16) return fail(fn + "the backward takes exactly one of d_emb and d_emb16");
+    if (d_emb && (misaligned(d_emb, 8) || ldd % 2 || ldd < F * 32))
+      return fail(fn + "d_emb must be 8-byte aligned with ldd even and >= F * 32 (ldd = " + str(ldd) + ")");
+    if (d_emb16 && (misaligned(d_emb16, 16) || ldd16 % 8 || ldd16 < F * 32))
+      return fail(fn + "d_emb16 must be 16-byte aligned with ldd16 a multiple of 8 and >= F * 32 (ldd16 = " + str(ldd16) + ")");
+    if (!beta_dev) return fail(fn + "the backward needs beta_dev");
+    int ex = 0;
+    if (!(gscale > 0.f) || std::isinf(gscale) || std::frexp(gscale, &ex) != 0.5f)
+      return fail(fn + "gscale must be a power of two (gscale = " + std::to_string(gscale) + ")");
+    if (!part || misaligned(part, 8) || split_stride % 2)
+      return fail(fn + "the backward needs part 8-byte aligned and split_stride even (split_stride = " + str(split_stride) + ")");
+  }
+  if (eps && misaligned(eps, 8)) return fail(fn + "eps must be 8-byte aligned");
+  // the descriptor tables live on the device, as dib_create leaves them
+  std::vector<long long> tab(6 * (size_t)F);
+  std::vector<int> itab(2 * (size_t)F);
+  for (int f = 0; f < F; ++f) {
+    tab[f] = w0_off[f]; tab[F + f] = b0_off[f]; tab[2 * F + f] = w1_off[f];
+    tab[3 * F + f] = b1_off[f]; tab[4 * F + f] = w2_off[f]; tab[5 * F + f] = b2_off[f];
+    itab[f] = x_off[f]; itab[F + f] = fdim[f];
+  }
+  const size_t tb = tab.size() * sizeof(long long), ib = itab.size() * sizeof(int);
+  char* dt = nullptr;
+  DIB_CUDA_OK(cudaMalloc(&dt, tb + ib));
+  cudaError_t e = cudaMemcpy(dt, tab.data(), tb, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(dt + tb, itab.data(), ib, cudaMemcpyHostToDevice);
+  const long long* lt = reinterpret_cast<const long long*>(dt);
+  const int* it = reinterpret_cast<const int*>(dt + tb);
+  DibEncFusedDesc d;
+  d.F = F; d.nfreq = nfreq; d.act = act; d.alpha = alpha; d.bf16 = bf16; d.logvar_offset = logvar_offset;
+  d.w0_off = lt; d.b0_off = lt + F; d.w1_off = lt + 2 * F; d.b1_off = lt + 3 * F; d.w2_off = lt + 4 * F; d.b2_off = lt + 5 * F;
+  d.x_off = it; d.fdim = it + F;
+  DibEncFusedIO io;
+  io.params = params; io.packed = packed; io.x = x; io.ldx = ldx; io.n = n;
+  io.eps = eps; io.seed = seed; io.step = step; io.step_dev = step_dev; io.sample_offset = sample_offset;
+  io.emb = nullptr; io.ldemb = 0; io.user_emb = nullptr; io.kl_part = nullptr; io.kl_stride = 0;
+  if (e == cudaSuccess && (phases & 1)) {
+    // the pack kernel also clears the KL partial table when it fits its grid, as forward_encoders has it do
+    const long long zn = kl_part ? (long long)F * kl_stride : 0;
+    const bool clear = zn > 0 && zn <= dib_enc_fused_pack_zero_capacity(F);
+    e = dib_enc_fused_pack(d, params, packed, clear ? kl_part : nullptr, clear ? zn : 0, st);
+  }
+  if (e == cudaSuccess && fwd) {
+    DibEncFusedIO fo = io;
+    fo.emb = emb; fo.ldemb = ldemb; fo.user_emb = user_emb; fo.kl_part = kl_part; fo.kl_stride = kl_stride;
+    fo.emb16 = emb16; fo.ldemb16 = ldemb16;
+    d.grid = grid_fwd;
+    e = dib_enc_fused_forward(d, fo, st);
+  }
+  if (e == cudaSuccess && bwd) {
+    DibEncFusedBwdIO b;
+    b.d_emb = d_emb; b.ldd = ldd; b.d_emb16 = d_emb16; b.ldd16 = d_emb16 ? ldd16 : 0;
+    b.beta_dev = beta_dev; b.inv_batch = inv_batch; b.gscale = gscale; b.part = part; b.split_stride = split_stride;
+    d.grid = grid_bwd;
+    e = dib_enc_fused_backward(d, io, b, st);
+  }
+  const int r = sync_result(fn, e, st);
+  cudaFree(dt);
+  return r;
 }
 #undef DIB_HOOK_CHECK
 

@@ -224,13 +224,18 @@ __device__ __forceinline__ void frag_dgrad_to_a(const float (&d)[64], uint32_t h
 
 // first-layer operand row: [x_0..x_{d-1}, sin(2x).., sin(4x).., ..., 1, 0...] (models.py:22-23 + the ones column
 // that carries every layer's bias through the bias-carrier matrices).  xv = the row's feature values.
-// sin for the positional encoding: reduce to one period in units of turns, then the SFU (sin.approx of an argument in
-// [-pi, pi] is good to ~1e-6 absolute; the reduction adds |arg| * 6e-8) -- no local-memory slow path like sinf's, and far
-// below the 16-bit operand rounding (5e-4 relative) that follows.
+// sin for the positional encoding: subtract the nearest whole number of turns k 2 pi in two fma steps (Cody-Waite: 2 pi =
+// C1 + C2, C1 = fl(2 pi)), then the SFU (sin.approx of an argument in [-pi, pi] is good to 2^-20.5 absolute).  The first
+// step is exact: k C1 is a multiple of C1's last bit 2^-21, a (|a| >= pi, else k = 0) of 2^-22, and their difference, a
+// multiple of 2^-22 below 4, fits 24 bits.  The second step rounds once, by at most 2^-23, so the reduced argument is within
+// 2^-23 (plus |k| 2^-24 |C2| for C2's own rounding) of a - 2 pi k for |a| < 2^17 -- no local-memory slow path like sinf's.  Reducing
+// in units of turns instead (t = a fl(1 / 2 pi), t - rint(t)) loses |a| 2^-24 turns to the rounding of t: 4e-3 at
+// nfreq = 15 and |x| = 4, several fp16 ulps of the operand.
 __device__ __forceinline__ float dib_sin_pe(float a) {
-  float t = a * 0.15915494309189535f;
-  t -= rintf(t);
-  return __sinf(6.283185307179586f * t);
+  const float k = rintf(a * 0.15915494309189535f);
+  float r = fmaf(-k, 6.28318548202514648f, a);
+  r = fmaf(-k, -1.7484555314695172e-07f, r);
+  return __sinf(r);
 }
 constexpr int kMaxFeatDim = 3;     // d * nfreq + 1 <= 16 and nfreq >= 1
 template <bool BF16>

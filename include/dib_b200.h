@@ -668,6 +668,33 @@ int dib_debug_int16_fwd2(int32_t bf16, const void* g_in, int32_t ld_in, int32_t 
                          void* dg2, void* dg1, float* dbpart, void* demb, float* user_pred, float* wpart, int32_t wpart_stride,
                          float* loss_part, float* acc_part, const float* weights, int32_t* nblocks, void* stream);
 
+/* dib_debug_enc_fused: the fused per-feature encoder kernels of the 'fp16' / 'bf16' precision (csrc/dib_enc_fused.cu), launched
+ * through the launchers the step uses; phases is a mask: 1 = pack the fp32 params into the 16-bit image `packed` (bias
+ * carriers, b2's logvar half + logvar_offset), and clear kl_part [F][kl_stride] when the pack grid covers it; 2 = forward:
+ * per row r < n and feature f, emb[r, 32 f + e] = TF32(u), user_emb[r, 32 f + e] = u, emb16 = r(u) (each nullable),
+ * u = mu + exp(lv / 2) eps, and kl_part[f kl_stride + slot] = the KL sum of the slot's rows; 4 = backward from d_emb [n, ldd]
+ * (fp32, times gscale) or d_emb16 [n, ldd16] (16-bit, already times gscale) -- exactly one -- into the weight-gradient
+ * partials part[slot split_stride + the parameter offsets].  The feature f has fdim[f] (1..3) x columns from x_off[f] of x
+ * [n, ldx], nfreq - 1 sinusoid blocks, and its parameters at the host tables w0_off .. b2_off in the model's layout (W0
+ * [fdim nfreq, 128], b0 [128], W1 [128, 128], b1 [128], W2 [128, 64], b2 [64]).  eps [n, F, 32] or, when null, the Philox
+ * noise of (seed, step + *step_dev, sample_offset + r).  grid 0 is the library's choice per phase (forward min(F tiles,
+ * 2 SMs), backward min(F tiles, SMs)); otherwise 1 <= grid <= F ceil(n / 128), the same for both phases.  With grid >= F
+ * CTA c serves feature c % F and its tiles c / F, c / F + nslots, ...; with grid < F it walks features c, c + grid, ....
+ * Slot rows of a feature served by fewer CTAs are not written (the step clears them).  Checks every argument on the host
+ * before any launch and fails naming the bad one: fdim nfreq + 1 <= 16, x columns and parameter blocks in range (and, in
+ * the backward, inside split_stride), even leading dimensions and 8-byte bases for the float2 accesses, a 16-byte d_emb16
+ * with ldd16 a multiple of 8 and >= 32 F, kl_stride >= ceil(grid / F), gscale a power of two.  Synchronises the stream.
+ * tests/test_gpu_enc_fused_kernels.py checks the kernels element by element against a float64 reference. */
+int dib_debug_enc_fused(int32_t phases, int32_t F, const int32_t* fdim, const int32_t* x_off, int32_t nfreq, int32_t act,
+                        float alpha, int32_t bf16, float logvar_offset, const float* params, int64_t param_count,
+                        const int64_t* w0_off, const int64_t* b0_off, const int64_t* w1_off, const int64_t* b1_off,
+                        const int64_t* w2_off, const int64_t* b2_off, int32_t grid, int64_t n, const float* x, int32_t ldx,
+                        const float* eps, uint64_t seed, uint32_t step, const uint32_t* step_dev, uint64_t sample_offset,
+                        float* emb, int32_t ldemb, float* user_emb, void* emb16, int32_t ldemb16, float* kl_part,
+                        int32_t kl_stride, const float* d_emb, int32_t ldd, const void* d_emb16, int32_t ldd16,
+                        const float* beta_dev, float inv_batch, float gscale, float* part, int64_t split_stride, void* packed,
+                        void* stream);
+
 /* bring-up switch for THIS handle (bit mask, 0 = the default kernels): 1 = unfused encoder kernels, 2 = integration network on
  * fp32-storage TF32 kernels, 4 = no fused integration tail (per-layer 16-bit GEMMs plus a head kernel), 8 = the generic head
  * kernel even when output_dimensionality == 1, 16 = the fused tail without its dgrad stages (the backward launches those

@@ -10,11 +10,11 @@ equal oracle/dib_oracle.py's ``forward`` / ``train_grads``: the two oracles diff
 
 Rounding points (kernel files under distributed-information-bottleneck.github.io_b200/csrc/):
   encoder forward (dib_enc_fused.cu)
-    * [pe | 1] operand                          write_a0_row :214-235 (pack2 of the sin / x values)
-    * W0, W1, W2, b0, b1, b2 + logvar_offset    dib_enc_pack_weights_kernel :733-765 (biases enter as bias-carrier rows)
-    * h1 = r(act(z1)), h2 = r(act(z2))          frag_to_a :152 (forward), frag_to_tile :137 (recomputed in the backward)
-    * (mu, logvar) = the fp32 accumulator; u = mu + exp(logvar / 2) eps and KL in fp32 (:460-469)
-    * emb16 = r(u); the user-visible emb is u itself (:470-471)
+    * [pe | 1] operand                          write_a0_row :242-264 (pack2 of the dib_sin_pe / x values)
+    * W0, W1, W2, b0, b1, b2 + logvar_offset    dib_enc_pack_weights_kernel :913-945 (biases enter as bias-carrier rows)
+    * h1 = r(act(z1)), h2 = r(act(z2))          frag_to_a :163-172 (forward :466, :472; the backward's recomputation :721, :733)
+    * (mu, logvar) = the fp32 accumulator; u = mu + exp(logvar / 2) eps and KL in fp32 (:495-498)
+    * emb16 = r(u); the user-visible emb is u itself (:500-506)
   integration network (dib_int16.cu)
     * W_j of the hidden layers                  dib_f32_to_16_segs_kernel :959 (biases, head weights and bias stay fp32)
     * g_{j+1} = r(act(g_j W_j + b_j))           FWD epilogue :215, fused tail e0 :443 and e1 :462
@@ -25,11 +25,13 @@ Rounding points (kernel files under distributed-information-bottleneck.github.io
     * d_emb16 = r(dg_0 W_0^T)                   DGRAD without act' (g_in = null), fused tail e3 :582
     * output layer: dW = g_L^T dzs, db = sum dzs (no S); hidden dW_j = g_j^T dg_j / S (WGRAD :212); bias sums / S (dib_api.cu:926, :942)
   encoder backward (dib_enc_fused.cu)
-    * g = d_emb16 as stored, or the fp32 d_emb times S (:619-622); bs = beta_eff * inv_batch * S (:567)
-    * dO = r([g + bs mu | g eps sigma / 2 + bs (sigma^2 - 1) / 2])   :627-634
-    * dz2 = r(G2 act'(h2)), dz1 = r(G1 act'(h1))   frag_dgrad_to_tile :180-199 (relu: rounded, then gated -- the same value)
+    * g = d_emb16 as stored, or the fp32 d_emb times S (:768-773); bs = beta_eff * inv_batch * S (:743)
+    * dO = r([g + bs mu | g eps sigma / 2 + bs (sigma^2 - 1) / 2])   :775-784
+    * dz2 = r(G2 act'(h2)), dz1 = r(G1 act'(h1))   frag_dgrad_to_a :205-223, called at :819 / :851 (relu: rounded, then
+      gated -- the same value)
     * dW2 = h2^T dO, dW1 = h1^T dz2, [dW0; db0] = dz1^T [pe | 1]; db2 / db1 are column sums of the 16-bit dO / dz2 (the ones
-      column of [pe | 1] is an MMA operand); everything * 1/S on the flush (:696)
+      column of [pe | 1] is an MMA operand); everything * 1/S on the flush (:877-905)
+  tests/enc_fused_reference.py restates these kernels per tile and per (feature, slot) for the element-by-element GPU test.
 """
 from __future__ import annotations
 
@@ -90,10 +92,10 @@ def _encoder_forward(cfg, layers, x_i, fmt):
     (W0, b0), (W1, b1), (W2, b2) = layers
     pe = O.positional_encoding(x_i, cfg.frequencies) if cfg.use_positional_encoding else x_i
     a0 = R(pe)                                                          # write_a0_row :234
-    h1 = R(_act(cfg, a0 @ R(W0) + R(b0)))                               # pack :749 (b0 = row w_in of W0p); frag_to_a :436
-    h2 = R(_act(cfg, R(b1) + h1 @ R(W1)))                               # bias-carrier step first (:351), then W1; :442
+    h1 = R(_act(cfg, a0 @ R(W0) + R(b0)))                               # pack (b0 = row w_in of W0p); frag_to_a
+    h2 = R(_act(cfg, R(b1) + h1 @ R(W1)))                               # bias-carrier step first (mma_layer1_rs), then W1
     off = np.concatenate([np.zeros(E), np.full(E, cfg.logvar_offset)])
-    o = R(b2 + off) + h2 @ R(W2)                                        # pack :760: the offset is inside the rounded carrier
+    o = R(b2 + off) + h2 @ R(W2)                                        # pack: the offset is inside the rounded carrier
     return a0, h1, h2, o[:, :E], o[:, E:]
 
 
@@ -110,11 +112,11 @@ def forward(cfg, flat, x, eps, beta, y=None, loss=None, fmt=None, keep=False):
     for i in range(cfg.number_features):
         a0, h1, h2, mu, lv = _encoder_forward(cfg, encoders[i], xs[i], fmt)
         sig = np.exp(lv / 2.0)
-        embs.append(mu + sig * eps[:, i, :])                            # :466-467
-        kls.append((0.5 * (mu ** 2 + (np.expm1(lv) - lv))).sum(axis=-1).mean())   # :493 (sv * sv - lv - 1)
+        embs.append(mu + sig * eps[:, i, :])                            # :497
+        kls.append((0.5 * (mu ** 2 + (np.expm1(lv) - lv))).sum(axis=-1).mean())   # :498 (sv * sv - lv - 1)
         enc.append((a0, h1, h2, mu, lv))
     emb = np.concatenate(embs, axis=-1)
-    g = R(emb)                                                          # emb16 :471
+    g = R(emb)                                                          # emb16 :502
     acts = [g]
     for j, (W, b) in enumerate(integration[:-1]):
         g = R(_act(cfg, g @ R(W) + b))                                  # FWD :215, e0 :443, e1 :462 (bias fp32)
@@ -140,20 +142,20 @@ def encoder_backward(cfg, fr, eps, g_emb, beta_eff, B, S, fmt):
     R = lambda v: round_to(v, fmt)
     E = cfg.feature_embedding_dimension
     eps = np.asarray(eps, dtype=np.float64)
-    bs = beta_eff / B * S                                               # :567
+    bs = beta_eff / B * S                                               # :744
     out = []
     for i in range(cfg.number_features):
         a0, h1, h2, mu, lv = fr.cache["enc"][i]
         (W0, _), (W1, _), (W2, _) = fr.cache["encoders"][i]
         g = g_emb[:, i * E:(i + 1) * E]
         sig = np.exp(lv / 2.0)
-        dO = R(np.concatenate([g + bs * mu, g * eps[:, i, :] * 0.5 * sig + bs * 0.5 * (sig * sig - 1.0)], axis=-1))   # :630-634
-        dz2 = R((dO @ R(W2).T) * _dact(cfg, h2))                        # frag_dgrad_to_tile :657
-        dz1 = R((dz2 @ R(W1).T) * _dact(cfg, h1))                       # :678
+        dO = R(np.concatenate([g + bs * mu, g * eps[:, i, :] * 0.5 * sig + bs * 0.5 * (sig * sig - 1.0)], axis=-1))   # :775-785
+        dz2 = R((dO @ R(W2).T) * _dact(cfg, h2))                        # frag_dgrad_to_a, :819
+        dz1 = R((dz2 @ R(W1).T) * _dact(cfg, h1))                       # frag_dgrad_to_a, :851
         w_in = W0.shape[0]
-        out += [(a0[:, :w_in].T @ dz1).ravel() / S, dz1.sum(axis=0) / S,                    # :686, :715-717
-                (h1.T @ dz2).ravel() / S, dz2.sum(axis=0) / S,                              # :670-673
-                (h2.T @ dO).ravel() / S, dO.sum(axis=0) / S]                                # :648-652
+        out += [(a0[:, :w_in].T @ dz1).ravel() / S, dz1.sum(axis=0) / S,                    # dW0p, :890-903
+                (h1.T @ dz2).ravel() / S, dz2.sum(axis=0) / S,                              # dW1 / db1
+                (h2.T @ dO).ravel() / S, dO.sum(axis=0) / S]                                # dW2 / db2
     return np.concatenate(out)
 
 
@@ -170,7 +172,7 @@ def train_grads(cfg, flat, x, y, eps, beta, loss, fmt=None, S=None, batch_for_me
     integration, acts = fr.cache["integration"], fr.cache["int_acts"]
     Li = len(integration) - 1
     if d_emb is not None:
-        g_emb = np.asarray(d_emb, dtype=np.float64).reshape(fr.emb.shape) * S            # :622
+        g_emb = np.asarray(d_emb, dtype=np.float64).reshape(fr.emb.shape) * S            # :772
         int_grads = [np.zeros(W.size + b.size) for W, b in integration]
     else:
         Wc, _ = integration[-1]
