@@ -95,7 +95,7 @@ GEMM_KERNELS = {"simt": 0, "tc": 1}
 GEMM_MODES = {"fwd": 0, "dgrad": 1, "wgrad": 2}
 
 
-# name -> (restype, argtypes); mirrors include/dib_b200.h one to one
+# name -> (restype, argtypes); mirrors include/dib_b200.h and include/dib_b200_test_hooks.h one to one
 SIGNATURES = {
     "dib_create": (c_int32, [POINTER(DibConfig), POINTER(c_void_p)]),
     "dib_destroy": (None, [c_void_p]),

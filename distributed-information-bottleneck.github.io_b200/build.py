@@ -22,7 +22,7 @@ CSRC = os.path.join(PKG_DIR, "csrc")
 OBJ_DIR = os.path.join(CSRC, "_obj")
 LIB_PATH = os.path.join(PKG_DIR, "libdib_b200.so")
 STAMP = LIB_PATH + ".srchash"
-HEADER = os.path.join(PKG_DIR, "..", "include", "dib_b200.h")
+HEADERS = [os.path.join(PKG_DIR, "..", "include", h) for h in ("dib_b200.h", "dib_b200_test_hooks.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
@@ -35,7 +35,7 @@ def _sources():
 
 
 def _headers():
-    return sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))) + [HEADER]
+    return sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))) + HEADERS
 
 
 def _digest(paths, extra=b""):

@@ -23,6 +23,8 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
+#include <vector>
+
 #include "dib_common.cuh"
 #include "dib_kernels.h"
 #include "dib_sm90.cuh"
@@ -1014,6 +1016,35 @@ cudaError_t launch_fused(K kern, int threads, int smem, int grid, cudaStream_t s
 size_t dib_enc_fused_pack_bytes(int F) { return (size_t)F * kPackElems * 2; }
 long long dib_enc_fused_pack_zero_capacity(int F) { return (long long)DIB_CEIL_DIV(kPackElems, 256) * 256 * F; }   // floats the pack kernel can also clear
 int dib_enc_fused_fwd_ctas_per_sm() { return 2; }
+
+// two hidden layers of HID, 2E = EO outputs, and a feature's fdim <= kMaxFeatDim x columns in nfreq blocks plus the bias
+// column within the K0 columns of the first layer's tile
+bool dib_enc_fused_shape_ok(int layers, const int* hidden, int E) {
+  return layers == 2 && hidden[0] == HID && hidden[1] == HID && 2 * E == EO;
+}
+bool dib_enc_fused_feature_ok(int fdim, int nfreq) {
+  return fdim >= 1 && fdim <= kMaxFeatDim && nfreq >= 1 && (long long)fdim * nfreq + 1 <= K0;
+}
+
+cudaError_t dib_enc_fused_upload_tables(DibEncFusedDesc& d, const int64_t* const off[6], const int* x_off, const int* fdim,
+                                        void** tables) {
+  const int F = d.F;
+  std::vector<long long> tab(6 * (size_t)F);
+  for (int k = 0; k < 6; ++k)
+    for (int f = 0; f < F; ++f) tab[(size_t)k * F + f] = off[k][f];
+  const size_t tb = tab.size() * sizeof(long long), ib = (size_t)F * sizeof(int);
+  char* dt = nullptr;
+  cudaError_t e = cudaMalloc(&dt, tb + 2 * ib);
+  if (e == cudaSuccess) e = cudaMemcpy(dt, tab.data(), tb, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(dt + tb, x_off, ib, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(dt + tb + ib, fdim, ib, cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) { cudaFree(dt); return e; }
+  const long long* lt = reinterpret_cast<const long long*>(dt);
+  d.w0_off = lt; d.b0_off = lt + F; d.w1_off = lt + 2 * F; d.b1_off = lt + 3 * F; d.w2_off = lt + 4 * F; d.b2_off = lt + 5 * F;
+  d.x_off = reinterpret_cast<const int*>(dt + tb); d.fdim = d.x_off + F;
+  *tables = dt;
+  return cudaSuccess;
+}
 
 cudaError_t dib_enc_fused_pack(const DibEncFusedDesc& d, const float* params, void* packed, float* zero, long long zero_n, cudaStream_t st) {
   dim3 grid(DIB_CEIL_DIV(kPackElems, 256), d.F);

@@ -1084,8 +1084,11 @@ cudaError_t dib_int16_wgrad(const DibInt16Wgrad* layers, int count, int M, long 
               : launch16<DIB_GEMM_WGRAD, false>(mA[0], mB[0], a[0], mA[1], mB[1], a[1], nt, st);
 }
 
+// whole kBK-column k-blocks of the fan-in and whole kBN-column tiles of the fan-out
+bool dib_int16_gemm_ok(int K, int N) { return K >= kBK && K % kBK == 0 && N >= kBN && N % kBN == 0; }
+
 bool dib_int16_fwd2_ok(int K0, int N1, int N2, int out_dim) {
-  return K0 % kBK == 0 && K0 >= kBK && N1 == kF2N && N2 == kF2N && out_dim == 1;
+  return dib_int16_gemm_ok(K0, N1) && N1 == kF2N && N2 == kF2N && out_dim == 1;
 }
 
 // g1 = act(g_in W0 + b0) -> HBM;  g2 = act(g1 W1 + b1) (on chip);  logit = g2 . wout + bout;  compiled loss / metric;
@@ -1148,11 +1151,16 @@ cudaError_t dib_int16_fwd2_head(const void* g_in, int ld_in, int K0, const void*
 
 int dib_int16_head_blocks(int num_sms) { return num_sms * 2; }
 
+// the kernels are launched with 8 hidden units per lane: K = 256
+bool dib_int16_head_ok(int K, int out_dim, bool head1) {
+  return K == 8 * 32 && out_dim >= 1 && out_dim <= kHeadMaxOut && (!head1 || out_dim == 1);
+}
+
 cudaError_t dib_int16_head(const void* g, int ldg, int K, const float* Wc, const float* bc, int out_dim, int out_act, int hid_act,
                            float alpha, int loss, const float* y, long long n, float inv_batch, float gscale, void* dg, int lddg,
                            float* user_pred, float* wpart, int wpart_stride, float* loss_part, float* acc_part, int nblocks,
                            bool head1, const float* weights, int bf16, cudaStream_t st) {
-  if (out_dim > kHeadMaxOut || out_dim < 1 || K != 256 || (head1 && out_dim != 1)) return cudaErrorInvalidValue;
+  if (!dib_int16_head_ok(K, out_dim, head1)) return cudaErrorInvalidValue;
 #define DIB_HEAD_T(OUT, BF, W)                                                                                          \
   dib_int16_head_kernel<8, OUT, (OUT <= 2 ? 4 : 1), BF, W><<<nblocks, kHeadWarps * 32, 0, st>>>(static_cast<const uint16_t*>(g), ldg, K, Wc, bc, out_dim,  \
       out_act, hid_act, alpha, loss, y, n, inv_batch, gscale, static_cast<uint16_t*>(dg), lddg, user_pred, wpart, wpart_stride, \

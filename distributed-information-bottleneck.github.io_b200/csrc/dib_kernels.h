@@ -3,10 +3,22 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <string>
+
 struct DibGemmProblem;
 
 // number of kernels launched by this library in this process (bench.py reports it as gpu_launches)
 void dib_note_launch(int n = 1);
+
+// records msg as this thread's dib_last_error() and returns 1, the C ABI's error code (dib_api.cu)
+int fail(const std::string& msg);
+
+#define DIB_CUDA_OK(expr)                                                                        \
+  do {                                                                                           \
+    cudaError_t _e = (expr);                                                                     \
+    if (_e != cudaSuccess)                                                                       \
+      return fail(std::string(#expr) + ": " + cudaGetErrorString(_e));                           \
+  } while (0)
 
 struct DibGemmLaunch {
   const DibGemmProblem* probs;  // device array, nprob entries
@@ -193,6 +205,12 @@ struct DibEncFusedIO {
   float* kl_part; int kl_stride;
   void* emb16 = nullptr; int ldemb16 = 0;   // optional fp16 copy of emb (16-bit integration path)
 };
+// the shapes the fused encoder kernels run; the descriptor tables (off[k][f]: offset k of w0, b0, w1, b1, w2, b2 of feature
+// f < d.F; x_off, fdim) copied to one device allocation *tables (the caller frees it) that d's table pointers point into
+bool dib_enc_fused_shape_ok(int layers, const int* hidden, int E);
+bool dib_enc_fused_feature_ok(int fdim, int nfreq);
+cudaError_t dib_enc_fused_upload_tables(DibEncFusedDesc& d, const int64_t* const off[6], const int* x_off, const int* fdim,
+                                        void** tables);
 size_t dib_enc_fused_pack_bytes(int F);
 long long dib_enc_fused_pack_zero_capacity(int F);
 int dib_enc_fused_fwd_ctas_per_sm();
@@ -226,6 +244,9 @@ struct DibInt16Wgrad { const void* g_in; int K; const void* dz; int N; float* dW
 cudaError_t dib_int16_wgrad(const DibInt16Wgrad* layers, int count, int M, long long split_stride, float out_scale, int bf16,
                             cudaStream_t st);
 int dib_int16_head_blocks(int num_sms);
+// widths the 16-bit GEMMs run (a layer of fan-in K, fan-out N) and the output head runs (hidden width K; head1: out = 1 kernel)
+bool dib_int16_gemm_ok(int K, int N);
+bool dib_int16_head_ok(int K, int out_dim, bool head1);
 // shapes the fused tail kernel (dib_int16_fwd2_head) handles: fan-in K0 of its first layer, its two widths, the output width
 bool dib_int16_fwd2_ok(int K0, int N1, int N2, int out_dim);
 cudaError_t dib_int16_fwd2_head(const void* g_in, int ld_in, int K0, const void* w16_0, const float* b0, const void* w16_1, const float* b1,
@@ -253,6 +274,10 @@ struct DibAttnArgs {
   // that reads set sizes takes one outside [1, L] as the nearest bound (dib_set_len)
   const int* set_sizes = nullptr; float* dsum = nullptr;
 };
+// set-transformer shapes the kernels run: the largest set (fixed-size or key-tiled), heads and key_dim, LayerNorm / pooling E
+int dib_attn_max_set_size(bool variable_sizes);
+bool dib_attn_heads_ok(int heads, int key_dim);
+bool dib_set_width_ok(int E);
 size_t dib_attn_smem_bytes(int L, int dk, bool backward);
 cudaError_t dib_attn_prepare();   // once per model: the kernels' shared-memory opt-in
 cudaError_t dib_launch_attn_fwd(const DibAttnArgs& a, cudaStream_t st);

@@ -253,6 +253,14 @@ __global__ void sum_rows_kernel(DibSumRows a) {
 
 }  // namespace
 
+// sets of up to 64 rows on the fixed-size kernels (shared memory sized in dib_attn_prepare) with key_dim <= 128, LayerNorm
+// and pooling over E <= 128 columns; heads * key_dim and E are multiples of 4, so the step's buffers need no pad columns
+int dib_attn_max_set_size(bool variable_sizes) { return variable_sizes ? DIB_MAX_VARIABLE_SET_SIZE : 64; }
+bool dib_attn_heads_ok(int heads, int key_dim) {
+  return heads >= 1 && key_dim >= 1 && key_dim <= 128 && (long long)heads * key_dim % 4 == 0;
+}
+bool dib_set_width_ok(int E) { return E >= 1 && E <= 128 && E % 4 == 0; }
+
 size_t dib_attn_smem_bytes(int L, int dk, bool backward) {
   const size_t rows = (size_t)L * (dk + 1), sq = (size_t)L * (L + 1);
   return sizeof(float) * (backward ? 4 * rows + 2 * sq + L : 3 * rows + sq);

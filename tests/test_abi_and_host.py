@@ -1,5 +1,5 @@
-"""CPU: the C-ABI library loads and exports every symbol include/dib_b200.h declares; host-side logic
-(beta schedule callback, shard arithmetic, Keras-compat objects, display-row selection)."""
+"""CPU: the C-ABI library loads and exports every symbol include/dib_b200.h and include/dib_b200_test_hooks.h declare;
+host-side logic (beta schedule callback, shard arithmetic, Keras-compat objects, display-row selection)."""
 import ctypes
 import os
 import re
@@ -8,15 +8,16 @@ import numpy as np
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+HEADERS = ("dib_b200.h", "dib_b200_test_hooks.h")
 
 
-def declared_symbols():
-    text = open(os.path.join(ROOT, "include", "dib_b200.h")).read()
+def declared_symbols(headers=HEADERS):
+    text = "".join(open(os.path.join(ROOT, "include", h)).read() for h in headers)
     text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
     return sorted(set(re.findall(r"\b(dib_[a-z_0-9]+)\s*\(", text)))
 
 
-def test_library_exports_every_declared_symbol():
+def test_library_exports_every_symbol_both_headers_declare():
     from dib_b200 import _lib
     lib = ctypes.CDLL(_lib.library_path() if os.path.exists(_lib.library_path()) else _lib._build.build_library())
     syms = declared_symbols()
@@ -24,6 +25,8 @@ def test_library_exports_every_declared_symbol():
     for s in syms:
         assert hasattr(lib, s), s
     assert set(syms) == set(_lib.SIGNATURES), set(syms) ^ set(_lib.SIGNATURES)
+    public = declared_symbols(HEADERS[:1])                  # the test hooks stay out of the public header
+    assert [s for s in public if s.startswith("dib_debug_")] == ["dib_debug_force_unfused"], public
     lib.dib_build_info.restype = ctypes.c_char_p
     assert b"sm_90a" in lib.dib_build_info()
 
@@ -124,17 +127,19 @@ def test_bench_accounting_matches_survey_numbers():
 
 
 def test_header_is_plain_c_and_links_from_c(tmp_path):
-    """The boundary is a C ABI: include/dib_b200.h must compile as C99 (no C++-isms outside the extern "C" guard) and a C
-    program must link against the library and reach a host-only entry point (the CTW estimator needs no GPU)."""
+    """The boundary is a C ABI: include/dib_b200.h and include/dib_b200_test_hooks.h must compile as C99 (no C++-isms outside
+    the extern "C" guard) and a C program must link against the library and reach a host-only entry point (the CTW estimator
+    needs no GPU)."""
     import os
     import shutil
     import subprocess
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    hdr = os.path.join(root, "include", "dib_b200.h")
     gcc = shutil.which("gcc")
     if gcc is None:
         pytest.skip("gcc not available")
-    subprocess.run([gcc, "-std=c99", "-Wall", "-pedantic", "-Werror", "-fsyntax-only", "-x", "c", hdr], check=True)
+    for h in HEADERS:
+        subprocess.run([gcc, "-std=c99", "-Wall", "-pedantic", "-Werror", "-fsyntax-only", "-x", "c",
+                        os.path.join(root, "include", h)], check=True)
     from dib_b200 import _lib
     lib_dir = os.path.dirname(_lib.library_path())
     src = tmp_path / "main.c"
@@ -161,7 +166,7 @@ def test_beta_variable_supports_the_reference_idioms():
     assert torch.equal(b * t, torch.tensor([0.25, 0.5])) and torch.equal(t / b, torch.tensor([4.0, 8.0]))
 
 
-def test_build_stamp_is_path_independent_and_locked(tmp_path):
+def test_build_stamp_covers_both_headers_and_is_path_independent(tmp_path):
     """ADVICE r1: the source stamp must not depend on where the tree lives (the GPU box snapshot is elsewhere)."""
     import importlib.util
     import shutil
@@ -170,10 +175,17 @@ def test_build_stamp_is_path_independent_and_locked(tmp_path):
     os.makedirs(dst.parent / "include")
     shutil.copytree(os.path.join(src, "csrc"), dst / "csrc", ignore=shutil.ignore_patterns("_obj"))
     shutil.copy(os.path.join(src, "build.py"), dst / "build.py")
-    shutil.copy(os.path.join(ROOT, "include", "dib_b200.h"), dst.parent / "include" / "dib_b200.h")
+    for h in HEADERS:
+        shutil.copy(os.path.join(ROOT, "include", h), dst.parent / "include" / h)
     def load(path):
         spec = importlib.util.spec_from_file_location("_b" + str(abs(hash(path))), path)
         mod = importlib.util.module_from_spec(spec)
         spec.loader.exec_module(mod)
         return mod
-    assert load(os.path.join(src, "build.py"))._hash() == load(str(dst / "build.py"))._hash()
+    copy = load(str(dst / "build.py"))
+    assert load(os.path.join(src, "build.py"))._hash() == copy._hash()
+    for h in HEADERS:                                       # editing either header changes the stamp: the library rebuilds
+        before = copy._hash()
+        with open(dst.parent / "include" / h, "a") as fh:
+            fh.write("\n")
+        assert copy._hash() != before, h
