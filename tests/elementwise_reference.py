@@ -89,9 +89,8 @@ from __future__ import annotations
 
 import numpy as np
 
-U = 2.0 ** -24
-C_BOUND = 2.0
-TINY = 2.0 ** -126
+from tests.fp_exact import C_BOUND, TINY, U, act_grad, gamma
+
 SUB = 2.0 ** -149            # an operation whose result is subnormal or underflows: up to one subnormal step absolutely
 Z_TOL = 2.0 ** -15
 TF32_HALF_ULP = 2.0 ** -11
@@ -102,18 +101,8 @@ ONE_M_EPS = float(np.float32(1.0) - np.float32(1e-7))
 ROWS_PER_BLOCK = 256
 
 
-def gamma(m):
-    m = np.asarray(m, np.float64)
-    return m * U / (1.0 - m * U)
-
-
 def f64(a):
     return np.asarray(a, np.float64)
-
-
-def f32(a):
-    """the fp32 value of a: what the kernels read"""
-    return np.asarray(a, np.float32).astype(np.float64)
 
 
 def sparse_label(t, C):
@@ -121,26 +110,6 @@ def sparse_label(t, C):
     t = f64(t)
     ok = (t > -1.0) & (t < C)
     return np.where(ok, np.trunc(np.where(ok, t, 0.0)), -1).astype(np.int64)
-
-
-# ---- activations --------------------------------------------------------------------------------------------------------
-def act_grad(act, h, alpha):
-    """dib_act_grad from the output h and its error bound"""
-    h = f64(h)
-    if act == "relu":
-        return (h > 0).astype(np.float64), np.zeros_like(h)
-    if act == "leaky_relu":
-        return np.where(h > 0, 1.0, float(np.float32(alpha))), np.zeros_like(h)
-    if act == "tanh":
-        v = 1.0 - h * h
-        return v, U * h * h + U * np.abs(v)
-    if act == "sigmoid":
-        v = h * (1.0 - h)
-        return v, U * np.abs(1.0 - h) * np.abs(h) + U * np.abs(v)
-    if act == "elu":
-        v = np.where(h > 0, 1.0, h + 1.0)
-        return v, np.where(h > 0, 0.0, U * np.abs(h + 1.0))
-    return np.ones_like(h), np.zeros_like(h)
 
 
 # ---- reparameterisation -------------------------------------------------------------------------------------------------

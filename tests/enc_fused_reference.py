@@ -5,7 +5,7 @@ tile and per (feature, slot), rounding exactly where the kernels round.  Not col
 Exactness (the exact regime).  relu, leaky ReLU with alpha = 1/4 and linear; dyadic x, weights, eps and d emb; a zero
 logvar: W2's logvar columns 0 and b2's logvar half -logvar_offset, so that the packed carrier fl32(b2 + logvar_offset) is 0,
 lv = 0 and both __expf(0) (forward) and expf(0) (backward) are 1.  Then every accumulator holds an exact sum (asserted with
-``int16_reference.fits`` on the terms' magnitudes, for the weight gradients over every tile one slot accumulates) and every
+``fp_exact.fits`` on the terms' magnitudes, for the weight gradients over every tile one slot accumulates) and every
 fp32 epilogue operation is restated in numpy float32, one operation per kernel operation:
   pack (:913-945)              W0p [16][128] = W0 rows k < w_in, b0 in row w_in, 0 below; W1; W2; Bb1 [16][128] = b1 in row
                                w_in; Bb2 [16][64] = fl32(b2 + logvar_offset (logvar half)) in row w_in -- each r() saturating
@@ -28,11 +28,11 @@ fp32 epilogue operation is restated in numpy float32, one operation per kernel o
                                nslots = ceil((G - f) / F); G < F: CTA c walks features c, c + G, ... with all their tiles
                                in slot 0.
 
-r() is ``fused16_oracle.round_to``: half to even, saturating (cvt.rn.satfinite).
+r() is ``fp_exact.round_to``: half to even, saturating (cvt.rn.satfinite).
 
 Bounded regime (``bounded_forward`` / ``bounded_backward``): lv != 0, tanh / sigmoid / elu, leaky ReLU with alpha = 0.2, and any
 sum that does not fit 24 bits.  Every value is the float64 function of the reference's own float64 intermediates, with a
-first-order bound e on its distance from the kernel's value, multiplied by ``elementwise_reference.C_BOUND`` at the outputs:
+first-order bound e on its distance from the kernel's value, multiplied by ``fp_exact.C_BOUND`` at the outputs:
   * SFU activations: ``int16_reference.act16`` (tanh.approx 2^-10.987 relative, ex2.approx 2^-22 relative plus the rounding
     of its argument) and one 16-bit ulp; |act'| <= 1 carries the pre-activation's error through; leaky ReLU / relu / linear
     restate fl32(alpha z) and r() and add one 16-bit ulp wherever the pre-activation is inexact.
@@ -62,16 +62,14 @@ from __future__ import annotations
 import numpy as np
 
 from tests import elementwise_reference as ER
-from tests.fused16_oracle import round_to
 from tests import int16_reference as I
-from tests.int16_reference import EXACT_BITS, dyadic, exact_matmul, fits, quantum, ulp16
+from tests.fp_exact import (C_BOUND, EXACT_BITS, U, dyadic, exact_matmul, f32, fits, gamma, quantum, r16, round_tf32,
+                             sparse_dyadic, ulp16)
 
 TM, HID, EO, K0, E = 128, 128, 64, 16, 32
 PACK_ELEMS = K0 * HID + HID * HID + HID * EO + K0 * HID + K0 * EO
 ACTS = ER.ACTS
 Z_TOL = ER.Z_TOL
-U = ER.U
-C_BOUND = ER.C_BOUND
 SIN_TOL = 2.0 ** -20.5 + 2.0 ** -22
 BLOCKS = ("w0", "b0", "w1", "b1", "w2", "b2")
 
@@ -79,22 +77,6 @@ BLOCKS = ("w0", "b0", "w1", "b1", "w2", "b2")
 def _has(fault, name):
     """fault is None, one fault name or a tuple of them"""
     return fault == name or (isinstance(fault, tuple) and name in fault)
-
-
-def r16(x, fmt):
-    return round_to(x, fmt)
-
-
-def f32(x):
-    return np.asarray(x, np.float64).astype(np.float32)
-
-
-def round_tf32(x):
-    """cvt.rna.tf32.f32 of fp32 values: 10 explicit mantissa bits, to nearest, ties away from zero."""
-    u = np.asarray(x, np.float32).view(np.uint32).astype(np.uint64)
-    r = ((u + np.uint64(0x1000)) & np.uint64(0xFFFFE000)).astype(np.uint32)
-    finite = np.isfinite(np.asarray(x, np.float32))
-    return np.where(finite, r.view(np.float32), np.asarray(x, np.float32)).astype(np.float64)
 
 
 # ---- parameter layout -----------------------------------------------------------------------------------------------------
@@ -233,7 +215,7 @@ def act16(act, z, alpha, fmt):
     return r16(z, fmt)
 
 
-def act_grad32(act, h, alpha):
+def exact_act_grad32(act, h, alpha):
     return np.where(h > 0, np.float32(1), np.float32(alpha)).astype(np.float32) if act == "leaky_relu" else (
         (h > 0).astype(np.float32) if act == "relu" else np.ones(np.shape(h), np.float32))
 
@@ -242,7 +224,7 @@ def dgrad16(act, G, h, alpha, fmt):
     """dz = r(G) gated by h > 0 (relu: relu_gate2 of the rounded h) or r(fl32(G act'(h)))."""
     if act == "relu":
         return r16(G, fmt) * (h > 0)
-    return r16((f32(G) * act_grad32(act, h, alpha)).astype(np.float64), fmt)
+    return r16((f32(G) * exact_act_grad32(act, h, alpha)).astype(np.float64), fmt)
 
 
 # ---- one feature, all rows ---------------------------------------------------------------------------------------------------
@@ -301,7 +283,7 @@ def forward(img_all, x, x_off, fdims, nfreq, act, alpha, fmt, n, eps, grid, faul
         v = chains[f]["kl_rows"][rows]
         fits(np.abs(v).sum(), quantum(v) if v.size else 1.0, "KL partial")
         kl[f, s] = v.sum()
-    return dict(user_emb=user, emb=round_tf32(f32(user)), emb16=r16(user, fmt), kl_part=kl, chains=chains)
+    return dict(user_emb=user, emb=round_tf32(f32(user)).astype(np.float64), emb16=r16(user, fmt), kl_part=kl, chains=chains)
 
 
 def backward(img_all, chains, fdims, nfreq, act, alpha, fmt, n, eps, g, beta, inv_batch, S, grid, lay, fault=None):
@@ -371,11 +353,6 @@ def partial_table(parts, lay, split_stride, nslots, sentinel):
 
 
 # ---- generators -------------------------------------------------------------------------------------------------------------
-def sparse_dyadic(rng, shape, k=4, den=4, density=0.25):
-    v = dyadic(rng, shape, k, den)
-    return np.where(rng.random(shape) < density, v, 0.0)
-
-
 def exact_params(rng, fdims, nfreq, logvar_offset, density=1 / 16):
     """Encoder parameters with lv = 0 on coarse grids, so that every sum fits 24 bits over thousands of rows: weights in
     {-1, 0, 1} (W1 and W2 sparse), biases on the grid 1/2; W2's logvar columns 0 and b2's logvar half -fl32(logvar_offset)."""
@@ -522,7 +499,7 @@ def bounded_forward(img_all, x, x_off, fdims, nfreq, act, alpha, fmt, n, eps, gr
         rows = np.concatenate([np.arange(t * TM, (t + 1) * TM) for t in ts])
         ch = chains[f]
         kl[f, s] = ch["kl"][rows].sum()
-        kl_b[f, s] = ch["kl_e"][rows].sum() + ER.gamma(len(rows) * E // 16 + 16) * ch["kl_abs"][rows].sum()
+        kl_b[f, s] = ch["kl_e"][rows].sum() + gamma(len(rows) * E // 16 + 16) * ch["kl_abs"][rows].sum()
     exact = user_b == 0
     return dict(user_emb=user, user_emb_bound=C_BOUND * user_b,
                 emb=np.where(exact, round_tf32(f32(user)), user), emb_bound=C_BOUND * (user_b + 2.0 ** -11 * np.abs(user)) * ~exact,

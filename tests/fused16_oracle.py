@@ -40,35 +40,7 @@ import math
 import numpy as np
 
 from oracle import dib_oracle as O
-
-# significand bits t (incl. the implicit one), minimum normal exponent, largest finite value
-FORMATS = {
-    "fp16": (11, -14, 65504.0),
-    "bf16": (8, -126, (2.0 - 2.0 ** -7) * 2.0 ** 127),
-}
-
-
-def round_to(x, fmt, saturate=True):
-    """Round half to even to the 16-bit format ``fmt`` ('fp16' | 'bf16' | None = no rounding), in float64.  Subnormals are
-    exact (the quantum never drops below 2^(emin - t + 1)).  ``saturate``: a result beyond the largest finite value becomes
-    +-max (cvt.rn.satfinite; infinities too), else +-inf (cvt.rn / __float2half_rn).  NaN stays NaN."""
-    x = np.asarray(x, dtype=np.float64)
-    if fmt is None:
-        return x
-    t, emin, vmax = FORMATS[fmt]
-    finite = np.isfinite(x)
-    xf = np.where(finite, x, 0.0)
-    _, ex = np.frexp(xf)                                    # |x| = m 2^ex, m in [0.5, 1): leading bit 2^(ex - 1)
-    e = np.maximum(ex - 1, emin)
-    q = np.ldexp(1.0, e - (t - 1))                          # the quantum (ulp) at that exponent
-    r = np.round(xf / q) * q                                # x / q is exact (power-of-two scaling); np.round: half to even
-    if saturate:
-        r = np.clip(r, -vmax, vmax)
-        r = np.where(np.isinf(x), np.sign(x) * vmax, r)
-    else:
-        r = np.where(np.abs(r) > vmax, np.copysign(np.inf, r), r)
-        r = np.where(np.isinf(x), x, r)
-    return np.where(np.isnan(x), np.nan, r)
+from tests.fp_exact import round_to
 
 
 def loss_scale(global_batch):

@@ -55,15 +55,11 @@ import math
 
 import numpy as np
 
-U = 2.0 ** -24
-C_BOUND = 2.0
-TINY = 2.0 ** -126
+from tests.fp_exact import C_BOUND, TINY, U, gamma, is_fp32
+
+
 L2_EPS = float(np.float32(1e-9))           # kL2Eps of the kernels: utils.py's 1e-9 in fp32
 KINDS = ("l2sq", "l2", "l1", "linf", "cosine")
-
-
-def gamma(m):
-    return m * U / (1.0 - m * U)
 
 
 def _on_exact_grid(x):
@@ -71,11 +67,7 @@ def _on_exact_grid(x):
     return bool(np.all(x * 256.0 == np.round(x * 256.0)) and np.all(np.abs(x) < 128.0))
 
 
-def _is_fp32(x):
-    return np.asarray(x, np.float32).astype(np.float64) == x
-
-
-def _pow2(t):
+def _is_pow2_float(t):
     return math.frexp(float(t))[0] == 0.5
 
 
@@ -113,7 +105,7 @@ class Pairs:
             self.cos, self.na, self.nb = cos, na, nb
         else:
             raise ValueError(kind)
-        if kind in ("l2sq", "l1", "linf") and _pow2(T) and _on_exact_grid(a) and _on_exact_grid(b):
+        if kind in ("l2sq", "l1", "linf") and _is_pow2_float(T) and _on_exact_grid(a) and _on_exact_grid(b):
             # float64 evaluates the kernel's chain exactly here: where every partial value is an fp32 value, so is the kernel's
             if kind == "l2sq":
                 part = np.cumsum(diff * diff, -1)
@@ -121,7 +113,7 @@ class Pairs:
                 part = np.cumsum(np.abs(diff), -1)
             else:
                 part = np.abs(diff)
-            exact = _is_fp32(part).all(-1) & _is_fp32(diff).all(-1) & _is_fp32(s) & ((s == 0) | (np.abs(s) >= 2.0 ** -126))
+            exact = is_fp32(part).all(-1) & is_fp32(diff).all(-1) & is_fp32(s) & ((s == 0) | (np.abs(s) >= 2.0 ** -126))
             sig = np.where(exact, 0.0, sig)
         self.s, self.sigma = s, sig
         if not want_derivative:

@@ -29,7 +29,7 @@ one operation per kernel operation, so its roundings are the kernel's:
                                                  tiles b, b + grid, ... (grid = min(tiles, SMs)) and writes [dW out (256) |
                                                  db out (1) | column sums of dg2 (256)], its loss and its accuracy.
 
-r() is ``fused16_oracle.round_to``: half to even, saturating (cvt.rn.satfinite), exact subnormals.
+r() is ``fp_exact.round_to``: half to even, saturating (cvt.rn.satfinite), exact subnormals.
 
 Inexact points carry a per-element bound instead (``*_bound`` arrays; zero where the value is exact):
   * the SFU activations of dib_act16: tanh.approx.f32 (PTX ISA: maximum relative error 2^-10.987), sigmoid
@@ -46,66 +46,13 @@ from __future__ import annotations
 import numpy as np
 
 from tests import elementwise_reference as ER
-from tests.fused16_oracle import FORMATS, round_to
+from tests.fp_exact import C_BOUND, U, act_grad, act_grad32, exact_matmul, f32, fits, gamma, quantum, r16, ulp16
 
 ACTS = ER.ACTS
-EXACT_BITS = 24
-U = ER.U
 TANH_APPROX_REL = 2.0 ** -10.987
 EX2_APPROX_REL = 2.0 ** -22
 HEAD_WARPS = 8
 F2N = 256
-
-
-# ---- grids and the 24-bit fit -------------------------------------------------------------------------------------------
-def dyadic(rng, shape, k=4, den=4):
-    """Operands on the grid i / den, |i| <= k (exact in fp16 and bf16 for den <= 2^7 and k <= 2^8)."""
-    return (rng.integers(-k, k + 1, size=shape) / den).astype(np.float64)
-
-
-def quantum(a):
-    """The smallest power of two every entry of ``a`` is a multiple of (1 for an all-zero array)."""
-    a = np.abs(np.asarray(a, np.float64)).ravel()
-    a = a[a > 0]
-    if a.size == 0:
-        return 1.0
-    m, e = np.frexp(a)                                                  # a = m 2^e, m in [0.5, 1)
-    mi = (m * 2.0 ** 53).astype(np.int64)                               # an integer: a = mi 2^(e - 53)
-    low = np.frexp((mi & -mi).astype(np.float64))[1] - 1               # its lowest set bit
-    return float(np.ldexp(1.0, int((e - 53 + low).min())))
-
-
-def fits(term_abs_sum, unit, what):
-    """Every value a kernel forms from terms whose magnitudes sum to ``term_abs_sum`` is an integer multiple of ``unit``
-    below 2^24 units: exact in fp32 in any order."""
-    m = float(np.max(np.asarray(term_abs_sum, np.float64), initial=0.0)) / unit
-    assert m < 2.0 ** EXACT_BITS, f"{what}: {m:.4g} units need more than {EXACT_BITS} bits"
-
-
-def exact_matmul(a, b, what):
-    """a @ b in float64, asserting that fp32 forms it exactly in any order."""
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    fits(np.abs(a) @ np.abs(b), quantum(a) * quantum(b), what)
-    return a @ b
-
-
-def r16(x, fmt):
-    return round_to(x, fmt)
-
-
-def ulp16(x, fmt):
-    """The 16-bit ulp at |x| (the quantum of round_to)."""
-    t, emin, _ = FORMATS[fmt]
-    _, ex = np.frexp(np.abs(np.asarray(x, np.float64)))
-    return np.ldexp(1.0, np.maximum(ex - 1, emin) - (t - 1))
-
-
-def f32(x):
-    return np.asarray(x, np.float64).astype(np.float32)
-
-
-def gamma(m):
-    return ER.gamma(m)
 
 
 # ---- activations --------------------------------------------------------------------------------------------------------
@@ -133,23 +80,6 @@ def act16(act, z32, alpha, fmt):
     else:
         raise ValueError(act)
     return v, e + ulp16(np.abs(v) + e, fmt)
-
-
-def act_grad32(act, h, alpha):
-    """dib_act_grad from the 16-bit output h, in fp32 (float32 array) as the kernels form it."""
-    h = f32(h)
-    one = np.float32(1)
-    if act == "relu":
-        return (h > 0).astype(np.float32)
-    if act == "tanh":
-        return one - h * h
-    if act == "leaky_relu":
-        return np.where(h > 0, one, np.float32(alpha)).astype(np.float32)
-    if act == "sigmoid":
-        return h * (one - h)
-    if act == "elu":
-        return np.where(h > 0, one, h + one).astype(np.float32)
-    return np.ones_like(h)
 
 
 # ---- GEMM ---------------------------------------------------------------------------------------------------------------
@@ -243,7 +173,7 @@ def _loss_rows(loss, out_act, alpha, z, zb, y, ib, w, exact):
         else:
             curv = 2.0 * np.ones_like(z)
         wv = np.ones(n) if w is None else np.asarray(w, np.float64)
-        r["dz_bound"] = r["dz_bound"] + ER.C_BOUND * curv * zb / C * (ib * wv)[:, None]
+        r["dz_bound"] = r["dz_bound"] + C_BOUND * curv * zb / C * (ib * wv)[:, None]
     return r
 
 
@@ -270,7 +200,7 @@ def head(g, Wc, bc, out_act, hid_act, alpha, loss, y, ib, S, w=None, nblocks=1, 
             zb = z * (1 - z) * e_logit + 7 * U * z
         else:
             raise ValueError("the bounded head takes a linear or sigmoid output")
-        zb = ER.C_BOUND * zb
+        zb = C_BOUND * zb
     res = dict(z=z, z_bound=zb)
     blk = head_block_of_rows(n, nblocks, out, head1)
     if y is None:
@@ -408,7 +338,7 @@ def fwd2_sfu(a, W0, b0, W1, b1, wout, bout, act, alpha, y, ib, S, sms, fmt, kern
     output gets one 16-bit ulp on top."""
     assert act in ("tanh", "sigmoid", "elu")
     a, W0, W1, wout = (np.asarray(v, np.float64) for v in (a, W0, W1, wout))
-    M, C = a.shape[0], ER.C_BOUND
+    M, C = a.shape[0], C_BOUND
     ulp = lambda v, e: e + ulp16(np.abs(v) + e, fmt)
     g1, g1_b = act16(act, f32(exact_matmul(a, W0, "D0")) + f32(b0)[None, :], alpha, fmt)        # e0 :464
     g1k = np.asarray(kern["g1"], np.float64)
@@ -461,7 +391,7 @@ def fwd2_sfu(a, W0, b0, W1, b1, wout, bout, act, alpha, y, ib, S, sms, fmt, kern
     dg2k = np.asarray(kern["dg2"], np.float64)
     acc2 = dg2k @ W1.T                                                                            # D1 :574
     e_acc2 = tc_gamma(F2N) * (np.abs(dg2k) @ np.abs(W1.T))
-    a1, e_a1 = ER.act_grad(act, np.asarray(kern["g1"], np.float64), alpha)
+    a1, e_a1 = act_grad(act, np.asarray(kern["g1"], np.float64), alpha)
     v1 = acc2 * a1                                                                                # e2 :585
     e_v1 = np.abs(a1) * e_acc2 + np.abs(acc2) * e_a1 + U * np.abs(v1)
     res["dg1"], res["dg1_bound"] = r16(v1, fmt), ulp(v1, C * e_v1)

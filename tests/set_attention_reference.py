@@ -68,7 +68,7 @@ LayerNorm (ln_fwd_kernel / ln_bwd_kernel; one warp per row, 4 columns per lane),
 Pooling (pool_fwd_kernel / pool_varlen_fwd_kernel): acc += x over the l rows, then acc / l:
       gamma_l sum_p |x_p| / l + u |out|;  exactly 0 where every partial sum is an fp32 value and l is a power of two.
 
-round_out is cvt.rna.tf32.f32 applied to an output: round_tf32 (the grouped-GEMM tests' restatement, imported, not copied).
+round_out is cvt.rna.tf32.f32 applied to an output: fp_exact.round_tf32.
 Every function returns float64 arrays.  The product path never imports this."""
 from __future__ import annotations
 
@@ -76,26 +76,15 @@ import math
 
 import numpy as np
 
-from tests.test_gpu_grouped_gemm import round_tf32  # noqa: F401  (re-exported: the rna rounding of round_out)
+from tests.fp_exact import C_BOUND, TINY, U, act_grad, gamma, is_fp32
 
-U = 2.0 ** -24
-C_BOUND = 2.0
-TINY = 2.0 ** -126
+
 ACTS = ("linear", "relu", "tanh", "leaky_relu", "sigmoid", "elu")
-
-
-def gamma(m):
-    m = np.asarray(m, np.float64)
-    return m * U / (1.0 - m * U)
 
 
 def scale32(dk):
     """fl(1 / sqrtf(dk)), the kernels' fp32 scale"""
     return np.float32(1.0) / np.sqrt(np.float32(dk))
-
-
-def _is_fp32(x):
-    return np.asarray(x, np.float64).astype(np.float32).astype(np.float64) == x
 
 
 def _on_grid(x):
@@ -104,7 +93,7 @@ def _on_grid(x):
     return bool(np.all(x * 4096.0 == np.round(x * 4096.0)) and np.all(np.abs(x) < 256.0))
 
 
-def _pow2(n):
+def _is_pow2_int(n):
     return (np.asarray(n) & (np.asarray(n) - 1)) == 0
 
 
@@ -146,7 +135,7 @@ def scores(qs, k, sizes=None):
         exact = np.ones(s.shape, bool)
         for d in range(dk):
             part = part + qs[..., :, None, d] * k[..., None, :, d]
-            exact &= _is_fp32(part)
+            exact &= is_fp32(part)
         sig = np.where(exact, 0.0, sig)
     _, _, kreal = _sizes(sizes, S, L)
     return np.where(kreal, s, -np.inf), np.where(kreal, sig, 0.0)
@@ -253,22 +242,6 @@ def layer_norm_forward(a, b, gamma_, beta, eps):
                 rstd_bound=C_BOUND * e_r[:, 0])
 
 
-def act_grad(act, h, alpha):
-    """dib_act_grad in float64 from the output h, and the error of its fp32 evaluation"""
-    h = np.asarray(h, np.float64)
-    if act == "relu":
-        return (h > 0).astype(np.float64), np.zeros_like(h)
-    if act == "tanh":
-        return 1.0 - h * h, U * h * h + U * np.abs(1.0 - h * h)
-    if act == "leaky_relu":
-        return np.where(h > 0, 1.0, float(np.float32(alpha))), np.zeros_like(h)
-    if act == "sigmoid":
-        return h * (1.0 - h), 2 * U * np.abs(h * (1.0 - h))
-    if act == "elu":
-        return np.where(h > 0, 1.0, h + 1.0), np.where(h > 0, 0.0, U * np.abs(h + 1.0))
-    return np.ones_like(h), np.zeros_like(h)
-
-
 def pooled_dy(dy_pool, rows, pool_rows, sizes=None, divide_by_lmax=False):
     """the pooled source of every row [rows, E]: dy_pool[r / pool_rows] fl(1 / pool_rows), or fl(1 / l_s) on the real rows
     (divide_by_lmax: the host mutation check's wrong divisor)"""
@@ -338,7 +311,7 @@ def pool(x, L, sizes=None):
     xr = np.where(real, xs, 0.0)
     out = xr.sum(1) / l[:, None]
     part = np.cumsum(xr, 1)
-    exact = _is_fp32(part).all(1) & _pow2(l)[:, None] & ((out == 0) | (np.abs(out) >= 2.0 ** -126))
+    exact = is_fp32(part).all(1) & _is_pow2_int(l)[:, None] & ((out == 0) | (np.abs(out) >= 2.0 ** -126))
     b = gamma(l)[:, None] * np.abs(xr).sum(1) / l[:, None] + U * np.abs(out)
     return out, C_BOUND * np.where(exact, 0.0, b)
 

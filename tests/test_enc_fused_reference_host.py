@@ -7,7 +7,7 @@ import pytest
 from oracle import dib_oracle as O
 from tests import enc_fused_reference as R
 from tests import fused16_oracle as Q
-from tests.int16_reference import dyadic
+from tests.fp_exact import dyadic
 
 
 def _case(fmt, fdims=(1, 2, 3), nfreq=1, act="relu", n=300, grid=5, seed=0, logvar_offset=-3.0, fault=None, density=1 / 16):

@@ -10,13 +10,14 @@ import torch
 
 from oracle import dib_oracle as O
 from tests import fused16_oracle as Q
+from tests.fp_exact import FORMATS
 
 MAX = {"fp16": 65504.0, "bf16": float(torch.finfo(torch.bfloat16).max)}
 TORCH = {"fp16": torch.float16, "bf16": torch.bfloat16}
 
 
 def _edge_values(fmt):
-    t, emin, vmax = Q.FORMATS[fmt]
+    t, emin, vmax = FORMATS[fmt]
     sub = 2.0 ** (emin - t + 1)                                  # smallest subnormal
     ulp1 = 2.0 ** (1 - t)                                        # quantum at 1
     v = [0.0, 1.0, 1.0 + ulp1 / 2, 1.0 + 1.5 * ulp1, 1.0 + ulp1 / 2 + 2.0 ** -23,      # ties to even, and just past a tie
@@ -39,7 +40,7 @@ def test_round_to_matches_torch_conversion(fmt):
     np.testing.assert_array_equal(sat, np.clip(want, -MAX[fmt], MAX[fmt]))
     # NaN stays NaN in both variants; ties round to even
     assert np.isnan(Q.round_to(np.array([np.nan]), fmt)).all() and np.isnan(Q.round_to(np.array([np.nan]), fmt, False)).all()
-    t = Q.FORMATS[fmt][0]
+    t = FORMATS[fmt][0]
     assert Q.round_to(np.array([1.0 + 2.0 ** -t]), fmt)[0] == 1.0
     assert Q.round_to(np.array([1.0 + 3 * 2.0 ** -t]), fmt)[0] == 1.0 + 2.0 ** (2 - t)
 
@@ -121,7 +122,7 @@ def test_rounded_oracle_departs_by_the_format_order(fmt, lo, hi):
     g, fr = Q.train_grads(cfg, p, x, y, eps, 0.01, O.LOSS_BCE_LOGITS, fmt=fmt)
     med = float(np.median(Q.per_variable_errors(cfg, g, g_ref)))
     assert lo < med < hi, med
-    unit = 2.0 ** -Q.FORMATS[fmt][0]
+    unit = 2.0 ** -FORMATS[fmt][0]
     e = np.abs(fr.pred - fr_ref.pred).max() / np.abs(fr_ref.pred).max()
     assert unit / 50 < e < 50 * unit, e
     # emb16 is the rounded embedding, the returned emb is not

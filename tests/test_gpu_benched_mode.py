@@ -12,7 +12,6 @@ Tolerances (stated here, asserted below):
     2e-4 in the fp32 mode, 5e-3 on the weights / 2e-3 on the history in the fp16 mode.
 """
 import os
-import socket
 import subprocess
 import sys
 
@@ -22,21 +21,10 @@ import torch
 
 from oracle import dib_oracle as O
 from oracle import philox
-from tests.test_gpu_parity import build_model, rel_err
+from tests.gpu_cases import _c0, _c0_batch, _fit_case, _free_port, build_model, rel_err
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _c0():
-    return O.DIBConfig([1] * 16, [128, 128], [256, 256], 1)
-
-
-def _c0_batch(B, seed=0):
-    rng = np.random.default_rng(seed)
-    x = rng.standard_normal((B, 16)).astype(np.float32)
-    y = (x[:, 0] * x[:, 1] + np.sin(2 * x[:, 2]) + 0.5 * x[:, 3] > 0).astype(np.float32)[:, None]
-    return x, y
 
 
 def _per_variable(cfg, g, g_ref):
@@ -85,14 +73,6 @@ def test_fp16_mode_full_metric_batch_matches_fp32_path(beta):
     gb, sb = m.compute_gradients(x[h:], y[h:], global_batch=B, sample_offset=h, step=3)
     assert rel_err((ga + gb).cpu().numpy(), g16) < 2e-4
     np.testing.assert_allclose((sa + sb).cpu().numpy(), out["fp16"][1], rtol=1e-5)
-
-
-def _fit_case():
-    """Boolean circuit (data.py:40; SURVEY 8d C1) on a fused-path-eligible model: 10 features, encoders [128,128],
-    E=32, integration [256], 4 epochs x 8 steps, beta annealed 1e-3 -> 1e-1 after one pre-training epoch."""
-    x, y = O.boolean_circuit_truth_table()
-    cfg = O.DIBConfig([1] * 10, [128, 128], [256], 1)
-    return x, y, cfg
 
 
 def test_fp16_mode_fit_trajectory_matches_oracle():
@@ -170,14 +150,6 @@ def test_fp16_mode_range_edges():
     assert rel_err(out["tf32"][0], out["fp32"][0]) < 2e-2
     assert rel_err(out["bf16"][0], out["fp32"][0]) < 1.6e-1
     assert rel_err(out["fp16"][0], out["fp32"][0]) > 5e-2                        # clamped at 65 504: visibly different, by design
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    port = s.getsockname()[1]
-    s.close()
-    return port
 
 
 _WORKER = r"""
@@ -263,8 +235,6 @@ def test_fp16_mode_batch_split_boundaries():
     ceil(n / 32) is an odd multiple of 32 (20 557 -> 672-row slices before the fix) double-counted the 32 rows after every slice
     boundary in the integration network's weight gradients.  fp16 mode against the fp32 path, per variable."""
     import dib_b200
-    from tests.test_gpu_parity import build_model, rel_err
-    from oracle import dib_oracle as O
     cfg = O.DIBConfig([1] * 16, [128, 128], [256, 256], 1)
     rng = np.random.default_rng(77)
     p = O.glorot_uniform_params(cfg, rng)

@@ -5,16 +5,13 @@ precisions and into live CUDA graphs, load_model, the refusals, data-parallel re
 
 The interruption is a plain Python exception raised by a callback listed after BackupAndRestore, at the end of epoch k."""
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 
+from tests.gpu_cases import CFG, YARCH, YD, data, run_workers, set_transformer_model, small, varlen_set_case
 
 pytestmark = pytest.mark.gpu
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 class _Stop(Exception):
@@ -111,7 +108,6 @@ def _other_model(kind):
         x, y = _c0_data(512)
         return (lambda: _c0_model("fp16", optimizer=opt())), dict(x=x, y=y, batch_size=128, validation_data=(x[:128], y[:128]))
     if kind == "infonce":
-        from tests.test_gpu_infonce import CFG, YARCH, YD, data
         x, y, _ = data(768, 12)
 
         def build():
@@ -121,13 +117,12 @@ def _other_model(kind):
                                                                                   temperature=0.5))
             return m
         return build, dict(x=x[:512], y=y[:512], batch_size=128, validation_data=(x[512:], y[512:]))
-    from tests.test_gpu_set_transformer_variable_sizes import case, make_model, small
     variable = kind == "set_variable"
     cfg = small(12)
     sizes = np.random.default_rng(4).integers(1, 13, 96).astype(np.int32)
-    _, xs, ys, _, sizes = case(cfg, sizes, 7)
+    _, xs, ys, _, sizes = varlen_set_case(cfg, sizes, 7)
     xin = (xs, sizes) if variable else xs
-    return (lambda: make_model(cfg, seed=2, variable=variable, metrics=["accuracy"])), dict(x=xin, y=ys, batch_size=32)
+    return (lambda: set_transformer_model(cfg, seed=2, variable=variable, metrics=["accuracy"])), dict(x=xin, y=ys, batch_size=32)
 
 
 @pytest.mark.parametrize("kind", ["sgd_nesterov", "rmsprop", "infonce", "set_fixed", "set_variable"])
@@ -285,7 +280,6 @@ def test_load_model_restores_configuration_and_counters(tmp_path):
 def test_refused_restores_change_nothing(tmp_path):
     import dib_b200
     from dib_b200 import checkpoint
-    from tests.test_gpu_infonce import CFG, YARCH, YD, data
     x, y = _c0_data(512)
     src = _c0_model("fp32", seed=1)
     src.fit(x, y, epochs=1, batch_size=128, verbose=False)
@@ -334,7 +328,7 @@ import numpy as np, torch, torch.distributed as dist
 sys.path.insert(0, os.environ["DIB_ROOT"])
 import dib_b200
 from dib_b200 import checkpoint
-from tests.test_gpu_benched_mode import _fit_case
+from tests.gpu_cases import _fit_case
 rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
 torch.cuda.set_device(0)
 if world > 1:
@@ -379,23 +373,7 @@ if world > 1:
 
 
 def _run_workers(tmp_path, name, world, backup, stop_at=-1):
-    from tests.test_gpu_infonce_data_parallel import _free_port
-    script = tmp_path / "worker.py"
-    script.write_text(_WORKER)
-    out = str(tmp_path / f"{name}.npz")
-    env = dict(os.environ, DIB_ROOT=ROOT, DIB_OUT=out, DIB_BACKUP=backup, DIB_STOP=str(stop_at), MASTER_ADDR="127.0.0.1",
-               MASTER_PORT=str(_free_port()), WORLD_SIZE=str(world), PYTHONPATH=ROOT)
-    procs = [subprocess.Popen([sys.executable, str(script)], env=dict(env, RANK=str(r), LOCAL_RANK=str(r)), cwd=ROOT)
-             for r in range(world)]
-    try:
-        codes = [pr.wait(timeout=600) for pr in procs]
-    finally:
-        for pr in procs:
-            if pr.poll() is None:
-                pr.kill()
-                pr.wait()
-    assert codes == [0] * world, codes
-    return dict(np.load(out))
+    return run_workers(tmp_path, _WORKER, world, str(tmp_path / f"{name}.npz"), DIB_BACKUP=backup, DIB_STOP=str(stop_at))
 
 
 def _hist(r):

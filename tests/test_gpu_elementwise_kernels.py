@@ -4,48 +4,20 @@ the positional encoding, dropout and the fixed-order reductions, through the tes
 dib_debug_pe / dib_debug_dropout / dib_debug_reduce, which launch them as the training step does.  Every call also checks the
 memory contracts: NaN in every input element a kernel must not read, a sentinel in every output element it must not write,
 and the launch count."""
-import ctypes
-
 import numpy as np
 import pytest
 import torch
 
 from oracle import philox
 from tests import elementwise_reference as R
+from tests.fp_exact import within_same_nans
+from tests.gpu_cases import _dev, _lib, _st
 
 pytestmark = pytest.mark.gpu
 
 SENTINEL = np.float32(-3.0e33)
 WORST = {}
 ACT = {a: i for i, a in enumerate(R.ACTS)}
-
-
-def _lib():
-    from dib_b200 import _lib as L
-    return L, L.load()
-
-
-def _dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
-def _st():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def within(what, got, ref, bound, tag):
-    got, ref, bound = np.asarray(got, np.float64), np.asarray(ref, np.float64), np.asarray(bound, np.float64)
-    nan = np.isnan(ref)
-    assert np.array_equal(np.isnan(got), nan), f"{tag} {what}: NaN where the reference has none, or the reverse"
-    got, ref, bound = got[~nan], ref[~nan], bound[~nan]
-    err = np.abs(got - ref)
-    bad = ~(err <= bound)
-    assert not bad.any(), (f"{tag} {what}: {bad.sum()} of {bad.size} elements outside their bound; first at "
-                           f"{np.argwhere(bad)[0].tolist()}: got {got[bad][0]!r} ref {ref[bad][0]!r} bound {bound[bad][0]!r}")
-    pos = bound > 0
-    ratio = float((err[pos] / bound[pos]).max()) if pos.any() else 0.0
-    WORST[what] = max(WORST.get(what, 0.0), ratio)
-    print(f"{tag} {what}: worst measured / bound {ratio:.3g}; exact elements {int((~pos).sum())}")
 
 
 def _launches(lib):
@@ -87,9 +59,9 @@ def check_loss(kind, act, z, y, inv_batch, tag, w=None, alpha=0.2):
     z = np.asarray(z, np.float32)
     out = run_loss(kind, act, z, y, inv_batch, w, alpha)
     ref = R.loss(kind, act, alpha, z, y, np.float32(inv_batch), w)
-    within(f"{kind} dz", out["dz"], ref["dz"], ref["dz_bound"], tag)
-    within(f"{kind} loss_part", out["loss_part"], ref["loss_part"], ref["loss_part_bound"], tag)
-    within(f"{kind} acc_part", out["acc_part"], ref["acc_part"], ref["acc_part_bound"], tag)
+    within_same_nans(WORST, f"{kind} dz", out["dz"], ref["dz"], ref["dz_bound"], tag)
+    within_same_nans(WORST, f"{kind} loss_part", out["loss_part"], ref["loss_part"], ref["loss_part_bound"], tag)
+    within_same_nans(WORST, f"{kind} acc_part", out["acc_part"], ref["acc_part"], ref["acc_part_bound"], tag)
     return out, ref
 
 
@@ -239,17 +211,17 @@ def check_reparam(mu, lv, tag, eps=None, philox_key=None, sizes=None, set_len=1,
     out = run_reparam(mu, lv, eps, sizes=sizes, set_len=set_len, du=du, beta=beta, inv_batch=inv_batch, round_out=round_out, **kw)
     real = out["real"] if sizes is not None else None
     f = R.reparam_forward(mu, lv, z, ztol, real)
-    within("reparam user_emb", out["user_emb"], f["u"], f["u_bound"], tag)
+    within_same_nans(WORST, "reparam user_emb", out["user_emb"], f["u"], f["u_bound"], tag)
     eb = f["u_bound"] + (R.TF32_HALF_ULP * (np.abs(f["u"]) + f["u_bound"]) if round_out else 0)
-    within("reparam emb", out["emb"], f["u"], eb, tag)
-    within("reparam kl_part", out["kl_part"], f["kl_part"], f["kl_part_bound"], tag)
+    within_same_nans(WORST, "reparam emb", out["emb"], f["u"], eb, tag)
+    within_same_nans(WORST, "reparam kl_part", out["kl_part"], f["kl_part"], f["kl_part_bound"], tag)
     if real is not None:
         assert np.all(out["user_emb"][:, ~real] == 0) and np.all(out["emb"][:, ~real] == 0)
     if du is not None:
         b = R.reparam_backward(mu, lv, z, du, beta, inv_batch, ztol, real)
         rb = (lambda r, bd: bd + (R.TF32_HALF_ULP * (np.abs(r) + bd) if round_out else 0))
-        within("reparam dmu", out["dmu"], b["dmu"], rb(b["dmu"], b["dmu_bound"]), tag)
-        within("reparam dlv", out["dlv"], b["dlv"], rb(b["dlv"], b["dlv_bound"]), tag)
+        within_same_nans(WORST, "reparam dmu", out["dmu"], b["dmu"], rb(b["dmu"], b["dmu_bound"]), tag)
+        within_same_nans(WORST, "reparam dlv", out["dlv"], b["dlv"], rb(b["dlv"], b["dlv_bound"]), tag)
     return out
 
 
@@ -274,7 +246,7 @@ def test_philox_noise_against_normal_noise():
     zero = np.zeros((F, n, E), np.float32)
     out = run_reparam(zero, zero, seed=7, step=3, step_dev=2, sample_offset=2 ** 32 + 5)
     z = np.transpose(philox.normal_noise(7, 5, 2 ** 32 + 5 + np.arange(n, dtype=np.uint64), F, E, dtype=np.float64), (1, 0, 2))
-    within("philox noise", out["user_emb"], z, R.Z_TOL * (1.0 + np.abs(z)), "philox")
+    within_same_nans(WORST, "philox noise", out["user_emb"], z, R.Z_TOL * (1.0 + np.abs(z)), "philox")
 
 
 @pytest.mark.parametrize("s", [1e-4, 1e-3])
@@ -334,7 +306,7 @@ def test_pe_columns_frequencies_and_row_clamp(gather):
     o = out.cpu().numpy()
     assert np.all(o[n:] == SENTINEL) and np.all(o[:, col_end - shift:] == SENTINEL)
     ref, b = R.pe(x, col_src, col_freq, col_begin, col_end, 0, row_index, col_feat, n_src, n)
-    within("pe", o[:n, :col_end - shift], ref, b, f"pe gather={gather}")
+    within_same_nans(WORST, "pe", o[:n, :col_end - shift], ref, b, f"pe gather={gather}")
     assert np.all(o[:n, col_end - shift - 2:col_end - shift] == 0)            # col_src = -1 columns
 
 
@@ -475,7 +447,7 @@ def test_positional_encoding_entry_point(nfreq):
     o = out.cpu().numpy()
     assert np.all(o[n * d * nfreq:] == SENTINEL)
     ref, b = R.pe_plain(x, nfreq)
-    within("pe_plain", o[:n * d * nfreq].reshape(n, d * nfreq), ref, b, f"pe_plain nfreq={nfreq}")
+    within_same_nans(WORST, "pe_plain", o[:n * d * nfreq].reshape(n, d * nfreq), ref, b, f"pe_plain nfreq={nfreq}")
 
 
 def _opt_case(rng, count):
@@ -511,9 +483,9 @@ def test_adam_entry_point(count):
         assert int(step.cpu()[0]) == t
         ref = R.adam(mw[:count], g[:count], mm[:count], mv[:count], 1e-3, t, b1, b2, eps)
         gw, gm, gv = (a.cpu().numpy() for a in (W, M, V))
-        within("adam w", gw[:count], ref["w"], ref["w_bound"], f"adam count={count} t={t}")
-        within("adam m", gm[:count], ref["m"], ref["m_bound"], f"adam count={count} t={t}")
-        within("adam v", gv[:count], ref["v"], ref["v_bound"], f"adam count={count} t={t}")
+        within_same_nans(WORST, "adam w", gw[:count], ref["w"], ref["w_bound"], f"adam count={count} t={t}")
+        within_same_nans(WORST, "adam m", gm[:count], ref["m"], ref["m_bound"], f"adam count={count} t={t}")
+        within_same_nans(WORST, "adam v", gv[:count], ref["v"], ref["v_bound"], f"adam count={count} t={t}")
         np.testing.assert_array_equal(gw[count:], w[count:])            # nothing past count
         mw, mm, mv = (np.concatenate([a[:count].astype(np.float64), b[count:]]) for a, b in ((gw, w), (gm, z), (gv, z)))
 
@@ -540,13 +512,13 @@ def test_sgd_and_rmsprop_entry_point(count, kind, hyper):
     tag = f"kind={kind} hyper={hyper} count={count}"
     if kind == 0:
         ref = R.sgd(w[:count], g[:count], s1[:count], 1e-2, hyper[0], hyper[1] != 0)
-        within("sgd w", gw[:count], ref["w"], ref["w_bound"], tag)
-        within("sgd v", g1[:count], ref["v"], ref["v_bound"], tag)
+        within_same_nans(WORST, "sgd w", gw[:count], ref["w"], ref["w_bound"], tag)
+        within_same_nans(WORST, "sgd v", g1[:count], ref["v"], ref["v_bound"], tag)
     else:
         ref = R.rmsprop(w[:count], g[:count], s1[:count], s2[:count], 1e-2, *hyper)
-        within("rmsprop w", gw[:count], ref["w"], ref["w_bound"], tag)
-        within("rmsprop ms", g1[:count], ref["ms"], ref["ms_bound"], tag)
-        within("rmsprop mom", g2[:count], ref["mom"], ref["mom_bound"], tag)
+        within_same_nans(WORST, "rmsprop w", gw[:count], ref["w"], ref["w_bound"], tag)
+        within_same_nans(WORST, "rmsprop ms", g1[:count], ref["ms"], ref["ms_bound"], tag)
+        within_same_nans(WORST, "rmsprop mom", g2[:count], ref["mom"], ref["mom_bound"], tag)
     for got, orig in ((gw, w), (g1, s1), (g2, s2)):
         np.testing.assert_array_equal(got[count:], orig[count:])
 
@@ -574,8 +546,8 @@ def test_pairwise_gaussian_entry_point(kind, E):
     assert np.all(o[n * m:] == SENTINEL) and np.all(c[n * m:] == SENTINEL)
     ref = R.pairwise_gaussian(kind, ml1, ml2)
     tag = f"pairwise kind={kind} E={E}"
-    within(f"pairwise{kind} D", o[:n * m].reshape(n, m), ref["D"], ref["D_bound"], tag)
-    within(f"pairwise{kind} exp(-D)", c[:n * m].reshape(n, m), ref["comp"], ref["comp_bound"], tag)
+    within_same_nans(WORST, f"pairwise{kind} D", o[:n * m].reshape(n, m), ref["D"], ref["D_bound"], tag)
+    within_same_nans(WORST, f"pairwise{kind} exp(-D)", c[:n * m].reshape(n, m), ref["comp"], ref["comp_bound"], tag)
 
 
 def test_hooks_reject_bad_arguments():

@@ -16,7 +16,7 @@ import pytest
 
 from oracle import philox
 from tests import fused16_oracle as Q
-from tests.test_gpu_fused16_vs_rounding_oracle import FUSED, TOL, _c, _check, _data, _model, _params, _sms, _stats_err
+from tests.gpu_cases import FUSED, TOL, _c, _check, _data, _model, _params, _sms, _stats_err
 
 pytestmark = pytest.mark.gpu
 

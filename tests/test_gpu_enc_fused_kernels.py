@@ -23,7 +23,8 @@ import torch
 
 from tests import enc_fused_reference as R
 from tests.fused16_oracle import loss_scale
-from tests.int16_reference import dyadic, ulp16
+from tests.fp_exact import dyadic, from16, r16, to16, ulp16
+from tests.gpu_cases import _L, _sms
 
 pytestmark = pytest.mark.gpu
 
@@ -33,34 +34,6 @@ NAN16 = {"fp16": 0x7E00, "bf16": 0x7FC0}
 SENT16 = np.int16(-8531)                 # 0xDEAD: finite in both formats, never a result here
 SENT32 = np.float32(-7777.25)
 WORST = {}
-
-
-def _L():
-    from dib_b200 import _lib as L
-    return L
-
-
-def _sms():
-    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
-
-
-def to16(v, fmt):
-    v = np.asarray(v, np.float64)
-    if fmt == "fp16":
-        h = v.astype(np.float16)
-        assert np.array_equal(h.astype(np.float64), v, equal_nan=True), "value not representable in fp16"
-        return h.view(np.int16)
-    f = v.astype(np.float32)
-    u = f.view(np.uint32)
-    assert np.array_equal(f.astype(np.float64), v, equal_nan=True) and not np.any(u & 0xFFFF), "value not representable in bf16"
-    return (u >> 16).astype(np.uint16).view(np.int16)
-
-
-def from16(b, fmt):
-    b = np.asarray(b).view(np.int16)
-    if fmt == "fp16":
-        return b.view(np.float16).astype(np.float64)
-    return (b.view(np.uint16).astype(np.uint32) << 16).view(np.float32).astype(np.float64)
 
 
 def dev(a):
@@ -350,7 +323,7 @@ def test_pe_operand_exact_where_the_sine_is_far_from_a_midpoint(fmt, act):
         xs = xs[R.pe_exact(xs, d, nfreq, fmt)][:n]
         assert len(xs) == n
         for got, s in pe_readout(fmt, act, (d,), nfreq, [xs], n):
-            same(got, R.r16(s, fmt), f"{fmt} {act} pe operand d={d} nfreq={nfreq}", bits=bits16(fmt))
+            same(got, r16(s, fmt), f"{fmt} {act} pe operand d={d} nfreq={nfreq}", bits=bits16(fmt))
 
 
 @pytest.mark.parametrize("fmt", FMTS)
@@ -363,7 +336,7 @@ def test_pe_accuracy_at_large_arguments(fmt, layout, xmax):
     n = 2000
     xs = rng.uniform(-xmax, xmax, (n, d)).astype(np.float32)
     (got, s), = pe_readout(fmt, "relu", (d,), nfreq, [xs], n)
-    lo, hi = R.r16(s - R.SIN_TOL, fmt), R.r16(s + R.SIN_TOL, fmt)
+    lo, hi = r16(s - R.SIN_TOL, fmt), r16(s + R.SIN_TOL, fmt)
     ok = (got >= lo) & (got <= hi)
     half = 0.5 * ulp16(s, fmt)
     ratio = np.maximum(np.abs(got - s) - half, 0.0) / R.SIN_TOL
@@ -391,7 +364,7 @@ def test_philox_noise_readout(fmt):
     WORST[f"noise {fmt}"] = float(err.max())
     print(f"noise {fmt}: worst |u - z| / (Z_TOL (1 + |z|)) = {err.max():.3g}")
     assert err.max() <= 1.0
-    same(from16(out["emb16"][:n, :c.F * R.E], fmt), R.r16(got.reshape(n, -1), fmt), "emb16 = r(noise)", bits=bits16(fmt))
+    same(from16(out["emb16"][:n, :c.F * R.E], fmt), r16(got.reshape(n, -1), fmt), "emb16 = r(noise)", bits=bits16(fmt))
     # step + *step_dev is the summed step, bit for bit
     out2 = run(c, 3, 0, seed=seed, step=step + sdev, sample_offset=off)
     assert np.array_equal(out2["user"].view(np.uint32), out["user"].view(np.uint32))
@@ -447,7 +420,7 @@ def test_pe_layouts_forward_and_backward(fmt, route):
 # ---------------------------------------------------------------------------------------------------------------------
 # the bounded regime: lv != 0, the SFU activations, leaky ReLU with alpha = 0.2
 # ---------------------------------------------------------------------------------------------------------------------
-def within(got, want, bound, what):
+def within_silent(got, want, bound, what):
     """|got - want| <= bound everywhere; elements with a zero bound equal the reference by value.  Records the worst
     measured / bound of the inexact elements in WORST under the output's name."""
     err = np.abs(got - want)
@@ -488,15 +461,15 @@ def test_bounded_regime(act, fmt, route, alpha, grid):
     assert np.abs(np.concatenate([ch["lv"] for ch in ref["chains"]])).max() > 1.0, "the case needs a live logvar"
     tag = f"{act} a={alpha}"
     assert np.all(out["emb"][n:] == SENT32) and np.all(out["emb16"][n:] == SENT16) and np.all(out["user"][n:] == SENT32)
-    within(out["user"][:n].astype(np.float64), ref["user_emb"], ref["user_emb_bound"], f"{tag} user_emb: {fmt} grid {grid}")
-    within(out["emb"][:n, :F * E].astype(np.float64), ref["emb"], ref["emb_bound"], f"{tag} emb: {fmt} grid {grid}")
-    within(from16(out["emb16"][:n, :F * E], fmt), ref["emb16"], ref["emb16_bound"], f"{tag} emb16: {fmt} grid {grid}")
+    within_silent(out["user"][:n].astype(np.float64), ref["user_emb"], ref["user_emb_bound"], f"{tag} user_emb: {fmt} grid {grid}")
+    within_silent(out["emb"][:n, :F * E].astype(np.float64), ref["emb"], ref["emb_bound"], f"{tag} emb: {fmt} grid {grid}")
+    within_silent(from16(out["emb16"][:n, :F * E], fmt), ref["emb16"], ref["emb16_bound"], f"{tag} emb16: {fmt} grid {grid}")
     kl, klb = np.zeros(out["kl"].shape), np.zeros(out["kl"].shape)
     kl[:, :ref["kl_part"].shape[1]], klb[:, :ref["kl_part"].shape[1]] = ref["kl_part"], ref["kl_part_bound"]
-    within(out["kl"].astype(np.float64), kl, klb, f"{tag} kl_part: {fmt} grid {grid}")
+    within_silent(out["kl"].astype(np.float64), kl, klb, f"{tag} kl_part: {fmt} grid {grid}")
     parts = R.bounded_backward(c.img, ref["chains"], c.fdims, 1, act, alpha, fmt, n, eps, g, beta, 1.0 / S, S, out["g_bwd"])
     want, bound = R.bounded_partial_table(parts, c.lay, out["split_stride"], out["slots"] + 1, float(SENT32))
-    within(out["part"].astype(np.float64), want, bound, f"{tag} partials: {fmt} grid {grid} {route}")
+    within_silent(out["part"].astype(np.float64), want, bound, f"{tag} partials: {fmt} grid {grid} {route}")
 
 
 # ---------------------------------------------------------------------------------------------------------------------

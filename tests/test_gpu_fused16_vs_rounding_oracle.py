@@ -22,127 +22,15 @@ import torch
 from oracle import dib_oracle as O
 from oracle import philox
 from tests import fused16_oracle as Q
-from tests.test_gpu_parity import rel_err
+from tests.fp_exact import ulp16
+from tests.gpu_cases import TOL, _c, _check, _data, _expect_route, _grad_case, _model, _params, _sms, _stats_err, rel_err
 
 pytestmark = pytest.mark.gpu
-
-FUSED = {"fp16": "encoders=fused-wgmma-f16 integration=int16-wgmma-f16", "bf16": "encoders=fused-wgmma-bf16 integration=int16-wgmma-bf16"}
-REPORT = []
-
-
-def _sms():
-    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
-
-
-def _model(cfg, prec, loss, mask=0, seed=0):
-    import dib_b200
-    m = dib_b200.DistributedIBNet(
-        cfg.feature_dimensionalities, cfg.feature_encoder_architecture, cfg.integration_network_architecture,
-        cfg.output_dimensionality, use_positional_encoding=cfg.use_positional_encoding,
-        number_positional_encoding_frequencies=cfg.number_positional_encoding_frequencies, activation_fn=cfg.activation_fn,
-        feature_embedding_dimension=cfg.feature_embedding_dimension, output_activation_fn=cfg.output_activation_fn,
-        precision=prec, seed=seed, leaky_alpha=cfg.leaky_alpha, logvar_offset=cfg.logvar_offset,
-        kl_loss_exponent=cfg.kl_loss_exponent)
-    m.compile(optimizer=dib_b200.Adam(1e-3), loss=loss)
-    m.debug_force_unfused(mask)
-    return m
-
-
-def _expect_route(m, prec, n, tail):
-    """kernel_info names the route the case means to test: tail in {'dgrad', 'fwd2', None (per-layer GEMMs + a head kernel)}."""
-    info = m.kernel_info(n)
-    assert FUSED[prec] in info, info
-    if tail == "dgrad":
-        assert "integration_tail=fwd2-head-dgrad" in info, info
-    elif tail == "fwd2":
-        assert "integration_tail=fwd2-head" in info and "integration_tail=fwd2-head-dgrad" not in info, info
-    else:
-        assert "integration_tail" not in info, info
-
-
-def _params(cfg, seed):
-    rng = np.random.default_rng(seed)
-    p = O.glorot_uniform_params(cfg, rng)
-    return p + (p == 0) * (0.05 * rng.standard_normal(p.size)).astype(np.float32)      # non-zero biases
-
-
-def _data(cfg, loss, n, seed):
-    rng = np.random.default_rng(seed + 1000)
-    D, F, E, out = sum(cfg.feature_dimensionalities), cfg.number_features, cfg.feature_embedding_dimension, cfg.output_dimensionality
-    x = rng.standard_normal((n, D)).astype(np.float32)
-    eps = rng.standard_normal((n, F, E)).astype(np.float32)
-    if loss == O.LOSS_SPARSE_CE_LOGITS:
-        y = rng.integers(0, out, size=n).astype(np.float32)
-    elif loss == O.LOSS_MSE:
-        y = rng.standard_normal((n, out)).astype(np.float32)
-    else:
-        y = (x[:, :1] * x[:, -1:] > 0).astype(np.float32) if out == 1 else rng.integers(0, 2, (n, out)).astype(np.float32)
-    return x, y, eps
-
-
-def _check(what, measured, bound):
-    REPORT.append((what, float(measured), bound))
-    print(f"[fused16-oracle] {what}: {measured:.3e} (bound {bound:.1e})")
-    assert measured < bound, (what, measured, bound)
-
-
-def _stats_err(st, fr, n):
-    """KL sums and the loss sum of the step's statistics row against the oracle's, relative."""
-    F = len(fr.kl_per_feature)
-    kl = np.abs(st[:F] - fr.kl_per_feature * n) / np.abs(fr.kl_per_feature * n)
-    lo = abs(st[F] - fr.cache["loss_sum"]) / abs(fr.cache["loss_sum"]) if "loss_sum" in fr.cache else 0.0
-    return max(float(kl.max()), float(lo))
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# bounds (per-variable max-norm relative unless said otherwise); measured worst values in the comments / DESIGN.md section 2
-# ---------------------------------------------------------------------------------------------------------------------
-TOL = {
-    # per variable, one step, relu / leaky_relu: bounded by relu-gate flips, not by accumulation (see the module notes);
-    # measured worst 6.3e-2 (fp16, n = 127), 2.1e-2 (fp16, n = 4173), 1.7e-2 (bf16, n = 4173)
-    ("grad", "fp16"): 0.1, ("grad", "bf16"): 0.1,
-    ("stats", "fp16"): 3e-5, ("stats", "bf16"): 3e-5,        # KL sums and loss sum; measured 8.5e-6 / 7.7e-6
-    ("pred", "fp16"): 2e-3, ("pred", "bf16"): 2e-2,          # max-norm relative prediction
-    ("emb", "fp16"): 2e-4, ("emb", "bf16"): 2e-3,            # per feature block, u vs the oracle's u; measured 5.0e-5 / 4.1e-4
-    ("flip", "fp16"): 1e-2, ("flip", "bf16"): 1e-2,          # fraction of emb16 elements that differ; measured 2.1e-3 / 2.0e-4
-    ("tanh", "fp16"): 3e-3, ("tanh", "bf16"): 1.5e-2,        # smooth act': measured 6.5e-4 / 3.5e-3 per variable
-    ("rowiso", "fp16"): 3e-3, ("rowiso", "bf16"): 1.5e-2,    # 14 isolated rows; measured 8.4e-4 / 3.3e-3
-}
-
-
-def _grad_case(cfg, prec, loss, n, beta, seed=0, mask=0, tail="dgrad", p=None, label=""):
-    p = _params(cfg, seed) if p is None else p
-    x, y, eps = _data(cfg, loss, n, seed)
-    m = _model(cfg, prec, loss, mask)
-    _expect_route(m, prec, n, tail)
-    m.set_flat_weights(p)
-    m.beta.assign(beta)
-    g, st = m.compute_gradients(x, y, eps=eps)
-    g, st = g.cpu().numpy().astype(np.float64), st.cpu().numpy().astype(np.float64)
-    assert np.isfinite(g).all() and np.isfinite(st).all()
-    g_ref, fr = Q.train_grads(cfg, p, x, y, eps, beta, loss, fmt=prec)
-    pv = Q.per_variable_errors(cfg, g, g_ref)
-    tag = f"{label} {prec} n={n} beta={beta}"
-    kind = "tanh" if cfg.activation_fn in ("tanh", "sigmoid", "elu") else "grad"      # smooth act
-    _check(f"grad/var {tag} (worst var {int(pv.argmax())})", pv.max(), TOL[(kind, prec)])
-    _check(f"stats {tag}", _stats_err(st, fr, n), TOL[("stats", prec)])
-    return pv
-
-
-def _c(F=16, integ=(256, 256), out=1, act="relu", dims=None, **kw):
-    out_act = "sigmoid" if kw.pop("probs", False) else None
-    return O.DIBConfig(list(dims or [1] * F), [128, 128], list(integ), out, activation_fn=act, output_activation_fn=out_act, **kw)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
 # a. forward, per element
 # ---------------------------------------------------------------------------------------------------------------------
-def _ulp(v, fmt):
-    t, emin, _ = Q.FORMATS[fmt]
-    _, ex = np.frexp(np.abs(v))
-    return np.ldexp(1.0, np.maximum(ex - 1, emin) - (t - 1))
-
-
 @pytest.mark.parametrize("prec", ["fp16", "bf16"])
 def test_forward_per_element(prec):
     cfg = _c(F=16, act="leaky_relu")
@@ -174,7 +62,7 @@ def test_forward_per_element(prec):
     terms = np.concatenate([np.maximum(np.abs(mu), np.abs(np.exp(lv / 2.0) * eps[:, f, :]))
                             for f, (_, _, _, mu, lv) in enumerate(fr.cache["enc"])], axis=-1)
     r_k, r_o = Q.round_to(emb, prec), Q.round_to(fr.emb, prec)
-    d_ulp = np.abs(r_k - r_o) / _ulp(np.maximum(terms, np.maximum(np.abs(r_k), np.abs(r_o))), prec)
+    d_ulp = np.abs(r_k - r_o) / ulp16(np.maximum(terms, np.maximum(np.abs(r_k), np.abs(r_o))), prec)
     print(f"[fused16-oracle] emb16 largest distance {prec}: {d_ulp.max():.1f} ulp of the larger term")
     _check(f"emb16 elements that differ {prec} (fraction)", np.mean(d_ulp > 0), TOL[("flip", prec)])
 

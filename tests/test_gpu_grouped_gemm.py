@@ -1,5 +1,6 @@
 """GPU (H100): the grouped dense-layer GEMM kernels -- dib_gemm_simt.cu (exact fp32 FMA) and dib_gemm_tc.cu (tf32 wgmma) --
-launched through dib_debug_gemm exactly as the library's steps launch them, against a float64 reference, bit for bit.
+launched through dib_debug_gemm exactly as the library's steps launch them, against the float64 reference of
+tests/grouped_gemm_reference.py, bit for bit.
 
 Exact operands: every A / B / bias entry is i / 4 with |i| <= 4 and every DGRAD activation source is k / 16 in (-1, 1).
 With reductions of at most 512 terms every product, every partial sum in any order and every o * act'(x) then fits in 24
@@ -23,135 +24,16 @@ import pytest
 import torch
 
 from oracle import dib_oracle as O
+from tests.fp_exact import dyadic, fits, round_tf32
+from tests.fused16_oracle import per_variable_errors
+from tests.gpu_cases import _L, build_model, rel_err
+from tests.grouped_gemm_reference import INEXACT_ACTS, act_source, assert_on_grid, ref_dgrad, ref_fwd, ref_wgrad, ulp32
 
 pytestmark = pytest.mark.gpu
 
 FWD, DGRAD, WGRAD = 0, 1, 2
 ACTS = {"linear": 0, "relu": 1, "tanh": 2, "leaky_relu": 3, "sigmoid": 4, "elu": 5}
-INEXACT_ACTS = ("tanh", "sigmoid", "elu")
 SENTINEL = np.float32(-7777.25)
-EXACT_BITS = 24
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# the float64 reference (plain numpy; also exercised on the CPU by test_grouped_gemm_reference_host.py)
-# ---------------------------------------------------------------------------------------------------------------------
-def round_tf32(x):
-    """cvt.rna.tf32.f32: round the fp32 value to 10 explicit mantissa bits, to nearest, ties away from zero.  On the bit
-    pattern of a finite value that is adding half of the dropped unit to the magnitude bits and clearing the low 13 bits
-    (a carry moves into the exponent); NaN and inf pass unchanged."""
-    x = np.ascontiguousarray(x, dtype=np.float32)
-    u = x.view(np.uint32)
-    r = (u + np.uint32(0x1000)) & np.uint32(0xFFFFE000)
-    return np.where(np.isfinite(x), r, u).astype(np.uint32).view(np.float32)
-
-
-def dyadic(rng, shape, k=4, den=4):
-    """Operands on the grid i / den, |i| <= k."""
-    return (rng.integers(-k, k + 1, size=shape) / den).astype(np.float32)
-
-
-def act_source(rng, shape):
-    """DGRAD activation sources k / 16 in (-1, 1), exact zeros included."""
-    return (rng.integers(-15, 16, size=shape) / 16).astype(np.float32)
-
-
-def _assert_on_grid(a, den):
-    a = np.asarray(a, np.float64)
-    assert np.array_equal(a * den, np.round(a * den)), f"operand off the 1/{den} grid"
-
-
-def _assert_fits(numerators, what):
-    """Every value a kernel forms is an integer multiple of the grid unit below this bound: exact in fp32 in any order."""
-    m = float(np.max(np.abs(numerators), initial=0.0))
-    assert m < 2.0 ** EXACT_BITS, f"{what}: {m} needs more than {EXACT_BITS} bits"
-
-
-def act_fwd32(act, z, alpha):
-    """The FWD epilogue act(z) on the exact fp32 z; leaky ReLU rounds alpha * z once in fp32.  Inexact activations are
-    returned in float64 (compared with a ulp bound)."""
-    if act == "linear":
-        return z
-    if act == "relu":
-        return np.maximum(z, 0.0)
-    if act == "leaky_relu":
-        z32 = z.astype(np.float32)
-        return np.where(z32 > 0, z32, np.float32(alpha) * z32).astype(np.float64)
-    return O.act_fwd(act, z)
-
-
-def act_grad32(act, h, alpha):
-    """act'(h) from the activation output h, in fp32 as the kernel forms it (exact for h on the 1/16 grid)."""
-    h = h.astype(np.float32)
-    one = np.float32(1)
-    if act == "relu":
-        return (h > 0).astype(np.float32)
-    if act == "tanh":
-        return one - h * h
-    if act == "leaky_relu":
-        return np.where(h > 0, one, np.float32(alpha)).astype(np.float32)
-    if act == "sigmoid":
-        return h * (one - h)
-    if act == "elu":
-        return np.where(h > 0, one, h + one).astype(np.float32)
-    raise ValueError(act)
-
-
-def ref_fwd(a, w, b, act, alpha, round_out):
-    """act(a w + b) of one problem: a [M x T], w [T x C], b [C]."""
-    for v in (a, w, b):
-        _assert_on_grid(v, 4)
-    _assert_fits((np.abs(a.astype(np.float64)) @ np.abs(w.astype(np.float64)) + np.abs(b)) * 16, "FWD sums")
-    z = a.astype(np.float64) @ w.astype(np.float64) + b.astype(np.float64)
-    out = act_fwd32(act, z, alpha)
-    if act in INEXACT_ACTS:
-        return out
-    out32 = out.astype(np.float32)
-    assert np.array_equal(out32.astype(np.float64), out)
-    return round_tf32(out32) if round_out else out32
-
-
-def ref_dgrad(dz, w, x, act, alpha, round_out):
-    """(dz w^T) * act'(x) of one problem: dz [M x T], w [C x T] (the layer's [fan-in x fan-out] kernel), x [M x C]."""
-    for v in (dz, w):
-        _assert_on_grid(v, 4)
-    o = dz.astype(np.float64) @ w.astype(np.float64).T
-    bound = np.abs(dz.astype(np.float64)) @ np.abs(w.astype(np.float64)).T * 16
-    if act == "linear":
-        _assert_fits(bound, "DGRAD sums")
-        out = o.astype(np.float32)
-    else:
-        _assert_on_grid(x, 16)
-        g = act_grad32(act, x, alpha)
-        if not (act == "leaky_relu" and np.float32(alpha) * 4 != np.round(np.float32(alpha) * 4)):
-            _assert_on_grid(g, 256)
-            _assert_fits(bound * 256, "DGRAD o * act'")
-        out = o.astype(np.float32) * g               # one fp32 rounding (exact unless alpha is off the grid)
-    return round_tf32(out) if round_out else out
-
-
-def ref_wgrad(h, dz, M, nsplit, rps):
-    """Per-split partials of h^T dz and of the column sums of dz over batch rows [s rps, min(M, (s + 1) rps))."""
-    for v in (h, dz):
-        _assert_on_grid(v, 4)
-    R, C = h.shape[1], dz.shape[1]
-    dw, db = np.zeros((nsplit, R, C), np.float32), np.zeros((nsplit, C), np.float32)
-    for s in range(nsplit):
-        lo, hi = s * rps, min(M, (s + 1) * rps)
-        if hi <= lo:
-            continue
-        hs, ds = h[lo:hi].astype(np.float64), dz[lo:hi].astype(np.float64)
-        _assert_fits(np.abs(hs).T @ np.abs(ds) * 16, "WGRAD sums")
-        _assert_fits(np.abs(ds).sum(0) * 4, "bias column sums")
-        dw[s] = (hs.T @ ds).astype(np.float32)
-        db[s] = ds.sum(0).astype(np.float32)
-    return dw, db
-
-
-def ulp32(x):
-    """fp32 unit in the last place of |x| (the spacing above it)."""
-    x = np.abs(np.asarray(x, np.float32))
-    return (np.nextafter(x, np.float32(np.inf)) - x).astype(np.float64)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -175,7 +57,7 @@ class Group:
         rng = np.random.default_rng(seed)
         Ma = M + extra_rows                                   # rows at or beyond M stay NaN: never read
         n = self.n
-        probs = (_lib().DibGemmProblem * n)()
+        probs = (_L().DibGemmProblem * n)()
         self.probs = probs
         if mode in (FWD, DGRAD):
             # A: [M x lda] activations (FWD: T = fan-in) or output gradients (DGRAD: T = fan-out)
@@ -195,14 +77,14 @@ class Group:
             self.a, self.w, self.b, self.x = [], [], [], []
             for g in range(n):
                 T_, C_ = self.T[g], self.C[g]
-                a = dyadic(rng, (M, T_))
+                a = dyadic(rng, (M, T_), dtype=np.float32)
                 blk = np.zeros((Ma, lda[g]), np.float32)
                 blk[M:] = np.nan
                 blk[:M, :T_] = a                              # pad columns are zeros (the buffers' invariant)
                 A[g * fsA:g * fsA + Ma * lda[g]] = blk.ravel()
-                w = dyadic(rng, (wrows[g], ldb[g]))
+                w = dyadic(rng, (wrows[g], ldb[g]), dtype=np.float32)
                 P[g * pstride:g * pstride + w.size] = w.ravel()
-                b = dyadic(rng, (C_,))
+                b = dyadic(rng, (C_,), dtype=np.float32)
                 if mode == FWD:
                     P[g * pstride + bias_at:g * pstride + bias_at + C_] = b
                 x = act_source(rng, (M, C_))
@@ -245,8 +127,8 @@ class Group:
             self.h, self.dz = [], []
             for g in range(n):
                 R_, C_ = self.R[g], self.C[g]
-                h = dyadic(rng, (M, R_))
-                dz = dyadic(rng, (M, C_))
+                h = dyadic(rng, (M, R_), dtype=np.float32)
+                dz = dyadic(rng, (M, C_), dtype=np.float32)
                 for buf, v, ld, fs in ((A, h, lda[g], fsA), (B, dz, ldb[g], fsB)):
                     blk = np.zeros((Ma, ld), np.float32)
                     blk[M:] = np.nan
@@ -298,7 +180,7 @@ class Group:
     def launch(self, kernel, chunks=1):
         """Run the group on `kernel` ('simt' | 'tc'); returns the output buffer.  Asserts the launch count: one launch, or
         `chunks` when the group's grid needs several."""
-        lib = _lib().load()
+        lib = _L().load()
         dev = torch.device("cuda")
         d = {k: torch.from_numpy(v).to(dev) for k, v in self.host.items()}
         bias = d.get("bias", d["B"])
@@ -306,18 +188,13 @@ class Group:
         st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
         maxC, maxR = max(self.C), max(self.R)
         before = int(lib.dib_launch_count())
-        rc = lib.dib_debug_gemm(_lib().GEMM_KERNELS[kernel], self.mode, ctypes.cast(self.probs, ctypes.c_void_p), self.n, _lib().ptr(d["A"]),
-                                _lib().ptr(d["B"]), _lib().ptr(d["C"]), _lib().ptr(X), _lib().ptr(bias), self.M, maxC, maxR,
+        rc = lib.dib_debug_gemm(_L().GEMM_KERNELS[kernel], self.mode, ctypes.cast(self.probs, ctypes.c_void_p), self.n, _L().ptr(d["A"]),
+                                _L().ptr(d["B"]), _L().ptr(d["C"]), _L().ptr(X), _L().ptr(bias), self.M, maxC, maxR,
                                 self.nsplit, self.rps, getattr(self, "split_stride", 0), self.alpha, self.round_out, st)
-        _lib().check(rc)
+        _L().check(rc)
         launches = int(lib.dib_launch_count()) - before
         assert launches == chunks, (kernel, launches, chunks)
         return d["C"].cpu().numpy()
-
-
-def _lib():
-    from dib_b200 import _lib as L
-    return L
 
 
 # worst errors of the inexact FWD epilogues seen in this process: (act, round_out) -> fp32 ulps (tf32 ulps under round_out)
@@ -415,11 +292,11 @@ def test_tc_refuses_what_it_cannot_run():
     for mode, T, C in ((FWD, 96, 100), (FWD, 8, 128), (DGRAD, 33, 128), (DGRAD, 96, 96)):
         g = Group(mode, [T] * 2, [C] * 2, M=64)
         assert not tc_eligible(mode, T, C)
-        with pytest.raises(_lib().DibError, match="tensor-core kernel cannot run"):
+        with pytest.raises(_L().DibError, match="tensor-core kernel cannot run"):
             g.launch("tc")
         check(g, g.launch("simt"))
     g = Group(FWD, [40, 48], [128, 128], M=64)        # heterogeneous T
-    with pytest.raises(_lib().DibError, match="tensor-core kernel cannot run"):
+    with pytest.raises(_L().DibError, match="tensor-core kernel cannot run"):
         g.launch("tc")
 
 
@@ -517,13 +394,13 @@ def test_wgrad_group_over_the_grid_limit():
 def _wgrad_expected_batched(g):
     """Group.expected for a large uniform WGRAD group: batched float64 contractions over blocks of problems."""
     n, ns, rps, R, C = g.n, g.nsplit, g.rps, g.R[0], g.C[0]
-    _assert_fits(np.array([rps * 16]), "WGRAD sums")        # |h|, |dz| <= 1: every sum is below rps in magnitude
+    fits(np.array([rps * 16]), 1.0, "WGRAD sums")        # |h|, |dz| <= 1: every sum is below rps in magnitude
     exp = g.host["C"].copy()
     for q0 in range(0, n, 64):
         q1 = min(n, q0 + 64)
         h = np.stack(g.h[q0:q1]).astype(np.float64).reshape(q1 - q0, ns, rps, R)
         dz = np.stack(g.dz[q0:q1]).astype(np.float64).reshape(q1 - q0, ns, rps, C)
-        _assert_on_grid(h, 4); _assert_on_grid(dz, 4)
+        assert_on_grid(h, 4); assert_on_grid(dz, 4)
         dw = np.matmul(h.transpose(0, 1, 3, 2), dz).astype(np.float32)      # [problems, ns, R, C]
         db = dz.sum(2).astype(np.float32)                                   # [problems, ns, C]
         for q in range(q0, q1):
@@ -538,21 +415,6 @@ def _wgrad_expected_batched(g):
 # ---------------------------------------------------------------------------------------------------------------------
 # 6. the generic training path at the model level
 # ---------------------------------------------------------------------------------------------------------------------
-def _model(cfg, prec, loss="bce_logits"):
-    from tests.test_gpu_parity import build_model
-    return build_model(cfg, precision=prec, loss=loss)
-
-
-def _per_var(cfg, g, g_ref):
-    from tests.fused16_oracle import per_variable_errors
-    return per_variable_errors(cfg, g, g_ref)
-
-
-def _rel(a, b):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    return np.abs(a - b).max() / max(np.abs(b).max(), 1e-30)
-
-
 @pytest.mark.parametrize("prec", ["fp32", "tf32", "fp16"])
 def test_2048_features_past_the_weight_gradient_grid_limit(prec):
     """2 048 scalar features and n = 8 001 rows: 32 weight-gradient splits, so the encoders' WGRAD group has 65 536 grid
@@ -566,7 +428,7 @@ def test_2048_features_past_the_weight_gradient_grid_limit(prec):
     x = rng.standard_normal((n, 2048)).astype(np.float32)
     y = rng.integers(0, 2, size=(n, 1)).astype(np.float32)
     eps = rng.standard_normal((n, 2048, 2)).astype(np.float32)
-    m = _model(cfg, prec)
+    m = build_model(cfg, precision=prec)
     if prec == "fp16":
         assert "encoders=grouped-wgmma-tf32" in m.kernel_info(n)
     m.set_flat_weights(p)
@@ -575,8 +437,8 @@ def test_2048_features_past_the_weight_gradient_grid_limit(prec):
     g = g.cpu().numpy()
     g_ref, fr = O.train_grads(cfg, p, x, y, eps, 0.01, O.LOSS_BCE_LOGITS)
     tol, tol_var = (5e-5, 2e-4) if prec == "fp32" else (5e-3, 0.1)        # test_gpu_parity / test_gpu_tf32
-    assert _rel(g, g_ref) < tol
-    pv = _per_var(cfg, g, g_ref)
+    assert rel_err(g, g_ref) < tol
+    pv = per_variable_errors(cfg, g, g_ref)
     assert pv.max() < tol_var, (int(pv.argmax()), float(pv.max()))
     np.testing.assert_allclose(st.cpu().numpy()[:2048] / n, fr.kl_per_feature, rtol=2e-5 if prec == "fp32" else 5e-3)
 
@@ -617,7 +479,7 @@ def test_row_isolation_generic_path(prec, shape):
     D = sum(cfg.feature_dimensionalities)
     x = rng.standard_normal((n, D)).astype(np.float32)
     eps = rng.standard_normal((n, cfg.number_features, 32)).astype(np.float32)
-    m = _model(cfg, prec, "mse")
+    m = build_model(cfg, precision=prec, loss="mse")
     m.set_flat_weights(p)
     m.beta.assign(0.0)
     y = np.asarray(m(x, eps=eps), dtype=np.float32)
@@ -636,13 +498,13 @@ def test_row_isolation_generic_path(prec, shape):
     want_loss = float(np.sum((y[rows].astype(np.float64) - y1[rows]) ** 2))
     assert abs(float(st[F]) - want_loss) <= 1e-6 * want_loss, (float(st[F]), want_loss)
     g_ref, _ = O.train_grads(cfg, p, x[rows], y1[rows], eps[rows], 0.0, O.LOSS_MSE, batch_for_mean=n)
-    pv = _per_var(cfg, g, g_ref)
+    pv = per_variable_errors(cfg, g, g_ref)
     # the same rows as a batch of their own (one weight-gradient split), scaled by the same 1 / n
-    m2 = _model(cfg, prec, "mse")
+    m2 = build_model(cfg, precision=prec, loss="mse")
     m2.set_flat_weights(p)
     m2.beta.assign(0.0)
     g_alone, _ = m2.compute_gradients(x[rows], y1[rows], eps=eps[rows], global_batch=n)
-    pv_self = _per_var(cfg, g, g_alone.cpu().numpy())
+    pv_self = per_variable_errors(cfg, g, g_alone.cpu().numpy())
     print(f"row isolation {shape} {prec}: {len(rows)} rows, worst per-variable error vs the oracle {pv.max():.3e} "
           f"(var {int(pv.argmax())}), vs the rows alone {pv_self.max():.3e} (var {int(pv_self.argmax())})")
     assert pv_self.max() < ROWISO_SELF, (int(pv_self.argmax()), float(pv_self.max()))
@@ -662,7 +524,7 @@ def test_one_handle_through_changing_split_counts(prec):
     for n in ns:
         x = rng.standard_normal((n, 16)).astype(np.float32)
         data.append((x, (x[:, :1] * x[:, 1:2] > 0).astype(np.float32)))
-    m = _model(cfg, prec)
+    m = build_model(cfg, precision=prec)
     m.kernel_info(max(ns))                              # size the handle for the largest step: no re-creation below
     m.set_flat_weights(p)
     m.beta.assign(0.01)
@@ -670,7 +532,7 @@ def test_one_handle_through_changing_split_counts(prec):
     for (x, y) in data:
         g, st = m.compute_gradients(x, y, step=3)
         assert m._handle.value == handle
-        f = _model(cfg, prec)
+        f = build_model(cfg, precision=prec)
         f.set_flat_weights(p)
         f.beta.assign(0.01)
         gf, stf = f.compute_gradients(x, y, step=3)

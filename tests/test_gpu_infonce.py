@@ -10,18 +10,9 @@ import torch
 from oracle import dib_oracle as O
 from oracle import philox
 from tests import infonce_oracle as IO
+from tests.gpu_cases import CFG, YARCH, YD, data, params, rel_err, temperature_of
 
 pytestmark = pytest.mark.gpu
-
-# the double-pendulum shape of train.py:116-126 / BASELINE config 3: features [2, 1, 2, 1], out = infonce dim 64,
-# output encoder 6 -> PE 30 -> [128, 128] -> 64
-CFG = O.DIBConfig([2, 1, 2, 1], [128, 128], [256, 256], 64)
-YD, YARCH = 6, [128, 128]
-
-
-def rel_err(a, b):
-    a, b = np.asarray(a, dtype=np.float64), np.asarray(b, dtype=np.float64)
-    return np.abs(a - b).max() / max(np.abs(b).max(), 1e-30)
 
 
 def make_model(similarity="l2", temperature=1.0, precision="fp32", seed=0, lr=1e-3, **kw):
@@ -32,24 +23,6 @@ def make_model(similarity="l2", temperature=1.0, precision="fp32", seed=0, lr=1e
     m.compile(optimizer=dib_b200.Adam(lr), loss=dib_b200.losses.InfoNCE(YD, YARCH, similarity=similarity,
                                                                         temperature=temperature))
     return m
-
-
-def data(n, seed):
-    rng = np.random.default_rng(seed)
-    x = rng.standard_normal((n, 6)).astype(np.float32)
-    y = np.stack([np.sin(x[:, 0]) * x[:, 1], x[:, 2] * x[:, 3], np.cos(x[:, 4]), x[:, 5] ** 2 - 1, np.tanh(x[:, 0] + x[:, 4]),
-                  x[:, 1] * x[:, 5]], -1).astype(np.float32)
-    eps = rng.standard_normal((n, 4, 32)).astype(np.float32)
-    return x, y, eps
-
-
-def params(seed):
-    rng = np.random.default_rng(seed)
-    return IO.glorot(IO.infonce_param_shapes(CFG, YD, YARCH), rng).astype(np.float32)
-
-
-def temperature_of(similarity):
-    return 0.1 if similarity == "cosine" else 1.0
 
 
 @pytest.mark.parametrize("n", [512, 4160])

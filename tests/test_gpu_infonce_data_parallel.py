@@ -16,10 +16,6 @@ Tolerances, with what an H100 measured (NVIDIA H100 80GB HBM3):
     virtual-rank bound above); in fp16 that moves some 16-bit operand roundings by one ulp, and the InfoNCE gradient
     and Adam amplify it over the steps.
 """
-import os
-import socket
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -27,14 +23,13 @@ import torch
 
 from oracle import dib_oracle as O
 from tests import infonce_oracle as IO
-from tests.test_gpu_infonce import CFG, YARCH, YD, data, params, rel_err, temperature_of
+from tests.gpu_cases import CFG, YARCH, YD, _compare_fits, data, params, rel_err, run_workers, temperature_of
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 F = CFG.number_features
 
 
-def make_model(similarity="l2", precision="fp32", seed=0, negatives="global"):
+def global_negatives_model(similarity="l2", precision="fp32", seed=0, negatives="global"):
     import dib_b200
     m = dib_b200.DistributedIBNet(CFG.feature_dimensionalities, CFG.feature_encoder_architecture,
                                   CFG.integration_network_architecture, CFG.output_dimensionality, output_activation_fn=None,
@@ -72,7 +67,7 @@ def shard_step(models, x, y, eps, step=0):
 @pytest.mark.parametrize("precision", ["fp32", "fp16"])
 @pytest.mark.parametrize("similarity", O.SIMILARITY_TYPES)
 def test_phases_at_one_rank_are_the_train_step_bit_for_bit(similarity, precision, n):
-    m = make_model(similarity, precision)
+    m = global_negatives_model(similarity, precision)
     m.set_flat_weights(params(1))
     m.beta.assign(0.01)
     x, y, eps = data(n, 2)
@@ -85,19 +80,19 @@ def test_phases_at_one_rank_are_the_train_step_bit_for_bit(similarity, precision
 def _virtual_ranks(similarity, precision, R, n=1024):
     p = params(3)
     x, y, eps = data(n, 4)
-    ref = make_model(similarity, precision)
+    ref = global_negatives_model(similarity, precision)
     ref.set_flat_weights(p)
     ref.beta.assign(0.01)
     g_ref, st_ref = ref.compute_gradients(x, y, eps=eps)
     models = []
     for _ in range(R):
-        m = make_model(similarity, precision)
+        m = global_negatives_model(similarity, precision)
         m.set_flat_weights(p)
         m.beta.assign(0.01)
         models.append(m)
     e_all, lse_all, grads, stats = shard_step(models, x, y, eps)
     # the one-rank sweep of the same e_all: phase 1 sets up the workspace, then its e_all is replaced by the gathered one
-    one = make_model(similarity, precision)
+    one = global_negatives_model(similarity, precision)
     one.set_flat_weights(p)
     e1_all, lse1_all = one._infonce_buffers(n)
     one._ensure_handle(n)
@@ -124,7 +119,7 @@ def test_virtual_ranks_fp32(similarity, R):
     g64, loss64, kl64 = IO.infonce_train_grads(CFG, p, x, y, eps, 0.01, y_dimensionality=YD, y_encoder_architecture=YARCH,
                                                similarity=similarity, temperature=temperature_of(similarity))
     assert rel_err(g, g64) < 5e-5
-    m = make_model(similarity)
+    m = global_negatives_model(similarity)
     for i, v in enumerate(m.trainable_variables):
         off = m._var_off[i]
         assert rel_err(g[off:off + v.numel()], g64[off:off + v.numel()]) < 2e-4, (similarity, i)
@@ -149,8 +144,8 @@ def test_refusals_come_before_any_collective(monkeypatch):
     def boom(*a, **k):
         raise AssertionError("a collective ran")
     x, y, _ = data(64, 5)
-    plain = make_model(negatives=None)
-    glob = make_model()
+    plain = global_negatives_model(negatives=None)
+    glob = global_negatives_model()
     monkeypatch.setattr(parallel, "all_gather_rows_", boom)
     monkeypatch.setattr(parallel, "allreduce_sum_", boom)
     monkeypatch.setattr(parallel, "world_and_rank", lambda group=None: (2, 0))
@@ -170,7 +165,7 @@ def test_refusals_come_before_any_collective(monkeypatch):
 
 def test_shard_entry_points_validate_their_arguments():
     from dib_b200 import _lib
-    m = make_model()
+    m = global_negatives_model()
     x, y, _ = data(64, 6)
     xs, ys = torch.from_numpy(x).cuda(), torch.from_numpy(y).cuda()
     m._ensure_handle(64)
@@ -181,19 +176,11 @@ def test_shard_entry_points_validate_their_arguments():
         m._infonce_lse(65, e_all, lse_all, 128, 0, m._gradstats[m._P:])
     with pytest.raises(_lib.DibError, match="16-byte"):
         m._infonce_lse(64, e_all.view(-1)[1:], lse_all, 128, 0, m._gradstats[m._P:])
-    other = make_model()
+    other = global_negatives_model()
     other.compile(loss="mse")
     other._ensure_handle(64)
     with pytest.raises(_lib.DibError, match="not DIB_LOSS_INFONCE"):
         other._infonce_lse(64, e_all, lse_all, 128, 0, other._gradstats[other._P:])
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    port = s.getsockname()[1]
-    s.close()
-    return port
 
 
 _WORKER = r"""
@@ -201,7 +188,7 @@ import os, sys
 import numpy as np, torch, torch.distributed as dist
 sys.path.insert(0, os.environ["DIB_ROOT"])
 import dib_b200
-from tests.test_gpu_infonce import CFG, YD, YARCH, data
+from tests.gpu_cases import CFG, YD, YARCH, data
 rank, world, backend = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), os.environ["DIB_BACKEND"]
 dev = torch.device("cuda", rank if backend == "nccl" else 0)
 torch.cuda.set_device(dev)
@@ -228,35 +215,8 @@ if world > 1:
 
 
 def _run_fit(tmp_path, world, prec, backend, graphs):
-    script = tmp_path / "worker.py"
-    script.write_text(_WORKER)
-    out = str(tmp_path / f"w{world}_{prec}_{backend}_{int(graphs)}.npz")
-    env = dict(os.environ, DIB_ROOT=ROOT, DIB_OUT=out, DIB_PREC=prec, DIB_BACKEND=backend, MASTER_ADDR="127.0.0.1",
-               MASTER_PORT=str(_free_port()), WORLD_SIZE=str(world), DIB_CUDA_GRAPH="auto" if graphs else "0",
-               PYTHONPATH=ROOT)
-    procs = [subprocess.Popen([sys.executable, str(script)], env=dict(env, RANK=str(r), LOCAL_RANK=str(r)), cwd=ROOT)
-             for r in range(world)]
-    try:
-        codes = [pr.wait(timeout=600) for pr in procs]
-    finally:
-        for pr in procs:
-            if pr.poll() is None:
-                pr.kill()
-                pr.wait()
-    assert codes == [0] * world, codes
-    return dict(np.load(out))
-
-
-def _compare_fits(a, b, prec):
-    tol_p, tol_h = (1.5e-2, 5e-3) if prec == "fp16" else (2e-4, 2e-4)
-    assert set(a) == set(b)
-    for k in a:
-        if k not in ("params", "graphs"):
-            print(f"{prec}: {k} world 2 vs world 1 {rel_err(b[k], a[k]):.3g}")
-            np.testing.assert_allclose(b[k], a[k], rtol=tol_h, atol=1e-6, err_msg=k)
-    e = rel_err(b["params"], a["params"])
-    print(f"{prec}: weights world 2 vs world 1 {e:.3g}")
-    assert e < tol_p, e
+    return run_workers(tmp_path, _WORKER, world, str(tmp_path / f"w{world}_{prec}_{backend}_{int(graphs)}.npz"), DIB_PREC=prec,
+                       DIB_BACKEND=backend, DIB_CUDA_GRAPH="auto" if graphs else "0")
 
 
 @pytest.mark.parametrize("prec", ["fp32", "fp16"])

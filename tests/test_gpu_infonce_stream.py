@@ -9,22 +9,14 @@ import pytest
 import torch
 
 from tests import infonce_stream_reference as R
-from tests.test_gpu_grouped_gemm import round_tf32
+from tests.fp_exact import C_BOUND, U, round_tf32, within
+from tests.gpu_cases import _dev, _lib
 
 pytestmark = pytest.mark.gpu
 
 KIND = {k: i for i, k in enumerate(R.KINDS)}
 SENTINEL = np.float32(-3.0e33)
 WORST = {}
-
-
-def _lib():
-    from dib_b200 import _lib as L
-    return L, L.load()
-
-
-def _dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
 
 
 def padded_input(e, ld):
@@ -105,27 +97,15 @@ def stream(kind, T, e1, e2, parts=None, phases=3, lse_stride=1, round_out=0, lse
     return out
 
 
-def within(what, got, ref, bound, tag):
-    got, ref, bound = np.asarray(got, np.float64), np.asarray(ref, np.float64), np.asarray(bound, np.float64)
-    err = np.abs(got - ref)
-    bad = ~(err <= bound)
-    assert not bad.any(), (f"{tag} {what}: {bad.sum()} of {bad.size} elements outside their bound; first at "
-                           f"{np.argwhere(bad)[0].tolist()}: got {got[bad][0]!r} ref {ref[bad][0]!r} bound {bound[bad][0]!r}")
-    pos = bound > 0
-    ratio = float((err[pos] / bound[pos]).max()) if pos.any() else 0.0
-    WORST[what] = max(WORST.get(what, 0.0), ratio)
-    print(f"{tag} {what}: worst measured / bound {ratio:.3g}; exact elements {int((~pos).sum())}")
-
-
 def check_stream(kind, T, e1, e2, ref, tag, grads=True):
     out = stream(kind, T, e1, e2, phases=3 if grads else 1)
-    within("r", out["r"], ref["r"], R.C_BOUND * ref["rho_r"], tag)
-    within("c", out["c"], ref["c"], R.C_BOUND * ref["rho_c"], tag)
-    within("s_ii", out["diag"], ref["diag"], R.C_BOUND * ref["sigma_diag"], tag)
-    within("loss_sum", out["loss"][0], ref["loss"], ref["loss_bound"], tag)
+    within(WORST, "r", out["r"], ref["r"], C_BOUND * ref["rho_r"], tag)
+    within(WORST, "c", out["c"], ref["c"], C_BOUND * ref["rho_c"], tag)
+    within(WORST, "s_ii", out["diag"], ref["diag"], C_BOUND * ref["sigma_diag"], tag)
+    within(WORST, "loss_sum", out["loss"][0], ref["loss"], ref["loss_bound"], tag)
     if grads:
-        within("d_e1", out["d1"], ref["d1"], ref["d1_bound"], tag)
-        within("d_e2", out["d2"], ref["d2"], ref["d2_bound"], tag)
+        within(WORST, "d_e1", out["d1"], ref["d1"], ref["d1_bound"], tag)
+        within(WORST, "d_e2", out["d2"], ref["d2"], ref["d2_bound"], tag)
     return out
 
 
@@ -170,13 +150,13 @@ def test_gradient_sweeps_alone_from_float64_log_sum_exps(kind):
     e1, e2, T = R.case_data(kind, n, d, "normal", seed=14)
     lse = R.log_sum_exps(e1, e2, kind, T)
     r32, c32 = lse["r"].astype(np.float32), lse["c"].astype(np.float32)
-    rho_r = np.abs(r32 - lse["r"]) + R.U * np.abs(lse["r"])
-    rho_c = np.abs(c32 - lse["c"]) + R.U * np.abs(lse["c"])
+    rho_r = np.abs(r32 - lse["r"]) + U * np.abs(lse["r"])
+    rho_c = np.abs(c32 - lse["c"]) + U * np.abs(lse["c"])
     out = stream(kind, T, e1, e2, phases=2, lse_in=(r32, c32))
     g1, b1 = R.side_gradient(e1, e2, kind, T, lse["r"], lse["c"], rho_r, rho_c)
     g2, b2 = R.side_gradient(e2, e1, kind, T, lse["c"], lse["r"], rho_c, rho_r)
-    within("d_e1 (phase 2)", out["d1"], g1, b1, kind)
-    within("d_e2 (phase 2)", out["d2"], g2, b2, kind)
+    within(WORST, "d_e1 (phase 2)", out["d1"], g1, b1, kind)
+    within(WORST, "d_e2 (phase 2)", out["d2"], g2, b2, kind)
 
 
 @pytest.mark.parametrize("kind", R.KINDS)
@@ -234,9 +214,9 @@ def test_materialised_head(kind, n, d):
     ref = R.reference(e1, e2, kind, T, head=True)
     loss, d1, d2 = utils.infonce_loss_and_grads(torch.from_numpy(e1).cuda(), torch.from_numpy(e2).cuda(), kind, T)
     tag = f"head {kind} n={n} d={d}"
-    within("head loss", loss.item(), ref["loss"] / n, ref["loss_bound"] / n + R.C_BOUND * R.U * abs(ref["loss"] / n), tag)
-    within("head d_e1", d1.cpu().numpy(), ref["d1"], ref["d1_bound"], tag)
-    within("head d_e2", d2.cpu().numpy(), ref["d2"], ref["d2_bound"], tag)
+    within(WORST, "head loss", loss.item(), ref["loss"] / n, ref["loss_bound"] / n + C_BOUND * U * abs(ref["loss"] / n), tag)
+    within(WORST, "head d_e1", d1.cpu().numpy(), ref["d1"], ref["d1_bound"], tag)
+    within(WORST, "head d_e2", d2.cpu().numpy(), ref["d2"], ref["d2_bound"], tag)
 
 
 @pytest.mark.parametrize("kind", ["l2sq", "l1", "linf"])
@@ -246,8 +226,8 @@ def test_materialised_head_on_dyadic_ties(kind):
     e1, e2, T = R.case_data(kind, n, d, "dyadic", seed=18)
     ref = R.reference(e1, e2, kind, T, head=True)
     _, d1, d2 = utils.infonce_loss_and_grads(torch.from_numpy(e1).cuda(), torch.from_numpy(e2).cuda(), kind, T)
-    within("head d_e1", d1.cpu().numpy(), ref["d1"], ref["d1_bound"], f"head {kind} dyadic")
-    within("head d_e2", d2.cpu().numpy(), ref["d2"], ref["d2_bound"], f"head {kind} dyadic")
+    within(WORST, "head d_e1", d1.cpu().numpy(), ref["d1"], ref["d1_bound"], f"head {kind} dyadic")
+    within(WORST, "head d_e2", d2.cpu().numpy(), ref["d2"], ref["d2_bound"], f"head {kind} dyadic")
 
 
 def test_zz_print_worst_ratios():

@@ -18,6 +18,8 @@ import pytest
 import torch
 
 from tests import int16_reference as R
+from tests.fp_exact import dyadic, from16, to16
+from tests.gpu_cases import _L, _c, _grad_case, _model, _sms, _st
 
 pytestmark = pytest.mark.gpu
 
@@ -29,39 +31,6 @@ NAN16 = {"fp16": 0x7E00, "bf16": 0x7FC0}
 SENT16 = np.int16(-8531)                 # 0xDEAD: finite in both formats, never a result here
 SENT32 = np.float32(-7777.25)
 WORST = {}
-
-
-def _L():
-    from dib_b200 import _lib as L
-    return L
-
-
-def _sms():
-    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
-
-
-def _st():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def to16(v, fmt):
-    """16-bit bit patterns (int16) of float64 values representable in fmt."""
-    v = np.asarray(v, np.float64)
-    if fmt == "fp16":
-        h = v.astype(np.float16)
-        assert np.array_equal(h.astype(np.float64), v, equal_nan=True), "value not representable in fp16"
-        return h.view(np.int16)
-    f = v.astype(np.float32)
-    u = f.view(np.uint32)
-    assert np.array_equal(f.astype(np.float64), v, equal_nan=True) and not np.any(u & 0xFFFF), "value not representable in bf16"
-    return (u >> 16).astype(np.uint16).view(np.int16)
-
-
-def from16(b, fmt):
-    b = np.asarray(b).view(np.int16)
-    if fmt == "fp16":
-        return b.view(np.float16).astype(np.float64)
-    return (b.view(np.uint16).astype(np.uint32) << 16).view(np.float32).astype(np.float64)
 
 
 def mat16(v, fmt, ld, extra_rows=3):
@@ -148,8 +117,8 @@ def _compare(got, got_bits, exp, bound, what, to_bits):
 # ---------------------------------------------------------------------------------------------------------------------
 def run_fwd(fmt, M, K, N, act="relu", alpha=0.25, seed=0, scale=1.0, bias_scale=None):
     rng = np.random.default_rng(seed)
-    a, w = R.dyadic(rng, (M, K)) * scale, R.dyadic(rng, (K, N)) * scale
-    b = R.dyadic(rng, (N,)) * (scale * scale if bias_scale is None else bias_scale)
+    a, w = dyadic(rng, (M, K)) * scale, dyadic(rng, (K, N)) * scale
+    b = dyadic(rng, (N,)) * (scale * scale if bias_scale is None else bias_scale)
     lda, ldc = K + 8, N + 8
     nan = np.int16(np.uint16(NAN16[fmt]).view(np.int16))
     A, W = dev(mat16(a, fmt, lda)), dev(np.concatenate([mat16(w, fmt, N, 0).ravel(), np.full(64, nan, np.int16)]))
@@ -166,7 +135,7 @@ def run_fwd(fmt, M, K, N, act="relu", alpha=0.25, seed=0, scale=1.0, bias_scale=
 
 def run_dgrad(fmt, M, K, N, act="relu", alpha=0.25, seed=0, with_x=True, with_colsum=True):
     rng = np.random.default_rng(seed)
-    dz, w = R.dyadic(rng, (M, N)), R.dyadic(rng, (K, N))
+    dz, w = dyadic(rng, (M, N)), dyadic(rng, (K, N))
     x = (rng.integers(-15, 16, size=(M, K)) / 16).astype(np.float64)
     if act == "relu":
         x = np.maximum(x, 0.0)                               # relu outputs are >= 0
@@ -202,7 +171,7 @@ def run_wgrad(fmt, M, layers, out_scale=0.25, seed=0):
     descs = (_L().DibInt16WgradLayer * len(layers))()
     keep, exp = [], np.full(ss * nsplit_max + 64, SENT32, np.float64)
     for q, (K, N, nsplit, rps) in enumerate(layers):
-        g, dz = R.dyadic(rng, (M, K)), R.dyadic(rng, (M, N))
+        g, dz = dyadic(rng, (M, K)), dyadic(rng, (M, N))
         G, D = dev(mat16(g, fmt, K)), dev(mat16(dz, fmt, N))
         keep += [G, D]
         d = descs[q]
@@ -302,24 +271,24 @@ def run_head(fmt, n, out, nblocks, loss="mse", out_act="linear", hid_act="relu",
              with_y=True, seed=0, alpha=0.25):
     rng = np.random.default_rng(seed)
     K = 256
-    g = R.dyadic(rng, (n, K), k=2, den=2)
+    g = dyadic(rng, (n, K), k=2, den=2)
     if hid_act == "relu":
         g = np.maximum(g, 0)
     elif hid_act in ("tanh", "sigmoid", "elu"):
         g = (rng.integers(-7, 8, size=(n, K)) / 8).astype(np.float64) * (0.5 if hid_act == "sigmoid" else 1)
         if hid_act == "sigmoid":
             g = np.abs(g)
-    Wc, bc = R.dyadic(rng, (K, out), k=1, den=8), R.dyadic(rng, (out,), k=4, den=16)
+    Wc, bc = dyadic(rng, (K, out), k=1, den=8), dyadic(rng, (out,), k=4, den=16)
     exact = loss == "mse" and out_act == "linear" and (out & (out - 1)) == 0
     if loss == "sparse_ce_logits":
         y = rng.integers(0, out, size=n).astype(np.float64)
         edge = [0.0, out - 1.0, -0.5, min(out - 1, 2) + 0.5]      # 0, C - 1, -0.5 (class 0), 2.5 (class 2, never a hit)
         y[:min(n, 4)] = edge[:min(n, 4)]
     elif loss == "mse":
-        y = g @ Wc + bc + R.dyadic(rng, (n, out), k=2, den=16)        # small residuals: every loss sum fits 24 bits
+        y = g @ Wc + bc + dyadic(rng, (n, out), k=2, den=16)        # small residuals: every loss sum fits 24 bits
     else:
         y = rng.integers(0, 2, size=(n, out)).astype(np.float64)
-    w = R.dyadic(rng, (n,), k=4, den=2) + 2.5 if weighted else None        # in [0.5, 4.5], dyadic
+    w = dyadic(rng, (n,), k=4, den=2) + 2.5 if weighted else None        # in [0.5, 4.5], dyadic
     ib = 2.0 ** -int(np.ceil(np.log2(n)))
     S = 2.0 ** 7
     ldg = K + 8
@@ -407,17 +376,17 @@ def test_head_inference_and_no_labels(fmt, head1):
 # ---------------------------------------------------------------------------------------------------------------------
 def run_fwd2(fmt, M, K0, act="relu", stages=3, demb=False, weighted=False, seed=0, alpha=0.25, with_y=True):
     rng = np.random.default_rng(seed)
-    a = R.dyadic(rng, (M, K0), k=2, den=2)
-    W0, W1 = R.dyadic(rng, (K0, 256), k=1, den=8), R.dyadic(rng, (256, 256), k=1, den=8)
-    b0, b1 = R.dyadic(rng, (256,), k=2, den=8), R.dyadic(rng, (256,), k=2, den=8)
-    wout, bout = R.dyadic(rng, (256,), k=2, den=8), np.array([0.125])
+    a = dyadic(rng, (M, K0), k=2, den=2)
+    W0, W1 = dyadic(rng, (K0, 256), k=1, den=8), dyadic(rng, (256, 256), k=1, den=8)
+    b0, b1 = dyadic(rng, (256,), k=2, den=8), dyadic(rng, (256,), k=2, den=8)
+    wout, bout = dyadic(rng, (256,), k=2, den=8), np.array([0.125])
     sfu = act in ("tanh", "sigmoid", "elu")
     if sfu:
-        y = R.dyadic(rng, (M, 1), k=4, den=4)
+        y = dyadic(rng, (M, 1), k=4, den=4)
     else:
         z = R.fwd2(a, W0, b0, W1, b1, wout, bout, act, alpha, None, 1.0, 1.0, 1, fmt, stages=1)["z"]
-        y = z[:, None] + R.dyadic(rng, (M, 1), k=2, den=16)             # small residuals: every loss sum fits 24 bits
-    w = R.dyadic(rng, (M,), k=4, den=2) + 2.5 if weighted else None
+        y = z[:, None] + dyadic(rng, (M, 1), k=2, den=16)             # small residuals: every loss sum fits 24 bits
+    w = dyadic(rng, (M,), k=4, den=2) + 2.5 if weighted else None
     ib, S = 2.0 ** -int(np.ceil(np.log2(M))), 2.0 ** 7
     nan = np.int16(np.uint16(NAN16[fmt]).view(np.int16))
     A = dev(mat16(a, fmt, K0 + 8))
@@ -615,7 +584,6 @@ MODEL_SHAPES = {
 @pytest.mark.parametrize("prec", FMTS)
 @pytest.mark.parametrize("shape", list(MODEL_SHAPES))
 def test_model_shapes_against_rounding_oracle(shape, prec):
-    from tests.test_gpu_fused16_vs_rounding_oracle import _c, _grad_case, _model
     kw, act, mask, tail = MODEL_SHAPES[shape]
     cfg = _c(act=act, **kw)
     n = 128 * 20 + 77

@@ -7,7 +7,7 @@ import pytest
 import torch
 
 from oracle import dib_oracle as O
-from tests.test_gpu_parity import build_model
+from tests.gpu_cases import build_model
 
 pytestmark = pytest.mark.gpu
 

@@ -1,9 +1,6 @@
 """GPU (H100): compiled Keras metrics (compile(metrics=, weighted_metrics=)) -- the metric tail of the statistics vector that
 dib_metrics.cu reduces from the step's own outputs -- against the float64 metric oracle (tests/metrics_oracle.py), and the
 rest of the step bit for bit against the same model without metrics on every loss site."""
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -11,13 +8,11 @@ import torch
 
 from oracle import dib_oracle as O
 from tests import metrics_oracle as MO
-from tests.test_gpu_fused16_vs_rounding_oracle import _c, _data, _expect_route, _params
-from tests.test_gpu_parity import build_model
-from tests.test_gpu_sample_weights import _weights
+from tests.gpu_cases import (_c, _c0, _c0_batch, _compare_fits, _data, _expect_route, _fit_case, _params, _weights, build_model,
+                              make_labels, run_workers)
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _all_metrics(loss, probs=False):
@@ -183,7 +178,6 @@ def test_metric_tail_matches_oracle_on_the_steps_outputs(case, n):
            "mse": O.LOSS_MSE}[loss]
     rng = np.random.default_rng(n)
     x = rng.standard_normal((n, 7)).astype(np.float32)
-    from tests.test_gpu_parity import make_labels
     y = make_labels(rng, lid, n, cfg.output_dimensionality)
     w = _weights(n, n)
     mets, wmets = _all_metrics(loss, probs=loss == "bce_probs")
@@ -240,7 +234,6 @@ def test_metric_tail_matches_oracle_on_the_steps_outputs(case, n):
 def test_fit_and_evaluate_metric_histories_match_oracle(prec):
     import dib_b200
     from dib_b200 import metrics as M
-    from tests.test_gpu_benched_mode import _fit_case
     x, y, cfg = _fit_case()
     rng = np.random.default_rng(1)
     sw = rng.uniform(0, 2, len(x)).astype(np.float32)
@@ -298,7 +291,6 @@ def test_fit_and_evaluate_metric_histories_match_oracle(prec):
 # graph replay, data parallelism, refusals
 # ---------------------------------------------------------------------------------------------------------------------
 def test_graph_replay_with_metrics_and_changing_weights_equals_eager():
-    from tests.test_gpu_benched_mode import _c0, _c0_batch
     cfg = _c0()
     x, y = _c0_batch(512, 3)
     rng = np.random.default_rng(3)
@@ -325,7 +317,7 @@ import numpy as np, torch, torch.distributed as dist
 sys.path.insert(0, os.environ["DIB_ROOT"])
 import dib_b200
 from dib_b200 import metrics as M
-from tests.test_gpu_benched_mode import _fit_case
+from tests.gpu_cases import _fit_case
 rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
 torch.cuda.set_device(0)
 if world > 1:
@@ -354,25 +346,7 @@ if world > 1:
 
 @pytest.mark.parametrize("prec", ["fp32", "fp16"])
 def test_two_process_gloo_fit_with_metrics_equals_one_process_fit(tmp_path, prec):
-    from tests.test_gpu_infonce_data_parallel import _compare_fits, _free_port
-    script = tmp_path / "worker.py"
-    script.write_text(_WORKER)
-    res = {}
-    for world in (1, 2):
-        out = str(tmp_path / f"w{world}.npz")
-        env = dict(os.environ, DIB_ROOT=ROOT, DIB_OUT=out, DIB_PREC=prec, MASTER_ADDR="127.0.0.1", MASTER_PORT=str(_free_port()),
-                   WORLD_SIZE=str(world), PYTHONPATH=ROOT)
-        procs = [subprocess.Popen([sys.executable, str(script)], env=dict(env, RANK=str(r), LOCAL_RANK=str(r)), cwd=ROOT)
-                 for r in range(world)]
-        try:
-            codes = [pr.wait(timeout=600) for pr in procs]
-        finally:
-            for pr in procs:
-                if pr.poll() is None:
-                    pr.kill()
-                    pr.wait()
-        assert codes == [0] * world, codes
-        res[world] = dict(np.load(out))
+    res = {world: run_workers(tmp_path, _WORKER, world, str(tmp_path / f"w{world}.npz"), DIB_PREC=prec) for world in (1, 2)}
     # the first step's tail: confusion counts (integer weights) exactly equal; the mean sums to float32 regrouping
     a, b = res[1].pop("tail"), res[2].pop("tail")
     conf = np.arange(2, 2 + 2 * 402)                 # the tail: mse [0, 2), auc [2, 404), weighted PR auc [404, 806), bce
@@ -388,7 +362,6 @@ def test_two_process_gloo_fit_with_metrics_equals_one_process_fit(tmp_path, prec
 def test_model_level_refusals():
     import dib_b200
     from dib_b200 import metrics as M
-    from tests.test_gpu_benched_mode import _c0
     m = build_model(_c0())
     for bad in ([M.AUC()], [M.Precision()], ["f1"], [lambda a, b: a]):
         with pytest.raises(ValueError):

@@ -11,41 +11,11 @@ import torch
 
 from oracle import dib_oracle as O
 from oracle import philox
+from tests.gpu_cases import LOSS_OF, build_model, load_case, make_labels, rel_err
 
 pytestmark = pytest.mark.gpu
 
 CASES = ["c0_small", "pendulum_like", "radial_like", "odd_shapes"]
-LOSS_OF = {"c0_small": ("bce_logits", O.LOSS_BCE_LOGITS), "pendulum_like": ("mse", O.LOSS_MSE),
-           "radial_like": ("bce_logits", O.LOSS_BCE_LOGITS), "odd_shapes": ("sparse_ce_logits", O.LOSS_SPARSE_CE_LOGITS)}
-
-
-def build_model(cfg, precision="fp32", loss="bce_logits", lr=1e-3, seed=0):
-    import dib_b200
-    m = dib_b200.DistributedIBNet(
-        cfg.feature_dimensionalities, cfg.feature_encoder_architecture, cfg.integration_network_architecture,
-        cfg.output_dimensionality, use_positional_encoding=cfg.use_positional_encoding,
-        number_positional_encoding_frequencies=cfg.number_positional_encoding_frequencies,
-        activation_fn=cfg.activation_fn, feature_embedding_dimension=cfg.feature_embedding_dimension,
-        output_activation_fn=cfg.output_activation_fn, precision=precision, seed=seed, leaky_alpha=cfg.leaky_alpha)
-    m.compile(optimizer=dib_b200.Adam(lr), loss=loss, metrics=["accuracy"])
-    return m
-
-
-def load_case(golden_dir, name):
-    return O.load_forward_golden(os.path.join(golden_dir, f"ref_forward_{name}.npz"))
-
-
-def make_labels(rng, loss, B, out):
-    if loss == O.LOSS_SPARSE_CE_LOGITS:
-        return rng.integers(0, out, size=B).astype(np.float32)
-    if loss == O.LOSS_BCE_LOGITS:
-        return rng.integers(0, 2, size=(B, out)).astype(np.float32)
-    return rng.standard_normal((B, out)).astype(np.float32)
-
-
-def rel_err(a, b):
-    a, b = np.asarray(a, dtype=np.float64), np.asarray(b, dtype=np.float64)
-    return np.abs(a - b).max() / max(np.abs(b).max(), 1e-30)
 
 
 @pytest.mark.parametrize("name", CASES)

@@ -10,6 +10,7 @@ import torch
 from oracle import philox
 from tests import probe_information_oracle as PO
 from tests import set_transformer_oracle as STO
+from tests.gpu_cases import set_transformer_model, small
 
 pytestmark = pytest.mark.gpu
 
@@ -81,31 +82,13 @@ def test_notebook_shape_in_one_call():
 
 
 # ---------------------------------------------------------------------------------------------------- SetTransformerIBNet
-def small(L):
-    return STO.STConfig(particle_feature_dimensions=3, particle_encoder_arch_spec=[16], bottleneck_dimension=8, number_particles=L,
-                        key_dim=12, number_heads=3, number_attention_blocks=2, ff_arch_per_block=[20, 8], final_processing_arch=[12],
-                        number_positional_encoding_frequencies=3)
-
-
-def make_model(cfg, variable=False, seed=0):
-    import dib_b200
-    m = dib_b200.SetTransformerIBNet(cfg.particle_feature_dimensions, cfg.particle_encoder_arch_spec, cfg.bottleneck_dimension,
-                                     cfg.number_particles, key_dim=cfg.key_dim, number_heads=cfg.number_heads,
-                                     number_attention_blocks=cfg.number_attention_blocks, ff_arch_per_block=cfg.ff_arch_per_block,
-                                     final_processing_arch=cfg.final_processing_arch,
-                                     number_positional_encoding_frequencies=cfg.number_positional_encoding_frequencies,
-                                     seed=seed, variable_set_sizes=variable)
-    m.compile(optimizer=dib_b200.Adam(1e-3), loss=dib_b200.losses.BinaryCrossentropy(from_logits=True))
-    return m
-
-
 @pytest.mark.parametrize("cfg", [small(7), STO.STConfig()], ids=["small", "notebook"])
 def test_set_transformer_probe_map_matches_oracle(cfg):
     from dib_b200 import utils
     rng = np.random.default_rng(8)
     N, M, bs, nb, seed = 40, 50, 12, 3, 21
     L, d, E = cfg.number_particles, cfg.particle_feature_dimensions, cfg.bottleneck_dimension
-    m = make_model(cfg)
+    m = set_transformer_model(cfg)
     x = rng.standard_normal((N, L, d)).astype(np.float32)
     probes = rng.standard_normal((M, d)).astype(np.float32)
     got = utils.estimate_mi_bounds_at_probes(m.particle_encoder, probes, x, bs, nb, seed)
@@ -124,7 +107,7 @@ def test_variable_model_uniform_sizes_and_nan_padding():
     cfg = small(7)
     rng = np.random.default_rng(9)
     N, M, L, d = 30, 20, 7, 3
-    fixed, var = make_model(cfg), make_model(cfg, variable=True)
+    fixed, var = set_transformer_model(cfg), set_transformer_model(cfg, variable=True)
     var.set_flat_weights(fixed.get_flat_weights())
     x = rng.standard_normal((N, L, d)).astype(np.float32)
     probes = rng.standard_normal((M, d)).astype(np.float32)
@@ -145,7 +128,7 @@ def test_probe_call_leaves_the_training_state_untouched():
     from dib_b200 import utils
     cfg = small(7)
     rng = np.random.default_rng(10)
-    m = make_model(cfg)
+    m = set_transformer_model(cfg)
     x = torch.from_numpy(rng.standard_normal((32, 7, 3)).astype(np.float32)).cuda()
     y = torch.from_numpy((rng.random((32, 1)) > 0.5).astype(np.float32)).cuda()
     for _ in range(4):
@@ -169,7 +152,7 @@ def test_fit_with_the_callback_is_bit_identical(tmp_path):
     probes = rng.standard_normal((15, 3)).astype(np.float32)
     runs = []
     for with_cb in (False, True):
-        m = make_model(cfg, seed=4)
+        m = set_transformer_model(cfg, seed=4)
         m.noise_seed = 5
         cbs = [dib_b200.InfoBottleneckAnnealingCallback(1e-3, 1e-1, 1, 2)]
         if with_cb:
@@ -192,7 +175,7 @@ def test_set_information_is_L_times_the_batched_kernel():
     from dib_b200 import _lib, utils
     cfg = small(7)
     rng = np.random.default_rng(12)
-    m = make_model(cfg)
+    m = set_transformer_model(cfg)
     N, bs, nb, seed, L, E = 50, 6, 3, 2, 7, 8
     x = rng.standard_normal((N, L, 3)).astype(np.float32)
     got = utils.estimate_set_information(m, x, bs, nb, seed)

@@ -2,9 +2,6 @@
 every loss kernel -- dib_loss_kernel (fp32 / tf32 / the set transformer's head), dib_int16_head_kernel, dib_int16_head1_kernel
 and the fused tail dib_int16_fwd2_kernel -- against the float64 oracles with weights, and all-ones weights against the
 unweighted launches bit for bit."""
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -14,21 +11,12 @@ from oracle import dib_oracle as O
 from oracle import philox
 from tests import fused16_oracle as Q
 from tests import sample_weight_oracle as SW
-from tests.test_gpu_parity import build_model, make_labels, rel_err
-from tests.test_gpu_fused16_vs_rounding_oracle import TOL, _c, _check, _data, _expect_route, _model, _params
+from tests.gpu_cases import (TOL, _c, _c0, _c0_batch, _check, _compare_fits, _data, _expect_route, _fit_case, _model, _params,
+                              _weights, build_model, make_labels, rel_err, run_workers, set_case, set_transformer_model, small,
+                              varlen_set_case)
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _weights(n, seed, hi=50.0):
-    """Weights in [0, hi] with zeros and a few exact integers."""
-    rng = np.random.default_rng(seed + 77)
-    w = rng.uniform(0.0, hi, n).astype(np.float32)
-    w[rng.choice(n, max(1, n // 10), replace=False)] = 0.0
-    w[:3] = [0.0, 1.0, hi]
-    return w
 
 
 def _grads(m, x, y, eps, w=None):
@@ -225,7 +213,6 @@ def test_zero_weight_step(prec):
 
 def test_fp16_large_weights_stay_in_range():
     """Weights up to 1e3: the S-scaled 16-bit gradient carries w * (d loss / d z); fp16 against fp32 on the same step."""
-    from tests.test_gpu_benched_mode import _c0, _c0_batch
     cfg = _c0()
     B = 4096
     x, y = _c0_batch(B, 7)
@@ -253,7 +240,6 @@ def test_fp16_large_weights_stay_in_range():
 # fit, graph replay, data parallelism
 # ---------------------------------------------------------------------------------------------------------------------
 def _fit_setup(prec, loss="bce_logits"):
-    from tests.test_gpu_benched_mode import _fit_case
     x, y, cfg = _fit_case()
     m = build_model(cfg, precision=prec, lr=1e-3, seed=4)
     m.noise_seed = 99
@@ -306,7 +292,6 @@ def test_fit_class_weight_equals_sample_weight_and_matches_oracle(prec):
 
 
 def test_graph_replay_with_changing_weights_equals_eager():
-    from tests.test_gpu_benched_mode import _c0, _c0_batch
     cfg = _c0()
     x, y = _c0_batch(512, 3)
     rng = np.random.default_rng(3)
@@ -326,7 +311,6 @@ def test_graph_replay_with_changing_weights_equals_eager():
 
 def test_train_on_batch_refuses_bad_weights_before_device_work():
     import dib_b200
-    from tests.test_gpu_benched_mode import _c0, _c0_batch
     x, y = _c0_batch(64, 1)
     m = build_model(_c0())
     p0 = m.get_flat_weights().copy()
@@ -355,7 +339,7 @@ import os, sys
 import numpy as np, torch, torch.distributed as dist
 sys.path.insert(0, os.environ["DIB_ROOT"])
 import dib_b200
-from tests.test_gpu_benched_mode import _fit_case
+from tests.gpu_cases import _fit_case
 rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
 torch.cuda.set_device(0)
 if world > 1:
@@ -378,25 +362,7 @@ if world > 1:
 
 @pytest.mark.parametrize("prec", ["fp32", "fp16"])
 def test_two_process_gloo_weighted_fit_equals_one_process_fit(tmp_path, prec):
-    from tests.test_gpu_infonce_data_parallel import _compare_fits, _free_port
-    script = tmp_path / "worker.py"
-    script.write_text(_WORKER)
-    res = {}
-    for world in (1, 2):
-        out = str(tmp_path / f"w{world}.npz")
-        env = dict(os.environ, DIB_ROOT=ROOT, DIB_OUT=out, DIB_PREC=prec, MASTER_ADDR="127.0.0.1", MASTER_PORT=str(_free_port()),
-                   WORLD_SIZE=str(world), PYTHONPATH=ROOT)
-        procs = [subprocess.Popen([sys.executable, str(script)], env=dict(env, RANK=str(r), LOCAL_RANK=str(r)), cwd=ROOT)
-                 for r in range(world)]
-        try:
-            codes = [pr.wait(timeout=600) for pr in procs]
-        finally:
-            for pr in procs:
-                if pr.poll() is None:
-                    pr.kill()
-                    pr.wait()
-        assert codes == [0] * world, codes
-        res[world] = dict(np.load(out))
+    res = {world: run_workers(tmp_path, _WORKER, world, str(tmp_path / f"w{world}.npz"), DIB_PREC=prec) for world in (1, 2)}
     # accuracies count rows: the ~1e-7 regrouping of the two ranks' sums may flip a row next to the 0.5 threshold (one of the
     # 256 validation rows in fp16), so they get the absolute bound of the fit test above; everything else _compare_fits' bounds
     acc = [k for k in res[1] if "accuracy" in k]
@@ -409,18 +375,16 @@ def test_two_process_gloo_weighted_fit_equals_one_process_fit(tmp_path, prec):
 def test_set_transformer_weighted_step_matches_oracle(varlen):
     """Per-set weights against the set-transformer oracles, at the bounds of test_gpu_set_transformer*.py."""
     if varlen:
-        from tests.test_gpu_set_transformer_variable_sizes import case, make_model, small
         cfg = small(7)
-        p, x, y, eps, sizes = case(cfg, np.array([1, 7, 3, 7, 5, 1, 2, 6, 4], np.int32), 1)
+        p, x, y, eps, sizes = varlen_set_case(cfg, np.array([1, 7, 3, 7, 5, 1, 2, 6, 4], np.int32), 1)
         xin = (x, sizes)
     else:
-        from tests.test_gpu_set_transformer import case, make_model, small
         cfg = small(7)
-        p, x, y, eps = case(cfg, 9, 1)
+        p, x, y, eps = set_case(cfg, 9, 1)
         xin = x
     B = x.shape[0]
     w = _weights(B, 9, hi=10.0)
-    m = make_model(cfg)
+    m = set_transformer_model(cfg, variable=varlen)
     m.set_flat_weights(p)
     m.beta.assign(0.02)
     g, st = _grads(m, xin, y, eps, w)

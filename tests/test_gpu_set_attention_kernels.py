@@ -3,44 +3,19 @@
 backward, mean pooling and zero_pad_rows, through the test hooks dib_debug_set_attention / dib_debug_layer_norm /
 dib_debug_set_pool, which launch them as the training step does.  Every call also checks the memory contracts: NaN in every
 input element a kernel must not read, a sentinel in every output element it must not write, and the launch count."""
-import ctypes
-
 import numpy as np
 import pytest
 import torch
 
 from tests import set_attention_reference as R
+from tests.fp_exact import round_tf32, within
+from tests.gpu_cases import _dev, _lib, _st, set_transformer_model, small, varlen_set_case
 
 pytestmark = pytest.mark.gpu
 
 SENTINEL = np.float32(-3.0e33)
 WORST = {}
 ACT = {a: i for i, a in enumerate(R.ACTS)}
-
-
-def _lib():
-    from dib_b200 import _lib as L
-    return L, L.load()
-
-
-def _dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
-def _st():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def within(what, got, ref, bound, tag):
-    got, ref, bound = np.asarray(got, np.float64), np.asarray(ref, np.float64), np.asarray(bound, np.float64)
-    err = np.abs(got - ref)
-    bad = ~(err <= bound)
-    assert not bad.any(), (f"{tag} {what}: {bad.sum()} of {bad.size} elements outside their bound; first at "
-                           f"{np.argwhere(bad)[0].tolist()}: got {got[bad][0]!r} ref {ref[bad][0]!r} bound {bound[bad][0]!r}")
-    pos = bound > 0
-    ratio = float((err[pos] / bound[pos]).max()) if pos.any() else 0.0
-    WORST[what] = max(WORST.get(what, 0.0), ratio)
-    print(f"{tag} {what}: worst measured / bound {ratio:.3g}; exact elements {int((~pos).sum())}")
 
 
 # ---- attention ----------------------------------------------------------------------------------------------------------
@@ -138,10 +113,10 @@ def check_attention(variable, q, k, v, g, sizes, tag, from_float64=False):
     f, b = reference(q, k, v, g, sizes, o_in, lse_in)
     kind = "varlen" if variable else "fixed"
     if not from_float64:
-        within(f"{kind} o", out["o"], f["o"], f["o_bound"], tag)
-        within(f"{kind} lse", out["lse"], f["lse"], f["lse_bound"], tag)
+        within(WORST, f"{kind} o", out["o"], f["o"], f["o_bound"], tag)
+        within(WORST, f"{kind} lse", out["lse"], f["lse"], f["lse_bound"], tag)
     for n in ("dq", "dk", "dv") + (("dsum",) if variable else ()):
-        within(f"{kind} {n}", out[n], b[n], b[n + "_bound"], tag)
+        within(WORST, f"{kind} {n}", out[n], b[n], b[n + "_bound"], tag)
     return out
 
 
@@ -250,7 +225,7 @@ def test_attention_identities(variable):
     for n in base:
         np.testing.assert_array_equal(again[n], base[n], err_msg=n)
     fwd = attention(variable, q, k, v, None, sizes, phases=1, round_out=1)
-    np.testing.assert_array_equal(fwd["o"], R.round_tf32(base["o"]))
+    np.testing.assert_array_equal(fwd["o"], round_tf32(base["o"]))
     np.testing.assert_array_equal(fwd["lse"], base["lse"])
     b0 = attention(variable, q, k, v, g, sizes, phases=2, o_in=base["o"], lse_in=base["lse"])
     b1 = attention(variable, q, k, v, g, sizes, phases=2, o_in=base["o"], lse_in=base["lse"], round_out=1)
@@ -258,7 +233,7 @@ def test_attention_identities(variable):
         if n == "lse":
             continue
         np.testing.assert_array_equal(b0[n], base[n], err_msg=f"backward alone {n}")
-        want = b0[n] if n == "dsum" else R.round_tf32(b0[n])
+        want = b0[n] if n == "dsum" else round_tf32(b0[n])
         np.testing.assert_array_equal(b1[n], want, err_msg=f"round_out {n}")
     sp, hp = np.array([3, 0, 5, 1, 4, 2]), np.array([2, 0, 3, 1])
     perm = attention(variable, *(t[sp][:, hp] for t in (q, k, v, g)), None if sizes is None else sizes[sp])
@@ -303,11 +278,10 @@ def test_out_of_range_sizes_are_the_nearest_bound_in_a_model_step():
     """the same through a whole variable-size step, whose reparameterisation forward and backward also read the sizes:
     gradients, statistics (the KL slot included) and predictions at sizes 0, -5 and Lmax + 1 equal those at 1, 1 and Lmax
     bit for bit.  The host check that rejects such sizes is bypassed to reach the kernels."""
-    from tests.test_gpu_set_transformer_variable_sizes import case as model_case, make_model, small
     cfg = small(65)
     bad, good = np.array([0, -5, 66, 3, 65], np.int32), np.array([1, 1, 65, 3, 65], np.int32)
-    p, x, y, eps, _ = model_case(cfg, good, 32)
-    m = make_model(cfg)
+    p, x, y, eps, _ = varlen_set_case(cfg, good, 32)
+    m = set_transformer_model(cfg, variable=True)
     m.set_flat_weights(p)
     m.beta.assign(0.1)
     m._device_sizes = lambda sizes, n: torch.from_numpy(np.asarray(sizes, np.int32)).cuda()
@@ -421,17 +395,17 @@ def layer_norm(c, phases=3, srcs=(0, 1, 2, 3), dy_pool=None, pool_rows=1, sizes=
 def check_layer_norm(c, tag, srcs=(0, 1, 2, 3), dy_pool=None, pool_rows=1, sizes=None, act=None, nsplit=1, rps=None):
     out = layer_norm(c, 3, srcs, dy_pool, pool_rows, sizes, act, nsplit=nsplit, rps=rps)
     f = R.layer_norm_forward(c["a"], c["b"], c["gamma"], c["beta"], c["eps"])
-    within("ln y", out["y"], f["y"], f["y_bound"], tag)
-    within("ln mean", out["mean"], f["mean"], f["mean_bound"], tag)
-    within("ln rstd", out["rstd"], f["rstd"], f["rstd_bound"], tag)
+    within(WORST, "ln y", out["y"], f["y"], f["y_bound"], tag)
+    within(WORST, "ln mean", out["mean"], f["mean"], f["mean_bound"], tag)
+    within(WORST, "ln rstd", out["rstd"], f["rstd"], f["rstd_bound"], tag)
     pooled = R.pooled_dy(dy_pool, c["rows"], pool_rows, sizes) if dy_pool is not None else None
     b = R.layer_norm_backward(c["a"], c["b"], c["gamma"], out["mean"], out["rstd"], dys=[c["dys"][i] for i in srcs],
                               pooled=pooled, branch_act=act, alpha=float(np.float32(0.2)), nsplit=nsplit, rows_per_split=rps)
-    within("ln d_res", out["d_res"], b["d_res"], b["d_res_bound"], tag)
+    within(WORST, "ln d_res", out["d_res"], b["d_res"], b["d_res_bound"], tag)
     if act is not None:
-        within("ln d_branch", out["d_branch"], b["d_branch"], b["d_branch_bound"], tag)
-    within("ln dgamma", out["dgamma"], b["dgamma"], b["dgamma_bound"], tag)
-    within("ln dbeta", out["dbeta"], b["dbeta"], b["dbeta_bound"], tag)
+        within(WORST, "ln d_branch", out["d_branch"], b["d_branch"], b["d_branch_bound"], tag)
+    within(WORST, "ln dgamma", out["dgamma"], b["dgamma"], b["dgamma_bound"], tag)
+    within(WORST, "ln dbeta", out["dbeta"], b["dbeta"], b["dbeta_bound"], tag)
     return out, b
 
 
@@ -502,13 +476,13 @@ def test_layer_norm_backward_alone_and_identities():
     out = layer_norm(c, phases=2, mean_in=m32, rstd_in=r32, act="elu", nsplit=2, rps=25)
     b = R.layer_norm_backward(c["a"], c["b"], c["gamma"], m32, r32, dys=c["dys"], branch_act="elu", nsplit=2, rows_per_split=25)
     for n in ("d_res", "d_branch", "dgamma", "dbeta"):
-        within(f"ln {n} (phase 2)", out[n], b[n], b[n + "_bound"], "ln backward alone")
+        within(WORST, f"ln {n} (phase 2)", out[n], b[n], b[n + "_bound"], "ln backward alone")
     base = layer_norm(c, act="sigmoid", nsplit=2, rps=25)
     again = layer_norm(c, act="sigmoid", nsplit=2, rps=25)
     rounded = layer_norm(c, act="sigmoid", nsplit=2, rps=25, round_out=1)
     for n in base:
         np.testing.assert_array_equal(again[n], base[n], err_msg=n)
-        want = R.round_tf32(base[n]) if n in ("y", "d_res", "d_branch") else base[n]
+        want = round_tf32(base[n]) if n in ("y", "d_res", "d_branch") else base[n]
         np.testing.assert_array_equal(rounded[n], want, err_msg=f"round_out {n}")
 
 
@@ -566,12 +540,12 @@ def test_pooling(L, sizes, dyadic):
     x = x.astype(np.float32)
     got = pool(x, L, 36, sizes)
     ref, bnd = R.pool(x[:, :36], L, sizes)
-    within("pool", got, ref, bnd, f"pool L={L} sizes={sizes} dyadic={dyadic}")
+    within(WORST, "pool", got, ref, bnd, f"pool L={L} sizes={sizes} dyadic={dyadic}")
     l = np.full(S, L) if sizes is None else np.clip(sizes, 1, L)
     if dyadic:
         exact = (l & (l - 1)) == 0
         np.testing.assert_array_equal(got[exact], ref[exact])
-    np.testing.assert_array_equal(pool(x, L, 36, sizes, round_out=1), R.round_tf32(got))
+    np.testing.assert_array_equal(pool(x, L, 36, sizes, round_out=1), round_tf32(got))
 
 
 def test_zero_pad_rows():

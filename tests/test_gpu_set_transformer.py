@@ -10,42 +10,11 @@ import torch
 from oracle import dib_oracle as O
 from oracle import philox
 from tests import set_transformer_oracle as STO
+from tests.gpu_cases import _config, rel_err, set_case, set_transformer_model, small
 
 pytestmark = pytest.mark.gpu
 
 NOTEBOOK = STO.STConfig()            # 12 features, PE 5, [128, 128], E 32, L 50, 6 blocks of 12 heads x 128, FF [128, 32], head [256]
-
-
-def small(L):
-    return STO.STConfig(particle_feature_dimensions=3, particle_encoder_arch_spec=[16], bottleneck_dimension=8, number_particles=L,
-                        key_dim=12, number_heads=3, number_attention_blocks=2, ff_arch_per_block=[20, 8], final_processing_arch=[12],
-                        number_positional_encoding_frequencies=3)
-
-
-def make_model(cfg, precision="fp32", seed=0, lr=1e-3, metrics=None):
-    import dib_b200
-    m = dib_b200.SetTransformerIBNet(cfg.particle_feature_dimensions, cfg.particle_encoder_arch_spec, cfg.bottleneck_dimension,
-                                     cfg.number_particles, key_dim=cfg.key_dim, number_heads=cfg.number_heads,
-                                     number_attention_blocks=cfg.number_attention_blocks, ff_arch_per_block=cfg.ff_arch_per_block,
-                                     final_processing_arch=cfg.final_processing_arch,
-                                     number_positional_encoding_frequencies=cfg.number_positional_encoding_frequencies,
-                                     precision=precision, seed=seed)
-    m.compile(optimizer=dib_b200.Adam(lr), loss=dib_b200.losses.BinaryCrossentropy(from_logits=True), metrics=metrics)
-    return m
-
-
-def case(cfg, B, seed):
-    rng = np.random.default_rng(seed)
-    p = STO.init_params(cfg, rng)
-    x = rng.standard_normal((B, cfg.number_particles, cfg.particle_feature_dimensions)).astype(np.float32)
-    eps = rng.standard_normal((B, cfg.number_particles, cfg.bottleneck_dimension)).astype(np.float32)
-    y = (rng.random((B, 1)) > 0.5).astype(np.float32)
-    return p, x, y, eps
-
-
-def rel(a, b):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    return np.abs(a - b).max() / max(np.abs(b).max(), 1e-30)
 
 
 # per-variable bound: 2e-4 of the variable's own maximum as DESIGN section 2 at the small shapes.  At the notebook depth (6 blocks)
@@ -54,16 +23,16 @@ def rel(a, b):
 @pytest.mark.parametrize("cfg, B, per_var", [(NOTEBOOK, 32, None), (small(1), 16, 2e-4), (small(7), 9, 2e-4), (small(64), 5, 2e-4)],
                          ids=["notebook", "L1", "L7", "L64"])
 def test_fp32_step_matches_float64_oracle(cfg, B, per_var):
-    m = make_model(cfg)
+    m = set_transformer_model(cfg)
     assert m.count_params() == cfg.param_count()
     assert "set_transformer=attention-simt-fp32" in m.kernel_info(B)
-    p, x, y, eps = case(cfg, B, 1)
+    p, x, y, eps = set_case(cfg, B, 1)
     m.set_flat_weights(p)
     m.beta.assign(0.02)
     g, st = m.compute_gradients(x, y, eps=eps)
     g, st = g.cpu().numpy(), st.cpu().numpy()
     g_ref, fr = STO.train_grads(cfg, p, x, y, eps, 0.02)
-    assert rel(g, g_ref) < 5e-5                                          # max-norm over the flat gradient
+    assert rel_err(g, g_ref) < 5e-5                                          # max-norm over the flat gradient
     scale = np.abs(g_ref).max()
     for i in range(len(m._var_off)):                                     # and per variable
         off, n = m._var_off[i], max(m._var_rows[i], 1) * m._var_cols[i]
@@ -82,13 +51,13 @@ def test_fp32_step_matches_float64_oracle(cfg, B, per_var):
     fr2 = STO.forward(cfg, p, x, eps, keep=True)
     E = cfg.bottleneck_dimension
     ref_ml = np.concatenate([fr2.cache["mu"], fr2.cache["lv"]], -1).reshape(B, cfg.number_particles, 2 * E)
-    assert rel(ml, ref_ml) < 2e-5
+    assert rel_err(ml, ref_ml) < 2e-5
     u = (fr2.cache["mu"] + np.exp(fr2.cache["lv"] / 2) * eps.reshape(-1, E)).reshape(B, cfg.number_particles, E)
     assert np.abs(m.set_transformer(u.astype(np.float32)) - fr.pred).max() < 2e-5 * max(1.0, np.abs(fr.pred).max())
 
 
 def test_param_layout_reports_flattened_attention_kernels():
-    m = make_model(NOTEBOOK)
+    m = set_transformer_model(NOTEBOOK)
     shapes = NOTEBOOK.param_shapes()
     assert len(m._var_off) == len(shapes)
     for r, c, s in zip(m._var_rows, m._var_cols, shapes):
@@ -98,34 +67,34 @@ def test_param_layout_reports_flattened_attention_kernels():
 
 def test_shards_add_up_to_the_full_batch():
     cfg, B = small(7), 12
-    m = make_model(cfg)
-    p, x, y, eps = case(cfg, B, 2)
+    m = set_transformer_model(cfg)
+    p, x, y, eps = set_case(cfg, B, 2)
     m.set_flat_weights(p)
     m.beta.assign(0.1)
     g, st = m.compute_gradients(x, y, eps=eps)
     g1, s1 = m.compute_gradients(x[:5], y[:5], eps=eps[:5], global_batch=B)
     g2, s2 = m.compute_gradients(x[5:], y[5:], eps=eps[5:], global_batch=B, sample_offset=5)
-    assert rel((g1 + g2).cpu().numpy(), g.cpu().numpy()) < 1e-5
+    assert rel_err((g1 + g2).cpu().numpy(), g.cpu().numpy()) < 1e-5
     np.testing.assert_allclose((s1 + s2).cpu().numpy(), st.cpu().numpy(), rtol=1e-5)
     # Philox noise is keyed by the global particle row: the shards draw the full batch's noise
     g, st = m.compute_gradients(x, y, step=3)
     g1, s1 = m.compute_gradients(x[:5], y[:5], global_batch=B, step=3)
     g2, s2 = m.compute_gradients(x[5:], y[5:], global_batch=B, step=3, sample_offset=5)
-    assert rel((g1 + g2).cpu().numpy(), g.cpu().numpy()) < 1e-5
+    assert rel_err((g1 + g2).cpu().numpy(), g.cpu().numpy()) < 1e-5
     np.testing.assert_allclose((s1 + s2).cpu().numpy(), st.cpu().numpy(), rtol=1e-5)
 
 
 def test_seeded_runs_and_graph_replay_are_bit_identical():
     cfg, B = small(7), 16
-    p, x, y, _ = case(cfg, B, 3)
-    a = make_model(cfg)
+    p, x, y, _ = set_case(cfg, B, 3)
+    a = set_transformer_model(cfg)
     a.set_flat_weights(p)
     g1, s1 = a.compute_gradients(x, y, step=5)
     g2, s2 = a.compute_gradients(x, y, step=5)
     assert torch.equal(g1, g2) and torch.equal(s1, s2)
     runs = []
     for graph in (False, True):
-        m = make_model(cfg)
+        m = set_transformer_model(cfg)
         m.use_cuda_graph = graph
         m.set_flat_weights(p)
         m.beta.assign(0.05)
@@ -140,9 +109,9 @@ def test_seeded_runs_and_graph_replay_are_bit_identical():
 def test_fit_follows_the_oracle_history():
     import dib_b200
     cfg, B, n, nv = small(7), 8, 28, 10
-    m = make_model(cfg, lr=2e-3, metrics=["accuracy"])
+    m = set_transformer_model(cfg, lr=2e-3, metrics=["accuracy"])
     m.noise_seed = 77
-    p, x, y, _ = case(cfg, n + nv, 4)
+    p, x, y, _ = set_case(cfg, n + nv, 4)
     m.set_flat_weights(p)
     cb = dib_b200.InfoBottleneckAnnealingCallback(1e-3, 1e-1, 1, 2)
     hist = m.fit(x[:n], y[:n], batch_size=B, epochs=3, callbacks=[cb], validation_data=(x[n:], y[n:]), verbose=0).history
@@ -165,37 +134,20 @@ def test_tf32_against_fp32():
     attention core and the LayerNorms stay fp32.  Through 6 blocks at the notebook shape the measured deviation of the
     gradient from fp32 is printed; the bounds below sit above it with room (DESIGN section 2)."""
     cfg, B = NOTEBOOK, 32
-    p, x, y, eps = case(cfg, B, 5)
+    p, x, y, eps = set_case(cfg, B, 5)
     out = {}
     for prec in ("fp32", "tf32", "fp16"):
-        m = make_model(cfg, precision=prec)
+        m = set_transformer_model(cfg, precision=prec)
         m.set_flat_weights(p)
         m.beta.assign(0.02)
         g, st = m.compute_gradients(x, y, eps=eps)
         out[prec] = (g.cpu().numpy(), st.cpu().numpy(), m(x, eps=eps), m.kernel_info(B))
     assert "operands=tf32" in out["fp16"][3]
-    eg, ep = rel(out["tf32"][0], out["fp32"][0]), np.abs(out["tf32"][2] - out["fp32"][2]).max()
+    eg, ep = rel_err(out["tf32"][0], out["fp32"][0]), np.abs(out["tf32"][2] - out["fp32"][2]).max()
     print(f"tf32 vs fp32: gradient max-norm rel {eg:.3e}, prediction abs {ep:.3e}")
     assert eg < 3e-2 and ep < 1e-2
     assert abs(out["tf32"][1][0] - out["fp32"][1][0]) < 5e-3 * abs(out["fp32"][1][0])
     assert np.array_equal(out["fp16"][0], out["tf32"][0])            # fp16 runs the TF32 kernels
-
-
-def _config(**kw):
-    from dib_b200 import _lib
-    fd = (ctypes.c_int32 * 1)(3)
-    ea = (ctypes.c_int32 * 1)(16)
-    ia = (ctypes.c_int32 * 1)(12)
-    ff = (ctypes.c_int32 * 2)(20, 8)
-    keep = [fd, ea, ia, ff]
-    base = dict(abi_version=_lib.ABI_VERSION, number_features=1, feature_dimensionalities=fd, number_encoder_layers=1,
-                feature_encoder_architecture=ea, number_integration_layers=1, integration_network_architecture=ia,
-                output_dimensionality=1, use_positional_encoding=1, number_positional_encoding_frequencies=3, activation_fn=3,
-                leaky_relu_alpha=0.1, feature_embedding_dimension=8, output_activation_fn=0, loss=0, precision=0, max_batch=16,
-                integration_kind=1, set_size=7, number_attention_blocks=2, number_heads=3, key_dim=12, number_ff_layers=2,
-                ff_architecture=ff, ff_activation_fn=1)
-    base.update(kw)
-    return _lib.DibConfig(**base), keep
 
 
 @pytest.mark.parametrize("kw, match", [

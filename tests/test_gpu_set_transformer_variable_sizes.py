@@ -12,44 +12,11 @@ from oracle import dib_oracle as O
 from oracle import philox
 from tests import set_transformer_oracle as STO
 from tests import set_transformer_varlen_oracle as VO
-from tests.test_gpu_set_transformer import _config
+from tests.gpu_cases import _config, rel_err, set_transformer_model, small, varlen_set_case
 
 pytestmark = pytest.mark.gpu
 
 NOTEBOOK100 = STO.STConfig(number_particles=100)     # nb-particle cell 8's network on neighbourhoods of up to 100 particles
-
-
-def small(L):
-    return STO.STConfig(particle_feature_dimensions=3, particle_encoder_arch_spec=[16], bottleneck_dimension=8, number_particles=L,
-                        key_dim=12, number_heads=3, number_attention_blocks=2, ff_arch_per_block=[20, 8], final_processing_arch=[12],
-                        number_positional_encoding_frequencies=3)
-
-
-def make_model(cfg, precision="fp32", seed=0, lr=1e-3, metrics=None, variable=True):
-    import dib_b200
-    m = dib_b200.SetTransformerIBNet(cfg.particle_feature_dimensions, cfg.particle_encoder_arch_spec, cfg.bottleneck_dimension,
-                                     cfg.number_particles, key_dim=cfg.key_dim, number_heads=cfg.number_heads,
-                                     number_attention_blocks=cfg.number_attention_blocks, ff_arch_per_block=cfg.ff_arch_per_block,
-                                     final_processing_arch=cfg.final_processing_arch,
-                                     number_positional_encoding_frequencies=cfg.number_positional_encoding_frequencies,
-                                     precision=precision, seed=seed, variable_set_sizes=variable)
-    m.compile(optimizer=dib_b200.Adam(lr), loss=dib_b200.losses.BinaryCrossentropy(from_logits=True), metrics=metrics)
-    return m
-
-
-def case(cfg, sizes, seed):
-    rng = np.random.default_rng(seed)
-    B, L = len(sizes), cfg.number_particles
-    p = STO.init_params(cfg, rng)
-    x = rng.standard_normal((B, L, cfg.particle_feature_dimensions)).astype(np.float32)
-    eps = rng.standard_normal((B, L, cfg.bottleneck_dimension)).astype(np.float32)
-    y = (rng.random((B, 1)) > 0.5).astype(np.float32)
-    return p, x, y, eps, np.asarray(sizes, dtype=np.int32)
-
-
-def rel(a, b):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    return np.abs(a - b).max() / max(np.abs(b).max(), 1e-30)
 
 
 def _sizes(lo, hi, B, seed):
@@ -66,15 +33,15 @@ CASES = [(NOTEBOOK100, _sizes(20, 100, 24, 0), None),
 @pytest.mark.parametrize("cfg, sizes, per_var", CASES, ids=["notebook-Lmax100", "Lmax1", "Lmax7", "Lmax65", "Lmax256"])
 def test_fp32_step_matches_masked_float64_oracle(cfg, sizes, per_var):
     B = len(sizes)
-    m = make_model(cfg)
+    m = set_transformer_model(cfg, variable=True)
     assert "set_transformer=attention-varlen-simt-fp32" in m.kernel_info(B)
-    p, x, y, eps, sizes = case(cfg, sizes, 1)
+    p, x, y, eps, sizes = varlen_set_case(cfg, sizes, 1)
     m.set_flat_weights(p)
     m.beta.assign(0.02)
     g, st = m.compute_gradients((x, sizes), y, eps=eps)
     g, st = g.cpu().numpy(), st.cpu().numpy()
     g_ref, fr = VO.train_grads(cfg, p, x, y, eps, sizes, 0.02)
-    assert rel(g, g_ref) < 5e-5
+    assert rel_err(g, g_ref) < 5e-5
     scale = np.abs(g_ref).max()
     for i in range(len(m._var_off)):
         off, n = m._var_off[i], max(m._var_rows[i], 1) * m._var_cols[i]
@@ -97,23 +64,23 @@ def test_fp32_step_matches_masked_float64_oracle(cfg, sizes, per_var):
 def test_matches_the_fixed_size_model_at_each_size():
     cfg = small(64)
     for l in (1, 13, 64):                                             # a uniform batch of size l = the fixed model at L = l
-        p, x, y, eps, _ = case(cfg, [l] * 6, 2)
-        fixed = make_model(small(l), variable=False)
-        var = make_model(cfg)
+        p, x, y, eps, _ = varlen_set_case(cfg, [l] * 6, 2)
+        fixed = set_transformer_model(small(l))
+        var = set_transformer_model(cfg, variable=True)
         for mm in (fixed, var):
             mm.set_flat_weights(p)
             mm.beta.assign(0.05)
         gf, sf = fixed.compute_gradients(x[:, :l], y, eps=eps[:, :l])
         gv, sv = var.compute_gradients((x, np.full(6, l, np.int32)), y, eps=eps)
-        assert rel(gv.cpu().numpy(), gf.cpu().numpy()) < 1e-5, l
+        assert rel_err(gv.cpu().numpy(), gf.cpu().numpy()) < 1e-5, l
         np.testing.assert_allclose(sv.cpu().numpy(), sf.cpu().numpy(), rtol=1e-5)
     sizes = np.array([1, 13, 64, 40, 2], np.int32)                    # per-set predictions of a mixed batch
-    p, x, y, eps, _ = case(cfg, sizes, 3)
-    var = make_model(cfg)
+    p, x, y, eps, _ = varlen_set_case(cfg, sizes, 3)
+    var = set_transformer_model(cfg, variable=True)
     var.set_flat_weights(p)
     pv = var((x, sizes), eps=eps)
     for s, l in enumerate(sizes):
-        fixed = make_model(small(int(l)), variable=False)
+        fixed = set_transformer_model(small(int(l)))
         fixed.set_flat_weights(p)
         pf = fixed(x[s:s + 1, :l], eps=eps[s:s + 1, :l])
         assert np.abs(pv[s] - pf[0]).max() < 1e-5 * max(1.0, np.abs(pf).max()), l
@@ -122,11 +89,11 @@ def test_matches_the_fixed_size_model_at_each_size():
 def test_padding_content_is_ignored_bit_for_bit():
     cfg = small(65)
     sizes = np.array([1, 65, 30, 64, 2, 17], np.int32)
-    p, x, y, eps, _ = case(cfg, sizes, 4)
+    p, x, y, eps, _ = varlen_set_case(cfg, sizes, 4)
     pad = VO.mask_of(sizes, cfg.number_particles) == 0
     xz, xn, en = x.copy(), x.copy(), eps.copy()
     xz[pad], xn[pad], en[pad] = 0.0, np.nan, np.inf
-    m = make_model(cfg)
+    m = set_transformer_model(cfg, variable=True)
     m.set_flat_weights(p)
     m.beta.assign(0.1)
     out = []
@@ -146,22 +113,22 @@ def test_shards_add_up_to_the_full_batch():
     cfg = small(7)
     sizes = np.array([1, 7, 3, 7, 5, 1, 2, 6, 4, 7, 2, 3], np.int32)
     B = len(sizes)
-    m = make_model(cfg)
-    p, x, y, eps, _ = case(cfg, sizes, 5)
+    m = set_transformer_model(cfg, variable=True)
+    p, x, y, eps, _ = varlen_set_case(cfg, sizes, 5)
     m.set_flat_weights(p)
     m.beta.assign(0.1)
     for kw in (lambda a, b: dict(eps=eps[a:b]), lambda a, b: dict(step=3)):
         g, st = m.compute_gradients((x, sizes), y, **kw(0, B))
         g1, s1 = m.compute_gradients((x[:5], sizes[:5]), y[:5], global_batch=B, **kw(0, 5))
         g2, s2 = m.compute_gradients((x[5:], sizes[5:]), y[5:], global_batch=B, sample_offset=5, **kw(5, B))
-        assert rel((g1 + g2).cpu().numpy(), g.cpu().numpy()) < 1e-5
+        assert rel_err((g1 + g2).cpu().numpy(), g.cpu().numpy()) < 1e-5
         np.testing.assert_allclose((s1 + s2).cpu().numpy(), st.cpu().numpy(), rtol=1e-5)
 
 
 def test_seeded_runs_and_graph_replay_with_changing_sizes_are_bit_identical():
     cfg, B = small(70), 16
-    p, x, y, _, _ = case(cfg, [1] * B, 6)
-    a = make_model(cfg)
+    p, x, y, _, _ = varlen_set_case(cfg, [1] * B, 6)
+    a = set_transformer_model(cfg, variable=True)
     a.set_flat_weights(p)
     s0 = _sizes(1, 70, B, 7)
     g1, t1 = a.compute_gradients((x, s0), y, step=5)
@@ -170,7 +137,7 @@ def test_seeded_runs_and_graph_replay_with_changing_sizes_are_bit_identical():
     size_steps = [_sizes(1, 70, B, 10 + k) for k in range(6)]
     runs = []
     for graph in (False, True):
-        m = make_model(cfg)
+        m = set_transformer_model(cfg, variable=True)
         m.use_cuda_graph = graph
         m.set_flat_weights(p)
         m.beta.assign(0.05)
@@ -185,11 +152,11 @@ def test_seeded_runs_and_graph_replay_with_changing_sizes_are_bit_identical():
 def test_fit_on_a_ragged_list_follows_the_oracle_history():
     import dib_b200
     cfg, B, n, nv = small(7), 8, 28, 10
-    m = make_model(cfg, lr=2e-3, metrics=["accuracy"])
+    m = set_transformer_model(cfg, variable=True, lr=2e-3, metrics=["accuracy"])
     m.noise_seed = 77
     sizes = _sizes(1, 7, n + nv, 8)
     sizes[:2] = (1, 7)
-    p, x, y, _, _ = case(cfg, sizes, 9)
+    p, x, y, _, _ = varlen_set_case(cfg, sizes, 9)
     sets = [x[i, :sizes[i]] for i in range(n + nv)]                   # the notebook's list before np.stack
     m.set_flat_weights(p)
     cb = dib_b200.InfoBottleneckAnnealingCallback(1e-3, 1e-1, 1, 2)
@@ -222,15 +189,15 @@ def test_fit_on_a_ragged_list_follows_the_oracle_history():
 def test_tf32_against_fp32():
     cfg = NOTEBOOK100
     sizes = _sizes(20, 100, 32, 11)
-    p, x, y, eps, _ = case(cfg, sizes, 12)
+    p, x, y, eps, _ = varlen_set_case(cfg, sizes, 12)
     out = {}
     for prec in ("fp32", "tf32"):
-        m = make_model(cfg, precision=prec)
+        m = set_transformer_model(cfg, variable=True, precision=prec)
         m.set_flat_weights(p)
         m.beta.assign(0.02)
         g, st = m.compute_gradients((x, sizes), y, eps=eps)
         out[prec] = (g.cpu().numpy(), st.cpu().numpy(), m((x, sizes), eps=eps))
-    eg, ep = rel(out["tf32"][0], out["fp32"][0]), np.abs(out["tf32"][2] - out["fp32"][2]).max()
+    eg, ep = rel_err(out["tf32"][0], out["fp32"][0]), np.abs(out["tf32"][2] - out["fp32"][2]).max()
     print(f"variable sizes, tf32 vs fp32: gradient max-norm rel {eg:.3e}, prediction abs {ep:.3e}")
     assert eg < 3e-2 and ep < 1e-2
     assert abs(out["tf32"][1][0] - out["fp32"][1][0]) < 5e-3 * abs(out["fp32"][1][0])
@@ -250,14 +217,14 @@ def test_dib_create_limits_and_unbound_sizes():
     cfg, _ = _config(set_size=65)
     assert lib.dib_create(ctypes.byref(cfg), ctypes.byref(h)) != 0 and "set_size" in lib.dib_last_error().decode()
     # a variable-size handle without bound sizes refuses to run; a fixed-size handle refuses sizes
-    m = make_model(small(7))
+    m = set_transformer_model(small(7), variable=True)
     m._ensure_handle(4)
     x = torch.zeros(4, 7 * 3, device="cuda")
     stats = torch.empty(4, device="cuda")
     assert lib.dib_forward(m._handle, _lib.ptr(m._params), _lib.ptr(x), None, 4, _lib.ptr(m.beta._dev), None, 0, 0, 0, None, None,
                            _lib.ptr(stats), _lib.ptr(m._workspace), None) != 0
     assert "dib_set_set_sizes_device" in lib.dib_last_error().decode()
-    f = make_model(small(7), variable=False)
+    f = set_transformer_model(small(7))
     f._ensure_handle(4)
     sz = torch.ones(4, dtype=torch.int32, device="cuda")
     assert lib.dib_set_set_sizes_device(f._handle, _lib.ptr(sz)) != 0

@@ -12,7 +12,7 @@ import pytest
 import torch
 
 from oracle import dib_oracle as O
-from tests.test_gpu_parity import LOSS_OF, build_model, load_case, make_labels, rel_err
+from tests.gpu_cases import LOSS_OF, build_model, load_case, make_labels, rel_err
 
 pytestmark = pytest.mark.gpu
 TOL = 5e-3

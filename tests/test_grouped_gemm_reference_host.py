@@ -1,11 +1,13 @@
-"""CPU: the float64 reference of tests/test_gpu_grouped_gemm.py -- its restatement of cvt.rna.tf32.f32 and the exactness
-its operand generators claim -- and dib_create's refusal of more features than the reparametrisation grid can index."""
+"""CPU: the grouped GEMM's float64 reference (tests/grouped_gemm_reference.py) and fp_exact.round_tf32, its restatement of
+cvt.rna.tf32.f32 -- and the exactness its operand generators claim -- and dib_create's refusal of more features than the
+reparametrisation grid can index."""
 import ctypes
 
 import numpy as np
 import pytest
 
-from tests.test_gpu_grouped_gemm import (act_grad32, act_source, dyadic, ref_dgrad, ref_fwd, ref_wgrad, round_tf32)
+from tests.fp_exact import act_grad32, dyadic, round_tf32
+from tests.grouped_gemm_reference import act_source, ref_dgrad, ref_fwd, ref_wgrad
 
 
 def _bits(u):
@@ -69,7 +71,7 @@ def test_operands_are_exact_in_any_summation_order():
     rng = np.random.default_rng(1)
     for trial in range(40):
         T = 512
-        a, w = dyadic(rng, T), dyadic(rng, T)
+        a, w = dyadic(rng, T, dtype=np.float32), dyadic(rng, T, dtype=np.float32)
         if trial % 4 == 0:
             a, w = np.full(T, 1.0, np.float32), np.full(T, 1.0 if trial % 8 else -1.0, np.float32)     # |sum| at its bound
         prods = (a * w).astype(np.float32)
@@ -87,17 +89,17 @@ def test_operands_are_exact_in_any_summation_order():
 
 def test_reference_rounds_only_where_the_kernels_round():
     rng = np.random.default_rng(2)
-    a, w, b = dyadic(rng, (9, 33)), dyadic(rng, (33, 7)), dyadic(rng, 7)
+    a, w, b = dyadic(rng, (9, 33), dtype=np.float32), dyadic(rng, (33, 7), dtype=np.float32), dyadic(rng, 7, dtype=np.float32)
     z = a.astype(np.float64) @ w + b
     assert np.array_equal(ref_fwd(a, w, b, "linear", 0.2, 0), z.astype(np.float32))
     np.testing.assert_array_equal(ref_fwd(a, w, b, "leaky_relu", 0.2, 0),
                                   np.where(z > 0, z, np.float32(0.2) * z.astype(np.float32)).astype(np.float32))
     assert np.array_equal(ref_fwd(a, w, b, "relu", 0.2, 1), round_tf32(np.maximum(z, 0).astype(np.float32)))
     x = act_source(rng, (9, 33))
-    dz = dyadic(rng, (9, 7))
+    dz = dyadic(rng, (9, 7), dtype=np.float32)
     want = (dz.astype(np.float64) @ w.T.astype(np.float64)) * (1 - x.astype(np.float64) ** 2)
     assert np.array_equal(ref_dgrad(dz, w, x, "tanh", 0.2, 0), want.astype(np.float32))
-    h, d = dyadic(rng, (300, 5)), dyadic(rng, (300, 6))
+    h, d = dyadic(rng, (300, 5), dtype=np.float32), dyadic(rng, (300, 6), dtype=np.float32)
     dw, db = ref_wgrad(h, d, 300, 3, 128)
     assert np.array_equal(dw.sum(0).astype(np.float64), h.astype(np.float64).T @ d)
     assert np.array_equal(db[1], d[128:256].sum(0)) and np.array_equal(db[2], d[256:].sum(0))

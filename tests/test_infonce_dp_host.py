@@ -4,7 +4,6 @@ loss and gradients; the loss object's ``negatives`` argument; the ctypes table o
 include/dib_b200.h."""
 import os
 import re
-import socket
 from ctypes import c_int32, c_int64, c_uint32, c_uint64, c_void_p
 
 import numpy as np
@@ -15,14 +14,9 @@ import torch.multiprocessing as mp
 
 from oracle import dib_oracle as O
 from tests import infonce_oracle as IO
+from tests.gpu_cases import _free_port
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
 
 
 def pair_similarity_grads(a, b, similarity, T):

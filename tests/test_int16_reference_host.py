@@ -6,16 +6,17 @@ import pytest
 from oracle import dib_oracle as O
 from tests import fused16_oracle as Q
 from tests import int16_reference as R
+from tests.fp_exact import FORMATS, dyadic, exact_matmul, quantum, ulp16
 
 FMTS = ["fp16", "bf16"]
 
 
 def _layers(seed, M=300, K0=192):
     rng = np.random.default_rng(seed)
-    a = R.dyadic(rng, (M, K0), k=2, den=2)
-    W0, W1 = R.dyadic(rng, (K0, 256), k=1, den=8), R.dyadic(rng, (256, 256), k=1, den=8)
-    b0, b1 = R.dyadic(rng, (256,), k=2, den=8), R.dyadic(rng, (256,), k=2, den=8)
-    wout, bout = R.dyadic(rng, (256,), k=2, den=8), np.array([0.125])
+    a = dyadic(rng, (M, K0), k=2, den=2)
+    W0, W1 = dyadic(rng, (K0, 256), k=1, den=8), dyadic(rng, (256, 256), k=1, den=8)
+    b0, b1 = dyadic(rng, (256,), k=2, den=8), dyadic(rng, (256,), k=2, den=8)
+    wout, bout = dyadic(rng, (256,), k=2, den=8), np.array([0.125])
     return a, W0, b0, W1, b1, wout, bout
 
 
@@ -52,19 +53,19 @@ def test_unrounded_tail_is_the_oracle(act):
 
 def test_unrounded_gemms_and_head_are_the_oracle():
     rng = np.random.default_rng(2)
-    a, w, b = R.dyadic(rng, (200, 192)), R.dyadic(rng, (192, 256)), R.dyadic(rng, (256,))
+    a, w, b = dyadic(rng, (200, 192)), dyadic(rng, (192, 256)), dyadic(rng, (256,))
     for act in ("linear", "relu", "leaky_relu"):
         assert _same(R.gemm_fwd(a, w, b, act, 0.25, None)[0], O.act_fwd(act, a @ w + b, 0.25))
     x = (rng.integers(-15, 16, size=(200, 192)) / 16)
-    dz = R.dyadic(rng, (200, 256))
+    dz = dyadic(rng, (200, 256))
     for act in R.ACTS:
         out, cs = R.gemm_dgrad(dz, w, x, act, 0.25, None)
         assert _same(out, (dz @ w.T) * O.act_grad_from_output(act, x, 0.25))
         assert np.allclose(cs.sum(0), out.sum(0), rtol=0, atol=1e-9)
     parts = R.gemm_wgrad(a, dz, 200, 5, 64, 0.5)                     # split 4 lies past the batch: zeros
     assert _same(parts.sum(0), 0.5 * a.T @ dz) and not parts[4].any()
-    g = np.maximum(R.dyadic(rng, (300, 256), k=2, den=2), 0)
-    Wc, bc = R.dyadic(rng, (256, 4), k=1, den=8), R.dyadic(rng, (4,), k=4, den=16)
+    g = np.maximum(dyadic(rng, (300, 256), k=2, den=2), 0)
+    Wc, bc = dyadic(rng, (256, 4), k=1, den=8), dyadic(rng, (4,), k=4, den=16)
     y = g @ Wc + bc + 0.0625
     h = R.head(g, Wc, bc, "linear", "relu", 0.2, "mse", y, 2.0 ** -9, 2.0 ** 9, nblocks=3, fmt=None, exact=True)
     dz = O.task_loss_grad(O.LOSS_MSE, g @ Wc + bc, y) * 2.0 ** -9
@@ -77,12 +78,12 @@ def test_unrounded_gemms_and_head_are_the_oracle():
 def test_generators_are_exact(fmt):
     rng = np.random.default_rng(3)
     for k, den in ((4, 4), (2, 2), (1, 8), (2, 16)):
-        v = R.dyadic(rng, (1000,), k, den)
-        assert _same(Q.round_to(v, fmt), v) and R.quantum(v) >= 1.0 / den
-    assert R.quantum([0.75, 3.0, 3 * 2.0 ** -20]) == 2.0 ** -20 and R.quantum([0.0]) == 1.0
+        v = dyadic(rng, (1000,), k, den)
+        assert _same(Q.round_to(v, fmt), v) and quantum(v) >= 1.0 / den
+    assert quantum([0.75, 3.0, 3 * 2.0 ** -20]) == 2.0 ** -20 and quantum([0.0]) == 1.0
     with pytest.raises(AssertionError, match="24 bits"):
-        R.exact_matmul(np.full((1, 2 ** 13), 0.25), np.full((2 ** 13, 1), 2.0 ** 10 + 0.25), "sum")
-    R.exact_matmul(np.full((1, 256), 0.25), np.full((256, 1), 0.75), "sum")
+        exact_matmul(np.full((1, 2 ** 13), 0.25), np.full((2 ** 13, 1), 2.0 ** 10 + 0.25), "sum")
+    exact_matmul(np.full((1, 256), 0.25), np.full((256, 1), 0.75), "sum")
 
 
 def test_round_to_edges():
@@ -96,9 +97,9 @@ def test_round_to_edges():
 # ---- every seeded fault breaks the exact comparison ---------------------------------------------------------------------
 def _trunc16(x, fmt):
     """Truncation toward zero instead of round-to-nearest-even."""
-    t, emin, _ = Q.FORMATS[fmt]
+    t, emin, _ = FORMATS[fmt]
     x = np.asarray(x, np.float64)
-    q = R.ulp16(x, fmt)
+    q = ulp16(x, fmt)
     return np.trunc(x / q) * q
 
 
@@ -106,20 +107,20 @@ def _trunc16(x, fmt):
 def test_seeded_gemm_faults(fmt):
     rng = np.random.default_rng(4)
     M, K, N = 257, 320, 256
-    a, w, b = R.dyadic(rng, (M, K)), R.dyadic(rng, (K, N)), R.dyadic(rng, (N,))
+    a, w, b = dyadic(rng, (M, K)), dyadic(rng, (K, N)), dyadic(rng, (N,))
     ref = R.gemm_fwd(a, w, b, "relu", 0.25, fmt)[0]
     # a dropped last 64-deep k-block
     assert not _same(R.gemm_fwd(a[:, :K - 64], w[:K - 64], b, "relu", 0.25, fmt)[0], ref)
     # the bias added after the activation
     assert not _same(Q.round_to(np.maximum(a @ w, 0) + b, fmt), ref)
     # truncation instead of RN-even (operands on a 1/256 grid, so that fp16 rounds too)
-    af = R.dyadic(rng, (M, K), k=255, den=256)
+    af = dyadic(rng, (M, K), k=255, den=256)
     assert not _same(_trunc16(np.maximum(af @ w + b, 0), fmt), R.gemm_fwd(af, w, b, "relu", 0.25, fmt)[0])
     # inf instead of saturation
     big = R.gemm_fwd(a * 64, w * 64, b, "linear", 0.25, "fp16")[0]
     assert not _same(Q.round_to(a * 64 @ (w * 64) + b, "fp16", saturate=False), big)
     # DGRAD: column sums of the rounded values; DGRAD without act'
-    dz, x = R.dyadic(rng, (M, N)), rng.integers(-15, 16, size=(M, K)) / 16
+    dz, x = dyadic(rng, (M, N)), rng.integers(-15, 16, size=(M, K)) / 16
     v = R.dgrad_values(dz, w, x, "tanh", 0.2)
     out, cs = R.gemm_dgrad(dz, w, x, "tanh", 0.2, fmt)
     assert not _same(R.dgrad_colsums(Q.round_to(v.astype(np.float64), fmt).astype(np.float32)), cs)
@@ -134,9 +135,9 @@ def test_seeded_gemm_faults(fmt):
 def test_seeded_head_faults(fmt):
     rng = np.random.default_rng(5)
     n, out, nb = 1000, 3, 3
-    g = np.maximum(R.dyadic(rng, (n, 256), k=2, den=2), 0)
-    Wc, bc = R.dyadic(rng, (256, out), k=1, den=8), R.dyadic(rng, (out,), k=4, den=16)
-    y = g @ Wc + bc + R.dyadic(rng, (n, out), k=2, den=16)
+    g = np.maximum(dyadic(rng, (n, 256), k=2, den=2), 0)
+    Wc, bc = dyadic(rng, (256, out), k=1, den=8), dyadic(rng, (out,), k=4, den=16)
+    y = g @ Wc + bc + dyadic(rng, (n, out), k=2, den=16)
     ib, S = 2.0 ** -10, 2.0 ** 10
     ref = R.head(g, Wc, bc, "linear", "relu", 0.2, "mse", y, ib, S, nblocks=nb, fmt=fmt, z_kernel=g @ Wc + bc)
     # a row credited to the wrong block: the generic kernel's ROWS = 1 assignment with ROWS = 4 instead
@@ -200,7 +201,7 @@ def test_sfu_tail_bounds(fmt, act):
     tile's dg1 column sums dropped leave them."""
     a, W0, b0, W1, b1, wout, bout = _layers(7, M=300, K0=320)
     rng = np.random.default_rng(8)
-    y = R.dyadic(rng, (300, 1))
+    y = dyadic(rng, (300, 1))
     ib, S = 2.0 ** -9, 2.0 ** 9
     d0 = a @ W0 + b0
     act_f = {"tanh": np.tanh, "sigmoid": lambda v: 1 / (1 + np.exp(-v)), "elu": lambda v: np.where(v > 0, v, np.expm1(np.minimum(v, 0)))}[act]

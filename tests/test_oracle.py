@@ -8,12 +8,9 @@ import pytest
 
 from oracle import dib_oracle as O
 from oracle import philox
+from tests.gpu_cases import load_case
 
 CASES = ["c0_small", "pendulum_like", "radial_like", "odd_shapes"]
-
-
-def load_case(golden_dir, name):
-    return O.load_forward_golden(os.path.join(golden_dir, f"ref_forward_{name}.npz"))
 
 
 @pytest.mark.parametrize("name", CASES)

@@ -3,7 +3,6 @@ batch, local SUMS (gradients scaled by 1/B_global, statistics unscaled), one fla
 -- reproduces the single-process result.  The arithmetic inside each rank is done by the CPU oracle here (the CUDA
 engine needs a GPU); the sharding / reduction code under test is dib_b200.parallel."""
 import os
-import socket
 
 import numpy as np
 import pytest
@@ -12,12 +11,7 @@ import torch.distributed as dist
 import torch.multiprocessing as mp
 
 from oracle import dib_oracle as O
-
-
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
+from tests.gpu_cases import _free_port
 
 
 def _worker(rank, world, port, B, out_path):
