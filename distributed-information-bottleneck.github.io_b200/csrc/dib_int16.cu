@@ -258,19 +258,21 @@ dib_int16_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
 //                      L1  D1 = g1 W1  (W1 k-blocks through the same ring)
 //                      e1  g2 = act(D1 + b1) kept PACKED IN REGISTERS, logit = g2 . w + b, compiled loss / metric,
 //                          d loss / d logit, dg2 = dz w act'(g2) -> HBM, output-layer weight / bias gradients and the bias gradient
-//                          of the last hidden layer as per-CTA partials.
+//                          of the last hidden layer as per-CTA partials.  relu / leaky relu / linear: each thread first keeps the
+//                          bits g1 > 0 of its own g1 words (all that act'(g1) needs) in 4 registers, then writes dg2 over those
+//                          words of the g1 tile -> TMA tensor store; other activations store dg2 from the fragments.
 //   training, backward stages on (dg1 != null), the dgrad chain of the same rows:
 //                      D1  acc = dg2 W1^T  (dg2 packed in registers = the wgmma A fragment; W1 K-major through the ring;
 //                          two 128-column chunks)
-//                      e2  dg1 = acc act'(g1) (g1 read back from the shared tile) -> over g1 in the shared tile -> TMA tensor
-//                          store, and packed into registers; its column sums per tile (bias gradient of the first fused layer)
-//                          -> dbpart, in the order of the DGRAD epilogue
+//                      e2  dg1 = acc act'(g1) (act' from the g1 > 0 bits, or g1 read back from the shared tile) -> over the
+//                          shared tile -> TMA tensor store, and packed into registers; its column sums per tile (bias
+//                          gradient of the first fused layer) -> dbpart, in the order of the DGRAD epilogue
 //                      D0  (only when the layer below is the embedding, which has no act') d emb = dg1 W0^T over 128-column
 //                          chunks (W0 K-major through the ring)
 //                      e3  16-bit d emb -> the g1 tile (free by then) -> TMA tensor store
 // The tensor stores leave no partial-sector writes behind and run while the MMAs go on; 4-byte fragment stores straight
-// from the accumulators stall the epilogue that issues them.  Only dg2, produced while the g1 tile still holds g1 (needed
-// by e2's act'), leaves as fragment stores.
+// from the accumulators stall the epilogue that issues them.  Only the dg2 of tanh / sigmoid / elu, produced while the g1
+// tile still holds the g1 that e2's act' needs, leaves as fragment stores.
 // g2 never reaches HBM, and the head's re-read of it (and its launch) disappears; with the backward stages, neither do
 // the two dgrad launches nor their re-reads of dg2, dg1 and g1.  A warp owns 16 whole rows of the accumulator, so each
 // row's logit is complete after a reduction over the 4 lanes that share the row.  Every MMA keeps the operands and the
@@ -282,6 +284,25 @@ dib_int16_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
 // and statically the bias / head-weight rows and one [8][256] column-sum scratch (used in turn by the output layer's dW,
 // the bias gradient of the last hidden layer and that of the first fused layer).
 // ====================================================================================================
+// The warp's column sums of 8 N columns: v[2 j + e] is this thread's partial of column 8 j + 2 q + e (the sum of its two
+// rows); the 8 lanes that share q add them over the same pairs of lanes, in the same order, as quad_col_sum (so every sum
+// has its bits), but each step keeps only half of the columns and sends the other half to the partner: 7 N / 4 shuffles in
+// three independent batches instead of 6 N in dependent chains of three.  Lane (q, b0 = lane bit 2, b1 = bit 3, b2 = bit 4)
+// ends with columns 8 (4 m + 2 b2 + b1) + 2 q + b0, which it writes to col (bank 8 b1 + 16 b2 + 2 q + b0: no conflicts).
+template <int N>
+__device__ __forceinline__ void quad_col_sums(const float (&v)[2 * N], float* col, int lane) {
+  const int q = lane & 3, b0 = (lane >> 2) & 1, b1 = (lane >> 3) & 1, b2 = (lane >> 4) & 1;
+  float s1[N], s2[N / 2], s3[N / 4];
+#pragma unroll
+  for (int m = 0; m < N; ++m) s1[m] = (b0 ? v[2 * m + 1] : v[2 * m]) + __shfl_xor_sync(0xffffffffu, b0 ? v[2 * m] : v[2 * m + 1], 4);
+#pragma unroll
+  for (int m = 0; m < N / 2; ++m) s2[m] = (b1 ? s1[2 * m + 1] : s1[2 * m]) + __shfl_xor_sync(0xffffffffu, b1 ? s1[2 * m] : s1[2 * m + 1], 8);
+#pragma unroll
+  for (int m = 0; m < N / 4; ++m) s3[m] = (b2 ? s2[2 * m + 1] : s2[2 * m]) + __shfl_xor_sync(0xffffffffu, b2 ? s2[2 * m] : s2[2 * m + 1], 16);
+#pragma unroll
+  for (int m = 0; m < N / 4; ++m) col[8 * (4 * m + 2 * b2 + b1) + 2 * q + b0] = s3[m];
+}
+
 constexpr int kF2N = 256, kF2Stages = 3;
 constexpr int kF2AB = kBM * 128, kF2BB = kF2N * 128, kF2Stage = kF2AB + kF2BB;      // 16 KB + 32 KB
 constexpr int kF2BtN = 128, kF2BtB = kF2BtN * 128;   // backward stages: B only, two k-blocks of 128 K-major rows (2 x 16 KB)
@@ -316,7 +337,11 @@ __global__ void __launch_bounds__(kF2Threads, 1)
 dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapW0,
                       const __grid_constant__ CUtensorMap mapW1, const __grid_constant__ CUtensorMap mapW1t,
                       const __grid_constant__ CUtensorMap mapW0t, const __grid_constant__ CUtensorMap mapDemb,
-                      const __grid_constant__ CUtensorMap mapG1, const __grid_constant__ CUtensorMap mapDg1, const Fwd2Args a) {
+                      const __grid_constant__ CUtensorMap mapG1, const __grid_constant__ CUtensorMap mapDg1,
+                      const __grid_constant__ CUtensorMap mapDg2, const Fwd2Args a) {
+  // relu, leaky relu and linear: act'(g1) is a function of the predicate g1 > 0 alone, so 128 bits per thread stand in for
+  // its g1 words, the g1 tile is free from e1 on, and dg2 leaves through it by TMA as dg1 does
+  constexpr bool kStageDg2 = ACT == DIB_ACT_RELU || ACT == DIB_ACT_LEAKY_RELU || ACT == DIB_ACT_LINEAR;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sb = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bar_base = sb + kF2BarOff;
@@ -518,44 +543,63 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
       ds[h] = dzs[h] * a.gscale;
       if (q == 0) dbo += dzs[h];
     }
+    // kStageDg2: bit 4 (j & 7) + 2 h + e of g1m[j / 8] is g1 > 0 for half e of this thread's g1 word (8 j + 2 q, rb + 8 h)
+    uint32_t g1m[4] = {0u, 0u, 0u, 0u};
     if (train) {
       // ---------------- e1, pass 2: column sums of g2 dz (output-layer dW).  The 8 warps cover the tile's 128 rows: fixed-order
       // combine into the thread-owned column
+      {
+        float cw[kF2N / 4];
 #pragma unroll
-      for (int j = 0; j < kF2N / 8; ++j) {
-        const int c = 8 * j + 2 * q;
-        float cw[2] = {0.f, 0.f};
+        for (int j = 0; j < kF2N / 8; ++j) {
+          cw[2 * j] = cw[2 * j + 1] = 0.f;
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          float h0, h1;
-          unpack_h2<BF16>(g2p[2 * j + h], h0, h1);
-          cw[0] += h0 * dzs[h]; cw[1] += h1 * dzs[h];
+          for (int h = 0; h < 2; ++h) {
+            float h0, h1;
+            unpack_h2<BF16>(g2p[2 * j + h], h0, h1);
+            cw[2 * j] += h0 * dzs[h]; cw[2 * j + 1] += h1 * dzs[h];
+          }
         }
-        cw[0] = quad_col_sum(cw[0]); cw[1] = quad_col_sum(cw[1]);
-        if (lane < 4) { s_col[warp][c] = cw[0]; s_col[warp][c + 1] = cw[1]; }
+        quad_col_sums<kF2N / 8>(cw, s_col[warp], lane);
       }
       named_bar_sync(1, kConsumers);
 #pragma unroll
       for (int w = 0; w < kConsumers / 32; ++w) acc_dw += s_col[w][tid];
       named_bar_sync(1, kConsumers);
-      // ---------------- e1, pass 3: dg2 = ds w act'(g2) -> HBM and packed into g2p (A of D1); its column sums (bias gradient)
+      // ---------------- e1, pass 3: dg2 = ds w act'(g2) -> HBM and packed into g2p (A of D1); its column sums (bias gradient).
+      // kStageDg2: each packed dg2 word first takes the place of the thread's g1 word of the same position (its g1 > 0 bits go
+      // to g1m), then the tile leaves as one tensor store group
+      if constexpr (kStageDg2) stores_drained(std::integral_constant<int, 0>());   // the g1 store has read the tile
+      float cb[kF2N / 4];
 #pragma unroll
       for (int j = 0; j < kF2N / 8; ++j) {
         const int c = 8 * j + 2 * q;
         const float2 wv = *reinterpret_cast<const float2*>(&s_w[c]);
-        float cb[2] = {0.f, 0.f};
+        cb[2 * j] = cb[2 * j + 1] = 0.f;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           float h0, h1;
           unpack_h2<BF16>(g2p[2 * j + h], h0, h1);
           const float d0 = ds[h] * wv.x * dib_act_grad(ACT, h0, a.alpha), d1 = ds[h] * wv.y * dib_act_grad(ACT, h1, a.alpha);
-          cb[0] += d0; cb[1] += d1;
+          cb[2 * j] += d0; cb[2 * j + 1] += d1;
           const uint32_t dp = pack_h2<BF16>(d0, d1);
           g2p[2 * j + h] = dp;
-          if (row_lo + 8 * h < a.M) *reinterpret_cast<uint32_t*>(a.dg2 + (row_lo + 8 * h) * a.lddg + c) = dp;
+          if constexpr (kStageDg2) {
+            const uint32_t wa = g1_word(c, rb + 8 * h);
+            if constexpr (ACT != DIB_ACT_LINEAR) {
+              float x0, x1;
+              unpack_h2<BF16>(ld_shared_b32(wa), x0, x1);
+              g1m[j >> 3] |= (x0 > 0.f ? 1u : 0u) << (4 * (j & 7) + 2 * h) | (x1 > 0.f ? 2u : 0u) << (4 * (j & 7) + 2 * h);
+            }
+            st_shared_b32(wa, dp);
+          } else if (row_lo + 8 * h < a.M) *reinterpret_cast<uint32_t*>(a.dg2 + (row_lo + 8 * h) * a.lddg + c) = dp;
         }
-        cb[0] = quad_col_sum(cb[0]); cb[1] = quad_col_sum(cb[1]);
-        if (lane < 4) { s_col[warp][c] = cb[0]; s_col[warp][c + 1] = cb[1]; }
+      }
+      quad_col_sums<kF2N / 8>(cb, s_col[warp], lane);
+      if constexpr (kStageDg2) {
+        fence_proxy_async_smem();
+        named_bar_sync(2 + wg, 128);
+        store_panels(&mapDg2, tile, 0, kF2N / 64, 0);
       }
       named_bar_sync(1, kConsumers);
 #pragma unroll
@@ -572,18 +616,28 @@ dib_int16_fwd2_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
 #pragma unroll
         for (int i = 0; i < 64; ++i) acc2[i] = 0.f;
         mainloop_rs(acc2, g2p);
-        if (cc == 0) stores_drained(std::integral_constant<int, 0>());   // the g1 store has read the tile
+        // the store group that last read the tile (kStageDg2: dg2's; else g1's) is done before dg1 goes over panels 0-1
+        if (cc == 0) stores_drained(std::integral_constant<int, 0>());
 #pragma unroll
         for (int j = 0; j < kF2BtN / 8; ++j) {
           const int c = kF2BtN * cc + 8 * j + 2 * q;
           float cs[2] = {0.f, 0.f};
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            float x0, x1;
             const uint32_t wa = g1_word(c, rb + 8 * h);
-            unpack_h2<BF16>(ld_shared_b32(wa), x0, x1);
-            const float v0 = acc2[4 * j + 2 * h] * dib_act_grad(ACT, x0, a.alpha);
-            const float v1 = acc2[4 * j + 2 * h + 1] * dib_act_grad(ACT, x1, a.alpha);
+            float f0, f1;                                  // act'(g1): the floats dib_act_grad returns, as factors
+            if constexpr (kStageDg2) {
+              const int jj = kF2BtN / 8 * cc + j, b = 4 * (jj & 7) + 2 * h;
+              const float off = ACT == DIB_ACT_LEAKY_RELU ? a.alpha : 0.f;
+              f0 = ACT == DIB_ACT_LINEAR || (g1m[jj >> 3] >> b & 1u) ? 1.f : off;
+              f1 = ACT == DIB_ACT_LINEAR || (g1m[jj >> 3] >> (b + 1) & 1u) ? 1.f : off;
+            } else {
+              float x0, x1;
+              unpack_h2<BF16>(ld_shared_b32(wa), x0, x1);
+              f0 = dib_act_grad(ACT, x0, a.alpha); f1 = dib_act_grad(ACT, x1, a.alpha);
+            }
+            const float v0 = acc2[4 * j + 2 * h] * f0;
+            const float v1 = acc2[4 * j + 2 * h + 1] * f1;
             const uint32_t p = pack_h2<BF16>(v0, v1);
             dg1p[2 * (kF2BtN / 8 * cc + j) + h] = p;
             st_shared_b32(wa, p);
@@ -1106,10 +1160,11 @@ cudaError_t dib_int16_fwd2_head(const void* g_in, int ld_in, int K0, const void*
   CUtensorMap mA, mW0, mW1;
   if (!map_k(&mA, g_in, K0, M, ld_in, kBM) || !map_mn(&mW0, w16_0, kF2N, K0, kF2N, kF2N / 64) || !map_mn(&mW1, w16_1, kF2N, kF2N, kF2N, kF2N / 64))
     return cudaErrorInvalidValue;
-  // the store maps of g1, dg1 and d emb (box 64 x 64: one panel of a warpgroup's rows); backward stages: W1 and W0 K-major
+  // the store maps of g1, dg1, dg2 and d emb (box 64 x 64: one panel of a warpgroup's rows); backward stages: W1 and W0 K-major
   // (box 64 x 128, as dib_int16_dgrad reads them)
-  CUtensorMap mG1, mW1t = mA, mW0t = mA, mDg1 = mA, mDemb = mA;
+  CUtensorMap mG1, mW1t = mA, mW0t = mA, mDg1 = mA, mDg2 = mA, mDemb = mA;
   if (!map_k(&mG1, g1, kF2N, M, kF2N, 64)) return cudaErrorInvalidValue;
+  if (dg2 && !map_k(&mDg2, dg2, kF2N, M, kF2N, 64)) return cudaErrorInvalidValue;   // relu / leaky relu / linear
   if (dg1 && (!map_k(&mW1t, w16_1, kF2N, kF2N, kF2N, kF2BtN) || !map_k(&mDg1, dg1, kF2N, M, kF2N, 64))) return cudaErrorInvalidValue;
   if (demb && (!map_k(&mW0t, w16_0, kF2N, K0, kF2N, kF2BtN) || !map_k(&mDemb, demb, K0, M, K0, 64))) return cudaErrorInvalidValue;
   Fwd2Args a{};
@@ -1129,7 +1184,7 @@ cudaError_t dib_int16_fwd2_head(const void* g_in, int ld_in, int K0, const void*
     e = attr ? cudaSuccess : cudaFuncSetAttribute(dib_int16_fwd2_kernel<BF, ACT, W>, cudaFuncAttributeMaxDynamicSharedMemorySize, kF2Smem); \
     if (e != cudaSuccess) return e;                                                                                                  \
     attr = true;                                                                                                                     \
-    dib_int16_fwd2_kernel<BF, ACT, W><<<grid, kF2Threads, kF2Smem, st>>>(mA, mW0, mW1, mW1t, mW0t, mDemb, mG1, mDg1, a);            \
+    dib_int16_fwd2_kernel<BF, ACT, W><<<grid, kF2Threads, kF2Smem, st>>>(mA, mW0, mW1, mW1t, mW0t, mDemb, mG1, mDg1, mDg2, a);      \
   } while (0)
 #define DIB_F2_BF(ACT, W) do { if (bf16) DIB_F2_LAUNCH(true, ACT, W); else DIB_F2_LAUNCH(false, ACT, W); } while (0)
 #define DIB_F2_ACT(ACT) do { if (weights) DIB_F2_BF(ACT, true); else DIB_F2_BF(ACT, false); } while (0)
